@@ -114,6 +114,11 @@ gemm_simt_kernel(const T* __restrict__ a_hi, const T* __restrict__ a_lo, int lda
 int gemm_simt_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                      int ldb, int M, int N, int K, const EpiParams& ep, bool f16, cudaStream_t st) {
   ANYLOC_REQUIRE(K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0, "gemm_simt: K/lda/ldb must be multiples of 4");
+  // load4 reads 4 elements at once: 16-byte (fp32) / 8-byte (fp16) aligned operands
+  const uintptr_t amask = f16 ? 7 : 15;
+  auto aligned = [&](const void* p) { return (reinterpret_cast<uintptr_t>(p) & amask) == 0; };
+  ANYLOC_REQUIRE(aligned(a_hi) && aligned(a_lo) && aligned(b_hi) && aligned(b_lo),
+                 "gemm_simt: operands must be %d-byte aligned", (int)amask + 1);
   dim3 grid(cdiv(N, BN), cdiv(M, BM));
   if (f16)
     gemm_simt_kernel<__half><<<grid, 256, 0, st>>>((const __half*)a_hi, (const __half*)a_lo, lda, (const __half*)b_hi,

@@ -6,7 +6,8 @@ import ctypes as C
 import pytest
 import torch
 
-from tests.util import rel_inf
+from tests.util import gemm, rel_inf, split_f16
+from tests.util import split_tf32 as split
 
 pytestmark = pytest.mark.gpu
 
@@ -18,25 +19,12 @@ def L(cuda):
     return _lib
 
 
-def split(L, x):
-    hi, lo = torch.empty_like(x), torch.empty_like(x)
-    L.check(L.load().anyloc_split_tf32(L.ptr(x), L.ptr(hi), L.ptr(lo), x.numel(), L.stream_ptr()), "split")
-    return hi, lo
-
-
 def test_split_exact(L):
     x = torch.randn(100003, device="cuda") * torch.logspace(-20, 20, 100003, device="cuda")
     hi, lo = split(L, x)
     assert torch.equal(hi + lo, x)
     assert bool(((hi.view(torch.int32) & 0x1FFF) == 0).all())          # tf32: low 13 mantissa bits clear
     assert bool((lo.abs() <= hi.abs() * 2.0 ** -10).all())
-
-
-def split_f16(L, x, scale):
-    hi, lo = torch.empty_like(x, dtype=torch.float16), torch.empty_like(x, dtype=torch.float16)
-    L.check(L.load().anyloc_split_f16(L.ptr(x), L.ptr(hi), L.ptr(lo), x.numel(), C.c_float(scale), L.stream_ptr()),
-            "split_f16")
-    return hi, lo
 
 
 def test_split_f16_precision(L):
@@ -46,34 +34,6 @@ def test_split_f16_precision(L):
     big = x.abs() > 0.05
     assert float(((rec - x.double()).abs() / x.double().abs())[big].max()) < 2.0 ** -21
     assert float((rec - x.double()).abs().max()) < 2.0 ** -21 * 3 * 6
-
-
-def gemm(L, a, b, epi="bias", bias=None, gamma=None, resid=None, engine="simt", pair="tf32"):
-    """C = a @ b.T through the (hi,lo) pair format `pair`; SPLIT epilogues return the reconstructed value."""
-    M, K = a.shape
-    N = b.shape[0]
-    if pair == "tf32":
-        (a_hi, a_lo), (b_hi, b_lo), alpha = split(L, a), split(L, b), 1.0
-    else:
-        s_b = 2.0 ** int(torch.floor(torch.log2(16384.0 / b.abs().max())).item())
-        (a_hi, a_lo), (b_hi, b_lo) = split_f16(L, a, L.ACT_SCALE), split_f16(L, b, s_b)
-        alpha = 1.0 / (L.ACT_SCALE * s_b)
-    n_out = N // 2 if epi == "swiglu_split" else N
-    is_split = "split" in epi
-    odt = torch.float16 if (is_split and pair == "f16") else torch.float32
-    out = torch.empty(M, n_out, device="cuda", dtype=odt)
-    out_lo = torch.empty(M, n_out, device="cuda", dtype=odt) if is_split else None
-    if epi == "ls_resid":
-        out.copy_(resid)
-        resid = out                                # in place, as the ViT uses it
-    rc = L.load().anyloc_gemm_nt(L.ptr(a_hi), L.ptr(a_lo), K, L.ptr(b_hi), L.ptr(b_lo), K, M, N, K, L.PAIR[pair],
-                                 C.c_float(alpha), L.EPI[epi], L.ptr(bias), L.ptr(gamma), L.ptr(resid), L.ptr(out),
-                                 L.ptr(out_lo), n_out, L.PAIR[pair], L.ENGINE[engine], L.stream_ptr())
-    L.check(rc, "gemm_nt")
-    if not is_split:
-        return out
-    rec = out.double() + out_lo.double()
-    return rec / L.ACT_SCALE if pair == "f16" else rec
 
 
 def ref_gemm(a, b, epi, bias, gamma, resid):
@@ -100,8 +60,6 @@ ENGINES = ["simt", "tc3"]
                                    (2048, 512, 4096), (77, 200, 36)])
 @pytest.mark.parametrize("epi", ["bias", "bias_split", "gelu_split", "swiglu_split", "ls_resid"])
 def test_gemm_epilogues(L, pair, engine, M, N, K, epi):
-    if engine == "tc3" and (K % 8 or N % 8):
-        pytest.skip("shape outside the tensor-core engine's contract")
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     a = torch.randn(M, K, device="cuda", generator=g)
     b = torch.randn(N, K, device="cuda", generator=g) * 0.05
@@ -109,6 +67,11 @@ def test_gemm_epilogues(L, pair, engine, M, N, K, epi):
     n_out = N // 2 if epi == "swiglu_split" else N
     gamma = torch.randn(N, device="cuda", generator=g) if epi == "ls_resid" else None
     resid = torch.randn(M, n_out, device="cuda", generator=g) if epi == "ls_resid" else None
+    q = 8 if pair == "f16" else 4               # gemm_tc_supported: K a multiple of 16 bytes (operands are aligned)
+    if engine == "tc3" and K % q:
+        with pytest.raises(L.AnylocError, match=r"rc=-4"):        # ANYLOC_ERR_UNSUPPORTED
+            gemm(L, a, b, epi, bias, gamma, resid, engine, pair)
+        return
     out = gemm(L, a, b, epi, bias, gamma, resid, engine, pair)
     ref = ref_gemm(a, b, epi, bias, gamma, resid)
     err = rel_inf(out.cpu(), ref.cpu())

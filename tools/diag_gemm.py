@@ -13,8 +13,9 @@ def split(x):
 def gemm(a_hi, a_lo, b_hi, b_lo, engine, out=None):
     M, K = a_hi.shape; N = b_hi.shape[0]
     if out is None: out = torch.empty(M, N, device="cuda")
-    rc = L.load().anyloc_gemm_nt(L.ptr(a_hi), L.ptr(a_lo), K, L.ptr(b_hi), L.ptr(b_lo), K, M, N, K, 0, None, None, None,
-                                 L.ptr(out), None, N, L.ENGINE[engine], L.stream_ptr())
+    rc = L.load().anyloc_gemm_nt(L.ptr(a_hi), L.ptr(a_lo), K, L.ptr(b_hi), L.ptr(b_lo), K, M, N, K, L.PAIR["tf32"],
+                                 1.0, L.EPI["bias"], None, None, None, L.ptr(out), None, N, L.PAIR["tf32"],
+                                 L.ENGINE[engine], L.stream_ptr())
     L.check(rc, "gemm")
     return out
 
