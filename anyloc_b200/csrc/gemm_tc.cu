@@ -96,6 +96,73 @@ __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int 
   }
 }
 
+// Epilogue of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16),
+// accumulators in the wgmma layout.  Applied pair by pair (epi_pair), every bias / gamma / residual load sits between
+// the previous pair's store and this pair's, so the thread waits for one memory round trip per pair -- 32 per tile.
+// Where every column pair of the tile lies inside N (and, except for SwiGLU, ldo is even), the loads of 2 column pairs
+// (both rows) are issued together ahead of their stores instead: 8 round trips per tile.  Same values, same
+// arithmetic.  (Groups of 4 or 8 pairs exceed the 168 registers a thread has here and spill.)
+__device__ __forceinline__ void epilogue_subtile(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
+  const int mode = ep.mode;
+  if (mode < 0) return;                    // diagnostic: discard (ANYLOC_GEMM_DEBUG_SKIP_EPI)
+  const int n0 = nq & ~(BN - 1);
+  const bool swiglu = mode == ANYLOC_EPI_SWIGLU_SPLIT, resid = mode == ANYLOC_EPI_LS_RESID;
+  if (n0 + BN > N || (!swiglu && (ep.ldo & 1))) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = nq + j * 8;
+      if (n >= N) continue;
+      if (r0 < M) epi_pair(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
+      if (r0 + 8 < M) epi_pair(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
+    }
+    return;
+  }
+  const bool row0 = r0 < M, row1 = r0 + 8 < M;
+  const size_t o0 = (size_t)r0 * ep.ldo, o1 = (size_t)(r0 + 8) * ep.ldo;
+  const float al = ep.alpha;
+#pragma unroll
+  for (int j0 = 0; j0 < 16; j0 += 2) {
+    float2 b[2], g[2], ra[2], rb[2];
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const int n = nq + (j0 + jj) * 8;
+      b[jj] = ep.bias ? __ldg(reinterpret_cast<const float2*>(ep.bias + n)) : make_float2(0.f, 0.f);
+      if (resid) {
+        g[jj] = __ldg(reinterpret_cast<const float2*>(ep.gamma + n));
+        if (row0) ra[jj] = *reinterpret_cast<const float2*>(ep.resid + o0 + n);
+        if (row1) rb[jj] = *reinterpret_cast<const float2*>(ep.resid + o1 + n);
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const int j = j0 + jj, n = nq + j * 8;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!(h ? row1 : row0)) continue;
+        const float v0 = sum[4 * j + 2 * h], v1 = sum[4 * j + 2 * h + 1];
+        const size_t ro = h ? o1 : o0;
+        if (swiglu) {                      // (x1_j, x2_j) = columns (n, n+1) -> column n/2
+          const float x1 = v0 * al + b[jj].x, x2 = v1 * al + b[jj].y;
+          epi_store_split(ep, ro + (n >> 1), silu(x1) * x2);
+          continue;
+        }
+        const float x0 = v0 * al + b[jj].x, x1 = v1 * al + b[jj].y;
+        const size_t o = ro + n;
+        if (mode == ANYLOC_EPI_BIAS) {
+          *reinterpret_cast<float2*>(ep.out + o) = make_float2(x0, x1);
+        } else if (resid) {
+          const float2 r = h ? rb[jj] : ra[jj];
+          *reinterpret_cast<float2*>(ep.out + o) = make_float2(r.x + g[jj].x * x0, r.y + g[jj].y * x1);
+        } else if (mode == ANYLOC_EPI_GELU_SPLIT) {
+          store_split2(ep, o, gelu_erf(x0), gelu_erf(x1));
+        } else {                           // BIAS_SPLIT
+          store_split2(ep, o, x0, x1);
+        }
+      }
+    }
+  }
+}
+
 // F16 = false: operands are fp32 words read as tf32 (32 elements per 128 B k-block, wgmma K=8)
 // F16 = true : operands are fp16            (64 elements per 128 B k-block, wgmma K=16, 2x rate)
 // ep.gate (nullable): the kernel returns at once when *gate == 0 (conditional fallbacks without a host sync).
@@ -190,14 +257,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       for (int j = 0; j < 64; ++j) sum[j] += acc[j];
     }
     if (t == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
-    const int r0 = m0 + warp * 16 + (lane >> 2);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int n = n0 + j * 8 + 2 * (lane & 3);
-      if (n >= N) continue;
-      if (r0 < M) epi_pair(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
-      if (r0 + 8 < M) epi_pair(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
-    }
+    epilogue_subtile(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
   }
 }
 
