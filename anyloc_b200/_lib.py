@@ -74,6 +74,12 @@ _SIGS = {
     "anyloc_kmeans_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
     "anyloc_kmeans_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 3 +
                              [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_kmeans_partition": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int64)]),
+    "anyloc_kmeans_round_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "anyloc_kmeans_accumulate_round": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int,
+                                                 C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_kmeans_finalize": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_void_p]),
     "anyloc_topk_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "anyloc_topk": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 6 +
                     [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

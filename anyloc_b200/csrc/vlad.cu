@@ -842,19 +842,24 @@ vlad_normalize_kernel(float* __restrict__ vlad, const float* __restrict__ partia
 // Deterministic: every (column slice, row chunk) CTA writes ITS partial sums / counts, the finalize kernel adds the
 // chunks in chunk order -- no floating-point atomics, so a fitted vocabulary is bit-reproducible for a fixed seed
 // (like the reference's single-threaded mask @ X).
+// x holds one ROUND: chunk c's piece is rows [c*piece, min(R, (c+1)*piece)) of x.  The in-memory update is one round
+// of whole chunks (piece = rows_per).  A streamed fit feeds each chunk's rows in several rounds; with `resume` the
+// running sums continue from psums / pcounts, and a sequential fp32 sum continued from a stored partial is the same
+// sum, so the partials after the last round are bit-identical to the in-memory ones.
 __global__ void kmeans_accumulate_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
-                                         int64_t R, int D, int K, float* __restrict__ psums /* [chunks,K,D] */,
+                                         int64_t R, int64_t piece, int D, int K, int resume,
+                                         float* __restrict__ psums /* [chunks,K,D] */,
                                          float* __restrict__ pcounts /* [chunks,K] */) {
   // grid (D/128 slices, row-chunks); shared [K][128] partial sums
   extern __shared__ float acc[];
   const int t = threadIdx.x, col = blockIdx.x * ACC_COLS + t;
   const bool colok = col < D;
-  for (int k = 0; k < K; ++k) acc[k * ACC_COLS + t] = 0.f;
+  float* ps = psums + (size_t)blockIdx.y * K * D;
+  for (int k = 0; k < K; ++k) acc[k * ACC_COLS + t] = resume && colok ? ps[(size_t)k * D + col] : 0.f;
   float* cnt = acc + (size_t)K * ACC_COLS;
-  for (int k = t; k < K; k += ACC_COLS) cnt[k] = 0.f;
+  for (int k = t; k < K; k += ACC_COLS) cnt[k] = resume && blockIdx.x == 0 ? pcounts[(size_t)blockIdx.y * K + k] : 0.f;
   __syncthreads();
-  int64_t rows_per = (R + gridDim.y - 1) / gridDim.y;
-  int64_t r0 = (int64_t)blockIdx.y * rows_per, r1 = min(R, r0 + rows_per);
+  int64_t r0 = (int64_t)blockIdx.y * piece, r1 = min(R, r0 + piece);
   for (int64_t r = r0; r < r1; ++r) {
     int l = labels[r];
     if (l < 0) continue;
@@ -862,7 +867,6 @@ __global__ void kmeans_accumulate_kernel(const float* __restrict__ x, const int3
     if (blockIdx.x == 0 && t == 0) cnt[l] += 1.f;
   }
   __syncthreads();
-  float* ps = psums + (size_t)blockIdx.y * K * D;
   for (int k = 0; k < K; ++k)
     if (colok) ps[(size_t)k * D + col] = acc[k * ACC_COLS + t];
   if (blockIdx.x == 0)
@@ -1227,43 +1231,99 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   return ANYLOC_OK;
 }
 
-static int kmeans_chunks(int R, int D) {
+// The fixed row partition of the k-means update: at most 64 contiguous chunks, enough (column slice, chunk) CTAs to
+// fill the device, at least 256 rows per chunk.  Its summation order is what a fitted vocabulary's bits depend on.
+static int kmeans_chunks(int64_t R, int D) {
   const int nslices = cdiv(D, ACC_COLS);
-  return std::max(1, std::min(std::min((int)((R + 255) / 256), 4 * device_sm_count() / std::max(1, nslices)), 64));
+  const int64_t fill = 4 * device_sm_count() / std::max(1, nslices);
+  return (int)std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>((R + 255) / 256, fill), 64));
 }
 constexpr int KMEANS_FIN_BLOCKS = 64;
 
-extern "C" size_t anyloc_kmeans_workspace_bytes(int R, int D, int K) {
+namespace {
+struct KmeansBufs { float *psums, *pcounts, *perr; int chunks; };
+bool take_kmeans_bufs(void* ws, size_t ws_bytes, int64_t R, int D, int K, KmeansBufs* b) {
+  b->chunks = kmeans_chunks(R, D);
+  Workspace w(ws, ws_bytes);
+  b->psums = w.take<float>((size_t)b->chunks * K * D);
+  b->pcounts = w.take<float>((size_t)b->chunks * K);
+  b->perr = w.take<float>(KMEANS_FIN_BLOCKS);
+  return b->psums && b->pcounts && b->perr;
+}
+}  // namespace
+
+extern "C" int anyloc_kmeans_partition(int64_t R, int D, int* chunks, int64_t* rows_per) {
+  ANYLOC_REQUIRE(chunks && rows_per, "kmeans_partition: null pointer");
+  ANYLOC_REQUIRE(R >= 0 && D > 0, "kmeans_partition: bad dims R=%lld D=%d", (long long)R, D);
+  *chunks = kmeans_chunks(R, D);
+  *rows_per = (R + *chunks - 1) / *chunks;
+  return ANYLOC_OK;
+}
+
+extern "C" size_t anyloc_kmeans_round_workspace_bytes(int64_t R, int D, int K) {
   const size_t chunks = (size_t)kmeans_chunks(R, D);
   return align_up(chunks * K * D * 4, 256) + align_up(chunks * K * 4, 256) + align_up(KMEANS_FIN_BLOCKS * 4, 256) + 256;
+}
+
+extern "C" size_t anyloc_kmeans_workspace_bytes(int R, int D, int K) {
+  return anyloc_kmeans_round_workspace_bytes(R, D, K);
+}
+
+extern "C" int anyloc_kmeans_accumulate_round(const float* x, const int32_t* labels, int64_t R, int64_t round_rows,
+                                              int64_t piece_rows, int D, int K, int resume, void* ws, size_t ws_bytes,
+                                              void* stream) {
+  ANYLOC_REQUIRE(x && labels && ws, "kmeans_accumulate_round: null pointer");
+  ANYLOC_REQUIRE(R >= 0 && D > 0 && K > 0 && piece_rows >= 0 && round_rows >= 0,
+                 "kmeans_accumulate_round: bad dims R=%lld D=%d K=%d", (long long)R, D, K);
+  KmeansBufs b;
+  if (!take_kmeans_bufs(ws, ws_bytes, R, D, K, &b)) {
+    set_error("kmeans_accumulate_round: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_kmeans_round_workspace_bytes(R, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  ANYLOC_REQUIRE(round_rows <= (int64_t)b.chunks * piece_rows,
+                 "kmeans_accumulate_round: %lld rows do not fit %d pieces of %lld", (long long)round_rows, b.chunks,
+                 (long long)piece_rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  size_t smem = ((size_t)K * ACC_COLS + K) * 4;
+  ANYLOC_REQUIRE(smem <= 220 * 1024, "kmeans_accumulate_round: K=%d too large", K);
+  ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(kmeans_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+  int nslices = cdiv(D, ACC_COLS);
+  kmeans_accumulate_kernel<<<dim3(nslices, b.chunks), ACC_COLS, smem, st>>>(x, labels, round_rows, piece_rows, D, K,
+                                                                            resume, b.psums, b.pcounts);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_kmeans_finalize(const float* old_centers, int64_t R, int D, int K, float* new_centers,
+                                      float* err_out, void* ws, size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(old_centers && new_centers && err_out && ws, "kmeans_finalize: null pointer");
+  KmeansBufs b;
+  if (!take_kmeans_bufs(ws, ws_bytes, R, D, K, &b)) {
+    set_error("kmeans_finalize: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_kmeans_round_workspace_bytes(R, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  kmeans_finalize_kernel<<<KMEANS_FIN_BLOCKS, 256, 0, st>>>(b.psums, b.pcounts, b.chunks, old_centers, D, K,
+                                                            new_centers, b.perr);
+  ANYLOC_CHECK_LAUNCH();
+  kmeans_err_kernel<<<1, 32, 0, st>>>(b.perr, KMEANS_FIN_BLOCKS, err_out);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
 }
 
 extern "C" int anyloc_kmeans_update(const float* x, const int32_t* labels, const float* old_centers,
                                     int R, int D, int K, float* new_centers, float* err_out, void* ws,
                                     size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(x && labels && old_centers && new_centers && err_out && ws, "kmeans_update: null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int chunks = kmeans_chunks(R, D);
-  Workspace w(ws, ws_bytes);
-  float* psums = w.take<float>((size_t)chunks * K * D);
-  float* pcounts = w.take<float>((size_t)chunks * K);
-  float* perr = w.take<float>(KMEANS_FIN_BLOCKS);
-  if (!psums || !pcounts || !perr) {
-    set_error("kmeans_update: workspace too small (%zu given, %zu needed)", ws_bytes, anyloc_kmeans_workspace_bytes(R, D, K));
-    return ANYLOC_ERR_WORKSPACE;
-  }
-  size_t smem = ((size_t)K * ACC_COLS + K) * 4;
-  ANYLOC_REQUIRE(smem <= 220 * 1024, "kmeans_update: K=%d too large", K);
-  ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(kmeans_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-  int nslices = cdiv(D, ACC_COLS);
-  kmeans_accumulate_kernel<<<dim3(nslices, chunks), ACC_COLS, smem, st>>>(x, labels, R, D, K, psums, pcounts);
-  ANYLOC_CHECK_LAUNCH();
-  kmeans_finalize_kernel<<<KMEANS_FIN_BLOCKS, 256, 0, st>>>(psums, pcounts, chunks, old_centers, D, K, new_centers, perr);
-  ANYLOC_CHECK_LAUNCH();
-  kmeans_err_kernel<<<1, 32, 0, st>>>(perr, KMEANS_FIN_BLOCKS, err_out);
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  int chunks;
+  int64_t rows_per;
+  int rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
+  if (!rc) rc = anyloc_kmeans_accumulate_round(x, labels, R, R, rows_per, D, K, 0, ws, ws_bytes, stream);
+  if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
+  return rc;
 }
 
 // ====================================================================================================================

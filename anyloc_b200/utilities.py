@@ -383,6 +383,71 @@ def _normalize_rows_dev(x):
     return y
 
 
+# ------------------------------------------------------------------ k-means on host rows larger than the device
+_STAGE_BYTES = 1 << 30      # each of the two pinned staging buffers of a streamed fit: at most 2 GiB of host memory pinned
+
+
+def _device_budget(dev):
+    """Device bytes a k-means fit may allocate: free memory once torch has returned its unused cached segments, less a
+    1 GiB margin for the allocator and other work on the device.  Cached bytes inside partly used segments are not
+    counted: a multi-GB allocation cannot be served from them."""
+    torch.cuda.empty_cache()
+    free, _ = torch.cuda.mem_get_info(dev)
+    return free - (1 << 30)
+
+
+def _stream_rounds(R, chunks, rows_per, P):
+    """The rounds of a streamed k-means pass over R rows split into `chunks` chunks of `rows_per` rows (the last may be
+    shorter; anyloc_kmeans_partition): round j holds rows [c*rows_per + j*P, c*rows_per + (j+1)*P) of every chunk c,
+    clipped to the chunk -> list of rounds, each a list of (first row, rows) per chunk.  Fed in order, the rounds give
+    every chunk its rows in row order, the order in which anyloc_kmeans_update sums them."""
+    rounds = []
+    for j in range(-(-rows_per // P)):
+        pieces = []
+        for c in range(chunks):
+            lo = c * rows_per + j * P
+            pieces.append((lo, max(0, min(R, (c + 1) * rows_per, lo + P) - lo)))
+        rounds.append(pieces)
+    return rounds
+
+
+def _kmeans_plan(R, D, chunks, rows_per, budget, copies, ws_bytes, stage_bytes):
+    """Where a fit on R host rows of dimension D runs, given `budget` free device bytes.  -> None: in memory, when
+    `copies` device copies of the rows plus `ws_bytes(R)` (workspaces and labels of an R-row pass) fit.  Else (P,
+    resident): streamed in rounds of P rows per chunk (a round fills a `stage_bytes` staging buffer), the first
+    `resident` rounds kept on the device after iteration 0 beside the labels of all rows and the round buffers."""
+    row = 4 * D
+    if copies * R * row + ws_bytes(R) <= budget:
+        return None
+    P = max(1, min(rows_per, stage_bytes // (chunks * row)))
+    n_rounds = -(-rows_per // P)
+    rr = chunks * P
+    fixed = ws_bytes(rr) + 4 * R + (1 + copies) * rr * row      # two transfer buffers, plus the normalised round
+    return P, int(max(0, min(n_rounds, (budget - fixed) // (rr * row))))
+
+
+def _host_fit_plan(X, dev, K, copies):
+    """_kmeans_plan for host rows X on `dev`; None (the in-memory fit) for device rows."""
+    if dev.type != "cuda" or X.is_cuda:
+        return None
+    lib = _lib.load()
+    R, D = X.shape
+    with torch.cuda.device(dev):
+        chunks, rows_per = _kmeans_partition(R, D)
+
+        def ws_bytes(n):
+            return (lib.anyloc_vlad_workspace_bytes(1, n, D, K) + lib.anyloc_kmeans_round_workspace_bytes(n, D, K) +
+                    4 * n)
+        return _kmeans_plan(R, D, chunks, rows_per, _device_budget(dev), copies, ws_bytes, _STAGE_BYTES)
+
+
+def _kmeans_partition(R, D):
+    """(chunks, rows_per) of anyloc_kmeans_update on the current device"""
+    chunks, rows_per = C.c_int(), C.c_int64()
+    _lib.check(_lib.load().anyloc_kmeans_partition(R, D, C.byref(chunks), C.byref(rows_per)), "anyloc_kmeans_partition")
+    return chunks.value, rows_per.value
+
+
 class _KMeans:
     """GPU stand-in for `fast_pytorch_kmeans.KMeans` as the reference uses it (utilities.py:766,
     :772, :786-787, :849): `.centroids`, `.fit(X)`, `.predict(X)`; cosine / euclidean similarity,
@@ -431,6 +496,9 @@ class _KMeans:
     def fit_predict(self, X, centroids=None):
         dev = _lib.require_cuda(X.device if X.is_cuda else None)
         was_cpu = not X.is_cuda
+        plan = _host_fit_plan(X, dev, self.n_clusters, copies=1)
+        if plan is not None:
+            return self._fit_streamed(X, centroids, False, plan, dev)
         x = _as_device_f32(X, dev)
         n, D = x.shape
         K = self.n_clusters
@@ -475,6 +543,95 @@ class _KMeans:
 
     def fit(self, X, centroids=None):
         self.fit_predict(X, centroids)
+
+    def _fit_streamed(self, X, centroids, normalize, plan, dev):
+        """fit_predict on host rows X [R,D] (any float dtype and strides) too large for the device, rows L2-normalised
+        first when `normalize` (VLAD.fit).  Each Lloyd pass feeds the rows in rounds of P rows per chunk of the
+        in-memory update (_stream_rounds), so centres and labels are bit-identical to the in-memory fit's.  The first
+        `resident` rounds are copied and normalised once, in iteration 0; the others cross the host link every
+        iteration through two pinned staging buffers, the copy of one round overlapping the device work on the one
+        before.  The shift is read after every iteration: a speculative extra pass would cost a full transfer."""
+        lib = _lib.load()
+        P, resident = plan
+        X = X.detach()
+        R, D = X.shape
+        K = self.n_clusters
+        with torch.cuda.device(dev):
+            chunks, rows_per = _kmeans_partition(R, D)
+            rounds = _stream_rounds(R, chunks, rows_per, P)
+            piece = [pcs[0][1] for pcs in rounds]                      # every chunk's piece but the last one's
+            sizes = [(chunks - 1) * pcs[0][1] + pcs[-1][1] for pcs in rounds]
+            offs = np.concatenate([[0], np.cumsum(sizes)]).tolist()
+            if centroids is None:
+                init = np.random.choice(R, size=[K], replace=False)      # the in-memory fit's draw
+                c = _as_device_f32(X[torch.from_numpy(init)], dev)
+                if normalize:
+                    c = _normalize_rows_dev(c)
+            else:
+                c = _as_device_f32(centroids, dev)
+            kept = torch.empty(offs[resident], D, device=dev)
+            raw = [torch.empty(sizes[0], D, device=dev) for _ in range(2)]
+            host = [torch.empty(sizes[0], D, pin_memory=True) for _ in range(2)]
+            ws = _lib.workspaces.get(dev, lib.anyloc_kmeans_round_workspace_bytes(R, D, K), "kmeans_upd")
+            cs, xs = torch.cuda.current_stream(), torch.cuda.Stream()
+            copied, freed = [None, None], [None, None]
+            transfers = ((it, j) for it in range(self.max_iter) for j in range(0 if it == 0 else resident, len(rounds)))
+            staged = []
+
+            def stage():
+                """gather the next transferred round into a staging buffer and queue its copy to the device"""
+                t = next(transfers, None)
+                if t is None:
+                    return
+                j, s = t[1], len(staged) & 1
+                if copied[s] is not None:
+                    copied[s].synchronize()                            # the staging buffer's previous copy is done
+                for ci, (lo, m) in enumerate(rounds[j]):
+                    host[s][ci * piece[j]:ci * piece[j] + m].copy_(X[lo:lo + m])
+                with torch.cuda.stream(xs):
+                    if freed[s] is not None:
+                        xs.wait_event(freed[s])
+                    raw[s][:sizes[j]].copy_(host[s][:sizes[j]], non_blocking=True)
+                    copied[s] = torch.cuda.Event()
+                    copied[s].record(xs)
+                staged.append((t, s, copied[s]))
+
+            stage()
+            taken = 0
+            for it in range(self.max_iter):
+                labels_r = []
+                for j in range(len(rounds)):
+                    x = kept[offs[j]:offs[j + 1]]
+                    if it == 0 or j >= resident:
+                        t, s, ev = staged[taken]
+                        taken += 1
+                        cs.wait_event(ev)
+                        x = raw[s][:sizes[j]]
+                        if normalize:
+                            x = _normalize_rows_dev(x)
+                        if j < resident:
+                            kept[offs[j]:offs[j + 1]].copy_(x)
+                    labels_r.append(self._assign(x, c))
+                    _lib.check(lib.anyloc_kmeans_accumulate_round(_lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j],
+                                                                  piece[j], D, K, int(j > 0), _lib.ptr(ws), ws.numel(),
+                                                                  _lib.stream_ptr()), "anyloc_kmeans_accumulate_round")
+                    if it == 0 or j >= resident:
+                        freed[s] = torch.cuda.Event()
+                        freed[s].record(cs)
+                        stage()
+                c_next, err = torch.empty_like(c), torch.zeros(1, device=dev)
+                _lib.check(lib.anyloc_kmeans_finalize(_lib.ptr(c), R, D, K, _lib.ptr(c_next), _lib.ptr(err),
+                                                      _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                           "anyloc_kmeans_finalize")
+                labels, c = labels_r, c_next
+                if float(err) <= self.tol:
+                    break
+            xs.synchronize()                                           # a round staged for an iteration not run
+            order = torch.from_numpy(np.concatenate([np.arange(lo, lo + m) for pcs in rounds for lo, m in pcs]))
+            out = torch.empty(R, dtype=torch.int64)
+            out[order] = torch.cat(labels).to(torch.int64).cpu()
+        self.centroids = c.cpu()
+        return out
 
 
 VLAD_KERNEL_DESCRIPTION = ("VLAD: gemm_tc3_kernel<false, 0> (wgmma tf32 coarse scores straight from the fp32 features) -> "
@@ -563,10 +720,14 @@ class VLAD:
             self.desc_dim = train_descs.shape[1]
         dev = _lib.require_cuda(train_descs.device if train_descs.is_cuda else None)
         was_cpu = not train_descs.is_cuda
-        x = _as_device_f32(train_descs, dev)
-        if self.norm_descs:
-            x = _normalize_rows_dev(x)
-        self.kmeans.fit(x)
+        plan = _host_fit_plan(train_descs, dev, self.num_clusters, copies=1 + bool(self.norm_descs))
+        if plan is not None:        # too large for the device: normalised round by round inside the streamed fit
+            self.kmeans._fit_streamed(train_descs, None, self.norm_descs, plan, dev)
+        else:
+            x = _as_device_f32(train_descs, dev)
+            if self.norm_descs:
+                x = _normalize_rows_dev(x)
+            self.kmeans.fit(x)
         self.c_centers = self.kmeans.centroids.cpu() if was_cpu else self.kmeans.centroids
         self.kmeans.centroids = self.c_centers
         if self.cache_dir is not None:

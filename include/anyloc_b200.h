@@ -134,6 +134,23 @@ size_t anyloc_kmeans_workspace_bytes(int R, int D, int K);
 int anyloc_kmeans_update(const float* x, const int32_t* labels, const float* old_centers, int R, int D,
                          int K, float* new_centers, float* err_out, void* ws, size_t ws_bytes,
                          void* stream);
+/* The same update in rounds, for rows that do not all fit on the device at once (VLAD.fit on host descriptors,
+ * utilities.py:749-791; fpk's Lloyd loop restated in oracle/fpk_restated.py).  anyloc_kmeans_update splits R rows
+ * into `chunks` contiguous chunks of `rows_per` rows (the last may be shorter) and sums each chunk sequentially;
+ * anyloc_kmeans_partition returns that partition (it depends on R, D and the device's SM count).
+ * anyloc_kmeans_accumulate_round takes one round: x [round_rows, D] and its labels hold, chunk after chunk, the next
+ * `piece_rows` rows of every chunk (the last chunk's piece is round_rows - (chunks-1)*piece_rows rows, possibly 0).
+ * resume=0 starts the per-chunk sums from zero, resume=1 continues those in the workspace.  After the last round,
+ * anyloc_kmeans_finalize writes new_centers and err_out as anyloc_kmeans_update would: feeding each chunk's rows in
+ * order, over any number of rounds, gives bit-identical centres.  R is the whole fit's row count in all three calls;
+ * both compute calls use one workspace of anyloc_kmeans_round_workspace_bytes(R, D, K) bytes. */
+int anyloc_kmeans_partition(int64_t R, int D, int* chunks, int64_t* rows_per);
+size_t anyloc_kmeans_round_workspace_bytes(int64_t R, int D, int K);
+int anyloc_kmeans_accumulate_round(const float* x, const int32_t* labels, int64_t R, int64_t round_rows,
+                                   int64_t piece_rows, int D, int K, int resume, void* ws, size_t ws_bytes,
+                                   void* stream);
+int anyloc_kmeans_finalize(const float* old_centers, int64_t R, int D, int K, float* new_centers, float* err_out,
+                           void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------- retrieval
  * Replaces the faiss part of get_top_k_recall (utilities.py:435-450): optional row
