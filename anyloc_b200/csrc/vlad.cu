@@ -11,7 +11,8 @@
 //   accumulate  : CTA per (image, 128-column slice), warps split the rows, float4 lanes:
 //                 sum_{label=k}(x^ - c_k) in shared memory, deterministic per-slice sums of squares
 //   normalise   : intra + global L2 normalisation, in place on the [B,K*D] output
-// (The v1 FFMA assignment kernel is kept for K > 256 / D > 2048 and as the k-means assignment step.)
+// (The v1 FFMA assignment kernel serves D > 2048, calls of fewer than 256 rows and workspaces without room for the
+// coarse scores, at any K.)
 #include <stdlib.h>
 #include <algorithm>
 #include <vector>
@@ -718,13 +719,18 @@ vlad_soft_assign_kernel(const float* __restrict__ x, const int32_t* __restrict__
     for (int i = 0; i < ROWS; ++i) {
       int64_t r = r0 + i;
       if (r >= R) continue;
+      if (!valid[i]) {        // padded row of a ragged batch: exactly 0, whatever it holds (its scores may be NaN)
+        for (int k = lane; k < K; k += 32) assign[r * K + k] = 0.f;
+        if (lane == 0 && inv_norm) inv_norm[r] = 0.f;
+        continue;
+      }
       float m = -INFINITY;
       for (int k = lane; k < K; k += 32) m = fmaxf(m, sc[i * K + k]);
       m = warp_max(m);
       float z = 0.f;
       for (int k = lane; k < K; k += 32) { float e = expf(sc[i * K + k] - m); sc[i * K + k] = e; z += e; }
       z = warp_sum(z);
-      const float iz = valid[i] ? 1.0f / z : 0.f;       // padded rows of ragged batches carry no weight
+      const float iz = 1.0f / z;
       for (int k = lane; k < K; k += 32) assign[r * K + k] = sc[i * K + k] * iz;
       if (lane == 0 && inv_norm) inv_norm[r] = 1.0f / fmaxf(ss[i], 1e-12f);
     }
@@ -734,20 +740,23 @@ vlad_soft_assign_kernel(const float* __restrict__ x, const int32_t* __restrict__
 
 // V[b,k,:] = sum_q a[q,k] * sum_c (x^_q - c_c) = K * sum_q a[q,k] x^_q - (sum_q a[q,k]) * sum_c c_c
 // (the reference sums cluster k's weight over the residuals to ALL centres, utilities.py:881-884).
-// CTA = (128-column slice, image); thread = column; KC cluster accumulators in registers per pass.
+// CTA = (128-column slice, image); thread = column; KC cluster accumulators in registers per pass.  Only the image's
+// first n_valid[b] rows are read: a padded row's weight is 0, but 0 * NaN would not be.
 constexpr int SOFT_KC = 32, SOFT_QT = 64;
 __global__ void __launch_bounds__(ACC_COLS)
-vlad_soft_accumulate_kernel(const float* __restrict__ x, const float* __restrict__ assign,
-                            const float* __restrict__ inv_norm, const float* __restrict__ centers, int N, int D, int K,
-                            int norm_descs, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid,
+                            const float* __restrict__ assign, const float* __restrict__ inv_norm,
+                            const float* __restrict__ centers, int N_per_img, int D, int K, int norm_descs,
+                            float* __restrict__ vlad, float* __restrict__ partial_ss) {
   __shared__ __align__(16) float a_tile[SOFT_QT][SOFT_KC];
   __shared__ float inv_tile[SOFT_QT];
   __shared__ float red[ACC_COLS / 32][SOFT_KC];
   const int t = threadIdx.x, slice = blockIdx.x, b = blockIdx.y, nslices = gridDim.x;
   const int col = slice * ACC_COLS + t;
   const bool colok = col < D;
-  const float* xb = x + (size_t)b * N * D;
-  const float* ab = assign + (size_t)b * N * K;
+  const int N = n_valid ? min(N_per_img, max(0, n_valid[b])) : N_per_img;
+  const float* xb = x + (size_t)b * N_per_img * D;
+  const float* ab = assign + (size_t)b * N_per_img * K;
   float csum = 0.f;
   if (colok) for (int c = 0; c < K; ++c) csum += __ldg(centers + (size_t)c * D + col);
   for (int k0 = 0; k0 < K; k0 += SOFT_KC) {
@@ -764,7 +773,7 @@ vlad_soft_accumulate_kernel(const float* __restrict__ x, const float* __restrict
         a_tile[q][j] = (q < qn && j < kc) ? __ldg(ab + (size_t)(q0 + q) * K + k0 + j) : 0.f;
       }
       for (int q = t; q < SOFT_QT; q += ACC_COLS)
-        inv_tile[q] = (q < qn) ? (norm_descs ? inv_norm[(size_t)b * N + q0 + q] : 1.0f) : 0.f;
+        inv_tile[q] = (q < qn) ? (norm_descs ? inv_norm[(size_t)b * N_per_img + q0 + q] : 1.0f) : 0.f;
       __syncthreads();
       if (t < SOFT_KC) for (int q = 0; q < qn; ++q) wsum += a_tile[q][t];
       if (colok) {
@@ -1123,8 +1132,8 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
     return ANYLOC_OK;
   }
   // v2: accumulate with as many row-splitting warps as shared memory allows ((1 + warps) * K * 128 floats), at most
-  // 4 row-splitting warps when two CTAs then fit per SM, else what fits in one
-  int warps = (int)std::min<size_t>(4, (200 * 1024) / ((size_t)K * 128 * 4) - 1);
+  // 4 row-splitting warps when two CTAs then fit per SM, else what fits in one (signed: K > 400 leaves none)
+  int warps = (int)std::min<long long>(4, (long long)((200 * 1024) / ((size_t)K * 128 * 4)) - 1);
   if (warps >= 1) {
     size_t smem = (size_t)(1 + warps) * K * 128 * 4;
     ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1219,8 +1228,8 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, n_valid, N, (int64_t)R, D, K, chat,
                                                                        soft_temp, assign, inv_norm);
   ANYLOC_CHECK_LAUNCH();
-  vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, assign, inv_norm, centers, N, D, K,
-                                                                    norm_descs, vlad, partial);
+  vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N, D,
+                                                                    K, norm_descs, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
   int ysplit = std::max(1, std::min(64, (int)(((size_t)K * D + 256 * 16 - 1) / (256 * 16))));
   vlad_normalize_kernel<<<dim3(B, ysplit), 256, 2 * K * sizeof(float), st>>>(vlad, partial, D, K, nslices,
