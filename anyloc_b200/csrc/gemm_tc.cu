@@ -11,7 +11,9 @@
 //                 from shared memory into registers.  The tensor core's fp32 accumulation is not round-to-nearest, a
 //                 bias that grows with K, so the wgmmas only accumulate a CHUNK of k-blocks; each chunk is then added
 //                 (round-to-nearest) into a second register accumulator that holds the whole 64 x 128 sub-tile.  After
-//                 the last chunk: bias / GELU / SwiGLU / LayerScale+residual / pair split, stored from registers.
+//                 the last chunk: bias / GELU / SwiGLU / LayerScale+residual / pair split, staged in shared memory
+//                 subtile by subtile and stored with TMA (epilogue_staged), so the stores drain behind the next
+//                 tile's mainloop.  The hi-only passes, and outputs TMA cannot store, are stored from registers.
 // Tiles are rastered in bands of BAND_N column blocks, n-fastest inside a band: the resident CTAs share a few A row
 // panels and one band of B that stays in L2 while the outputs stream through.
 #include <cuda.h>
@@ -28,6 +30,7 @@ constexpr int KSTEPS = 4;                  // wgmma k-steps per 128-byte k-block
 constexpr int A_BYTES = BM * 128;          // 16 KB: 128 rows x 128 B
 constexpr int B_BYTES = BN * 128;          // 16 KB
 constexpr int THREADS = 384;
+constexpr int STG_BYTES = 8192;            // one epilogue staging buffer (see epilogue_staged)
 
 // LO = true : stages hold {A_hi, A_lo, B_hi, B_lo} (3-term split, 64 KB).  LO = false: hi-only single pass (coarse
 // scores): {A_hi, B_hi} = 32 KB per stage -> twice the pipeline depth in the same shared memory.
@@ -36,7 +39,15 @@ template <bool LO> struct Cfg {
   static constexpr int STAGE_BYTES = (LO ? 2 : 1) * (A_BYTES + B_BYTES);
   static constexpr int B_OFF = (LO ? 2 : 1) * A_BYTES;
   static constexpr int STAGES = LO ? 3 : 6;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;          // mbarriers (< 256 B)
+  static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024 /*align*/;
+  // epilogue staging buffers (2 per consumer warpgroup), 3-term passes only.  The hi-only coarse passes keep the
+  // register epilogue, a small share of their time: with the staged path compiled in, their mainloop ran slower
+  // (H100, retrieval coarse pass with the epilogue discarded: 2.46 -> 2.65 ms).  A launch that does not stage asks
+  // for SMEM_BYTES only, the staged ones for SMEM_BYTES_STAGED.
+  static constexpr bool STAGED = LO;
+  static constexpr int STG_OFF = BAR_OFF + 1024;
+  static constexpr int SMEM_BYTES_STAGED = STG_OFF + 4 * STG_BYTES + 1024 /*align*/;
 };
 constexpr int CHUNK_KB_TF32 = 2;           // k-blocks accumulated by the tensor core between two round-to-nearest adds
 constexpr int CHUNK_KB_F16 = 8;            // (24 / 96 wgmma k-steps per chunk)
@@ -96,25 +107,30 @@ __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int 
   }
 }
 
-// Epilogue of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16),
-// accumulators in the wgmma layout.  Applied pair by pair (epi_pair), every bias / gamma / residual load sits between
-// the previous pair's store and this pair's, so the thread waits for one memory round trip per pair -- 32 per tile.
-// Where every column pair of the tile lies inside N (and, except for SwiGLU, ldo is even), the loads of 2 column pairs
-// (both rows) are issued together ahead of their stores instead: 8 round trips per tile.  Same values, same
-// arithmetic.  (Groups of 4 or 8 pairs exceed the 168 registers a thread has here and spill.)
-__device__ __forceinline__ void epilogue_subtile(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
+// Register epilogue of the 3-term passes that do not stage (gated launches, outputs TMA cannot store: see
+// make_epi_maps) of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16), accumulators in the wgmma layout,
+// applied and stored pair by pair.
+__device__ __forceinline__ void epilogue_pairs(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int n = nq + j * 8;
+    if (n >= N) continue;
+    if (r0 < M) epi_pair(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
+    if (r0 + 8 < M) epi_pair(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
+  }
+}
+
+// Register epilogue of the hi-only passes (the VLAD and retrieval coarse scores): where every column pair of the tile
+// lies inside N (and, except for SwiGLU, ldo is even), the bias / gamma / residual loads of 2 column pairs (both rows)
+// are issued together ahead of their stores -- 8 memory round trips per thread and tile instead of 32 -- otherwise
+// pair by pair.  Same values, same arithmetic as epilogue_pairs.  (Groups of 4 or 8 pairs spill.)
+__device__ __forceinline__ void epilogue_regs_batched(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
   const int mode = ep.mode;
   if (mode < 0) return;                    // diagnostic: discard (ANYLOC_GEMM_DEBUG_SKIP_EPI)
   const int n0 = nq & ~(BN - 1);
   const bool swiglu = mode == ANYLOC_EPI_SWIGLU_SPLIT, resid = mode == ANYLOC_EPI_LS_RESID;
   if (n0 + BN > N || (!swiglu && (ep.ldo & 1))) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int n = nq + j * 8;
-      if (n >= N) continue;
-      if (r0 < M) epi_pair(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
-      if (r0 + 8 < M) epi_pair(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
-    }
+    epilogue_pairs(ep, r0, nq, M, N, sum);
     return;
   }
   const bool row0 = r0 < M, row1 = r0 + 8 < M;
@@ -163,21 +179,157 @@ __device__ __forceinline__ void epilogue_subtile(const EpiParams& ep, int r0, in
   }
 }
 
+// ------------------------------------------------------------------ staged epilogue
+// Output formats of the staged path.  A subtile is 64 rows x COLS output columns; one 8 KB staging buffer holds it:
+// 64 x 32 fp32, or the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs.
+enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2 };
+constexpr int STG_HALF = STG_BYTES / 2;    // offset of the lo array (pair formats)
+constexpr int STG_ROWS = 64;               // TMA box rows of the output maps: one consumer warpgroup's rows
+
+template <int KIND>
+struct StageFmt {
+  static constexpr int ESZ = KIND == STG_F16_PAIR ? 2 : 4;
+  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : 32;     // output columns per subtile
+  static constexpr int ROW_BYTES = COLS * ESZ;                       // 128 (fp32) or 64 bytes per row of one array
+  static constexpr uint32_t SWZ = ROW_BYTES == 128 ? 7 : 3;          // TMA SWIZZLE_128B / SWIZZLE_64B
+};
+
+// Byte offset of byte b of staging row `row`, placed as TMA's SWIZZLE_128B / _64B expects it: the 16-byte chunk index
+// XOR offset bits 7.. .  The 8 rows that one warp's store instruction covers land in distinct banks.
+template <int KIND>
+__device__ __forceinline__ uint32_t stg_off(int row, int b) {
+  const uint32_t o = (uint32_t)(row * StageFmt<KIND>::ROW_BYTES + b);
+  return o ^ (((o >> 7) & StageFmt<KIND>::SWZ) << 4);
+}
+
+// bias / gamma of columns (n, n+1); columns at or past N (which TMA clips) read nothing
+__device__ __forceinline__ float2 ldg_col_pair(const float* p, int n, int N) {
+  if (n + 1 < N) return __ldg(reinterpret_cast<const float2*>(p + n));
+  return make_float2(n < N ? __ldg(p + n) : 0.f, 0.f);
+}
+
+// TMA load of the residual subtile (64 rows from m0, 32 fp32 columns from oc) into a staging buffer
+__device__ __forceinline__ void resid_load(const CUtensorMap* tm, uint8_t* buf, uint64_t* bar, int oc, int m0) {
+  mbar_expect_tx(smem_u32(bar), STG_BYTES);
+  tma_load_2d(smem_u32(buf), tm, smem_u32(bar), oc, m0);
+}
+
+// Staged epilogue of one consumer warpgroup's 64 x 128 sub-tile (rows from m0, accumulator columns from n0), one
+// subtile at a time: every thread applies the epilogue to its accumulators of the subtile and writes the results into
+// the warpgroup's staging buffer -- for LS_RESID the buffer already holds the TMA-loaded residual and is updated in
+// place -- then, after a proxy fence and the warpgroup's named barrier, one thread stores the buffer with TMA, which
+// clips the M and N tails.  The stores drain while the warpgroup works on the next subtile and the next tile's
+// mainloop.  Two buffers alternate (running subtile count `cnt`); a buffer is rewritten only once the store issued
+// from it has read it (waited before the barrier of the subtile in between).  Same arithmetic as epi_pair.
+template <int KIND, bool SWIGLU, bool RESID>
+__device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUtensorMap* tm_out, const CUtensorMap* tm_lo,
+                                                const CUtensorMap* tm_resid, uint8_t* stg, uint64_t* rbar,
+                                                uint32_t& rphase, uint32_t& cnt, int wg, int t, int m0, int n0, int N,
+                                                const float* sum) {
+  using F = StageFmt<KIND>;
+  constexpr int ACC = SWIGLU ? 2 * F::COLS : F::COLS;    // accumulator columns per subtile
+  constexpr int JS = ACC / 8;                             // 8-column accumulator groups per subtile
+  const int lane = t & 31, q = lane & 3, row = (t >> 5) * 16 + (lane >> 2);
+  const int n_out = SWIGLU ? N >> 1 : N;
+  const int oc_base = SWIGLU ? n0 >> 1 : n0;
+  const bool gelu = ep.mode == ANYLOC_EPI_GELU_SPLIT;
+  const float al = ep.alpha;
+#pragma unroll
+  for (int s = 0; s < BN / ACC; ++s) {
+    const int oc0 = oc_base + s * F::COLS;
+    if (oc0 >= n_out) break;
+    const uint32_t b = cnt & 1;
+    uint8_t* buf = stg + b * STG_BYTES;
+    if (RESID) { mbar_wait(smem_u32(rbar + b), (rphase >> b) & 1); rphase ^= 1u << b; }
+#pragma unroll
+    for (int jj = 0; jj < JS; ++jj) {
+      const int j = s * JS + jj, n = n0 + j * 8 + 2 * q;
+      const float2 bb = ep.bias ? ldg_col_pair(ep.bias, n, N) : make_float2(0.f, 0.f);
+      float2 g;
+      if (RESID) g = ldg_col_pair(ep.gamma, n, N);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = row + 8 * h;
+        const float x0 = sum[4 * j + 2 * h] * al + bb.x, x1 = sum[4 * j + 2 * h + 1] * al + bb.y;
+        if (SWIGLU) {                      // (x1_j, x2_j) = columns (n, n+1) -> output column n/2
+          const float v = silu(x0) * x1;
+          const uint32_t o = stg_off<KIND>(r, (4 * jj + q) * F::ESZ);
+          if (KIND == STG_F16_PAIR) {
+            __half hi, lo;
+            split_f16(v * kActScale, hi, lo);
+            *reinterpret_cast<__half*>(buf + o) = hi;
+            *reinterpret_cast<__half*>(buf + STG_HALF + o) = lo;
+          } else {
+            float hi, lo;
+            split_tf32(v, hi, lo);
+            *reinterpret_cast<float*>(buf + o) = hi;
+            *reinterpret_cast<float*>(buf + STG_HALF + o) = lo;
+          }
+          continue;
+        }
+        const uint32_t o = stg_off<KIND>(r, (8 * jj + 2 * q) * F::ESZ);
+        if (KIND == STG_F32) {
+          float2* p = reinterpret_cast<float2*>(buf + o);
+          if (RESID) {
+            const float2 rr = *p;
+            *p = make_float2(rr.x + g.x * x0, rr.y + g.y * x1);
+          } else {
+            *p = make_float2(x0, x1);
+          }
+        } else {
+          const float y0 = gelu ? gelu_erf(x0) : x0, y1 = gelu ? gelu_erf(x1) : x1;
+          if (KIND == STG_F16_PAIR) {
+            uint32_t hi, lo;
+            split_f16x2(y0 * kActScale, y1 * kActScale, hi, lo);
+            *reinterpret_cast<uint32_t*>(buf + o) = hi;
+            *reinterpret_cast<uint32_t*>(buf + STG_HALF + o) = lo;
+          } else {
+            float2 hi, lo;
+            split_tf32(y0, hi.x, lo.x); split_tf32(y1, hi.y, lo.y);
+            *reinterpret_cast<float2*>(buf + o) = hi;
+            *reinterpret_cast<float2*>(buf + STG_HALF + o) = lo;
+          }
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    if (t == 0) bulk_wait_read<0>();       // the previous subtile's store has read the other buffer: free after the barrier
+    if (wg == 1) named_bar_sync<1>(128);    // the warpgroup's own barrier (0 is __syncthreads')
+    else named_bar_sync<2>(128);
+    if (t == 0) {
+      tma_store_2d(tm_out, smem_u32(buf), oc0, m0);
+      if (KIND != STG_F32) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
+      bulk_commit();
+      if (RESID && s + 2 < BN / ACC && oc0 + 2 * F::COLS < n_out) {
+        // residual of subtile s + 2 into this buffer, once the store has read it
+        bulk_wait_read<0>();
+        resid_load(tm_resid, buf, rbar + b, oc0 + 2 * F::COLS, m0);
+      }
+    }
+    ++cnt;
+  }
+}
+
 // F16 = false: operands are fp32 words read as tf32 (32 elements per 128 B k-block, wgmma K=8)
 // F16 = true : operands are fp16            (64 elements per 128 B k-block, wgmma K=16, 2x rate)
 // ep.gate (nullable): the kernel returns at once when *gate == 0 (conditional fallbacks without a host sync).
+// staged != 0: the epilogue goes through shared memory and TMA stores (tm_out, tm_out_lo for the pair formats,
+// tm_resid for LS_RESID: (n_out, M) maps with 64-row boxes); 0: stored pair by pair from registers.
 template <bool F16, int LOM>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                const __grid_constant__ CUtensorMap tm_out, const __grid_constant__ CUtensorMap tm_out_lo,
+                const __grid_constant__ CUtensorMap tm_resid, int staged,
                 int M, int N, int K, int band_n, int chunk_kb, EpiParams ep) {
   constexpr bool LO = LOM != 0, has_a_lo = (LOM & 1) != 0, has_b_lo = (LOM & 2) != 0;
   using C = Cfg<LO>;
   if (ep.gate != nullptr && *reinterpret_cast<const volatile int*>(ep.gate) == 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);   // [STAGES]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);                    // [STAGES]
   uint64_t* empty_bar = full_bar + C::STAGES;                                             // [STAGES]
+  uint64_t* resid_bar = empty_bar + C::STAGES;                   // [2 per consumer warpgroup]: residual subtile landed
 
   const int wg = threadIdx.x >> 7;
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
@@ -189,6 +341,8 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_hi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_hi) : "memory");
     for (int s = 0; s < C::STAGES; ++s) { mbar_init(smem_u32(full_bar + s), 1); mbar_init(smem_u32(empty_bar + s), 2); }
+    if (C::STAGED)
+      for (int i = 0; i < 4; ++i) mbar_init(smem_u32(resid_bar + i), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -220,6 +374,12 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   // ---------------------------------------- consumers: rows [64 (wg-1), +64) of the tile
   const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
   const uint32_t a_sub = (uint32_t)(wg - 1) * 64 * 128;       // byte offset of this warpgroup's 64 A rows
+  uint8_t* stg = smem + C::STG_OFF + (wg - 1) * 2 * STG_BYTES;  // this warpgroup's two staging buffers
+  uint64_t* rbar = resid_bar + (wg - 1) * 2;
+  const int mode = ep.mode;
+  staged = C::STAGED && staged;
+  const bool resid_staged = staged && mode == ANYLOC_EPI_LS_RESID;
+  uint32_t stg_cnt = 0, rphase = 0;                           // staged subtiles so far; resid_bar parities
   int stage = 0; uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int mb, nb; tile_coords(tile, num_m, num_n, band_n, mb, nb);
@@ -230,6 +390,16 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
     int prev_stage = -1;
     for (int kb0 = 0; kb0 < num_k; kb0 += chunk_kb) {
       const int kb1 = min(num_k, kb0 + chunk_kb);
+      if (resid_staged && kb1 == num_k && t == 0 && m0 < M) {
+        // the last chunk starts: fetch the residual of the first two subtiles into the staging buffers, which the
+        // previous tile's stores have finished reading by now
+        bulk_wait_read<0>();
+        for (int i = 0; i < 2; ++i) {
+          const uint32_t b = (stg_cnt + i) & 1;
+          const int oc = n0 + i * StageFmt<STG_F32>::COLS;
+          if (oc < N) resid_load(&tm_resid, stg + b * STG_BYTES, rbar + b, oc, m0);
+        }
+      }
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(smem_u32(full_bar + stage), phase);
         const uint32_t sbase = smem_u32(smem + stage * C::STAGE_BYTES);
@@ -257,8 +427,30 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       for (int j = 0; j < 64; ++j) sum[j] += acc[j];
     }
     if (t == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
-    epilogue_subtile(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+    if (mode < 0 || m0 >= M) continue;       // discard (ANYLOC_GEMM_DEBUG_SKIP_EPI) / no rows for this warpgroup
+    if constexpr (!C::STAGED) {
+      epilogue_regs_batched(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      continue;
+    }
+    if (!staged) {
+      epilogue_pairs(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      continue;
+    }
+#define ANYLOC_EPI_STAGED(KIND_, SWIGLU_, RESID_)                                                                   \
+  epilogue_staged<KIND_, SWIGLU_, RESID_>(ep, &tm_out, &tm_out_lo, &tm_resid, stg, rbar, rphase, stg_cnt, wg, t, m0, \
+                                          n0, N, sum)
+    if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(STG_F32, false, false);
+    else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(STG_F32, false, true);
+    else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
+      if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, true, false);
+      else ANYLOC_EPI_STAGED(STG_TF32_PAIR, true, false);
+    } else {                                 // BIAS_SPLIT / GELU_SPLIT
+      if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, false, false);
+      else ANYLOC_EPI_STAGED(STG_TF32_PAIR, false, false);
+    }
+#undef ANYLOC_EPI_STAGED
   }
+  if (staged && t == 0) bulk_wait<0>();     // the last stores complete before the CTA exits
 }
 
 // ------------------------------------------------------------------ host side
@@ -294,6 +486,45 @@ int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box
   return ANYLOC_OK;
 }
 
+// output map of the staged epilogue: [rows, cols] of esz-byte elements, row pitch ld, boxes of 64 rows x box_cols
+// swizzled as stg_off places them.  TMA clips the boxes at rows and cols, so the ld padding is never written.
+static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int esz, int box_cols) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)STG_ROWS};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr,
+                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   box_cols * esz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("gemm_tc: cuTensorMapEncodeTiled failed (%d) for the output: rows=%d cols=%d ld=%d", (int)r, rows, cols, ld); return ANYLOC_ERR_CUDA; }
+  return ANYLOC_OK;
+}
+
+// Output maps of the staged epilogue.  *staged = false (maps zeroed) where the result is discarded or TMA cannot
+// store the output: row pitch or row length not a multiple of 16 bytes (the start addresses are 16-byte aligned by
+// gemm_tc_supported).  The row-length condition is conservative: in one H100 run of the staged-path test without it,
+// a 68-column fp16 output (136 bytes per row) came back with its ldo padding columns 68..71 written, as if the store
+// clipped columns only to 16-byte units.  Not reproduced since (the condition keeps such shapes off the staged path).
+static int make_epi_maps(const EpiParams& ep, int M, int N, CUtensorMap* m_out, CUtensorMap* m_lo, CUtensorMap* m_resid,
+                         bool* staged) {
+  memset(m_out, 0, sizeof(*m_out)); memset(m_lo, 0, sizeof(*m_lo)); memset(m_resid, 0, sizeof(*m_resid));
+  const bool split = ep.mode == ANYLOC_EPI_BIAS_SPLIT || ep.mode == ANYLOC_EPI_GELU_SPLIT ||
+                     ep.mode == ANYLOC_EPI_SWIGLU_SPLIT;
+  const int esz = split && ep.out_f16 ? 2 : 4;
+  const int n_out = ep.mode == ANYLOC_EPI_SWIGLU_SPLIT ? N / 2 : N;
+  *staged = ep.mode >= 0 && ((long long)ep.ldo * esz) % 16 == 0 && ((long long)n_out * esz) % 16 == 0;
+  if (!*staged) return ANYLOC_OK;
+  const int cols = split && !ep.out_f16 ? StageFmt<STG_TF32_PAIR>::COLS : StageFmt<STG_F32>::COLS;
+  int rc;
+  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols))) return rc;
+  if (split && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
+  if (ep.mode == ANYLOC_EPI_LS_RESID && (rc = make_out_map(m_resid, ep.resid, M, n_out, ep.ldo, esz, cols))) return rc;
+  return ANYLOC_OK;
+}
+
 }  // namespace tc
 
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb,
@@ -309,6 +540,9 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
   return true;
 }
 
+// epilogue of this host thread's last launch (anyloc_gemm_tc_last_staged)
+static thread_local int g_last_staged = -1;
+
 template <bool F16, int LOM>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                        int N, int K, const EpiParams& ep, int band_n, int chunk, cudaStream_t st) {
@@ -320,15 +554,24 @@ static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* 
   if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16))) return rc;
   if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16))) return rc;
   if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16))) return rc;
+  CUtensorMap mo, mo_lo, mr;
+  bool staged = false;
+  memset(&mo, 0, sizeof(mo)); memset(&mo_lo, 0, sizeof(mo_lo)); memset(&mr, 0, sizeof(mr));
+  // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
+  // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
+  // for more would make the SM switch its shared-memory configuration back and forth).
+  if (Cfg<LO>::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged))) return rc;
+  const int smem = staged ? Cfg<LO>::SMEM_BYTES_STAGED : Cfg<LO>::SMEM_BYTES;
+  g_last_staged = staged ? 1 : 0;
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen)) {
     ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<LO>::SMEM_BYTES));
+                                           Cfg<LO>::STAGED ? Cfg<LO>::SMEM_BYTES_STAGED : Cfg<LO>::SMEM_BYTES));
   }
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
-  gemm_tc3_kernel<F16, LOM><<<grid, THREADS, Cfg<LO>::SMEM_BYTES, st>>>(
-      ma_hi, ma_lo, mb_hi, mb_lo, M, N, K, std::min(band_n, cdiv(N, BN)), chunk, ep);
+  gemm_tc3_kernel<F16, LOM><<<grid, THREADS, smem, st>>>(
+      ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(band_n, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -365,3 +608,5 @@ int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi
 }
 
 }  // namespace anyloc
+
+extern "C" int anyloc_gemm_tc_last_staged(void) { return anyloc::g_last_staged; }

@@ -39,6 +39,26 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
 
+// TMA store of a box from shared memory (bulk-group completion), and the bulk-group bookkeeping around it
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed bulk group but the newest N has finished reading its shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every committed bulk group but the newest N has completed (its global writes performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// orders this thread's generic-proxy shared-memory accesses before later async-proxy (TMA) accesses
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier ID over `count` threads (id 0 is __syncthreads')
+template <int ID>
+__device__ __forceinline__ void named_bar_sync(int count) {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(count) : "memory");
+}
+
 // wgmma matrix descriptor: K-major, 128B swizzle (8-row x 128 B atoms, 1024 B apart = SBO; LBO unused for swizzled
 // K-major operands), layout type 1 = SWIZZLE_128B.  A k-step of 32 bytes inside the atom advances the start address.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {

@@ -249,6 +249,9 @@ int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const void* b_hi
                    int ldb, int M, int N, int K, int in_dtype, float alpha, int epilogue, const float* bias,
                    const float* gamma, const float* resid, void* out, void* out_lo, int ldo, int out_dtype,
                    int engine, void* stream);
+/* which epilogue the calling thread's last tensor-core GEMM launch used: 1 = staged through shared memory and TMA
+ * stores, 0 = stored from registers, -1 = none launched yet (a test observable; no effect on results) */
+int anyloc_gemm_tc_last_staged(void);
 int anyloc_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stream);
 int anyloc_split_f16(const float* x, void* hi, void* lo, size_t n, float scale, void* stream);
 int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D, float eps,
