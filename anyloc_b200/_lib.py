@@ -19,6 +19,8 @@ EPI = {"bias": 0, "bias_split": 1, "gelu_split": 2, "swiglu_split": 3, "ls_resid
 ENGINE = {"auto": 0, "simt": 1, "tc3": 2}
 PAIR = {"tf32": 0, "f16": 1}
 ACT_SCALE = 8.0     # kActScale in csrc/common.cuh
+VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_extract_varlen call
+ERR = {"arg": -1, "cuda": -2, "workspace": -3, "unsupported": -4}
 
 
 class AnylocError(RuntimeError):
@@ -98,6 +100,11 @@ _SIGS = {
     "anyloc_vit_extract": (C.c_int, [C.POINTER(VitCfg), C.POINTER(VitWeightsStruct), C.c_void_p,
                                      C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "anyloc_vit_varlen_workspace_bytes": (C.c_size_t, [C.POINTER(VitCfg), C.c_int, C.POINTER(C.c_int32)]),
+    "anyloc_vit_extract_varlen": (C.c_int, [C.POINTER(VitCfg), C.POINTER(VitWeightsStruct), C.c_int,
+                                            C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_void_p),
+                                            C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+                                            C.c_int, C.c_void_p]),
     "anyloc_gemm_nt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                  C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),

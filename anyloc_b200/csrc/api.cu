@@ -3,6 +3,7 @@
 // /root/reference/utilities.py:245-252,263-285 + upstream DinoVisionTransformer).
 #include <stdarg.h>
 #include <string.h>
+#include <algorithm>
 #include <atomic>
 #include <vector>
 #include "epilogue.cuh"
@@ -66,6 +67,11 @@ int launch_l2norm(const float*, int64_t, int, int64_t, float*, cudaStream_t);
 int attention_launch(const float*, const float*, int, int, int, int, void*, void*, bool, cudaStream_t);
 int attention_tc_launch(const void*, const void*, int, int, int, int, void*, void*, bool, cudaStream_t);
 int attention_tc16_standalone(const float*, const float*, int, int, int, int, void*, void*, cudaStream_t);
+int attention_tc_varlen_launch(const void*, const void*, const VarlenAttnTable&, int, int, int, void*, void*, bool,
+                               cudaStream_t);
+int launch_im2col_varlen(const VarlenImgTable&, int, int, int, void*, void*, bool, cudaStream_t);
+int launch_assemble_varlen(const float*, const float*, const VarlenImgTable&, int, int, float*, cudaStream_t);
+int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, int, int, int, int, float*, cudaStream_t);
 
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                          int ldb, int M, int N, int K, const EpiParams& ep, int engine, bool f16, cudaStream_t st) {
@@ -221,13 +227,13 @@ namespace {
 struct VitBuffers {
   float *pa_hi, *pa_lo, *ptmp, *x, *y_hi, *y_lo, *qkv, *qkv_lo, *h_hi, *h_lo;
 };
-size_t vit_carve(const AnylocVitCfg* c, int B, int H, int W, void* ws, size_t ws_bytes, VitBuffers* out) {
-  const int P = c->patch, N = (H / P) * (W / P), T = N + 1, D = c->embed_dim, Kp = anyloc_vit_patch_k(P);
-  const size_t M = (size_t)B * T;
+// n_patch patch rows and M token rows in all
+size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, void* ws, size_t ws_bytes, VitBuffers* out) {
+  const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   VitBuffers b;
-  b.pa_hi = w.take<float>((size_t)B * N * Kp); b.pa_lo = w.take<float>((size_t)B * N * Kp);
-  b.ptmp = w.take<float>((size_t)B * N * D);
+  b.pa_hi = w.take<float>(n_patch * Kp); b.pa_lo = w.take<float>(n_patch * Kp);
+  b.ptmp = w.take<float>(n_patch * D);
   b.x = w.take<float>(M * D);
   b.y_hi = w.take<float>(M * D); b.y_lo = w.take<float>(M * D);
   b.qkv = w.take<float>(M * 3 * D); b.qkv_lo = w.take<float>(M * 3 * D);
@@ -236,6 +242,19 @@ size_t vit_carve(const AnylocVitCfg* c, int B, int H, int W, void* ws, size_t ws
   if (ws && (!b.pa_hi || !b.pa_lo || !b.ptmp || !b.x || !b.y_hi || !b.y_lo || !b.qkv || !b.qkv_lo || !b.h_hi || !b.h_lo)) return 0;
   return w.off;
 }
+size_t vit_carve(const AnylocVitCfg* c, int B, int H, int W, void* ws, size_t ws_bytes, VitBuffers* out) {
+  const size_t N = (size_t)(H / c->patch) * (W / c->patch);
+  return vit_carve(c, B * N, B * (N + 1), ws, ws_bytes, out);
+}
+
+// The sequences the attention runs over: B images of T tokens each, or (tab != nullptr) the packed images of a
+// variable-length call, n_tiles 64-query tiles in all
+struct VitSeqs {
+  int B, T;
+  const VarlenAttnTable* tab;
+  int n_tiles;
+  double attn_flops;
+};
 }  // namespace
 
 extern "C" size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W) {
@@ -243,9 +262,9 @@ extern "C" size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int
   return vit_carve(cfg, B, H, W, nullptr, 0, nullptr) + 4096;
 }
 
-static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitBuffers& bf, int B, int T,
+static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitBuffers& bf, int M, const VitSeqs& sq,
                      int engine, cudaStream_t st) {
-  const int D = c->embed_dim, M = B * T, Hf = c->ffn_hidden;
+  const int D = c->embed_dim, Hf = c->ffn_hidden;
   const bool f16 = c->pair_dtype == ANYLOC_PAIR_F16;
   int rc;
   const double ln_bytes = (f16 ? 8.0 : 12.0) * M * D;
@@ -258,8 +277,15 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   e_qkv.out_f16 = f16_attn;
   e_qkv.alpha = wb.qkv_alpha;
   if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
-  if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, B, T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine, st, f16_attn)))
+  if (sq.tab) {
+    ProfScope ps(PC_ATTENTION, st, sq.attn_flops);
+    if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, bf.y_hi, bf.y_lo,
+                                         f16, st)))
+      return rc;
+  } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine,
+                                      st, f16_attn))) {
     return rc;
+  }
   EpiParams e_proj{ANYLOC_EPI_LS_RESID, wb.proj_b, wb.ls1, bf.x, bf.x, nullptr, D};
   e_proj.alpha = wb.proj_alpha;
   if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.proj_w_hi, wb.proj_w_lo, D, M, D, D, e_proj, engine, f16, st))) return rc;
@@ -273,6 +299,30 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   EpiParams e_out{ANYLOC_EPI_LS_RESID, wb.out_b, wb.ls2, bf.x, bf.x, nullptr, D};
   e_out.alpha = wb.out_alpha;
   return gemm_dispatch(bf.h_hi, bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf, e_out, engine, f16, st);
+}
+
+// Blocks 0..layer-1 over the M assembled token rows in bf.x, then the hooked module: the whole block `layer` (token
+// facet) or its norm1 and the requested third of its qkv projection.  *feat = the [M, D] rows the facet reads.
+static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
+                     int layer, int facet, int gemm_engine, cudaStream_t st, const float** feat) {
+  const int D = cfg->embed_dim;
+  const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
+  int rc;
+  for (int l = 0; l < layer; ++l)
+    if ((rc = vit_block(cfg, w->blocks[l], bf, M, sq, gemm_engine, st))) return rc;
+  const AnylocVitBlock& wb = w->blocks[layer];
+  if (facet == ANYLOC_FACET_TOKEN) {
+    *feat = bf.x;
+    return vit_block(cfg, wb, bf, M, sq, gemm_engine, st);
+  }
+  // q/k/v facet: only the requested third of the qkv projection of block `layer`
+  if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc;
+  const size_t woff = (size_t)facet * D * D * (f16 ? 2 : 4);      // bytes: weights are __half or float
+  EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
+  e_f.alpha = wb.qkv_alpha;
+  *feat = bf.qkv;
+  return gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff, (const char*)wb.qkv_w_lo + woff, D, M, D,
+                       D, e_f, gemm_engine, f16, st);
 }
 
 extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img,
@@ -303,19 +353,110 @@ extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeight
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, B * N, D, Kp, e_pe,
                           gemm_engine, f16, st))) return rc;
   if ((rc = launch_assemble(bf.ptmp, w->cls_token, pos_embed, B, N, D, bf.x, st))) return rc;
-  for (int l = 0; l < layer; ++l)
-    if ((rc = vit_block(cfg, w->blocks[l], bf, B, T, gemm_engine, st))) return rc;
-  const AnylocVitBlock& wb = w->blocks[layer];
-  if (facet == ANYLOC_FACET_TOKEN) {
-    if ((rc = vit_block(cfg, wb, bf, B, T, gemm_engine, st))) return rc;
-    return launch_facet_out(bf.x, B, T, D, 0, D, use_cls, norm_descs, out, st);
+  const VitSeqs sq{B, T, nullptr, 0, 0.0};
+  const float* feat = nullptr;
+  if ((rc = vit_trunk(cfg, w, bf, M, sq, layer, facet, gemm_engine, st, &feat))) return rc;
+  return launch_facet_out(feat, B, T, D, 0, D, use_cls, norm_descs, out, st);
+}
+
+namespace {
+struct VarlenPlan {
+  VarlenImgTable img;         // img.ptr: the images for im2col, then the positional tables for the assembly
+  VarlenAttnTable attn;
+  int n_patch, n_tok, n_tiles;
+  double attn_flops;
+};
+// Geometry of a variable-length batch, from the host arrays of anyloc_vit_extract_varlen.  Returns false (with the
+// error text set) on a bad B or size.
+bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* p) {
+  if (!cfg || cfg->patch <= 0) { set_error("vit_extract_varlen: null or bad config"); return false; }
+  if (B < 1 || B > ANYLOC_VIT_VARLEN_MAX_B) {
+    set_error("vit_extract_varlen: B=%d out of range [1,%d]", B, ANYLOC_VIT_VARLEN_MAX_B);
+    return false;
   }
-  // q/k/v facet: only the requested third of the qkv projection of block `layer`
-  if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc;
-  const size_t woff = (size_t)facet * D * D * (f16 ? 2 : 4);      // bytes: weights are __half or float
-  EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
-  e_f.alpha = wb.qkv_alpha;
-  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff,
-                          (const char*)wb.qkv_w_lo + woff, D, M, D, D, e_f, gemm_engine, f16, st))) return rc;
-  return launch_facet_out(bf.qkv, B, T, D, 0, D, use_cls, norm_descs, out, st);
+  if (!hw) { set_error("vit_extract_varlen: null hw"); return false; }
+  const int P = cfg->patch;
+  int64_t tok = 0, patches = 0, tiles = 0;
+  double flops = 0.0;
+  p->img.n = B; p->attn.n = B;
+  int order[ANYLOC_VIT_VARLEN_MAX_B];
+  for (int i = 0; i < B; ++i) {
+    const int H = hw[2 * i], W = hw[2 * i + 1];
+    if (H <= 0 || W <= 0 || H % P || W % P) {
+      set_error("vit_extract_varlen: image %d is %dx%d; H and W must be positive multiples of the patch size %d", i, H,
+                W, P);
+      return false;
+    }
+    const int64_t n = (int64_t)(H / P) * (W / P);
+    if (tok + n + 1 > (int64_t)INT32_MAX / 32) {     // the row-per-warp kernels index threads in 32 bits
+      set_error("vit_extract_varlen: too many tokens in one call");
+      return false;
+    }
+    p->img.tok0[i] = (int)tok;
+    p->img.gh[i] = H / P; p->img.gw[i] = W / P;
+    p->img.ptr[i] = nullptr;
+    tok += n + 1; patches += n;
+    flops += 4.0 * (double)(n + 1) * (n + 1) * cfg->embed_dim;
+    order[i] = i;
+  }
+  // attention entries longest first (the longest key loops start first); ties keep the input order
+  std::stable_sort(order, order + B, [&](int a, int b) { return p->img.gh[a] * p->img.gw[a] > p->img.gh[b] * p->img.gw[b]; });
+  for (int k = 0; k < B; ++k) {
+    const int i = order[k], T = p->img.gh[i] * p->img.gw[i] + 1;
+    p->attn.tile0[k] = (int)tiles; p->attn.row0[k] = p->img.tok0[i]; p->attn.len[k] = T;
+    tiles += cdiv(T, 64);
+  }
+  p->n_patch = (int)patches; p->n_tok = (int)tok; p->n_tiles = (int)tiles; p->attn_flops = flops;
+  return true;
+}
+}  // namespace
+
+extern "C" size_t anyloc_vit_varlen_workspace_bytes(const AnylocVitCfg* cfg, int B, const int32_t* hw) {
+  VarlenPlan p;
+  if (!varlen_plan(cfg, B, hw, &p)) return 0;
+  return vit_carve(cfg, (size_t)p.n_patch, (size_t)p.n_tok, nullptr, 0, nullptr) + 4096;
+}
+
+extern "C" int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
+                                         const float* const* img, const int32_t* hw, const float* const* pos_embed,
+                                         int layer, int facet, int use_cls, int norm_descs, float* out, void* ws,
+                                         size_t ws_bytes, int gemm_engine, void* stream) {
+  ANYLOC_REQUIRE(cfg && w && img && pos_embed && out && ws, "vit_extract_varlen: null pointer");
+  ANYLOC_REQUIRE(layer >= 0 && layer < cfg->depth, "vit_extract_varlen: layer %d out of range [0,%d)", layer,
+                 cfg->depth);
+  ANYLOC_REQUIRE(facet >= ANYLOC_FACET_QUERY && facet <= ANYLOC_FACET_TOKEN, "vit_extract_varlen: bad facet %d", facet);
+  ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "vit_extract_varlen: head_dim must be 64");
+  if (gemm_engine == ANYLOC_GEMM_SIMT) {
+    set_error("vit_extract_varlen: needs the tensor-core attention (gemm_engine auto or tc3, not simt)");
+    return ANYLOC_ERR_UNSUPPORTED;
+  }
+  ANYLOC_REQUIRE(gemm_engine == ANYLOC_GEMM_AUTO || gemm_engine == ANYLOC_GEMM_TC3,
+                 "vit_extract_varlen: bad gemm_engine %d", gemm_engine);
+  VarlenPlan p;
+  if (!varlen_plan(cfg, B, hw, &p)) return ANYLOC_ERR_ARG;
+  for (int i = 0; i < B; ++i)
+    ANYLOC_REQUIRE(img[i] && pos_embed[i], "vit_extract_varlen: null image or positional table %d", i);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int P = cfg->patch, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P), M = p.n_tok;
+  VitBuffers bf;
+  if (!vit_carve(cfg, (size_t)p.n_patch, (size_t)M, ws, ws_bytes, &bf)) {
+    set_error("vit_extract_varlen: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_vit_varlen_workspace_bytes(cfg, B, hw));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  int rc;
+  const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
+  for (int i = 0; i < B; ++i) p.img.ptr[i] = img[i];
+  if ((rc = launch_im2col_varlen(p.img, p.n_patch, P, Kp, bf.pa_hi, bf.pa_lo, f16, st))) return rc;
+  EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};
+  e_pe.alpha = w->patch_alpha;
+  if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, p.n_patch, D, Kp, e_pe,
+                          gemm_engine, f16, st))) return rc;
+  for (int i = 0; i < B; ++i) p.img.ptr[i] = pos_embed[i];
+  if ((rc = launch_assemble_varlen(bf.ptmp, w->cls_token, p.img, M, D, bf.x, st))) return rc;
+  const VitSeqs sq{B, 0, &p.attn, p.n_tiles, p.attn_flops};
+  const float* feat = nullptr;
+  if ((rc = vit_trunk(cfg, w, bf, M, sq, layer, facet, gemm_engine, st, &feat))) return rc;
+  const int rows = M - (use_cls ? 0 : B);
+  return launch_facet_out_varlen(feat, p.img, rows, D, 0, D, use_cls, norm_descs, out, st);
 }

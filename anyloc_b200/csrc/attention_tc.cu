@@ -62,20 +62,31 @@ __device__ __forceinline__ float ex2(float x) {
 __device__ __forceinline__ uint32_t f2u(float x) { return __float_as_uint(x); }
 __device__ __forceinline__ uint32_t ld_h2(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
-template <bool F16>
-__global__ void __launch_bounds__(THREADS)
-attention_tc_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T, int D,
-                    void* __restrict__ o_hi_, void* __restrict__ o_lo_) {
+// One CTA's work.  Uniform (VARLEN = false): blockIdx = (query tile, head, image) over B images of T tokens.  VARLEN:
+// blockIdx = (tile of the packed grid, head); the table gives the image's first row, its length T and its first tile.
+template <bool F16, bool VARLEN>
+__device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T,
+                                              int D, void* __restrict__ o_hi_, void* __restrict__ o_lo_,
+                                              const VarlenAttnTable* tab) {
   using C = Cfg<F16>;
   using E = typename C::T;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   E* smem = reinterpret_cast<E*>(smem_raw);
   const E* qkv_hi = reinterpret_cast<const E*>(qkv_hi_);
   const E* qkv_lo = reinterpret_cast<const E*>(qkv_lo_);
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  int qt = blockIdx.x;
+  const int h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
   const size_t ld = 3 * (size_t)D;
-  const size_t img0 = (size_t)b * T;
+  size_t img0 = (size_t)b * T;
+  if constexpr (VARLEN) {
+    int lo = 0, hi = tab->n - 1;          // the last entry with tile0 <= qt
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (tab->tile0[mid] <= qt) lo = mid; else hi = mid - 1;
+    }
+    qt -= tab->tile0[lo]; T = tab->len[lo]; img0 = (size_t)tab->row0[lo];
+  }
   const int nblk = (T + BKV - 1) / BKV;
   const float P_SCALE = F16 ? 1024.0f : 1.0f;
   // S holds (s q).(s k), s = kActScale for fp16 pairs: fold 1/s^2 into the 1/sqrt(64) * log2(e) scale
@@ -284,6 +295,24 @@ attention_tc_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ q
   }
 }
 
+// B images of T tokens each: grid (query tiles, heads, B)
+template <bool F16>
+__global__ void __launch_bounds__(THREADS)
+attention_tc_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T, int D,
+                    void* __restrict__ o_hi_, void* __restrict__ o_lo_) {
+  attention_cta<F16, false>(qkv_hi_, qkv_lo_, T, D, o_hi_, o_lo_, nullptr);
+}
+
+// Images of different lengths packed row after row: grid (sum of every image's query tiles, heads).  The host lists
+// the images longest first, so the CTAs with the longest key loops start first and short images fill the tail.
+template <bool F16>
+__global__ void __launch_bounds__(THREADS)
+attention_tc_varlen_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_,
+                           const __grid_constant__ VarlenAttnTable tab, int D, void* __restrict__ o_hi_,
+                           void* __restrict__ o_lo_) {
+  attention_cta<F16, true>(qkv_hi_, qkv_lo_, 0, D, o_hi_, o_lo_, &tab);
+}
+
 // fp32 (hi,lo) qkv pairs -> fp16 pairs of 8*x (same [M,3D] layout).  Standalone building-block path only.
 __global__ void __launch_bounds__(256)
 qkv_to_f16_kernel(const float* __restrict__ qkv_hi, const float* __restrict__ qkv_lo, size_t n, __half* __restrict__ q16_hi,
@@ -312,6 +341,28 @@ int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, in
   const dim3 grid(cdiv(T, BQ), heads, B);
   if (f16) attention_tc_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
   else attention_tc_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+
+// the same over images of different lengths packed into one [sum T_i, 3D] qkv buffer; tab.tile0 runs to n_tiles
+int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int n_tiles, int D,
+                               int heads, void* o_hi, void* o_lo, bool f16, cudaStream_t st) {
+  using namespace atc;
+  ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
+  ANYLOC_REQUIRE(heads <= 65535, "attention_tc: grid too large (heads=%d)", heads);
+  static unsigned long long attr_seen = 0;
+  if (first_use_on_this_device(&attr_seen)) {
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel<true>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<true>::SMEM_BYTES));
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel<false>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<false>::SMEM_BYTES));
+  }
+  const dim3 grid(n_tiles, heads);
+  if (f16)
+    attention_tc_varlen_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
+  else
+    attention_tc_varlen_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

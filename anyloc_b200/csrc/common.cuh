@@ -95,6 +95,37 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uin
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(lb), "f"(la));
 }
 
+// Per-image geometry of a packed batch of differently sized images (anyloc_vit_extract_varlen).  The tables reach the
+// kernels by value as __grid_constant__ parameters: the launch copies them, so a call neither synchronises with the
+// host nor keeps a host pointer, and each stays under the classic 4 KB kernel-parameter limit.
+constexpr int kVarlenMaxB = ANYLOC_VIT_VARLEN_MAX_B;
+// im2col, token assembly and the facet slice.  Image i has tokens [tok0[i], tok0[i] + 1 + gh[i]*gw[i]) of the packed
+// sequence, patch rows from tok0[i] - i and, without the cls token, output rows from tok0[i] - i.
+struct VarlenImgTable {
+  int n;
+  int tok0[kVarlenMaxB];
+  int gh[kVarlenMaxB], gw[kVarlenMaxB];
+  const float* ptr[kVarlenMaxB];        // the image [3, gh*P, gw*P] (im2col) or its positional table (assembly)
+};
+static_assert(sizeof(VarlenImgTable) <= 4096, "kernel parameter over 4 KB");
+// the last image i whose first row tok0[i] - skip*i (skip = rows the kernel's grid omits per image) is <= row
+__device__ __forceinline__ int varlen_image_of(const VarlenImgTable& t, int row, int skip) {
+  int lo = 0, hi = t.n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (t.tok0[mid] - skip * mid <= row) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+// the attention: one entry per image, in any order; tile0 ascending, tile0[0] = 0
+struct VarlenAttnTable {
+  int n;
+  int tile0[kVarlenMaxB];               // first 64-query tile of the entry in the grid
+  int row0[kVarlenMaxB];                // first token row of the image
+  int len[kVarlenMaxB];                 // its tokens
+};
+static_assert(sizeof(VarlenAttnTable) <= 4096, "kernel parameter over 4 KB");
+
 int device_sm_count();
 // true the first time it is called on the CURRENT device for this flag word: cudaFuncSetAttribute is per device, so a
 // process that drives several GPUs must repeat it on each of them (one bit per device ordinal; atomic because two host

@@ -32,13 +32,13 @@ template <> struct PairOut<true> {
   static __device__ __forceinline__ void put(__half* hi, __half* lo, size_t i, float v) { __half h, l; split_f16(v * kActScale, h, l); hi[i] = h; lo[i] = l; }
 };
 
-// img [B,3,H,W] -> patches (hi,lo) [B*gh*gw, Kp], column order (c, ky, kx) like conv weight.flatten(1)
+// patch pi of image b of img [B,3,H,W] -> patch row `row` of (hi,lo), column order (c, ky, kx) like conv
+// weight.flatten(1)
 template <bool F16>
-__global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H, int W, int P, int Kp,
-                                    typename PairOut<F16>::T* __restrict__ hi, typename PairOut<F16>::T* __restrict__ lo) {
-  const int gh = H / P, gw = W / P;
-  const size_t row = blockIdx.x;               // patch index
-  const int b = (int)(row / (gh * gw)), pi = (int)(row % (gh * gw));
+__device__ __forceinline__ void im2col_row(const float* __restrict__ img, int b, int H, int W, int P, int Kp, size_t row,
+                                           int pi, typename PairOut<F16>::T* __restrict__ hi,
+                                           typename PairOut<F16>::T* __restrict__ lo) {
+  const int gw = W / P;
   const int py = pi / gw, px = pi % gw;
   const int Kreal = 3 * P * P;
   for (int c = threadIdx.x; c < Kp; c += blockDim.x) {
@@ -51,15 +51,47 @@ __global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H,
   }
 }
 
-// x[b,0,:] = cls + pos[0];  x[b,1+n,:] = patch[b*N+n,:] + pos[1+n]     (prepare_tokens)
+// img [B,3,H,W] -> patches (hi,lo) [B*gh*gw, Kp]
+template <bool F16>
+__global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H, int W, int P, int Kp,
+                                    typename PairOut<F16>::T* __restrict__ hi, typename PairOut<F16>::T* __restrict__ lo) {
+  const int gh = H / P, gw = W / P;
+  const size_t row = blockIdx.x;               // patch index
+  const int b = (int)(row / (gh * gw)), pi = (int)(row % (gh * gw));
+  im2col_row<F16>(img, b, H, W, P, Kp, row, pi, hi, lo);
+}
+
+// images of different sizes, one block per patch row of the packed [sum gh_i*gw_i, Kp] output
+template <bool F16>
+__global__ void im2col_split_varlen_kernel(const __grid_constant__ VarlenImgTable tab, int P, int Kp,
+                                           typename PairOut<F16>::T* __restrict__ hi,
+                                           typename PairOut<F16>::T* __restrict__ lo) {
+  const int row = blockIdx.x, i = varlen_image_of(tab, row, 1);
+  im2col_row<F16>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - i), hi, lo);
+}
+
+// x[row,:] = cls + pos[0] (t = 0) or patch[b*N + t-1,:] + pos[t]     (prepare_tokens)
+__device__ __forceinline__ void assemble_row(const float* __restrict__ patch, const float* __restrict__ cls,
+                                             const float* __restrict__ pos, int b, int N, int D, size_t row, int t,
+                                             float* __restrict__ x) {
+  const float* src = t == 0 ? cls : patch + ((size_t)b * N + (t - 1)) * D;
+  const float* pe = pos + (size_t)t * D;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) x[row * D + d] = src[d] + pe[d];
+}
+
 __global__ void assemble_tokens_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
                                        const float* __restrict__ pos, int B, int N, int D,
                                        float* __restrict__ x) {
   const size_t row = blockIdx.x;     // over B*(N+1)
   const int b = (int)(row / (N + 1)), t = (int)(row % (N + 1));
-  const float* src = t == 0 ? cls : patch + ((size_t)b * N + (t - 1)) * D;
-  const float* pe = pos + (size_t)t * D;
-  for (int d = threadIdx.x; d < D; d += blockDim.x) x[row * D + d] = src[d] + pe[d];
+  assemble_row(patch, cls, pos, b, N, D, row, t, x);
+}
+
+// images of different sizes, one block per token row of the packed sequence; image i reads its own positional table
+__global__ void assemble_tokens_varlen_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
+                                              const __grid_constant__ VarlenImgTable tab, int D, float* __restrict__ x) {
+  const int row = blockIdx.x, i = varlen_image_of(tab, row, 0);
+  assemble_row(patch + (size_t)(tab.tok0[i] - i) * D, cls, tab.ptr[i], 0, 0, D, row, row - tab.tok0[i], x);
 }
 
 // LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo). One warp per row.
@@ -136,17 +168,11 @@ l2norm_rows_kernel(const float* __restrict__ x, int64_t rows, int D, int64_t ld_
   }
 }
 
-// gather token rows [B, T, ld] (skipping cls unless use_cls, column offset col0) -> [B, T', D] then normalise
-__global__ void __launch_bounds__(256)
-facet_out_kernel(const float* __restrict__ src, int B, int T, int64_t ld, int col0, int D, int use_cls,
-                 int do_norm, float* __restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const int Tout = use_cls ? T : T - 1;
-  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (row >= (int64_t)B * Tout) return;
-  const int b = (int)(row / Tout), t = (int)(row % Tout) + (use_cls ? 0 : 1);
-  const float4* xr = reinterpret_cast<const float4*>(src + ((int64_t)b * T + t) * ld + col0);
-  float4* yr = reinterpret_cast<float4*>(out + row * D);
+// one token row -> one output row (normalised if do_norm), one warp
+__device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x, int D, int do_norm,
+                                          float* __restrict__ y) {
+  const float4* xr = reinterpret_cast<const float4*>(x);
+  float4* yr = reinterpret_cast<float4*>(y);
   const int D4 = D >> 2;
   float ss = 0.f;
   for (int d = lane; d < D4; d += 32) { float4 v = xr[d]; ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w; }
@@ -156,6 +182,30 @@ facet_out_kernel(const float* __restrict__ src, int B, int T, int64_t ld, int co
     if (do_norm) { v.x /= nrm; v.y /= nrm; v.z /= nrm; v.w /= nrm; }
     yr[d] = v;
   }
+}
+
+// gather token rows [B, T, ld] (skipping cls unless use_cls, column offset col0) -> [B, T', D] then normalise
+__global__ void __launch_bounds__(256)
+facet_out_kernel(const float* __restrict__ src, int B, int T, int64_t ld, int col0, int D, int use_cls,
+                 int do_norm, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int Tout = use_cls ? T : T - 1;
+  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (row >= (int64_t)B * Tout) return;
+  const int b = (int)(row / Tout), t = (int)(row % Tout) + (use_cls ? 0 : 1);
+  facet_row(lane, src + ((int64_t)b * T + t) * ld + col0, D, do_norm, out + row * D);
+}
+
+// images of different sizes packed row after row: `rows` output rows, image i's from tok0[i] (- i without cls)
+__global__ void __launch_bounds__(256)
+facet_out_varlen_kernel(const float* __restrict__ src, const __grid_constant__ VarlenImgTable tab, int rows, int64_t ld,
+                        int col0, int D, int use_cls, int do_norm, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= rows) return;
+  const int skip = use_cls ? 0 : 1, i = varlen_image_of(tab, row, skip);
+  const int tok = row + skip * (i + 1);         // the token row: every earlier image and this one skipped their cls
+  facet_row(lane, src + (int64_t)tok * ld + col0, D, do_norm, out + (int64_t)row * D);
 }
 
 int launch_split(const float* x, float* hi, float* lo, size_t n, cudaStream_t st) {
@@ -205,6 +255,26 @@ int launch_facet_out(const float* src, int B, int T, int64_t ld, int col0, int D
                      float* out, cudaStream_t st) {
   int64_t rows = (int64_t)B * (use_cls ? T : T - 1);
   facet_out_kernel<<<(int)((rows + 7) / 8), 256, 0, st>>>(src, B, T, ld, col0, D, use_cls, do_norm, out);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+// packed batches of differently sized images: tab.ptr holds the images (im2col) or the positional tables (assembly)
+int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp, void* hi, void* lo, bool f16,
+                         cudaStream_t st) {
+  if (f16) im2col_split_varlen_kernel<true><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, (__half*)lo);
+  else im2col_split_varlen_kernel<false><<<n_patches, 128, 0, st>>>(tab, P, Kp, (float*)hi, (float*)lo);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+int launch_assemble_varlen(const float* patch, const float* cls, const VarlenImgTable& tab, int n_tokens, int D,
+                           float* x, cudaStream_t st) {
+  assemble_tokens_varlen_kernel<<<n_tokens, 256, 0, st>>>(patch, cls, tab, D, x);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int rows, int64_t ld, int col0, int D,
+                            int use_cls, int do_norm, float* out, cudaStream_t st) {
+  facet_out_varlen_kernel<<<(rows + 7) / 8, 256, 0, st>>>(src, tab, rows, ld, col0, D, use_cls, do_norm, out);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

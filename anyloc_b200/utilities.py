@@ -343,15 +343,27 @@ class DinoV2ExtractFeatures:
         self.dino_model = _vit.VitWeights(name, self._state_dict, dev, depth=self.layer + 1, pair="tf32")
         self.precision, self._auto, self._state_dict = "tf32x3", False, None
 
-    def __call__(self, img: torch.Tensor) -> torch.Tensor:
+    def _extract(self, img):
+        """-> (every output row in one tensor, what __call__ returns)"""
+        if isinstance(img, (list, tuple)):
+            packed, n = self.dino_model.extract_varlen(img, self.layer, self.facet, self.use_cls, self.norm_descs,
+                                                       self.gemm_engine)
+            return packed, list(packed.split(n))
+        out = self.dino_model.extract(img, self.layer, self.facet, self.use_cls, self.norm_descs, self.gemm_engine)
+        return out, out
+
+    def __call__(self, img):
+        """img [B,3,H,W] -> [B, N(+1), D]; or a list/tuple of differently sized images [3,H_i,W_i] / [1,3,H_i,W_i],
+        all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
+        pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
+        image of fewer than 32 tokens takes the SIMT GEMMs)."""
         with torch.no_grad():
             if self.check_finite == "deferred" and not self._auto:
                 self.raise_if_overflowed()
-            out = self.dino_model.extract(img, self.layer, self.facet, self.use_cls, self.norm_descs,
-                                          self.gemm_engine)
+            packed, out = self._extract(img)
             if self.precision != "f16x3" or (self.check_finite == "off" and not self._auto):
                 return out
-            flag = torch.isfinite(out).all()
+            flag = torch.isfinite(packed).all()
             if self.check_finite == "deferred" and not self._auto:
                 self._pending_flag = flag
                 return out
@@ -360,8 +372,7 @@ class DinoV2ExtractFeatures:
             if not self._auto:
                 raise _lib.AnylocError(self._OVERFLOW_MSG)
             self._switch_to_tf32()
-            return self.dino_model.extract(img, self.layer, self.facet, self.use_cls, self.norm_descs,
-                                           self.gemm_engine)
+            return self._extract(img)[1]
 
     def __del__(self):
         pass

@@ -220,6 +220,71 @@ class VitWeights:
         _lib.check(rc, "anyloc_vit_extract")
         return out
 
+    def extract_varlen(self, imgs, layer, facet="value", use_cls=False, norm_descs=True, engine="auto"):
+        """A list of differently sized images [3,H_i,W_i] (or [1,3,H_i,W_i]) fp32 on self.device in one packed forward
+        pass (anyloc_vit_extract_varlen) -> (packed [sum n_i, D] fp32, [n_i]), n_i = gh_i*gw_i (+1 with use_cls).
+        Image i's rows equal extract(imgs[i][None])[0] bit for bit.  Lists longer than the library's per-call limit
+        run as consecutive calls into the same packed output."""
+        if not 0 <= layer < self.depth:
+            raise IndexError(f"layer {layer} out of range for {self.name} with {self.depth} blocks loaded")
+        imgs = check_varlen_images(imgs, self.device)
+        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B)
+        out = torch.empty(lay.rows, self.dim, device=self.device, dtype=torch.float32)
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            for s, e in lay.chunks:
+                B = e - s
+                hw = (C.c_int32 * (2 * B))(*[v for x in imgs[s:e] for v in x.shape[1:]])
+                img_p = (C.c_void_p * B)(*[x.data_ptr() for x in imgs[s:e]])
+                pos_p = (C.c_void_p * B)(*[self.pos_for(*g).data_ptr() for g in lay.grids[s:e]])
+                nbytes = lib.anyloc_vit_varlen_workspace_bytes(C.byref(self.cfg), B, hw)
+                ws = _lib.workspaces.get(self.device, nbytes, "vit")
+                rc = lib.anyloc_vit_extract_varlen(C.byref(self.cfg), C.byref(self.struct), B, img_p, hw, pos_p, layer,
+                                                   _lib.FACET[facet], int(bool(use_cls)), int(bool(norm_descs)),
+                                                   C.c_void_p(out[lay.row0[s]:].data_ptr()), _lib.ptr(ws), ws.numel(),
+                                                   _lib.ENGINE[engine], _lib.stream_ptr())
+                _lib.check(rc, "anyloc_vit_extract_varlen")
+        return out, lay.n_out
+
+
+def check_varlen_images(imgs, device):
+    """The items of a list input as [3,H,W] fp32 contiguous tensors on `device`; ValueError on an empty list, a wrong
+    rank or channel count, a size that is not a positive multiple of the patch size, or an image on another device.
+    Images are used in place (their data pointers go to the library), converted only if not fp32 contiguous."""
+    if not isinstance(imgs, (list, tuple)) or len(imgs) == 0:
+        raise ValueError("expected a non-empty list of images [3,H,W] or [1,3,H,W]")
+    res = []
+    for i, x in enumerate(imgs):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError(f"image {i} is a {type(x).__name__}, not a tensor")
+        if x.dim() == 4 and x.shape[0] == 1:
+            x = x[0]
+        if x.dim() != 3 or x.shape[0] != 3:
+            raise ValueError(f"image {i}: expected [3,H,W] or [1,3,H,W], got {tuple(x.shape)}")
+        H, W = x.shape[1:]
+        if H == 0 or W == 0 or H % PATCH or W % PATCH:
+            raise ValueError(f"image {i}: size {(H, W)} is not a multiple of the patch size {PATCH}")
+        if x.device != device:
+            raise ValueError(f"image {i} is on {x.device}, the extractor on {device}")
+        res.append(x.to(dtype=torch.float32).contiguous())
+    return res
+
+
+class VarlenLayout:
+    """Where each image of a list input lands: grids (gh_i, gw_i), tokens T_i = gh_i*gw_i + 1, output rows n_i
+    (T_i - 1 without the cls token), their offsets row0 in the packed output (row0[-1] = rows) and the consecutive
+    (start, stop) slices of at most max_b images, one library call each."""
+
+    def __init__(self, sizes, use_cls, max_b):
+        self.grids = [(H // PATCH, W // PATCH) for H, W in sizes]
+        self.tokens = [gh * gw + 1 for gh, gw in self.grids]
+        self.n_out = [t - (0 if use_cls else 1) for t in self.tokens]
+        self.row0 = [0]
+        for n in self.n_out:
+            self.row0.append(self.row0[-1] + n)
+        self.rows = self.row0[-1]
+        self.chunks = [(s, min(s + max_b, len(sizes))) for s in range(0, len(sizes), max_b)]
+
 
 def resolve_state_dict(name, device):
     """Where the weights come from, in order: $ANYLOC_B200_WEIGHTS_DIR/<name>.pth (a plain upstream

@@ -242,6 +242,28 @@ int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, 
                        int use_cls, int norm_descs, float* out, void* ws, size_t ws_bytes,
                        int gemm_engine, void* stream);
 
+/* B images of DIFFERENT sizes in one forward pass.  Outside the benchmark datasets images keep their aspect ratio
+ * (the reference demo, demo/anyloc_vlad_generate.py:160-185, shrinks the longest side to 1024 only when larger and
+ * centre-crops to a multiple of 14), so two photos reach the ViT at different patch grids; padding them to one size
+ * would change every softmax and the interpolated positional embedding.  Instead the token rows of all images are
+ * packed one after another: the GEMMs and LayerNorms run once over all sum_i T_i rows, and the attention, im2col,
+ * token assembly and facet slice read each image's geometry from a per-image table.
+ *   img       HOST array of B device pointers; image i is [3, H_i, W_i] fp32
+ *   hw        HOST int32 [B][2] = (H_i, W_i), positive multiples of the patch size
+ *   pos_embed HOST array of B device pointers; pos_embed[i] = the table [1 + g_h,i * g_w,i, D] interpolated for image
+ *             i's grid (images of the same grid may share one)
+ *   out       packed [sum_i n_i, D] with n_i = g_h,i * g_w,i (+1 if use_cls); image i's rows start at sum_{j<i} n_j.
+ * Each image's rows are bit-identical to anyloc_vit_extract on that image alone with the same GEMM engine (under
+ * ANYLOC_GEMM_AUTO, a lone image of fewer than 32 tokens takes the SIMT GEMMs there, so compare those under TC3).
+ * gemm_engine = ANYLOC_GEMM_SIMT returns ANYLOC_ERR_UNSUPPORTED: the packed attention is a tensor-core kernel.  The
+ * call copies the geometry into kernel parameters; it neither synchronises with the host nor keeps any host pointer
+ * it was given.  1 <= B <= ANYLOC_VIT_VARLEN_MAX_B. */
+#define ANYLOC_VIT_VARLEN_MAX_B 128
+size_t anyloc_vit_varlen_workspace_bytes(const AnylocVitCfg* cfg, int B, const int32_t* hw);
+int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, int B, const float* const* img,
+                              const int32_t* hw, const float* const* pos_embed, int layer, int facet, int use_cls,
+                              int norm_descs, float* out, void* ws, size_t ws_bytes, int gemm_engine, void* stream);
+
 /* ------------------------------------------- building blocks (exported for parity tests)
  * C[M,N] = (A_hi+A_lo)[M,K] . (B_hi+B_lo)[N,K]^T with epilogue; *_lo nullable (treated as 0).
  * lda/ldb/ldo in elements.  out_lo/bias/gamma/resid per epilogue. */
