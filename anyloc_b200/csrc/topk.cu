@@ -1,6 +1,7 @@
 // Query->database retrieval (reference: /root/reference/utilities.py:435-450, faiss IndexFlatIP /
 // IndexFlatL2 exact search).  normalise rows -> score GEMM (fp32-equivalent) -> k-best per query,
 // best first, lowest database index first among equal scores.
+#include <float.h>
 #include <stdlib.h>
 #include <algorithm>
 #include "common.cuh"
@@ -87,7 +88,10 @@ normalize_rows_split_kernel(const float* __restrict__ x, int D, int do_norm, voi
       float t = 0.f; for (int w = 0; w < 8; ++w) t += red[w];
       const float b = (sqrtf(t) * 1.001f + sqrtf((float)D) * 2.98e-8f) / kRetrievalScale;
       dn[row] = b;
-      if (dn_max_bits) atomicMax(dn_max_bits, __float_as_int(b));      // positive floats order like their bit patterns
+      // positive floats order like their bit patterns.  A row holding a NaN or an Inf (b = NaN) stays out of the header:
+      // a NaN there would make every query's threshold NaN, i.e. no candidates and an empty answer.  The row's own
+      // coarse scores are NaN, so it is never a candidate, as it is never selected on the exact route.
+      if (dn_max_bits && b <= FLT_MAX) atomicMax(dn_max_bits, __float_as_int(b));
     }
   }
   }
@@ -162,7 +166,7 @@ normalize_rows_split_reg_kernel(const float* __restrict__ x, int D, int do_norm,
         float t = 0.f; for (int w = 0; w < 32; ++w) t += red[w];
         const float b = (sqrtf(t) * 1.001f + sqrtf((float)D) * 2.98e-8f) / kRetrievalScale;
         dn[row] = b;
-        if (dn_max_bits) atomicMax(dn_max_bits, __float_as_int(b));
+        if (dn_max_bits && b <= FLT_MAX) atomicMax(dn_max_bits, __float_as_int(b));     // finite rows only, as above
       }
     }
   }
@@ -625,7 +629,8 @@ extern "C" int anyloc_topk(const float* db, const float* qu, int n_db, int n_q, 
   ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "topk: unknown metric %d", metric);
   if (n_q == 0) return ANYLOC_OK;
   const size_t ib = anyloc_index_bytes(n_db, Dv, normalize);
-  const size_t need = align_up(ib, 256) + anyloc_index_search_workspace_bytes(n_db, n_q, Dv, normalize);
+  // the documented size, whichever pair format this call picks (it covers the carve below in every case)
+  const size_t need = anyloc_topk_workspace_bytes(n_db, n_q, Dv, k);
   if (ws_bytes < need) {
     set_error("topk: workspace too small (%zu given, %zu needed)", ws_bytes, need);
     return ANYLOC_ERR_WORKSPACE;

@@ -86,7 +86,7 @@ def _check_vs_fp64(db, qu, dist, idx, k):
 
 
 def test_topk_coarse_pass_and_fallback(u):
-    """The inner-product search on an fp16-pair index: hi-only tensor-core pass (2-CTA kernel at >= 512 queries) + exact
+    """The inner-product search on an fp16-pair index: hi-only pass of the wgmma GEMM (640 queries) + exact
     re-scoring of the candidates, and the device-gated 3-term fallback when a candidate list overflows (here: 400
     identical database rows next to the query -> 400 candidates > CAND_MAX; ties must still come out lowest index first)."""
     g = torch.Generator(device="cuda").manual_seed(5)
