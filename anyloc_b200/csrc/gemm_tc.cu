@@ -49,7 +49,8 @@ template <bool LO> struct Cfg {
   static constexpr int STG_OFF = BAR_OFF + 1024;
   static constexpr int SMEM_BYTES_STAGED = STG_OFF + 4 * STG_BYTES + 1024 /*align*/;
 };
-constexpr int CHUNK_KB_TF32 = 2;           // k-blocks accumulated by the tensor core between two round-to-nearest adds
+constexpr int BAND_N = 16;                 // column blocks per raster band
+constexpr int CHUNK_KB_TF32 = 2;          // k-blocks accumulated by the tensor core between two round-to-nearest adds
 constexpr int CHUNK_KB_F16 = 8;            // (24 / 96 wgmma k-steps per chunk)
 constexpr int CHUNK_KB_COARSE = 32;        // hi-only fp16 coarse pass (retrieval): <= 128 k-steps per chunk, the bound
                                            // topk.cu re-scores against
@@ -545,7 +546,7 @@ static thread_local int g_last_staged = -1;
 
 template <bool F16, int LOM>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
-                       int N, int K, const EpiParams& ep, int band_n, int chunk, cudaStream_t st) {
+                       int N, int K, const EpiParams& ep, int chunk, cudaStream_t st) {
   using namespace tc;
   constexpr bool LO = LOM != 0;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
@@ -571,15 +572,13 @@ static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* 
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
   gemm_tc3_kernel<F16, LOM><<<grid, THREADS, smem, st>>>(
-      ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(band_n, cdiv(N, BN)), chunk, ep);
+      ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(BAND_N, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
 
 int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                    int N, int K, const EpiParams& ep_in, bool f16, cudaStream_t st) {
-  static int band_n = -1;
-  if (band_n < 0) { const char* e = getenv("ANYLOC_GEMM_BAND"); band_n = e ? atoi(e) : 16; if (band_n < 1) band_n = 1 << 20; }
   // ANYLOC_GEMM_CHUNK: k-blocks per round-to-nearest chunk of the 3-term GEMMs (A/B knob)
   static int chunk_env = -1;
   if (chunk_env < 0) { const char* e = getenv("ANYLOC_GEMM_CHUNK"); chunk_env = e ? atoi(e) : 0; }
@@ -593,7 +592,7 @@ int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi
   // hi-only fp16 pass = the retrieval's coarse scores, whose error bound allows long chunks
   const int chunk = lom == 0 ? (f16 ? tc::CHUNK_KB_COARSE : tc::CHUNK_KB_TF32)
                              : chunk_env > 0 ? chunk_env : (f16 ? tc::CHUNK_KB_F16 : tc::CHUNK_KB_TF32);
-#define ANYLOC_GEMM_LAUNCH(F16_, LOM_) launch_impl<F16_, LOM_>(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, band_n, chunk, st)
+#define ANYLOC_GEMM_LAUNCH(F16_, LOM_) launch_impl<F16_, LOM_>(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, chunk, st)
   switch (lom + (f16 ? 4 : 0)) {
     case 0: return ANYLOC_GEMM_LAUNCH(false, 0);
     case 1: return ANYLOC_GEMM_LAUNCH(false, 1);

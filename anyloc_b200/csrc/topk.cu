@@ -2,7 +2,6 @@
 // IndexFlatL2 exact search).  normalise rows -> score GEMM (fp32-equivalent) -> k-best per query,
 // best first, lowest database index first among equal scores.
 #include <float.h>
-#include <stdlib.h>
 #include <algorithm>
 #include "common.cuh"
 
@@ -454,12 +453,8 @@ using namespace anyloc;
 //   hi [capacity, Dv] | lo [capacity, Dv] | sq [capacity] fp32 (|y|^2 per row, the L2 metric needs it) |
 //   dn [capacity] fp32 (|s y - hi| / s per row: what a hi-only product ignores; fp16 layout only) | header (256 B: max dn)
 // with hi/lo either fp16 pairs of 4096*y (unit rows: normalize != 0, Dv % 8 == 0 -- the 2x faster kind::f16 tensor
-// path) or tf32 pairs of y (rows of unknown range).  ANYLOC_TOPK_F16=0 forces the tf32 pairs (A/B).
-static bool index_uses_f16(int Dv, int normalize) {
-  static int f16_env = -1;
-  if (f16_env < 0) { const char* e = getenv("ANYLOC_TOPK_F16"); f16_env = e ? atoi(e) : 1; }
-  return f16_env && normalize && (Dv % 8) == 0;
-}
+// path) or tf32 pairs of y (rows of unknown range).
+static bool index_uses_f16(int Dv, int normalize) { return normalize && (Dv % 8) == 0; }
 struct IndexView { void* hi; void* lo; float* sq; float* dn; int* hdr; bool f16; size_t pair_bytes_per_row; };
 static bool carve_index(void* blob, size_t bytes, int64_t capacity, int Dv, int normalize, IndexView* v) {
   v->f16 = index_uses_f16(Dv, normalize);
@@ -580,10 +575,8 @@ extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_
   }
   const float alpha = v.f16 ? 1.0f / (kRetrievalScale * kRetrievalScale) : 1.0f;
   const int pair = v.f16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32;
-  // ---- coarse pass + exact re-scoring of the candidates (inner product, fp16 index); ANYLOC_TOPK_COARSE=0 disables
-  static int coarse_env = -1;
-  if (coarse_env < 0) { const char* e = getenv("ANYLOC_TOPK_COARSE"); coarse_env = e ? atoi(e) : 1; }
-  const bool coarse = coarse_env && v.f16 && metric == ANYLOC_METRIC_IP && k <= 64 && n_db >= 1024 && n_q >= 32;
+  // ---- coarse pass + exact re-scoring of the candidates (inner product, fp16 index)
+  const bool coarse = v.f16 && metric == ANYLOC_METRIC_IP && k <= 64 && n_db >= 1024 && n_q >= 32;
   const int* gate = nullptr;
   if (coarse) {
     ANYLOC_CHECK_CUDA(cudaMemsetAsync(flags, 0, 256, st));

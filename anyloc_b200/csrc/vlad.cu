@@ -1,21 +1,20 @@
 // Hard-assignment VLAD (reference: /root/reference/utilities.py:819-926, residuals :956-962,
 // assignment fpk.KMeans.predict :849).  See include/anyloc_b200.h for the contract.
 //
-// v2 pipeline (5 launches per batch):
+// Hard VLAD per call:
 //   centre_prep : c^_k = c_k/(|c_k|+1e-8) (cosine) or c_k with bias -|c_k|^2/2 (euclid), plus a tf32-rounded copy
+//                 (once per vocabulary with anyloc_vlad_prepare)
 //   coarse      : S~[R,K] = X . c^T on the tensor-core (wgmma) GEMM engine, single tf32 pass straight from the raw fp32
 //                 features (no conversion pass; the tensor core truncates) -- HBM-bound, reads X once
 //   rescore     : warp per row: |x|, candidate set {k : S~_k >= max - 2 eps} with the rigorous tf32 bound
 //                 eps = 2^-9 |x| max|c^|, exact fp32 dot products only for the candidates (row held in registers),
 //                 first-max argmax -> labels identical to an exact fp32 evaluation; 1/max(|x|,1e-12)
-//   accumulate  : CTA per (image, 128-column slice), warps split the rows, float4 lanes:
-//                 sum_{label=k}(x^ - c_k) in shared memory, deterministic per-slice sums of squares
-//   normalise   : intra + global L2 normalisation, in place on the [B,K*D] output
-// (The v1 FFMA assignment kernel serves D > 2048, calls of fewer than 256 rows and workspaces without room for the
+//   accumulate3 : CTA per (128-column slice, image): rows sorted by label, sum_{label=k}(x^ - c_k) in registers, then
+//                 the intra + global L2 normalisation in the same kernel.  Images of more rows than its shared memory
+//                 holds take accumulate2 (shared-memory accumulators) + the normalise launch.
+// (The FFMA assignment kernel serves D > 2048, calls of fewer than 256 rows and workspaces without room for the
 // coarse scores, at any K.)
-#include <stdlib.h>
 #include <algorithm>
-#include <vector>
 #include "epilogue.cuh"
 
 namespace anyloc {
@@ -24,12 +23,9 @@ namespace anyloc {
 __global__ void vlad_centre_prep_kernel(const float* __restrict__ c, int K, int D, int dist_mode,
                                         float* __restrict__ chat, float* __restrict__ cbias,
                                         float* __restrict__ chat_tf32, float* __restrict__ cnorm,
-                                        float* __restrict__ cdnorm /* |c^ - tf32(c^)|, nullable */,
-                                        int32_t* __restrict__ zero_a, int zero_a_n, int32_t* __restrict__ zero_b,
-                                        int zero_b_n) {
-  // the counters of the later launches on this stream are cleared here (saves two memset nodes)
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < zero_a_n; i += gridDim.x * blockDim.x) zero_a[i] = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < zero_b_n; i += gridDim.x * blockDim.x) zero_b[i] = 0;
+                                        int32_t* __restrict__ tickets, int n_tickets) {
+  // the accumulate3 tickets of this call are cleared here (saves a memset node)
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_tickets; i += gridDim.x * blockDim.x) tickets[i] = 0;
   int k = blockIdx.x;
   const float* row = c + (size_t)k * D;
   float ss = 0.f;
@@ -45,13 +41,12 @@ __global__ void vlad_centre_prep_kernel(const float* __restrict__ c, int K, int 
   }
   __syncthreads();
   ss = red[0];
-  float dd = 0.f;                                  // sum (c^ - tf32(c^))^2 over this thread's elements
   if (dist_mode == ANYLOC_DIST_COSINE) {
     const float den = sqrtf(ss) + 1e-8f;            // fpk cos_sim: b / (|b| + 1e-8)
     for (int d = threadIdx.x; d < D; d += blockDim.x) {
       float v = row[d] / den, h, l;
       chat[(size_t)k * D + d] = v;
-      if (chat_tf32) { split_tf32(v, h, l); chat_tf32[(size_t)k * D + d] = h; dd += l * l; }
+      if (chat_tf32) { split_tf32(v, h, l); chat_tf32[(size_t)k * D + d] = h; }
     }
     if (threadIdx.x == 0) { cbias[k] = 0.f; if (cnorm) cnorm[k] = sqrtf(ss) / den; }
   } else {
@@ -59,20 +54,9 @@ __global__ void vlad_centre_prep_kernel(const float* __restrict__ c, int K, int 
     for (int d = threadIdx.x; d < D; d += blockDim.x) {
       float v = row[d], h, l;
       chat[(size_t)k * D + d] = v;
-      if (chat_tf32) { split_tf32(v, h, l); chat_tf32[(size_t)k * D + d] = h; dd += l * l; }
+      if (chat_tf32) { split_tf32(v, h, l); chat_tf32[(size_t)k * D + d] = h; }
     }
     if (threadIdx.x == 0) { cbias[k] = -0.5f * ss; if (cnorm) cnorm[k] = sqrtf(ss); }
-  }
-  if (cdnorm) {
-    __syncthreads();
-    dd = warp_sum(dd);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = dd;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float tot = 0.f;
-      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
-      cdnorm[k] = sqrtf(tot);
-    }
   }
 }
 
@@ -289,6 +273,34 @@ vlad_accumulate2_kernel(const float* __restrict__ x, const int32_t* __restrict__
   }
 }
 
+// ------------------------------------------------------------------ normalisation factors
+// Image b's intra-normalisation scales scale[k] = 1/max(|V_k|,1e-12) (1 without intra_norm) and its global factor
+// 1/max(|(scale_k V_k)_k|,1e-12), from the per-slice sums of squares partial_ss [B,K,nslices], in one fixed order
+// (slices in order, then clusters in order), so every CTA that derives them gets the same bits.  scale and sq are [K]
+// in shared memory; the block's threads stride over k.  __ldcg: within accumulate3 the sums come from other CTAs of
+// the running kernel.  Every thread of the block must call it; it returns the global factor to all of them.
+__device__ __forceinline__ float vlad_norm_factors(const float* partial_ss, int b, int K, int nslices, int intra_norm,
+                                                   float* scale, float* sq) {
+  __shared__ float s_gnorm;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    float ss = 0.f;
+    for (int s = 0; s < nslices; ++s) ss += __ldcg(partial_ss + ((size_t)b * K + k) * nslices + s);
+    const float nk = sqrtf(ss);
+    const float sc = intra_norm ? 1.0f / fmaxf(nk, 1e-12f) : 1.0f;
+    scale[k] = sc;
+    const float nb = nk * sc;                               // norm of the block after intra-normalisation
+    sq[k] = nb * nb;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tot = 0.f;
+    for (int k = 0; k < K; ++k) tot += sq[k];
+    s_gnorm = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
+  }
+  __syncthreads();
+  return s_gnorm;
+}
+
 // ------------------------------------------------------------------ accumulate v3 (+ fused normalisation)
 // CTA = (128-column slice, image), 8 warps, 4-5 CTAs per SM (one wave at the BASELINE shapes).  The image's rows are
 // counting-sorted by label in shared memory (stable: rows of a cluster stay in row order), the sorted list is cut into
@@ -311,19 +323,8 @@ __global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
 vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
                         const float* __restrict__ inv_norm, const float* __restrict__ centers, int N, int D, int K,
                         int norm_descs, int intra_norm, float* vlad, float* partial_ss /* [B,K,nslices] */,
-                        int32_t* done /* [B], zero on entry */, int32_t* reset_ctr /* nullable */, int prefetch, int wait_all,
-                        unsigned long long* dbg /* ANYLOC_VLAD_TIMELINE only: 8 ns stamps per CTA, nullable */) {
-  auto stamp = [&](int i) {
-    if (dbg && threadIdx.x == 0) {
-      unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      dbg[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 8 + i] = t;
-    }
-  };
-  stamp(0);
+                        int32_t* done /* [B], zero on entry */, int wait_all) {
   extern __shared__ __align__(16) int sm3[];
-  // prepared-vocabulary calls: the work-list counter of the assignment stage (already consumed on this stream) is
-  // cleared here for the next call, so no launch is spent on it
-  if (reset_ctr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *reset_ctr = 0;
   int* ooff = sm3;                                          // [N] n * D of the rows, sorted by label (stable)
   int* lab = ooff + N;                                      // [N]
   float* inv_s = reinterpret_cast<float*>(lab + N);         // [N] 1/|x| in the same sorted order
@@ -338,7 +339,6 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
   float* slots = reinterpret_cast<float*>(sm3) +
                  (((size_t)4 * N + 3 * (size_t)(K + 1) + (size_t)ACC3_WARPS * K + 2 * (size_t)K + acc3_max_tasks_dev(N, K) + 3) & ~(size_t)3);
   __shared__ int next_task, s_last;
-  __shared__ float s_gnorm;
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
   // images in reverse order: the assignment pass streamed them in ascending order, so the last ones are the most
   // likely to still sit in L2 when this kernel starts
@@ -352,7 +352,6 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
   for (int i = t; i < ACC3_WARPS * K; i += blockDim.x) cntw[i] = 0;
   if (t == 0) next_task = 0;
   __syncthreads();
-  stamp(1);
   // per-warp histograms over contiguous row chunks
   const int chunk = (((N + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
   const int r0 = min(N, w * chunk), r1 = min(N, r0 + chunk);
@@ -407,27 +406,13 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
     __syncwarp();
   }
   __syncthreads();
-  stamp(2);
-  // tasks -> registers.  Every warp grabs its NEXT task one task early; with `prefetch` it also bulk-prefetches that
-  // task's row segments into L2 (cp.async.bulk.prefetch.L2: no destination registers).  Measured neutral: this phase
-  // already streams at 5.2-5.4 TB/s (profiles/r01_vlad_v3.md, section 4b), so the prefetch is off by default.
+  // tasks -> registers.  Every warp grabs its NEXT task one task early.
   const float* xb = x + (size_t)b * N * D + col;
-  const float* xs = x + (size_t)b * N * D + slice * 128;                     // this slice, lane-independent
-  const uint32_t rowbytes = (uint32_t)min(128, D - slice * 128) * 4u;
   const int ntasks = tstart[K];
   auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
-  auto prefetch_task = [&](int q) {
-    if (q >= ntasks || !prefetch) return;
-    const int k = task_k[q];
-    const int s = start[k] + (q - tstart[k]) * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
-    for (int i = s + lane; i < e; i += 32)
-      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(xs + ooff[i]), "r"(rowbytes) : "memory");
-  };
   int q = grab();
-  prefetch_task(q);
   while (q < ntasks) {
     const int qn = grab();
-    prefetch_task(qn);
     const int k = task_k[q];
     const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
     const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
@@ -471,7 +456,6 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
     q = qn;
   }
   __syncthreads();
-  stamp(3);
   for (int k = w; k < K; k += ACC3_WARPS) {                 // clusters of several tasks: combine in task order
     const int nt = tstart[k + 1] - tstart[k];
     if (nt <= 1) continue;
@@ -493,7 +477,6 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
     s_last = (atomicAdd(&done[b], 1) == nslices - 1);
   }
   __syncthreads();
-  stamp(4);
   if (wait_all) {
     // Whole grid co-resident (checked on the host): every slice-CTA waits until all slices of its image have published
     // their sums of squares, derives the SAME scales in the same order, and normalises ITS OWN 128-column slice -- the
@@ -510,23 +493,7 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
       }
     }
     __syncthreads();
-    for (int k = t; k < K; k += blockDim.x) {
-      float ss = 0.f;
-      for (int s = 0; s < nslices; ++s) ss += __ldcg(partial_ss + ((size_t)b * K + k) * nslices + s);
-      const float nk = sqrtf(ss);
-      const float sc = intra_norm ? 1.0f / fmaxf(nk, 1e-12f) : 1.0f;
-      kss[k] = sc;
-      const float nb = nk * sc;
-      ksq[k] = nb * nb;
-    }
-    __syncthreads();
-    if (t == 0) {
-      float tot = 0.f;
-      for (int k = 0; k < K; ++k) tot += ksq[k];
-      s_gnorm = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
-    }
-    __syncthreads();
-    const float g = s_gnorm;
+    const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
     const int nq = K * 32;                                  // float4 elements of this slice
     constexpr int UW = 8;
     for (int i0 = t; i0 < nq; i0 += blockDim.x * UW) {
@@ -546,31 +513,13 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
         }
       }
     }
-    __syncthreads();
-    stamp(5);
     return;
   }
   if (!s_last) return;
-  // ---- last CTA of this image: intra- and global normalisation (same arithmetic as vlad_normalize_kernel)
+  // ---- last CTA of this image: intra- and global normalisation (same factors as vlad_normalize_kernel)
   __threadfence();
-  for (int k = t; k < K; k += blockDim.x) {
-    float ss = 0.f;
-    for (int s = 0; s < nslices; ++s) ss += __ldcg(partial_ss + ((size_t)b * K + k) * nslices + s);
-    const float nk = sqrtf(ss);
-    const float sc = intra_norm ? 1.0f / fmaxf(nk, 1e-12f) : 1.0f;
-    kss[k] = sc;
-    const float nb = nk * sc;
-    ksq[k] = nb * nb;
-  }
-  __syncthreads();
-  if (t == 0) {
-    float tot = 0.f;
-    for (int k = 0; k < K; ++k) tot += ksq[k];
-    s_gnorm = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
-    done[b] = 0;
-  }
-  __syncthreads();
-  const float g = s_gnorm;
+  if (t == 0) done[b] = 0;
+  const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
   float4* vb = reinterpret_cast<float4*>(vlad + (size_t)b * K * D);
   const int D4 = D >> 2, total4 = K * D4;
   constexpr int UN = 8;                                     // loads batched ahead of the stores (L2 latency chain)
@@ -592,70 +541,10 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
       }
     }
   }
-  __syncthreads();
-  stamp(5);
 }
 
-// ------------------------------------------------------------------ accumulate
+// columns per slice: every VLAD path cuts D into 128-column slices (one thread per column in the kernels below)
 constexpr int ACC_COLS = 128;
-__global__ void __launch_bounds__(ACC_COLS)
-vlad_accumulate_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
-                       const float* __restrict__ inv_norm, const float* __restrict__ centers,
-                       int N, int D, int K, int norm_descs, float* __restrict__ vlad,
-                       float* __restrict__ partial_ss /* [B,K,nslices] */) {
-  extern __shared__ float sm[];
-  float* acc = sm;                    // [K][ACC_COLS]
-  float* cen = sm + (size_t)K * ACC_COLS;  // [K][ACC_COLS]
-  int* lab = reinterpret_cast<int*>(cen + (size_t)K * ACC_COLS);   // [N]
-  float* inv = reinterpret_cast<float*>(lab + N);                  // [N]
-  const int b = blockIdx.y, slice = blockIdx.x, t = threadIdx.x;
-  const int col = slice * ACC_COLS + t;
-  const bool colok = col < D;
-  for (int k = 0; k < K; ++k) {
-    acc[k * ACC_COLS + t] = 0.f;
-    cen[k * ACC_COLS + t] = colok ? centers[(size_t)k * D + col] : 0.f;
-  }
-  for (int n = t; n < N; n += ACC_COLS) {
-    lab[n] = labels[(size_t)b * N + n];
-    inv[n] = norm_descs ? inv_norm[(size_t)b * N + n] : 1.0f;
-  }
-  __syncthreads();
-  const float* xb = x + (size_t)b * N * D + col;
-  if (colok) {
-    int n = 0;
-    for (; n + 4 <= N; n += 4) {
-      float v0 = __ldg(xb + (size_t)(n + 0) * D), v1 = __ldg(xb + (size_t)(n + 1) * D);
-      float v2 = __ldg(xb + (size_t)(n + 2) * D), v3 = __ldg(xb + (size_t)(n + 3) * D);
-      int l0 = lab[n], l1 = lab[n + 1], l2 = lab[n + 2], l3 = lab[n + 3];
-      if (l0 >= 0) acc[l0 * ACC_COLS + t] += v0 * inv[n + 0] - cen[l0 * ACC_COLS + t];
-      if (l1 >= 0) acc[l1 * ACC_COLS + t] += v1 * inv[n + 1] - cen[l1 * ACC_COLS + t];
-      if (l2 >= 0) acc[l2 * ACC_COLS + t] += v2 * inv[n + 2] - cen[l2 * ACC_COLS + t];
-      if (l3 >= 0) acc[l3 * ACC_COLS + t] += v3 * inv[n + 3] - cen[l3 * ACC_COLS + t];
-    }
-    for (; n < N; ++n) {
-      float v = __ldg(xb + (size_t)n * D);
-      int l = lab[n];
-      if (l >= 0) acc[l * ACC_COLS + t] += v * inv[n] - cen[l * ACC_COLS + t];
-    }
-  }
-  __syncthreads();
-  // write un-normalised V and the per-slice sum of squares (warp 0..3 -> fixed order reduce)
-  __shared__ float red[ACC_COLS / 32];
-  const int nslices = gridDim.x;
-  for (int k = 0; k < K; ++k) {
-    float v = acc[k * ACC_COLS + t];
-    if (colok) vlad[((size_t)b * K + k) * D + col] = v;
-    float s = warp_sum(colok ? v * v : 0.f);
-    if ((t & 31) == 0) red[t >> 5] = s;
-    __syncthreads();
-    if (t == 0) {
-      float tot = 0.f;
-      for (int w = 0; w < ACC_COLS / 32; ++w) tot += red[w];
-      partial_ss[((size_t)b * K + k) * nslices + slice] = tot;
-    }
-    __syncthreads();
-  }
-}
 
 // ------------------------------------------------------------------ soft assignment (utilities.py:862-887)
 // a[r,k] = softmax_k(temp * cos(x_r, c_k)) with F.cosine_similarity's clamps (each norm clamped at 1e-8).
@@ -817,26 +706,9 @@ vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restri
 __global__ void __launch_bounds__(256)
 vlad_normalize_kernel(float* __restrict__ vlad, const float* __restrict__ partial_ss, int D, int K,
                       int nslices, int intra_norm) {
-  extern __shared__ float scale[];   // [K]
-  __shared__ float gnorm;
+  extern __shared__ float scale[];   // [2K]: scales, then the blocks' squared norms
   const int b = blockIdx.x;
-  for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    float ss = 0.f;
-    for (int s = 0; s < nslices; ++s) ss += partial_ss[((size_t)b * K + k) * nslices + s];
-    float nk = sqrtf(ss);
-    float sc = intra_norm ? 1.0f / fmaxf(nk, 1e-12f) : 1.0f;
-    scale[k] = sc;
-    // squared norm of the block after intra-normalisation
-    float nb = nk * sc;
-    scale[K + k] = nb * nb;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float tot = 0.f;
-    for (int k = 0; k < K; ++k) tot += scale[K + k];
-    gnorm = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
-  }
-  __syncthreads();
+  const float gnorm = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, scale, scale + K);
   float* v = vlad + (size_t)b * K * D;
   const size_t total = (size_t)K * D;
   for (size_t i = (size_t)blockIdx.y * blockDim.x + threadIdx.x; i < total;
@@ -925,34 +797,9 @@ bool gemm_tc_supported(const void*, const void*, int, const void*, const void*, 
                        bool);
 }  // namespace anyloc
 
-// ANYLOC_VLAD=2 selects the v2 pipeline (coarse GEMM + full rescoring pass + shared-memory accumulate + normalise
-// launch) for A/B measurements; default 3 = streaming tensor-core assignment + sorted register accumulate with the
-// normalisation fused into it.
-static int acc3_prefetch() {      // ANYLOC_VLAD_PREFETCH=1: accumulate3 bulk-prefetches each warp's next task into L2.  Off by
-  static int v = -1;               // default: measured neutral at c2 (86.3 vs 85.7 us) and slightly negative at c5 (276 vs 270 us)
-  if (v < 0) { const char* e = getenv("ANYLOC_VLAD_PREFETCH"); v = e ? atoi(e) : 0; }
-  return v;
-}
-static int vlad_version() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ANYLOC_VLAD"); v = e ? atoi(e) : 3; }
-  return v;
-}
-
-extern "C" size_t anyloc_vlad_workspace_bytes(int B, int N, int D, int K) {
-  size_t R = (size_t)B * N;
-  int nslices = cdiv(D, ACC_COLS);
-  return 2 * align_up((size_t)K * D * 4, 256) + 2 * align_up((size_t)K * 4, 256) + align_up(R * 4, 256) * 2 +
-         align_up(R * (size_t)K * 4, 256) + align_up((size_t)B * K * nslices * 4, 256) +
-         align_up(((size_t)K * D + K) * 4, 256) + align_up((size_t)K * 4, 256) + align_up((size_t)B * 4, 256) +
-         4096;
-}
-
 namespace {
 struct AssignBufs {
   float *chat, *chat_tf32, *cbias, *cnorm, *coarse;
-  float* cdnorm = nullptr;                                                           // v3: |c^ - tf32(c^)| per centre
-  int32_t* amb_count = nullptr;                                                      // reserved word of the prepared blob (round-1 work-list counter; kept zero)
   int32_t* done = nullptr; int n_done = 0;                                           // accumulate3 tickets (optional)
 };
 
@@ -965,7 +812,7 @@ int launch_assign(const float* feats, const int32_t* n_valid, int N_per_img, int
     if (ab.done) ANYLOC_CHECK_CUDA(cudaMemsetAsync(ab.done, 0, (size_t)ab.n_done * sizeof(int32_t), st));
   } else {
     vlad_centre_prep_kernel<<<K, 256, 0, st>>>(centers, K, D, dist_mode, ab.chat, ab.cbias, ab.chat_tf32, ab.cnorm,
-                                               ab.cdnorm, ab.amb_count, ab.amb_count ? 1 : 0, ab.done, ab.done ? ab.n_done : 0);
+                                               ab.done, ab.done ? ab.n_done : 0);
     ANYLOC_CHECK_LAUNCH();
   }
   EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, K};
@@ -1003,11 +850,39 @@ bool take_assign_bufs(Workspace& w, int64_t R, int D, int K, AssignBufs* ab) {
   ab->cbias = w.take<float>(K);
   ab->cnorm = w.take<float>(K);
   ab->coarse = w.take<float>((size_t)R * K);        // may be null when the caller's workspace is the small one
-  ab->cdnorm = w.take<float>(K);
-  ab->amb_count = w.take<int32_t>(64);
   return ab->chat && ab->chat_tf32 && ab->cbias && ab->cnorm;
 }
+
+// The hard path's workspace: labels, 1/|x|, per-slice sums of squares, the assignment buffers and, with `tickets`,
+// the accumulate3 tickets.  It is a superset of the soft path's carve (1/|x|, sums of squares, c^ and the [R,K]
+// assignment in the coarse scores' place) and of anyloc_vlad_assign's, so anyloc_vlad_workspace_bytes sizes all
+// three.  With ws == nullptr it is a dry run; returns the bytes taken, 0 when the workspace is too small.
+struct HardBufs { int32_t* labels; float *inv_norm, *partial; AssignBufs ab; };
+size_t carve_hard(void* ws, size_t ws_bytes, int B, int N, int D, int K, bool tickets, HardBufs* hb) {
+  Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  const size_t R = (size_t)B * N;
+  hb->labels = w.take<int32_t>(R);
+  hb->inv_norm = w.take<float>(R);
+  hb->partial = w.take<float>((size_t)B * K * cdiv(D, ACC_COLS));
+  const bool ok = hb->labels && hb->inv_norm && hb->partial && take_assign_bufs(w, (int64_t)R, D, K, &hb->ab);
+  if (tickets) { hb->ab.done = w.take<int32_t>((size_t)B); hb->ab.n_done = B; }
+  return ok ? w.off : 0;
+}
+
+// intra- and global L2 normalisation of B descriptors [B,K*D] in place, from their per-slice sums of squares
+int launch_normalize(float* vlad, const float* partial, int B, int D, int K, int intra_norm, cudaStream_t st) {
+  const int ysplit = std::max(1, std::min(64, (int)(((size_t)K * D + 256 * 16 - 1) / (256 * 16))));
+  vlad_normalize_kernel<<<dim3(B, ysplit), 256, 2 * K * sizeof(float), st>>>(vlad, partial, D, K, cdiv(D, ACC_COLS),
+                                                                           intra_norm);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
 }  // namespace
+
+extern "C" size_t anyloc_vlad_workspace_bytes(int B, int N, int D, int K) {
+  HardBufs hb;
+  return carve_hard(nullptr, 0, B, N, D, K, true, &hb);
+}
 
 extern "C" int anyloc_vlad_assign(const float* feats, const float* centers, int R, int D, int K,
                                   int dist_mode, int32_t* labels, void* ws, size_t ws_bytes,
@@ -1021,22 +896,22 @@ extern "C" int anyloc_vlad_assign(const float* feats, const float* centers, int 
   return launch_assign(feats, nullptr, R, R, D, K, centers, dist_mode, ab, labels, nullptr, (cudaStream_t)stream);
 }
 
-// Prepared vocabulary blob (anyloc_vlad_prepare): c^ [K,D] | tf32(c^) [K,D] | bias [K] | |c^| [K] | |c^ - tf32(c^)| [K] |
-// work-list counter.  Everything the per-call centre-prep launch would produce.
-struct PreparedView { float *chat, *chat_tf32, *cbias, *cnorm, *cdnorm; int32_t* amb_count; };
-static bool carve_prepared(void* blob, size_t bytes, int D, int K, PreparedView* pv) {
-  Workspace w(blob, bytes);
+// Prepared vocabulary blob (anyloc_vlad_prepare): c^ [K,D] | tf32(c^) [K,D] | bias [K] | |c^| [K].  Everything the
+// per-call centre-prep launch would produce.  With blob == nullptr a dry run; returns the bytes taken, 0 when the blob
+// is too small.
+struct PreparedView { float *chat, *chat_tf32, *cbias, *cnorm; };
+static size_t carve_prepared(void* blob, size_t bytes, int D, int K, PreparedView* pv) {
+  Workspace w(blob ? blob : (void*)256, blob ? bytes : (size_t)-1 / 2);
   pv->chat = w.take<float>((size_t)K * D);
   pv->chat_tf32 = w.take<float>((size_t)K * D);
   pv->cbias = w.take<float>(K);
   pv->cnorm = w.take<float>(K);
-  pv->cdnorm = w.take<float>(K);
-  pv->amb_count = w.take<int32_t>(64);
-  return pv->amb_count != nullptr;
+  return pv->chat && pv->chat_tf32 && pv->cbias && pv->cnorm ? w.off : 0;
 }
 
 extern "C" size_t anyloc_vlad_prepared_bytes(int D, int K) {
-  return 2 * align_up((size_t)K * D * 4, 256) + 3 * align_up((size_t)K * 4, 256) + 256;
+  PreparedView pv;
+  return carve_prepared(nullptr, 0, D, K, &pv);
 }
 
 extern "C" int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_mode, void* prepared,
@@ -1048,7 +923,7 @@ extern "C" int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_
   PreparedView pv;
   if (!carve_prepared(prepared, prepared_bytes, D, K, &pv)) { set_error("vlad_prepare: blob too small"); return ANYLOC_ERR_WORKSPACE; }
   vlad_centre_prep_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(centers, K, D, dist_mode, pv.chat, pv.cbias, pv.chat_tf32,
-                                                               pv.cnorm, pv.cdnorm, pv.amb_count, 1, nullptr, 0);
+                                                               pv.cnorm, nullptr, 0);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -1064,95 +939,55 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
-  Workspace w(ws, ws_bytes);
   const size_t R = (size_t)B * N;
   const int nslices = cdiv(D, ACC_COLS);
-  int32_t* labels = w.take<int32_t>(R);
-  float* inv_norm = w.take<float>(R);
-  float* partial = w.take<float>((size_t)B * K * nslices);
-  AssignBufs ab;
-  if (!labels || !inv_norm || !partial || !take_assign_bufs(w, (int64_t)R, D, K, &ab)) {
+  const size_t smem3 = acc3_smem_bytes(N, K);
+  const bool fits3 = smem3 <= 100 * 1024 && (int64_t)N * D < (1ll << 31);
+  HardBufs hb;
+  if (!carve_hard(ws, ws_bytes, B, N, D, K, fits3, &hb)) {
     set_error("vlad_generate: workspace too small (%zu bytes given)", ws_bytes);
     return ANYLOC_ERR_WORKSPACE;
   }
-  const size_t smem3 = acc3_smem_bytes(N, K);
-  const bool acc3 = vlad_version() >= 3 && smem3 <= 100 * 1024 && (int64_t)N * D < (1ll << 31);
-  if (acc3) { ab.done = w.take<int32_t>((size_t)B); ab.n_done = B; }
-  // prepared vocabulary: usable when this call takes the v3 assignment + accumulate3 route
+  AssignBufs& ab = hb.ab;
+  const bool acc3 = ab.done != nullptr;             // fits3 and room for the tickets
+  // else accumulate2 with as many row-splitting warps as shared memory allows ((1 + warps) * K * 128 floats), at most
+  // 4 row-splitting warps when two CTAs then fit per SM, else what fits in one (signed: K > 400 leaves none)
+  const int warps = (int)std::min<long long>(4, (long long)((200 * 1024) / ((size_t)K * 128 * 4)) - 1);
+  ANYLOC_REQUIRE(acc3 || warps >= 1, "vlad_generate: K=%d N=%d needs %zu B shared memory (accumulate3 has 100 KB)", K,
+                 N, smem3);
+  // a prepared vocabulary replaces the per-call centre prep on every route
   PreparedView pv;
-  const bool use_prep = prepared && acc3 && ab.done && carve_prepared(prepared, prepared_bytes, D, K, &pv);
-  if (use_prep) {
-    ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; ab.cdnorm = pv.cdnorm;
-    ab.amb_count = pv.amb_count;
-  }
+  const bool use_prep = prepared && carve_prepared(prepared, prepared_bytes, D, K, &pv);
+  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
-  int rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, labels, inv_norm, st, use_prep);
+  int rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st,
+                         use_prep);
   if (rc) return rc;
-  if (acc3 && ab.done) {
+  if (acc3) {
     static unsigned long long attr_seen = 0;
     if (first_use_on_this_device(&attr_seen)) {
       ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     }
     // all CTAs co-resident -> the slice-CTAs of an image may wait for each other (distributed normalisation);
-    // otherwise the image's last CTA normalises alone.  ANYLOC_VLAD_WAIT=0 forces the latter (A/B).
+    // otherwise the image's last CTA normalises alone
     int occ = 0;
     ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_kernel, ACC3_WARPS * 32, smem3));
-    static int wait_env = -1;
-    if (wait_env < 0) { const char* e = getenv("ANYLOC_VLAD_WAIT"); wait_env = e ? atoi(e) : 1; }
-    const int wait_all = (wait_env && (long long)nslices * B <= (long long)occ * device_sm_count()) ? 1 : 0;
-    static int timeline = -1;          // ANYLOC_VLAD_TIMELINE=1 (tools only): per-CTA phase stamps, summary on stderr
-    if (timeline < 0) { const char* e = getenv("ANYLOC_VLAD_TIMELINE"); timeline = e ? atoi(e) : 0; }
-    unsigned long long* dbg = nullptr;
-    const size_t nctas = (size_t)nslices * B;
-    if (timeline) { ANYLOC_CHECK_CUDA(cudaMalloc(&dbg, nctas * 64)); ANYLOC_CHECK_CUDA(cudaMemsetAsync(dbg, 0, nctas * 64, st)); }
-    vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(feats, labels, inv_norm, centers, N, D, K,
-                                                                             norm_descs, intra_norm, vlad, partial, ab.done,
-                                                                             use_prep ? ab.amb_count : nullptr, acc3_prefetch(), wait_all, dbg);
+    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
+    vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(feats, hb.labels, hb.inv_norm, centers, N,
+                                                                             D, K, norm_descs, intra_norm, vlad,
+                                                                             hb.partial, ab.done, wait_all);
     ANYLOC_CHECK_LAUNCH();
-    if (timeline) {
-      std::vector<unsigned long long> h(nctas * 8);
-      ANYLOC_CHECK_CUDA(cudaStreamSynchronize(st));
-      ANYLOC_CHECK_CUDA(cudaMemcpy(h.data(), dbg, nctas * 64, cudaMemcpyDeviceToHost));
-      cudaFree(dbg);
-      unsigned long long t0 = ~0ull, t_end = 0;
-      for (size_t c = 0; c < nctas; ++c) t0 = std::min(t0, h[c * 8]);
-      double sum[6] = {0}, mx[6] = {0}; size_t nlast = 0;
-      for (size_t c = 0; c < nctas; ++c) {
-        for (int i = 0; i < 5; ++i) { double v = (double)(h[c * 8 + i] - t0) * 1e-3; sum[i] += v; mx[i] = std::max(mx[i], v); }
-        if (h[c * 8 + 5]) { double v = (double)(h[c * 8 + 5] - t0) * 1e-3; sum[5] += v; mx[5] = std::max(mx[5], v); ++nlast; }
-        t_end = std::max(t_end, std::max(h[c * 8 + 4], h[c * 8 + 5]));
-      }
-      fprintf(stderr, "[accumulate3 timeline, us since first CTA start; mean / max over %zu CTAs] start %.1f/%.1f  labels-loaded %.1f/%.1f  "
-              "sorted %.1f/%.1f  tasks-done %.1f/%.1f  ticket %.1f/%.1f  normalised(%zu CTAs) %.1f/%.1f  kernel-end %.1f\n",
-              nctas, sum[0] / nctas, mx[0], sum[1] / nctas, mx[1], sum[2] / nctas, mx[2], sum[3] / nctas, mx[3], sum[4] / nctas, mx[4],
-              nlast, nlast ? sum[5] / nlast : 0.0, mx[5], (double)(t_end - t0) * 1e-3);
-    }
-    if (labels_out)
-      ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, labels, R * 4, cudaMemcpyDeviceToDevice, st));
-    return ANYLOC_OK;
-  }
-  // v2: accumulate with as many row-splitting warps as shared memory allows ((1 + warps) * K * 128 floats), at most
-  // 4 row-splitting warps when two CTAs then fit per SM, else what fits in one (signed: K > 400 leaves none)
-  int warps = (int)std::min<long long>(4, (long long)((200 * 1024) / ((size_t)K * 128 * 4)) - 1);
-  if (warps >= 1) {
-    size_t smem = (size_t)(1 + warps) * K * 128 * 4;
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, N, D, K, norm_descs,
-                                                                 warps, vlad, partial);
   } else {
-    size_t smem = ((size_t)2 * K * ACC_COLS + 2 * (size_t)N) * 4;
-    ANYLOC_REQUIRE(smem <= 220 * 1024, "vlad_generate: K=%d N=%d needs %zu B shared memory", K, N, smem);
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    vlad_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, smem, st>>>(feats, labels, inv_norm, centers, N, D, K,
-                                                                    norm_descs, vlad, partial);
+    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, hb.labels, hb.inv_norm, centers, N, D, K,
+                                                                 norm_descs, warps, vlad, hb.partial);
+    ANYLOC_CHECK_LAUNCH();
+    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
+    if (rc) return rc;
   }
-  ANYLOC_CHECK_LAUNCH();
-  int ysplit = std::max(1, std::min(64, (int)(((size_t)K * D + 256 * 16 - 1) / (256 * 16))));
-  vlad_normalize_kernel<<<dim3(B, ysplit), 256, 2 * K * sizeof(float), st>>>(vlad, partial, D, K, nslices,
-                                                                           intra_norm);
-  ANYLOC_CHECK_LAUNCH();
   if (labels_out)
-    ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, labels, R * 4, cudaMemcpyDeviceToDevice, st));
+    ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, hb.labels, R * 4, cudaMemcpyDeviceToDevice, st));
   return ANYLOC_OK;
 }
 
@@ -1231,10 +1066,8 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N, D,
                                                                     K, norm_descs, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
-  int ysplit = std::max(1, std::min(64, (int)(((size_t)K * D + 256 * 16 - 1) / (256 * 16))));
-  vlad_normalize_kernel<<<dim3(B, ysplit), 256, 2 * K * sizeof(float), st>>>(vlad, partial, D, K, nslices,
-                                                                           intra_norm);
-  ANYLOC_CHECK_LAUNCH();
+  int rc = launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  if (rc) return rc;
   if (assign_out)
     ANYLOC_CHECK_CUDA(cudaMemcpyAsync(assign_out, assign, R * K * 4, cudaMemcpyDeviceToDevice, st));
   return ANYLOC_OK;
@@ -1463,8 +1296,5 @@ extern "C" int anyloc_vlad_from_residuals(const float* resid, const int32_t* lab
   if (labels) vlad_from_residuals_hard_kernel<<<dim3(nslices, K), ACC_COLS, 0, st>>>(resid, labels, N, D, K, vlad, partial);
   else vlad_from_residuals_soft_kernel<<<nslices, ACC_COLS, 0, st>>>(resid, assign, N, D, K, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
-  int ysplit = std::max(1, std::min(64, (int)(((size_t)K * D + 256 * 16 - 1) / (256 * 16))));
-  vlad_normalize_kernel<<<dim3(1, ysplit), 256, 2 * K * sizeof(float), st>>>(vlad, partial, D, K, nslices, intra_norm);
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  return launch_normalize(vlad, partial, 1, D, K, intra_norm, st);
 }

@@ -96,9 +96,9 @@ int anyloc_vlad_generate(const float* feats, const int32_t* n_valid, const float
  * (utilities.py:216-217 of scripts/dino_v2_vlad.py fits once, then :233-237 generates for every image), so the
  * centre normalisation c/(|c|+1e-8) of fpk cos_sim, its tf32 copy and norms can be computed once.
  * anyloc_vlad_prepare fills a caller-owned device blob (anyloc_vlad_prepared_bytes); anyloc_vlad_generate_prepared
- * is anyloc_vlad_generate minus the per-call centre-prep launch.  The blob also holds a work-list counter that each
- * call leaves at zero: calls sharing a blob must be stream-ordered, and the blob must be re-prepared whenever the
- * centres (or dist_mode) change.  Results are bitwise identical to anyloc_vlad_generate. */
+ * is anyloc_vlad_generate minus the per-call centre-prep launch, on every route.  It only reads the blob, so concurrent
+ * calls may share one once anyloc_vlad_prepare has completed; the blob must be re-prepared whenever the centres (or dist_mode) change.  Results are
+ * bitwise identical to anyloc_vlad_generate. */
 size_t anyloc_vlad_prepared_bytes(int D, int K);
 int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_mode, void* prepared, size_t prepared_bytes,
                         void* stream);

@@ -12,7 +12,7 @@ and every element must satisfy, with u = 2^-24 and the sqrt-style constant of te
     |v - v64|_kj <= 16 u ( g s_k E_kj + (sqrt(D + K) + rho_k) |v64_kj| ),
     E_kj = sqrt(n_k + 2) sum_{l_q = k} (|x^_qj| + |c_kj|),   rho_k = |E_k| / |u_k|  (intra_norm)  or  |E| / |U|.
 
-Derivation from the kernels' arithmetic (accumulate3, accumulate2 and the v1 accumulate all do the same per element):
+Derivation from the kernels' arithmetic (accumulate3 and accumulate2 do the same per element):
   * 1/|x_q| comes from an fp32 sum of D squares (D/128 terms per lane, then a 5-level warp tree), a sqrt and a
     division: a relative error of about (D/256 + 8) u, common to the row.  fl(fl(x_qj s_q) - c_kj) then adds two
     roundings, so each term is off by at most ~(D/256 + 10) u |x^_qj| + u |c_kj|.
@@ -38,15 +38,11 @@ enough to catch them.  Every route of vlad_generate_impl is reached by shape and
 a call makes (anyloc_launch_count) or, for the two normalisations of accumulate3, by the number of CTAs against the SM
 count; NaN canaries surround every output.  The worst bound ratio per (route, input family) is printed at the end."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
-from tests.util import ROOT, dptr
+from tests.util import dptr
 
 pytestmark = pytest.mark.gpu
 
@@ -84,7 +80,7 @@ def note(route, fam, r):
 
 # ------------------------------------------------------------------------------------------------ dispatch mirror
 # vlad_generate_impl, read off vlad.cu: accumulate3 when its shared memory fits 100 KB, else accumulate2 with
-# min(4, 200 KB / (K 128 4) - 1) row-splitting warps, else the v1 accumulate (<= 220 KB) or an error.
+# min(4, 200 KB / (K 128 4) - 1) row-splitting warps, else an error.
 def acc3_smem(N, K):
     tasks, slots = N // 64 + K + 1, 2 * (N // 64) + 2
     return (4 * N + 3 * (K + 1) + 8 * K + 2 * K + tasks + 4) * 4 + slots * 512
@@ -94,23 +90,21 @@ def acc2_warps(K):
     return min(4, (200 * 1024) // (K * 128 * 4) - 1)
 
 
-def accumulate_route(N, D, K, version=3):
-    if version >= 3 and acc3_smem(N, K) <= 100 * 1024 and N * D < 2 ** 31:
+def accumulate_route(N, D, K):
+    if acc3_smem(N, K) <= 100 * 1024 and N * D < 2 ** 31:
         return "accumulate3"
-    if acc2_warps(K) >= 1:
-        return "accumulate2"
-    return "accumulate_v1" if (2 * K * 128 + 2 * N) * 4 <= 220 * 1024 else "error"
+    return "accumulate2" if acc2_warps(K) >= 1 else "error"
 
 
 def fast_assign(R, D):
     return D <= 2048 and R >= 256
 
 
-def expected_launches(B, N, D, K, prepared=False, version=3):
-    """centre prep (unless the prepared blob is used, which only accumulate3 does), coarse GEMM + rescore or the FFMA
-    assignment, then accumulate3 alone or accumulate2 / v1 + normalise"""
-    route = accumulate_route(N, D, K, version)
-    prep = 0 if (prepared and route == "accumulate3") else 1
+def expected_launches(B, N, D, K, prepared=False):
+    """centre prep (unless the prepared blob is used), coarse GEMM + rescore or the FFMA assignment, then accumulate3
+    alone or accumulate2 + normalise"""
+    route = accumulate_route(N, D, K)
+    prep = 0 if prepared else 1
     assign = 2 if fast_assign(B * N, D) else 1
     return prep + assign + (1 if route == "accumulate3" else 2)
 
@@ -303,11 +297,10 @@ def permuted_targets(B, counts, seed):
 
 
 # ----------------------------------------------------------------------------------------- hard VLAD by route
-def run_hard(L, route_name, fam, B, N, D, K, *, case="", dist=COS, norm=1, intra=1, target=None, seed=0,
-             version=3):
+def run_hard(L, route_name, fam, B, N, D, K, *, case="", dist=COS, norm=1, intra=1, target=None, seed=0):
     x, centers = make_inputs(fam, B, N, D, K, seed, target)
     v, lab, launches = generate(L, x, centers, B, N, D, K, dist=dist, norm=norm, intra=intra)
-    assert launches == expected_launches(B, N, D, K, version=version), (launches, route_name)
+    assert launches == expected_launches(B, N, D, K), (launches, route_name)
     assert int(lab.min()) >= 0 and int(lab.max()) < K
     if target is not None:
         assert torch.equal(lab.long(), target), "rows did not land on the clusters they were built for"
@@ -411,9 +404,10 @@ def test_hard_last_cta_normalise(L, sms):
 
 
 @pytest.mark.parametrize("N,K", [(3942, 32), (5329, 32), (4096, 128), (3000, 200)])
-def test_hard_accumulate2(L, N, K):
+def test_hard_accumulate2_prepared(L, N, K):
     """N beyond accumulate3's 100 KB (the demo's 1024-px ViT-G images: 73 x 54 and 73 x 73 patches): accumulate2 with
-    4, 2 or 1 row-splitting warps + the normalise launch.  Bound, batch == single image, prepared == plain"""
+    4, 2 or 1 row-splitting warps + the normalise launch.  Bound, batch == single image, prepared == plain with one
+    launch fewer (no centre prep), and the prepared blob is left as it was"""
     D = 1536 if K == 32 else 1024
     B = 2
     assert accumulate_route(N, D, K) == "accumulate2"
@@ -429,9 +423,12 @@ def test_hard_accumulate2(L, N, K):
     vs, ls, _ = generate(L, x[1:].contiguous(), centers, 1, N, D, K)
     assert torch.equal(vs[0], v[1]) and torch.equal(ls[0], lab[1]), "batch != single image"
     blob = prepare(L, centers, D, K)
+    torch.cuda.synchronize()
+    blob0 = blob.clone()
     vp, lp, lp_launches = generate(L, x, centers, B, N, D, K, blob=blob)
-    assert lp_launches == expected_launches(B, N, D, K, prepared=True) == 5     # per-call centre prep on this route
+    assert lp_launches == expected_launches(B, N, D, K, prepared=True) == 4
     assert torch.equal(vp, v) and torch.equal(lp, lab), "prepared != plain"
+    assert torch.equal(blob, blob0), "generate_prepared changed the prepared blob"
 
 
 @pytest.mark.parametrize("D", [512, 516, 1024, 1028, 2048, 2052, 3072])
@@ -455,38 +452,10 @@ def test_assign_routes(L, D):
         check_labels(x, centers, inner(lab, R), dist, f"assign D={D}")
 
 
-def _v1_main():
-    """ANYLOC_VLAD=2 (read once per process): the v1 accumulate at K = 210 and accumulate2 at a small K"""
-    from anyloc_b200 import _lib as L
-    L.load()
-    res = {}
-    for name, (B, N, D, K) in {"accumulate_v1": (2, 400, 256, 210), "accumulate2": (2, 300, 256, 32)}.items():
-        assert accumulate_route(N, D, K, version=2) == name
-        x, centers = make_inputs("random", B, N, D, K, seed=K)
-        v, lab, launches = generate(L, x, centers, B, N, D, K)
-        v64, bound, _ = hard_reference(x, centers, lab)
-        res[name] = dict(ratio=ratio(v, v64, bound), launches=launches,
-                         expected=expected_launches(B, N, D, K, version=2))
-    print(json.dumps(res))
-
-
-def test_hard_v1_accumulate_subprocess(L):
-    env = dict(os.environ, ANYLOC_VLAD="2", PYTHONPATH=ROOT)
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \
-        ["-c", "from tests.test_vlad_engine_gpu import _v1_main; _v1_main()"]
-    p = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
-    assert p.returncode == 0, p.stderr[-3000:]
-    res = json.loads(p.stdout.strip().splitlines()[-1])
-    for name, r in res.items():
-        note(f"{name} (ANYLOC_VLAD=2)", "random", r["ratio"])
-        assert r["launches"] == r["expected"], (name, r)
-        assert r["ratio"] <= 1.0, (name, r)
-
-
 def test_envelope_errors(L):
     """outside the shared-memory envelope the call returns an error and writes nothing: hard VLAD at K = 256 with
-    N = 4000 (v1 accumulate would need 287 KB), at K = 1000 with N = 2000, and a k-means update whose K needs more than
-    220 KB"""
+    N = 4000 and at K = 1000 with N = 2000 (too many rows for accumulate3's 100 KB, too many clusters for one
+    accumulate2 row-splitting warp), and a k-means update whose K needs more than 220 KB"""
     for B, N, D, K in ((1, 4000, 128, 256), (1, 2000, 64, 1000)):
         assert accumulate_route(N, D, K) == "error"
         x, centers = make_inputs("random", B, N, D, K, seed=K)

@@ -122,10 +122,9 @@ def test_vlad_c5_shape_properties(u):
 
 @pytest.mark.parametrize("B,N,D,K", [(48, 1369, 256, 128), (64, 1369, 1024, 128), (200, 529, 64, 16)])
 def test_vlad_many_tiles_per_cta(u, B, N, D, K):
-    """More 128-row tiles than SMs (the full BASELINE config 5 batch: 87 616 rows = 4-5 tiles per persistent CTA): the
-    per-tile hand-over of ambiguous rows to the re-scoring warps, their double-buffered lists and the all-warp tail on
-    each CTA's last tile.  Labels exact outside the fp64-ambiguous set on two images, descriptors against the oracle,
-    batch == single image (bitwise)."""
+    """More 128-row tiles of the coarse-score GEMM than SMs (the full BASELINE config 5 batch: 87 616 rows = 4-5 tiles
+    per persistent CTA), and many images for the rescoring and accumulate3 passes.  Labels exact outside the
+    fp64-ambiguous set on two images, descriptors against the oracle, batch == single image (bitwise)."""
     g = torch.Generator(device="cuda").manual_seed(B + D)
     x = torch.nn.functional.normalize(torch.randn(B, N, D, device="cuda", generator=g), dim=-1)
     centers = 0.6 * x.reshape(-1, D)[torch.randperm(B * N, device="cuda", generator=g)[:K]].contiguous()
@@ -219,7 +218,8 @@ def test_vlad_fit_cache_roundtrip(u, tmp_path):
 
 def test_vlad_prepared_equals_plain(u):
     """anyloc_vlad_prepare + anyloc_vlad_generate_prepared (centre prep once per vocabulary, the path VLAD.generate*
-    takes) is bitwise identical to the plain anyloc_vlad_generate call, and the blob is reusable across calls."""
+    takes) is bitwise identical to the plain anyloc_vlad_generate call, and the blob is reusable across calls: they
+    leave it byte for byte as anyloc_vlad_prepare wrote it."""
     from anyloc_b200 import _lib
     lib = _lib.load()
     B, N, D, K = 3, 300, 384, 16
@@ -235,11 +235,15 @@ def test_vlad_prepared_equals_plain(u):
             blob = torch.empty(lib.anyloc_vlad_prepared_bytes(D, K), dtype=torch.uint8, device="cuda")
             _lib.check(lib.anyloc_vlad_prepare(_lib.ptr(centers), D, K, 0, _lib.ptr(blob), blob.numel(), _lib.stream_ptr()),
                        "anyloc_vlad_prepare")
+            torch.cuda.synchronize()
+            blob0 = blob.clone()
             for _ in range(2):
                 _lib.check(lib.anyloc_vlad_generate_prepared(_lib.ptr(x), None, _lib.ptr(centers), _lib.ptr(blob), blob.numel(),
                                                              B, N, D, K, 0, 1, 1, _lib.ptr(out), _lib.ptr(labels),
                                                              _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
                            "anyloc_vlad_generate_prepared")
+            torch.cuda.synchronize()
+            assert torch.equal(blob, blob0), "generate_prepared changed the prepared blob"
         else:
             _lib.check(lib.anyloc_vlad_generate(_lib.ptr(x), None, _lib.ptr(centers), B, N, D, K, 0, 1, 1, _lib.ptr(out),
                                                 _lib.ptr(labels), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
