@@ -46,6 +46,10 @@ class VitWeightsStruct(C.Structure):
                 ("cls_token", C.c_void_p), ("blocks", C.POINTER(VitBlock)), ("patch_alpha", C.c_float)]
 
 
+class VitTap(C.Structure):
+    _fields_ = [("layer", C.c_int), ("facet", C.c_int), ("out", C.c_void_p)]
+
+
 _SIGS = {
     "anyloc_last_error": (C.c_char_p, []),
     "anyloc_version": (C.c_int, []),
@@ -105,6 +109,17 @@ _SIGS = {
                                             C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_void_p),
                                             C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
                                             C.c_int, C.c_void_p]),
+    "anyloc_vit_taps_workspace_bytes": (C.c_size_t, [C.POINTER(VitCfg), C.c_int, C.c_int, C.c_int, C.POINTER(VitTap),
+                                                     C.c_int]),
+    "anyloc_vit_extract_taps": (C.c_int, [C.POINTER(VitCfg), C.POINTER(VitWeightsStruct), C.c_void_p, C.c_int, C.c_int,
+                                          C.c_int, C.c_void_p, C.POINTER(VitTap), C.c_int, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
+    "anyloc_vit_taps_varlen_workspace_bytes": (C.c_size_t, [C.POINTER(VitCfg), C.c_int, C.POINTER(C.c_int32),
+                                                            C.POINTER(VitTap), C.c_int]),
+    "anyloc_vit_extract_taps_varlen": (C.c_int, [C.POINTER(VitCfg), C.POINTER(VitWeightsStruct), C.c_int,
+                                                 C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_void_p),
+                                                 C.POINTER(VitTap), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
+                                                 C.c_int, C.c_void_p]),
     "anyloc_gemm_nt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                  C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),

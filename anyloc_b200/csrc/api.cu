@@ -4,6 +4,7 @@
 #include <stdarg.h>
 #include <string.h>
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <vector>
 #include "epilogue.cuh"
@@ -72,6 +73,8 @@ int attention_tc_varlen_launch(const void*, const void*, const VarlenAttnTable&,
 int launch_im2col_varlen(const VarlenImgTable&, int, int, int, void*, void*, bool, cudaStream_t);
 int launch_assemble_varlen(const float*, const float*, const VarlenImgTable&, int, int, float*, cudaStream_t);
 int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, int, int, int, int, float*, cudaStream_t);
+int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
+                   cudaStream_t);
 
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                          int ldb, int M, int N, int K, const EpiParams& ep, int engine, bool f16, cudaStream_t st) {
@@ -226,9 +229,11 @@ extern "C" int anyloc_vit_patch_k(int patch) { return (int)align_up((size_t)3 * 
 namespace {
 struct VitBuffers {
   float *pa_hi, *pa_lo, *ptmp, *x, *y_hi, *y_lo, *qkv, *qkv_lo, *h_hi, *h_lo;
+  float* qkv32;     // [M, 3D] fp32 rows of a tapped layer's qkv GEMM (null unless the tap list needs them)
 };
-// n_patch patch rows and M token rows in all
-size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, void* ws, size_t ws_bytes, VitBuffers* out) {
+// n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`
+size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
+                 VitBuffers* out) {
   const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   VitBuffers b;
@@ -238,32 +243,105 @@ size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, void* ws, size
   b.y_hi = w.take<float>(M * D); b.y_lo = w.take<float>(M * D);
   b.qkv = w.take<float>(M * 3 * D); b.qkv_lo = w.take<float>(M * 3 * D);
   b.h_hi = w.take<float>(M * c->ffn_hidden); b.h_lo = w.take<float>(M * c->ffn_hidden);
+  b.qkv32 = qkv32 ? w.take<float>(M * 3 * D) : nullptr;
   if (out) *out = b;
-  if (ws && (!b.pa_hi || !b.pa_lo || !b.ptmp || !b.x || !b.y_hi || !b.y_lo || !b.qkv || !b.qkv_lo || !b.h_hi || !b.h_lo)) return 0;
+  if (ws && (!b.pa_hi || !b.pa_lo || !b.ptmp || !b.x || !b.y_hi || !b.y_lo || !b.qkv || !b.qkv_lo || !b.h_hi || !b.h_lo ||
+             (qkv32 && !b.qkv32)))
+    return 0;
   return w.off;
-}
-size_t vit_carve(const AnylocVitCfg* c, int B, int H, int W, void* ws, size_t ws_bytes, VitBuffers* out) {
-  const size_t N = (size_t)(H / c->patch) * (W / c->patch);
-  return vit_carve(c, B * N, B * (N + 1), ws, ws_bytes, out);
 }
 
 // The sequences the attention runs over: B images of T tokens each, or (tab != nullptr) the packed images of a
-// variable-length call, n_tiles 64-query tiles in all
+// variable-length call, n_tiles 64-query tiles in all, whose output rows img maps
 struct VitSeqs {
   int B, T;
   const VarlenAttnTable* tab;
   int n_tiles;
   double attn_flops;
+  const VarlenImgTable* img;
 };
+
+// The taps of one call by layer: bit f of mask[l] set = facet f (ANYLOC_FACET_*) of layer l is returned, into
+// out[l][f].  Layers 0..l_max run, each once.
+struct TapPlan {
+  int l_max;
+  std::vector<uint8_t> mask;
+  std::vector<std::array<float*, 4>> out;
+  bool qkv32;          // some layer's fp32 qkv rows are kept (see vit_trunk)
+  int use_cls, norm_descs;
+};
+int popcount3(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1); }
+// Returns false (with the error text set) on an empty list, a bad layer or facet, a repeated tap or (need_out) a null
+// output.
+bool tap_plan(const char* fn, const AnylocVitCfg* cfg, const AnylocVitTap* taps, int n_taps, bool need_out,
+              TapPlan* p) {
+  if (!taps || n_taps < 1) { set_error("%s: no taps", fn); return false; }
+  p->l_max = -1;
+  p->mask.assign(cfg->depth, 0);
+  p->out.assign(cfg->depth, std::array<float*, 4>{});
+  for (int i = 0; i < n_taps; ++i) {
+    const int l = taps[i].layer, f = taps[i].facet;
+    if (l < 0 || l >= cfg->depth) { set_error("%s: tap %d: layer %d out of range [0,%d)", fn, i, l, cfg->depth); return false; }
+    if (f < ANYLOC_FACET_QUERY || f > ANYLOC_FACET_TOKEN) { set_error("%s: tap %d: bad facet %d", fn, i, f); return false; }
+    if (p->mask[l] & (1 << f)) { set_error("%s: tap %d: layer %d facet %d is requested twice", fn, i, l, f); return false; }
+    if (need_out && !taps[i].out) { set_error("%s: tap %d: null output", fn, i); return false; }
+    p->mask[l] |= 1 << f;
+    p->out[l][f] = taps[i].out;
+    p->l_max = std::max(p->l_max, l);
+  }
+  // the fp32 rows are needed at a q/k/v-tapped layer the forward continues through, and at the last layer when it
+  // returns two or three of q, k, v (one alone takes that third's own GEMM)
+  const int last = p->mask[p->l_max];
+  p->qkv32 = (last & 8) ? (last & 7) != 0 : popcount3(last) >= 2;
+  for (int l = 0; l < p->l_max; ++l) p->qkv32 = p->qkv32 || (p->mask[l] & 7) != 0;
+  return true;
+}
 }  // namespace
 
 extern "C" size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W) {
   if (!cfg || B <= 0 || H < cfg->patch || W < cfg->patch) return 0;
-  return vit_carve(cfg, B, H, W, nullptr, 0, nullptr) + 4096;
+  const size_t N = (size_t)(H / cfg->patch) * (W / cfg->patch);
+  return vit_carve(cfg, B * N, B * (N + 1), false, nullptr, 0, nullptr) + 4096;
 }
 
+extern "C" size_t anyloc_vit_taps_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W, const AnylocVitTap* taps,
+                                                  int n_taps) {
+  TapPlan tp;
+  if (!cfg || B <= 0 || H < cfg->patch || W < cfg->patch || !tap_plan("vit_taps_workspace_bytes", cfg, taps, n_taps,
+                                                                      false, &tp))
+    return 0;
+  const size_t N = (size_t)(H / cfg->patch) * (W / cfg->patch);
+  return vit_carve(cfg, B * N, B * (N + 1), tp.qkv32, nullptr, 0, nullptr) + 4096;
+}
+
+// the facet slice of the M token rows in src (row stride ld) -> out
+static int facet_out(const VitSeqs& sq, int M, const float* src, int64_t ld, int D, const TapPlan& tp, float* out,
+                     cudaStream_t st) {
+  if (sq.img)
+    return launch_facet_out_varlen(src, *sq.img, M - (tp.use_cls ? 0 : sq.B), ld, 0, D, tp.use_cls, tp.norm_descs, out,
+                                   st);
+  return launch_facet_out(src, sq.B, sq.T, ld, 0, D, tp.use_cls, tp.norm_descs, out, st);
+}
+
+// the fp32 qkv rows of layer l in bf.qkv32 -> the facets of l the plan asks for and, when `pairs`, the attention's
+// (hi, lo) operands in bf.qkv / bf.qkv_lo (fp16 pairs when f16_attn, else tf32 pairs)
+static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const VitSeqs& sq, const TapPlan& tp, int l,
+                   bool pairs, bool f16_attn, cudaStream_t st) {
+  const int D = c->embed_dim, m = tp.mask[l];
+  const QkvTapOuts o{{(m & 1) ? tp.out[l][0] : nullptr, (m & 2) ? tp.out[l][1] : nullptr,
+                      (m & 4) ? tp.out[l][2] : nullptr}};
+  const int pair = pairs ? (f16_attn ? 2 : 1) : 0;
+  const double rows_out = (double)M - (tp.use_cls ? 0 : sq.B);
+  const double bytes = 12.0 * M * D + (pair ? (pair == 2 ? 12.0 : 24.0) * M * D : 0.0) + 4.0 * rows_out * D * popcount3(m);
+  ProfScope ps(PC_VIT_MISC, st, bytes);
+  return launch_qkv_tap(bf.qkv32, M, sq.T, sq.img, D, pair, pairs ? bf.qkv : nullptr, pairs ? bf.qkv_lo : nullptr, o,
+                        tp.use_cls, tp.norm_descs, st);
+}
+
+// One transformer block over the M token rows in bf.x, in place.  With tp (layer l has q/k/v taps) the qkv GEMM
+// writes fp32 rows and the tap kernel derives the attention's operands and the tapped facets from them.
 static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitBuffers& bf, int M, const VitSeqs& sq,
-                     int engine, cudaStream_t st) {
+                     int engine, cudaStream_t st, const TapPlan* tp = nullptr, int l = 0) {
   const int D = c->embed_dim, Hf = c->ffn_hidden;
   const bool f16 = c->pair_dtype == ANYLOC_PAIR_F16;
   int rc;
@@ -273,10 +351,17 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   // q, k and v leave the qkv GEMM row-major through the plain split epilogue; for the tensor-core attention in the
   // fp16-pair precision they are fp16 pairs of 8*x, the attention kernel's operand format
   const bool f16_attn = engine != ANYLOC_GEMM_SIMT && f16;
-  EpiParams e_qkv{ANYLOC_EPI_BIAS_SPLIT, wb.qkv_b, nullptr, nullptr, bf.qkv, bf.qkv_lo, 3 * D};
-  e_qkv.out_f16 = f16_attn;
-  e_qkv.alpha = wb.qkv_alpha;
-  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
+  if (tp) {
+    EpiParams e_qkv{ANYLOC_EPI_BIAS, wb.qkv_b, nullptr, nullptr, bf.qkv32, nullptr, 3 * D};
+    e_qkv.alpha = wb.qkv_alpha;
+    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
+    if ((rc = qkv_tap(c, bf, M, sq, *tp, l, true, f16_attn, st))) return rc;
+  } else {
+    EpiParams e_qkv{ANYLOC_EPI_BIAS_SPLIT, wb.qkv_b, nullptr, nullptr, bf.qkv, bf.qkv_lo, 3 * D};
+    e_qkv.out_f16 = f16_attn;
+    e_qkv.alpha = wb.qkv_alpha;
+    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
+  }
   if (sq.tab) {
     ProfScope ps(PC_ATTENTION, st, sq.attn_flops);
     if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, bf.y_hi, bf.y_lo,
@@ -301,48 +386,63 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   return gemm_dispatch(bf.h_hi, bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf, e_out, engine, f16, st);
 }
 
-// Blocks 0..layer-1 over the M assembled token rows in bf.x, then the hooked module: the whole block `layer` (token
-// facet) or its norm1 and the requested third of its qkv projection.  *feat = the [M, D] rows the facet reads.
+// Blocks 0..l_max over the M assembled token rows in bf.x, each run once, writing every tap of the plan:
+//  - a layer with q/k/v taps that the forward continues through runs its qkv GEMM into fp32 rows (bf.qkv32), from
+//    which the tap kernel writes the attention's operand pairs and the tapped facets; other layers run unchanged;
+//  - a token tap of layer l is the facet slice of x after block l, before block l + 1 overwrites it;
+//  - the last layer without a token tap exits early after norm1 and what its q/k/v taps need: one facet alone is that
+//    third's own N = D GEMM and the facet slice, two or three are the N = 3D GEMM and the tap kernel without pairs.
 static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
-                     int layer, int facet, int gemm_engine, cudaStream_t st, const float** feat) {
+                     const TapPlan& tp, int gemm_engine, cudaStream_t st) {
   const int D = cfg->embed_dim;
   const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
   int rc;
-  for (int l = 0; l < layer; ++l)
-    if ((rc = vit_block(cfg, w->blocks[l], bf, M, sq, gemm_engine, st))) return rc;
-  const AnylocVitBlock& wb = w->blocks[layer];
-  if (facet == ANYLOC_FACET_TOKEN) {
-    *feat = bf.x;
-    return vit_block(cfg, wb, bf, M, sq, gemm_engine, st);
+  for (int l = 0; l <= tp.l_max; ++l) {
+    const AnylocVitBlock& wb = w->blocks[l];
+    const int qkv = tp.mask[l] & 7;
+    const bool token = (tp.mask[l] & 8) != 0;
+    if (l == tp.l_max && !token) {
+      if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc;
+      if (popcount3(qkv) == 1) {
+        const int facet = qkv == 1 ? 0 : qkv == 2 ? 1 : 2;
+        const size_t woff = (size_t)facet * D * D * (f16 ? 2 : 4);      // bytes: weights are __half or float
+        EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
+        e_f.alpha = wb.qkv_alpha;
+        if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff, (const char*)wb.qkv_w_lo + woff,
+                                D, M, D, D, e_f, gemm_engine, f16, st)))
+          return rc;
+        return facet_out(sq, M, bf.qkv, D, D, tp, tp.out[l][facet], st);
+      }
+      EpiParams e_qkv{ANYLOC_EPI_BIAS, wb.qkv_b, nullptr, nullptr, bf.qkv32, nullptr, 3 * D};
+      e_qkv.alpha = wb.qkv_alpha;
+      if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, gemm_engine, f16,
+                              st)))
+        return rc;
+      return qkv_tap(cfg, bf, M, sq, tp, l, false, false, st);
+    }
+    if ((rc = vit_block(cfg, wb, bf, M, sq, gemm_engine, st, qkv ? &tp : nullptr, l))) return rc;
+    if (token && (rc = facet_out(sq, M, bf.x, D, D, tp, tp.out[l][ANYLOC_FACET_TOKEN], st))) return rc;
   }
-  // q/k/v facet: only the requested third of the qkv projection of block `layer`
-  if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc;
-  const size_t woff = (size_t)facet * D * D * (f16 ? 2 : 4);      // bytes: weights are __half or float
-  EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
-  e_f.alpha = wb.qkv_alpha;
-  *feat = bf.qkv;
-  return gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff, (const char*)wb.qkv_w_lo + woff, D, M, D,
-                       D, e_f, gemm_engine, f16, st);
+  return ANYLOC_OK;
 }
 
-extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img,
-                                  int B, int H, int W, const float* pos_embed, int layer, int facet,
-                                  int use_cls, int norm_descs, float* out, void* ws, size_t ws_bytes,
-                                  int gemm_engine, void* stream) {
-  ANYLOC_REQUIRE(cfg && w && img && pos_embed && out && ws, "vit_extract: null pointer");
+static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B,
+                            int H, int W, const float* pos_embed, const AnylocVitTap* taps, int n_taps, int use_cls,
+                            int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, cudaStream_t st) {
+  ANYLOC_REQUIRE(cfg && w && img && pos_embed && ws, "%s: null pointer", fn);
   ANYLOC_REQUIRE(cfg->patch > 0 && H % cfg->patch == 0 && W % cfg->patch == 0 && H > 0 && W > 0,
-                 "vit_extract: H=%d W=%d must be positive multiples of the patch size %d", H, W, cfg->patch);
-  ANYLOC_REQUIRE(layer >= 0 && layer < cfg->depth, "vit_extract: layer %d out of range [0,%d)", layer, cfg->depth);
-  ANYLOC_REQUIRE(facet >= ANYLOC_FACET_QUERY && facet <= ANYLOC_FACET_TOKEN, "vit_extract: bad facet %d", facet);
-  ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "vit_extract: head_dim must be 64");
-  ANYLOC_REQUIRE(B > 0, "vit_extract: empty batch");
-  cudaStream_t st = (cudaStream_t)stream;
+                 "%s: H=%d W=%d must be positive multiples of the patch size %d", fn, H, W, cfg->patch);
+  TapPlan tp;
+  if (!tap_plan(fn, cfg, taps, n_taps, true, &tp)) return ANYLOC_ERR_ARG;
+  tp.use_cls = use_cls; tp.norm_descs = norm_descs;
+  ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "%s: head_dim must be 64", fn);
+  ANYLOC_REQUIRE(B > 0, "%s: empty batch", fn);
   const int P = cfg->patch, N = (H / P) * (W / P), T = N + 1, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P);
   const int M = B * T;
   VitBuffers bf;
-  if (!vit_carve(cfg, B, H, W, ws, ws_bytes, &bf)) {
-    set_error("vit_extract: workspace too small (%zu given, %zu needed)", ws_bytes,
-              anyloc_vit_workspace_bytes(cfg, B, H, W));
+  if (!vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, ws, ws_bytes, &bf)) {
+    set_error("%s: workspace too small (%zu given, %zu needed)", fn, ws_bytes,
+              vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
   int rc;
@@ -353,10 +453,26 @@ extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeight
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, B * N, D, Kp, e_pe,
                           gemm_engine, f16, st))) return rc;
   if ((rc = launch_assemble(bf.ptmp, w->cls_token, pos_embed, B, N, D, bf.x, st))) return rc;
-  const VitSeqs sq{B, T, nullptr, 0, 0.0};
-  const float* feat = nullptr;
-  if ((rc = vit_trunk(cfg, w, bf, M, sq, layer, facet, gemm_engine, st, &feat))) return rc;
-  return launch_facet_out(feat, B, T, D, 0, D, use_cls, norm_descs, out, st);
+  const VitSeqs sq{B, T, nullptr, 0, 0.0, nullptr};
+  return vit_trunk(cfg, w, bf, M, sq, tp, gemm_engine, st);
+}
+
+extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img,
+                                  int B, int H, int W, const float* pos_embed, int layer, int facet,
+                                  int use_cls, int norm_descs, float* out, void* ws, size_t ws_bytes,
+                                  int gemm_engine, void* stream) {
+  ANYLOC_REQUIRE(cfg && out, "vit_extract: null pointer");
+  const AnylocVitTap tap{layer, facet, out};
+  return vit_extract_taps("vit_extract", cfg, w, img, B, H, W, pos_embed, &tap, 1, use_cls, norm_descs, ws, ws_bytes,
+                          gemm_engine, (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_vit_extract_taps(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B, int H,
+                                       int W, const float* pos_embed, const AnylocVitTap* taps, int n_taps, int use_cls,
+                                       int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, void* stream) {
+  ANYLOC_REQUIRE(cfg, "vit_extract_taps: null pointer");
+  return vit_extract_taps("vit_extract_taps", cfg, w, img, B, H, W, pos_embed, taps, n_taps, use_cls, norm_descs, ws,
+                          ws_bytes, gemm_engine, (cudaStream_t)stream);
 }
 
 namespace {
@@ -414,34 +530,42 @@ bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* 
 extern "C" size_t anyloc_vit_varlen_workspace_bytes(const AnylocVitCfg* cfg, int B, const int32_t* hw) {
   VarlenPlan p;
   if (!varlen_plan(cfg, B, hw, &p)) return 0;
-  return vit_carve(cfg, (size_t)p.n_patch, (size_t)p.n_tok, nullptr, 0, nullptr) + 4096;
+  return vit_carve(cfg, (size_t)p.n_patch, (size_t)p.n_tok, false, nullptr, 0, nullptr) + 4096;
 }
 
-extern "C" int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
-                                         const float* const* img, const int32_t* hw, const float* const* pos_embed,
-                                         int layer, int facet, int use_cls, int norm_descs, float* out, void* ws,
-                                         size_t ws_bytes, int gemm_engine, void* stream) {
-  ANYLOC_REQUIRE(cfg && w && img && pos_embed && out && ws, "vit_extract_varlen: null pointer");
-  ANYLOC_REQUIRE(layer >= 0 && layer < cfg->depth, "vit_extract_varlen: layer %d out of range [0,%d)", layer,
-                 cfg->depth);
-  ANYLOC_REQUIRE(facet >= ANYLOC_FACET_QUERY && facet <= ANYLOC_FACET_TOKEN, "vit_extract_varlen: bad facet %d", facet);
-  ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "vit_extract_varlen: head_dim must be 64");
+extern "C" size_t anyloc_vit_taps_varlen_workspace_bytes(const AnylocVitCfg* cfg, int B, const int32_t* hw,
+                                                         const AnylocVitTap* taps, int n_taps) {
+  VarlenPlan p;
+  TapPlan tp;
+  if (!varlen_plan(cfg, B, hw, &p) || !tap_plan("vit_taps_varlen_workspace_bytes", cfg, taps, n_taps, false, &tp))
+    return 0;
+  return vit_carve(cfg, (size_t)p.n_patch, (size_t)p.n_tok, tp.qkv32, nullptr, 0, nullptr) + 4096;
+}
+
+static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
+                                   const float* const* img, const int32_t* hw, const float* const* pos_embed,
+                                   const AnylocVitTap* taps, int n_taps, int use_cls, int norm_descs, void* ws,
+                                   size_t ws_bytes, int gemm_engine, cudaStream_t st) {
+  ANYLOC_REQUIRE(cfg && w && img && pos_embed && ws, "%s: null pointer", fn);
+  TapPlan tp;
+  if (!tap_plan(fn, cfg, taps, n_taps, true, &tp)) return ANYLOC_ERR_ARG;
+  tp.use_cls = use_cls; tp.norm_descs = norm_descs;
+  ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "%s: head_dim must be 64", fn);
   if (gemm_engine == ANYLOC_GEMM_SIMT) {
-    set_error("vit_extract_varlen: needs the tensor-core attention (gemm_engine auto or tc3, not simt)");
+    set_error("%s: needs the tensor-core attention (gemm_engine auto or tc3, not simt)", fn);
     return ANYLOC_ERR_UNSUPPORTED;
   }
-  ANYLOC_REQUIRE(gemm_engine == ANYLOC_GEMM_AUTO || gemm_engine == ANYLOC_GEMM_TC3,
-                 "vit_extract_varlen: bad gemm_engine %d", gemm_engine);
+  ANYLOC_REQUIRE(gemm_engine == ANYLOC_GEMM_AUTO || gemm_engine == ANYLOC_GEMM_TC3, "%s: bad gemm_engine %d", fn,
+                 gemm_engine);
   VarlenPlan p;
   if (!varlen_plan(cfg, B, hw, &p)) return ANYLOC_ERR_ARG;
   for (int i = 0; i < B; ++i)
-    ANYLOC_REQUIRE(img[i] && pos_embed[i], "vit_extract_varlen: null image or positional table %d", i);
-  cudaStream_t st = (cudaStream_t)stream;
+    ANYLOC_REQUIRE(img[i] && pos_embed[i], "%s: null image or positional table %d", fn, i);
   const int P = cfg->patch, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P), M = p.n_tok;
   VitBuffers bf;
-  if (!vit_carve(cfg, (size_t)p.n_patch, (size_t)M, ws, ws_bytes, &bf)) {
-    set_error("vit_extract_varlen: workspace too small (%zu given, %zu needed)", ws_bytes,
-              anyloc_vit_varlen_workspace_bytes(cfg, B, hw));
+  if (!vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, ws, ws_bytes, &bf)) {
+    set_error("%s: workspace too small (%zu given, %zu needed)", fn, ws_bytes,
+              vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
   int rc;
@@ -454,9 +578,26 @@ extern "C" int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVi
                           gemm_engine, f16, st))) return rc;
   for (int i = 0; i < B; ++i) p.img.ptr[i] = pos_embed[i];
   if ((rc = launch_assemble_varlen(bf.ptmp, w->cls_token, p.img, M, D, bf.x, st))) return rc;
-  const VitSeqs sq{B, 0, &p.attn, p.n_tiles, p.attn_flops};
-  const float* feat = nullptr;
-  if ((rc = vit_trunk(cfg, w, bf, M, sq, layer, facet, gemm_engine, st, &feat))) return rc;
-  const int rows = M - (use_cls ? 0 : B);
-  return launch_facet_out_varlen(feat, p.img, rows, D, 0, D, use_cls, norm_descs, out, st);
+  const VitSeqs sq{B, 0, &p.attn, p.n_tiles, p.attn_flops, &p.img};
+  return vit_trunk(cfg, w, bf, M, sq, tp, gemm_engine, st);
+}
+
+extern "C" int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
+                                         const float* const* img, const int32_t* hw, const float* const* pos_embed,
+                                         int layer, int facet, int use_cls, int norm_descs, float* out, void* ws,
+                                         size_t ws_bytes, int gemm_engine, void* stream) {
+  ANYLOC_REQUIRE(cfg && out, "vit_extract_varlen: null pointer");
+  const AnylocVitTap tap{layer, facet, out};
+  return vit_extract_taps_varlen("vit_extract_varlen", cfg, w, B, img, hw, pos_embed, &tap, 1, use_cls, norm_descs, ws,
+                                 ws_bytes, gemm_engine, (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
+                                              const float* const* img, const int32_t* hw,
+                                              const float* const* pos_embed, const AnylocVitTap* taps, int n_taps,
+                                              int use_cls, int norm_descs, void* ws, size_t ws_bytes, int gemm_engine,
+                                              void* stream) {
+  ANYLOC_REQUIRE(cfg, "vit_extract_taps_varlen: null pointer");
+  return vit_extract_taps_varlen("vit_extract_taps_varlen", cfg, w, B, img, hw, pos_embed, taps, n_taps, use_cls,
+                                 norm_descs, ws, ws_bytes, gemm_engine, (cudaStream_t)stream);
 }

@@ -126,6 +126,11 @@ struct VarlenAttnTable {
 };
 static_assert(sizeof(VarlenAttnTable) <= 4096, "kernel parameter over 4 KB");
 
+// where the qkv tap kernel writes the q, k and v facet rows of one layer (null: that facet is not tapped)
+struct QkvTapOuts {
+  float* out[3];
+};
+
 int device_sm_count();
 // true the first time it is called on the CURRENT device for this flag word: cudaFuncSetAttribute is per device, so a
 // process that drives several GPUs must repeat it on each of them (one bit per device ordinal; atomic because two host

@@ -1,8 +1,9 @@
 // Element-wise / row-wise pieces of the DINOv2 forward (upstream dinov2 DinoVisionTransformer,
 // reached from /root/reference/utilities.py:269): im2col for the 14x14/s14 patch embedding,
 // token assembly (+cls, +pos-embed), LayerNorm (eps 1e-6) fused with the tf32 (hi,lo) split
-// that feeds the tensor-core GEMMs, and the facet slice + F.normalize epilogue of
-// DinoV2ExtractFeatures.__call__ (utilities.py:270-283).
+// that feeds the tensor-core GEMMs, the facet slice + F.normalize epilogue of
+// DinoV2ExtractFeatures.__call__ (utilities.py:270-283), and the qkv tap that keeps the q/k/v facets of a layer the
+// forward continues through.
 #include "common.cuh"
 
 namespace anyloc {
@@ -168,6 +169,11 @@ l2norm_rows_kernel(const float* __restrict__ x, int64_t rows, int D, int64_t ld_
   }
 }
 
+// the arithmetic of the facet slice's F.normalize, shared by facet_row and the qkv tap: each lane sums the squares
+// of its float4s d = lane, lane + 32, ... in that order, then every element is divided by max(|x|, 1e-12)
+__device__ __forceinline__ float sumsq_add(float ss, float4 v) { return ss + (v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w); }
+__device__ __forceinline__ float4 div4(float4 v, float nrm) { v.x /= nrm; v.y /= nrm; v.z /= nrm; v.w /= nrm; return v; }
+
 // one token row -> one output row (normalised if do_norm), one warp
 __device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x, int D, int do_norm,
                                           float* __restrict__ y) {
@@ -175,13 +181,98 @@ __device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x,
   float4* yr = reinterpret_cast<float4*>(y);
   const int D4 = D >> 2;
   float ss = 0.f;
-  for (int d = lane; d < D4; d += 32) { float4 v = xr[d]; ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w; }
+  for (int d = lane; d < D4; d += 32) ss = sumsq_add(ss, xr[d]);
   const float nrm = fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
   for (int d = lane; d < D4; d += 32) {
     float4 v = xr[d];
-    if (do_norm) { v.x /= nrm; v.y /= nrm; v.z /= nrm; v.w /= nrm; }
+    if (do_norm) v = div4(v, nrm);
     yr[d] = v;
   }
+}
+
+// One fp32 row [q | k | v] of a tapped layer's qkv GEMM (3D columns, one warp, each element read once) -> the
+// attention's operand pairs of the row, in the format the qkv GEMM's split epilogue writes (pair: 0 none, 1 tf32
+// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split), and the rows of the requested facets (out[f] != null),
+// through facet_row's arithmetic.
+template <int MAXV>     // float4 per lane and third: D <= 128 * MAXV
+__device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int pair, void* hi,
+                                            void* lo, const QkvTapOuts& o, int64_t orow, int do_norm) {
+  const int D4 = D >> 2;
+#pragma unroll 1
+  for (int f = 0; f < 3; ++f) {
+    const float4* xr = reinterpret_cast<const float4*>(src + (size_t)f * D);
+    float4 v[MAXV];
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i)
+      if (lane + i * 32 < D4) v[i] = xr[lane + i * 32];
+    if (pair == 2) {
+      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
+      uint2* l2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(lo) + (size_t)f * D);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int d = lane + i * 32;
+        if (d < D4) {
+          uint2 h, l;
+          split_f16x2(v[i].x * kActScale, v[i].y * kActScale, h.x, l.x);
+          split_f16x2(v[i].z * kActScale, v[i].w * kActScale, h.y, l.y);
+          h2[d] = h; l2[d] = l;
+        }
+      }
+    } else if (pair == 1) {
+      float4* h4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(hi) + (size_t)f * D);
+      float4* l4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(lo) + (size_t)f * D);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int d = lane + i * 32;
+        if (d < D4) {
+          float4 h, l;
+          split_tf32(v[i].x, h.x, l.x); split_tf32(v[i].y, h.y, l.y); split_tf32(v[i].z, h.z, l.z); split_tf32(v[i].w, h.w, l.w);
+          h4[d] = h; l4[d] = l;
+        }
+      }
+    }
+    float* out = f == 0 ? o.out[0] : f == 1 ? o.out[1] : o.out[2];     // (not o.out[f]: no local-memory copy)
+    if (out == nullptr || orow < 0) continue;
+    float4* yr = reinterpret_cast<float4*>(out + orow * D);
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i)
+      if (lane + i * 32 < D4) ss = sumsq_add(ss, v[i]);
+    const float nrm = fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i)
+      if (lane + i * 32 < D4) yr[lane + i * 32] = do_norm ? div4(v[i], nrm) : v[i];
+  }
+}
+
+// B images of T tokens: token row r -> output row r (use_cls) or r - b - 1 (its cls row has none)
+template <int MAXV>
+__global__ void __launch_bounds__(256)
+qkv_tap_kernel(const float* __restrict__ src, int M, int T, int D, int pair, void* hi, void* lo, const QkvTapOuts o,
+               int use_cls, int do_norm) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= M) return;
+  const int b = row / T, t = row - b * T;
+  const int64_t orow = use_cls ? row : (t == 0 ? -1 : row - b - 1);
+  const size_t e = (size_t)row * 3 * D * (pair == 2 ? 2 : 4);     // byte offset of the row's pairs
+  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
+                    pair ? (char*)lo + e : nullptr, o, orow, do_norm);
+}
+
+// images of different sizes packed row after row: image i's tokens from tab.tok0[i]
+template <int MAXV>
+__global__ void __launch_bounds__(256)
+qkv_tap_varlen_kernel(const float* __restrict__ src, const __grid_constant__ VarlenImgTable tab, int M, int D, int pair,
+                      void* hi, void* lo, const QkvTapOuts o, int use_cls, int do_norm) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= M) return;
+  const int i = varlen_image_of(tab, row, 0);
+  const int64_t orow = use_cls ? row : (row == tab.tok0[i] ? -1 : row - i - 1);
+  const size_t e = (size_t)row * 3 * D * (pair == 2 ? 2 : 4);
+  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
+                    pair ? (char*)lo + e : nullptr, o, orow, do_norm);
 }
 
 // gather token rows [B, T, ld] (skipping cls unless use_cls, column offset col0) -> [B, T', D] then normalise
@@ -275,6 +366,23 @@ int launch_assemble_varlen(const float* patch, const float* cls, const VarlenImg
 int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int rows, int64_t ld, int col0, int D,
                             int use_cls, int do_norm, float* out, cudaStream_t st) {
   facet_out_varlen_kernel<<<(rows + 7) / 8, 256, 0, st>>>(src, tab, rows, ld, col0, D, use_cls, do_norm, out);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none) and facet rows; tab: packed images, else
+// B images of T tokens
+template <int MAXV>
+static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi,
+                           void* lo, const QkvTapOuts& o, int use_cls, int do_norm, cudaStream_t st) {
+  if (tab) qkv_tap_varlen_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, pair, hi, lo, o, use_cls, do_norm);
+  else qkv_tap_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, M, T, D, pair, hi, lo, o, use_cls, do_norm);
+}
+int launch_qkv_tap(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi, void* lo,
+                   const QkvTapOuts& o, int use_cls, int do_norm, cudaStream_t st) {
+  ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "qkv_tap: D=%d unsupported (multiple of 4, <= 2048)", D);
+  if (D <= 512) qkv_tap_launch<4>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
+  else if (D <= 1024) qkv_tap_launch<8>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
+  else qkv_tap_launch<16>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

@@ -276,44 +276,22 @@ class _HookHandle:
         pass
 
 
-class DinoV2ExtractFeatures:
-    """Extract features from an intermediate layer of DINOv2 (utilities.py:219-288).
+class _GuardedExtractor:
+    """What DinoV2ExtractFeatures and DinoV2MultiExtractFeatures share: the uploaded backbone (blocks 0.._depth()-1),
+    the precision choice and the fp16-range guard around each call.  A subclass sets the call options and defines
+    `_depth()` and `_extract(img)` -> (every output row in one tensor, what __call__ returns)."""
 
-    Same constructor and call signature.  The forward stops at the hooked module (blocks
-    0..layer-1, then either the whole block `layer` ("token") or norm1 + the requested third of
-    its qkv projection), which is output-identical to the reference's full forward + hook.
-    Extra keyword-only arguments: `weights` (an upstream state_dict, else see
-    vit.resolve_state_dict), `gemm_engine` ("auto" | "tc3" | "simt") and `precision`: how fp32
-    operands are fed to the tensor cores -- "tf32x3" (tf32 (hi,lo) pairs, full fp32 exponent range),
-    "f16x3" (fp16 (hi,lo) pairs with power-of-two scaling: same ~22-bit products on the 2x faster
-    kind::f16 path; operands beyond the fp16 range overflow to inf/NaN instead of losing accuracy
-    silently, and the call raises) or "auto" (the default: f16x3 until a call overflows, then that
-    call is redone and the extractor stays in tf32x3 -- trained DINOv2 checkpoints have outlier
-    activations that random-init weights do not).  All accumulate in fp32 with round-to-nearest
-    chunk accumulation."""
-
-    def __init__(self, dino_model: _DINO_V2_MODELS, layer: int, facet: _DINO_FACETS = "token",
-                 use_cls=False, norm_descs=True, device: str = "cpu", *, weights=None,
-                 gemm_engine: str = "auto", precision: str = None) -> None:
-        self.vit_type: str = dino_model
-        self.device = torch.device(device)
-        dev = _lib.require_cuda(self.device)
-        if facet not in _lib.FACET:
-            raise ValueError(f"facet must be one of {sorted(_lib.FACET)}, got {facet!r}")
+    def _load(self, dino_model, dev, weights, gemm_engine, precision):
         sd = weights if weights is not None else _vit.resolve_state_dict(dino_model, dev)
-        # only blocks 0..layer are ever executed (early exit), so only those are uploaded
+        # only the blocks the forward runs (early exit at the deepest hooked module) are uploaded
         precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
         if precision not in ("tf32x3", "f16x3", "auto"):
             raise ValueError(f"precision must be 'auto', 'tf32x3' or 'f16x3', got {precision!r}")
         self._auto = precision == "auto"
         self._state_dict = sd if self._auto else None     # kept for the tf32x3 re-upload on an fp16-range overflow
         self.precision = "f16x3" if self._auto else precision
-        self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=layer + 1,
+        self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=self._depth(),
                                           pair="f16" if self.precision == "f16x3" else "tf32")
-        self.layer: int = layer
-        self.facet = facet
-        self.use_cls = use_cls
-        self.norm_descs = norm_descs
         self.gemm_engine = gemm_engine
         self.fh_handle = _HookHandle()
         self._hook_out = None
@@ -340,23 +318,11 @@ class DinoV2ExtractFeatures:
         dev, name = self.dino_model.device, self.dino_model.name
         self.dino_model = None
         torch.cuda.empty_cache()
-        self.dino_model = _vit.VitWeights(name, self._state_dict, dev, depth=self.layer + 1, pair="tf32")
+        self.dino_model = _vit.VitWeights(name, self._state_dict, dev, depth=self._depth(), pair="tf32")
         self.precision, self._auto, self._state_dict = "tf32x3", False, None
 
-    def _extract(self, img):
-        """-> (every output row in one tensor, what __call__ returns)"""
-        if isinstance(img, (list, tuple)):
-            packed, n = self.dino_model.extract_varlen(img, self.layer, self.facet, self.use_cls, self.norm_descs,
-                                                       self.gemm_engine)
-            return packed, list(packed.split(n))
-        out = self.dino_model.extract(img, self.layer, self.facet, self.use_cls, self.norm_descs, self.gemm_engine)
-        return out, out
-
-    def __call__(self, img):
-        """img [B,3,H,W] -> [B, N(+1), D]; or a list/tuple of differently sized images [3,H_i,W_i] / [1,3,H_i,W_i],
-        all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
-        pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
-        image of fewer than 32 tokens takes the SIMT GEMMs)."""
+    def _guarded(self, img):
+        """self._extract(img)[1] under the fp16-range guard: every output row is checked in one reduction"""
         with torch.no_grad():
             if self.check_finite == "deferred" and not self._auto:
                 self.raise_if_overflowed()
@@ -374,8 +340,98 @@ class DinoV2ExtractFeatures:
             self._switch_to_tf32()
             return self._extract(img)[1]
 
+
+class DinoV2ExtractFeatures(_GuardedExtractor):
+    """Extract features from an intermediate layer of DINOv2 (utilities.py:219-288).
+
+    Same constructor and call signature.  The forward stops at the hooked module (blocks
+    0..layer-1, then either the whole block `layer` ("token") or norm1 + the requested third of
+    its qkv projection), which is output-identical to the reference's full forward + hook.
+    Extra keyword-only arguments: `weights` (an upstream state_dict, else see
+    vit.resolve_state_dict), `gemm_engine` ("auto" | "tc3" | "simt") and `precision`: how fp32
+    operands are fed to the tensor cores -- "tf32x3" (tf32 (hi,lo) pairs, full fp32 exponent range),
+    "f16x3" (fp16 (hi,lo) pairs with power-of-two scaling: same ~22-bit products on the 2x faster
+    kind::f16 path; operands beyond the fp16 range overflow to inf/NaN instead of losing accuracy
+    silently, and the call raises) or "auto" (the default: f16x3 until a call overflows, then that
+    call is redone and the extractor stays in tf32x3 -- trained DINOv2 checkpoints have outlier
+    activations that random-init weights do not).  All accumulate in fp32 with round-to-nearest
+    chunk accumulation."""
+
+    def __init__(self, dino_model: _DINO_V2_MODELS, layer: int, facet: _DINO_FACETS = "token",
+                 use_cls=False, norm_descs=True, device: str = "cpu", *, weights=None,
+                 gemm_engine: str = "auto", precision: str = None) -> None:
+        self.vit_type: str = dino_model
+        self.device = torch.device(device)
+        dev = _lib.require_cuda(self.device)
+        if facet not in _lib.FACET:
+            raise ValueError(f"facet must be one of {sorted(_lib.FACET)}, got {facet!r}")
+        self.layer: int = layer
+        self.facet = facet
+        self.use_cls = use_cls
+        self.norm_descs = norm_descs
+        self._load(dino_model, dev, weights, gemm_engine, precision)
+
+    def _depth(self):
+        return self.layer + 1
+
+    def _extract(self, img):
+        """-> (every output row in one tensor, what __call__ returns)"""
+        if isinstance(img, (list, tuple)):
+            packed, n = self.dino_model.extract_varlen(img, self.layer, self.facet, self.use_cls, self.norm_descs,
+                                                       self.gemm_engine)
+            return packed, list(packed.split(n))
+        out = self.dino_model.extract(img, self.layer, self.facet, self.use_cls, self.norm_descs, self.gemm_engine)
+        return out, out
+
+    def __call__(self, img):
+        """img [B,3,H,W] -> [B, N(+1), D]; or a list/tuple of differently sized images [3,H_i,W_i] / [1,3,H_i,W_i],
+        all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
+        pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
+        image of fewer than 32 tokens takes the SIMT GEMMs)."""
+        return self._guarded(img)
+
     def __del__(self):
         pass
+
+
+class DinoV2MultiExtractFeatures(_GuardedExtractor):
+    """Extension (not in the reference): the features of several (layer, facet) taps of DINOv2 from ONE forward pass.
+
+    AnyLoc's layer and facet ablations read many taps of the same images (scripts/dino_v2_vlad_ablations.sh,
+    dino_v2_vlad_viz.py, dino_v2_sim_facets.py); with one DinoV2ExtractFeatures per tap each of them reruns blocks
+    0..layer and uploads its own weights.  Here blocks 0..max(layer) are uploaded once and run once per call, and every
+    tap keeps what that pass computes.  `taps` is a list of distinct (layer, facet) pairs; `use_cls`, `norm_descs`,
+    `device`, `weights`, `gemm_engine` and `precision` mean what they mean for DinoV2ExtractFeatures and apply to
+    every tap.  Each output is bit-identical to DinoV2ExtractFeatures(dino_model, layer, facet, use_cls, norm_descs)
+    on the same images with the same weights, precision and engine."""
+
+    def __init__(self, dino_model: _DINO_V2_MODELS, taps, use_cls=False, norm_descs=True, device: str = "cpu", *,
+                 weights=None, gemm_engine: str = "auto", precision: str = None) -> None:
+        self.vit_type: str = dino_model
+        self.device = torch.device(device)
+        dev = _lib.require_cuda(self.device)
+        if dino_model not in _vit.ARCHS:
+            raise ValueError(f"unknown DINOv2 model {dino_model!r}; expected one of {sorted(_vit.ARCHS)}")
+        self.taps = _vit.check_taps(taps, _vit.ARCHS[dino_model][1])
+        self.use_cls = use_cls
+        self.norm_descs = norm_descs
+        self._load(dino_model, dev, weights, gemm_engine, precision)
+
+    def _depth(self):
+        return 1 + max(layer for layer, _ in self.taps)
+
+    def _extract(self, img):
+        if isinstance(img, (list, tuple)):
+            packed, n = self.dino_model.extract_taps_varlen(img, self.taps, self.use_cls, self.norm_descs,
+                                                            self.gemm_engine)
+            return packed, {t: list(packed[k].split(n)) for k, t in enumerate(self.taps)}
+        packed = self.dino_model.extract_taps(img, self.taps, self.use_cls, self.norm_descs, self.gemm_engine)
+        return packed, {t: packed[k] for k, t in enumerate(self.taps)}
+
+    def __call__(self, img):
+        """img [B,3,H,W] -> {(layer, facet): [B, N(+1), D]}; a list/tuple of differently sized images (as for
+        DinoV2ExtractFeatures) -> {(layer, facet): [list of [n_i, D]]}.  All outputs are views of one allocation."""
+        return self._guarded(img)
 
 
 # ------------------------------------------------------------------ VLAD

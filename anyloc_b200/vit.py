@@ -8,6 +8,7 @@ loads (facebookresearch/dinov2; spec in SURVEY.md Appendix A).
 """
 import ctypes as C
 import math
+import operator
 import os
 
 import torch
@@ -245,6 +246,86 @@ class VitWeights:
                                                    _lib.ENGINE[engine], _lib.stream_ptr())
                 _lib.check(rc, "anyloc_vit_extract_varlen")
         return out, lay.n_out
+
+    def _tap_array(self, taps, out):
+        """taps [(layer, facet)] and their outputs out[k] -> the library's tap array"""
+        return (_lib.VitTap * len(taps))(*[_lib.VitTap(l, _lib.FACET[f], o.data_ptr()) for (l, f), o in zip(taps, out)])
+
+    def extract_taps(self, img, taps, use_cls=False, norm_descs=True, engine="auto"):
+        """Several (layer, facet) features of img [B,3,H,W] from one forward pass (anyloc_vit_extract_taps) ->
+        [len(taps), B, N(+1), D] fp32; item k is taps[k]'s output, equal bit for bit to extract(img, *taps[k])."""
+        if img.dim() != 4 or img.shape[1] != 3:
+            raise ValueError(f"expected an image batch [B,3,H,W], got {tuple(img.shape)}")
+        B, _, H, W = img.shape
+        if H % PATCH or W % PATCH:
+            raise ValueError(f"image size {(H, W)} is not a multiple of the patch size {PATCH}")
+        taps = check_taps(taps, self.depth)
+        img = img.to(device=self.device, dtype=torch.float32).contiguous()
+        gh, gw = H // PATCH, W // PATCH
+        n_out = gh * gw + (1 if use_cls else 0)
+        out = torch.empty(len(taps), B, n_out, self.dim, device=self.device, dtype=torch.float32)
+        arr = self._tap_array(taps, out)
+        lib = _lib.load()
+        pos = self.pos_for(gh, gw)
+        with torch.cuda.device(self.device):
+            nbytes = lib.anyloc_vit_taps_workspace_bytes(C.byref(self.cfg), B, H, W, arr, len(taps))
+            ws = _lib.workspaces.get(self.device, nbytes, "vit")
+            rc = lib.anyloc_vit_extract_taps(C.byref(self.cfg), C.byref(self.struct), _lib.ptr(img), B, H, W,
+                                             _lib.ptr(pos), arr, len(taps), int(bool(use_cls)), int(bool(norm_descs)),
+                                             _lib.ptr(ws), ws.numel(), _lib.ENGINE[engine], _lib.stream_ptr())
+        _lib.check(rc, "anyloc_vit_extract_taps")
+        return out
+
+    def extract_taps_varlen(self, imgs, taps, use_cls=False, norm_descs=True, engine="auto"):
+        """extract_taps for a list of differently sized images (anyloc_vit_extract_taps_varlen) -> (packed
+        [len(taps), sum n_i, D] fp32, [n_i]), laid out per tap as extract_varlen's output.  Lists longer than the
+        library's per-call limit run as consecutive calls into the same packed output."""
+        taps = check_taps(taps, self.depth)
+        imgs = check_varlen_images(imgs, self.device)
+        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B)
+        out = torch.empty(len(taps), lay.rows, self.dim, device=self.device, dtype=torch.float32)
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            for s, e in lay.chunks:
+                B = e - s
+                hw = (C.c_int32 * (2 * B))(*[v for x in imgs[s:e] for v in x.shape[1:]])
+                img_p = (C.c_void_p * B)(*[x.data_ptr() for x in imgs[s:e]])
+                pos_p = (C.c_void_p * B)(*[self.pos_for(*g).data_ptr() for g in lay.grids[s:e]])
+                arr = self._tap_array(taps, out[:, lay.row0[s]:])
+                nbytes = lib.anyloc_vit_taps_varlen_workspace_bytes(C.byref(self.cfg), B, hw, arr, len(taps))
+                ws = _lib.workspaces.get(self.device, nbytes, "vit")
+                rc = lib.anyloc_vit_extract_taps_varlen(C.byref(self.cfg), C.byref(self.struct), B, img_p, hw, pos_p,
+                                                        arr, len(taps), int(bool(use_cls)), int(bool(norm_descs)),
+                                                        _lib.ptr(ws), ws.numel(), _lib.ENGINE[engine],
+                                                        _lib.stream_ptr())
+                _lib.check(rc, "anyloc_vit_extract_taps_varlen")
+        return out, lay.n_out
+
+
+def check_taps(taps, depth):
+    """A tap list as [(layer, facet)] in the given order; ValueError on an empty list, an item that is not a
+    (layer, facet) pair, an unknown facet or a repeated tap, IndexError on a layer outside [0, depth)."""
+    if isinstance(taps, (str, bytes)) or not hasattr(taps, "__iter__"):
+        raise ValueError(f"expected a list of (layer, facet) taps, got {taps!r}")
+    res = []
+    for t in taps:
+        if not isinstance(t, (tuple, list)) or len(t) != 2 or isinstance(t[0], bool):
+            raise ValueError(f"a tap is a (layer, facet) pair, got {t!r}")
+        try:
+            layer = operator.index(t[0])
+        except TypeError:
+            raise ValueError(f"tap {t!r}: the layer must be an integer") from None
+        facet = t[1]
+        if facet not in _lib.FACET:
+            raise ValueError(f"tap {t!r}: facet must be one of {sorted(_lib.FACET)}")
+        if not 0 <= layer < depth:
+            raise IndexError(f"tap {t!r}: layer out of range for {depth} blocks")
+        if (layer, facet) in res:
+            raise ValueError(f"tap {(layer, facet)!r} is requested twice")
+        res.append((layer, facet))
+    if not res:
+        raise ValueError("expected a non-empty list of (layer, facet) taps")
+    return res
 
 
 def check_varlen_images(imgs, device):

@@ -264,6 +264,40 @@ int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w
                               const int32_t* hw, const float* const* pos_embed, int layer, int facet, int use_cls,
                               int norm_descs, float* out, void* ws, size_t ws_bytes, int gemm_engine, void* stream);
 
+/* Several (layer, facet) features from ONE forward pass.  AnyLoc's results hinge on which layer and facet are read,
+ * and its ablations sweep them: scripts/dino_v2_vlad_ablations.sh:16-25 runs layers {39..0} x facets,
+ * scripts/dino_v2_vlad_viz.py:175-176 and dino_v2_vlad_viz_layers.py:370-376 build one DinoV2ExtractFeatures per layer
+ * over the same images, scripts/dino_v2_sim_facets.py:145-151 reads all four facets of one layer.  The hooks of
+ * utilities.py:245-252 define each facet: q/k/v of layer l are the thirds of blocks[l].attn.qkv(norm1(x)) (block l's
+ * input), "token" is the output of blocks[l].  So blocks 0..L_max (the deepest tapped layer) run once each and every
+ * tap keeps what that pass computes anyway.
+ *   taps_host  HOST array of n_taps >= 1 distinct (layer, facet) pairs in any order, each with its own output: [B, N(+1
+ *              with use_cls), D] (anyloc_vit_extract_taps) or packed [sum_i n_i, D] (the _varlen form, layout as in
+ *              anyloc_vit_extract_varlen).
+ * Every output is bit-identical to anyloc_vit_extract / anyloc_vit_extract_varlen for that tap alone with the same
+ * weights, images and GEMM engine; those two are the one-tap case of these calls.  An empty list, a layer outside
+ * [0, depth), a bad facet, a repeated (layer, facet) or a null output returns ANYLOC_ERR_ARG, and a short workspace
+ * ANYLOC_ERR_WORKSPACE, before anything is launched.  The call copies what it needs from taps_host, keeps no host
+ * pointer and does not synchronise.  The workspace exceeds the one-tap size by M * 3D * 4 bytes (M = token rows) when
+ * some layer's full fp32 qkv rows have to be kept: a layer with q/k/v taps below the deepest one, or a deepest layer
+ * with a token tap and a q/k/v tap, or with two or three q/k/v taps. */
+typedef struct {
+  int layer;
+  int facet;       /* ANYLOC_FACET_* */
+  float* out;
+} AnylocVitTap;
+size_t anyloc_vit_taps_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W, const AnylocVitTap* taps_host,
+                                       int n_taps);
+int anyloc_vit_extract_taps(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, const float* img, int B, int H,
+                            int W, const float* pos_embed, const AnylocVitTap* taps_host, int n_taps, int use_cls,
+                            int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, void* stream);
+size_t anyloc_vit_taps_varlen_workspace_bytes(const AnylocVitCfg* cfg, int B, const int32_t* hw,
+                                              const AnylocVitTap* taps_host, int n_taps);
+int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, int B,
+                                   const float* const* img, const int32_t* hw, const float* const* pos_embed,
+                                   const AnylocVitTap* taps_host, int n_taps, int use_cls, int norm_descs, void* ws,
+                                   size_t ws_bytes, int gemm_engine, void* stream);
+
 /* ------------------------------------------- building blocks (exported for parity tests)
  * C[M,N] = (A_hi+A_lo)[M,K] . (B_hi+B_lo)[N,K]^T with epilogue; *_lo nullable (treated as 0).
  * lda/ldb/ldo in elements.  out_lo/bias/gamma/resid per epilogue. */
