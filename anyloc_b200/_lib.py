@@ -29,7 +29,7 @@ class AnylocError(RuntimeError):
 
 class VitCfg(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("embed_dim", "depth", "num_heads", "ffn_kind", "ffn_hidden", "patch",
-                                       "pair_dtype")]
+                                       "pair_dtype", "num_registers")]
 
 
 _BLOCK_FIELDS = ["ln1_w", "ln1_b", "qkv_w_hi", "qkv_w_lo", "qkv_b", "proj_w_hi", "proj_w_lo", "proj_b",
@@ -43,7 +43,8 @@ class VitBlock(C.Structure):
 
 class VitWeightsStruct(C.Structure):
     _fields_ = [("patch_w_hi", C.c_void_p), ("patch_w_lo", C.c_void_p), ("patch_b", C.c_void_p),
-                ("cls_token", C.c_void_p), ("blocks", C.POINTER(VitBlock)), ("patch_alpha", C.c_float)]
+                ("cls_token", C.c_void_p), ("blocks", C.POINTER(VitBlock)), ("patch_alpha", C.c_float),
+                ("register_tokens", C.c_void_p)]
 
 
 class VitTap(C.Structure):

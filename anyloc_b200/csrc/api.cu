@@ -61,7 +61,7 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
 int launch_split(const float*, float*, float*, size_t, cudaStream_t);
 int launch_split_f16(const float*, void*, void*, size_t, float, cudaStream_t);
 int launch_im2col(const float*, int, int, int, int, int, void*, void*, bool, cudaStream_t);
-int launch_assemble(const float*, const float*, const float*, int, int, int, float*, cudaStream_t);
+int launch_assemble(const float*, const float*, const float*, const float*, int, int, int, int, float*, cudaStream_t);
 int launch_layernorm(const float*, const float*, const float*, int, int, float, void*, void*, bool, cudaStream_t);
 int launch_facet_out(const float*, int, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_l2norm(const float*, int64_t, int, int64_t, float*, cudaStream_t);
@@ -71,7 +71,8 @@ int attention_tc16_standalone(const float*, const float*, int, int, int, int, vo
 int attention_tc_varlen_launch(const void*, const void*, const VarlenAttnTable&, int, int, int, void*, void*, bool,
                                cudaStream_t);
 int launch_im2col_varlen(const VarlenImgTable&, int, int, int, void*, void*, bool, cudaStream_t);
-int launch_assemble_varlen(const float*, const float*, const VarlenImgTable&, int, int, float*, cudaStream_t);
+int launch_assemble_varlen(const float*, const float*, const float*, const VarlenImgTable&, int, int, float*,
+                           cudaStream_t);
 int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
                    cudaStream_t);
@@ -99,7 +100,7 @@ static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void
 using namespace anyloc;
 
 extern "C" const char* anyloc_last_error(void) { return g_err; }
-extern "C" int anyloc_version(void) { return 100; }
+extern "C" int anyloc_version(void) { return 101; }
 extern "C" long long anyloc_launch_count(void) { return g_launches.load(); }
 extern "C" int anyloc_profile_enable(int on) { g_prof_on = on != 0; g_prof_used = 0; return ANYLOC_OK; }
 extern "C" int anyloc_profile_read(double* ms, long long* groups, double* work) {
@@ -271,6 +272,15 @@ struct TapPlan {
   int use_cls, norm_descs;
 };
 int popcount3(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1); }
+// false (with the error text set) on R < 0 or on R > 0 register tokens without their weights
+bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w) {
+  if (cfg->num_registers < 0) { set_error("%s: num_registers=%d < 0", fn, cfg->num_registers); return false; }
+  if (cfg->num_registers > 0 && !w->register_tokens) {
+    set_error("%s: num_registers=%d but register_tokens is null", fn, cfg->num_registers);
+    return false;
+  }
+  return true;
+}
 // Returns false (with the error text set) on an empty list, a bad layer or facet, a repeated tap or (need_out) a null
 // output.
 bool tap_plan(const char* fn, const AnylocVitCfg* cfg, const AnylocVitTap* taps, int n_taps, bool need_out,
@@ -299,19 +309,19 @@ bool tap_plan(const char* fn, const AnylocVitCfg* cfg, const AnylocVitTap* taps,
 }  // namespace
 
 extern "C" size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W) {
-  if (!cfg || B <= 0 || H < cfg->patch || W < cfg->patch) return 0;
+  if (!cfg || cfg->num_registers < 0 || B <= 0 || H < cfg->patch || W < cfg->patch) return 0;
   const size_t N = (size_t)(H / cfg->patch) * (W / cfg->patch);
-  return vit_carve(cfg, B * N, B * (N + 1), false, nullptr, 0, nullptr) + 4096;
+  return vit_carve(cfg, B * N, B * (N + 1 + cfg->num_registers), false, nullptr, 0, nullptr) + 4096;
 }
 
 extern "C" size_t anyloc_vit_taps_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W, const AnylocVitTap* taps,
                                                   int n_taps) {
   TapPlan tp;
-  if (!cfg || B <= 0 || H < cfg->patch || W < cfg->patch || !tap_plan("vit_taps_workspace_bytes", cfg, taps, n_taps,
-                                                                      false, &tp))
+  if (!cfg || cfg->num_registers < 0 || B <= 0 || H < cfg->patch || W < cfg->patch ||
+      !tap_plan("vit_taps_workspace_bytes", cfg, taps, n_taps, false, &tp))
     return 0;
   const size_t N = (size_t)(H / cfg->patch) * (W / cfg->patch);
-  return vit_carve(cfg, B * N, B * (N + 1), tp.qkv32, nullptr, 0, nullptr) + 4096;
+  return vit_carve(cfg, B * N, B * (N + 1 + cfg->num_registers), tp.qkv32, nullptr, 0, nullptr) + 4096;
 }
 
 // the facet slice of the M token rows in src (row stride ld) -> out
@@ -437,7 +447,9 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
   tp.use_cls = use_cls; tp.norm_descs = norm_descs;
   ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "%s: head_dim must be 64", fn);
   ANYLOC_REQUIRE(B > 0, "%s: empty batch", fn);
-  const int P = cfg->patch, N = (H / P) * (W / P), T = N + 1, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P);
+  if (!registers_ok(fn, cfg, w)) return ANYLOC_ERR_ARG;
+  const int R = cfg->num_registers;
+  const int P = cfg->patch, N = (H / P) * (W / P), T = N + 1 + R, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P);
   const int M = B * T;
   VitBuffers bf;
   if (!vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, ws, ws_bytes, &bf)) {
@@ -452,7 +464,7 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
   e_pe.alpha = w->patch_alpha;
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, B * N, D, Kp, e_pe,
                           gemm_engine, f16, st))) return rc;
-  if ((rc = launch_assemble(bf.ptmp, w->cls_token, pos_embed, B, N, D, bf.x, st))) return rc;
+  if ((rc = launch_assemble(bf.ptmp, w->cls_token, w->register_tokens, pos_embed, B, N, R, D, bf.x, st))) return rc;
   const VitSeqs sq{B, T, nullptr, 0, 0.0, nullptr};
   return vit_trunk(cfg, w, bf, M, sq, tp, gemm_engine, st);
 }
@@ -486,15 +498,16 @@ struct VarlenPlan {
 // error text set) on a bad B or size.
 bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* p) {
   if (!cfg || cfg->patch <= 0) { set_error("vit_extract_varlen: null or bad config"); return false; }
+  if (cfg->num_registers < 0) { set_error("vit_extract_varlen: num_registers=%d < 0", cfg->num_registers); return false; }
   if (B < 1 || B > ANYLOC_VIT_VARLEN_MAX_B) {
     set_error("vit_extract_varlen: B=%d out of range [1,%d]", B, ANYLOC_VIT_VARLEN_MAX_B);
     return false;
   }
   if (!hw) { set_error("vit_extract_varlen: null hw"); return false; }
-  const int P = cfg->patch;
+  const int P = cfg->patch, R = cfg->num_registers;
   int64_t tok = 0, patches = 0, tiles = 0;
   double flops = 0.0;
-  p->img.n = B; p->attn.n = B;
+  p->img.n = B; p->img.nreg = R; p->attn.n = B;
   int order[ANYLOC_VIT_VARLEN_MAX_B];
   for (int i = 0; i < B; ++i) {
     const int H = hw[2 * i], W = hw[2 * i + 1];
@@ -504,21 +517,21 @@ bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* 
       return false;
     }
     const int64_t n = (int64_t)(H / P) * (W / P);
-    if (tok + n + 1 > (int64_t)INT32_MAX / 32) {     // the row-per-warp kernels index threads in 32 bits
+    if (tok + n + 1 + R > (int64_t)INT32_MAX / 32) {     // the row-per-warp kernels index threads in 32 bits
       set_error("vit_extract_varlen: too many tokens in one call");
       return false;
     }
     p->img.tok0[i] = (int)tok;
     p->img.gh[i] = H / P; p->img.gw[i] = W / P;
     p->img.ptr[i] = nullptr;
-    tok += n + 1; patches += n;
-    flops += 4.0 * (double)(n + 1) * (n + 1) * cfg->embed_dim;
+    tok += n + 1 + R; patches += n;
+    flops += 4.0 * (double)(n + 1 + R) * (n + 1 + R) * cfg->embed_dim;
     order[i] = i;
   }
   // attention entries longest first (the longest key loops start first); ties keep the input order
   std::stable_sort(order, order + B, [&](int a, int b) { return p->img.gh[a] * p->img.gw[a] > p->img.gh[b] * p->img.gw[b]; });
   for (int k = 0; k < B; ++k) {
-    const int i = order[k], T = p->img.gh[i] * p->img.gw[i] + 1;
+    const int i = order[k], T = p->img.gh[i] * p->img.gw[i] + 1 + R;
     p->attn.tile0[k] = (int)tiles; p->attn.row0[k] = p->img.tok0[i]; p->attn.len[k] = T;
     tiles += cdiv(T, 64);
   }
@@ -557,6 +570,7 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
   }
   ANYLOC_REQUIRE(gemm_engine == ANYLOC_GEMM_AUTO || gemm_engine == ANYLOC_GEMM_TC3, "%s: bad gemm_engine %d", fn,
                  gemm_engine);
+  if (!registers_ok(fn, cfg, w)) return ANYLOC_ERR_ARG;
   VarlenPlan p;
   if (!varlen_plan(cfg, B, hw, &p)) return ANYLOC_ERR_ARG;
   for (int i = 0; i < B; ++i)
@@ -577,7 +591,7 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, p.n_patch, D, Kp, e_pe,
                           gemm_engine, f16, st))) return rc;
   for (int i = 0; i < B; ++i) p.img.ptr[i] = pos_embed[i];
-  if ((rc = launch_assemble_varlen(bf.ptmp, w->cls_token, p.img, M, D, bf.x, st))) return rc;
+  if ((rc = launch_assemble_varlen(bf.ptmp, w->cls_token, w->register_tokens, p.img, M, D, bf.x, st))) return rc;
   const VitSeqs sq{B, 0, &p.attn, p.n_tiles, p.attn_flops, &p.img};
   return vit_trunk(cfg, w, bf, M, sq, tp, gemm_engine, st);
 }

@@ -99,13 +99,15 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uin
 // kernels by value as __grid_constant__ parameters: the launch copies them, so a call neither synchronises with the
 // host nor keeps a host pointer, and each stays under the classic 4 KB kernel-parameter limit.
 constexpr int kVarlenMaxB = ANYLOC_VIT_VARLEN_MAX_B;
-// im2col, token assembly and the facet slice.  Image i has tokens [tok0[i], tok0[i] + 1 + gh[i]*gw[i]) of the packed
-// sequence, patch rows from tok0[i] - i and, without the cls token, output rows from tok0[i] - i.
+// im2col, token assembly and the facet slice.  Image i has tokens [tok0[i], tok0[i] + 1 + nreg + gh[i]*gw[i]) of the
+// packed sequence (cls, nreg registers, patches), patch rows from tok0[i] - (1 + nreg) * i and, without the cls token,
+// output rows from tok0[i] - i.
 struct VarlenImgTable {
   int n;
   int tok0[kVarlenMaxB];
   int gh[kVarlenMaxB], gw[kVarlenMaxB];
   const float* ptr[kVarlenMaxB];        // the image [3, gh*P, gw*P] (im2col) or its positional table (assembly)
+  int nreg;                             // register tokens per image (last: the fields above keep their offsets)
 };
 static_assert(sizeof(VarlenImgTable) <= 4096, "kernel parameter over 4 KB");
 // the last image i whose first row tok0[i] - skip*i (skip = rows the kernel's grid omits per image) is <= row

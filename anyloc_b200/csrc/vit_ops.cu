@@ -67,32 +67,42 @@ template <bool F16>
 __global__ void im2col_split_varlen_kernel(const __grid_constant__ VarlenImgTable tab, int P, int Kp,
                                            typename PairOut<F16>::T* __restrict__ hi,
                                            typename PairOut<F16>::T* __restrict__ lo) {
-  const int row = blockIdx.x, i = varlen_image_of(tab, row, 1);
-  im2col_row<F16>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - i), hi, lo);
+  const int skip = 1 + tab.nreg, row = blockIdx.x, i = varlen_image_of(tab, row, skip);
+  im2col_row<F16>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - skip * i), hi, lo);
 }
 
-// x[row,:] = cls + pos[0] (t = 0) or patch[b*N + t-1,:] + pos[t]     (prepare_tokens)
+// x[row,:] = cls + pos[0] (t = 0), reg[t-1] (1 <= t <= R: no positional embedding) or patch[b*N + p,:] + pos[1+p]
+// (t = 1 + R + p)     (prepare_tokens)
 __device__ __forceinline__ void assemble_row(const float* __restrict__ patch, const float* __restrict__ cls,
-                                             const float* __restrict__ pos, int b, int N, int D, size_t row, int t,
-                                             float* __restrict__ x) {
-  const float* src = t == 0 ? cls : patch + ((size_t)b * N + (t - 1)) * D;
-  const float* pe = pos + (size_t)t * D;
+                                             const float* __restrict__ reg, const float* __restrict__ pos, int b, int N,
+                                             int R, int D, size_t row, int t, float* __restrict__ x) {
+  if (t >= 1 && t <= R) {
+    const float* r = reg + (size_t)(t - 1) * D;
+    for (int d = threadIdx.x; d < D; d += blockDim.x) x[row * D + d] = r[d];
+    return;
+  }
+  const int tp = t == 0 ? 0 : t - R;     // the token's row of the positional table
+  const float* src = tp == 0 ? cls : patch + ((size_t)b * N + (tp - 1)) * D;
+  const float* pe = pos + (size_t)tp * D;
   for (int d = threadIdx.x; d < D; d += blockDim.x) x[row * D + d] = src[d] + pe[d];
 }
 
 __global__ void assemble_tokens_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
-                                       const float* __restrict__ pos, int B, int N, int D,
-                                       float* __restrict__ x) {
-  const size_t row = blockIdx.x;     // over B*(N+1)
-  const int b = (int)(row / (N + 1)), t = (int)(row % (N + 1));
-  assemble_row(patch, cls, pos, b, N, D, row, t, x);
+                                       const float* __restrict__ reg, const float* __restrict__ pos, int B, int N,
+                                       int R, int D, float* __restrict__ x) {
+  const size_t row = blockIdx.x;     // over B*T, T = 1 + R + N
+  const int T = N + 1 + R;
+  const int b = (int)(row / T), t = (int)(row % T);
+  assemble_row(patch, cls, reg, pos, b, N, R, D, row, t, x);
 }
 
 // images of different sizes, one block per token row of the packed sequence; image i reads its own positional table
 __global__ void assemble_tokens_varlen_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
-                                              const __grid_constant__ VarlenImgTable tab, int D, float* __restrict__ x) {
+                                              const float* __restrict__ reg, const __grid_constant__ VarlenImgTable tab,
+                                              int D, float* __restrict__ x) {
   const int row = blockIdx.x, i = varlen_image_of(tab, row, 0);
-  assemble_row(patch + (size_t)(tab.tok0[i] - i) * D, cls, tab.ptr[i], 0, 0, D, row, row - tab.tok0[i], x);
+  assemble_row(patch + (size_t)(tab.tok0[i] - (1 + tab.nreg) * i) * D, cls, reg, tab.ptr[i], 0, 0, tab.nreg, D, row,
+               row - tab.tok0[i], x);
 }
 
 // LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo). One warp per row.
@@ -319,9 +329,9 @@ int launch_im2col(const float* img, int B, int H, int W, int P, int Kp, void* hi
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-int launch_assemble(const float* patch, const float* cls, const float* pos, int B, int N, int D, float* x,
-                    cudaStream_t st) {
-  assemble_tokens_kernel<<<B * (N + 1), 256, 0, st>>>(patch, cls, pos, B, N, D, x);
+int launch_assemble(const float* patch, const float* cls, const float* reg, const float* pos, int B, int N, int R, int D,
+                    float* x, cudaStream_t st) {
+  assemble_tokens_kernel<<<B * (N + 1 + R), 256, 0, st>>>(patch, cls, reg, pos, B, N, R, D, x);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -357,9 +367,9 @@ int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-int launch_assemble_varlen(const float* patch, const float* cls, const VarlenImgTable& tab, int n_tokens, int D,
-                           float* x, cudaStream_t st) {
-  assemble_tokens_varlen_kernel<<<n_tokens, 256, 0, st>>>(patch, cls, tab, D, x);
+int launch_assemble_varlen(const float* patch, const float* cls, const float* reg, const VarlenImgTable& tab,
+                           int n_tokens, int D, float* x, cudaStream_t st) {
+  assemble_tokens_varlen_kernel<<<n_tokens, 256, 0, st>>>(patch, cls, reg, tab, D, x);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

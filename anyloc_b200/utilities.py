@@ -19,7 +19,8 @@ import torch
 from . import _lib
 from . import vit as _vit
 
-_DINO_V2_MODELS = Literal["dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14"]
+_DINO_V2_MODELS = Literal["dinov2_vits14", "dinov2_vitb14", "dinov2_vitl14", "dinov2_vitg14",
+                          "dinov2_vits14_reg", "dinov2_vitb14_reg", "dinov2_vitl14_reg", "dinov2_vitg14_reg"]
 _DINO_FACETS = Literal["query", "key", "value", "token"]
 
 
@@ -355,7 +356,12 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
     silently, and the call raises) or "auto" (the default: f16x3 until a call overflows, then that
     call is redone and the extractor stays in tf32x3 -- trained DINOv2 checkpoints have outlier
     activations that random-init weights do not).  All accumulate in fp32 with round-to-nearest
-    chunk accumulation."""
+    chunk accumulation.
+
+    `dino_model` may also name a backbone with register tokens, `dinov2_vit{s,b,l,g}14_reg`.  As
+    in the reference, only row 0 (cls) is dropped, so its 4 register rows come first: an output
+    holds [cls (with use_cls), r0..r3, the N patch rows], and `out[:, 4:]` (without use_cls) or
+    `out[:, 5:]` (with it) are the patch features alone."""
 
     def __init__(self, dino_model: _DINO_V2_MODELS, layer: int, facet: _DINO_FACETS = "token",
                  use_cls=False, norm_descs=True, device: str = "cpu", *, weights=None,
@@ -384,8 +390,8 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
         return out, out
 
     def __call__(self, img):
-        """img [B,3,H,W] -> [B, N(+1), D]; or a list/tuple of differently sized images [3,H_i,W_i] / [1,3,H_i,W_i],
-        all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
+        """img [B,3,H,W] -> [B, (1 +) R + N, D] (R = 4 register rows for the *_reg models, else 0); or a list/tuple of
+        differently sized images [3,H_i,W_i] / [1,3,H_i,W_i], all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
         pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
         image of fewer than 32 tokens takes the SIMT GEMMs)."""
         return self._guarded(img)
@@ -403,7 +409,8 @@ class DinoV2MultiExtractFeatures(_GuardedExtractor):
     tap keeps what that pass computes.  `taps` is a list of distinct (layer, facet) pairs; `use_cls`, `norm_descs`,
     `device`, `weights`, `gemm_engine` and `precision` mean what they mean for DinoV2ExtractFeatures and apply to
     every tap.  Each output is bit-identical to DinoV2ExtractFeatures(dino_model, layer, facet, use_cls, norm_descs)
-    on the same images with the same weights, precision and engine."""
+    on the same images with the same weights, precision and engine, and has its row layout: [cls (with use_cls),
+    the 4 register rows of a *_reg model, the patch rows]."""
 
     def __init__(self, dino_model: _DINO_V2_MODELS, taps, use_cls=False, norm_descs=True, device: str = "cpu", *,
                  weights=None, gemm_engine: str = "auto", precision: str = None) -> None:
@@ -429,7 +436,7 @@ class DinoV2MultiExtractFeatures(_GuardedExtractor):
         return packed, {t: packed[k] for k, t in enumerate(self.taps)}
 
     def __call__(self, img):
-        """img [B,3,H,W] -> {(layer, facet): [B, N(+1), D]}; a list/tuple of differently sized images (as for
+        """img [B,3,H,W] -> {(layer, facet): [B, (1 +) R + N, D]}; a list/tuple of differently sized images (as for
         DinoV2ExtractFeatures) -> {(layer, facet): [list of [n_i, D]]}.  All outputs are views of one allocation."""
         return self._guarded(img)
 

@@ -23,9 +23,14 @@ ARCHS = {
     "dinov2_vitl14": (1024, 24, 16, "mlp"),
     "dinov2_vitg14": (1536, 40, 24, "swiglufused"),
 }
+# the register variants (upstream hub/backbones.py *_reg): same architectures with 4 register tokens between cls and
+# the patches, and their own positional-embedding resize
+ARCHS.update({n + "_reg": a for n, a in list(ARCHS.items())})
 PATCH = 14
 POS_GRID = 37           # pretrained at 518x518
-INTERP_OFFSET = 0.1     # upstream interpolate_offset
+INTERP_OFFSET = 0.1     # upstream interpolate_offset of the plain models
+# name: (num_register_tokens, interpolate_offset, interpolate_antialias)
+TOKENS = {n: (4, 0.0, True) if n.endswith("_reg") else (0, INTERP_OFFSET, False) for n in ARCHS}
 
 
 def ffn_hidden(dim, kind):
@@ -35,7 +40,8 @@ def ffn_hidden(dim, kind):
 def random_state_dict(name, seed=0, device="cpu", depth=None):
     """Random weights with the upstream init recipe (trunc_normal std .02 for Linear / pos_embed,
     cls ~ N(0,1e-6), zero bias, LayerNorm (1,0), LayerScale 1.0), generated directly on `device`.
-    Synthetic-benchmark use only: no pretrained checkpoint can be fetched offline."""
+    Register models get `register_tokens` ~ N(0,1e-6), drawn last, so every other tensor equals the plain model's of the
+    same seed.  Synthetic-benchmark use only: no pretrained checkpoint can be fetched offline."""
     dim, full_depth, heads, kind = ARCHS[name]
     depth = full_depth if depth is None else depth
     hid = ffn_hidden(dim, kind)
@@ -72,12 +78,17 @@ def random_state_dict(name, seed=0, device="cpu", depth=None):
             sd[p + "mlp.w12.weight"], sd[p + "mlp.w12.bias"] = tn(2 * hid, dim), zeros(2 * hid)
             sd[p + "mlp.w3.weight"], sd[p + "mlp.w3.bias"] = tn(dim, hid), zeros(dim)
         sd[p + "ls2.gamma"] = ones(dim)
+    n_reg = TOKENS[name][0]
+    if n_reg:
+        sd["register_tokens"] = torch.empty(1, n_reg, dim, device=device).normal_(0.0, 1e-6, generator=g)
     return sd
 
 
-def interpolate_pos_embed(pos_embed, gh, gw):
+def interpolate_pos_embed(pos_embed, gh, gw, offset=INTERP_OFFSET, antialias=False):
     """Upstream DinoVisionTransformer.interpolate_pos_encoding for a gh x gw patch grid
-    (gh = H//14 rows, gw = W//14 columns).  pos_embed [1, 1+37*37, D] -> [1+gh*gw, D]."""
+    (gh = H//14 rows, gw = W//14 columns).  pos_embed [1, 1+37*37, D] -> [1+gh*gw, D].
+    offset / antialias: the model's interpolate_offset / interpolate_antialias (TOKENS); offset 0 resizes to
+    size=(gh, gw) instead of scale_factor=((g + offset) / 37)."""
     pos_embed = pos_embed.detach().float().cpu()
     n = pos_embed.shape[1] - 1
     m = int(math.sqrt(n))
@@ -85,9 +96,9 @@ def interpolate_pos_embed(pos_embed, gh, gw):
         return pos_embed[0].contiguous()
     dim = pos_embed.shape[-1]
     cls_pos, patch_pos = pos_embed[:, 0], pos_embed[:, 1:]
-    sy, sx = float(gh + INTERP_OFFSET) / m, float(gw + INTERP_OFFSET) / m
-    patch_pos = F.interpolate(patch_pos.reshape(1, m, m, dim).permute(0, 3, 1, 2),
-                              scale_factor=(sy, sx), mode="bicubic", antialias=False)
+    kw = {"scale_factor": (float(gh + offset) / m, float(gw + offset) / m)} if offset else {"size": (gh, gw)}
+    patch_pos = F.interpolate(patch_pos.reshape(1, m, m, dim).permute(0, 3, 1, 2), mode="bicubic",
+                              antialias=antialias, **kw)
     if tuple(patch_pos.shape[-2:]) != (gh, gw):
         raise _lib.AnylocError(f"pos-embed interpolation produced {tuple(patch_pos.shape[-2:])}, wanted {(gh, gw)}")
     patch_pos = patch_pos.permute(0, 2, 3, 1).reshape(-1, dim)
@@ -95,7 +106,8 @@ def interpolate_pos_embed(pos_embed, gh, gw):
 
 
 class VitWeights:
-    """Device-resident, kernel-ready weights of one DINOv2 backbone (blocks 0..depth-1)."""
+    """Device-resident, kernel-ready weights of one DINOv2 backbone (blocks 0..depth-1).  A register model's outputs
+    hold its num_registers register rows between the cls row and the patch rows, as the reference returns them."""
 
     def __init__(self, name, state_dict, device, depth=None, pair="tf32"):
         if name not in ARCHS:
@@ -104,8 +116,15 @@ class VitWeights:
             raise ValueError(f"pair must be one of {sorted(_lib.PAIR)}, got {pair!r}")
         self.name = name
         self.pair = pair
-        self.device = _lib.require_cuda(device)
         self.dim, full_depth, self.heads, self.ffn_kind = ARCHS[name]
+        self.num_registers, self.interp_offset, self.interp_antialias = TOKENS[name]
+        if self.num_registers:
+            reg = state_dict.get("register_tokens")
+            want = (1, self.num_registers, self.dim)
+            if reg is None or tuple(reg.shape) != want:
+                got = "missing" if reg is None else f"has shape {tuple(reg.shape)}"
+                raise ValueError(f"{name} state_dict: 'register_tokens' {got}, expected shape {want}")
+        self.device = _lib.require_cuda(device)
         n_blocks = 1 + max([int(k.split(".")[1]) for k in state_dict if k.startswith("blocks.")], default=-1)
         self.depth = min(n_blocks, full_depth if depth is None else depth)
         self.hidden = ffn_hidden(self.dim, self.ffn_kind)
@@ -153,6 +172,8 @@ class VitWeights:
         patch_alpha = self.patch_w[2]
         self.patch_b = keep(sd["patch_embed.proj.bias"])
         self.cls_token = keep(sd["cls_token"].reshape(-1))
+        self.register_tokens = keep(sd["register_tokens"].reshape(self.num_registers, self.dim)) if self.num_registers \
+            else None
         self.pos_embed = sd["pos_embed"].detach().float().cpu()
         self.blocks = (_lib.VitBlock * self.depth)()
         for i in range(self.depth):
@@ -184,20 +205,23 @@ class VitWeights:
             hi, lo, blk.out_alpha = split(w_out); put("out_w_hi", hi); put("out_w_lo", lo); put("out_b", keep(b_out))
             put("ls2", keep(sd[p + "ls2.gamma"]))
         self.cfg = _lib.VitCfg(self.dim, self.depth, self.heads, _lib.FFN[self.ffn_kind], self.hidden, PATCH,
-                               _lib.PAIR[pair])
+                               _lib.PAIR[pair], self.num_registers)
         self.struct = _lib.VitWeightsStruct(self.patch_w[0].data_ptr(), self.patch_w[1].data_ptr(),
                                             self.patch_b.data_ptr(), self.cls_token.data_ptr(), self.blocks,
-                                            patch_alpha)
+                                            patch_alpha,
+                                            self.register_tokens.data_ptr() if self.num_registers else None)
         torch.cuda.synchronize(dev)
 
     def pos_for(self, gh, gw):
         key = (gh, gw)
         if key not in self._pos_cache:
-            self._pos_cache[key] = interpolate_pos_embed(self.pos_embed, gh, gw).to(self.device)
+            self._pos_cache[key] = interpolate_pos_embed(self.pos_embed, gh, gw, self.interp_offset,
+                                                         self.interp_antialias).to(self.device)
         return self._pos_cache[key]
 
     def extract(self, img, layer, facet="value", use_cls=False, norm_descs=True, engine="auto"):
-        """img [B,3,H,W] fp32 on self.device -> [B, N(+1), D] fp32 (utilities.py:263-285)."""
+        """img [B,3,H,W] fp32 on self.device -> [B, (1 +) R + N, D] fp32 (utilities.py:263-285): the cls row with
+        use_cls, then the R = num_registers register rows, then the N patch rows."""
         if img.dim() != 4 or img.shape[1] != 3:
             raise ValueError(f"expected an image batch [B,3,H,W], got {tuple(img.shape)}")
         B, _, H, W = img.shape
@@ -207,7 +231,7 @@ class VitWeights:
             raise IndexError(f"layer {layer} out of range for {self.name} with {self.depth} blocks loaded")
         img = img.to(device=self.device, dtype=torch.float32).contiguous()
         gh, gw = H // PATCH, W // PATCH
-        n_out = gh * gw + (1 if use_cls else 0)
+        n_out = gh * gw + self.num_registers + (1 if use_cls else 0)
         out = torch.empty(B, n_out, self.dim, device=self.device, dtype=torch.float32)
         lib = _lib.load()
         pos = self.pos_for(gh, gw)
@@ -223,13 +247,13 @@ class VitWeights:
 
     def extract_varlen(self, imgs, layer, facet="value", use_cls=False, norm_descs=True, engine="auto"):
         """A list of differently sized images [3,H_i,W_i] (or [1,3,H_i,W_i]) fp32 on self.device in one packed forward
-        pass (anyloc_vit_extract_varlen) -> (packed [sum n_i, D] fp32, [n_i]), n_i = gh_i*gw_i (+1 with use_cls).
+        pass (anyloc_vit_extract_varlen) -> (packed [sum n_i, D] fp32, [n_i]), n_i = R + gh_i*gw_i (+1 with use_cls).
         Image i's rows equal extract(imgs[i][None])[0] bit for bit.  Lists longer than the library's per-call limit
         run as consecutive calls into the same packed output."""
         if not 0 <= layer < self.depth:
             raise IndexError(f"layer {layer} out of range for {self.name} with {self.depth} blocks loaded")
         imgs = check_varlen_images(imgs, self.device)
-        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B)
+        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B, self.num_registers)
         out = torch.empty(lay.rows, self.dim, device=self.device, dtype=torch.float32)
         lib = _lib.load()
         with torch.cuda.device(self.device):
@@ -253,7 +277,7 @@ class VitWeights:
 
     def extract_taps(self, img, taps, use_cls=False, norm_descs=True, engine="auto"):
         """Several (layer, facet) features of img [B,3,H,W] from one forward pass (anyloc_vit_extract_taps) ->
-        [len(taps), B, N(+1), D] fp32; item k is taps[k]'s output, equal bit for bit to extract(img, *taps[k])."""
+        [len(taps), B, (1 +) R + N, D] fp32; item k is taps[k]'s output, equal bit for bit to extract(img, *taps[k])."""
         if img.dim() != 4 or img.shape[1] != 3:
             raise ValueError(f"expected an image batch [B,3,H,W], got {tuple(img.shape)}")
         B, _, H, W = img.shape
@@ -262,7 +286,7 @@ class VitWeights:
         taps = check_taps(taps, self.depth)
         img = img.to(device=self.device, dtype=torch.float32).contiguous()
         gh, gw = H // PATCH, W // PATCH
-        n_out = gh * gw + (1 if use_cls else 0)
+        n_out = gh * gw + self.num_registers + (1 if use_cls else 0)
         out = torch.empty(len(taps), B, n_out, self.dim, device=self.device, dtype=torch.float32)
         arr = self._tap_array(taps, out)
         lib = _lib.load()
@@ -282,7 +306,7 @@ class VitWeights:
         library's per-call limit run as consecutive calls into the same packed output."""
         taps = check_taps(taps, self.depth)
         imgs = check_varlen_images(imgs, self.device)
-        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B)
+        lay = VarlenLayout([tuple(x.shape[1:]) for x in imgs], use_cls, _lib.VIT_VARLEN_MAX_B, self.num_registers)
         out = torch.empty(len(taps), lay.rows, self.dim, device=self.device, dtype=torch.float32)
         lib = _lib.load()
         with torch.cuda.device(self.device):
@@ -352,13 +376,13 @@ def check_varlen_images(imgs, device):
 
 
 class VarlenLayout:
-    """Where each image of a list input lands: grids (gh_i, gw_i), tokens T_i = gh_i*gw_i + 1, output rows n_i
-    (T_i - 1 without the cls token), their offsets row0 in the packed output (row0[-1] = rows) and the consecutive
+    """Where each image of a list input lands: grids (gh_i, gw_i), tokens T_i = 1 + registers + gh_i*gw_i, output rows
+    n_i (T_i - 1 without the cls token), their offsets row0 in the packed output (row0[-1] = rows) and the consecutive
     (start, stop) slices of at most max_b images, one library call each."""
 
-    def __init__(self, sizes, use_cls, max_b):
+    def __init__(self, sizes, use_cls, max_b, registers=0):
         self.grids = [(H // PATCH, W // PATCH) for H, W in sizes]
-        self.tokens = [gh * gw + 1 for gh, gw in self.grids]
+        self.tokens = [1 + registers + gh * gw for gh, gw in self.grids]
         self.n_out = [t - (0 if use_cls else 1) for t in self.tokens]
         self.row0 = [0]
         for n in self.n_out:

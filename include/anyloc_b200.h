@@ -206,6 +206,7 @@ typedef struct {
   int ffn_hidden;  /* 4*D (mlp) or 4096-style fused hidden (swiglu) */
   int patch;       /* 14 */
   int pair_dtype;  /* ANYLOC_PAIR_*: format of the weight pairs and of all GEMM-input activations */
+  int num_registers; /* R register tokens (dinov2_vit*14_reg: 4; 0 for the plain models) */
 } AnylocVitCfg;
 
 /* Per-block device pointers.  Matrices are [out,in] row-major like nn.Linear.weight, supplied as
@@ -230,13 +231,20 @@ typedef struct {
   const float *cls_token;               /* [D] */
   const AnylocVitBlock* blocks;         /* HOST array [depth] of device pointers */
   float patch_alpha;
+  const float *register_tokens;         /* [R, D] (num_registers > 0), else unused */
 } AnylocVitWeights;
 
+/* Register tokens (upstream prepare_tokens with num_register_tokens = R): image b's token sequence is
+ * [cls + pos[0], reg[0..R-1], patch[p] + pos[1+p]], T = 1 + R + N tokens; the registers get no positional embedding.
+ * The output drops only the cls row (without use_cls), as DinoV2ExtractFeatures drops row 0 (utilities.py:273), so the
+ * R register rows come first: [B, (1 +) R + N, D].  Every token count below (workspaces, the 32-bit token limit of the
+ * _varlen calls) counts T per image.  R < 0, or R > 0 with a null register_tokens, returns ANYLOC_ERR_ARG (the
+ * *_workspace_bytes functions return 0).  R = 0 is the plain model. */
 /* padded patch-embed reduction length (3*14*14=588 -> multiple of 32) */
 int anyloc_vit_patch_k(int patch);
 size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W);
 /* img [B,3,H,W] fp32 (H,W multiples of 14); pos_embed [1+g_h*g_w, D] already interpolated for this
- * grid (upstream interpolate_pos_encoding); out [B, N(+1 if use_cls), D]. */
+ * grid (upstream interpolate_pos_encoding, with the model's own recipe); out [B, R + N (+1 if use_cls), D]. */
 int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, const float* img,
                        int B, int H, int W, const float* pos_embed, int layer, int facet,
                        int use_cls, int norm_descs, float* out, void* ws, size_t ws_bytes,
@@ -252,7 +260,7 @@ int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, 
  *   hw        HOST int32 [B][2] = (H_i, W_i), positive multiples of the patch size
  *   pos_embed HOST array of B device pointers; pos_embed[i] = the table [1 + g_h,i * g_w,i, D] interpolated for image
  *             i's grid (images of the same grid may share one)
- *   out       packed [sum_i n_i, D] with n_i = g_h,i * g_w,i (+1 if use_cls); image i's rows start at sum_{j<i} n_j.
+ *   out       packed [sum_i n_i, D] with n_i = R + g_h,i * g_w,i (+1 if use_cls); image i's rows start at sum_{j<i} n_j.
  * Each image's rows are bit-identical to anyloc_vit_extract on that image alone with the same GEMM engine (under
  * ANYLOC_GEMM_AUTO, a lone image of fewer than 32 tokens takes the SIMT GEMMs there, so compare those under TC3).
  * gemm_engine = ANYLOC_GEMM_SIMT returns ANYLOC_ERR_UNSUPPORTED: the packed attention is a tensor-core kernel.  The
@@ -271,8 +279,8 @@ int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w
  * utilities.py:245-252 define each facet: q/k/v of layer l are the thirds of blocks[l].attn.qkv(norm1(x)) (block l's
  * input), "token" is the output of blocks[l].  So blocks 0..L_max (the deepest tapped layer) run once each and every
  * tap keeps what that pass computes anyway.
- *   taps_host  HOST array of n_taps >= 1 distinct (layer, facet) pairs in any order, each with its own output: [B, N(+1
- *              with use_cls), D] (anyloc_vit_extract_taps) or packed [sum_i n_i, D] (the _varlen form, layout as in
+ *   taps_host  HOST array of n_taps >= 1 distinct (layer, facet) pairs in any order, each with its own output: [B, R + N
+ *              (+1 with use_cls), D] (anyloc_vit_extract_taps) or packed [sum_i n_i, D] (the _varlen form, layout as in
  *              anyloc_vit_extract_varlen).
  * Every output is bit-identical to anyloc_vit_extract / anyloc_vit_extract_varlen for that tap alone with the same
  * weights, images and GEMM engine; those two are the one-tap case of these calls.  An empty list, a layer outside
