@@ -57,29 +57,45 @@ int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int,
                    const EpiParams&, bool f16, cudaStream_t);
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                        int ldb, int M, int N, int K, const EpiParams& ep, bool f16);
+int gemm_tc_bf16_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
 // vit_ops.cu / attention.cu
 int launch_split(const float*, float*, float*, size_t, cudaStream_t);
 int launch_split_f16(const float*, void*, void*, size_t, float, cudaStream_t);
-int launch_im2col(const float*, int, int, int, int, int, void*, void*, bool, cudaStream_t);
+int launch_split_bf16(const float*, void*, size_t, cudaStream_t);
+int launch_im2col(const float*, int, int, int, int, int, void*, void*, int, cudaStream_t);
 int launch_assemble(const float*, const float*, const float*, const float*, int, int, int, int, float*, cudaStream_t);
-int launch_layernorm(const float*, const float*, const float*, int, int, float, void*, void*, bool, cudaStream_t);
+int launch_layernorm(const float*, const float*, const float*, int, int, float, void*, void*, int, cudaStream_t);
 int launch_facet_out(const float*, int, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_l2norm(const float*, int64_t, int, int64_t, float*, cudaStream_t);
 int attention_launch(const float*, const float*, int, int, int, int, void*, void*, bool, cudaStream_t);
-int attention_tc_launch(const void*, const void*, int, int, int, int, void*, void*, bool, cudaStream_t);
+int attention_tc_launch(const void*, const void*, int, int, int, int, void*, void*, int, cudaStream_t);
 int attention_tc16_standalone(const float*, const float*, int, int, int, int, void*, void*, cudaStream_t);
-int attention_tc_varlen_launch(const void*, const void*, const VarlenAttnTable&, int, int, int, void*, void*, bool,
+int attention_tc_varlen_launch(const void*, const void*, const VarlenAttnTable&, int, int, int, void*, void*, int,
                                cudaStream_t);
-int launch_im2col_varlen(const VarlenImgTable&, int, int, int, void*, void*, bool, cudaStream_t);
+int launch_im2col_varlen(const VarlenImgTable&, int, int, int, void*, void*, int, cudaStream_t);
 int launch_assemble_varlen(const float*, const float*, const float*, const VarlenImgTable&, int, int, float*,
                            cudaStream_t);
 int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
                    cudaStream_t);
 
+// fmt: ANYLOC_PAIR_* of the operands.  Single bf16 is a tensor-core-only format: it runs the wgmma kernel at every M
+// (no SIMT route, so a row's result never depends on how many rows share the call) and refuses the SIMT engine.
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
-                         int ldb, int M, int N, int K, const EpiParams& ep, int engine, bool f16, cudaStream_t st) {
+                         int ldb, int M, int N, int K, const EpiParams& ep, int engine, int fmt, cudaStream_t st) {
   if (M == 0 || N == 0) return ANYLOC_OK;
+  if (fmt == ANYLOC_PAIR_BF16) {
+    if (engine == ANYLOC_GEMM_SIMT || a_lo || b_lo ||
+        !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, true)) {
+      set_error("gemm: the single-bf16 format runs on the tensor-core engine only, with 16-byte aligned operands, "
+                "K, lda and ldb multiples of 8 and no lo operands (M=%d N=%d K=%d lda=%d ldb=%d engine=%d)",
+                M, N, K, lda, ldb, engine);
+      return ANYLOC_ERR_UNSUPPORTED;
+    }
+    ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
+    return gemm_tc_bf16_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
+  }
+  const bool f16 = fmt == ANYLOC_PAIR_F16;
   bool tc_ok = gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16);
   if (engine == ANYLOC_GEMM_TC3 && !tc_ok) {
     set_error("gemm: tensor-core engine does not support this shape/alignment (M=%d N=%d K=%d lda=%d ldb=%d f16=%d)",
@@ -137,18 +153,23 @@ extern "C" int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const
                               int ldo, int out_dtype, int engine, void* stream) {
   ANYLOC_REQUIRE(a_hi && b_hi && out, "gemm_nt: null pointer");
   ANYLOC_REQUIRE(M >= 0 && N >= 0 && K > 0, "gemm_nt: bad dims");
-  ANYLOC_REQUIRE(in_dtype == ANYLOC_PAIR_TF32 || in_dtype == ANYLOC_PAIR_F16, "gemm_nt: bad in_dtype %d", in_dtype);
-  ANYLOC_REQUIRE(out_dtype == ANYLOC_PAIR_TF32 || out_dtype == ANYLOC_PAIR_F16, "gemm_nt: bad out_dtype %d", out_dtype);
+  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_BF16, "gemm_nt: bad in_dtype %d", in_dtype);
+  ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_BF16, "gemm_nt: bad out_dtype %d", out_dtype);
   ANYLOC_REQUIRE(epilogue >= ANYLOC_EPI_BIAS && epilogue <= ANYLOC_EPI_LS_RESID, "gemm_nt: bad epilogue %d", epilogue);
-  if (epilogue == ANYLOC_EPI_BIAS_SPLIT || epilogue == ANYLOC_EPI_GELU_SPLIT || epilogue == ANYLOC_EPI_SWIGLU_SPLIT)
+  const bool bf16 = in_dtype == ANYLOC_PAIR_BF16;
+  ANYLOC_REQUIRE(bf16 == (out_dtype == ANYLOC_PAIR_BF16), "gemm_nt: single bf16 is both the input and the output format "
+                 "(in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
+  if (bf16)
+    ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-bf16 format has no lo arrays (a_lo, b_lo, out_lo "
+                   "must be NULL)");
+  else if (epilogue == ANYLOC_EPI_BIAS_SPLIT || epilogue == ANYLOC_EPI_GELU_SPLIT || epilogue == ANYLOC_EPI_SWIGLU_SPLIT)
     ANYLOC_REQUIRE(out_lo, "gemm_nt: split epilogue needs out_lo");
   if (epilogue == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_REQUIRE(N % 2 == 0, "gemm_nt: swiglu needs even N");
   if (epilogue == ANYLOC_EPI_LS_RESID) ANYLOC_REQUIRE(gamma && resid, "gemm_nt: LS_RESID needs gamma and resid");
   EpiParams ep{epilogue, bias, gamma, resid, (float*)out, (float*)out_lo, ldo};
   ep.alpha = alpha;
   ep.out_f16 = out_dtype == ANYLOC_PAIR_F16;
-  return gemm_dispatch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, engine, in_dtype == ANYLOC_PAIR_F16,
-                       (cudaStream_t)stream);
+  return gemm_dispatch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, engine, in_dtype, (cudaStream_t)stream);
 }
 
 // internal (topk.cu): plain-store GEMM with a device gate; not part of the public header
@@ -182,11 +203,21 @@ extern "C" int anyloc_split_f16(const float* x, void* hi, void* lo, size_t n, fl
   return launch_split_f16(x, hi, lo, n, scale, (cudaStream_t)stream);
 }
 
+extern "C" int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream) {
+  ANYLOC_REQUIRE(x && y, "split_bf16: null pointer");
+  if (n == 0) return ANYLOC_OK;
+  return launch_split_bf16(x, y, n, (cudaStream_t)stream);
+}
+
 extern "C" int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D,
                                       float eps, void* y_hi, void* y_lo, int out_dtype, void* stream) {
-  ANYLOC_REQUIRE(x && w && b && y_hi && y_lo, "layernorm: null pointer");
+  const bool bf16 = out_dtype == ANYLOC_PAIR_BF16;
+  ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || bf16), "layernorm: null pointer");
+  ANYLOC_REQUIRE(!(bf16 && y_lo), "layernorm: the single-bf16 output has no lo array (y_lo must be NULL)");
   if (M == 0) return ANYLOC_OK;
-  return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo, out_dtype == ANYLOC_PAIR_F16, (cudaStream_t)stream);
+  return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo,
+                          bf16 ? ANYLOC_PAIR_BF16 : out_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32,
+                          (cudaStream_t)stream);
 }
 
 // qkv_f16: qkv_{hi,lo} already hold fp16 pairs of 8*x for all three thirds (the ViT's qkv epilogue wrote them).
@@ -202,14 +233,26 @@ static int attention_dispatch(const float* qkv_hi, const float* qkv_lo, int B, i
   if (engine == ANYLOC_GEMM_SIMT || !tc_ok)
     return attention_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, out_f16, st);
   if (out_f16) {     // fp16-pair precision: operands are fp16 pairs too (inside the ViT the qkv epilogue wrote them)
-    if (qkv_f16) return attention_tc_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, true, st);
+    if (qkv_f16) return attention_tc_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, ANYLOC_PAIR_F16, st);
     return attention_tc16_standalone(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, st);
   }
-  return attention_tc_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, false, st);
+  return attention_tc_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, ANYLOC_PAIR_TF32, st);
 }
 
 extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                                 void* o_hi, void* o_lo, int out_dtype, int engine, void* stream) {
+  if (out_dtype == ANYLOC_PAIR_BF16) {     // single bf16 in and out: the qkv epilogue's output format
+    ANYLOC_REQUIRE(qkv_hi && o_hi, "attention: null pointer");
+    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the single-bf16 format has no lo arrays (qkv_lo, o_lo must be NULL)");
+    ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
+    if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0) {
+      set_error("attention: the single-bf16 format runs on the tensor-core engine only, with a 16-byte aligned qkv");
+      return ANYLOC_ERR_UNSUPPORTED;
+    }
+    if (B == 0 || T == 0) return ANYLOC_OK;
+    ProfScope ps(PC_ATTENTION, (cudaStream_t)stream, 4.0 * B * (double)T * T * D);
+    return attention_tc_launch(qkv_hi, nullptr, B, T, D, heads, o_hi, nullptr, ANYLOC_PAIR_BF16, (cudaStream_t)stream);
+  }
   ANYLOC_REQUIRE(qkv_hi && o_hi && o_lo, "attention: null pointer");
   ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
   if (B == 0 || T == 0) return ANYLOC_OK;
@@ -232,22 +275,34 @@ struct VitBuffers {
   float *pa_hi, *pa_lo, *ptmp, *x, *y_hi, *y_lo, *qkv, *qkv_lo, *h_hi, *h_lo;
   float* qkv32;     // [M, 3D] fp32 rows of a tapped layer's qkv GEMM (null unless the tap list needs them)
 };
-// n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`
+// n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  The single-bf16 format carves no
+// lo buffers and 2-byte GEMM inputs: pa [n_patch, Kp], y [M, D], qkv [M, 3D] (which also holds the fp32 [M, D] output
+// of a lone q/k/v tap), h [M, hidden] as bf16.
 size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
                  VitBuffers* out) {
   const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
+  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16;
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   VitBuffers b;
-  b.pa_hi = w.take<float>(n_patch * Kp); b.pa_lo = w.take<float>(n_patch * Kp);
-  b.ptmp = w.take<float>(n_patch * D);
-  b.x = w.take<float>(M * D);
-  b.y_hi = w.take<float>(M * D); b.y_lo = w.take<float>(M * D);
-  b.qkv = w.take<float>(M * 3 * D); b.qkv_lo = w.take<float>(M * 3 * D);
-  b.h_hi = w.take<float>(M * c->ffn_hidden); b.h_lo = w.take<float>(M * c->ffn_hidden);
+  if (bf16) {
+    b.pa_hi = (float*)w.take<uint16_t>(n_patch * Kp); b.pa_lo = nullptr;
+    b.ptmp = w.take<float>(n_patch * D);
+    b.x = w.take<float>(M * D);
+    b.y_hi = (float*)w.take<uint16_t>(M * D); b.y_lo = nullptr;
+    b.qkv = (float*)w.take<uint16_t>(M * 3 * D); b.qkv_lo = nullptr;
+    b.h_hi = (float*)w.take<uint16_t>(M * c->ffn_hidden); b.h_lo = nullptr;
+  } else {
+    b.pa_hi = w.take<float>(n_patch * Kp); b.pa_lo = w.take<float>(n_patch * Kp);
+    b.ptmp = w.take<float>(n_patch * D);
+    b.x = w.take<float>(M * D);
+    b.y_hi = w.take<float>(M * D); b.y_lo = w.take<float>(M * D);
+    b.qkv = w.take<float>(M * 3 * D); b.qkv_lo = w.take<float>(M * 3 * D);
+    b.h_hi = w.take<float>(M * c->ffn_hidden); b.h_lo = w.take<float>(M * c->ffn_hidden);
+  }
   b.qkv32 = qkv32 ? w.take<float>(M * 3 * D) : nullptr;
   if (out) *out = b;
-  if (ws && (!b.pa_hi || !b.pa_lo || !b.ptmp || !b.x || !b.y_hi || !b.y_lo || !b.qkv || !b.qkv_lo || !b.h_hi || !b.h_lo ||
-             (qkv32 && !b.qkv32)))
+  if (ws && (!b.pa_hi || !b.ptmp || !b.x || !b.y_hi || !b.qkv || !b.h_hi || (qkv32 && !b.qkv32) ||
+             (!bf16 && (!b.pa_lo || !b.y_lo || !b.qkv_lo || !b.h_lo))))
     return 0;
   return w.off;
 }
@@ -280,6 +335,25 @@ bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeight
     return false;
   }
   return true;
+}
+// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16 weights with a
+// non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for single bf16 on the SIMT engine
+int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int engine) {
+  if (cfg->pair_dtype != ANYLOC_PAIR_BF16) return ANYLOC_OK;
+  bool lo = w->patch_w_lo != nullptr;
+  for (int l = 0; l < cfg->depth && w->blocks; ++l) {
+    const AnylocVitBlock& b = w->blocks[l];
+    lo = lo || b.qkv_w_lo || b.proj_w_lo || b.in_w_lo || b.out_w_lo;
+  }
+  if (lo) {
+    set_error("%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
+    return ANYLOC_ERR_ARG;
+  }
+  if (engine == ANYLOC_GEMM_SIMT) {
+    set_error("%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)", fn);
+    return ANYLOC_ERR_UNSUPPORTED;
+  }
+  return ANYLOC_OK;
 }
 // Returns false (with the error text set) on an empty list, a bad layer or facet, a repeated tap or (need_out) a null
 // output.
@@ -334,15 +408,17 @@ static int facet_out(const VitSeqs& sq, int M, const float* src, int64_t ld, int
 }
 
 // the fp32 qkv rows of layer l in bf.qkv32 -> the facets of l the plan asks for and, when `pairs`, the attention's
-// (hi, lo) operands in bf.qkv / bf.qkv_lo (fp16 pairs when f16_attn, else tf32 pairs)
+// operands in bf.qkv / bf.qkv_lo (single bf16 in bf.qkv for the bf16 format, else fp16 pairs when f16_attn, else tf32
+// pairs)
 static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const VitSeqs& sq, const TapPlan& tp, int l,
                    bool pairs, bool f16_attn, cudaStream_t st) {
   const int D = c->embed_dim, m = tp.mask[l];
   const QkvTapOuts o{{(m & 1) ? tp.out[l][0] : nullptr, (m & 2) ? tp.out[l][1] : nullptr,
                       (m & 4) ? tp.out[l][2] : nullptr}};
-  const int pair = pairs ? (f16_attn ? 2 : 1) : 0;
+  const int pair = pairs ? (c->pair_dtype == ANYLOC_PAIR_BF16 ? 3 : f16_attn ? 2 : 1) : 0;
   const double rows_out = (double)M - (tp.use_cls ? 0 : sq.B);
-  const double bytes = 12.0 * M * D + (pair ? (pair == 2 ? 12.0 : 24.0) * M * D : 0.0) + 4.0 * rows_out * D * popcount3(m);
+  const double bytes = 12.0 * M * D + (pair ? (pair == 3 ? 6.0 : pair == 2 ? 12.0 : 24.0) * M * D : 0.0) +
+                       4.0 * rows_out * D * popcount3(m);
   ProfScope ps(PC_VIT_MISC, st, bytes);
   return launch_qkv_tap(bf.qkv32, M, sq.T, sq.img, D, pair, pairs ? bf.qkv : nullptr, pairs ? bf.qkv_lo : nullptr, o,
                         tp.use_cls, tp.norm_descs, st);
@@ -353,47 +429,51 @@ static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const Vit
 static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitBuffers& bf, int M, const VitSeqs& sq,
                      int engine, cudaStream_t st, const TapPlan* tp = nullptr, int l = 0) {
   const int D = c->embed_dim, Hf = c->ffn_hidden;
-  const bool f16 = c->pair_dtype == ANYLOC_PAIR_F16;
+  const int fmt = c->pair_dtype;
+  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16;
   int rc;
-  const double ln_bytes = (f16 ? 8.0 : 12.0) * M * D;
+  const double ln_bytes = (bf16 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
   { ProfScope ps(PC_LAYERNORM, st, ln_bytes);
-    if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc; }
+    if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
   // q, k and v leave the qkv GEMM row-major through the plain split epilogue; for the tensor-core attention in the
   // fp16-pair precision they are fp16 pairs of 8*x, the attention kernel's operand format
   const bool f16_attn = engine != ANYLOC_GEMM_SIMT && f16;
   if (tp) {
     EpiParams e_qkv{ANYLOC_EPI_BIAS, wb.qkv_b, nullptr, nullptr, bf.qkv32, nullptr, 3 * D};
     e_qkv.alpha = wb.qkv_alpha;
-    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
+    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, fmt, st))) return rc;
     if ((rc = qkv_tap(c, bf, M, sq, *tp, l, true, f16_attn, st))) return rc;
   } else {
     EpiParams e_qkv{ANYLOC_EPI_BIAS_SPLIT, wb.qkv_b, nullptr, nullptr, bf.qkv, bf.qkv_lo, 3 * D};
     e_qkv.out_f16 = f16_attn;
     e_qkv.alpha = wb.qkv_alpha;
-    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, f16, st))) return rc;
+    if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, fmt, st))) return rc;
   }
   if (sq.tab) {
     ProfScope ps(PC_ATTENTION, st, sq.attn_flops);
     if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, bf.y_hi, bf.y_lo,
-                                         f16, st)))
+                                         fmt, st)))
       return rc;
+  } else if (bf16) {
+    ProfScope ps(PC_ATTENTION, st, 4.0 * sq.B * (double)sq.T * sq.T * D);
+    if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, bf.y_hi, nullptr, fmt, st))) return rc;
   } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine,
                                       st, f16_attn))) {
     return rc;
   }
   EpiParams e_proj{ANYLOC_EPI_LS_RESID, wb.proj_b, wb.ls1, bf.x, bf.x, nullptr, D};
   e_proj.alpha = wb.proj_alpha;
-  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.proj_w_hi, wb.proj_w_lo, D, M, D, D, e_proj, engine, f16, st))) return rc;
+  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.proj_w_hi, wb.proj_w_lo, D, M, D, D, e_proj, engine, fmt, st))) return rc;
   { ProfScope ps(PC_LAYERNORM, st, ln_bytes);
-    if ((rc = launch_layernorm(bf.x, wb.ln2_w, wb.ln2_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc; }
+    if ((rc = launch_layernorm(bf.x, wb.ln2_w, wb.ln2_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
   EpiParams e_in{c->ffn_kind == ANYLOC_FFN_MLP ? ANYLOC_EPI_GELU_SPLIT : ANYLOC_EPI_SWIGLU_SPLIT, wb.in_b, nullptr,
                  nullptr, bf.h_hi, bf.h_lo, Hf};
   e_in.alpha = wb.in_alpha; e_in.out_f16 = f16;
   const int n_in = c->ffn_kind == ANYLOC_FFN_MLP ? Hf : 2 * Hf;
-  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.in_w_hi, wb.in_w_lo, D, M, n_in, D, e_in, engine, f16, st))) return rc;
+  if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.in_w_hi, wb.in_w_lo, D, M, n_in, D, e_in, engine, fmt, st))) return rc;
   EpiParams e_out{ANYLOC_EPI_LS_RESID, wb.out_b, wb.ls2, bf.x, bf.x, nullptr, D};
   e_out.alpha = wb.out_alpha;
-  return gemm_dispatch(bf.h_hi, bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf, e_out, engine, f16, st);
+  return gemm_dispatch(bf.h_hi, bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf, e_out, engine, fmt, st);
 }
 
 // Blocks 0..l_max over the M assembled token rows in bf.x, each run once, writing every tap of the plan:
@@ -404,28 +484,29 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
 //    third's own N = D GEMM and the facet slice, two or three are the N = 3D GEMM and the tap kernel without pairs.
 static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
                      const TapPlan& tp, int gemm_engine, cudaStream_t st) {
-  const int D = cfg->embed_dim;
-  const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
+  const int D = cfg->embed_dim, fmt = cfg->pair_dtype;
+  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16;
   int rc;
   for (int l = 0; l <= tp.l_max; ++l) {
     const AnylocVitBlock& wb = w->blocks[l];
     const int qkv = tp.mask[l] & 7;
     const bool token = (tp.mask[l] & 8) != 0;
     if (l == tp.l_max && !token) {
-      if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, f16, st))) return rc;
+      if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc;
       if (popcount3(qkv) == 1) {
         const int facet = qkv == 1 ? 0 : qkv == 2 ? 1 : 2;
-        const size_t woff = (size_t)facet * D * D * (f16 ? 2 : 4);      // bytes: weights are __half or float
+        const size_t woff = (size_t)facet * D * D * (f16 || bf16 ? 2 : 4);  // bytes: weights are __half/bf16 or float
         EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
         e_f.alpha = wb.qkv_alpha;
-        if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff, (const char*)wb.qkv_w_lo + woff,
-                                D, M, D, D, e_f, gemm_engine, f16, st)))
+        if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff,
+                                wb.qkv_w_lo ? (const char*)wb.qkv_w_lo + woff : nullptr, D, M, D, D, e_f, gemm_engine,
+                                fmt, st)))
           return rc;
         return facet_out(sq, M, bf.qkv, D, D, tp, tp.out[l][facet], st);
       }
       EpiParams e_qkv{ANYLOC_EPI_BIAS, wb.qkv_b, nullptr, nullptr, bf.qkv32, nullptr, 3 * D};
       e_qkv.alpha = wb.qkv_alpha;
-      if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, gemm_engine, f16,
+      if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, gemm_engine, fmt,
                               st)))
         return rc;
       return qkv_tap(cfg, bf, M, sq, tp, l, false, false, st);
@@ -448,6 +529,8 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
   ANYLOC_REQUIRE(cfg->embed_dim == cfg->num_heads * 64, "%s: head_dim must be 64", fn);
   ANYLOC_REQUIRE(B > 0, "%s: empty batch", fn);
   if (!registers_ok(fn, cfg, w)) return ANYLOC_ERR_ARG;
+  int rc;
+  if ((rc = format_check(fn, cfg, w, gemm_engine))) return rc;
   const int R = cfg->num_registers;
   const int P = cfg->patch, N = (H / P) * (W / P), T = N + 1 + R, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P);
   const int M = B * T;
@@ -457,13 +540,12 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
               vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  int rc;
-  const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
-  if ((rc = launch_im2col(img, B, H, W, P, Kp, bf.pa_hi, bf.pa_lo, f16, st))) return rc;
+  const int fmt = cfg->pair_dtype;
+  if ((rc = launch_im2col(img, B, H, W, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};
   e_pe.alpha = w->patch_alpha;
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, B * N, D, Kp, e_pe,
-                          gemm_engine, f16, st))) return rc;
+                          gemm_engine, fmt, st))) return rc;
   if ((rc = launch_assemble(bf.ptmp, w->cls_token, w->register_tokens, pos_embed, B, N, R, D, bf.x, st))) return rc;
   const VitSeqs sq{B, T, nullptr, 0, 0.0, nullptr};
   return vit_trunk(cfg, w, bf, M, sq, tp, gemm_engine, st);
@@ -571,6 +653,8 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
   ANYLOC_REQUIRE(gemm_engine == ANYLOC_GEMM_AUTO || gemm_engine == ANYLOC_GEMM_TC3, "%s: bad gemm_engine %d", fn,
                  gemm_engine);
   if (!registers_ok(fn, cfg, w)) return ANYLOC_ERR_ARG;
+  int rc;
+  if ((rc = format_check(fn, cfg, w, gemm_engine))) return rc;
   VarlenPlan p;
   if (!varlen_plan(cfg, B, hw, &p)) return ANYLOC_ERR_ARG;
   for (int i = 0; i < B; ++i)
@@ -582,14 +666,13 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
               vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  int rc;
-  const bool f16 = cfg->pair_dtype == ANYLOC_PAIR_F16;
+  const int fmt = cfg->pair_dtype;
   for (int i = 0; i < B; ++i) p.img.ptr[i] = img[i];
-  if ((rc = launch_im2col_varlen(p.img, p.n_patch, P, Kp, bf.pa_hi, bf.pa_lo, f16, st))) return rc;
+  if ((rc = launch_im2col_varlen(p.img, p.n_patch, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};
   e_pe.alpha = w->patch_alpha;
   if ((rc = gemm_dispatch(bf.pa_hi, bf.pa_lo, Kp, w->patch_w_hi, w->patch_w_lo, Kp, p.n_patch, D, Kp, e_pe,
-                          gemm_engine, f16, st))) return rc;
+                          gemm_engine, fmt, st))) return rc;
   for (int i = 0; i < B; ++i) p.img.ptr[i] = pos_embed[i];
   if ((rc = launch_assemble_varlen(bf.ptmp, w->cls_token, w->register_tokens, p.img, M, D, bf.x, st))) return rc;
   const VitSeqs sq{B, 0, &p.attn, p.n_tiles, p.attn_flops, &p.img};

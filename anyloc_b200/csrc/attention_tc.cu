@@ -10,6 +10,10 @@
 // double-buffered shared-memory ring with cp.async (rows beyond T are zero-filled and masked to -inf in S).  The S
 // accumulator fragments are exactly the A-operand fragments of P.V (fp16: two n8 tiles = one k16 step; tf32: the key
 // order inside a k8 step is permuted to match and V is read in the same order), so P never leaves registers.
+//
+// BF16 = true (with F16, the 2-byte layout): the single bf16 format -- q, k, v are one bf16 array bf16_rn(x) (no lo, no
+// scale); one mma.sync m16n8k16.bf16 per k-step for Q K^T and for P V in place of three, P rounded once to bf16 (no
+// P_SCALE: bf16 has fp32's exponent range), output one bf16 array bf16_rn(o).  Softmax and accumulators stay fp32.
 #include <stdlib.h>
 #include "common.cuh"
 
@@ -18,11 +22,12 @@ namespace atc {
 
 constexpr int BQ = 64, BKV = 64, HD = 64, WARPS = 4, THREADS = WARPS * 32;
 
-template <bool F16> struct Cfg {
-  using T = typename std::conditional<F16, __half, float>::type;
+template <bool F16, bool BF16 = false> struct Cfg {
+  using T = typename std::conditional<BF16, __nv_bfloat16, typename std::conditional<F16, __half, float>::type>::type;
   static constexpr int PITCH = F16 ? HD + 8 : HD + 4;                 // elements per smem row (bank-conflict-free reads)
   static constexpr int MAT = BKV * PITCH;                              // elements of one [64 keys x 64 dims] tile
-  static constexpr int STAGE = 4 * MAT;                                // K_hi, K_lo, V_hi, V_lo
+  static constexpr int NMAT = BF16 ? 2 : 4;                            // K_hi, K_lo, V_hi, V_lo (bf16: K, V)
+  static constexpr int STAGE = NMAT * MAT;
   static constexpr int SMEM_BYTES = 2 * STAGE * (int)sizeof(T);
   static constexpr int CHUNKS_PER_ROW = HD * (int)sizeof(T) / 16;     // 16-byte cp.async pieces per 64-dim row
 };
@@ -37,6 +42,13 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 __device__ __forceinline__ void mma_f16(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_bf16(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
       "{%0, %1, %2, %3};"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
@@ -60,15 +72,17 @@ __device__ __forceinline__ float ex2(float x) {
   float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 }
 __device__ __forceinline__ uint32_t f2u(float x) { return __float_as_uint(x); }
-__device__ __forceinline__ uint32_t ld_h2(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
+template <typename E>     // two adjacent 2-byte elements (fp16 or bf16) as one word
+__device__ __forceinline__ uint32_t ld_h2(const E* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
 // One CTA's work.  Uniform (VARLEN = false): blockIdx = (query tile, head, image) over B images of T tokens.  VARLEN:
 // blockIdx = (tile of the packed grid, head); the table gives the image's first row, its length T and its first tile.
-template <bool F16, bool VARLEN>
+template <bool F16, bool VARLEN, bool BF16 = false>
 __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T,
                                               int D, void* __restrict__ o_hi_, void* __restrict__ o_lo_,
                                               const VarlenAttnTable* tab) {
-  using C = Cfg<F16>;
+  static_assert(!BF16 || F16, "bf16 uses the 2-byte (k16) layout");
+  using C = Cfg<F16, BF16>;
   using E = typename C::T;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   E* smem = reinterpret_cast<E*>(smem_raw);
@@ -88,20 +102,22 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     qt -= tab->tile0[lo]; T = tab->len[lo]; img0 = (size_t)tab->row0[lo];
   }
   const int nblk = (T + BKV - 1) / BKV;
-  const float P_SCALE = F16 ? 1024.0f : 1.0f;
+  constexpr bool SCALED = F16 && !BF16;      // fp16 pairs carry s = kActScale and P is scaled into fp16's range
+  const float P_SCALE = SCALED ? 1024.0f : 1.0f;
   // S holds (s q).(s k), s = kActScale for fp16 pairs: fold 1/s^2 into the 1/sqrt(64) * log2(e) scale
-  const float kScale = 0.125f * 1.4426950408889634f * (F16 ? 1.0f / (kActScale * kActScale) : 1.0f);
+  const float kScale = 0.125f * 1.4426950408889634f * (SCALED ? 1.0f / (kActScale * kActScale) : 1.0f);
 
-  // ---- K/V block loader: 64 rows x {K_hi, K_lo, V_hi, V_lo}, 16-byte pieces, rows >= T zero-filled
+  // ---- K/V block loader: 64 rows x {K_hi, K_lo, V_hi, V_lo} (bf16: {K, V}), 16-byte pieces, rows >= T zero-filled
   auto load_block = [&](int j, int buf) {
     E* st = smem + buf * C::STAGE;
-    constexpr int PIECES = 4 * BKV * C::CHUNKS_PER_ROW;
+    constexpr int PIECES = C::NMAT * BKV * C::CHUNKS_PER_ROW;
     for (int p = threadIdx.x; p < PIECES; p += THREADS) {
       const int mat = p / (BKV * C::CHUNKS_PER_ROW), r = (p / C::CHUNKS_PER_ROW) % BKV, c = p % C::CHUNKS_PER_ROW;
       const int key = j * BKV + r;
       const bool valid = key < T;
-      const E* src = (mat & 1) ? qkv_lo : qkv_hi;
-      const size_t col = (size_t)((mat < 2) ? D : 2 * D) + (size_t)h * HD + (size_t)c * (16 / sizeof(E));
+      const E* src = (!BF16 && (mat & 1)) ? qkv_lo : qkv_hi;
+      const bool is_k = BF16 ? mat == 0 : mat < 2;
+      const size_t col = (size_t)(is_k ? D : 2 * D) + (size_t)h * HD + (size_t)c * (16 / sizeof(E));
       const E* gp = src + (valid ? (img0 + key) * ld + col : 0);
       cp_async16((uint32_t)__cvta_generic_to_shared(st + mat * C::MAT + r * C::PITCH + c * (16 / sizeof(E))), gp, valid);
     }
@@ -122,6 +138,7 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
         const int c0 = ks * 16 + 2 * t4, c1 = c0 + 8;
         qa_hi[ks][0] = v0 ? ld_h2(qkv_hi + r0 + c0) : 0u; qa_hi[ks][1] = v1 ? ld_h2(qkv_hi + r1 + c0) : 0u;
         qa_hi[ks][2] = v0 ? ld_h2(qkv_hi + r0 + c1) : 0u; qa_hi[ks][3] = v1 ? ld_h2(qkv_hi + r1 + c1) : 0u;
+        if (BF16) continue;
         qa_lo[ks][0] = v0 ? ld_h2(qkv_lo + r0 + c0) : 0u; qa_lo[ks][1] = v1 ? ld_h2(qkv_lo + r1 + c0) : 0u;
         qa_lo[ks][2] = v0 ? ld_h2(qkv_lo + r0 + c1) : 0u; qa_lo[ks][3] = v1 ? ld_h2(qkv_lo + r1 + c1) : 0u;
       } else {
@@ -146,7 +163,7 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     __syncthreads();
     const E* sK_hi = smem + buf * C::STAGE;
     const E* sK_lo = sK_hi + C::MAT;
-    const E* sV_hi = sK_hi + 2 * C::MAT;
+    const E* sV_hi = sK_hi + (BF16 ? 1 : 2) * C::MAT;
     const E* sV_lo = sK_hi + 3 * C::MAT;
 
     // ---- S = Q K^T (3-term) for this warp's 16 rows x 64 keys
@@ -162,6 +179,11 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
         for (int c = 0; c < 2; ++c) {
           uint32_t bh[4], bl[4];
           ldsm_x4((uint32_t)__cvta_generic_to_shared(sK_hi + key * C::PITCH + 32 * c + dim), bh);
+          if constexpr (BF16) {
+#pragma unroll
+            for (int u = 0; u < 2; ++u) mma_bf16(s[nt], qa_hi[2 * c + u], bh[2 * u], bh[2 * u + 1]);
+            continue;
+          }
           ldsm_x4((uint32_t)__cvta_generic_to_shared(sK_lo + key * C::PITCH + 32 * c + dim), bl);
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
@@ -215,7 +237,24 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     float pv[8][4];
 #pragma unroll
     for (int nd = 0; nd < 8; ++nd) pv[nd][0] = pv[nd][1] = pv[nd][2] = pv[nd][3] = 0.f;
-    if constexpr (F16) {
+    if constexpr (BF16) {
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {          // as the fp16 branch below, with P rounded once to bf16
+        uint32_t ph[4];
+        ph[0] = pack_bf16x2(s[2 * ks][0], s[2 * ks][1]);
+        ph[1] = pack_bf16x2(s[2 * ks][2], s[2 * ks][3]);
+        ph[2] = pack_bf16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
+        ph[3] = pack_bf16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
+        const int key = ks * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), dsel = 8 * (lane >> 4);
+#pragma unroll
+        for (int nd = 0; nd < 8; nd += 2) {
+          uint32_t vh[4];
+          ldsm_x4_t((uint32_t)__cvta_generic_to_shared(sV_hi + key * C::PITCH + nd * 8 + dsel), vh);
+#pragma unroll
+          for (int u = 0; u < 2; ++u) mma_bf16(pv[nd + u], ph, vh[2 * u], vh[2 * u + 1]);
+        }
+      }
+    } else if constexpr (F16) {
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {          // 16 keys per step = S tiles 2ks, 2ks+1
         uint32_t ph[4], pl[4];
@@ -280,7 +319,9 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
 #pragma unroll
     for (int nd = 0; nd < 8; ++nd) {
       const float a = o[nd][2 * half] * inv, c = o[nd][2 * half + 1] * inv;
-      if constexpr (F16) {
+      if constexpr (BF16) {
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(o_hi_) + off + nd * 8) = pack_bf16x2(a, c);
+      } else if constexpr (F16) {
         uint32_t hh, ll;
         split_f16x2(a, c, hh, ll);
         *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_hi_) + off + nd * 8) = hh;
@@ -296,21 +337,21 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
 }
 
 // B images of T tokens each: grid (query tiles, heads, B)
-template <bool F16>
+template <bool F16, bool BF16 = false>
 __global__ void __launch_bounds__(THREADS)
 attention_tc_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T, int D,
                     void* __restrict__ o_hi_, void* __restrict__ o_lo_) {
-  attention_cta<F16, false>(qkv_hi_, qkv_lo_, T, D, o_hi_, o_lo_, nullptr);
+  attention_cta<F16, false, BF16>(qkv_hi_, qkv_lo_, T, D, o_hi_, o_lo_, nullptr);
 }
 
 // Images of different lengths packed row after row: grid (sum of every image's query tiles, heads).  The host lists
 // the images longest first, so the CTAs with the longest key loops start first and short images fill the tail.
-template <bool F16>
+template <bool F16, bool BF16 = false>
 __global__ void __launch_bounds__(THREADS)
 attention_tc_varlen_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_,
                            const __grid_constant__ VarlenAttnTable tab, int D, void* __restrict__ o_hi_,
                            void* __restrict__ o_lo_) {
-  attention_cta<F16, true>(qkv_hi_, qkv_lo_, 0, D, o_hi_, o_lo_, &tab);
+  attention_cta<F16, true, BF16>(qkv_hi_, qkv_lo_, 0, D, o_hi_, o_lo_, &tab);
 }
 
 // fp32 (hi,lo) qkv pairs -> fp16 pairs of 8*x (same [M,3D] layout).  Standalone building-block path only.
@@ -325,9 +366,10 @@ qkv_to_f16_kernel(const float* __restrict__ qkv_hi, const float* __restrict__ qk
 
 }  // namespace atc
 
-// qkv_{hi,lo}: [B*T, 3D] pairs (fp16 pairs of 8*x when f16, else tf32 pairs); o_{hi,lo}: [B*T, D] pairs of the same kind.
+// qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, or single bf16 with qkv_lo
+// unused); o_{hi,lo}: [B*T, D] of the same kind (bf16: o_hi only).
 int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
-                        bool f16, cudaStream_t st) {
+                        int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(B <= 65535 && heads <= 65535, "attention_tc: grid too large (B=%d heads=%d)", B, heads);
@@ -339,7 +381,9 @@ int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, in
                                            Cfg<false>::SMEM_BYTES));
   }
   const dim3 grid(cdiv(T, BQ), heads, B);
-  if (f16) attention_tc_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
+  if (fmt == ANYLOC_PAIR_BF16)     // 36 KB of shared memory: under the default limit, no attribute needed
+    attention_tc_kernel<true, true><<<grid, THREADS, Cfg<true, true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
+  else if (fmt == ANYLOC_PAIR_F16) attention_tc_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
   else attention_tc_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
@@ -347,7 +391,7 @@ int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, in
 
 // the same over images of different lengths packed into one [sum T_i, 3D] qkv buffer; tab.tile0 runs to n_tiles
 int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int n_tiles, int D,
-                               int heads, void* o_hi, void* o_lo, bool f16, cudaStream_t st) {
+                               int heads, void* o_hi, void* o_lo, int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(heads <= 65535, "attention_tc: grid too large (heads=%d)", heads);
@@ -359,7 +403,10 @@ int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const Var
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<false>::SMEM_BYTES));
   }
   const dim3 grid(n_tiles, heads);
-  if (f16)
+  if (fmt == ANYLOC_PAIR_BF16)
+    attention_tc_varlen_kernel<true, true><<<grid, THREADS, Cfg<true, true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D,
+                                                                                             o_hi, o_lo);
+  else if (fmt == ANYLOC_PAIR_F16)
     attention_tc_varlen_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
   else
     attention_tc_varlen_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
@@ -377,7 +424,7 @@ int attention_tc16_standalone(const float* qkv_hi, const float* qkv_lo, int B, i
   const int blocks = (int)std::min<size_t>((nq + 255) / 256, (size_t)device_sm_count() * 16);
   atc::qkv_to_f16_kernel<<<blocks, 256, 0, st>>>(qkv_hi, qkv_lo, nq, buf, buf + nq);
   ANYLOC_CHECK_LAUNCH();
-  int rc = attention_tc_launch(buf, buf + nq, B, T, D, heads, o_hi, o_lo, true, st);
+  int rc = attention_tc_launch(buf, buf + nq, B, T, D, heads, o_hi, o_lo, ANYLOC_PAIR_F16, st);
   cudaFreeAsync(buf, st);
   return rc;
 }

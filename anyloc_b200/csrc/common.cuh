@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <math.h>
@@ -93,6 +94,14 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uin
   const float la = __fsub_rn(a, ha), lb = __fsub_rn(b, hb);
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hi2) : "f"(hb), "f"(ha));
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(lb), "f"(la));
+}
+
+// Single bf16 format (ANYLOC_PAIR_BF16): one array of bf16_rn(x), no lo word and no scale.  Two values -> one packed
+// word; `a` lands in the low 16 bits (element k), `b` in the high 16 bits (k+1).
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+  return r;
 }
 
 // Per-image geometry of a packed batch of differently sized images (anyloc_vit_extract_varlen).  The tables reach the

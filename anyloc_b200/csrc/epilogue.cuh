@@ -17,8 +17,12 @@ struct EpiParams {
   const int* gate = nullptr;   // device flag (nullable): tensor-core GEMM kernels return immediately when *gate == 0 (conditional fallbacks without a host sync)
 };
 
+// BF16 (the tensor-core GEMM's single-bf16 instantiation): the SPLIT outputs are one bf16 array, out = bf16_rn(v)
+template <bool BF16 = false>
 __device__ __forceinline__ void epi_store_split(const EpiParams& p, size_t o, float v) {
-  if (p.out_f16) {
+  if (BF16) {
+    reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16_rn(v);
+  } else if (p.out_f16) {
     __half h, l; split_f16(v * kActScale, h, l);
     reinterpret_cast<__half*>(p.out)[o] = h; reinterpret_cast<__half*>(p.out_lo)[o] = l;
   } else {
@@ -42,22 +46,24 @@ __device__ __forceinline__ float silu_fast(float x) {
 
 // Apply the epilogue to one accumulator element (m, n).  For SWIGLU the caller passes the PAIR
 // (acc0 at column n even, acc1 at column n+1) and the result lands in column n/2.
+template <bool BF16 = false>
 __device__ __forceinline__ void epi_store1(const EpiParams& p, int m, int n, float acc) {
   float v = acc * p.alpha + (p.bias ? __ldg(p.bias + n) : 0.f);
   size_t o = (size_t)m * p.ldo + n;
   switch (p.mode) {
     case ANYLOC_EPI_BIAS: p.out[o] = v; break;
-    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split(p, o, v); break;
-    case ANYLOC_EPI_GELU_SPLIT: epi_store_split(p, o, gelu_erf(v)); break;
+    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split<BF16>(p, o, v); break;
+    case ANYLOC_EPI_GELU_SPLIT: epi_store_split<BF16>(p, o, gelu_erf(v)); break;
     case ANYLOC_EPI_LS_RESID: p.out[o] = p.resid[o] + __ldg(p.gamma + n) * v; break;
     default: break;
   }
 }
+template <bool BF16 = false>
 __device__ __forceinline__ void epi_store_pair(const EpiParams& p, int m, int n_even, float acc0, float acc1) {
   // SWIGLU: columns (n_even, n_even+1) = (x1_j, x2_j), j = n_even/2
   float x1 = acc0 * p.alpha + (p.bias ? __ldg(p.bias + n_even) : 0.f);
   float x2 = acc1 * p.alpha + (p.bias ? __ldg(p.bias + n_even + 1) : 0.f);
-  epi_store_split(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
+  epi_store_split<BF16>(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
 }
 
 }  // namespace anyloc

@@ -13,7 +13,10 @@
 //                 (round-to-nearest) into a second register accumulator that holds the whole 64 x 128 sub-tile.  After
 //                 the last chunk: bias / GELU / SwiGLU / LayerScale+residual / pair split, staged in shared memory
 //                 subtile by subtile and stored with TMA (epilogue_staged), so the stores drain behind the next
-//                 tile's mainloop.  The hi-only passes, and outputs TMA cannot store, are stored from registers.
+//                 tile's mainloop.  The hi-only coarse passes, and outputs TMA cannot store, are stored from registers.
+// A third operand format, single bf16 (ANYLOC_PAIR_BF16: one bf16 array of bf16_rn(x), no lo, no scale), runs one
+// wgmma.f32.bf16.bf16 per k-step through the same pipeline with hi-only stages and the staged epilogue
+// (gemm_tc_bf16_launch): a third of the 3-term MMAs, not fp32-equivalent.
 // Tiles are rastered in bands of BAND_N column blocks, n-fastest inside a band: the resident CTAs share a few A row
 // panels and one band of B that stays in L2 while the outputs stream through.
 #include <cuda.h>
@@ -35,7 +38,9 @@ constexpr int STG_BYTES = 8192;            // one epilogue staging buffer (see e
 // LO = true : stages hold {A_hi, A_lo, B_hi, B_lo} (3-term split, 64 KB).  LO = false: hi-only single pass (coarse
 // scores): {A_hi, B_hi} = 32 KB per stage -> twice the pipeline depth in the same shared memory.
 // LOM (lo operands present): bit 0 = A_lo, bit 1 = B_lo; a compile-time mask keeps the wgmma sequence branch-free.
-template <bool LO> struct Cfg {
+// STG: the staged epilogue is compiled in -- the 3-term passes and the single-bf16 pass (hi-only, so 6 stages of 32 KB
+// plus 4 x 8 KB staging = 231 424 B of H100's 232 448 B opt-in), not the hi-only coarse passes (below).
+template <bool LO, bool STG = LO> struct Cfg {
   static constexpr int STAGE_BYTES = (LO ? 2 : 1) * (A_BYTES + B_BYTES);
   static constexpr int B_OFF = (LO ? 2 : 1) * A_BYTES;
   static constexpr int STAGES = LO ? 3 : 6;
@@ -45,13 +50,17 @@ template <bool LO> struct Cfg {
   // register epilogue, a small share of their time: with the staged path compiled in, their mainloop ran slower
   // (H100, retrieval coarse pass with the epilogue discarded: 2.46 -> 2.65 ms).  A launch that does not stage asks
   // for SMEM_BYTES only, the staged ones for SMEM_BYTES_STAGED.
-  static constexpr bool STAGED = LO;
+  static constexpr bool STAGED = STG;
   static constexpr int STG_OFF = BAR_OFF + 1024;
   static constexpr int SMEM_BYTES_STAGED = STG_OFF + 4 * STG_BYTES + 1024 /*align*/;
 };
 constexpr int BAND_N = 16;                 // column blocks per raster band
 constexpr int CHUNK_KB_TF32 = 2;          // k-blocks accumulated by the tensor core between two round-to-nearest adds
 constexpr int CHUNK_KB_F16 = 8;            // (24 / 96 wgmma k-steps per chunk)
+// The single-bf16 pass keeps the round-to-nearest chunks of the fp16 pairs (CHUNK_KB_F16: 32 wgmmas per chunk).  Its
+// second 64-register accumulator fits without spills (ptxas -v), the chunk add is 64 FADDs per thread per 32 wgmmas,
+// and it keeps the accumulation term of the error (c u sqrt(K) |A||B|, u = 2^-24) that of the f16x3 GEMMs, so the
+// operands' own bf16 rounding (2^-8 relative) is the only new error term.
 constexpr int CHUNK_KB_COARSE = 32;        // hi-only fp16 coarse pass (retrieval): <= 128 k-steps per chunk, the bound
                                            // topk.cu re-scores against
 
@@ -63,8 +72,11 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   n_blk = band * band_n + (r - m_blk * w);
 }
 
+template <bool BF16 = false>
 __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, float a, float b) {
-  if (ep.out_f16) {      // fp16 pair of kActScale*x
+  if (BF16) {            // single bf16
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + o) = pack_bf16x2(a, b);
+  } else if (ep.out_f16) {      // fp16 pair of kActScale*x
     uint32_t h, l;
     split_f16x2(a * kActScale, b * kActScale, h, l);
     *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(ep.out) + o) = h;
@@ -78,16 +90,17 @@ __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, floa
 }
 
 // epilogue of two adjacent accumulator columns (n even, n+1) of row m
+template <bool BF16 = false>
 __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int N, float v0, float v1) {
   const int mode = ep.mode;
   if (mode < 0) return;                    // diagnostic: discard (ANYLOC_GEMM_DEBUG_SKIP_EPI)
   if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {   // (x1_j, x2_j) = columns (2j, 2j+1); N is even
-    epi_store_pair(ep, m, n, v0, v1);
+    epi_store_pair<BF16>(ep, m, n, v0, v1);
     return;
   }
   if (n + 1 >= N || (ep.ldo & 1)) {
-    epi_store1(ep, m, n, v0);
-    if (n + 1 < N) epi_store1(ep, m, n + 1, v1);
+    epi_store1<BF16>(ep, m, n, v0);
+    if (n + 1 < N) epi_store1<BF16>(ep, m, n + 1, v1);
     return;
   }
   const float al = ep.alpha;
@@ -102,22 +115,23 @@ __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int 
     const float2 r = *reinterpret_cast<const float2*>(ep.resid + o);
     *reinterpret_cast<float2*>(ep.out + o) = make_float2(r.x + g.x * x0, r.y + g.y * x1);
   } else if (mode == ANYLOC_EPI_GELU_SPLIT) {
-    store_split2(ep, o, gelu_erf(x0), gelu_erf(x1));
+    store_split2<BF16>(ep, o, gelu_erf(x0), gelu_erf(x1));
   } else {                                 // BIAS_SPLIT
-    store_split2(ep, o, x0, x1);
+    store_split2<BF16>(ep, o, x0, x1);
   }
 }
 
 // Register epilogue of the 3-term passes that do not stage (gated launches, outputs TMA cannot store: see
 // make_epi_maps) of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16), accumulators in the wgmma layout,
 // applied and stored pair by pair.
+template <bool BF16 = false>
 __device__ __forceinline__ void epilogue_pairs(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int n = nq + j * 8;
     if (n >= N) continue;
-    if (r0 < M) epi_pair(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
-    if (r0 + 8 < M) epi_pair(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
+    if (r0 < M) epi_pair<BF16>(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
+    if (r0 + 8 < M) epi_pair<BF16>(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
   }
 }
 
@@ -182,15 +196,15 @@ __device__ __forceinline__ void epilogue_regs_batched(const EpiParams& ep, int r
 
 // ------------------------------------------------------------------ staged epilogue
 // Output formats of the staged path.  A subtile is 64 rows x COLS output columns; one 8 KB staging buffer holds it:
-// 64 x 32 fp32, or the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs.
-enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2 };
+// 64 x 32 fp32, the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs, or 64 x 64 single bf16.
+enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2, STG_BF16 = 3 };
 constexpr int STG_HALF = STG_BYTES / 2;    // offset of the lo array (pair formats)
 constexpr int STG_ROWS = 64;               // TMA box rows of the output maps: one consumer warpgroup's rows
 
 template <int KIND>
 struct StageFmt {
-  static constexpr int ESZ = KIND == STG_F16_PAIR ? 2 : 4;
-  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : 32;     // output columns per subtile
+  static constexpr int ESZ = KIND == STG_F16_PAIR || KIND == STG_BF16 ? 2 : 4;
+  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : KIND == STG_BF16 ? 64 : 32;   // output columns per subtile
   static constexpr int ROW_BYTES = COLS * ESZ;                       // 128 (fp32) or 64 bytes per row of one array
   static constexpr uint32_t SWZ = ROW_BYTES == 128 ? 7 : 3;          // TMA SWIZZLE_128B / SWIZZLE_64B
 };
@@ -255,7 +269,9 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
         if (SWIGLU) {                      // (x1_j, x2_j) = columns (n, n+1) -> output column n/2
           const float v = silu(x0) * x1;
           const uint32_t o = stg_off<KIND>(r, (4 * jj + q) * F::ESZ);
-          if (KIND == STG_F16_PAIR) {
+          if (KIND == STG_BF16) {
+            *reinterpret_cast<__nv_bfloat16*>(buf + o) = __float2bfloat16_rn(v);
+          } else if (KIND == STG_F16_PAIR) {
             __half hi, lo;
             split_f16(v * kActScale, hi, lo);
             *reinterpret_cast<__half*>(buf + o) = hi;
@@ -279,7 +295,9 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
           }
         } else {
           const float y0 = gelu ? gelu_erf(x0) : x0, y1 = gelu ? gelu_erf(x1) : x1;
-          if (KIND == STG_F16_PAIR) {
+          if (KIND == STG_BF16) {
+            *reinterpret_cast<uint32_t*>(buf + o) = pack_bf16x2(y0, y1);
+          } else if (KIND == STG_F16_PAIR) {
             uint32_t hi, lo;
             split_f16x2(y0 * kActScale, y1 * kActScale, hi, lo);
             *reinterpret_cast<uint32_t*>(buf + o) = hi;
@@ -299,7 +317,7 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
     else named_bar_sync<2>(128);
     if (t == 0) {
       tma_store_2d(tm_out, smem_u32(buf), oc0, m0);
-      if (KIND != STG_F32) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
+      if (KIND != STG_F32 && KIND != STG_BF16) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
       bulk_commit();
       if (RESID && s + 2 < BN / ACC && oc0 + 2 * F::COLS < n_out) {
         // residual of subtile s + 2 into this buffer, once the store has read it
@@ -313,10 +331,12 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
 
 // F16 = false: operands are fp32 words read as tf32 (32 elements per 128 B k-block, wgmma K=8)
 // F16 = true : operands are fp16            (64 elements per 128 B k-block, wgmma K=16, 2x rate)
+// BF16 = true (with F16 and LOM = 0): single bf16 operands, same layout and rate as fp16, one wgmma per k-step; the
+//             staged epilogue writes single bf16 SPLIT outputs (STG_BF16).
 // ep.gate (nullable): the kernel returns at once when *gate == 0 (conditional fallbacks without a host sync).
 // staged != 0: the epilogue goes through shared memory and TMA stores (tm_out, tm_out_lo for the pair formats,
 // tm_resid for LS_RESID: (n_out, M) maps with 64-row boxes); 0: stored pair by pair from registers.
-template <bool F16, int LOM>
+template <bool F16, int LOM, bool BF16 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
@@ -324,7 +344,8 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                 const __grid_constant__ CUtensorMap tm_resid, int staged,
                 int M, int N, int K, int band_n, int chunk_kb, EpiParams ep) {
   constexpr bool LO = LOM != 0, has_a_lo = (LOM & 1) != 0, has_b_lo = (LOM & 2) != 0;
-  using C = Cfg<LO>;
+  static_assert(!BF16 || (F16 && LOM == 0), "bf16 is a single-operand 2-byte format");
+  using C = Cfg<LO, LO || BF16>;
   if (ep.gate != nullptr && *reinterpret_cast<const volatile int*>(ep.gate) == 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -410,7 +431,8 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
           const uint64_t adv = (uint64_t)((k * 32) >> 4);      // +32 B per k-step inside the atom (both types)
-          wgmma_m64n128<F16>(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
+          if constexpr (BF16) wgmma_m64n128_bf16(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
+          else wgmma_m64n128<F16>(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
           if (has_a_lo) wgmma_m64n128<F16>(acc, a_lo + adv, b_hi + adv, 1u);
           if (has_b_lo) wgmma_m64n128<F16>(acc, a_hi + adv, b_lo + adv, 1u);
         }
@@ -434,7 +456,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       continue;
     }
     if (!staged) {
-      epilogue_pairs(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      epilogue_pairs<BF16>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
       continue;
     }
 #define ANYLOC_EPI_STAGED(KIND_, SWIGLU_, RESID_)                                                                   \
@@ -442,7 +464,10 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                                           n0, N, sum)
     if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(STG_F32, false, false);
     else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(STG_F32, false, true);
-    else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
+    else if (BF16) {                         // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> single bf16
+      if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_BF16, true, false);
+      else ANYLOC_EPI_STAGED(STG_BF16, false, false);
+    } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
       if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, true, false);
       else ANYLOC_EPI_STAGED(STG_TF32_PAIR, true, false);
     } else {                                 // BIAS_SPLIT / GELU_SPLIT
@@ -472,7 +497,7 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16) {
+int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
   const int esz = f16 ? 2 : 4;
@@ -480,8 +505,9 @@ int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box
   cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esz), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr, dims,
-                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = enc(map, dt, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("gemm_tc: cuTensorMapEncodeTiled failed (%d) rows=%d K=%d ld=%d", (int)r, rows, K, ld); return ANYLOC_ERR_CUDA; }
   return ANYLOC_OK;
@@ -489,15 +515,17 @@ int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box
 
 // output map of the staged epilogue: [rows, cols] of esz-byte elements, row pitch ld, boxes of 64 rows x box_cols
 // swizzled as stg_off places them.  TMA clips the boxes at rows and cols, so the ld padding is never written.
-static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int esz, int box_cols) {
+static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int esz, int box_cols,
+                        bool bf16 = false) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)STG_ROWS};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr,
-                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = enc(map, dt, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    box_cols * esz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("gemm_tc: cuTensorMapEncodeTiled failed (%d) for the output: rows=%d cols=%d ld=%d", (int)r, rows, cols, ld); return ANYLOC_ERR_CUDA; }
@@ -509,19 +537,21 @@ static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, i
 // gemm_tc_supported).  The row-length condition is conservative: in one H100 run of the staged-path test without it,
 // a 68-column fp16 output (136 bytes per row) came back with its ldo padding columns 68..71 written, as if the store
 // clipped columns only to 16-byte units.  Not reproduced since (the condition keeps such shapes off the staged path).
+// bf16: the SPLIT outputs are one bf16 array (64-column boxes, no lo map).
 static int make_epi_maps(const EpiParams& ep, int M, int N, CUtensorMap* m_out, CUtensorMap* m_lo, CUtensorMap* m_resid,
-                         bool* staged) {
+                         bool* staged, bool bf16) {
   memset(m_out, 0, sizeof(*m_out)); memset(m_lo, 0, sizeof(*m_lo)); memset(m_resid, 0, sizeof(*m_resid));
   const bool split = ep.mode == ANYLOC_EPI_BIAS_SPLIT || ep.mode == ANYLOC_EPI_GELU_SPLIT ||
                      ep.mode == ANYLOC_EPI_SWIGLU_SPLIT;
-  const int esz = split && ep.out_f16 ? 2 : 4;
+  const int esz = split && (ep.out_f16 || bf16) ? 2 : 4;
   const int n_out = ep.mode == ANYLOC_EPI_SWIGLU_SPLIT ? N / 2 : N;
   *staged = ep.mode >= 0 && ((long long)ep.ldo * esz) % 16 == 0 && ((long long)n_out * esz) % 16 == 0;
   if (!*staged) return ANYLOC_OK;
-  const int cols = split && !ep.out_f16 ? StageFmt<STG_TF32_PAIR>::COLS : StageFmt<STG_F32>::COLS;
+  const int cols = split && bf16 ? StageFmt<STG_BF16>::COLS
+                   : split && !ep.out_f16 ? StageFmt<STG_TF32_PAIR>::COLS : StageFmt<STG_F32>::COLS;
   int rc;
-  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols))) return rc;
-  if (split && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
+  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols, split && bf16))) return rc;
+  if (split && !bf16 && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
   if (ep.mode == ANYLOC_EPI_LS_RESID && (rc = make_out_map(m_resid, ep.resid, M, n_out, ep.ldo, esz, cols))) return rc;
   return ANYLOC_OK;
 }
@@ -544,34 +574,35 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
 // epilogue of this host thread's last launch (anyloc_gemm_tc_last_staged)
 static thread_local int g_last_staged = -1;
 
-template <bool F16, int LOM>
+template <bool F16, int LOM, bool BF16 = false>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                        int N, int K, const EpiParams& ep, int chunk, cudaStream_t st) {
   using namespace tc;
   constexpr bool LO = LOM != 0;
+  using CF = Cfg<LO, LO || BF16>;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
-  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16))) return rc;
-  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16))) return rc;
-  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16))) return rc;
-  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16))) return rc;
+  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16, BF16))) return rc;
+  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16, BF16))) return rc;
+  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16, BF16))) return rc;
+  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16, BF16))) return rc;
   CUtensorMap mo, mo_lo, mr;
   bool staged = false;
   memset(&mo, 0, sizeof(mo)); memset(&mo_lo, 0, sizeof(mo_lo)); memset(&mr, 0, sizeof(mr));
   // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
   // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
   // for more would make the SM switch its shared-memory configuration back and forth).
-  if (Cfg<LO>::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged))) return rc;
-  const int smem = staged ? Cfg<LO>::SMEM_BYTES_STAGED : Cfg<LO>::SMEM_BYTES;
+  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, BF16))) return rc;
+  const int smem = staged ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES;
   g_last_staged = staged ? 1 : 0;
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<LO>::STAGED ? Cfg<LO>::SMEM_BYTES_STAGED : Cfg<LO>::SMEM_BYTES));
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           CF::STAGED ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES));
   }
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
-  gemm_tc3_kernel<F16, LOM><<<grid, THREADS, smem, st>>>(
+  gemm_tc3_kernel<F16, LOM, BF16><<<grid, THREADS, smem, st>>>(
       ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(BAND_N, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
@@ -604,6 +635,14 @@ int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi
     default: return ANYLOC_GEMM_LAUNCH(true, 3);
   }
 #undef ANYLOC_GEMM_LAUNCH
+}
+
+// single-bf16 GEMM (ANYLOC_PAIR_BF16): one bf16 operand per side, one wgmma per k-step, fp32 accumulation in
+// round-to-nearest chunks as the fp16 pairs, staged epilogue; SPLIT outputs are one bf16 array
+int gemm_tc_bf16_launch(const void* a, int lda, const void* b, int ldb, int M, int N, int K, const EpiParams& ep,
+                        cudaStream_t st) {
+  static_assert(tc::Cfg<false, true>::SMEM_BYTES_STAGED <= 232448, "bf16 GEMM over H100's shared-memory opt-in");
+  return launch_impl<true, 0, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
 }
 
 }  // namespace anyloc

@@ -23,22 +23,35 @@ __global__ void split_f16_kernel(const float* __restrict__ x, __half* __restrict
   for (; i < n; i += stride) { __half h, l; split_f16(x[i] * scale, h, l); hi[i] = h; lo[i] = l; }
 }
 
-template <bool F16> struct PairOut;
-template <> struct PairOut<false> {
+// GEMM-input formats of the row kernels: FMT = ANYLOC_PAIR_TF32 (tf32 pairs), _F16 (fp16 pairs of kActScale*x) or
+// _BF16 (one bf16 array bf16_rn(x); the lo pointer is unused)
+// x -> bf16_rn(x) (single bf16 format)
+__global__ void split_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, size_t n) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) y[i] = __float2bfloat16_rn(x[i]);
+}
+
+template <int FMT> struct PairOut;
+template <> struct PairOut<ANYLOC_PAIR_TF32> {
   typedef float T;
   static __device__ __forceinline__ void put(float* hi, float* lo, size_t i, float v) { float h, l; split_tf32(v, h, l); hi[i] = h; lo[i] = l; }
 };
-template <> struct PairOut<true> {
+template <> struct PairOut<ANYLOC_PAIR_F16> {
   typedef __half T;
   static __device__ __forceinline__ void put(__half* hi, __half* lo, size_t i, float v) { __half h, l; split_f16(v * kActScale, h, l); hi[i] = h; lo[i] = l; }
+};
+template <> struct PairOut<ANYLOC_PAIR_BF16> {
+  typedef __nv_bfloat16 T;
+  static __device__ __forceinline__ void put(__nv_bfloat16* hi, __nv_bfloat16*, size_t i, float v) { hi[i] = __float2bfloat16_rn(v); }
 };
 
 // patch pi of image b of img [B,3,H,W] -> patch row `row` of (hi,lo), column order (c, ky, kx) like conv
 // weight.flatten(1)
-template <bool F16>
+template <int FMT>
 __device__ __forceinline__ void im2col_row(const float* __restrict__ img, int b, int H, int W, int P, int Kp, size_t row,
-                                           int pi, typename PairOut<F16>::T* __restrict__ hi,
-                                           typename PairOut<F16>::T* __restrict__ lo) {
+                                           int pi, typename PairOut<FMT>::T* __restrict__ hi,
+                                           typename PairOut<FMT>::T* __restrict__ lo) {
   const int gw = W / P;
   const int py = pi / gw, px = pi % gw;
   const int Kreal = 3 * P * P;
@@ -48,27 +61,27 @@ __device__ __forceinline__ void im2col_row(const float* __restrict__ img, int b,
       int ch = c / (P * P), rem = c % (P * P), ky = rem / P, kx = rem % P;
       v = __ldg(img + (((size_t)b * 3 + ch) * H + (py * P + ky)) * W + (px * P + kx));
     }
-    PairOut<F16>::put(hi, lo, row * Kp + c, v);
+    PairOut<FMT>::put(hi, lo, row * Kp + c, v);
   }
 }
 
 // img [B,3,H,W] -> patches (hi,lo) [B*gh*gw, Kp]
-template <bool F16>
+template <int FMT>
 __global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H, int W, int P, int Kp,
-                                    typename PairOut<F16>::T* __restrict__ hi, typename PairOut<F16>::T* __restrict__ lo) {
+                                    typename PairOut<FMT>::T* __restrict__ hi, typename PairOut<FMT>::T* __restrict__ lo) {
   const int gh = H / P, gw = W / P;
   const size_t row = blockIdx.x;               // patch index
   const int b = (int)(row / (gh * gw)), pi = (int)(row % (gh * gw));
-  im2col_row<F16>(img, b, H, W, P, Kp, row, pi, hi, lo);
+  im2col_row<FMT>(img, b, H, W, P, Kp, row, pi, hi, lo);
 }
 
 // images of different sizes, one block per patch row of the packed [sum gh_i*gw_i, Kp] output
-template <bool F16>
+template <int FMT>
 __global__ void im2col_split_varlen_kernel(const __grid_constant__ VarlenImgTable tab, int P, int Kp,
-                                           typename PairOut<F16>::T* __restrict__ hi,
-                                           typename PairOut<F16>::T* __restrict__ lo) {
+                                           typename PairOut<FMT>::T* __restrict__ hi,
+                                           typename PairOut<FMT>::T* __restrict__ lo) {
   const int skip = 1 + tab.nreg, row = blockIdx.x, i = varlen_image_of(tab, row, skip);
-  im2col_row<F16>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - skip * i), hi, lo);
+  im2col_row<FMT>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - skip * i), hi, lo);
 }
 
 // x[row,:] = cls + pos[0] (t = 0), reg[t-1] (1 <= t <= R: no positional embedding) or patch[b*N + p,:] + pos[1+p]
@@ -105,12 +118,13 @@ __global__ void assemble_tokens_varlen_kernel(const float* __restrict__ patch, c
                row - tab.tok0[i], x);
 }
 
-// LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo). One warp per row.
-template <int MAXV, bool F16>   // float4 per lane
+// LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo), or single bf16 (statistics in fp32 either
+// way). One warp per row.
+template <int MAXV, int FMT>   // float4 per lane
 __global__ void __launch_bounds__(256)
 layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
                        const float* __restrict__ b, int M, int D, float eps,
-                       typename PairOut<F16>::T* __restrict__ y_hi, typename PairOut<F16>::T* __restrict__ y_lo) {
+                       typename PairOut<FMT>::T* __restrict__ y_hi, typename PairOut<FMT>::T* __restrict__ y_lo) {
   const int lane = threadIdx.x & 31;
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (row >= M) return;
@@ -143,7 +157,9 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
       float4 ww = __ldg(w4 + d), bb = __ldg(b4 + d);
       const float y0 = (v[i].x - mean) * rstd * ww.x + bb.x, y1 = (v[i].y - mean) * rstd * ww.y + bb.y;
       const float y2 = (v[i].z - mean) * rstd * ww.z + bb.z, y3 = (v[i].w - mean) * rstd * ww.w + bb.w;
-      if constexpr (F16) {
+      if constexpr (FMT == ANYLOC_PAIR_BF16) {
+        reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] = make_uint2(pack_bf16x2(y0, y1), pack_bf16x2(y2, y3));
+      } else if constexpr (FMT == ANYLOC_PAIR_F16) {
         uint2 h, l;
         split_f16x2(y0 * kActScale, y1 * kActScale, h.x, l.x);
         split_f16x2(y2 * kActScale, y3 * kActScale, h.y, l.y);
@@ -202,7 +218,7 @@ __device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x,
 
 // One fp32 row [q | k | v] of a tapped layer's qkv GEMM (3D columns, one warp, each element read once) -> the
 // attention's operand pairs of the row, in the format the qkv GEMM's split epilogue writes (pair: 0 none, 1 tf32
-// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split), and the rows of the requested facets (out[f] != null),
+// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split; 3 single bf16, lo unused), and the rows of the requested facets (out[f] != null),
 // through facet_row's arithmetic.
 template <int MAXV>     // float4 per lane and third: D <= 128 * MAXV
 __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int pair, void* hi,
@@ -215,7 +231,14 @@ __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < MAXV; ++i)
       if (lane + i * 32 < D4) v[i] = xr[lane + i * 32];
-    if (pair == 2) {
+    if (pair == 3) {
+      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(hi) + (size_t)f * D);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int d = lane + i * 32;
+        if (d < D4) h2[d] = make_uint2(pack_bf16x2(v[i].x, v[i].y), pack_bf16x2(v[i].z, v[i].w));
+      }
+    } else if (pair == 2) {
       uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
       uint2* l2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(lo) + (size_t)f * D);
 #pragma unroll
@@ -265,9 +288,9 @@ qkv_tap_kernel(const float* __restrict__ src, int M, int T, int D, int pair, voi
   if (row >= M) return;
   const int b = row / T, t = row - b * T;
   const int64_t orow = use_cls ? row : (t == 0 ? -1 : row - b - 1);
-  const size_t e = (size_t)row * 3 * D * (pair == 2 ? 2 : 4);     // byte offset of the row's pairs
+  const size_t e = (size_t)row * 3 * D * (pair >= 2 ? 2 : 4);     // byte offset of the row's pairs
   qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
-                    pair ? (char*)lo + e : nullptr, o, orow, do_norm);
+                    lo ? (char*)lo + e : nullptr, o, orow, do_norm);
 }
 
 // images of different sizes packed row after row: image i's tokens from tab.tok0[i]
@@ -280,9 +303,9 @@ qkv_tap_varlen_kernel(const float* __restrict__ src, const __grid_constant__ Var
   if (row >= M) return;
   const int i = varlen_image_of(tab, row, 0);
   const int64_t orow = use_cls ? row : (row == tab.tok0[i] ? -1 : row - i - 1);
-  const size_t e = (size_t)row * 3 * D * (pair == 2 ? 2 : 4);
+  const size_t e = (size_t)row * 3 * D * (pair >= 2 ? 2 : 4);
   qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
-                    pair ? (char*)lo + e : nullptr, o, orow, do_norm);
+                    lo ? (char*)lo + e : nullptr, o, orow, do_norm);
 }
 
 // gather token rows [B, T, ld] (skipping cls unless use_cls, column offset col0) -> [B, T', D] then normalise
@@ -323,9 +346,21 @@ int launch_split_f16(const float* x, void* hi, void* lo, size_t n, float scale, 
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-int launch_im2col(const float* img, int B, int H, int W, int P, int Kp, void* hi, void* lo, bool f16, cudaStream_t st) {
-  if (f16) im2col_split_kernel<true><<<B * (H / P) * (W / P), 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, (__half*)lo);
-  else im2col_split_kernel<false><<<B * (H / P) * (W / P), 128, 0, st>>>(img, B, H, W, P, Kp, (float*)hi, (float*)lo);
+int launch_split_bf16(const float* x, void* y, size_t n, cudaStream_t st) {
+  int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)device_sm_count() * 16);
+  if (blocks < 1) blocks = 1;
+  split_bf16_kernel<<<blocks, 256, 0, st>>>(x, (__nv_bfloat16*)y, n);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+// fmt: ANYLOC_PAIR_* of the patch rows (bf16: lo unused)
+int launch_im2col(const float* img, int B, int H, int W, int P, int Kp, void* hi, void* lo, int fmt, cudaStream_t st) {
+  const int n = B * (H / P) * (W / P);
+  if (fmt == ANYLOC_PAIR_BF16)
+    im2col_split_kernel<ANYLOC_PAIR_BF16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__nv_bfloat16*)hi, nullptr);
+  else if (fmt == ANYLOC_PAIR_F16)
+    im2col_split_kernel<ANYLOC_PAIR_F16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, (__half*)lo);
+  else im2col_split_kernel<ANYLOC_PAIR_TF32><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (float*)hi, (float*)lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -335,20 +370,22 @@ int launch_assemble(const float* patch, const float* cls, const float* reg, cons
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-template <bool F16>
+template <int FMT>
 static void ln_launch(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi, void* y_lo,
                       cudaStream_t st) {
-  typedef typename PairOut<F16>::T T;
+  typedef typename PairOut<FMT>::T T;
   int blocks = cdiv(M, 8);
-  if (D <= 512) layernorm_split_kernel<4, F16><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
-  else if (D <= 1024) layernorm_split_kernel<8, F16><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
-  else layernorm_split_kernel<16, F16><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+  if (D <= 512) layernorm_split_kernel<4, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+  else if (D <= 1024) layernorm_split_kernel<8, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+  else layernorm_split_kernel<16, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
 }
+// fmt: ANYLOC_PAIR_* of the output (bf16: y_lo unused)
 int launch_layernorm(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi,
-                     void* y_lo, bool f16, cudaStream_t st) {
+                     void* y_lo, int fmt, cudaStream_t st) {
   ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "layernorm: D=%d unsupported (multiple of 4, <= 2048)", D);
-  if (f16) ln_launch<true>(x, w, b, M, D, eps, y_hi, y_lo, st);
-  else ln_launch<false>(x, w, b, M, D, eps, y_hi, y_lo, st);
+  if (fmt == ANYLOC_PAIR_BF16) ln_launch<ANYLOC_PAIR_BF16>(x, w, b, M, D, eps, y_hi, nullptr, st);
+  else if (fmt == ANYLOC_PAIR_F16) ln_launch<ANYLOC_PAIR_F16>(x, w, b, M, D, eps, y_hi, y_lo, st);
+  else ln_launch<ANYLOC_PAIR_TF32>(x, w, b, M, D, eps, y_hi, y_lo, st);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -360,10 +397,13 @@ int launch_facet_out(const float* src, int B, int T, int64_t ld, int col0, int D
   return ANYLOC_OK;
 }
 // packed batches of differently sized images: tab.ptr holds the images (im2col) or the positional tables (assembly)
-int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp, void* hi, void* lo, bool f16,
+int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp, void* hi, void* lo, int fmt,
                          cudaStream_t st) {
-  if (f16) im2col_split_varlen_kernel<true><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, (__half*)lo);
-  else im2col_split_varlen_kernel<false><<<n_patches, 128, 0, st>>>(tab, P, Kp, (float*)hi, (float*)lo);
+  if (fmt == ANYLOC_PAIR_BF16)
+    im2col_split_varlen_kernel<ANYLOC_PAIR_BF16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__nv_bfloat16*)hi, nullptr);
+  else if (fmt == ANYLOC_PAIR_F16)
+    im2col_split_varlen_kernel<ANYLOC_PAIR_F16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, (__half*)lo);
+  else im2col_split_varlen_kernel<ANYLOC_PAIR_TF32><<<n_patches, 128, 0, st>>>(tab, P, Kp, (float*)hi, (float*)lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -379,7 +419,7 @@ int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int row
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none) and facet rows; tab: packed images, else
+// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none; pair 3: single bf16 in hi) and facet rows; tab: packed images, else
 // B images of T tokens
 template <int MAXV>
 static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi,

@@ -277,6 +277,20 @@ class _HookHandle:
         pass
 
 
+PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16")
+
+
+def resolve_precision(precision, gemm_engine="auto"):
+    """The extractor's precision: the argument, else $ANYLOC_B200_PRECISION, else "auto".  ValueError on an unknown
+    name, and on "bf16" with gemm_engine="simt" (single bf16 runs on the tensor cores only)."""
+    precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3' or 'bf16', got {precision!r}")
+    if precision == "bf16" and gemm_engine == "simt":
+        raise ValueError("precision='bf16' runs on the tensor cores only; use gemm_engine='auto' or 'tc3'")
+    return precision
+
+
 class _GuardedExtractor:
     """What DinoV2ExtractFeatures and DinoV2MultiExtractFeatures share: the uploaded backbone (blocks 0.._depth()-1),
     the precision choice and the fp16-range guard around each call.  A subclass sets the call options and defines
@@ -285,14 +299,12 @@ class _GuardedExtractor:
     def _load(self, dino_model, dev, weights, gemm_engine, precision):
         sd = weights if weights is not None else _vit.resolve_state_dict(dino_model, dev)
         # only the blocks the forward runs (early exit at the deepest hooked module) are uploaded
-        precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
-        if precision not in ("tf32x3", "f16x3", "auto"):
-            raise ValueError(f"precision must be 'auto', 'tf32x3' or 'f16x3', got {precision!r}")
+        precision = resolve_precision(precision, gemm_engine)
         self._auto = precision == "auto"
         self._state_dict = sd if self._auto else None     # kept for the tf32x3 re-upload on an fp16-range overflow
         self.precision = "f16x3" if self._auto else precision
         self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=self._depth(),
-                                          pair="f16" if self.precision == "f16x3" else "tf32")
+                                          pair={"f16x3": "f16", "tf32x3": "tf32", "bf16": "bf16"}[self.precision])
         self.gemm_engine = gemm_engine
         self.fh_handle = _HookHandle()
         self._hook_out = None
@@ -356,7 +368,11 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
     silently, and the call raises) or "auto" (the default: f16x3 until a call overflows, then that
     call is redone and the extractor stays in tf32x3 -- trained DINOv2 checkpoints have outlier
     activations that random-init weights do not).  All accumulate in fp32 with round-to-nearest
-    chunk accumulation.
+    chunk accumulation.  "bf16" is the fast mode, never chosen by "auto": every GEMM and attention
+    operand is one round-to-nearest bf16 value (fp32's exponent range, so no overflow guard), one
+    bf16 MMA per product instead of three; the residual stream, LayerNorm statistics, softmax,
+    accumulators and outputs stay fp32.  Its outputs are those of the model run on bf16-rounded
+    activations (about 1e-2 relative), not fp32 parity; it needs gemm_engine "auto" or "tc3".
 
     `dino_model` may also name a backbone with register tokens, `dinov2_vit{s,b,l,g}14_reg`.  As
     in the reference, only row 0 (cls) is dropped, so its 4 register rows come first: an output
@@ -393,7 +409,7 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
         """img [B,3,H,W] -> [B, (1 +) R + N, D] (R = 4 register rows for the *_reg models, else 0); or a list/tuple of
         differently sized images [3,H_i,W_i] / [1,3,H_i,W_i], all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
         pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
-        image of fewer than 32 tokens takes the SIMT GEMMs)."""
+        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16", which always runs them)."""
         return self._guarded(img)
 
     def __del__(self):

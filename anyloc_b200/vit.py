@@ -107,7 +107,9 @@ def interpolate_pos_embed(pos_embed, gh, gw, offset=INTERP_OFFSET, antialias=Fal
 
 class VitWeights:
     """Device-resident, kernel-ready weights of one DINOv2 backbone (blocks 0..depth-1).  A register model's outputs
-    hold its num_registers register rows between the cls row and the patch rows, as the reference returns them."""
+    hold its num_registers register rows between the cls row and the patch rows, as the reference returns them.
+    pair: the operand format of every GEMM -- "tf32" / "f16" (fp32-equivalent (hi, lo) pairs) or "bf16" (one
+    round-to-nearest bf16 copy of each weight matrix, half the bytes of the pairs; a fast mode, not a parity mode)."""
 
     def __init__(self, name, state_dict, device, depth=None, pair="tf32"):
         if name not in ARCHS:
@@ -139,9 +141,15 @@ class VitWeights:
 
         def split(t):
             """-> (hi, lo, alpha): the kernel-ready pair of a weight matrix and the accumulator scale
-            1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs)."""
+            1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs; bf16: (bf16_rn(w), None, 1.0))."""
             t = f32(t)
             with torch.cuda.device(dev):
+                if pair == "bf16":
+                    hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
+                    _lib.check(lib.anyloc_split_bf16(_lib.ptr(t), _lib.ptr(hi), t.numel(), _lib.stream_ptr()),
+                               "split_bf16")
+                    self._keep.append(hi)
+                    return hi, None, 1.0
                 if pair == "tf32":
                     hi, lo = torch.empty_like(t), torch.empty_like(t)
                     _lib.check(lib.anyloc_split_tf32(_lib.ptr(t), _lib.ptr(hi), _lib.ptr(lo), t.numel(),
@@ -181,7 +189,7 @@ class VitWeights:
             blk = self.blocks[i]
 
             def put(field, t):
-                setattr(blk, field, t.data_ptr())
+                setattr(blk, field, None if t is None else t.data_ptr())
 
             put("ln1_w", keep(sd[p + "norm1.weight"])); put("ln1_b", keep(sd[p + "norm1.bias"]))
             hi, lo, blk.qkv_alpha = split(sd[p + "attn.qkv.weight"]); put("qkv_w_hi", hi); put("qkv_w_lo", lo)
@@ -206,7 +214,8 @@ class VitWeights:
             put("ls2", keep(sd[p + "ls2.gamma"]))
         self.cfg = _lib.VitCfg(self.dim, self.depth, self.heads, _lib.FFN[self.ffn_kind], self.hidden, PATCH,
                                _lib.PAIR[pair], self.num_registers)
-        self.struct = _lib.VitWeightsStruct(self.patch_w[0].data_ptr(), self.patch_w[1].data_ptr(),
+        self.struct = _lib.VitWeightsStruct(self.patch_w[0].data_ptr(),
+                                            None if self.patch_w[1] is None else self.patch_w[1].data_ptr(),
                                             self.patch_b.data_ptr(), self.cls_token.data_ptr(), self.blocks,
                                             patch_alpha,
                                             self.register_tokens.data_ptr() if self.num_registers else None)

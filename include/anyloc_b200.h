@@ -56,6 +56,12 @@ extern "C" {
 #define ANYLOC_PAIR_F16 1          /* two fp16 arrays of s*x (s power of two): hi = fp16(s x), lo = fp16(s x - hi);
                                       kind::f16 tensor path (2x rate); activations use s = 8, the epilogue's alpha
                                       undoes s_A*s_B.  Values beyond the fp16 range (|s x| > 65504) overflow. */
+#define ANYLOC_PAIR_BF16 2         /* NOT a pair and NOT fp32-equivalent: one bf16 array of bf16_rn(x) (8 significant
+                                      bits, fp32's exponent range), no lo array (every *_lo pointer NULL), no scale
+                                      (alpha 1); one bf16 MMA per product instead of three.  Tensor-core engine only
+                                      (wgmma GEMM at every M, mma.sync attention): ANYLOC_GEMM_SIMT returns
+                                      ANYLOC_ERR_UNSUPPORTED.  Accumulators, LayerNorm statistics, softmax, the
+                                      residual stream and every feature output stay fp32. */
 /* GEMM engines */
 #define ANYLOC_GEMM_AUTO 0
 #define ANYLOC_GEMM_SIMT 1         /* fp32 FFMA (validation / odd shapes)               */
@@ -205,7 +211,8 @@ typedef struct {
   int ffn_kind;    /* ANYLOC_FFN_* */
   int ffn_hidden;  /* 4*D (mlp) or 4096-style fused hidden (swiglu) */
   int patch;       /* 14 */
-  int pair_dtype;  /* ANYLOC_PAIR_*: format of the weight pairs and of all GEMM-input activations */
+  int pair_dtype;  /* ANYLOC_PAIR_*: format of the weight pairs and of all GEMM-input activations (see below for
+                      ANYLOC_PAIR_BF16) */
   int num_registers; /* R register tokens (dinov2_vit*14_reg: 4; 0 for the plain models) */
 } AnylocVitCfg;
 
@@ -240,6 +247,17 @@ typedef struct {
  * R register rows come first: [B, (1 +) R + N, D].  Every token count below (workspaces, the 32-bit token limit of the
  * _varlen calls) counts T per image.  R < 0, or R > 0 with a null register_tokens, returns ANYLOC_ERR_ARG (the
  * *_workspace_bytes functions return 0).  R = 0 is the plain model. */
+/* Single bf16 (pair_dtype = ANYLOC_PAIR_BF16), the fast mode of every anyloc_vit_extract* call below: the weight
+ * matrices are one bf16 array each (anyloc_split_bf16) with every *_w_lo NULL and every *_alpha 1; LayerNorm, im2col,
+ * the qkv epilogue / tap and the attention write one bf16 array; the GEMMs and the attention run one bf16 MMA per
+ * product.  The residual stream, LayerNorm statistics, softmax, every accumulator and every output stay fp32.  It is
+ * not a parity mode: an output's error is that of the model run on bf16-rounded activations (about 2^-8 relative per
+ * operand), not the 3-term formats' ~1e-6.  A non-NULL *_w_lo returns ANYLOC_ERR_ARG and gemm_engine =
+ * ANYLOC_GEMM_SIMT ANYLOC_ERR_UNSUPPORTED, before anything is launched.  Every GEMM runs on the tensor cores whatever
+ * M, so under ANYLOC_GEMM_AUTO too an image's rows are bit-identical across single, list (_varlen) and tap calls.
+ * Workspace: with A(x) = x rounded up to 256 bytes, n_p patch rows, M token rows and H = ffn_hidden,
+ *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(2 M D) + A(6 M D) + A(2 M H) [+ A(12 M D) for the fp32 qkv rows of the
+ *   tap calls, as below] + 4096 bytes. */
 /* padded patch-embed reduction length (3*14*14=588 -> multiple of 32) */
 int anyloc_vit_patch_k(int patch);
 size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W);
@@ -262,7 +280,8 @@ int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeights* w_host, 
  *             i's grid (images of the same grid may share one)
  *   out       packed [sum_i n_i, D] with n_i = R + g_h,i * g_w,i (+1 if use_cls); image i's rows start at sum_{j<i} n_j.
  * Each image's rows are bit-identical to anyloc_vit_extract on that image alone with the same GEMM engine (under
- * ANYLOC_GEMM_AUTO, a lone image of fewer than 32 tokens takes the SIMT GEMMs there, so compare those under TC3).
+ * ANYLOC_GEMM_AUTO, a lone image of fewer than 32 tokens takes the SIMT GEMMs there, so compare those under TC3; the
+ * single-bf16 format never does).
  * gemm_engine = ANYLOC_GEMM_SIMT returns ANYLOC_ERR_UNSUPPORTED: the packed attention is a tensor-core kernel.  The
  * call copies the geometry into kernel parameters; it neither synchronises with the host nor keeps any host pointer
  * it was given.  1 <= B <= ANYLOC_VIT_VARLEN_MAX_B. */
@@ -308,7 +327,10 @@ int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeigh
 
 /* ------------------------------------------- building blocks (exported for parity tests)
  * C[M,N] = (A_hi+A_lo)[M,K] . (B_hi+B_lo)[N,K]^T with epilogue; *_lo nullable (treated as 0).
- * lda/ldb/ldo in elements.  out_lo/bias/gamma/resid per epilogue. */
+ * lda/ldb/ldo in elements.  out_lo/bias/gamma/resid per epilogue.
+ * in_dtype = out_dtype = ANYLOC_PAIR_BF16: C = A . B^T of single bf16 operands (a_lo, b_lo, out_lo NULL, else
+ * ANYLOC_ERR_ARG; bf16 in with another out_dtype, or the reverse, ANYLOC_ERR_ARG); the SPLIT epilogues write one bf16
+ * array bf16_rn(v), BIAS / LS_RESID fp32 as usual.  Tensor-core engine only, at every M (SIMT: ANYLOC_ERR_UNSUPPORTED). */
 int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                    int ldb, int M, int N, int K, int in_dtype, float alpha, int epilogue, const float* bias,
                    const float* gamma, const float* resid, void* out, void* out_lo, int ldo, int out_dtype,
@@ -318,10 +340,16 @@ int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const void* b_hi
 int anyloc_gemm_tc_last_staged(void);
 int anyloc_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stream);
 int anyloc_split_f16(const float* x, void* hi, void* lo, size_t n, float scale, void* stream);
+/* y = bf16_rn(x), the single-bf16 weight format */
+int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream);
+/* out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG) */
 int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D, float eps,
                            void* y_hi, void* y_lo, int out_dtype, void* stream);
 /* softmax(q k^T / 8) v per head (head_dim 64).  qkv (hi,lo) pairs [B,T,3D] ([q|k|v] thirds); qkv_lo may
- * be NULL for the SIMT engine (plain fp32 input).  -> o (hi,lo) [B,T,D].  engine: ANYLOC_GEMM_*. */
+ * be NULL for the SIMT engine (plain fp32 input).  -> o (hi,lo) [B,T,D].  engine: ANYLOC_GEMM_*.
+ * out_dtype = ANYLOC_PAIR_BF16: qkv_hi is single bf16 [B,T,3D] (what the qkv GEMM's bf16 split epilogue writes) and
+ * o_hi single bf16 [B,T,D], qkv_lo and o_lo NULL (else ANYLOC_ERR_ARG); one bf16 MMA per product, P rounded once to
+ * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED). */
 int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                      void* o_hi, void* o_lo, int out_dtype, int engine, void* stream);
 int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y, void* stream);
