@@ -1,19 +1,15 @@
-// Tensor-core flash attention, softmax(Q K^T / 8) V per head (head_dim 64), for both pair precisions:
-//   F16 = true : q, k, v are fp16 pairs (hi,lo) of 8*x in the row-major qkv buffer [B*T, 3D] (q | k | v thirds, written by
-//                the qkv GEMM's split epilogue); mma.sync m16n8k16 (fp16 in, fp32 accumulate); output fp16 pairs of 8*o.
-//   F16 = false: q, k, v are tf32 pairs (two fp32 arrays); mma.sync m16n8k8 (tf32); output tf32 pairs.
+// Tensor-core flash attention, softmax(Q K^T / 8) V per head (head_dim 64), tf32 pairs: q, k, v are tf32 pairs (two
+// fp32 arrays) in the row-major qkv buffer [B*T, 3D] (q | k | v thirds); mma.sync m16n8k8 (tf32); output tf32 pairs.
 // Both GEMMs use the 3-term split  X.Y ~= X_hi.Y_hi + X_lo.Y_hi + X_hi.Y_lo  (fp32-equivalent accuracy), and each key
 // block's P.V partial is accumulated from zero and then added to the running output with round-to-nearest fp32 adds.
+// The two 2-byte formats (fp16 pairs, single bf16) run the wgmma kernel of attention_wg.cu instead: wgmma's transposed
+// B operand, which P.V needs for V, exists for 16-bit types only.
 //
 // CTA = (64-query tile, head, image), 4 warps; warp w owns query rows [16w, 16w+16) of the tile and keeps its Q
 // fragments (hi, lo) in registers for the whole key loop.  K and V blocks of 64 keys (hi and lo) are streamed through a
 // double-buffered shared-memory ring with cp.async (rows beyond T are zero-filled and masked to -inf in S).  The S
-// accumulator fragments are exactly the A-operand fragments of P.V (fp16: two n8 tiles = one k16 step; tf32: the key
-// order inside a k8 step is permuted to match and V is read in the same order), so P never leaves registers.
-//
-// BF16 = true (with F16, the 2-byte layout): the single bf16 format -- q, k, v are one bf16 array bf16_rn(x) (no lo, no
-// scale); one mma.sync m16n8k16.bf16 per k-step for Q K^T and for P V in place of three, P rounded once to bf16 (no
-// P_SCALE: bf16 has fp32's exponent range), output one bf16 array bf16_rn(o).  Softmax and accumulators stay fp32.
+// accumulator fragments are exactly the A-operand fragments of P.V (the key order inside a k8 step is permuted to match
+// and V is read in the same order), so P never leaves registers.
 #include <stdlib.h>
 #include "common.cuh"
 
@@ -22,11 +18,11 @@ namespace atc {
 
 constexpr int BQ = 64, BKV = 64, HD = 64, WARPS = 4, THREADS = WARPS * 32;
 
-template <bool F16, bool BF16 = false> struct Cfg {
-  using T = typename std::conditional<BF16, __nv_bfloat16, typename std::conditional<F16, __half, float>::type>::type;
-  static constexpr int PITCH = F16 ? HD + 8 : HD + 4;                 // elements per smem row (bank-conflict-free reads)
+struct Cfg {
+  using T = float;
+  static constexpr int PITCH = HD + 4;                                 // elements per smem row (bank-conflict-free reads)
   static constexpr int MAT = BKV * PITCH;                              // elements of one [64 keys x 64 dims] tile
-  static constexpr int NMAT = BF16 ? 2 : 4;                            // K_hi, K_lo, V_hi, V_lo (bf16: K, V)
+  static constexpr int NMAT = 4;                                       // K_hi, K_lo, V_hi, V_lo
   static constexpr int STAGE = NMAT * MAT;
   static constexpr int SMEM_BYTES = 2 * STAGE * (int)sizeof(T);
   static constexpr int CHUNKS_PER_ROW = HD * (int)sizeof(T) / 16;     // 16-byte cp.async pieces per 64-dim row
@@ -39,20 +35,6 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void mma_f16(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_bf16(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ void mma_tf32(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
@@ -60,29 +42,18 @@ __device__ __forceinline__ void mma_tf32(float* d, const uint32_t* a, uint32_t b
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t* r) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t* r) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
 __device__ __forceinline__ float ex2(float x) {
   float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 }
 __device__ __forceinline__ uint32_t f2u(float x) { return __float_as_uint(x); }
-template <typename E>     // two adjacent 2-byte elements (fp16 or bf16) as one word
-__device__ __forceinline__ uint32_t ld_h2(const E* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
 // One CTA's work.  Uniform (VARLEN = false): blockIdx = (query tile, head, image) over B images of T tokens.  VARLEN:
 // blockIdx = (tile of the packed grid, head); the table gives the image's first row, its length T and its first tile.
-template <bool F16, bool VARLEN, bool BF16 = false>
+template <bool VARLEN>
 __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T,
                                               int D, void* __restrict__ o_hi_, void* __restrict__ o_lo_,
                                               const VarlenAttnTable* tab) {
-  static_assert(!BF16 || F16, "bf16 uses the 2-byte (k16) layout");
-  using C = Cfg<F16, BF16>;
+  using C = Cfg;
   using E = typename C::T;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   E* smem = reinterpret_cast<E*>(smem_raw);
@@ -102,12 +73,9 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     qt -= tab->tile0[lo]; T = tab->len[lo]; img0 = (size_t)tab->row0[lo];
   }
   const int nblk = (T + BKV - 1) / BKV;
-  constexpr bool SCALED = F16 && !BF16;      // fp16 pairs carry s = kActScale and P is scaled into fp16's range
-  const float P_SCALE = SCALED ? 1024.0f : 1.0f;
-  // S holds (s q).(s k), s = kActScale for fp16 pairs: fold 1/s^2 into the 1/sqrt(64) * log2(e) scale
-  const float kScale = 0.125f * 1.4426950408889634f * (SCALED ? 1.0f / (kActScale * kActScale) : 1.0f);
+  const float kScale = 0.125f * 1.4426950408889634f;     // 1/sqrt(64) * log2(e)
 
-  // ---- K/V block loader: 64 rows x {K_hi, K_lo, V_hi, V_lo} (bf16: {K, V}), 16-byte pieces, rows >= T zero-filled
+  // ---- K/V block loader: 64 rows x {K_hi, K_lo, V_hi, V_lo}, 16-byte pieces, rows >= T zero-filled
   auto load_block = [&](int j, int buf) {
     E* st = smem + buf * C::STAGE;
     constexpr int PIECES = C::NMAT * BKV * C::CHUNKS_PER_ROW;
@@ -115,8 +83,8 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
       const int mat = p / (BKV * C::CHUNKS_PER_ROW), r = (p / C::CHUNKS_PER_ROW) % BKV, c = p % C::CHUNKS_PER_ROW;
       const int key = j * BKV + r;
       const bool valid = key < T;
-      const E* src = (!BF16 && (mat & 1)) ? qkv_lo : qkv_hi;
-      const bool is_k = BF16 ? mat == 0 : mat < 2;
+      const E* src = (mat & 1) ? qkv_lo : qkv_hi;
+      const bool is_k = mat < 2;
       const size_t col = (size_t)(is_k ? D : 2 * D) + (size_t)h * HD + (size_t)c * (16 / sizeof(E));
       const E* gp = src + (valid ? (img0 + key) * ld + col : 0);
       cp_async16((uint32_t)__cvta_generic_to_shared(st + mat * C::MAT + r * C::PITCH + c * (16 / sizeof(E))), gp, valid);
@@ -127,27 +95,18 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
 
   // ---- Q fragments of this warp's 16 rows (hi, lo), zero beyond T
   const int q0 = qt * BQ + warp * 16 + g, q1 = q0 + 8;
-  constexpr int QK_STEPS = F16 ? HD / 16 : HD / 8;
+  constexpr int QK_STEPS = HD / 8;
   uint32_t qa_hi[QK_STEPS][4], qa_lo[QK_STEPS][4];
   {
     const size_t r0 = (img0 + q0) * ld + (size_t)h * HD, r1 = (img0 + q1) * ld + (size_t)h * HD;
     const bool v0 = q0 < T, v1 = q1 < T;
 #pragma unroll
     for (int ks = 0; ks < QK_STEPS; ++ks) {
-      if constexpr (F16) {
-        const int c0 = ks * 16 + 2 * t4, c1 = c0 + 8;
-        qa_hi[ks][0] = v0 ? ld_h2(qkv_hi + r0 + c0) : 0u; qa_hi[ks][1] = v1 ? ld_h2(qkv_hi + r1 + c0) : 0u;
-        qa_hi[ks][2] = v0 ? ld_h2(qkv_hi + r0 + c1) : 0u; qa_hi[ks][3] = v1 ? ld_h2(qkv_hi + r1 + c1) : 0u;
-        if (BF16) continue;
-        qa_lo[ks][0] = v0 ? ld_h2(qkv_lo + r0 + c0) : 0u; qa_lo[ks][1] = v1 ? ld_h2(qkv_lo + r1 + c0) : 0u;
-        qa_lo[ks][2] = v0 ? ld_h2(qkv_lo + r0 + c1) : 0u; qa_lo[ks][3] = v1 ? ld_h2(qkv_lo + r1 + c1) : 0u;
-      } else {
-        const int c0 = ks * 8 + t4, c1 = c0 + 4;
-        qa_hi[ks][0] = v0 ? f2u(qkv_hi[r0 + c0]) : 0u; qa_hi[ks][1] = v1 ? f2u(qkv_hi[r1 + c0]) : 0u;
-        qa_hi[ks][2] = v0 ? f2u(qkv_hi[r0 + c1]) : 0u; qa_hi[ks][3] = v1 ? f2u(qkv_hi[r1 + c1]) : 0u;
-        qa_lo[ks][0] = v0 ? f2u(qkv_lo[r0 + c0]) : 0u; qa_lo[ks][1] = v1 ? f2u(qkv_lo[r1 + c0]) : 0u;
-        qa_lo[ks][2] = v0 ? f2u(qkv_lo[r0 + c1]) : 0u; qa_lo[ks][3] = v1 ? f2u(qkv_lo[r1 + c1]) : 0u;
-      }
+      const int c0 = ks * 8 + t4, c1 = c0 + 4;
+      qa_hi[ks][0] = v0 ? f2u(qkv_hi[r0 + c0]) : 0u; qa_hi[ks][1] = v1 ? f2u(qkv_hi[r1 + c0]) : 0u;
+      qa_hi[ks][2] = v0 ? f2u(qkv_hi[r0 + c1]) : 0u; qa_hi[ks][3] = v1 ? f2u(qkv_hi[r1 + c1]) : 0u;
+      qa_lo[ks][0] = v0 ? f2u(qkv_lo[r0 + c0]) : 0u; qa_lo[ks][1] = v1 ? f2u(qkv_lo[r1 + c0]) : 0u;
+      qa_lo[ks][2] = v0 ? f2u(qkv_lo[r0 + c1]) : 0u; qa_lo[ks][3] = v1 ? f2u(qkv_lo[r1 + c1]) : 0u;
     }
   }
 
@@ -163,7 +122,7 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     __syncthreads();
     const E* sK_hi = smem + buf * C::STAGE;
     const E* sK_lo = sK_hi + C::MAT;
-    const E* sV_hi = sK_hi + (BF16 ? 1 : 2) * C::MAT;
+    const E* sV_hi = sK_hi + 2 * C::MAT;
     const E* sV_lo = sK_hi + 3 * C::MAT;
 
     // ---- S = Q K^T (3-term) for this warp's 16 rows x 64 keys
@@ -172,38 +131,15 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
-      if constexpr (F16) {
-        // ldmatrix: keys [8nt, +8) x dims {0, 8, 16, 24} + 32c -> B fragments of k-steps 2c and 2c+1
-        const int key = nt * 8 + (lane & 7), dim = 8 * (lane >> 3);
+      const float* kh = sK_hi + (nt * 8 + g) * C::PITCH;
+      const float* kl = sK_lo + (nt * 8 + g) * C::PITCH;
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t bh[4], bl[4];
-          ldsm_x4((uint32_t)__cvta_generic_to_shared(sK_hi + key * C::PITCH + 32 * c + dim), bh);
-          if constexpr (BF16) {
-#pragma unroll
-            for (int u = 0; u < 2; ++u) mma_bf16(s[nt], qa_hi[2 * c + u], bh[2 * u], bh[2 * u + 1]);
-            continue;
-          }
-          ldsm_x4((uint32_t)__cvta_generic_to_shared(sK_lo + key * C::PITCH + 32 * c + dim), bl);
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int ks = 2 * c + u;
-            mma_f16(s[nt], qa_hi[ks], bh[2 * u], bh[2 * u + 1]);
-            mma_f16(s[nt], qa_lo[ks], bh[2 * u], bh[2 * u + 1]);
-            mma_f16(s[nt], qa_hi[ks], bl[2 * u], bl[2 * u + 1]);
-          }
-        }
-      } else {
-        const float* kh = sK_hi + (nt * 8 + g) * C::PITCH;
-        const float* kl = sK_lo + (nt * 8 + g) * C::PITCH;
-#pragma unroll
-        for (int ks = 0; ks < QK_STEPS; ++ks) {
-          const uint32_t bh0 = f2u(kh[ks * 8 + t4]), bh1 = f2u(kh[ks * 8 + t4 + 4]);
-          const uint32_t bl0 = f2u(kl[ks * 8 + t4]), bl1 = f2u(kl[ks * 8 + t4 + 4]);
-          mma_tf32(s[nt], qa_hi[ks], bh0, bh1);
-          mma_tf32(s[nt], qa_lo[ks], bh0, bh1);
-          mma_tf32(s[nt], qa_hi[ks], bl0, bl1);
-        }
+      for (int ks = 0; ks < QK_STEPS; ++ks) {
+        const uint32_t bh0 = f2u(kh[ks * 8 + t4]), bh1 = f2u(kh[ks * 8 + t4 + 4]);
+        const uint32_t bl0 = f2u(kl[ks * 8 + t4]), bl1 = f2u(kl[ks * 8 + t4 + 4]);
+        mma_tf32(s[nt], qa_hi[ks], bh0, bh1);
+        mma_tf32(s[nt], qa_lo[ks], bh0, bh1);
+        mma_tf32(s[nt], qa_hi[ks], bl0, bl1);
       }
     }
 
@@ -237,65 +173,23 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
     float pv[8][4];
 #pragma unroll
     for (int nd = 0; nd < 8; ++nd) pv[nd][0] = pv[nd][1] = pv[nd][2] = pv[nd][3] = 0.f;
-    if constexpr (BF16) {
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {          // as the fp16 branch below, with P rounded once to bf16
-        uint32_t ph[4];
-        ph[0] = pack_bf16x2(s[2 * ks][0], s[2 * ks][1]);
-        ph[1] = pack_bf16x2(s[2 * ks][2], s[2 * ks][3]);
-        ph[2] = pack_bf16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
-        ph[3] = pack_bf16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
-        const int key = ks * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), dsel = 8 * (lane >> 4);
+    for (int ks = 0; ks < 8; ++ks) {          // 8 keys per step = S tile ks; A slot t4 <-> key 2 t4, slot t4+4 <-> 2 t4 + 1
+      uint32_t ph[4], pl[4];
+      float hh, ll;
+      split_tf32(s[ks][0], hh, ll); ph[0] = f2u(hh); pl[0] = f2u(ll);
+      split_tf32(s[ks][2], hh, ll); ph[1] = f2u(hh); pl[1] = f2u(ll);
+      split_tf32(s[ks][1], hh, ll); ph[2] = f2u(hh); pl[2] = f2u(ll);
+      split_tf32(s[ks][3], hh, ll); ph[3] = f2u(hh); pl[3] = f2u(ll);
+      const float* vh0 = sV_hi + (ks * 8 + 2 * t4) * C::PITCH;
+      const float* vl0 = sV_lo + (ks * 8 + 2 * t4) * C::PITCH;
 #pragma unroll
-        for (int nd = 0; nd < 8; nd += 2) {
-          uint32_t vh[4];
-          ldsm_x4_t((uint32_t)__cvta_generic_to_shared(sV_hi + key * C::PITCH + nd * 8 + dsel), vh);
-#pragma unroll
-          for (int u = 0; u < 2; ++u) mma_bf16(pv[nd + u], ph, vh[2 * u], vh[2 * u + 1]);
-        }
-      }
-    } else if constexpr (F16) {
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {          // 16 keys per step = S tiles 2ks, 2ks+1
-        uint32_t ph[4], pl[4];
-        split_f16x2(s[2 * ks][0] * P_SCALE, s[2 * ks][1] * P_SCALE, ph[0], pl[0]);
-        split_f16x2(s[2 * ks][2] * P_SCALE, s[2 * ks][3] * P_SCALE, ph[1], pl[1]);
-        split_f16x2(s[2 * ks + 1][0] * P_SCALE, s[2 * ks + 1][1] * P_SCALE, ph[2], pl[2]);
-        split_f16x2(s[2 * ks + 1][2] * P_SCALE, s[2 * ks + 1][3] * P_SCALE, ph[3], pl[3]);
-        // ldmatrix.trans: keys 16ks + {0..7, 8..15} x dims [8nd, +8) for nd, nd+1
-        const int key = ks * 16 + (lane & 7) + 8 * ((lane >> 3) & 1), dsel = 8 * (lane >> 4);
-#pragma unroll
-        for (int nd = 0; nd < 8; nd += 2) {
-          uint32_t vh[4], vl[4];
-          ldsm_x4_t((uint32_t)__cvta_generic_to_shared(sV_hi + key * C::PITCH + nd * 8 + dsel), vh);
-          ldsm_x4_t((uint32_t)__cvta_generic_to_shared(sV_lo + key * C::PITCH + nd * 8 + dsel), vl);
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            mma_f16(pv[nd + u], ph, vh[2 * u], vh[2 * u + 1]);
-            mma_f16(pv[nd + u], pl, vh[2 * u], vh[2 * u + 1]);
-            mma_f16(pv[nd + u], ph, vl[2 * u], vl[2 * u + 1]);
-          }
-        }
-      }
-    } else {
-#pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {          // 8 keys per step = S tile ks; A slot t4 <-> key 2 t4, slot t4+4 <-> 2 t4 + 1
-        uint32_t ph[4], pl[4];
-        float hh, ll;
-        split_tf32(s[ks][0], hh, ll); ph[0] = f2u(hh); pl[0] = f2u(ll);
-        split_tf32(s[ks][2], hh, ll); ph[1] = f2u(hh); pl[1] = f2u(ll);
-        split_tf32(s[ks][1], hh, ll); ph[2] = f2u(hh); pl[2] = f2u(ll);
-        split_tf32(s[ks][3], hh, ll); ph[3] = f2u(hh); pl[3] = f2u(ll);
-        const float* vh0 = sV_hi + (ks * 8 + 2 * t4) * C::PITCH;
-        const float* vl0 = sV_lo + (ks * 8 + 2 * t4) * C::PITCH;
-#pragma unroll
-        for (int nd = 0; nd < 8; ++nd) {
-          const uint32_t bh0 = f2u(vh0[nd * 8 + g]), bh1 = f2u(vh0[C::PITCH + nd * 8 + g]);
-          const uint32_t bl0 = f2u(vl0[nd * 8 + g]), bl1 = f2u(vl0[C::PITCH + nd * 8 + g]);
-          mma_tf32(pv[nd], ph, bh0, bh1);
-          mma_tf32(pv[nd], pl, bh0, bh1);
-          mma_tf32(pv[nd], ph, bl0, bl1);
-        }
+      for (int nd = 0; nd < 8; ++nd) {
+        const uint32_t bh0 = f2u(vh0[nd * 8 + g]), bh1 = f2u(vh0[C::PITCH + nd * 8 + g]);
+        const uint32_t bl0 = f2u(vl0[nd * 8 + g]), bl1 = f2u(vl0[C::PITCH + nd * 8 + g]);
+        mma_tf32(pv[nd], ph, bh0, bh1);
+        mma_tf32(pv[nd], pl, bh0, bh1);
+        mma_tf32(pv[nd], ph, bl0, bl1);
       }
     }
 #pragma unroll
@@ -308,8 +202,7 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
 
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  // o holds (P_SCALE p) . (s v) and fp16 outputs are pairs of s*o, so only P_SCALE and the softmax denominator remain
-  const float inv0 = 1.0f / (l0 * P_SCALE), inv1 = 1.0f / (l1 * P_SCALE);
+  const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int q = half ? q1 : q0;
@@ -319,39 +212,28 @@ __device__ __forceinline__ void attention_cta(const void* __restrict__ qkv_hi_, 
 #pragma unroll
     for (int nd = 0; nd < 8; ++nd) {
       const float a = o[nd][2 * half] * inv, c = o[nd][2 * half + 1] * inv;
-      if constexpr (BF16) {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(o_hi_) + off + nd * 8) = pack_bf16x2(a, c);
-      } else if constexpr (F16) {
-        uint32_t hh, ll;
-        split_f16x2(a, c, hh, ll);
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_hi_) + off + nd * 8) = hh;
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_lo_) + off + nd * 8) = ll;
-      } else {
-        float2 hh, ll;
-        split_tf32(a, hh.x, ll.x); split_tf32(c, hh.y, ll.y);
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(o_hi_) + off + nd * 8) = hh;
-        *reinterpret_cast<float2*>(reinterpret_cast<float*>(o_lo_) + off + nd * 8) = ll;
-      }
+      float2 hh, ll;
+      split_tf32(a, hh.x, ll.x); split_tf32(c, hh.y, ll.y);
+      *reinterpret_cast<float2*>(reinterpret_cast<float*>(o_hi_) + off + nd * 8) = hh;
+      *reinterpret_cast<float2*>(reinterpret_cast<float*>(o_lo_) + off + nd * 8) = ll;
     }
   }
 }
 
 // B images of T tokens each: grid (query tiles, heads, B)
-template <bool F16, bool BF16 = false>
 __global__ void __launch_bounds__(THREADS)
 attention_tc_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_, int T, int D,
                     void* __restrict__ o_hi_, void* __restrict__ o_lo_) {
-  attention_cta<F16, false, BF16>(qkv_hi_, qkv_lo_, T, D, o_hi_, o_lo_, nullptr);
+  attention_cta<false>(qkv_hi_, qkv_lo_, T, D, o_hi_, o_lo_, nullptr);
 }
 
 // Images of different lengths packed row after row: grid (sum of every image's query tiles, heads).  The host lists
 // the images longest first, so the CTAs with the longest key loops start first and short images fill the tail.
-template <bool F16, bool BF16 = false>
 __global__ void __launch_bounds__(THREADS)
 attention_tc_varlen_kernel(const void* __restrict__ qkv_hi_, const void* __restrict__ qkv_lo_,
                            const __grid_constant__ VarlenAttnTable tab, int D, void* __restrict__ o_hi_,
                            void* __restrict__ o_lo_) {
-  attention_cta<F16, true, BF16>(qkv_hi_, qkv_lo_, 0, D, o_hi_, o_lo_, &tab);
+  attention_cta<true>(qkv_hi_, qkv_lo_, 0, D, o_hi_, o_lo_, &tab);
 }
 
 // fp32 (hi,lo) qkv pairs -> fp16 pairs of 8*x (same [M,3D] layout).  Standalone building-block path only.
@@ -366,50 +248,45 @@ qkv_to_f16_kernel(const float* __restrict__ qkv_hi, const float* __restrict__ qk
 
 }  // namespace atc
 
+int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
+                        bool bf16, cudaStream_t st);
+int attention_wg_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int D, int heads,
+                               void* o_hi, void* o_lo, bool bf16, cudaStream_t st);
+
 // qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, or single bf16 with qkv_lo
-// unused); o_{hi,lo}: [B*T, D] of the same kind (bf16: o_hi only).
+// unused); o_{hi,lo}: [B*T, D] of the same kind (bf16: o_hi only).  The 2-byte formats run attention_wg.cu's kernel.
 int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
                         int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(B <= 65535 && heads <= 65535, "attention_tc: grid too large (B=%d heads=%d)", B, heads);
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16)
+    return attention_wg_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, fmt == ANYLOC_PAIR_BF16, st);
   static unsigned long long attr_seen = 0;
-  if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<true>::SMEM_BYTES));
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<false>::SMEM_BYTES));
-  }
+  if (first_use_on_this_device(&attr_seen))
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           Cfg::SMEM_BYTES));
   const dim3 grid(cdiv(T, BQ), heads, B);
-  if (fmt == ANYLOC_PAIR_BF16)     // 36 KB of shared memory: under the default limit, no attribute needed
-    attention_tc_kernel<true, true><<<grid, THREADS, Cfg<true, true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
-  else if (fmt == ANYLOC_PAIR_F16) attention_tc_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
-  else attention_tc_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
+  attention_tc_kernel<<<grid, THREADS, Cfg::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, T, D, o_hi, o_lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
 
-// the same over images of different lengths packed into one [sum T_i, 3D] qkv buffer; tab.tile0 runs to n_tiles
+// the same over images of different lengths packed into one [sum T_i, 3D] qkv buffer; tab.tile0 (64-query tiles) runs
+// to n_tiles
 int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int n_tiles, int D,
                                int heads, void* o_hi, void* o_lo, int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(heads <= 65535, "attention_tc: grid too large (heads=%d)", heads);
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16)
+    return attention_wg_varlen_launch(qkv_hi, qkv_lo, tab, D, heads, o_hi, o_lo, fmt == ANYLOC_PAIR_BF16, st);
   static unsigned long long attr_seen = 0;
-  if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel<true>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<true>::SMEM_BYTES));
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel<false>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<false>::SMEM_BYTES));
-  }
+  if (first_use_on_this_device(&attr_seen))
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           Cfg::SMEM_BYTES));
   const dim3 grid(n_tiles, heads);
-  if (fmt == ANYLOC_PAIR_BF16)
-    attention_tc_varlen_kernel<true, true><<<grid, THREADS, Cfg<true, true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D,
-                                                                                             o_hi, o_lo);
-  else if (fmt == ANYLOC_PAIR_F16)
-    attention_tc_varlen_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
-  else
-    attention_tc_varlen_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
+  attention_tc_varlen_kernel<<<grid, THREADS, Cfg::SMEM_BYTES, st>>>(qkv_hi, qkv_lo, tab, D, o_hi, o_lo);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

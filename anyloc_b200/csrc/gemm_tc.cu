@@ -513,6 +513,20 @@ int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box
   return ANYLOC_OK;
 }
 
+int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, bool bf16) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { set_error("tensor map: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)imgs};
+  cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)rows * cols * 2};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)ptr, dims,
+                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("tensor map: cuTensorMapEncodeTiled failed (%d) imgs=%d rows=%d cols=%d", (int)r, imgs, rows, cols); return ANYLOC_ERR_CUDA; }
+  return ANYLOC_OK;
+}
+
 // output map of the staged epilogue: [rows, cols] of esz-byte elements, row pitch ld, boxes of 64 rows x box_cols
 // swizzled as stg_off places them.  TMA clips the boxes at rows and cols, so the ld padding is never written.
 static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int esz, int box_cols,

@@ -142,9 +142,79 @@ __device__ __forceinline__ void wgmma_m64n128_bf16(float* d, uint64_t adesc, uin
       : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+
+// setmaxnreg: hand registers from the producer warpgroup to the consumers (every warp of a warpgroup executes it)
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// wgmma matrix descriptor of an MN-major 16-bit operand with 128B swizzle: rows of 128 B (64 elements of N) are
+// consecutive k, 8-row atoms 1024 B apart.  With N = 64 the operand is one atom wide, so only the stride between the
+// 8-row groups along K matters (SBO); LBO (the stride between atoms along N) is given the same value.  A k16 step
+// advances the start address by 2 atoms (2048 B).
+__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(1024 >> 4) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+
+#define ANYLOC_WG_D32                                                                                               \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),       \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),        \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),       \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define ANYLOC_WG_D32_STR                                                                                           \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31}"
+
+// D[64 x 64] (+)= A[64 x 16] . B[64 x 16]^T, A and B K-major in shared memory (SS form); 16-bit operands, fp16 or bf16.
+// Accumulator layout as wgmma_m64n128's: d[4j + {0,1}] = row 16w + l/4, columns 8j + 2(l%4) + {0,1}; d[4j + {2,3}] =
+// row 16w + l/4 + 8.
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : ANYLOC_WG_D32 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " ANYLOC_WG_D32_STR ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : ANYLOC_WG_D32 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+
+// D[64 x 64] (+)= A[64 x 16] . B[16 x 64], A from registers (RS form), B MN-major in shared memory (transposed B, 16-bit
+// types only).  The A fragment of warp w is mma.sync m16n8k16's for rows [16w, 16w + 16): a[0] = (row l/4, k 2(l%4) +
+// {0,1}), a[1] = row + 8, a[2] = k + 8, a[3] = both -- which is the accumulator layout of a 16-bit wgmma, two n8
+// column groups per k16 step.
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR
+                 ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+                 : ANYLOC_WG_D32 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " ANYLOC_WG_D32_STR
+                 ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+                 : ANYLOC_WG_D32 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+}
+#undef ANYLOC_WG_D32
+#undef ANYLOC_WG_D32_STR
+
 // host: 2-D tiled tensor map over a row-major [rows, K] matrix (row pitch ld elements), box = 128 bytes of K x box_rows
 // rows, 128B swizzle (defined in gemm_tc.cu); elements are fp32, fp16 (f16) or bf16 (f16 and bf16)
 int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16 = false);
+// host: 3-D tiled tensor map over imgs row-major [rows, cols] matrices of 2-byte elements (fp16, or bf16) laid end to
+// end, box = 64 columns (128 B) x box_rows rows x 1 matrix, 128B swizzle; boxes past `rows` of a matrix read zeros
+int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, bool bf16);
 
 }  // namespace tc
 }  // namespace anyloc
