@@ -132,6 +132,9 @@ _SIGS = {
                                          C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "anyloc_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                    C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "anyloc_attention_varlen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                          C.c_void_p]),
     "anyloc_l2_normalize_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
 }
 EXPORTS = sorted(_SIGS)

@@ -260,6 +260,60 @@ extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B,
                             (cudaStream_t)stream);
 }
 
+// The attention table of n packed images (image i: rows [row0[i], row0[i] + len[i])): entries longest first, so the
+// longest key loops start first, ties in input order; each entry's first 64-query tile.  Returns the tile count.  The
+// ViT's list calls and anyloc_attention_varlen both build their tables here.
+static int varlen_attn_table(int n, const int* row0, const int* len, VarlenAttnTable* t) {
+  int order[kVarlenMaxB];
+  for (int i = 0; i < n; ++i) order[i] = i;
+  std::stable_sort(order, order + n, [&](int a, int b) { return len[a] > len[b]; });
+  int tiles = 0;
+  t->n = n;
+  for (int k = 0; k < n; ++k) {
+    const int i = order[k];
+    t->tile0[k] = tiles; t->row0[k] = row0[i]; t->len[k] = len[i];
+    tiles += cdiv(len[i], 64);
+  }
+  return tiles;
+}
+
+extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const int32_t* row0,
+                                       const int32_t* len, int D, int heads, void* o_hi, void* o_lo, int fmt,
+                                       void* stream) {
+  ANYLOC_REQUIRE(fmt == ANYLOC_PAIR_TF32 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16,
+                 "attention_varlen: bad fmt %d", fmt);
+  const bool bf16 = fmt == ANYLOC_PAIR_BF16;
+  ANYLOC_REQUIRE(qkv_hi && o_hi && row0 && len, "attention_varlen: null pointer");
+  if (bf16)
+    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention_varlen: the single-bf16 format has no lo arrays (qkv_lo, o_lo must be "
+                   "NULL)");
+  else
+    ANYLOC_REQUIRE(qkv_lo && o_lo, "attention_varlen: the pair formats need qkv_lo and o_lo");
+  ANYLOC_REQUIRE(n >= 1 && n <= ANYLOC_VIT_VARLEN_MAX_B, "attention_varlen: n=%d out of range [1,%d]", n,
+                 ANYLOC_VIT_VARLEN_MAX_B);
+  ANYLOC_REQUIRE(heads >= 1 && D == heads * 64, "attention_varlen: head_dim must be 64 (D=%d heads=%d)", D, heads);
+  int by_row[ANYLOC_VIT_VARLEN_MAX_B];
+  for (int i = 0; i < n; ++i) {
+    ANYLOC_REQUIRE(len[i] >= 1 && row0[i] >= 0 && (int64_t)row0[i] + len[i] <= INT32_MAX,
+                   "attention_varlen: image %d has row0=%d len=%d", i, row0[i], len[i]);
+    by_row[i] = i;
+  }
+  std::sort(by_row, by_row + n, [&](int a, int b) { return row0[a] < row0[b]; });
+  for (int k = 1; k < n; ++k)
+    ANYLOC_REQUIRE(row0[by_row[k - 1]] + len[by_row[k - 1]] <= row0[by_row[k]],
+                   "attention_varlen: images %d and %d overlap", by_row[k - 1], by_row[k]);
+  if ((reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0 || (reinterpret_cast<uintptr_t>(qkv_lo) & 15) != 0) {
+    set_error("attention_varlen: qkv_hi and qkv_lo must be 16-byte aligned (TMA and cp.async)");
+    return ANYLOC_ERR_UNSUPPORTED;
+  }
+  VarlenAttnTable tab;
+  const int tiles = varlen_attn_table(n, row0, len, &tab);
+  double flops = 0.0;
+  for (int i = 0; i < n; ++i) flops += 4.0 * (double)len[i] * len[i] * D;
+  ProfScope ps(PC_ATTENTION, (cudaStream_t)stream, flops);
+  return attention_tc_varlen_launch(qkv_hi, qkv_lo, tab, tiles, D, heads, o_hi, o_lo, fmt, (cudaStream_t)stream);
+}
+
 extern "C" int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y,
                                         void* stream) {
   ANYLOC_REQUIRE(x && y && D % 4 == 0 && ld_in % 4 == 0, "l2_normalize_rows: bad args");
@@ -587,10 +641,10 @@ bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* 
   }
   if (!hw) { set_error("vit_extract_varlen: null hw"); return false; }
   const int P = cfg->patch, R = cfg->num_registers;
-  int64_t tok = 0, patches = 0, tiles = 0;
+  int64_t tok = 0, patches = 0;
   double flops = 0.0;
-  p->img.n = B; p->img.nreg = R; p->attn.n = B;
-  int order[ANYLOC_VIT_VARLEN_MAX_B];
+  p->img.n = B; p->img.nreg = R;
+  int len[ANYLOC_VIT_VARLEN_MAX_B];
   for (int i = 0; i < B; ++i) {
     const int H = hw[2 * i], W = hw[2 * i + 1];
     if (H <= 0 || W <= 0 || H % P || W % P) {
@@ -608,16 +662,10 @@ bool varlen_plan(const AnylocVitCfg* cfg, int B, const int32_t* hw, VarlenPlan* 
     p->img.ptr[i] = nullptr;
     tok += n + 1 + R; patches += n;
     flops += 4.0 * (double)(n + 1 + R) * (n + 1 + R) * cfg->embed_dim;
-    order[i] = i;
+    len[i] = (int)n + 1 + R;
   }
-  // attention entries longest first (the longest key loops start first); ties keep the input order
-  std::stable_sort(order, order + B, [&](int a, int b) { return p->img.gh[a] * p->img.gw[a] > p->img.gh[b] * p->img.gw[b]; });
-  for (int k = 0; k < B; ++k) {
-    const int i = order[k], T = p->img.gh[i] * p->img.gw[i] + 1 + R;
-    p->attn.tile0[k] = (int)tiles; p->attn.row0[k] = p->img.tok0[i]; p->attn.len[k] = T;
-    tiles += cdiv(T, 64);
-  }
-  p->n_patch = (int)patches; p->n_tok = (int)tok; p->n_tiles = (int)tiles; p->attn_flops = flops;
+  p->n_tiles = varlen_attn_table(B, p->img.tok0, len, &p->attn);
+  p->n_patch = (int)patches; p->n_tok = (int)tok; p->attn_flops = flops;
   return true;
 }
 }  // namespace

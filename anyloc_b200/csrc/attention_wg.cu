@@ -19,7 +19,8 @@
 //                   at or beyond T does nothing (the empty barriers count only the active consumers), so a tile count
 //                   per image that is odd costs no padded MMAs.
 // Keys at or beyond T read zeros (past the image in the 3-D map) or the next image's rows (the packed map) and are
-// masked to p = 0 exactly; query rows at or beyond T are computed and never written.
+// masked to p = 0 exactly; in the packed kernel the consumers also zero those V rows of the last key block before P.V,
+// so a non-finite row of another image cannot reach O_j.  Query rows at or beyond T are computed and never written.
 #include <stdlib.h>
 #include "tc_common.cuh"
 
@@ -190,6 +191,22 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
     }
     // ---- O_j = P V (3-term), accumulated from zero, then o = alpha o + O_j (round-to-nearest)
     const uint32_t sb = stage_addr(j);
+    if constexpr (VARLEN) {
+      // The last key block of a packed image ends inside the stage, and its V rows from T on are the next image's
+      // (or whatever lies between images): p = 0 there, but 0 * Inf or NaN would still reach O_j.  The active
+      // consumers zero those rows (a 128 B swizzled row stays within its own 128 B), as the padded kernel reads them.
+      const int rem = T - j * BKV;                      // keys of this block below T
+      if (rem < BKV) {
+        const int pieces = (BKV - rem) * 8;             // 16 B pieces per V tile
+        for (int i = cw * 128 + t; i < C::NT * pieces; i += active * 128) {
+          const int a = i / pieces, r = rem + (i % pieces) / 8;
+          asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(sb + C::V_OFF + a * TILE_BYTES + r * 128 +
+                                                                          (i % 8) * 16), "r"(0u) : "memory");
+        }
+        fence_proxy_async_smem();                       // before P.V's wgmma reads them
+        named_bar_sync<1>(active * 128);
+      }
+    }
     const uint64_t dv_hi = make_desc_mn(sb + C::V_OFF), dv_lo = make_desc_mn(sb + C::V_OFF + TILE_BYTES);
     float pv[32];
 #pragma unroll

@@ -352,6 +352,18 @@ int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M
  * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED). */
 int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                      void* o_hi, void* o_lo, int out_dtype, int engine, void* stream);
+/* The packed attention of the _varlen ViT calls, on n images of different lengths in one [rows, 3D] qkv buffer:
+ * row0, len HOST int32 [n]; image i's q|k|v rows are [row0[i], row0[i] + len[i]) and its output rows the same rows of
+ * o [rows, D].  Images may lie in any order with gaps between them; rows outside every image are neither used nor
+ * written.  The operands are in the format fmt of the ViT's qkv epilogue, not converted: ANYLOC_PAIR_TF32 (tf32
+ * pairs), ANYLOC_PAIR_F16 (fp16 pairs of 8*x, output pairs of 8*o) or ANYLOC_PAIR_BF16 (qkv_lo, o_lo NULL).  The same
+ * table (longest first) and launcher as the ViT; an image's rows are bit-identical to anyloc_attention on that image
+ * alone (fp16 pairs: fed the tf32 pair of x) whatever the other images and the rows around it hold.
+ * ANYLOC_ERR_ARG for a null pointer, n outside [1, ANYLOC_VIT_VARLEN_MAX_B], len[i] < 1, row0[i] < 0, overlapping
+ * images, D != 64 heads, lo arrays with bf16 or without a pair format, or a bad fmt; ANYLOC_ERR_UNSUPPORTED for a qkv
+ * that is not 16-byte aligned.  Both return before anything is launched. */
+int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const int32_t* row0, const int32_t* len,
+                            int D, int heads, void* o_hi, void* o_lo, int fmt, void* stream);
 int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y, void* stream);
 
 /* ------------------------------------------------------------------ sibling aggregators

@@ -7,7 +7,8 @@ GEMM (wgmma, one bf16 MMA per k-step, fp32 accumulation in round-to-nearest chun
 one round-to-nearest bf16 output rounding, 2^-8 |v| (8 significant bits), to the propagated bound.  BIAS and LS_RESID
 write fp32 as before.
 
-Attention (mma.sync m16n8k16.bf16, softmax in fp32): with q, k, v the bf16 operands and P = softmax(q k^T / 8),
+Attention (wgmma m64n64k16 with bf16 operands, fp32 accumulators, softmax in fp32): with q, k, v the bf16 operands
+and P = softmax(q k^T / 8),
     |o - o64| <= (2^-8 + 2 d_s + 2 (T + 64) u + 2^-20) (P |V|) + 2^-8 |o64|
 where 2^-8 (P|V|) is P rounded once to bf16 (p <= 1 after the max subtraction; the denominator sums the unrounded p),
 d_s = 2 u 64 |q_i| max_j |k_j| / 8 bounds the fp32 error of a logit (2 u: the tensor core's accumulation need not round
@@ -16,8 +17,8 @@ the key blocks, 2^-20 the ex2.approx error, and 2^-8 |o64| the bf16 output round
 
 Also: the bf16 conversion and LayerNorm bit for bit against torch's round-to-nearest cast, NaN canaries around every
 output, the staged-epilogue observable, and the refusals (non-NULL lo arrays, the SIMT engine), which leave the
-canaries untouched.  The packed (varlen) attention kernel has no building-block entry point; its rows are checked bit
-for bit against the padded kernel through the ViT in tests/test_vit_bf16_gpu.py."""
+canaries untouched.  attn_bound() is the attention bound; tests/test_attention_varlen_gpu.py applies it to the packed
+(varlen) attention, image by image."""
 import ctypes as C
 
 import pytest
@@ -269,6 +270,15 @@ def attn_reference(X):
     return o, pv, qk
 
 
+def attn_bound(X):
+    """fp64 softmax(q k^T / 8) v of the bf16 operands X [B, T, 3, H, 64] (as doubles) and the bound of the module
+    docstring, both [B, H, T, 64]"""
+    ref, pv, qk = attn_reference(X)
+    T = X.shape[1]
+    d_s = 2 * 64 * U * qk / 8
+    return ref, (R16 + 2 * d_s + 2 * (T + 64) * U + 2.0 ** -20) * pv + R16 * ref.abs()
+
+
 @pytest.mark.parametrize("T", [1, 2, 63, 64, 127, 1025])
 def test_attention_against_fp64(L, T):
     B, D = 2, 384
@@ -280,9 +290,7 @@ def test_attention_against_fp64(L, T):
         torch.cuda.synchronize()
         assert untouched_outside(o, B * T, D, D) == 0, (T, logit, equal)
         got = window(o, B * T, D, D).double().reshape(B, T, D // 64, 64).transpose(1, 2)
-        ref, pv, qk = attn_reference(X)
-        d_s = 2 * 64 * U * qk / 8
-        bound = (R16 + 2 * d_s + 2 * (T + 64) * U + 2.0 ** -20) * pv + R16 * ref.abs()
+        ref, bound = attn_bound(X)
         excess = (got - ref).abs() - bound
         assert float(excess.max()) <= 0, (T, logit, equal, float(excess.max()))
         if equal:         # equal keys: P is uniform (exp(0) = 1 exactly), o is the mean of v in every row

@@ -2,6 +2,7 @@
 Every image's features must be BIT-IDENTICAL to a call on that image alone with the same GEMM engine, so the feature
 adds no tolerance; the oracle check ties the packed path to the reference model as well."""
 import ctypes as C
+import random
 
 import pytest
 import torch
@@ -84,6 +85,35 @@ def test_list_vs_oracle(u, precision):
             ref = ao.extract_features(model, x[None].cpu(), 3, facet)[0]
             err = rel_inf(o.cpu(), ref)
             assert err < TOL, (facet, tuple(x.shape), err)
+
+
+def _small_sizes(n, seed):
+    """n images with sides of 14..126 px (1..9 patches), among them equal patch counts in different shapes"""
+    rng = random.Random(seed)
+    sides = [14 * k for k in range(1, 10)]
+    sizes = [(28, 56), (56, 28), (14, 112), (112, 14), (42, 84), (84, 42), (14, 126), (126, 14), (14, 14), (126, 126)]
+    sizes += [(rng.choice(sides), rng.choice(sides)) for _ in range(n - len(sizes))]
+    rng.shuffle(sizes)
+    return sizes
+
+
+@pytest.mark.parametrize("precision", ["f16x3", "tf32x3", "bf16"])
+def test_full_tables_bit_identical_to_per_image_calls(u, precision):
+    """ViT-S with 2 blocks: 128 small images fill one call's table (ANYLOC_VIT_VARLEN_MAX_B entries), 300 run as three
+    calls (128, 128, 44) into one output; every image's rows equal its lone call's"""
+    from anyloc_b200 import _lib
+    assert _lib.VIT_VARLEN_MAX_B == 128
+    sd = dr.perturb(dr.build("dinov2_vits14", seed=0, depth_override=2), seed=1).state_dict()
+    ext = u.DinoV2ExtractFeatures("dinov2_vits14", 1, "value", device="cuda", weights=sd, gemm_engine="tc3",
+                                  precision=precision)
+    for n in (128, 300):
+        imgs = _imgs(_small_sizes(n, seed=n), seed=n)
+        for facet in ("value", "token"):
+            ext.facet = facet
+            out = ext(imgs)
+            assert len(out) == n
+            for i, x in enumerate(imgs):
+                assert torch.equal(out[i], ext(x[None])[0]), (precision, n, facet, i, tuple(x.shape))
 
 
 def test_list_is_one_forward_pass(u):
