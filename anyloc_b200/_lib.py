@@ -17,7 +17,7 @@ FACET = {"query": 0, "key": 1, "value": 2, "token": 3}
 FFN = {"mlp": 0, "swiglufused": 1}
 EPI = {"bias": 0, "bias_split": 1, "gelu_split": 2, "swiglu_split": 3, "ls_resid": 4}
 ENGINE = {"auto": 0, "simt": 1, "tc3": 2}
-PAIR = {"tf32": 0, "f16": 1, "bf16": 2}     # bf16: single bf16 (ANYLOC_PAIR_BF16), not a pair
+PAIR = {"tf32": 0, "f16": 1, "bf16": 2, "fp8": 3}     # bf16 / fp8: single bf16 / e4m3 (ANYLOC_PAIR_BF16 / _FP8)
 ACT_SCALE = 8.0     # kActScale in csrc/common.cuh
 VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_extract_varlen call
 ERR = {"arg": -1, "cuda": -2, "workspace": -3, "unsupported": -4}
@@ -130,6 +130,9 @@ _SIGS = {
     "anyloc_split_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_layernorm_split": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float,
                                          C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "anyloc_fp8_scale": (C.c_float, [C.c_float]),
+    "anyloc_quantize_fp8_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "anyloc_quantize_fp8_tensor": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_float), C.c_void_p]),
     "anyloc_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                    C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "anyloc_attention_varlen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int32),

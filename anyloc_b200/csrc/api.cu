@@ -58,6 +58,7 @@ int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int,
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                        int ldb, int M, int N, int K, const EpiParams& ep, bool f16);
 int gemm_tc_bf16_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
+int gemm_tc_fp8_launch(const void*, const float*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
 // vit_ops.cu / attention.cu
 int launch_split(const float*, float*, float*, size_t, cudaStream_t);
 int launch_split_f16(const float*, void*, void*, size_t, float, cudaStream_t);
@@ -65,6 +66,8 @@ int launch_split_bf16(const float*, void*, size_t, cudaStream_t);
 int launch_im2col(const float*, int, int, int, int, int, void*, void*, int, cudaStream_t);
 int launch_assemble(const float*, const float*, const float*, const float*, int, int, int, int, float*, cudaStream_t);
 int launch_layernorm(const float*, const float*, const float*, int, int, float, void*, void*, int, cudaStream_t);
+int launch_quantize_fp8_rows(const void*, int, int, void*, float*, cudaStream_t);
+int launch_quantize_fp8_tensor(const float*, size_t, void*, float*, cudaStream_t);
 int launch_facet_out(const float*, int, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_l2norm(const float*, int64_t, int, int64_t, float*, cudaStream_t);
 int attention_launch(const float*, const float*, int, int, int, int, void*, void*, bool, cudaStream_t);
@@ -94,6 +97,17 @@ static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void
     }
     ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
     return gemm_tc_bf16_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
+  }
+  if (fmt == ANYLOC_PAIR_FP8) {     // a_lo: A's fp32 row scales
+    if (engine == ANYLOC_GEMM_SIMT || !a_lo || b_lo || (reinterpret_cast<uintptr_t>(a_lo) & 3) || K % 16 ||
+        lda % 16 || ldb % 16 || !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, true)) {
+      set_error("gemm: the single-e4m3 format runs on the tensor-core engine only, with 16-byte aligned operands, "
+                "K, lda and ldb multiples of 16, A's row scales and no B lo operand (M=%d N=%d K=%d lda=%d ldb=%d "
+                "engine=%d)", M, N, K, lda, ldb, engine);
+      return ANYLOC_ERR_UNSUPPORTED;
+    }
+    ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
+    return gemm_tc_fp8_launch(a_hi, (const float*)a_lo, lda, b_hi, ldb, M, N, K, ep, st);
   }
   const bool f16 = fmt == ANYLOC_PAIR_F16;
   bool tc_ok = gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16);
@@ -153,13 +167,15 @@ extern "C" int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const
                               int ldo, int out_dtype, int engine, void* stream) {
   ANYLOC_REQUIRE(a_hi && b_hi && out, "gemm_nt: null pointer");
   ANYLOC_REQUIRE(M >= 0 && N >= 0 && K > 0, "gemm_nt: bad dims");
-  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_BF16, "gemm_nt: bad in_dtype %d", in_dtype);
+  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_FP8, "gemm_nt: bad in_dtype %d", in_dtype);
   ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_BF16, "gemm_nt: bad out_dtype %d", out_dtype);
   ANYLOC_REQUIRE(epilogue >= ANYLOC_EPI_BIAS && epilogue <= ANYLOC_EPI_LS_RESID, "gemm_nt: bad epilogue %d", epilogue);
-  const bool bf16 = in_dtype == ANYLOC_PAIR_BF16;
-  ANYLOC_REQUIRE(bf16 == (out_dtype == ANYLOC_PAIR_BF16), "gemm_nt: single bf16 is both the input and the output format "
-                 "(in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
-  if (bf16)
+  const bool bf16 = in_dtype == ANYLOC_PAIR_BF16, fp8 = in_dtype == ANYLOC_PAIR_FP8;
+  ANYLOC_REQUIRE((bf16 || fp8) == (out_dtype == ANYLOC_PAIR_BF16), "gemm_nt: single bf16 is the output format of the "
+                 "single bf16 and e4m3 inputs, and of no other (in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
+  if (fp8)
+    ANYLOC_REQUIRE(a_lo && !b_lo && !out_lo, "gemm_nt: e4m3 inputs take A's row scales in a_lo, no b_lo and no out_lo");
+  else if (bf16)
     ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-bf16 format has no lo arrays (a_lo, b_lo, out_lo "
                    "must be NULL)");
   else if (epilogue == ANYLOC_EPI_BIAS_SPLIT || epilogue == ANYLOC_EPI_GELU_SPLIT || epilogue == ANYLOC_EPI_SWIGLU_SPLIT)
@@ -216,8 +232,27 @@ extern "C" int anyloc_layernorm_split(const float* x, const float* w, const floa
   ANYLOC_REQUIRE(!(bf16 && y_lo), "layernorm: the single-bf16 output has no lo array (y_lo must be NULL)");
   if (M == 0) return ANYLOC_OK;
   return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo,
-                          bf16 ? ANYLOC_PAIR_BF16 : out_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32,
+                          bf16 ? ANYLOC_PAIR_BF16 : out_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_FP8
+                          : out_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32,
                           (cudaStream_t)stream);
+}
+
+extern "C" float anyloc_fp8_scale(float amax) { return pow2f(fp8_scale_exp(amax)); }
+
+extern "C" int anyloc_quantize_fp8_rows(const void* x, int M, int K, void* q, float* scales, void* stream) {
+  ANYLOC_REQUIRE(x && q && scales, "quantize_fp8_rows: null pointer");
+  ANYLOC_REQUIRE(M >= 0 && K > 0 && K % 8 == 0, "quantize_fp8_rows: M=%d K=%d (K a positive multiple of 8)", M, K);
+  ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 7) == 0 &&
+                 (reinterpret_cast<uintptr_t>(scales) & 3) == 0,
+                 "quantize_fp8_rows: x must be 16-byte, q 8-byte and scales 4-byte aligned");
+  if (M == 0) return ANYLOC_OK;
+  return launch_quantize_fp8_rows(x, M, K, q, scales, (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_quantize_fp8_tensor(const float* x, void* q, size_t n, float* scale_host, void* stream) {
+  ANYLOC_REQUIRE(x && q && scale_host, "quantize_fp8_tensor: null pointer");
+  ANYLOC_REQUIRE(n > 0, "quantize_fp8_tensor: empty tensor");
+  return launch_quantize_fp8_tensor(x, n, q, scale_host, (cudaStream_t)stream);
 }
 
 // qkv_f16: qkv_{hi,lo} already hold fp16 pairs of 8*x for all three thirds (the ViT's qkv epilogue wrote them).
@@ -328,17 +363,31 @@ namespace {
 struct VitBuffers {
   float *pa_hi, *pa_lo, *ptmp, *x, *y_hi, *y_lo, *qkv, *qkv_lo, *h_hi, *h_lo;
   float* qkv32;     // [M, 3D] fp32 rows of a tapped layer's qkv GEMM (null unless the tap list needs them)
+  void* h8;         // single e4m3: the FFN hidden layer quantised [M, H] and its row scales [M] (else null)
+  float* h8_s;
 };
 // n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  The single-bf16 format carves no
 // lo buffers and 2-byte GEMM inputs: pa [n_patch, Kp], y [M, D], qkv [M, 3D] (which also holds the fp32 [M, D] output
 // of a lone q/k/v tap), h [M, hidden] as bf16.
+// The single-e4m3 format carves the bf16 patch rows as above, e4m3 LayerNorm rows y [M, D] with their row scales
+// [M], the bf16 qkv [M, 3D], the bf16 hidden layer h [M, H] (which also holds the attention's bf16 output [M, D]) and
+// the e4m3 hidden layer h8 [M, H] with its row scales [M].
 size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
                  VitBuffers* out) {
   const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
-  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16;
+  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16, fp8 = c->pair_dtype == ANYLOC_PAIR_FP8;
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   VitBuffers b;
-  if (bf16) {
+  b.h8 = nullptr; b.h8_s = nullptr;
+  if (fp8) {
+    b.pa_hi = (float*)w.take<uint16_t>(n_patch * Kp); b.pa_lo = nullptr;
+    b.ptmp = w.take<float>(n_patch * D);
+    b.x = w.take<float>(M * D);
+    b.y_hi = (float*)w.take<uint8_t>(M * D); b.y_lo = w.take<float>(M);
+    b.qkv = (float*)w.take<uint16_t>(M * 3 * D); b.qkv_lo = nullptr;
+    b.h_hi = (float*)w.take<uint16_t>(M * c->ffn_hidden); b.h_lo = nullptr;
+    b.h8 = w.take<uint8_t>(M * c->ffn_hidden); b.h8_s = w.take<float>(M);
+  } else if (bf16) {
     b.pa_hi = (float*)w.take<uint16_t>(n_patch * Kp); b.pa_lo = nullptr;
     b.ptmp = w.take<float>(n_patch * D);
     b.x = w.take<float>(M * D);
@@ -356,7 +405,7 @@ size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, vo
   b.qkv32 = qkv32 ? w.take<float>(M * 3 * D) : nullptr;
   if (out) *out = b;
   if (ws && (!b.pa_hi || !b.ptmp || !b.x || !b.y_hi || !b.qkv || !b.h_hi || (qkv32 && !b.qkv32) ||
-             (!bf16 && (!b.pa_lo || !b.y_lo || !b.qkv_lo || !b.h_lo))))
+             (fp8 && (!b.y_lo || !b.h8 || !b.h8_s)) || (!bf16 && !fp8 && (!b.pa_lo || !b.y_lo || !b.qkv_lo || !b.h_lo))))
     return 0;
   return w.off;
 }
@@ -390,21 +439,26 @@ bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeight
   }
   return true;
 }
-// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16 weights with a
-// non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for single bf16 on the SIMT engine
+// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16 or e4m3 weights
+// with a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for those formats on the SIMT engine
 int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int engine) {
-  if (cfg->pair_dtype != ANYLOC_PAIR_BF16) return ANYLOC_OK;
+  const bool fp8 = cfg->pair_dtype == ANYLOC_PAIR_FP8;
+  if (cfg->pair_dtype != ANYLOC_PAIR_BF16 && !fp8) return ANYLOC_OK;
   bool lo = w->patch_w_lo != nullptr;
   for (int l = 0; l < cfg->depth && w->blocks; ++l) {
     const AnylocVitBlock& b = w->blocks[l];
     lo = lo || b.qkv_w_lo || b.proj_w_lo || b.in_w_lo || b.out_w_lo;
   }
   if (lo) {
-    set_error("%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
+    set_error(fp8 ? "%s: pair_dtype ANYLOC_PAIR_FP8 takes e4m3 block weights and bf16 patch weights; every *_w_lo must "
+                    "be NULL"
+                  : "%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
     return ANYLOC_ERR_ARG;
   }
   if (engine == ANYLOC_GEMM_SIMT) {
-    set_error("%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)", fn);
+    set_error(fp8 ? "%s: the single-e4m3 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)"
+                  : "%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)",
+              fn);
     return ANYLOC_ERR_UNSUPPORTED;
   }
   return ANYLOC_OK;
@@ -469,7 +523,8 @@ static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const Vit
   const int D = c->embed_dim, m = tp.mask[l];
   const QkvTapOuts o{{(m & 1) ? tp.out[l][0] : nullptr, (m & 2) ? tp.out[l][1] : nullptr,
                       (m & 4) ? tp.out[l][2] : nullptr}};
-  const int pair = pairs ? (c->pair_dtype == ANYLOC_PAIR_BF16 ? 3 : f16_attn ? 2 : 1) : 0;
+  const bool single = c->pair_dtype == ANYLOC_PAIR_BF16 || c->pair_dtype == ANYLOC_PAIR_FP8;   // bf16 attention
+  const int pair = pairs ? (single ? 3 : f16_attn ? 2 : 1) : 0;
   const double rows_out = (double)M - (tp.use_cls ? 0 : sq.B);
   const double bytes = 12.0 * M * D + (pair ? (pair == 3 ? 6.0 : pair == 2 ? 12.0 : 24.0) * M * D : 0.0) +
                        4.0 * rows_out * D * popcount3(m);
@@ -484,9 +539,9 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
                      int engine, cudaStream_t st, const TapPlan* tp = nullptr, int l = 0) {
   const int D = c->embed_dim, Hf = c->ffn_hidden;
   const int fmt = c->pair_dtype;
-  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16;
+  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16, fp8 = fmt == ANYLOC_PAIR_FP8;
   int rc;
-  const double ln_bytes = (bf16 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
+  const double ln_bytes = (fp8 ? 5.0 : bf16 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
   { ProfScope ps(PC_LAYERNORM, st, ln_bytes);
     if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
   // q, k and v leave the qkv GEMM row-major through the plain split epilogue; for the tensor-core attention in the
@@ -503,17 +558,25 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
     e_qkv.alpha = wb.qkv_alpha;
     if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, fmt, st))) return rc;
   }
+  // single e4m3: the qkv epilogue wrote single bf16 and the bf16 attention runs; its output (in h) is quantised to the
+  // proj GEMM's e4m3 rows
+  float* o_hi = fp8 ? bf.h_hi : bf.y_hi;
+  const int attn_fmt = fp8 ? ANYLOC_PAIR_BF16 : fmt;
   if (sq.tab) {
     ProfScope ps(PC_ATTENTION, st, sq.attn_flops);
-    if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, bf.y_hi, bf.y_lo,
-                                         fmt, st)))
+    if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, o_hi,
+                                         fp8 ? nullptr : bf.y_lo, attn_fmt, st)))
       return rc;
-  } else if (bf16) {
+  } else if (bf16 || fp8) {
     ProfScope ps(PC_ATTENTION, st, 4.0 * sq.B * (double)sq.T * sq.T * D);
-    if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, bf.y_hi, nullptr, fmt, st))) return rc;
+    if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, o_hi, nullptr, attn_fmt, st))) return rc;
   } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine,
                                       st, f16_attn))) {
     return rc;
+  }
+  if (fp8) {
+    ProfScope ps(PC_VIT_MISC, st, 3.0 * M * D);
+    if ((rc = launch_quantize_fp8_rows(bf.h_hi, M, D, bf.y_hi, bf.y_lo, st))) return rc;
   }
   EpiParams e_proj{ANYLOC_EPI_LS_RESID, wb.proj_b, wb.ls1, bf.x, bf.x, nullptr, D};
   e_proj.alpha = wb.proj_alpha;
@@ -525,9 +588,14 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   e_in.alpha = wb.in_alpha; e_in.out_f16 = f16;
   const int n_in = c->ffn_kind == ANYLOC_FFN_MLP ? Hf : 2 * Hf;
   if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.in_w_hi, wb.in_w_lo, D, M, n_in, D, e_in, engine, fmt, st))) return rc;
+  if (fp8) {
+    ProfScope ps(PC_VIT_MISC, st, 3.0 * M * Hf);
+    if ((rc = launch_quantize_fp8_rows(bf.h_hi, M, Hf, bf.h8, bf.h8_s, st))) return rc;
+  }
   EpiParams e_out{ANYLOC_EPI_LS_RESID, wb.out_b, wb.ls2, bf.x, bf.x, nullptr, D};
   e_out.alpha = wb.out_alpha;
-  return gemm_dispatch(bf.h_hi, bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf, e_out, engine, fmt, st);
+  return gemm_dispatch(fp8 ? bf.h8 : bf.h_hi, fp8 ? bf.h8_s : bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf,
+                       e_out, engine, fmt, st);
 }
 
 // Blocks 0..l_max over the M assembled token rows in bf.x, each run once, writing every tap of the plan:
@@ -539,7 +607,7 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
 static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
                      const TapPlan& tp, int gemm_engine, cudaStream_t st) {
   const int D = cfg->embed_dim, fmt = cfg->pair_dtype;
-  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16;
+  const size_t wsz = fmt == ANYLOC_PAIR_FP8 ? 1 : fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 ? 2 : 4;
   int rc;
   for (int l = 0; l <= tp.l_max; ++l) {
     const AnylocVitBlock& wb = w->blocks[l];
@@ -549,7 +617,7 @@ static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const V
       if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc;
       if (popcount3(qkv) == 1) {
         const int facet = qkv == 1 ? 0 : qkv == 2 ? 1 : 2;
-        const size_t woff = (size_t)facet * D * D * (f16 || bf16 ? 2 : 4);  // bytes: weights are __half/bf16 or float
+        const size_t woff = (size_t)facet * D * D * wsz;  // bytes: weights are e4m3, __half/bf16 or float
         EpiParams e_f{ANYLOC_EPI_BIAS, wb.qkv_b + (size_t)facet * D, nullptr, nullptr, bf.qkv, nullptr, D};
         e_f.alpha = wb.qkv_alpha;
         if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, (const char*)wb.qkv_w_hi + woff,
@@ -569,6 +637,12 @@ static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const V
     if (token && (rc = facet_out(sq, M, bf.x, D, D, tp, tp.out[l][ANYLOC_FACET_TOKEN], st))) return rc;
   }
   return ANYLOC_OK;
+}
+
+// the patch embedding's operand format: the single-e4m3 format keeps the bf16 im2col and GEMM (K = 3 14 14, a small
+// share of the FLOPs)
+static int patch_format(const AnylocVitCfg* cfg) {
+  return cfg->pair_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_BF16 : cfg->pair_dtype;
 }
 
 static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B,
@@ -594,7 +668,7 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
               vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  const int fmt = cfg->pair_dtype;
+  const int fmt = patch_format(cfg);
   if ((rc = launch_im2col(img, B, H, W, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};
   e_pe.alpha = w->patch_alpha;
@@ -714,7 +788,7 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
               vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  const int fmt = cfg->pair_dtype;
+  const int fmt = patch_format(cfg);
   for (int i = 0; i < B; ++i) p.img.ptr[i] = img[i];
   if ((rc = launch_im2col_varlen(p.img, p.n_patch, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};

@@ -104,6 +104,34 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return r;
 }
 
+// Single e4m3 format (ANYLOC_PAIR_FP8): a row (activations) or a matrix (weights) is one e4m3 array q = e4m3_rn(x / s)
+// with one power-of-two scale s, x ~ q s.  s = 2^k with k the smallest integer that puts max|x| / s <= 448 (e4m3's
+// largest finite value), at least -126 so that s and 1/s are normal fp32 numbers; s = 1 for an all-zero (or NaN) row.
+// Scaling by a power of two is exact, so e4m3_rn is the only rounding.  448 = 0.875 2^9: with max|x| = m 2^e, m in
+// [0.5, 1), k = e - 9, or e - 8 when m > 0.875.
+__host__ __device__ inline int fp8_scale_exp(float amax) {
+  if (!(amax > 0.f) || amax > 3.402823466e38f) return 0;
+  int e;
+  const float m = frexpf(amax, &e);
+  const int k = e - 9 + (m > 0.875f ? 1 : 0);
+  return k < -126 ? -126 : k;
+}
+// 2^k for k in [-126, 127]
+__host__ __device__ inline float pow2f(int k) {
+  union { uint32_t u; float f; } v;
+  v.u = (uint32_t)(127 + k) << 23;
+  return v.f;
+}
+// e4m3_rn of two values (satfinite: beyond +-448 clamps, NaN stays NaN) -> `a` in the low byte, `b` in the high byte
+__device__ __forceinline__ uint32_t pack_e4m3x2(float a, float b) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(b), "f"(a));
+  return r;
+}
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+  return pack_e4m3x2(a, b) | (pack_e4m3x2(c, d) << 16);
+}
+
 // Per-image geometry of a packed batch of differently sized images (anyloc_vit_extract_varlen).  The tables reach the
 // kernels by value as __grid_constant__ parameters: the launch copies them, so a call neither synchronises with the
 // host nor keeps a host pointer, and each stays under the classic 4 KB kernel-parameter limit.

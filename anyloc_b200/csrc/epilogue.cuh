@@ -15,6 +15,7 @@ struct EpiParams {
   float alpha = 1.0f;   // accumulator scale (1/(s_A*s_B) for fp16-pair inputs, else 1)
   int out_f16 = 0;      // SPLIT outputs as fp16 pairs of kActScale*v (out/out_lo then point to __half)
   const int* gate = nullptr;   // device flag (nullable): tensor-core GEMM kernels return immediately when *gate == 0 (conditional fallbacks without a host sync)
+  const float* row_scale = nullptr;   // [M] e4m3 A operand's row scales (single e4m3 GEMM only): acc of row m times row_scale[m]
 };
 
 // BF16 (the tensor-core GEMM's single-bf16 instantiation): the SPLIT outputs are one bf16 array, out = bf16_rn(v)

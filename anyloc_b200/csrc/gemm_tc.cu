@@ -17,6 +17,10 @@
 // A third operand format, single bf16 (ANYLOC_PAIR_BF16: one bf16 array of bf16_rn(x), no lo, no scale), runs one
 // wgmma.f32.bf16.bf16 per k-step through the same pipeline with hi-only stages and the staged epilogue
 // (gemm_tc_bf16_launch): a third of the 3-term MMAs, not fp32-equivalent.
+// A fourth, single e4m3 (ANYLOC_PAIR_FP8: A = e4m3 rows with one power-of-two scale per row, B = one e4m3 matrix),
+// runs one wgmma.f32.e4m3.e4m3 per 32-element k-step on UINT8 tensor maps (128-element k-blocks) with the bf16 pass's
+// stages and staged epilogue; the accumulator of row m is multiplied by A's row scale before the epilogue, and the
+// SPLIT outputs are one bf16 array (gemm_tc_fp8_launch).
 // Tiles are rastered in bands of BAND_N column blocks, n-fastest inside a band: the resident CTAs share a few A row
 // panels and one band of B that stays in L2 while the outputs stream through.
 #include <cuda.h>
@@ -63,6 +67,9 @@ constexpr int CHUNK_KB_F16 = 8;            // (24 / 96 wgmma k-steps per chunk)
 // operands' own bf16 rounding (2^-8 relative) is the only new error term.
 constexpr int CHUNK_KB_COARSE = 32;        // hi-only fp16 coarse pass (retrieval): <= 128 k-steps per chunk, the bound
                                            // topk.cu re-scores against
+// The e4m3 pass promotes the tensor core's partial sums into the round-to-nearest fp32 accumulator every k-block (128
+// elements, 4 wgmmas): the fp8 wgmma is not known to accumulate in full fp32 (DESIGN §4.9 states what was measured).
+constexpr int CHUNK_KB_FP8 = 1;
 
 __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int band_n, int& m_blk, int& n_blk) {
   const int per_band = num_m * band_n;
@@ -336,7 +343,9 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
 // ep.gate (nullable): the kernel returns at once when *gate == 0 (conditional fallbacks without a host sync).
 // staged != 0: the epilogue goes through shared memory and TMA stores (tm_out, tm_out_lo for the pair formats,
 // tm_resid for LS_RESID: (n_out, M) maps with 64-row boxes); 0: stored pair by pair from registers.
-template <bool F16, int LOM, bool BF16 = false>
+// FP8 = true (with F16 and LOM = 0): single e4m3 operands (128 elements per 128 B k-block, wgmma K=32), A's row
+//             scales in ep.row_scale; SPLIT outputs as BF16.
+template <bool F16, int LOM, bool BF16 = false, bool FP8 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
@@ -345,7 +354,9 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                 int M, int N, int K, int band_n, int chunk_kb, EpiParams ep) {
   constexpr bool LO = LOM != 0, has_a_lo = (LOM & 1) != 0, has_b_lo = (LOM & 2) != 0;
   static_assert(!BF16 || (F16 && LOM == 0), "bf16 is a single-operand 2-byte format");
-  using C = Cfg<LO, LO || BF16>;
+  static_assert(!FP8 || (F16 && LOM == 0 && !BF16), "e4m3 is a single-operand 1-byte format");
+  constexpr bool OUT_BF16 = BF16 || FP8;     // SPLIT outputs: one bf16 array
+  using C = Cfg<LO, LO || OUT_BF16>;
   if (ep.gate != nullptr && *reinterpret_cast<const volatile int*>(ep.gate) == 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -356,7 +367,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   const int wg = threadIdx.x >> 7;
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
-  constexpr int BKE = F16 ? 64 : 32;         // elements per k-block (128 bytes)
+  constexpr int BKE = FP8 ? 128 : F16 ? 64 : 32;         // elements per k-block (128 bytes)
   const int num_k = (K + BKE - 1) / BKE;
 
   if (threadIdx.x == 0) {
@@ -431,7 +442,8 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
           const uint64_t adv = (uint64_t)((k * 32) >> 4);      // +32 B per k-step inside the atom (both types)
-          if constexpr (BF16) wgmma_m64n128_bf16(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
+          if constexpr (FP8) wgmma_m64n128_e4m3(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
+          else if constexpr (BF16) wgmma_m64n128_bf16(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
           else wgmma_m64n128<F16>(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
           if (has_a_lo) wgmma_m64n128<F16>(acc, a_lo + adv, b_hi + adv, 1u);
           if (has_b_lo) wgmma_m64n128<F16>(acc, a_hi + adv, b_lo + adv, 1u);
@@ -451,12 +463,18 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
     }
     if (t == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
     if (mode < 0 || m0 >= M) continue;       // discard (ANYLOC_GEMM_DEBUG_SKIP_EPI) / no rows for this warpgroup
+    if constexpr (FP8) {                     // dequantise A: row m's sums times its power-of-two scale (exact)
+      const int r = m0 + warp * 16 + (lane >> 2);
+      const float s0 = r < M ? __ldg(ep.row_scale + r) : 0.f, s1 = r + 8 < M ? __ldg(ep.row_scale + r + 8) : 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) { sum[4 * j] *= s0; sum[4 * j + 1] *= s0; sum[4 * j + 2] *= s1; sum[4 * j + 3] *= s1; }
+    }
     if constexpr (!C::STAGED) {
       epilogue_regs_batched(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
       continue;
     }
     if (!staged) {
-      epilogue_pairs<BF16>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      epilogue_pairs<OUT_BF16>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
       continue;
     }
 #define ANYLOC_EPI_STAGED(KIND_, SWIGLU_, RESID_)                                                                   \
@@ -464,7 +482,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                                           n0, N, sum)
     if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(STG_F32, false, false);
     else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(STG_F32, false, true);
-    else if (BF16) {                         // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> single bf16
+    else if (OUT_BF16) {                     // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> single bf16
       if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_BF16, true, false);
       else ANYLOC_EPI_STAGED(STG_BF16, false, false);
     } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
@@ -497,15 +515,15 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16) {
+int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16, bool fp8) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
-  const int esz = f16 ? 2 : 4;
+  const int esz = fp8 ? 1 : f16 ? 2 : 4;
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esz), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+  const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                  : f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = enc(map, dt, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -588,45 +606,50 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
 // epilogue of this host thread's last launch (anyloc_gemm_tc_last_staged)
 static thread_local int g_last_staged = -1;
 
-template <bool F16, int LOM, bool BF16 = false>
+template <bool F16, int LOM, bool BF16 = false, bool FP8 = false>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                        int N, int K, const EpiParams& ep, int chunk, cudaStream_t st) {
   using namespace tc;
   constexpr bool LO = LOM != 0;
-  using CF = Cfg<LO, LO || BF16>;
+  using CF = Cfg<LO, LO || BF16 || FP8>;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
-  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16, BF16))) return rc;
-  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16, BF16))) return rc;
-  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16, BF16))) return rc;
-  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16, BF16))) return rc;
+  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16, BF16, FP8))) return rc;
+  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16, BF16, FP8))) return rc;
+  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16, BF16, FP8))) return rc;
+  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16, BF16, FP8))) return rc;
   CUtensorMap mo, mo_lo, mr;
   bool staged = false;
   memset(&mo, 0, sizeof(mo)); memset(&mo_lo, 0, sizeof(mo_lo)); memset(&mr, 0, sizeof(mr));
   // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
   // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
   // for more would make the SM switch its shared-memory configuration back and forth).
-  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, BF16))) return rc;
+  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, BF16 || FP8))) return rc;
   const int smem = staged ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES;
   g_last_staged = staged ? 1 : 0;
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            CF::STAGED ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES));
   }
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
-  gemm_tc3_kernel<F16, LOM, BF16><<<grid, THREADS, smem, st>>>(
+  gemm_tc3_kernel<F16, LOM, BF16, FP8><<<grid, THREADS, smem, st>>>(
       ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(BAND_N, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
 
-int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
-                   int N, int K, const EpiParams& ep_in, bool f16, cudaStream_t st) {
-  // ANYLOC_GEMM_CHUNK: k-blocks per round-to-nearest chunk of the 3-term GEMMs (A/B knob)
+// ANYLOC_GEMM_CHUNK: k-blocks per round-to-nearest chunk of the 3-term and e4m3 GEMMs (A/B knob; 0 = default)
+static int gemm_chunk_env() {
   static int chunk_env = -1;
   if (chunk_env < 0) { const char* e = getenv("ANYLOC_GEMM_CHUNK"); chunk_env = e ? atoi(e) : 0; }
+  return chunk_env;
+}
+
+int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
+                   int N, int K, const EpiParams& ep_in, bool f16, cudaStream_t st) {
+  const int chunk_env = gemm_chunk_env();
   // diagnostic only (tools/, never set by the product): bit m set -> GEMMs with epilogue mode m discard their result,
   // which exposes how much of a GEMM's time is its epilogue
   static int skip_epi = -1;
@@ -657,6 +680,17 @@ int gemm_tc_bf16_launch(const void* a, int lda, const void* b, int ldb, int M, i
                         cudaStream_t st) {
   static_assert(tc::Cfg<false, true>::SMEM_BYTES_STAGED <= 232448, "bf16 GEMM over H100's shared-memory opt-in");
   return launch_impl<true, 0, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
+}
+
+// single-e4m3 GEMM (ANYLOC_PAIR_FP8): e4m3 A rows with their scales a_scale [M], one e4m3 B, one wgmma per 32-element
+// k-step, the partial sums promoted every CHUNK_KB_FP8 k-blocks, staged epilogue; SPLIT outputs are one bf16 array
+int gemm_tc_fp8_launch(const void* a, const float* a_scale, int lda, const void* b, int ldb, int M, int N, int K,
+                       const EpiParams& ep_in, cudaStream_t st) {
+  EpiParams ep = ep_in;
+  ep.row_scale = a_scale;
+  const int chunk_env = gemm_chunk_env();
+  return launch_impl<true, 0, false, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep,
+                                           chunk_env > 0 ? chunk_env : tc::CHUNK_KB_FP8, st);
 }
 
 }  // namespace anyloc

@@ -4,6 +4,8 @@
 // that feeds the tensor-core GEMMs, the facet slice + F.normalize epilogue of
 // DinoV2ExtractFeatures.__call__ (utilities.py:270-283), and the qkv tap that keeps the q/k/v facets of a layer the
 // forward continues through.
+#include <string.h>
+#include <algorithm>
 #include "common.cuh"
 
 namespace anyloc {
@@ -44,6 +46,9 @@ template <> struct PairOut<ANYLOC_PAIR_F16> {
 template <> struct PairOut<ANYLOC_PAIR_BF16> {
   typedef __nv_bfloat16 T;
   static __device__ __forceinline__ void put(__nv_bfloat16* hi, __nv_bfloat16*, size_t i, float v) { hi[i] = __float2bfloat16_rn(v); }
+};
+template <> struct PairOut<ANYLOC_PAIR_FP8> {     // LayerNorm only: e4m3 rows, y_lo holds the fp32 row scales
+  typedef uint8_t T;
 };
 
 // patch pi of image b of img [B,3,H,W] -> patch row `row` of (hi,lo), column order (c, ky, kx) like conv
@@ -118,8 +123,8 @@ __global__ void assemble_tokens_varlen_kernel(const float* __restrict__ patch, c
                row - tab.tok0[i], x);
 }
 
-// LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo), or single bf16 (statistics in fp32 either
-// way). One warp per row.
+// LayerNorm over the last dim (biased variance, eps inside sqrt) -> (hi,lo), single bf16, or single e4m3 with the row's
+// scale in y_lo (statistics in fp32 every way; the e4m3 row's amax is reduced with them). One warp per row.
 template <int MAXV, int FMT>   // float4 per lane
 __global__ void __launch_bounds__(256)
 layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
@@ -150,6 +155,29 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
   const float rstd = rsqrtf(warp_sum(q) / (float)D + eps);
   const float4* w4 = reinterpret_cast<const float4*>(w);
   const float4* b4 = reinterpret_cast<const float4*>(b);
+  if constexpr (FMT == ANYLOC_PAIR_FP8) {
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      int d = lane + i * 32;
+      if (d < D4) {
+        float4 ww = __ldg(w4 + d), bb = __ldg(b4 + d);
+        v[i].x = (v[i].x - mean) * rstd * ww.x + bb.x; v[i].y = (v[i].y - mean) * rstd * ww.y + bb.y;
+        v[i].z = (v[i].z - mean) * rstd * ww.z + bb.z; v[i].w = (v[i].w - mean) * rstd * ww.w + bb.w;
+        amax = fmaxf(fmaxf(amax, fmaxf(fabsf(v[i].x), fabsf(v[i].y))), fmaxf(fabsf(v[i].z), fabsf(v[i].w)));
+      }
+    }
+    const int k = fp8_scale_exp(warp_max(amax));
+    const float inv = pow2f(-k);
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      int d = lane + i * 32;
+      if (d < D4)
+        reinterpret_cast<uint32_t*>(y_hi + (size_t)row * D)[d] =
+            pack_e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
+    }
+    if (lane == 0) reinterpret_cast<float*>(y_lo)[row] = pow2f(k);
+  } else {
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     int d = lane + i * 32;
@@ -173,6 +201,57 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
       }
     }
   }
+  }
+}
+
+// bf16 rows [M, K] -> e4m3 rows and their scales (single e4m3 format, see fp8_scale_exp): the GEMM inputs that
+// another GEMM or the attention wrote as bf16.  One warp per row, 8 elements per lane and step; the second pass
+// re-reads the row from L1/L2.
+__global__ void __launch_bounds__(256)
+quantize_fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, int M, int K, uint8_t* __restrict__ q,
+                         float* __restrict__ scale) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= M) return;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * K);
+  const int K8 = K >> 3;
+  auto lo = [](uint32_t u) { return __uint_as_float(u << 16); };
+  auto hi = [](uint32_t u) { return __uint_as_float(u & 0xffff0000u); };
+  float amax = 0.f;
+  for (int i = lane; i < K8; i += 32) {
+    const uint4 u = xr[i];
+    amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(lo(u.x)), fabsf(hi(u.x))), fmaxf(fabsf(lo(u.y)), fabsf(hi(u.y)))),
+                             fmaxf(fmaxf(fabsf(lo(u.z)), fabsf(hi(u.z))), fmaxf(fabsf(lo(u.w)), fabsf(hi(u.w))))));
+  }
+  const int k = fp8_scale_exp(warp_max(amax));
+  const float inv = pow2f(-k);
+  uint2* qr = reinterpret_cast<uint2*>(q + (size_t)row * K);
+  for (int i = lane; i < K8; i += 32) {
+    const uint4 u = xr[i];
+    qr[i] = make_uint2(pack_e4m3x4(lo(u.x) * inv, hi(u.x) * inv, lo(u.y) * inv, hi(u.y) * inv),
+                       pack_e4m3x4(lo(u.z) * inv, hi(u.z) * inv, lo(u.w) * inv, hi(u.w) * inv));
+  }
+  if (lane == 0) scale[row] = pow2f(k);
+}
+
+// max |x| of a tensor into *amax (an fp32 bit pattern: non-negative floats order as integers; NaN above every other)
+__global__ void amax_kernel(const float* __restrict__ x, size_t n, unsigned int* amax) {
+  float m = 0.f;
+  bool nan = false;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float a = fabsf(x[i]);
+    nan = nan || a != a;
+    m = fmaxf(m, a);
+  }
+  m = warp_max(m);
+  if (__any_sync(0xffffffffu, nan)) m = __uint_as_float(0x7fc00000u);
+  if ((threadIdx.x & 31) == 0) atomicMax(amax, __float_as_uint(m));
+}
+
+// q = e4m3_rn(x * inv) (inv = 1/s, a power of two)
+__global__ void quantize_fp8_kernel(const float* __restrict__ x, size_t n, float inv, uint8_t* __restrict__ q) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    q[i] = (uint8_t)pack_e4m3x2(x[i] * inv, 0.f);
 }
 
 // y[r,:] = x[r, 0:D] / max(|x[r]|,1e-12) (or plain copy), x rows strided by ld_in. One warp per row.
@@ -379,13 +458,46 @@ static void ln_launch(const float* x, const float* w, const float* b, int M, int
   else if (D <= 1024) layernorm_split_kernel<8, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
   else layernorm_split_kernel<16, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
 }
-// fmt: ANYLOC_PAIR_* of the output (bf16: y_lo unused)
+// fmt: ANYLOC_PAIR_* of the output (bf16: y_lo unused; fp8: y_lo = the fp32 row scales [M])
 int launch_layernorm(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi,
                      void* y_lo, int fmt, cudaStream_t st) {
   ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "layernorm: D=%d unsupported (multiple of 4, <= 2048)", D);
-  if (fmt == ANYLOC_PAIR_BF16) ln_launch<ANYLOC_PAIR_BF16>(x, w, b, M, D, eps, y_hi, nullptr, st);
+  if (fmt == ANYLOC_PAIR_FP8) ln_launch<ANYLOC_PAIR_FP8>(x, w, b, M, D, eps, y_hi, y_lo, st);
+  else if (fmt == ANYLOC_PAIR_BF16) ln_launch<ANYLOC_PAIR_BF16>(x, w, b, M, D, eps, y_hi, nullptr, st);
   else if (fmt == ANYLOC_PAIR_F16) ln_launch<ANYLOC_PAIR_F16>(x, w, b, M, D, eps, y_hi, y_lo, st);
   else ln_launch<ANYLOC_PAIR_TF32>(x, w, b, M, D, eps, y_hi, y_lo, st);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+// bf16 [M, K] -> e4m3 [M, K] and row scales [M]; K a multiple of 8, x and q 16- and 8-byte aligned
+int launch_quantize_fp8_rows(const void* x, int M, int K, void* q, float* scale, cudaStream_t st) {
+  quantize_fp8_rows_kernel<<<cdiv(M, 8), 256, 0, st>>>((const __nv_bfloat16*)x, M, K, (uint8_t*)q, scale);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+// fp32 [n] -> e4m3 [n] with one power-of-two scale *s_host (x ~ q s).  Synchronises the stream: the scale is decided
+// on the host from the tensor's amax (weight preparation, once per model).  A NaN or Inf returns ANYLOC_ERR_ARG.
+int launch_quantize_fp8_tensor(const float* x, size_t n, void* q, float* s_host, cudaStream_t st) {
+  unsigned int* d_amax = nullptr;
+  ANYLOC_CHECK_CUDA(cudaMallocAsync(&d_amax, sizeof(unsigned int), st));
+  unsigned int amax_bits = 0;
+  cudaError_t e = cudaMemsetAsync(d_amax, 0, sizeof(unsigned int), st);
+  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)device_sm_count() * 8);
+  if (e == cudaSuccess) {
+    amax_kernel<<<blocks, 256, 0, st>>>(x, n, d_amax);
+    count_launch();
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&amax_bits, d_amax, sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
+  cudaFreeAsync(d_amax, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  ANYLOC_CHECK_CUDA(e);
+  float amax;
+  memcpy(&amax, &amax_bits, sizeof(amax));
+  ANYLOC_REQUIRE(amax <= 3.402823466e38f, "quantize_fp8_tensor: the tensor holds a NaN or an Inf");
+  const int k = fp8_scale_exp(amax);
+  *s_host = pow2f(k);
+  quantize_fp8_kernel<<<blocks, 256, 0, st>>>(x, n, pow2f(-k), (uint8_t*)q);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

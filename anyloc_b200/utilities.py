@@ -277,17 +277,17 @@ class _HookHandle:
         pass
 
 
-PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16")
+PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16", "fp8")
 
 
 def resolve_precision(precision, gemm_engine="auto"):
     """The extractor's precision: the argument, else $ANYLOC_B200_PRECISION, else "auto".  ValueError on an unknown
-    name, and on "bf16" with gemm_engine="simt" (single bf16 runs on the tensor cores only)."""
+    name, and on "bf16" or "fp8" with gemm_engine="simt" (single bf16 and e4m3 run on the tensor cores only)."""
     precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
     if precision not in PRECISIONS:
-        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3' or 'bf16', got {precision!r}")
-    if precision == "bf16" and gemm_engine == "simt":
-        raise ValueError("precision='bf16' runs on the tensor cores only; use gemm_engine='auto' or 'tc3'")
+        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3', 'bf16' or 'fp8', got {precision!r}")
+    if precision in ("bf16", "fp8") and gemm_engine == "simt":
+        raise ValueError(f"precision={precision!r} runs on the tensor cores only; use gemm_engine='auto' or 'tc3'")
     return precision
 
 
@@ -304,7 +304,8 @@ class _GuardedExtractor:
         self._state_dict = sd if self._auto else None     # kept for the tf32x3 re-upload on an fp16-range overflow
         self.precision = "f16x3" if self._auto else precision
         self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=self._depth(),
-                                          pair={"f16x3": "f16", "tf32x3": "tf32", "bf16": "bf16"}[self.precision])
+                                          pair={"f16x3": "f16", "tf32x3": "tf32", "bf16": "bf16",
+                                                "fp8": "fp8"}[self.precision])
         self.gemm_engine = gemm_engine
         self.fh_handle = _HookHandle()
         self._hook_out = None
@@ -373,6 +374,12 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
     bf16 MMA per product instead of three; the residual stream, LayerNorm statistics, softmax,
     accumulators and outputs stay fp32.  Its outputs are those of the model run on bf16-rounded
     activations (about 1e-2 relative), not fp32 parity; it needs gemm_engine "auto" or "tc3".
+    "fp8" is faster still and also never chosen by "auto": the block GEMMs run one e4m3 MMA per
+    product on e4m3 weights (one power-of-two scale per matrix) and e4m3 activations (one
+    power-of-two scale per token row, so an image's rows never depend on the other images of a
+    call); the patch embedding and the attention run as in "bf16", and what stays fp32 in "bf16"
+    stays fp32.  Its error is that of the model run on e4m3-rounded GEMM inputs (about 2^-4
+    relative per operand); it needs gemm_engine "auto" or "tc3".
 
     `dino_model` may also name a backbone with register tokens, `dinov2_vit{s,b,l,g}14_reg`.  As
     in the reference, only row 0 (cls) is dropped, so its 4 register rows come first: an output
@@ -409,7 +416,7 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
         """img [B,3,H,W] -> [B, (1 +) R + N, D] (R = 4 register rows for the *_reg models, else 0); or a list/tuple of
         differently sized images [3,H_i,W_i] / [1,3,H_i,W_i], all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
         pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
-        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16", which always runs them)."""
+        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16" or "fp8", which always run them)."""
         return self._guarded(img)
 
     def __del__(self):

@@ -108,8 +108,10 @@ def interpolate_pos_embed(pos_embed, gh, gw, offset=INTERP_OFFSET, antialias=Fal
 class VitWeights:
     """Device-resident, kernel-ready weights of one DINOv2 backbone (blocks 0..depth-1).  A register model's outputs
     hold its num_registers register rows between the cls row and the patch rows, as the reference returns them.
-    pair: the operand format of every GEMM -- "tf32" / "f16" (fp32-equivalent (hi, lo) pairs) or "bf16" (one
-    round-to-nearest bf16 copy of each weight matrix, half the bytes of the pairs; a fast mode, not a parity mode)."""
+    pair: the operand format of every GEMM -- "tf32" / "f16" (fp32-equivalent (hi, lo) pairs), "bf16" (one
+    round-to-nearest bf16 copy of each weight matrix, half the bytes of the pairs; a fast mode, not a parity mode) or
+    "fp8" (one e4m3 copy of each block weight matrix with a power-of-two scale, a quarter of the pairs' bytes, and a bf16
+    patch embedding; a faster mode, not a parity mode)."""
 
     def __init__(self, name, state_dict, device, depth=None, pair="tf32"):
         if name not in ARCHS:
@@ -139,12 +141,20 @@ class VitWeights:
         def f32(t):
             return t.detach().to(device=dev, dtype=torch.float32).contiguous()
 
-        def split(t):
+        def split(t, patch=False):
             """-> (hi, lo, alpha): the kernel-ready pair of a weight matrix and the accumulator scale
-            1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs; bf16: (bf16_rn(w), None, 1.0))."""
+            1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs; bf16: (bf16_rn(w), None, 1.0); fp8 block
+            matrices: (e4m3_rn(w / s_w), None, s_w), the patch embedding as bf16)."""
             t = f32(t)
             with torch.cuda.device(dev):
-                if pair == "bf16":
+                if pair == "fp8" and not patch:
+                    q = torch.empty(t.shape, dtype=torch.float8_e4m3fn, device=dev)
+                    s_w = C.c_float()
+                    _lib.check(lib.anyloc_quantize_fp8_tensor(_lib.ptr(t), _lib.ptr(q), t.numel(), C.byref(s_w),
+                                                              _lib.stream_ptr()), "quantize_fp8_tensor")
+                    self._keep.append(q)
+                    return q, None, s_w.value
+                if pair in ("bf16", "fp8"):
                     hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
                     _lib.check(lib.anyloc_split_bf16(_lib.ptr(t), _lib.ptr(hi), t.numel(), _lib.stream_ptr()),
                                "split_bf16")
@@ -176,7 +186,7 @@ class VitWeights:
         sd = state_dict
         pw = f32(sd["patch_embed.proj.weight"]).reshape(self.dim, -1)
         pw = F.pad(pw, (0, self.patch_k - pw.shape[1]))
-        self.patch_w = split(pw)
+        self.patch_w = split(pw, patch=True)
         patch_alpha = self.patch_w[2]
         self.patch_b = keep(sd["patch_embed.proj.bias"])
         self.cls_token = keep(sd["cls_token"].reshape(-1))

@@ -62,6 +62,15 @@ extern "C" {
                                       (wgmma GEMM at every M, mma.sync attention): ANYLOC_GEMM_SIMT returns
                                       ANYLOC_ERR_UNSUPPORTED.  Accumulators, LayerNorm statistics, softmax, the
                                       residual stream and every feature output stay fp32. */
+#define ANYLOC_PAIR_FP8 3          /* NOT a pair and NOT fp32-equivalent: single e4m3 GEMM inputs with power-of-two scales.
+                                      A GEMM's A operand is e4m3 rows q = e4m3_rn(x / s_r) with one fp32 scale s_r per
+                                      row (the "lo" array carries the [M] scales); its B operand (a weight matrix) is
+                                      one e4m3 array e4m3_rn(w / s_w) with one scale s_w per matrix, which the GEMM's
+                                      alpha carries.  s = 2^k, k the smallest integer with max|x| / s <= 448, k >= -126;
+                                      s = 1 for an all-zero row (anyloc_fp8_scale).  One e4m3 MMA per product,
+                                      promoted into the fp32 accumulator every 128 elements of K; SPLIT outputs, the
+                                      attention and the patch embedding are single bf16 (ANYLOC_PAIR_BF16).
+                                      Tensor-core engine only. */
 /* GEMM engines */
 #define ANYLOC_GEMM_AUTO 0
 #define ANYLOC_GEMM_SIMT 1         /* fp32 FFMA (validation / odd shapes)               */
@@ -258,6 +267,18 @@ typedef struct {
  * Workspace: with A(x) = x rounded up to 256 bytes, n_p patch rows, M token rows and H = ffn_hidden,
  *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(2 M D) + A(6 M D) + A(2 M H) [+ A(12 M D) for the fp32 qkv rows of the
  *   tap calls, as below] + 4096 bytes. */
+/* Single e4m3 (pair_dtype = ANYLOC_PAIR_FP8), a faster mode than single bf16: the block weight matrices (qkv, proj,
+ * in, out) are e4m3 arrays e4m3_rn(w / s_w) (anyloc_quantize_fp8_tensor) with every *_w_lo NULL and *_alpha = s_w;
+ * patch_w_hi is single bf16 (anyloc_split_bf16) with patch_w_lo NULL and patch_alpha 1.  LayerNorm writes e4m3 rows
+ * and their scales in one pass; the qkv GEMM writes single bf16 for the bf16 attention (and the qkv tap); the
+ * attention output and the FFN hidden layer are quantised to e4m3 rows (anyloc_quantize_fp8_rows) before the proj and
+ * out GEMMs.  The patch embedding runs in single bf16.  The residual stream, LayerNorm statistics, softmax, every
+ * accumulator and every output stay fp32.  Per-row activation scales keep an image's rows independent of the rows
+ * around them, so single, list (_varlen) and tap calls are bit-identical as for single bf16.  A non-NULL *_w_lo returns
+ * ANYLOC_ERR_ARG and gemm_engine = ANYLOC_GEMM_SIMT ANYLOC_ERR_UNSUPPORTED, before anything is launched.
+ * Workspace: with A(x), n_p, M and H as above,
+ *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(M D) + A(4 M) + A(6 M D) + A(2 M H) + A(M H) + A(4 M) [+ A(12 M D) for
+ *   the fp32 qkv rows of the tap calls] + 4096 bytes. */
 /* padded patch-embed reduction length (3*14*14=588 -> multiple of 32) */
 int anyloc_vit_patch_k(int patch);
 size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W);
@@ -331,6 +352,9 @@ int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeigh
  * in_dtype = out_dtype = ANYLOC_PAIR_BF16: C = A . B^T of single bf16 operands (a_lo, b_lo, out_lo NULL, else
  * ANYLOC_ERR_ARG; bf16 in with another out_dtype, or the reverse, ANYLOC_ERR_ARG); the SPLIT epilogues write one bf16
  * array bf16_rn(v), BIAS / LS_RESID fp32 as usual.  Tensor-core engine only, at every M (SIMT: ANYLOC_ERR_UNSUPPORTED). */
+/* in_dtype = ANYLOC_PAIR_FP8, out_dtype = ANYLOC_PAIR_BF16: C = (s_r[m] alpha) (A . B^T) with A e4m3 [M, K] and its
+ * fp32 row scales s_r in a_lo, B e4m3 (b_lo NULL) and alpha = s_w; out_lo NULL; the SPLIT epilogues write one bf16
+ * array, BIAS / LS_RESID fp32.  K, lda and ldb multiples of 16.  Tensor-core engine only, at every M. */
 int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                    int ldb, int M, int N, int K, int in_dtype, float alpha, int epilogue, const float* bias,
                    const float* gamma, const float* resid, void* out, void* out_lo, int ldo, int out_dtype,
@@ -342,9 +366,19 @@ int anyloc_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stre
 int anyloc_split_f16(const float* x, void* hi, void* lo, size_t n, float scale, void* stream);
 /* y = bf16_rn(x), the single-bf16 weight format */
 int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream);
-/* out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG) */
+/* out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG);
+ * out_dtype = ANYLOC_PAIR_FP8: y_hi = e4m3 rows of LayerNorm(x) [M, D], y_lo = their fp32 scales [M] */
 int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D, float eps,
                            void* y_hi, void* y_lo, int out_dtype, void* stream);
+/* The scale rule of ANYLOC_PAIR_FP8: the power of two s for a row or matrix whose largest magnitude is amax (host). */
+float anyloc_fp8_scale(float amax);
+/* bf16 rows x [M, K] -> e4m3 rows q [M, K] and their fp32 scales [M] (ANYLOC_PAIR_FP8's A operand).  K a multiple of 8;
+ * x 16-byte, q 8-byte aligned. */
+int anyloc_quantize_fp8_rows(const void* x, int M, int K, void* q, float* scales, void* stream);
+/* fp32 x [n] -> e4m3 q [n] = e4m3_rn(x / s) with one scale s, returned in *scale_host (a weight matrix of
+ * ANYLOC_PAIR_FP8: its GEMM's alpha is s).  Synchronises the stream (the scale is chosen on the host); a NaN or Inf
+ * in x returns ANYLOC_ERR_ARG. */
+int anyloc_quantize_fp8_tensor(const float* x, void* q, size_t n, float* scale_host, void* stream);
 /* softmax(q k^T / 8) v per head (head_dim 64).  qkv (hi,lo) pairs [B,T,3D] ([q|k|v] thirds); qkv_lo may
  * be NULL for the SIMT engine (plain fp32 input).  -> o (hi,lo) [B,T,D].  engine: ANYLOC_GEMM_*.
  * out_dtype = ANYLOC_PAIR_BF16: qkv_hi is single bf16 [B,T,3D] (what the qkv GEMM's bf16 split epilogue writes) and
