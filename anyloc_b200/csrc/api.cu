@@ -230,6 +230,16 @@ extern "C" int anyloc_layernorm_split(const float* x, const float* w, const floa
   const bool bf16 = out_dtype == ANYLOC_PAIR_BF16;
   ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || bf16), "layernorm: null pointer");
   ANYLOC_REQUIRE(!(bf16 && y_lo), "layernorm: the single-bf16 output has no lo array (y_lo must be NULL)");
+  ANYLOC_REQUIRE(M >= 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm: M=%d D=%d (M >= 0, D a multiple of 4 in "
+                 "[4, 2048])", M, D);
+  // float4 loads of x, w and b; y_hi is stored 4 elements at a time (16, 8 or 4 bytes); fp8's y_lo holds fp32 scales
+  const uintptr_t lo_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
+  const uintptr_t hi_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : bf16 || out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
+  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(b)) &
+                  15) == 0 && (reinterpret_cast<uintptr_t>(y_hi) & hi_align) == 0 &&
+                 (reinterpret_cast<uintptr_t>(y_lo) & lo_align) == 0,
+                 "layernorm: x, w and b must be 16-byte aligned, y_hi and y_lo aligned to 4 of their elements (fp8: "
+                 "y_hi 4-byte, y_lo 4-byte)");
   if (M == 0) return ANYLOC_OK;
   return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo,
                           bf16 ? ANYLOC_PAIR_BF16 : out_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_FP8
@@ -352,6 +362,10 @@ extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, i
 extern "C" int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y,
                                         void* stream) {
   ANYLOC_REQUIRE(x && y && D % 4 == 0 && ld_in % 4 == 0, "l2_normalize_rows: bad args");
+  ANYLOC_REQUIRE(rows >= 0 && D > 0 && ld_in >= D, "l2_normalize_rows: rows=%lld D=%d ld_in=%lld (rows >= 0, D > 0, "
+                 "ld_in >= D)", (long long)rows, D, (long long)ld_in);
+  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0,
+                 "l2_normalize_rows: x and y must be 16-byte aligned (float4 access)");
   if (rows == 0) return ANYLOC_OK;
   return launch_l2norm(x, rows, D, ld_in, y, (cudaStream_t)stream);
 }

@@ -366,8 +366,13 @@ int anyloc_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stre
 int anyloc_split_f16(const float* x, void* hi, void* lo, size_t n, float scale, void* stream);
 /* y = bf16_rn(x), the single-bf16 weight format */
 int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream);
-/* out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG);
- * out_dtype = ANYLOC_PAIR_FP8: y_hi = e4m3 rows of LayerNorm(x) [M, D], y_lo = their fp32 scales [M] */
+/* y = LayerNorm(x) over rows of D (biased variance, eps inside the square root) with gain w and bias b, x [M, D] fp32.
+ * out_dtype = ANYLOC_PAIR_TF32 / _F16: y_hi, y_lo [M, D] the pair of y (fp16 pairs: of 8 y);
+ * out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG);
+ * out_dtype = ANYLOC_PAIR_FP8: y_hi = e4m3 rows of LayerNorm(x) [M, D], y_lo = their fp32 scales [M].
+ * D a multiple of 4 in [4, 2048].  ANYLOC_ERR_ARG before anything is launched for a null pointer, M < 0, D outside that
+ * range, x, w or b not 16-byte aligned, or y_hi / y_lo not aligned to 4 of their elements (fp8: y_hi and the scales
+ * 4-byte aligned).  M = 0 launches nothing. */
 int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D, float eps,
                            void* y_hi, void* y_lo, int out_dtype, void* stream);
 /* The scale rule of ANYLOC_PAIR_FP8: the power of two s for a row or matrix whose largest magnitude is amax (host). */
@@ -398,6 +403,9 @@ int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int
  * that is not 16-byte aligned.  Both return before anything is launched. */
 int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const int32_t* row0, const int32_t* len,
                             int D, int heads, void* o_hi, void* o_lo, int fmt, void* stream);
+/* y[r, :] = x[r, 0:D] / max(|x[r, 0:D]|, 1e-12) (F.normalize), x rows ld_in elements apart, y [rows, D] packed.
+ * ANYLOC_ERR_ARG before anything is launched for a null pointer, rows < 0, D <= 0, D or ld_in not a multiple of 4,
+ * ld_in < D, or x or y not 16-byte aligned.  rows = 0 launches nothing. */
 int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y, void* stream);
 
 /* ------------------------------------------------------------------ sibling aggregators
