@@ -58,6 +58,7 @@ int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int,
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                        int ldb, int M, int N, int K, const EpiParams& ep, bool f16);
 int gemm_tc_bf16_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
+int gemm_tc_f16x1_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
 int gemm_tc_fp8_launch(const void*, const float*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
 // vit_ops.cu / attention.cu
 int launch_split(const float*, float*, float*, size_t, cudaStream_t);
@@ -82,20 +83,22 @@ int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, i
 int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
                    cudaStream_t);
 
-// fmt: ANYLOC_PAIR_* of the operands.  Single bf16 is a tensor-core-only format: it runs the wgmma kernel at every M
-// (no SIMT route, so a row's result never depends on how many rows share the call) and refuses the SIMT engine.
+// fmt: ANYLOC_PAIR_* of the operands.  Single bf16 and single fp16 are tensor-core-only formats: they run the wgmma
+// kernel at every M (no SIMT route, so a row's result never depends on how many rows share the call) and refuse the
+// SIMT engine.
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                          int ldb, int M, int N, int K, const EpiParams& ep, int engine, int fmt, cudaStream_t st) {
   if (M == 0 || N == 0) return ANYLOC_OK;
-  if (fmt == ANYLOC_PAIR_BF16) {
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1) {
     if (engine == ANYLOC_GEMM_SIMT || a_lo || b_lo ||
         !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, true)) {
-      set_error("gemm: the single-bf16 format runs on the tensor-core engine only, with 16-byte aligned operands, "
+      set_error("gemm: the %s format runs on the tensor-core engine only, with 16-byte aligned operands, "
                 "K, lda and ldb multiples of 8 and no lo operands (M=%d N=%d K=%d lda=%d ldb=%d engine=%d)",
-                M, N, K, lda, ldb, engine);
+                fmt == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16", M, N, K, lda, ldb, engine);
       return ANYLOC_ERR_UNSUPPORTED;
     }
     ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
+    if (fmt == ANYLOC_PAIR_F16X1) return gemm_tc_f16x1_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
     return gemm_tc_bf16_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
   }
   if (fmt == ANYLOC_PAIR_FP8) {     // a_lo: A's fp32 row scales
@@ -167,16 +170,23 @@ extern "C" int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const
                               int ldo, int out_dtype, int engine, void* stream) {
   ANYLOC_REQUIRE(a_hi && b_hi && out, "gemm_nt: null pointer");
   ANYLOC_REQUIRE(M >= 0 && N >= 0 && K > 0, "gemm_nt: bad dims");
-  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_FP8, "gemm_nt: bad in_dtype %d", in_dtype);
-  ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_BF16, "gemm_nt: bad out_dtype %d", out_dtype);
+  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_F16X1, "gemm_nt: bad in_dtype %d", in_dtype);
+  ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_F16X1 && out_dtype != ANYLOC_PAIR_FP8,
+                 "gemm_nt: bad out_dtype %d", out_dtype);
   ANYLOC_REQUIRE(epilogue >= ANYLOC_EPI_BIAS && epilogue <= ANYLOC_EPI_LS_RESID, "gemm_nt: bad epilogue %d", epilogue);
   const bool bf16 = in_dtype == ANYLOC_PAIR_BF16, fp8 = in_dtype == ANYLOC_PAIR_FP8;
+  const bool h1 = in_dtype == ANYLOC_PAIR_F16X1;
   ANYLOC_REQUIRE((bf16 || fp8) == (out_dtype == ANYLOC_PAIR_BF16), "gemm_nt: single bf16 is the output format of the "
                  "single bf16 and e4m3 inputs, and of no other (in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
+  ANYLOC_REQUIRE(h1 == (out_dtype == ANYLOC_PAIR_F16X1), "gemm_nt: single fp16 is the output format of the single "
+                 "fp16 inputs, and of no other (in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
   if (fp8)
     ANYLOC_REQUIRE(a_lo && !b_lo && !out_lo, "gemm_nt: e4m3 inputs take A's row scales in a_lo, no b_lo and no out_lo");
   else if (bf16)
     ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-bf16 format has no lo arrays (a_lo, b_lo, out_lo "
+                   "must be NULL)");
+  else if (h1)
+    ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-fp16 format has no lo arrays (a_lo, b_lo, out_lo "
                    "must be NULL)");
   else if (epilogue == ANYLOC_EPI_BIAS_SPLIT || epilogue == ANYLOC_EPI_GELU_SPLIT || epilogue == ANYLOC_EPI_SWIGLU_SPLIT)
     ANYLOC_REQUIRE(out_lo, "gemm_nt: split epilogue needs out_lo");
@@ -227,14 +237,15 @@ extern "C" int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream
 
 extern "C" int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D,
                                       float eps, void* y_hi, void* y_lo, int out_dtype, void* stream) {
-  const bool bf16 = out_dtype == ANYLOC_PAIR_BF16;
-  ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || bf16), "layernorm: null pointer");
+  const bool bf16 = out_dtype == ANYLOC_PAIR_BF16, h1 = out_dtype == ANYLOC_PAIR_F16X1;
+  ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || bf16 || h1), "layernorm: null pointer");
   ANYLOC_REQUIRE(!(bf16 && y_lo), "layernorm: the single-bf16 output has no lo array (y_lo must be NULL)");
+  ANYLOC_REQUIRE(!(h1 && y_lo), "layernorm: the single-fp16 output has no lo array (y_lo must be NULL)");
   ANYLOC_REQUIRE(M >= 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm: M=%d D=%d (M >= 0, D a multiple of 4 in "
                  "[4, 2048])", M, D);
   // float4 loads of x, w and b; y_hi is stored 4 elements at a time (16, 8 or 4 bytes); fp8's y_lo holds fp32 scales
   const uintptr_t lo_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
-  const uintptr_t hi_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : bf16 || out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
+  const uintptr_t hi_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : bf16 || h1 || out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
   ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(b)) &
                   15) == 0 && (reinterpret_cast<uintptr_t>(y_hi) & hi_align) == 0 &&
                  (reinterpret_cast<uintptr_t>(y_lo) & lo_align) == 0,
@@ -242,7 +253,7 @@ extern "C" int anyloc_layernorm_split(const float* x, const float* w, const floa
                  "y_hi 4-byte, y_lo 4-byte)");
   if (M == 0) return ANYLOC_OK;
   return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo,
-                          bf16 ? ANYLOC_PAIR_BF16 : out_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_FP8
+                          bf16 ? ANYLOC_PAIR_BF16 : h1 ? ANYLOC_PAIR_F16X1 : out_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_FP8
                           : out_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32,
                           (cudaStream_t)stream);
 }
@@ -286,17 +297,18 @@ static int attention_dispatch(const float* qkv_hi, const float* qkv_lo, int B, i
 
 extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                                 void* o_hi, void* o_lo, int out_dtype, int engine, void* stream) {
-  if (out_dtype == ANYLOC_PAIR_BF16) {     // single bf16 in and out: the qkv epilogue's output format
+  if (out_dtype == ANYLOC_PAIR_BF16 || out_dtype == ANYLOC_PAIR_F16X1) {   // single in and out: the qkv epilogue's
+    const char* name = out_dtype == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16";           // output format
     ANYLOC_REQUIRE(qkv_hi && o_hi, "attention: null pointer");
-    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the single-bf16 format has no lo arrays (qkv_lo, o_lo must be NULL)");
+    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", name);
     ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
     if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0) {
-      set_error("attention: the single-bf16 format runs on the tensor-core engine only, with a 16-byte aligned qkv");
+      set_error("attention: the %s format runs on the tensor-core engine only, with a 16-byte aligned qkv", name);
       return ANYLOC_ERR_UNSUPPORTED;
     }
     if (B == 0 || T == 0) return ANYLOC_OK;
     ProfScope ps(PC_ATTENTION, (cudaStream_t)stream, 4.0 * B * (double)T * T * D);
-    return attention_tc_launch(qkv_hi, nullptr, B, T, D, heads, o_hi, nullptr, ANYLOC_PAIR_BF16, (cudaStream_t)stream);
+    return attention_tc_launch(qkv_hi, nullptr, B, T, D, heads, o_hi, nullptr, out_dtype, (cudaStream_t)stream);
   }
   ANYLOC_REQUIRE(qkv_hi && o_hi && o_lo, "attention: null pointer");
   ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
@@ -325,13 +337,13 @@ static int varlen_attn_table(int n, const int* row0, const int* len, VarlenAttnT
 extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const int32_t* row0,
                                        const int32_t* len, int D, int heads, void* o_hi, void* o_lo, int fmt,
                                        void* stream) {
-  ANYLOC_REQUIRE(fmt == ANYLOC_PAIR_TF32 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16,
-                 "attention_varlen: bad fmt %d", fmt);
-  const bool bf16 = fmt == ANYLOC_PAIR_BF16;
+  ANYLOC_REQUIRE(fmt == ANYLOC_PAIR_TF32 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 ||
+                 fmt == ANYLOC_PAIR_F16X1, "attention_varlen: bad fmt %d", fmt);
+  const bool single = fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1;
   ANYLOC_REQUIRE(qkv_hi && o_hi && row0 && len, "attention_varlen: null pointer");
-  if (bf16)
-    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention_varlen: the single-bf16 format has no lo arrays (qkv_lo, o_lo must be "
-                   "NULL)");
+  if (single)
+    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention_varlen: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)",
+                   fmt == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16");
   else
     ANYLOC_REQUIRE(qkv_lo && o_lo, "attention_varlen: the pair formats need qkv_lo and o_lo");
   ANYLOC_REQUIRE(n >= 1 && n <= ANYLOC_VIT_VARLEN_MAX_B, "attention_varlen: n=%d out of range [1,%d]", n,
@@ -383,13 +395,15 @@ struct VitBuffers {
 // n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  The single-bf16 format carves no
 // lo buffers and 2-byte GEMM inputs: pa [n_patch, Kp], y [M, D], qkv [M, 3D] (which also holds the fp32 [M, D] output
 // of a lone q/k/v tap), h [M, hidden] as bf16.
+// The single-fp16 format carves the same buffers as single bf16, of fp16.
 // The single-e4m3 format carves the bf16 patch rows as above, e4m3 LayerNorm rows y [M, D] with their row scales
 // [M], the bf16 qkv [M, 3D], the bf16 hidden layer h [M, H] (which also holds the attention's bf16 output [M, D]) and
 // the e4m3 hidden layer h8 [M, H] with its row scales [M].
 size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
                  VitBuffers* out) {
   const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
-  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16, fp8 = c->pair_dtype == ANYLOC_PAIR_FP8;
+  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16 || c->pair_dtype == ANYLOC_PAIR_F16X1;   // one 2-byte array
+  const bool fp8 = c->pair_dtype == ANYLOC_PAIR_FP8;
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   VitBuffers b;
   b.h8 = nullptr; b.h8_s = nullptr;
@@ -453,11 +467,11 @@ bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeight
   }
   return true;
 }
-// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16 or e4m3 weights
-// with a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for those formats on the SIMT engine
+// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16, single-fp16 or
+// e4m3 weights with a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for those formats on the SIMT engine
 int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int engine) {
-  const bool fp8 = cfg->pair_dtype == ANYLOC_PAIR_FP8;
-  if (cfg->pair_dtype != ANYLOC_PAIR_BF16 && !fp8) return ANYLOC_OK;
+  const bool fp8 = cfg->pair_dtype == ANYLOC_PAIR_FP8, h1 = cfg->pair_dtype == ANYLOC_PAIR_F16X1;
+  if (cfg->pair_dtype != ANYLOC_PAIR_BF16 && !fp8 && !h1) return ANYLOC_OK;
   bool lo = w->patch_w_lo != nullptr;
   for (int l = 0; l < cfg->depth && w->blocks; ++l) {
     const AnylocVitBlock& b = w->blocks[l];
@@ -466,12 +480,14 @@ int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights
   if (lo) {
     set_error(fp8 ? "%s: pair_dtype ANYLOC_PAIR_FP8 takes e4m3 block weights and bf16 patch weights; every *_w_lo must "
                     "be NULL"
-                  : "%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
+              : h1  ? "%s: pair_dtype ANYLOC_PAIR_F16X1 takes single fp16 weights; every *_w_lo must be NULL"
+                    : "%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
     return ANYLOC_ERR_ARG;
   }
   if (engine == ANYLOC_GEMM_SIMT) {
     set_error(fp8 ? "%s: the single-e4m3 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)"
-                  : "%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)",
+              : h1  ? "%s: the single-fp16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)"
+                    : "%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)",
               fn);
     return ANYLOC_ERR_UNSUPPORTED;
   }
@@ -530,17 +546,18 @@ static int facet_out(const VitSeqs& sq, int M, const float* src, int64_t ld, int
 }
 
 // the fp32 qkv rows of layer l in bf.qkv32 -> the facets of l the plan asks for and, when `pairs`, the attention's
-// operands in bf.qkv / bf.qkv_lo (single bf16 in bf.qkv for the bf16 format, else fp16 pairs when f16_attn, else tf32
-// pairs)
+// operands in bf.qkv / bf.qkv_lo (single bf16 in bf.qkv for the bf16 and e4m3 formats, single fp16 for the single-fp16
+// format, else fp16 pairs when f16_attn, else tf32 pairs)
 static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const VitSeqs& sq, const TapPlan& tp, int l,
                    bool pairs, bool f16_attn, cudaStream_t st) {
   const int D = c->embed_dim, m = tp.mask[l];
   const QkvTapOuts o{{(m & 1) ? tp.out[l][0] : nullptr, (m & 2) ? tp.out[l][1] : nullptr,
                       (m & 4) ? tp.out[l][2] : nullptr}};
   const bool single = c->pair_dtype == ANYLOC_PAIR_BF16 || c->pair_dtype == ANYLOC_PAIR_FP8;   // bf16 attention
-  const int pair = pairs ? (single ? 3 : f16_attn ? 2 : 1) : 0;
+  const bool h1 = c->pair_dtype == ANYLOC_PAIR_F16X1;
+  const int pair = pairs ? (single ? 3 : h1 ? 4 : f16_attn ? 2 : 1) : 0;
   const double rows_out = (double)M - (tp.use_cls ? 0 : sq.B);
-  const double bytes = 12.0 * M * D + (pair ? (pair == 3 ? 6.0 : pair == 2 ? 12.0 : 24.0) * M * D : 0.0) +
+  const double bytes = 12.0 * M * D + (pair ? (pair >= 3 ? 6.0 : pair == 2 ? 12.0 : 24.0) * M * D : 0.0) +
                        4.0 * rows_out * D * popcount3(m);
   ProfScope ps(PC_VIT_MISC, st, bytes);
   return launch_qkv_tap(bf.qkv32, M, sq.T, sq.img, D, pair, pairs ? bf.qkv : nullptr, pairs ? bf.qkv_lo : nullptr, o,
@@ -554,8 +571,9 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
   const int D = c->embed_dim, Hf = c->ffn_hidden;
   const int fmt = c->pair_dtype;
   const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16, fp8 = fmt == ANYLOC_PAIR_FP8;
+  const bool h1 = fmt == ANYLOC_PAIR_F16X1;
   int rc;
-  const double ln_bytes = (fp8 ? 5.0 : bf16 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
+  const double ln_bytes = (fp8 ? 5.0 : bf16 || h1 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
   { ProfScope ps(PC_LAYERNORM, st, ln_bytes);
     if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
   // q, k and v leave the qkv GEMM row-major through the plain split epilogue; for the tensor-core attention in the
@@ -581,7 +599,7 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
     if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, o_hi,
                                          fp8 ? nullptr : bf.y_lo, attn_fmt, st)))
       return rc;
-  } else if (bf16 || fp8) {
+  } else if (bf16 || fp8 || h1) {
     ProfScope ps(PC_ATTENTION, st, 4.0 * sq.B * (double)sq.T * sq.T * D);
     if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, o_hi, nullptr, attn_fmt, st))) return rc;
   } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine,
@@ -621,7 +639,8 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
 static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
                      const TapPlan& tp, int gemm_engine, cudaStream_t st) {
   const int D = cfg->embed_dim, fmt = cfg->pair_dtype;
-  const size_t wsz = fmt == ANYLOC_PAIR_FP8 ? 1 : fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 ? 2 : 4;
+  const size_t wsz = fmt == ANYLOC_PAIR_FP8 ? 1
+                     : fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1 ? 2 : 4;
   int rc;
   for (int l = 0; l <= tp.l_max; ++l) {
     const AnylocVitBlock& wb = w->blocks[l];

@@ -2,8 +2,8 @@
 // fp32 arrays) in the row-major qkv buffer [B*T, 3D] (q | k | v thirds); mma.sync m16n8k8 (tf32); output tf32 pairs.
 // Both GEMMs use the 3-term split  X.Y ~= X_hi.Y_hi + X_lo.Y_hi + X_hi.Y_lo  (fp32-equivalent accuracy), and each key
 // block's P.V partial is accumulated from zero and then added to the running output with round-to-nearest fp32 adds.
-// The two 2-byte formats (fp16 pairs, single bf16) run the wgmma kernel of attention_wg.cu instead: wgmma's transposed
-// B operand, which P.V needs for V, exists for 16-bit types only.
+// The 2-byte formats (fp16 pairs, single bf16, single fp16) run the wgmma kernel of attention_wg.cu instead: wgmma's
+// transposed B operand, which P.V needs for V, exists for 16-bit types only.
 //
 // CTA = (64-query tile, head, image), 4 warps; warp w owns query rows [16w, 16w+16) of the tile and keeps its Q
 // fragments (hi, lo) in registers for the whole key loop.  K and V blocks of 64 keys (hi and lo) are streamed through a
@@ -249,19 +249,19 @@ qkv_to_f16_kernel(const float* __restrict__ qkv_hi, const float* __restrict__ qk
 }  // namespace atc
 
 int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
-                        bool bf16, cudaStream_t st);
+                        int fmt, cudaStream_t st);
 int attention_wg_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int D, int heads,
-                               void* o_hi, void* o_lo, bool bf16, cudaStream_t st);
+                               void* o_hi, void* o_lo, int fmt, cudaStream_t st);
 
-// qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, or single bf16 with qkv_lo
-// unused); o_{hi,lo}: [B*T, D] of the same kind (bf16: o_hi only).  The 2-byte formats run attention_wg.cu's kernel.
+// qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, or single bf16 or single fp16
+// with qkv_lo unused); o_{hi,lo}: [B*T, D] of the same kind (single formats: o_hi only).  The 2-byte formats run attention_wg.cu's kernel.
 int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
                         int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(B <= 65535 && heads <= 65535, "attention_tc: grid too large (B=%d heads=%d)", B, heads);
-  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16)
-    return attention_wg_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, fmt == ANYLOC_PAIR_BF16, st);
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1)
+    return attention_wg_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, fmt, st);
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen))
     ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -279,8 +279,8 @@ int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const Var
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(heads <= 65535, "attention_tc: grid too large (heads=%d)", heads);
-  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16)
-    return attention_wg_varlen_launch(qkv_hi, qkv_lo, tab, D, heads, o_hi, o_lo, fmt == ANYLOC_PAIR_BF16, st);
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1)
+    return attention_wg_varlen_launch(qkv_hi, qkv_lo, tab, D, heads, o_hi, o_lo, fmt, st);
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen))
     ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -96,6 +96,16 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uin
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(lb), "f"(la));
 }
 
+// Single fp16 format (ANYLOC_PAIR_F16X1): the hi half of the fp16 pair alone, bit for bit what split_f16 /
+// split_f16x2 write into hi for the same (scaled) input.  Two values -> one packed word; `a` in the low 16 bits.
+__device__ __forceinline__ uint32_t pack_f16x2_hi(float a, float b) {
+  const float ha = veltkamp_hi11(a), hb = veltkamp_hi11(b);
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hb), "f"(ha));
+  return r;
+}
+__device__ __forceinline__ __half f16_hi(float xs) { return __float2half_rn(veltkamp_hi11(xs)); }
+
 // Single bf16 format (ANYLOC_PAIR_BF16): one array of bf16_rn(x), no lo word and no scale.  Two values -> one packed
 // word; `a` lands in the low 16 bits (element k), `b` in the high 16 bits (k+1).
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {

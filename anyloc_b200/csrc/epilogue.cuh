@@ -18,11 +18,15 @@ struct EpiParams {
   const float* row_scale = nullptr;   // [M] e4m3 A operand's row scales (single e4m3 GEMM only): acc of row m times row_scale[m]
 };
 
-// BF16 (the tensor-core GEMM's single-bf16 instantiation): the SPLIT outputs are one bf16 array, out = bf16_rn(v)
-template <bool BF16 = false>
+// SPLIT output format of a GEMM instantiation: the pair formats (chosen at run time by out_f16), or one array of the
+// tensor-core GEMM's single-bf16 / single-fp16 instantiations (out = bf16_rn(v), or the hi of split_f16(kActScale v))
+enum SingleOut { SGL_PAIRS = 0, SGL_BF16 = 1, SGL_F16X1 = 2 };
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void epi_store_split(const EpiParams& p, size_t o, float v) {
-  if (BF16) {
+  if (SGL == SGL_BF16) {
     reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16_rn(v);
+  } else if (SGL == SGL_F16X1) {
+    reinterpret_cast<__half*>(p.out)[o] = f16_hi(v * kActScale);
   } else if (p.out_f16) {
     __half h, l; split_f16(v * kActScale, h, l);
     reinterpret_cast<__half*>(p.out)[o] = h; reinterpret_cast<__half*>(p.out_lo)[o] = l;
@@ -47,24 +51,24 @@ __device__ __forceinline__ float silu_fast(float x) {
 
 // Apply the epilogue to one accumulator element (m, n).  For SWIGLU the caller passes the PAIR
 // (acc0 at column n even, acc1 at column n+1) and the result lands in column n/2.
-template <bool BF16 = false>
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void epi_store1(const EpiParams& p, int m, int n, float acc) {
   float v = acc * p.alpha + (p.bias ? __ldg(p.bias + n) : 0.f);
   size_t o = (size_t)m * p.ldo + n;
   switch (p.mode) {
     case ANYLOC_EPI_BIAS: p.out[o] = v; break;
-    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split<BF16>(p, o, v); break;
-    case ANYLOC_EPI_GELU_SPLIT: epi_store_split<BF16>(p, o, gelu_erf(v)); break;
+    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split<SGL>(p, o, v); break;
+    case ANYLOC_EPI_GELU_SPLIT: epi_store_split<SGL>(p, o, gelu_erf(v)); break;
     case ANYLOC_EPI_LS_RESID: p.out[o] = p.resid[o] + __ldg(p.gamma + n) * v; break;
     default: break;
   }
 }
-template <bool BF16 = false>
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void epi_store_pair(const EpiParams& p, int m, int n_even, float acc0, float acc1) {
   // SWIGLU: columns (n_even, n_even+1) = (x1_j, x2_j), j = n_even/2
   float x1 = acc0 * p.alpha + (p.bias ? __ldg(p.bias + n_even) : 0.f);
   float x2 = acc1 * p.alpha + (p.bias ? __ldg(p.bias + n_even + 1) : 0.f);
-  epi_store_split<BF16>(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
+  epi_store_split<SGL>(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
 }
 
 }  // namespace anyloc

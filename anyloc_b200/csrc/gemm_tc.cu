@@ -21,6 +21,8 @@
 // runs one wgmma.f32.e4m3.e4m3 per 32-element k-step on UINT8 tensor maps (128-element k-blocks) with the bf16 pass's
 // stages and staged epilogue; the accumulator of row m is multiplied by A's row scale before the epilogue, and the
 // SPLIT outputs are one bf16 array (gemm_tc_fp8_launch).
+// A fifth, single fp16 (ANYLOC_PAIR_F16X1: the hi array of the fp16 pairs alone), runs the fp16 wgmma once per k-step
+// with the bf16 pass's stages and a staged epilogue that writes the hi of the fp16 pair (gemm_tc_f16x1_launch).
 // Tiles are rastered in bands of BAND_N column blocks, n-fastest inside a band: the resident CTAs share a few A row
 // panels and one band of B that stays in L2 while the outputs stream through.
 #include <cuda.h>
@@ -79,10 +81,12 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   n_blk = band * band_n + (r - m_blk * w);
 }
 
-template <bool BF16 = false>
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, float a, float b) {
-  if (BF16) {            // single bf16
+  if (SGL == SGL_BF16) {        // single bf16
     *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + o) = pack_bf16x2(a, b);
+  } else if (SGL == SGL_F16X1) {     // single fp16: the hi of the fp16 pair of kActScale*x
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(ep.out) + o) = pack_f16x2_hi(a * kActScale, b * kActScale);
   } else if (ep.out_f16) {      // fp16 pair of kActScale*x
     uint32_t h, l;
     split_f16x2(a * kActScale, b * kActScale, h, l);
@@ -97,17 +101,17 @@ __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, floa
 }
 
 // epilogue of two adjacent accumulator columns (n even, n+1) of row m
-template <bool BF16 = false>
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int N, float v0, float v1) {
   const int mode = ep.mode;
   if (mode < 0) return;                    // diagnostic: discard (ANYLOC_GEMM_DEBUG_SKIP_EPI)
   if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {   // (x1_j, x2_j) = columns (2j, 2j+1); N is even
-    epi_store_pair<BF16>(ep, m, n, v0, v1);
+    epi_store_pair<SGL>(ep, m, n, v0, v1);
     return;
   }
   if (n + 1 >= N || (ep.ldo & 1)) {
-    epi_store1<BF16>(ep, m, n, v0);
-    if (n + 1 < N) epi_store1<BF16>(ep, m, n + 1, v1);
+    epi_store1<SGL>(ep, m, n, v0);
+    if (n + 1 < N) epi_store1<SGL>(ep, m, n + 1, v1);
     return;
   }
   const float al = ep.alpha;
@@ -122,23 +126,23 @@ __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int 
     const float2 r = *reinterpret_cast<const float2*>(ep.resid + o);
     *reinterpret_cast<float2*>(ep.out + o) = make_float2(r.x + g.x * x0, r.y + g.y * x1);
   } else if (mode == ANYLOC_EPI_GELU_SPLIT) {
-    store_split2<BF16>(ep, o, gelu_erf(x0), gelu_erf(x1));
+    store_split2<SGL>(ep, o, gelu_erf(x0), gelu_erf(x1));
   } else {                                 // BIAS_SPLIT
-    store_split2<BF16>(ep, o, x0, x1);
+    store_split2<SGL>(ep, o, x0, x1);
   }
 }
 
 // Register epilogue of the 3-term passes that do not stage (gated launches, outputs TMA cannot store: see
 // make_epi_maps) of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16), accumulators in the wgmma layout,
 // applied and stored pair by pair.
-template <bool BF16 = false>
+template <int SGL = SGL_PAIRS>
 __device__ __forceinline__ void epilogue_pairs(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int n = nq + j * 8;
     if (n >= N) continue;
-    if (r0 < M) epi_pair<BF16>(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
-    if (r0 + 8 < M) epi_pair<BF16>(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
+    if (r0 < M) epi_pair<SGL>(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
+    if (r0 + 8 < M) epi_pair<SGL>(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
   }
 }
 
@@ -203,15 +207,17 @@ __device__ __forceinline__ void epilogue_regs_batched(const EpiParams& ep, int r
 
 // ------------------------------------------------------------------ staged epilogue
 // Output formats of the staged path.  A subtile is 64 rows x COLS output columns; one 8 KB staging buffer holds it:
-// 64 x 32 fp32, the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs, or 64 x 64 single bf16.
-enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2, STG_BF16 = 3 };
+// 64 x 32 fp32, the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs, or 64 x 64 single bf16 or
+// single fp16.
+enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2, STG_BF16 = 3, STG_F16 = 4 };
 constexpr int STG_HALF = STG_BYTES / 2;    // offset of the lo array (pair formats)
 constexpr int STG_ROWS = 64;               // TMA box rows of the output maps: one consumer warpgroup's rows
 
 template <int KIND>
 struct StageFmt {
-  static constexpr int ESZ = KIND == STG_F16_PAIR || KIND == STG_BF16 ? 2 : 4;
-  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : KIND == STG_BF16 ? 64 : 32;   // output columns per subtile
+  static constexpr bool SINGLE16 = KIND == STG_BF16 || KIND == STG_F16;   // one 2-byte array
+  static constexpr int ESZ = KIND == STG_F16_PAIR || SINGLE16 ? 2 : 4;
+  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : SINGLE16 ? 64 : 32;   // output columns per subtile
   static constexpr int ROW_BYTES = COLS * ESZ;                       // 128 (fp32) or 64 bytes per row of one array
   static constexpr uint32_t SWZ = ROW_BYTES == 128 ? 7 : 3;          // TMA SWIZZLE_128B / SWIZZLE_64B
 };
@@ -278,6 +284,8 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
           const uint32_t o = stg_off<KIND>(r, (4 * jj + q) * F::ESZ);
           if (KIND == STG_BF16) {
             *reinterpret_cast<__nv_bfloat16*>(buf + o) = __float2bfloat16_rn(v);
+          } else if (KIND == STG_F16) {
+            *reinterpret_cast<__half*>(buf + o) = f16_hi(v * kActScale);
           } else if (KIND == STG_F16_PAIR) {
             __half hi, lo;
             split_f16(v * kActScale, hi, lo);
@@ -304,6 +312,8 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
           const float y0 = gelu ? gelu_erf(x0) : x0, y1 = gelu ? gelu_erf(x1) : x1;
           if (KIND == STG_BF16) {
             *reinterpret_cast<uint32_t*>(buf + o) = pack_bf16x2(y0, y1);
+          } else if (KIND == STG_F16) {
+            *reinterpret_cast<uint32_t*>(buf + o) = pack_f16x2_hi(y0 * kActScale, y1 * kActScale);
           } else if (KIND == STG_F16_PAIR) {
             uint32_t hi, lo;
             split_f16x2(y0 * kActScale, y1 * kActScale, hi, lo);
@@ -324,7 +334,7 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
     else named_bar_sync<2>(128);
     if (t == 0) {
       tma_store_2d(tm_out, smem_u32(buf), oc0, m0);
-      if (KIND != STG_F32 && KIND != STG_BF16) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
+      if (KIND != STG_F32 && !F::SINGLE16) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
       bulk_commit();
       if (RESID && s + 2 < BN / ACC && oc0 + 2 * F::COLS < n_out) {
         // residual of subtile s + 2 into this buffer, once the store has read it
@@ -345,7 +355,9 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
 // tm_resid for LS_RESID: (n_out, M) maps with 64-row boxes); 0: stored pair by pair from registers.
 // FP8 = true (with F16 and LOM = 0): single e4m3 operands (128 elements per 128 B k-block, wgmma K=32), A's row
 //             scales in ep.row_scale; SPLIT outputs as BF16.
-template <bool F16, int LOM, bool BF16 = false, bool FP8 = false>
+// F16X1 = true (with F16 and LOM = 0): single fp16 operands (the hi halves of fp16 pairs), the fp16 pairs' k-steps and
+//             alpha, one wgmma per k-step; the staged epilogue writes single fp16 SPLIT outputs (STG_F16).
+template <bool F16, int LOM, bool BF16 = false, bool FP8 = false, bool F16X1 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
@@ -355,8 +367,10 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   constexpr bool LO = LOM != 0, has_a_lo = (LOM & 1) != 0, has_b_lo = (LOM & 2) != 0;
   static_assert(!BF16 || (F16 && LOM == 0), "bf16 is a single-operand 2-byte format");
   static_assert(!FP8 || (F16 && LOM == 0 && !BF16), "e4m3 is a single-operand 1-byte format");
+  static_assert(!F16X1 || (F16 && LOM == 0 && !BF16 && !FP8), "single fp16 is a single-operand 2-byte format");
   constexpr bool OUT_BF16 = BF16 || FP8;     // SPLIT outputs: one bf16 array
-  using C = Cfg<LO, LO || OUT_BF16>;
+  constexpr int SGL = OUT_BF16 ? SGL_BF16 : F16X1 ? SGL_F16X1 : SGL_PAIRS;
+  using C = Cfg<LO, LO || OUT_BF16 || F16X1>;
   if (ep.gate != nullptr && *reinterpret_cast<const volatile int*>(ep.gate) == 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -474,7 +488,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       continue;
     }
     if (!staged) {
-      epilogue_pairs<OUT_BF16>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      epilogue_pairs<SGL>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
       continue;
     }
 #define ANYLOC_EPI_STAGED(KIND_, SWIGLU_, RESID_)                                                                   \
@@ -485,6 +499,9 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
     else if (OUT_BF16) {                     // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> single bf16
       if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_BF16, true, false);
       else ANYLOC_EPI_STAGED(STG_BF16, false, false);
+    } else if (F16X1) {                      // -> single fp16
+      if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_F16, true, false);
+      else ANYLOC_EPI_STAGED(STG_F16, false, false);
     } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
       if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, true, false);
       else ANYLOC_EPI_STAGED(STG_TF32_PAIR, true, false);
@@ -569,21 +586,22 @@ static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, i
 // gemm_tc_supported).  The row-length condition is conservative: in one H100 run of the staged-path test without it,
 // a 68-column fp16 output (136 bytes per row) came back with its ldo padding columns 68..71 written, as if the store
 // clipped columns only to 16-byte units.  Not reproduced since (the condition keeps such shapes off the staged path).
-// bf16: the SPLIT outputs are one bf16 array (64-column boxes, no lo map).
+// sgl (SGL_BF16 / SGL_F16X1): the SPLIT outputs are one bf16 or fp16 array (64-column boxes, no lo map).
 static int make_epi_maps(const EpiParams& ep, int M, int N, CUtensorMap* m_out, CUtensorMap* m_lo, CUtensorMap* m_resid,
-                         bool* staged, bool bf16) {
+                         bool* staged, int sgl) {
   memset(m_out, 0, sizeof(*m_out)); memset(m_lo, 0, sizeof(*m_lo)); memset(m_resid, 0, sizeof(*m_resid));
   const bool split = ep.mode == ANYLOC_EPI_BIAS_SPLIT || ep.mode == ANYLOC_EPI_GELU_SPLIT ||
                      ep.mode == ANYLOC_EPI_SWIGLU_SPLIT;
-  const int esz = split && (ep.out_f16 || bf16) ? 2 : 4;
+  const bool single = sgl != SGL_PAIRS;
+  const int esz = split && (ep.out_f16 || single) ? 2 : 4;
   const int n_out = ep.mode == ANYLOC_EPI_SWIGLU_SPLIT ? N / 2 : N;
   *staged = ep.mode >= 0 && ((long long)ep.ldo * esz) % 16 == 0 && ((long long)n_out * esz) % 16 == 0;
   if (!*staged) return ANYLOC_OK;
-  const int cols = split && bf16 ? StageFmt<STG_BF16>::COLS
+  const int cols = split && single ? StageFmt<STG_BF16>::COLS
                    : split && !ep.out_f16 ? StageFmt<STG_TF32_PAIR>::COLS : StageFmt<STG_F32>::COLS;
   int rc;
-  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols, split && bf16))) return rc;
-  if (split && !bf16 && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
+  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols, split && sgl == SGL_BF16))) return rc;
+  if (split && !single && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
   if (ep.mode == ANYLOC_EPI_LS_RESID && (rc = make_out_map(m_resid, ep.resid, M, n_out, ep.ldo, esz, cols))) return rc;
   return ANYLOC_OK;
 }
@@ -606,12 +624,12 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
 // epilogue of this host thread's last launch (anyloc_gemm_tc_last_staged)
 static thread_local int g_last_staged = -1;
 
-template <bool F16, int LOM, bool BF16 = false, bool FP8 = false>
+template <bool F16, int LOM, bool BF16 = false, bool FP8 = false, bool F16X1 = false>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                        int N, int K, const EpiParams& ep, int chunk, cudaStream_t st) {
   using namespace tc;
   constexpr bool LO = LOM != 0;
-  using CF = Cfg<LO, LO || BF16 || FP8>;
+  using CF = Cfg<LO, LO || BF16 || FP8 || F16X1>;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
   if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16, BF16, FP8))) return rc;
@@ -624,17 +642,19 @@ static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* 
   // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
   // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
   // for more would make the SM switch its shared-memory configuration back and forth).
-  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, BF16 || FP8))) return rc;
+  constexpr int SGL = BF16 || FP8 ? SGL_BF16 : F16X1 ? SGL_F16X1 : SGL_PAIRS;
+  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, SGL))) return rc;
   const int smem = staged ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES;
   g_last_staged = staged ? 1 : 0;
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16, FP8, F16X1>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            CF::STAGED ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES));
   }
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
-  gemm_tc3_kernel<F16, LOM, BF16, FP8><<<grid, THREADS, smem, st>>>(
+  gemm_tc3_kernel<F16, LOM, BF16, FP8, F16X1><<<grid, THREADS, smem, st>>>(
       ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(BAND_N, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
@@ -680,6 +700,14 @@ int gemm_tc_bf16_launch(const void* a, int lda, const void* b, int ldb, int M, i
                         cudaStream_t st) {
   static_assert(tc::Cfg<false, true>::SMEM_BYTES_STAGED <= 232448, "bf16 GEMM over H100's shared-memory opt-in");
   return launch_impl<true, 0, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
+}
+
+// single-fp16 GEMM (ANYLOC_PAIR_F16X1): the hi halves of fp16 pairs, one wgmma per k-step, the fp16 pairs' chunks and
+// alpha, staged epilogue; SPLIT outputs are one fp16 array (the hi of the fp16 pair of kActScale v).  Its own
+// instantiation, so the hi-only coarse pass (gemm_tc3_kernel<true, 0>) keeps its register epilogue and shared memory.
+int gemm_tc_f16x1_launch(const void* a, int lda, const void* b, int ldb, int M, int N, int K, const EpiParams& ep,
+                         cudaStream_t st) {
+  return launch_impl<true, 0, false, false, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
 }
 
 // single-e4m3 GEMM (ANYLOC_PAIR_FP8): e4m3 A rows with their scales a_scale [M], one e4m3 B, one wgmma per 32-element

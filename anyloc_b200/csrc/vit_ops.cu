@@ -25,8 +25,8 @@ __global__ void split_f16_kernel(const float* __restrict__ x, __half* __restrict
   for (; i < n; i += stride) { __half h, l; split_f16(x[i] * scale, h, l); hi[i] = h; lo[i] = l; }
 }
 
-// GEMM-input formats of the row kernels: FMT = ANYLOC_PAIR_TF32 (tf32 pairs), _F16 (fp16 pairs of kActScale*x) or
-// _BF16 (one bf16 array bf16_rn(x); the lo pointer is unused)
+// GEMM-input formats of the row kernels: FMT = ANYLOC_PAIR_TF32 (tf32 pairs), _F16 (fp16 pairs of kActScale*x), _BF16
+// (one bf16 array bf16_rn(x); the lo pointer is unused) or _F16X1 (the hi array of _F16 alone; lo unused)
 // x -> bf16_rn(x) (single bf16 format)
 __global__ void split_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -46,6 +46,10 @@ template <> struct PairOut<ANYLOC_PAIR_F16> {
 template <> struct PairOut<ANYLOC_PAIR_BF16> {
   typedef __nv_bfloat16 T;
   static __device__ __forceinline__ void put(__nv_bfloat16* hi, __nv_bfloat16*, size_t i, float v) { hi[i] = __float2bfloat16_rn(v); }
+};
+template <> struct PairOut<ANYLOC_PAIR_F16X1> {    // the hi half of PairOut<ANYLOC_PAIR_F16>'s pair; lo unused
+  typedef __half T;
+  static __device__ __forceinline__ void put(__half* hi, __half*, size_t i, float v) { hi[i] = f16_hi(v * kActScale); }
 };
 template <> struct PairOut<ANYLOC_PAIR_FP8> {     // LayerNorm only: e4m3 rows, y_lo holds the fp32 row scales
   typedef uint8_t T;
@@ -187,6 +191,9 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
       const float y2 = (v[i].z - mean) * rstd * ww.z + bb.z, y3 = (v[i].w - mean) * rstd * ww.w + bb.w;
       if constexpr (FMT == ANYLOC_PAIR_BF16) {
         reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] = make_uint2(pack_bf16x2(y0, y1), pack_bf16x2(y2, y3));
+      } else if constexpr (FMT == ANYLOC_PAIR_F16X1) {
+        reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] =
+            make_uint2(pack_f16x2_hi(y0 * kActScale, y1 * kActScale), pack_f16x2_hi(y2 * kActScale, y3 * kActScale));
       } else if constexpr (FMT == ANYLOC_PAIR_F16) {
         uint2 h, l;
         split_f16x2(y0 * kActScale, y1 * kActScale, h.x, l.x);
@@ -297,8 +304,8 @@ __device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x,
 
 // One fp32 row [q | k | v] of a tapped layer's qkv GEMM (3D columns, one warp, each element read once) -> the
 // attention's operand pairs of the row, in the format the qkv GEMM's split epilogue writes (pair: 0 none, 1 tf32
-// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split; 3 single bf16, lo unused), and the rows of the requested facets (out[f] != null),
-// through facet_row's arithmetic.
+// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split; 3 single bf16, lo unused; 4 single fp16, the hi of
+// pair 2's fp16 pair, lo unused), and the rows of the requested facets (out[f] != null), through facet_row's arithmetic.
 template <int MAXV>     // float4 per lane and third: D <= 128 * MAXV
 __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int pair, void* hi,
                                             void* lo, const QkvTapOuts& o, int64_t orow, int do_norm) {
@@ -316,6 +323,15 @@ __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ 
       for (int i = 0; i < MAXV; ++i) {
         const int d = lane + i * 32;
         if (d < D4) h2[d] = make_uint2(pack_bf16x2(v[i].x, v[i].y), pack_bf16x2(v[i].z, v[i].w));
+      }
+    } else if (pair == 4) {
+      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int d = lane + i * 32;
+        if (d < D4)
+          h2[d] = make_uint2(pack_f16x2_hi(v[i].x * kActScale, v[i].y * kActScale),
+                             pack_f16x2_hi(v[i].z * kActScale, v[i].w * kActScale));
       }
     } else if (pair == 2) {
       uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
@@ -432,11 +448,13 @@ int launch_split_bf16(const float* x, void* y, size_t n, cudaStream_t st) {
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-// fmt: ANYLOC_PAIR_* of the patch rows (bf16: lo unused)
+// fmt: ANYLOC_PAIR_* of the patch rows (bf16 and single fp16: lo unused)
 int launch_im2col(const float* img, int B, int H, int W, int P, int Kp, void* hi, void* lo, int fmt, cudaStream_t st) {
   const int n = B * (H / P) * (W / P);
   if (fmt == ANYLOC_PAIR_BF16)
     im2col_split_kernel<ANYLOC_PAIR_BF16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__nv_bfloat16*)hi, nullptr);
+  else if (fmt == ANYLOC_PAIR_F16X1)
+    im2col_split_kernel<ANYLOC_PAIR_F16X1><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, nullptr);
   else if (fmt == ANYLOC_PAIR_F16)
     im2col_split_kernel<ANYLOC_PAIR_F16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, (__half*)lo);
   else im2col_split_kernel<ANYLOC_PAIR_TF32><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (float*)hi, (float*)lo);
@@ -458,12 +476,13 @@ static void ln_launch(const float* x, const float* w, const float* b, int M, int
   else if (D <= 1024) layernorm_split_kernel<8, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
   else layernorm_split_kernel<16, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
 }
-// fmt: ANYLOC_PAIR_* of the output (bf16: y_lo unused; fp8: y_lo = the fp32 row scales [M])
+// fmt: ANYLOC_PAIR_* of the output (bf16 and single fp16: y_lo unused; fp8: y_lo = the fp32 row scales [M])
 int launch_layernorm(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi,
                      void* y_lo, int fmt, cudaStream_t st) {
   ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "layernorm: D=%d unsupported (multiple of 4, <= 2048)", D);
   if (fmt == ANYLOC_PAIR_FP8) ln_launch<ANYLOC_PAIR_FP8>(x, w, b, M, D, eps, y_hi, y_lo, st);
   else if (fmt == ANYLOC_PAIR_BF16) ln_launch<ANYLOC_PAIR_BF16>(x, w, b, M, D, eps, y_hi, nullptr, st);
+  else if (fmt == ANYLOC_PAIR_F16X1) ln_launch<ANYLOC_PAIR_F16X1>(x, w, b, M, D, eps, y_hi, nullptr, st);
   else if (fmt == ANYLOC_PAIR_F16) ln_launch<ANYLOC_PAIR_F16>(x, w, b, M, D, eps, y_hi, y_lo, st);
   else ln_launch<ANYLOC_PAIR_TF32>(x, w, b, M, D, eps, y_hi, y_lo, st);
   ANYLOC_CHECK_LAUNCH();
@@ -513,6 +532,8 @@ int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp
                          cudaStream_t st) {
   if (fmt == ANYLOC_PAIR_BF16)
     im2col_split_varlen_kernel<ANYLOC_PAIR_BF16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__nv_bfloat16*)hi, nullptr);
+  else if (fmt == ANYLOC_PAIR_F16X1)
+    im2col_split_varlen_kernel<ANYLOC_PAIR_F16X1><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, nullptr);
   else if (fmt == ANYLOC_PAIR_F16)
     im2col_split_varlen_kernel<ANYLOC_PAIR_F16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, (__half*)lo);
   else im2col_split_varlen_kernel<ANYLOC_PAIR_TF32><<<n_patches, 128, 0, st>>>(tab, P, Kp, (float*)hi, (float*)lo);
@@ -531,7 +552,8 @@ int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int row
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none; pair 3: single bf16 in hi) and facet rows; tab: packed images, else
+// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none; pair 3 / 4: single bf16 / fp16 in hi) and
+// facet rows; tab: packed images, else
 // B images of T tokens
 template <int MAXV>
 static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi,

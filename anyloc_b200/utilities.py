@@ -277,16 +277,19 @@ class _HookHandle:
         pass
 
 
-PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16", "fp8")
+PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16", "fp8", "f16x1")
+# precisions whose GEMM operands are fp16 (scaled by 8): an operand beyond fp16's range overflows, which the guard catches
+_FP16_RANGE = ("f16x3", "f16x1")
 
 
 def resolve_precision(precision, gemm_engine="auto"):
     """The extractor's precision: the argument, else $ANYLOC_B200_PRECISION, else "auto".  ValueError on an unknown
-    name, and on "bf16" or "fp8" with gemm_engine="simt" (single bf16 and e4m3 run on the tensor cores only)."""
+    name, and on "bf16", "fp8" or "f16x1" with gemm_engine="simt" (single bf16, e4m3 and fp16 run on the tensor cores
+    only)."""
     precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
     if precision not in PRECISIONS:
-        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3', 'bf16' or 'fp8', got {precision!r}")
-    if precision in ("bf16", "fp8") and gemm_engine == "simt":
+        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3', 'bf16', 'fp8' or 'f16x1', got {precision!r}")
+    if precision in ("bf16", "fp8", "f16x1") and gemm_engine == "simt":
         raise ValueError(f"precision={precision!r} runs on the tensor cores only; use gemm_engine='auto' or 'tc3'")
     return precision
 
@@ -305,11 +308,11 @@ class _GuardedExtractor:
         self.precision = "f16x3" if self._auto else precision
         self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=self._depth(),
                                           pair={"f16x3": "f16", "tf32x3": "tf32", "bf16": "bf16",
-                                                "fp8": "fp8"}[self.precision])
+                                                "fp8": "fp8", "f16x1": "f16x1"}[self.precision])
         self.gemm_engine = gemm_engine
         self.fh_handle = _HookHandle()
         self._hook_out = None
-        # fp16-range guard of the f16x3 format: "sync" = checked before __call__ returns (one host sync per call),
+        # fp16-range guard of the f16x3 and f16x1 formats: "sync" = checked before __call__ returns (one host sync per call),
         # "deferred" = the flag of call i is read at call i+1 / raise_if_overflowed() (no sync on the hot loop),
         # "off".  precision="auto" always checks synchronously (it has to decide before returning).
         self.check_finite = os.environ.get("ANYLOC_B200_CHECK_FINITE", "sync")
@@ -319,12 +322,17 @@ class _GuardedExtractor:
 
     _OVERFLOW_MSG = ("f16x3 precision overflowed the fp16 operand range (|8*x| > 65504 somewhere in the network); "
                      "construct the extractor with precision='tf32x3' (or 'auto')")
+    _OVERFLOW_MSG_F16X1 = ("f16x1 precision overflowed the fp16 operand range (|8*x| > 65504 somewhere in the network); "
+                           "construct the extractor with precision='bf16' (the same speed, with fp32's exponent range)")
+
+    def _overflow_msg(self):
+        return self._OVERFLOW_MSG_F16X1 if self.precision == "f16x1" else self._OVERFLOW_MSG
 
     def raise_if_overflowed(self):
         """Deferred mode: reads the finite-flag of the last call (one host sync)."""
         flag, self._pending_flag = self._pending_flag, None
         if flag is not None and not bool(flag):
-            raise _lib.AnylocError(self._OVERFLOW_MSG)
+            raise _lib.AnylocError(self._overflow_msg())
 
     def _switch_to_tf32(self):
         print("anyloc_b200: f16x3 operands overflowed the fp16 range -- switching this extractor to tf32x3 "
@@ -341,7 +349,7 @@ class _GuardedExtractor:
             if self.check_finite == "deferred" and not self._auto:
                 self.raise_if_overflowed()
             packed, out = self._extract(img)
-            if self.precision != "f16x3" or (self.check_finite == "off" and not self._auto):
+            if self.precision not in _FP16_RANGE or (self.check_finite == "off" and not self._auto):
                 return out
             flag = torch.isfinite(packed).all()
             if self.check_finite == "deferred" and not self._auto:
@@ -350,7 +358,7 @@ class _GuardedExtractor:
             if bool(flag):
                 return out
             if not self._auto:
-                raise _lib.AnylocError(self._OVERFLOW_MSG)
+                raise _lib.AnylocError(self._overflow_msg())
             self._switch_to_tf32()
             return self._extract(img)[1]
 
@@ -380,6 +388,12 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
     call); the patch embedding and the attention run as in "bf16", and what stays fp32 in "bf16"
     stays fp32.  Its error is that of the model run on e4m3-rounded GEMM inputs (about 2^-4
     relative per operand); it needs gemm_engine "auto" or "tc3".
+    "f16x1" runs at bf16's rate with fp16's 11 significant bits, and is also never chosen by
+    "auto": every GEMM and attention operand is one fp16 value, the hi half of the f16x3 pair
+    (about 2^-11 relative per operand, 8x finer than bf16), one fp16 MMA per product; what stays
+    fp32 in "bf16" stays fp32.  It keeps fp16's range, so the f16x3 overflow guard applies, and an
+    overflow raises naming "bf16" (same speed, fp32's exponent range) as the way out.  Not a
+    parity mode; it needs gemm_engine "auto" or "tc3".
 
     `dino_model` may also name a backbone with register tokens, `dinov2_vit{s,b,l,g}14_reg`.  As
     in the reference, only row 0 (cls) is dropped, so its 4 register rows come first: an output
@@ -416,7 +430,8 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
         """img [B,3,H,W] -> [B, (1 +) R + N, D] (R = 4 register rows for the *_reg models, else 0); or a list/tuple of
         differently sized images [3,H_i,W_i] / [1,3,H_i,W_i], all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
         pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
-        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16" or "fp8", which always run them)."""
+        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16", "fp8" or "f16x1", which always
+        run them)."""
         return self._guarded(img)
 
     def __del__(self):

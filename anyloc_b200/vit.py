@@ -111,7 +111,8 @@ class VitWeights:
     pair: the operand format of every GEMM -- "tf32" / "f16" (fp32-equivalent (hi, lo) pairs), "bf16" (one
     round-to-nearest bf16 copy of each weight matrix, half the bytes of the pairs; a fast mode, not a parity mode) or
     "fp8" (one e4m3 copy of each block weight matrix with a power-of-two scale, a quarter of the pairs' bytes, and a bf16
-    patch embedding; a faster mode, not a parity mode)."""
+    patch embedding; a faster mode, not a parity mode) or "f16x1" (the hi array of the "f16" pair of each weight matrix
+    alone, bit for bit, half the bytes of the pairs; bf16's speed with 3 more significant bits, not a parity mode)."""
 
     def __init__(self, name, state_dict, device, depth=None, pair="tf32"):
         if name not in ARCHS:
@@ -144,7 +145,8 @@ class VitWeights:
         def split(t, patch=False):
             """-> (hi, lo, alpha): the kernel-ready pair of a weight matrix and the accumulator scale
             1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs; bf16: (bf16_rn(w), None, 1.0); fp8 block
-            matrices: (e4m3_rn(w / s_w), None, s_w), the patch embedding as bf16)."""
+            matrices: (e4m3_rn(w / s_w), None, s_w), the patch embedding as bf16; f16x1: the f16 pair's (hi, None,
+            alpha))."""
             t = f32(t)
             with torch.cuda.device(dev):
                 if pair == "fp8" and not patch:
@@ -175,6 +177,8 @@ class VitWeights:
                     _lib.check(lib.anyloc_split_f16(_lib.ptr(t), _lib.ptr(hi), _lib.ptr(lo), t.numel(),
                                                     C.c_float(s_w), _lib.stream_ptr()), "split_f16")
                     alpha = 1.0 / (_lib.ACT_SCALE * s_w)
+                    if pair == "f16x1":        # the pair's hi alone; lo's memory is reused in stream order
+                        lo = None
             self._keep += [hi, lo]
             return hi, lo, alpha
 

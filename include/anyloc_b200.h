@@ -71,6 +71,17 @@ extern "C" {
                                       promoted into the fp32 accumulator every 128 elements of K; SPLIT outputs, the
                                       attention and the patch embedding are single bf16 (ANYLOC_PAIR_BF16).
                                       Tensor-core engine only. */
+#define ANYLOC_PAIR_F16X1 4        /* NOT a pair and NOT fp32-equivalent: the hi array of ANYLOC_PAIR_F16 alone.  One fp16
+                                      array of s*x, bit for bit the hi that ANYLOC_PAIR_F16 writes for the same input:
+                                      Veltkamp's split rounds s*x to nearest at 11 significant bits, then cvt.rn packs
+                                      it into fp16 (ties and values in the fp16 subnormal range may differ from
+                                      __float2half_rn(s*x)).  Activations use s = 8, weights the per-tensor power of
+                                      two s_w of the fp16 pairs (the weights' hi of anyloc_split_f16); alpha =
+                                      1/(8 s_w).  No lo array (every *_lo pointer NULL).  One fp16 MMA per product;
+                                      2^-11 relative per operand, 8x finer than single bf16, with fp16's range: an
+                                      |s x| > 65504 overflows to Inf.  Tensor-core engine only (wgmma GEMM at every
+                                      M, wgmma attention).  Accumulators, LayerNorm statistics, softmax, the residual
+                                      stream and every feature output stay fp32. */
 /* GEMM engines */
 #define ANYLOC_GEMM_AUTO 0
 #define ANYLOC_GEMM_SIMT 1         /* fp32 FFMA (validation / odd shapes)               */
@@ -279,6 +290,16 @@ typedef struct {
  * Workspace: with A(x), n_p, M and H as above,
  *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(M D) + A(4 M) + A(6 M D) + A(2 M H) + A(M H) + A(4 M) [+ A(12 M D) for
  *   the fp32 qkv rows of the tap calls] + 4096 bytes. */
+/* Single fp16 (pair_dtype = ANYLOC_PAIR_F16X1), single bf16's speed at 2^-11 instead of 2^-8 per operand: the weight
+ * matrices are the hi arrays of the fp16 pairs (anyloc_split_f16 with the pairs' per-tensor scale s_w, lo discarded),
+ * every *_w_lo NULL and every *_alpha 1/(8 s_w); LayerNorm, im2col, the qkv epilogue / tap and the attention write one
+ * fp16 array of 8 x; the GEMMs and the attention run one fp16 MMA per product.  What stays fp32 under single bf16 stays
+ * fp32.  Not a parity mode; fp16's range applies (|8 x| > 65504 overflows to Inf, as for the fp16 pairs).  A non-NULL
+ * *_w_lo returns ANYLOC_ERR_ARG and gemm_engine = ANYLOC_GEMM_SIMT ANYLOC_ERR_UNSUPPORTED, before anything is launched.
+ * Every GEMM runs on the tensor cores whatever M, so single, list (_varlen) and tap calls are bit-identical.
+ * Workspace: single bf16's formula (2-byte GEMM inputs, no lo buffers), with A(x), n_p, M and H as above:
+ *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(2 M D) + A(6 M D) + A(2 M H) [+ A(12 M D) for the fp32 qkv rows of the
+ *   tap calls] + 4096 bytes. */
 /* padded patch-embed reduction length (3*14*14=588 -> multiple of 32) */
 int anyloc_vit_patch_k(int patch);
 size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W);
@@ -352,6 +373,9 @@ int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeigh
  * in_dtype = out_dtype = ANYLOC_PAIR_BF16: C = A . B^T of single bf16 operands (a_lo, b_lo, out_lo NULL, else
  * ANYLOC_ERR_ARG; bf16 in with another out_dtype, or the reverse, ANYLOC_ERR_ARG); the SPLIT epilogues write one bf16
  * array bf16_rn(v), BIAS / LS_RESID fp32 as usual.  Tensor-core engine only, at every M (SIMT: ANYLOC_ERR_UNSUPPORTED). */
+/* in_dtype = out_dtype = ANYLOC_PAIR_F16X1: C = alpha A . B^T of single fp16 operands (a_lo, b_lo, out_lo NULL, else
+ * ANYLOC_ERR_ARG; single fp16 in with another out_dtype, or the reverse, ANYLOC_ERR_ARG); the SPLIT epilogues write
+ * one fp16 array, the hi of the fp16 pair of 8 v, BIAS / LS_RESID fp32.  Tensor-core engine only, at every M. */
 /* in_dtype = ANYLOC_PAIR_FP8, out_dtype = ANYLOC_PAIR_BF16: C = (s_r[m] alpha) (A . B^T) with A e4m3 [M, K] and its
  * fp32 row scales s_r in a_lo, B e4m3 (b_lo NULL) and alpha = s_w; out_lo NULL; the SPLIT epilogues write one bf16
  * array, BIAS / LS_RESID fp32.  K, lda and ldb multiples of 16.  Tensor-core engine only, at every M. */
@@ -369,6 +393,7 @@ int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream);
 /* y = LayerNorm(x) over rows of D (biased variance, eps inside the square root) with gain w and bias b, x [M, D] fp32.
  * out_dtype = ANYLOC_PAIR_TF32 / _F16: y_hi, y_lo [M, D] the pair of y (fp16 pairs: of 8 y);
  * out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG);
+ * out_dtype = ANYLOC_PAIR_F16X1: y_hi = the hi array of the fp16 pair of 8 y, y_lo NULL (else ANYLOC_ERR_ARG);
  * out_dtype = ANYLOC_PAIR_FP8: y_hi = e4m3 rows of LayerNorm(x) [M, D], y_lo = their fp32 scales [M].
  * D a multiple of 4 in [4, 2048].  ANYLOC_ERR_ARG before anything is launched for a null pointer, M < 0, D outside that
  * range, x, w or b not 16-byte aligned, or y_hi / y_lo not aligned to 4 of their elements (fp8: y_hi and the scales
@@ -388,14 +413,17 @@ int anyloc_quantize_fp8_tensor(const float* x, void* q, size_t n, float* scale_h
  * be NULL for the SIMT engine (plain fp32 input).  -> o (hi,lo) [B,T,D].  engine: ANYLOC_GEMM_*.
  * out_dtype = ANYLOC_PAIR_BF16: qkv_hi is single bf16 [B,T,3D] (what the qkv GEMM's bf16 split epilogue writes) and
  * o_hi single bf16 [B,T,D], qkv_lo and o_lo NULL (else ANYLOC_ERR_ARG); one bf16 MMA per product, P rounded once to
- * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED). */
+ * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED).
+ * out_dtype = ANYLOC_PAIR_F16X1: the same with single fp16 qkv_hi of 8 x and o_hi of 8 o (the hi arrays of the fp16
+ * pairs); 1/64 folded into the logit scale and P = 1024 p, as for the fp16 pairs, P rounded once. */
 int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                      void* o_hi, void* o_lo, int out_dtype, int engine, void* stream);
 /* The packed attention of the _varlen ViT calls, on n images of different lengths in one [rows, 3D] qkv buffer:
  * row0, len HOST int32 [n]; image i's q|k|v rows are [row0[i], row0[i] + len[i]) and its output rows the same rows of
  * o [rows, D].  Images may lie in any order with gaps between them; rows outside every image are neither used nor
  * written.  The operands are in the format fmt of the ViT's qkv epilogue, not converted: ANYLOC_PAIR_TF32 (tf32
- * pairs), ANYLOC_PAIR_F16 (fp16 pairs of 8*x, output pairs of 8*o) or ANYLOC_PAIR_BF16 (qkv_lo, o_lo NULL).  The same
+ * pairs), ANYLOC_PAIR_F16 (fp16 pairs of 8*x, output pairs of 8*o), ANYLOC_PAIR_BF16 or ANYLOC_PAIR_F16X1 (qkv_lo, o_lo
+ * NULL).  The same
  * table (longest first) and launcher as the ViT; an image's rows are bit-identical to anyloc_attention on that image
  * alone (fp16 pairs: fed the tf32 pair of x) whatever the other images and the rows around it hold.
  * ANYLOC_ERR_ARG for a null pointer, n outside [1, ANYLOC_VIT_VARLEN_MAX_B], len[i] < 1, row0[i] < 0, overlapping
