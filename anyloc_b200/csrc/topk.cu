@@ -196,6 +196,10 @@ static cudaError_t launch_normalize_rows(const float* x, int n_rows, int D, int 
 //   C: second sweep, the elements >= tau (usually k .. a few k of them) are compacted into a shared-memory list;
 //   D: k rounds of arg-best over the list (score descending, lowest index first among equal scores).
 // More than SEL_CAP candidates (a row with thousands of equal scores) -> k ordered sweeps over the row (read-only).
+// MERGE (streamed search, k <= SEL_CAP): the row is a piece of the database holding global rows [row0, row0 + n_db),
+// and dist / idx hold the running k best of the rows before it.  Those k enter the list first (slots 0 .. k-1, so they
+// stay in shared memory through the sweeps) and the k best of the union are written back in place.  tau is still taken
+// over the piece alone: the union's k-th best is at least the piece's, so every union top-k member of the piece is >= tau.
 constexpr int SEL_CAP = 4096;
 __device__ __forceinline__ bool better(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
 
@@ -225,27 +229,41 @@ __device__ __forceinline__ void block_argbest(float& best, int& besti, float* bv
   __syncthreads();
 }
 
+template <bool MERGE>
 __global__ void __launch_bounds__(1024)
 topk_select2_kernel(const float* __restrict__ scores, int n_db, int64_t ld, int k, int metric,
                     const float* __restrict__ qq, const float* __restrict__ dd,
-                    float* __restrict__ dist, int64_t* __restrict__ idx, const int* __restrict__ gate /* nullable */) {
+                    float* __restrict__ dist, int64_t* __restrict__ idx, const int* __restrict__ gate /* nullable */,
+                    int row0 /* MERGE only */) {
   if (gate != nullptr && *reinterpret_cast<const volatile int*>(gate) == 0) return;
   const int q = blockIdx.x;
   const float* s = scores + (size_t)q * ld;
   const bool l2 = metric == ANYLOC_METRIC_L2;
   const float a = l2 ? qq[q] : 0.f;
   auto key = [&](int j) { const float v = s[j]; return l2 ? -((a - 2.0f * v) + dd[j]) : v; };   // larger = better
+  auto gid = [&](int j) { return MERGE ? row0 + j : j; };                                         // global row index
   __shared__ float bv[33];
   __shared__ int bi[33];
   __shared__ float cv[SEL_CAP];
   __shared__ int ci[SEL_CAP];
   __shared__ int count;
-  if (threadIdx.x == 0) count = 0;
+  if constexpr (MERGE) {
+    // the running list (read before anything is written back); its -1 pads can never be selected
+    for (int r = threadIdx.x; r < k; r += blockDim.x) {
+      const int64_t i = idx[(size_t)q * k + r];
+      const float d = dist[(size_t)q * k + r];
+      cv[r] = i >= 0 ? (l2 ? -d : d) : -INFINITY;
+      ci[r] = i >= 0 ? (int)i : 0x7fffffff;
+    }
+    if (threadIdx.x == 0) count = k;
+  } else {
+    if (threadIdx.x == 0) count = 0;
+  }
   // A
   float mine = -INFINITY; int minei = 0x7fffffff;
   for (int j = threadIdx.x; j < n_db; j += blockDim.x) {
     const float v = key(j);
-    if (better(v, j, mine, minei)) { mine = v; minei = j; }
+    if (better(v, gid(j), mine, minei)) { mine = v; minei = gid(j); }
   }
   // B
   float tau = -INFINITY;
@@ -265,7 +283,7 @@ topk_select2_kernel(const float* __restrict__ scores, int n_db, int64_t ld, int 
     const float v = key(j);
     if (v >= tau) {
       const int slot = atomicAdd(&count, 1);
-      if (slot < SEL_CAP) { cv[slot] = v; ci[slot] = j; }
+      if (slot < SEL_CAP) { cv[slot] = v; ci[slot] = gid(j); }
     }
   }
   __syncthreads();
@@ -278,7 +296,13 @@ topk_select2_kernel(const float* __restrict__ scores, int n_db, int64_t ld, int 
       float b = -INFINITY; int bidx = 0x7fffffff;
       for (int j = threadIdx.x; j < n_db; j += blockDim.x) {
         const float v = key(j);
-        if ((v < pv || (v == pv && j > pj)) && better(v, j, b, bidx)) { b = v; bidx = j; }
+        if ((v < pv || (v == pv && gid(j) > pj)) && better(v, gid(j), b, bidx)) { b = v; bidx = gid(j); }
+      }
+      if constexpr (MERGE) {             // the running list, still in slots 0 .. k-1
+        for (int c = threadIdx.x; c < k; c += blockDim.x) {
+          const float v = cv[c]; const int i = ci[c];
+          if ((v < pv || (v == pv && i > pj)) && better(v, i, b, bidx)) { b = v; bidx = i; }
+        }
       }
       block_argbest(b, bidx, bv, bi);
       if (threadIdx.x == 0) {
@@ -322,12 +346,19 @@ topk_select2_kernel(const float* __restrict__ scores, int n_db, int64_t ld, int 
 // pairs in fp32 and the k best of them -- score descending, lowest index first -- are the answer: identical to the
 // 3-term path up to fp32 rounding of the scores, at a third of the tensor-core work.  A query with more than CAND_MAX
 // candidates raises a device flag that switches on the 3-term fallback (launched behind it, gated, no host sync).
+// MERGE (streamed search): the rows are one piece of the database and run_dist holds the k best EXACT scores of the
+// rows before it (-inf while fewer than k).  Its k-th, R, is a second lower bound: a row of this piece enters the final
+// top-k only by beating all k running entries (their indices are lower, so a tie loses), i.e. with S > R, and then
+// S~ >= S - eps_q > R - eps_q.  The threshold is max(tau, R) - 2 eps_q: R - eps_q would do, the second eps_q leaves the
+// same margin for the fp32 rounding of the re-scored S that tau - 2 eps_q leaves.
 constexpr int CAND_MAX = 256;
 
+template <bool MERGE>
 __global__ void __launch_bounds__(1024)
 topk_candidates_kernel(const float* __restrict__ scores, int n_db, int64_t ld, int k, const float* __restrict__ dn_q,
                        const int* __restrict__ dn_max_bits, int32_t* __restrict__ cand /* [n_q, CAND_MAX] */,
-                       int32_t* __restrict__ cand_n /* [n_q] */, int* __restrict__ overflow) {
+                       int32_t* __restrict__ cand_n /* [n_q] */, int* __restrict__ overflow,
+                       const float* __restrict__ run_dist /* MERGE only: [n_q, k] */) {
   const int q = blockIdx.x;
   const float* s = scores + (size_t)q * ld;
   __shared__ float bv[33];
@@ -353,7 +384,9 @@ topk_candidates_kernel(const float* __restrict__ scores, int n_db, int64_t ld, i
   }
   const float DN = __int_as_float(*dn_max_bits), dq = dn_q[q];
   const float eps = (dq + DN + dq * DN) * 1.001f + 3.0e-5f;
-  const float thr = tau - 2.0f * eps;
+  float thr;
+  if constexpr (MERGE) thr = fmaxf(tau, run_dist[(size_t)q * k + k - 1]) - 2.0f * eps;
+  else thr = tau - 2.0f * eps;
   __syncthreads();
   for (int j = threadIdx.x; j < n_db; j += blockDim.x) {
     if (s[j] >= thr) {
@@ -376,16 +409,21 @@ __device__ __forceinline__ float2 h2f(uint32_t u) {
   return __half22float2(*reinterpret_cast<const __half2*>(&u));
 }
 constexpr int RS_CHUNK = 4096;          // query elements staged per pass (fp32: 16 KB of shared memory)
+constexpr int COARSE_K_MAX = 64;        // the coarse route's largest k
+// MERGE (streamed search): the candidates are rows of a piece holding global rows [row0, ...), and dist / idx hold the
+// running k best of the rows before it; those join the re-scored candidates and the k best of both go back in place.
+template <bool MERGE>
 __global__ void __launch_bounds__(256)
 topk_rescore_kernel(const __half* __restrict__ db_hi, const __half* __restrict__ db_lo, const __half* __restrict__ qu_hi,
                     const __half* __restrict__ qu_lo, int Dv, int k, const int32_t* __restrict__ cand,
                     const int32_t* __restrict__ cand_n, const int* __restrict__ overflow, float* __restrict__ dist,
-                    int64_t* __restrict__ idx) {
+                    int64_t* __restrict__ idx, int row0 /* MERGE only */) {
   if (*reinterpret_cast<const volatile int*>(overflow) != 0) return;       // the 3-term fallback answers every query
   const int q = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  constexpr int LIST = CAND_MAX + (MERGE ? COARSE_K_MAX : 0);
   __shared__ __align__(16) float xq[RS_CHUNK];      // this pass' slice of the query, hi + lo (exact: 22 significant bits)
-  __shared__ float cv[CAND_MAX];
-  __shared__ int ci[CAND_MAX];
+  __shared__ float cv[LIST];
+  __shared__ int ci[LIST];
   __shared__ float bv[33];
   __shared__ int bi[33];
   const int n_c = cand_n[q];
@@ -428,9 +466,20 @@ topk_rescore_kernel(const __half* __restrict__ db_hi, const __half* __restrict__
   __syncthreads();
   for (int c = threadIdx.x; c < n_c; c += blockDim.x) cv[c] *= 1.0f / (kRetrievalScale * kRetrievalScale);
   __syncthreads();
+  int n_l = n_c;
+  if constexpr (MERGE) {
+    for (int c = threadIdx.x; c < n_c; c += blockDim.x) ci[c] += row0;
+    for (int r = threadIdx.x; r < k; r += blockDim.x) {      // -1 pads can never be selected
+      const int64_t i = idx[(size_t)q * k + r];
+      cv[n_c + r] = i >= 0 ? dist[(size_t)q * k + r] : -INFINITY;
+      ci[n_c + r] = i >= 0 ? (int)i : 0x7fffffff;
+    }
+    __syncthreads();
+    n_l = n_c + k;
+  }
   for (int r = 0; r < k; ++r) {
     float b = -INFINITY; int bidx = 0x7fffffff; int bslot = -1;
-    for (int c = threadIdx.x; c < n_c; c += blockDim.x)
+    for (int c = threadIdx.x; c < n_l; c += blockDim.x)
       if (better(cv[c], ci[c], b, bidx)) { b = cv[c]; bidx = ci[c]; bslot = c; }
     float wb = b; int wi = bidx;
     block_argbest(wb, wi, bv, bi);
@@ -536,22 +585,24 @@ extern "C" size_t anyloc_index_search_workspace_bytes(int64_t n_db, int n_q, int
          align_up((size_t)n_q * 4, 256) + 256 + 1024;
 }
 
-extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_t capacity, int64_t n_db, const float* qu,
-                                   int n_q, int Dv, int k, int metric, int normalize, float* dist, int64_t* idx, void* ws,
-                                   size_t ws_bytes, void* stream) {
-  ANYLOC_REQUIRE(index && qu && dist && idx && ws, "index_search: null pointer");
-  ANYLOC_REQUIRE(n_db > 0 && n_db <= capacity && n_db < (1ll << 31) && n_q >= 0 && Dv > 0 && k > 0,
-                 "index_search: bad dims n_db=%lld n_q=%d Dv=%d k=%d", (long long)n_db, n_q, Dv, k);
-  ANYLOC_REQUIRE(Dv % 4 == 0, "index_search: Dv=%d must be a multiple of 4", Dv);
-  ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "index_search: unknown metric %d", metric);
-  if (n_q == 0) return ANYLOC_OK;
-  IndexView v;
-  if (!carve_index(const_cast<void*>(index), index_bytes, capacity, Dv, normalize, &v)) {
-    set_error("index_search: index blob too small");
-    return ANYLOC_ERR_WORKSPACE;
+// The search of rows [first, first + n_db) of a carved index.  Resident (MERGE = false, first = row0 = 0, n_total = n_db):
+// the k best are written to dist / idx.  Continuation (MERGE): those rows are global rows [row0, row0 + n_db) of a
+// database of n_total rows, and their k best are merged into the running list dist / idx.  The route follows n_total,
+// so that every piece is answered by the product the resident search of the whole database would use.
+template <bool MERGE>
+static int search_rows(const IndexView& v0, int64_t first, int64_t n_db, int64_t row0, int64_t n_total, const float* qu,
+                       int n_q, int Dv, int k, int metric, int normalize, float* dist, int64_t* idx, void* ws,
+                       size_t ws_bytes, cudaStream_t st) {
+  void* stream = st;
+  const size_t esz = v0.f16 ? 2 : 4;
+  IndexView v = v0;
+  if constexpr (MERGE) {
+    v.hi = (char*)v0.hi + (size_t)first * Dv * esz;
+    v.lo = (char*)v0.lo + (size_t)first * Dv * esz;
+    v.sq = v0.sq + first;
+  } else {
+    (void)first; (void)row0; (void)n_total;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t esz = v.f16 ? 2 : 4;
   Workspace w(ws, ws_bytes);
   void* qu_hi = w.take<char>((size_t)n_q * Dv * esz);
   void* qu_lo = w.take<char>((size_t)n_q * Dv * esz);
@@ -576,7 +627,8 @@ extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_
   const float alpha = v.f16 ? 1.0f / (kRetrievalScale * kRetrievalScale) : 1.0f;
   const int pair = v.f16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32;
   // ---- coarse pass + exact re-scoring of the candidates (inner product, fp16 index)
-  const bool coarse = v.f16 && metric == ANYLOC_METRIC_IP && k <= 64 && n_db >= 1024 && n_q >= 32;
+  const bool coarse = v.f16 && metric == ANYLOC_METRIC_IP && k <= COARSE_K_MAX && (MERGE ? n_total : n_db) >= 1024 &&
+                      n_q >= 32;
   const int* gate = nullptr;
   if (coarse) {
     ANYLOC_CHECK_CUDA(cudaMemsetAsync(flags, 0, 256, st));
@@ -586,10 +638,12 @@ extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_
                         nullptr, nullptr, scores, nullptr, (int)n_db, ANYLOC_PAIR_TF32, ANYLOC_GEMM_TC3, stream);
     if (rc) return rc;
     ProfScope ps(PC_TOPK, st, 8.0 * (double)n_q * (double)n_db);
-    topk_candidates_kernel<<<n_q, 1024, 0, st>>>(scores, (int)n_db, n_db, k, dnq, v.hdr, cand, cand_n, flags);
+    topk_candidates_kernel<MERGE><<<n_q, 1024, 0, st>>>(scores, (int)n_db, n_db, k, dnq, v.hdr, cand, cand_n, flags,
+                                                        dist);
     ANYLOC_CHECK_LAUNCH();
-    topk_rescore_kernel<<<n_q, 256, 0, st>>>((const __half*)v.hi, (const __half*)v.lo, (const __half*)qu_hi,
-                                             (const __half*)qu_lo, Dv, k, cand, cand_n, flags, dist, idx);
+    topk_rescore_kernel<MERGE><<<n_q, 256, 0, st>>>((const __half*)v.hi, (const __half*)v.lo, (const __half*)qu_hi,
+                                                    (const __half*)qu_lo, Dv, k, cand, cand_n, flags, dist, idx,
+                                                    (int)row0);
     ANYLOC_CHECK_LAUNCH();
     gate = flags;            // the exact path below only runs (on the device) if a candidate list overflowed
   }
@@ -598,10 +652,54 @@ extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_
   if (rc) return rc;
   {
     ProfScope ps(PC_TOPK, st, gate ? 0.0 : 8.0 * (double)n_q * (double)n_db);
-    topk_select2_kernel<<<n_q, 1024, 0, st>>>(scores, (int)n_db, n_db, k, metric, qq, v.sq, dist, idx, gate);
+    topk_select2_kernel<MERGE><<<n_q, 1024, 0, st>>>(scores, (int)n_db, n_db, k, metric, qq, v.sq, dist, idx, gate,
+                                                     (int)row0);
     ANYLOC_CHECK_LAUNCH();
   }
   return ANYLOC_OK;
+}
+
+extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_t capacity, int64_t n_db, const float* qu,
+                                   int n_q, int Dv, int k, int metric, int normalize, float* dist, int64_t* idx, void* ws,
+                                   size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(index && qu && dist && idx && ws, "index_search: null pointer");
+  ANYLOC_REQUIRE(n_db > 0 && n_db <= capacity && n_db < (1ll << 31) && n_q >= 0 && Dv > 0 && k > 0,
+                 "index_search: bad dims n_db=%lld n_q=%d Dv=%d k=%d", (long long)n_db, n_q, Dv, k);
+  ANYLOC_REQUIRE(Dv % 4 == 0, "index_search: Dv=%d must be a multiple of 4", Dv);
+  ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "index_search: unknown metric %d", metric);
+  if (n_q == 0) return ANYLOC_OK;
+  IndexView v;
+  if (!carve_index(const_cast<void*>(index), index_bytes, capacity, Dv, normalize, &v)) {
+    set_error("index_search: index blob too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  return search_rows<false>(v, 0, n_db, 0, n_db, qu, n_q, Dv, k, metric, normalize, dist, idx, ws, ws_bytes,
+                            (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_index_search_continue(const void* index, size_t index_bytes, int64_t capacity, int64_t first,
+                                            int64_t n_rows, int64_t row0, int64_t n_total, const float* qu, int n_q,
+                                            int Dv, int k, int metric, int normalize, float* dist, int64_t* idx,
+                                            void* ws, size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(index && qu && dist && idx && ws, "index_search_continue: null pointer");
+  ANYLOC_REQUIRE(n_rows > 0 && first >= 0 && first + n_rows <= capacity && row0 >= 0 && row0 + n_rows <= n_total &&
+                 n_total < (1ll << 31) && n_q >= 0 && Dv > 0 && k > 0,
+                 "index_search_continue: bad dims first=%lld n_rows=%lld row0=%lld n_total=%lld capacity=%lld n_q=%d "
+                 "Dv=%d k=%d", (long long)first, (long long)n_rows, (long long)row0, (long long)n_total,
+                 (long long)capacity, n_q, Dv, k);
+  ANYLOC_REQUIRE(k <= SEL_CAP, "index_search_continue: k=%d above %d (the running list is merged in shared memory)", k,
+                 SEL_CAP);
+  ANYLOC_REQUIRE(Dv % 4 == 0, "index_search_continue: Dv=%d must be a multiple of 4", Dv);
+  ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "index_search_continue: unknown metric %d",
+                 metric);
+  if (n_q == 0) return ANYLOC_OK;
+  IndexView v;
+  if (!carve_index(const_cast<void*>(index), index_bytes, capacity, Dv, normalize, &v)) {
+    set_error("index_search_continue: index blob too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  return search_rows<true>(v, first, n_rows, row0, n_total, qu, n_q, Dv, k, metric, normalize, dist, idx, ws, ws_bytes,
+                           (cudaStream_t)stream);
 }
 
 // One-shot form (get_top_k_recall builds the index and searches it once, utilities.py:449-450): a temporary index in

@@ -499,11 +499,13 @@ def _normalize_rows_dev(x):
 _STAGE_BYTES = 1 << 30      # each of the two pinned staging buffers of a streamed fit: at most 2 GiB of host memory pinned
 
 
-def _device_budget(dev):
-    """Device bytes a k-means fit may allocate: free memory once torch has returned its unused cached segments, less a
-    1 GiB margin for the allocator and other work on the device.  Cached bytes inside partly used segments are not
-    counted: a multi-GB allocation cannot be served from them."""
-    torch.cuda.empty_cache()
+def _device_budget(dev, release_cache=True):
+    """Device bytes a k-means fit or an index may allocate: free memory once torch has returned its unused cached
+    segments, less a 1 GiB margin for the allocator and other work on the device.  Cached bytes inside partly used
+    segments are not counted: a multi-GB allocation cannot be served from them.  release_cache=False leaves torch's
+    cache alone and counts none of it, a lower bound for callers that only need to know that something fits."""
+    if release_cache:
+        torch.cuda.empty_cache()
     free, _ = torch.cuda.mem_get_info(dev)
     return free - (1 << 30)
 
@@ -1090,6 +1092,82 @@ def pool_descriptors(patch_descs: torch.Tensor, method: str = "gem", gem_p: floa
 
 
 # ------------------------------------------------------------------ retrieval
+_SEARCH_Q_CHUNK = 4096      # queries per anyloc_index_search call: bounds the [n_q, n_db] score matrix
+_STREAM_K_MAX = 4096        # anyloc_index_search_continue merges the running k best in shared memory
+
+
+def _stream_fixed_bytes(P, row, index_bytes, ws_bytes):
+    """device bytes of a streamed search besides its resident pieces: two transfer buffers of P fp32 rows (the copy of
+    one piece overlaps the work on the one before), the blob a piece is prepared into and a P-row search workspace"""
+    return 2 * P * row + index_bytes(P) + ws_bytes(P)
+
+
+def _search_plan(n_db, Dv, n_q_chunk, budget, stage_bytes, index_bytes, ws_bytes):
+    """Where a search over n_db rows of dimension Dv runs, given `budget` free device bytes.  -> None (resident): the
+    index, index_bytes(n_db), and the workspace of an n_q_chunk-query search, ws_bytes(n_db, n_q_chunk), fit.  Else
+    (P, resident): the database is searched in pieces of P rows -- as many as fill a `stage_bytes` staging buffer, fewer
+    when one piece's device buffers would not fit the budget -- and the first `resident` pieces are prepared once and
+    kept on the device; the others are prepared again for every search from the index's host copy."""
+    if index_bytes(n_db) + ws_bytes(n_db, n_q_chunk) <= budget:
+        return None
+    fixed = _piece_fixed(Dv, n_q_chunk, index_bytes, ws_bytes)
+    P = _piece_rows(n_db, Dv, budget, stage_bytes, fixed)
+    n_pieces = -(-n_db // P)
+    return P, int(max(0, min(n_pieces, (budget - fixed(P)) // index_bytes(P))))
+
+
+def _piece_fixed(Dv, n_q_chunk, index_bytes, ws_bytes):
+    """P -> _stream_fixed_bytes of P-row pieces"""
+    return lambda p: _stream_fixed_bytes(p, 4 * Dv, index_bytes, lambda n: ws_bytes(n, n_q_chunk))
+
+
+def _piece_rows(n_db, Dv, budget, stage_bytes, fixed):
+    """rows per piece: as many as fill the staging buffer, fewer when one piece's buffers, fixed(P), would not fit the
+    budget (at least one row)"""
+    P = max(1, min(n_db, stage_bytes // (4 * Dv)))
+    if fixed(P) > budget:
+        lo, hi = 1, P
+        while lo < hi:
+            mid = (lo + hi + 1) // 2
+            lo, hi = (mid, hi) if fixed(mid) <= budget else (lo, mid - 1)
+        P = lo
+    return P
+
+
+def _add_plan(ntotal, n, capacity, held, grow, Dv, n_q_chunk, budget, stage_bytes, index_bytes, ws_bytes):
+    """Where n host rows go when they join an index of `ntotal` rows.  Its blob has room for `capacity` rows and takes
+    `held` device bytes (0: no blob).  Those bytes are already allocated, so `budget` does not include them.  `grow` is
+    the capacity a resident add would reserve (FlatIndex doubles).
+    -> ("resident", capacity to reserve): the rows stay on the device.  Growing the blob holds the old and the new blob
+       at once while the rows are copied, and a search then holds the new blob and its workspace; both peaks must fit.
+       When the doubled blob does not fit, a blob of exactly the rows is tried.
+    -> ("stream", P, resident pieces): a fresh index is planned by _search_plan.  An index that already holds a blob
+       keeps it, since its rows have no host copy.  The blob stays counted as used, and only one piece's buffers must
+       fit beside it; no further pieces are kept."""
+    total = ntotal + n
+    if not held:
+        plan = _search_plan(total, Dv, n_q_chunk, budget, stage_bytes, index_bytes, ws_bytes)
+        return ("resident", total) if plan is None else ("stream",) + plan
+    ws = ws_bytes(total, n_q_chunk)
+    if total <= capacity:
+        if ws <= budget:
+            return "resident", capacity
+    else:
+        for cap in dict.fromkeys((grow, total)):
+            new = index_bytes(cap)
+            if new <= budget and new + ws <= budget + held:
+                return "resident", cap
+    fixed = _piece_fixed(Dv, n_q_chunk, index_bytes, ws_bytes)
+    return "stream", _piece_rows(total, Dv, budget, stage_bytes, fixed), 0
+
+
+def _search_pieces(n_db, n_resident, P):
+    """The pieces of a streamed search, in row order: (first row, rows, resident) -- the n_resident rows kept on the
+    device, then the host rows, each in pieces of at most P rows."""
+    return ([(r, min(P, n_resident - r), True) for r in range(0, n_resident, P)] +
+            [(r, min(P, n_db - r), False) for r in range(n_resident, n_db, P)])
+
+
 TOPK_KERNEL_DESCRIPTION = ("retrieval: gemm_tc3_kernel<true, 0> (wgmma, hi-only: ONE fp16 pass = coarse "
                            "scores with a rigorous per-query error bound) over a prepared database index -> "
                            "topk_candidates_kernel -> topk_rescore_kernel (exact fp32 re-scoring of the candidates from the "
@@ -1100,7 +1178,16 @@ class FlatIndex:
     """GPU stand-in for `faiss.IndexFlatIP` / `IndexFlatL2` as get_top_k_recall drives them (utilities.py:439-450):
     `add(db)` normalises the rows (when `norm_descs`) and stores them once as the operand pairs of the score GEMM
     (anyloc_index_add); `search(qu, k)` is exact -- k best per query, best first, lowest database index first among
-    equal scores.  Rows may be added in chunks (e.g. descriptor batches as they leave the all-gather)."""
+    equal scores.  Rows may be added in chunks (e.g. descriptor batches as they leave the all-gather).
+
+    Host rows whose index (plus the score workspace of a 4096-query search) does not fit the free device memory make
+    the index stream: it keeps its own host copy of the rows that do not fit, as faiss keeps its own, and every search
+    moves them over the link once, piece by piece, merging each piece's k best on the device
+    (anyloc_index_search_continue).  The rows added before streaming began, and as many leading pieces as the device
+    holds, stay prepared on the device.  The answer is the resident search's, bit for bit, except in a query batch where
+    the coarse route's 3-term fallback fires (DESIGN §4.5).  A streamed index answers k <= 4096.  Device rows never make
+    an index stream; device rows added to an index that already streams join its host copy once its device blob is
+    full, as host rows do."""
 
     def __init__(self, d: int, method: str = "cosine", norm_descs: bool = True, capacity: int = 0, device=None):
         if method not in _lib.METRIC:
@@ -1109,6 +1196,9 @@ class FlatIndex:
         self.dp = self.d + (-self.d) % 4            # zero columns change neither norms nor scores
         self.ntotal, self.capacity = 0, 0
         self._blob, self._dev = None, (torch.device(device) if device is not None else None)
+        # streamed index: {"P": rows per piece, "host": [(first row, fp32 rows [m, d] on the host), ...]}; the device
+        # blob then holds rows [0, capacity) and the host copy rows [capacity, ntotal)
+        self._stream = None
         if capacity:
             self._reserve(int(capacity), _lib.require_cuda(self._dev))
 
@@ -1126,10 +1216,13 @@ class FlatIndex:
         self._blob, self.capacity, self._dev = blob, capacity, dev
 
     def reset(self):
-        """faiss `index.reset()`: forget the rows, keep the allocation."""
+        """faiss `index.reset()`: forget the rows, keep the allocation (a streamed index drops its host copy and
+        chooses again at the next add)."""
+        self._stream = None
         if self._blob is not None and self.ntotal:
             self.ntotal = 0
             self._reserve_header_only()
+        self.ntotal = 0
 
     def _reserve_header_only(self):
         with torch.cuda.device(self._dev):
@@ -1142,8 +1235,39 @@ class FlatIndex:
         n = x.shape[0]
         if x.shape[1] != self.d:
             raise ValueError(f"index dimension {self.d}, got rows of {x.shape[1]}")
+        grow = max(self.ntotal + n, 2 * self.capacity if self.ntotal else 0)
+        if self._stream is None and not on_dev and n:
+            # first against the free memory as it is; torch's cache is emptied only when that is not enough
+            plan = self._plan(n, grow, dev, release_cache=False)
+            if plan[0] != "resident":
+                plan = self._plan(n, grow, dev)
+            if plan[0] == "resident":
+                grow = plan[1]
+            else:
+                self._stream = {"P": plan[1], "host": []}
+                if self._blob is None and plan[2]:          # the leading pieces that stay prepared on the device
+                    self._reserve(min(plan[1] * plan[2], n), dev)
+                self._dev = dev
+        if self._stream is not None:
+            m = max(0, min(n, self.capacity - self.ntotal))     # the device blob fills first, the host copy after it
+            if m:
+                self._prepare(x[:m], dev)
+            if n > m:
+                rows = torch.from_numpy(x[m:]) if type(x) == np.ndarray else x[m:].detach()
+                host = torch.empty(tuple(rows.shape), dtype=torch.float32)
+                host.copy_(rows)
+                self._stream["host"].append((self.ntotal + m, host))
+            self.ntotal += n
+            return
         if self.ntotal + n > self.capacity:
-            self._reserve(max(self.ntotal + n, 2 * self.capacity if self.ntotal else 0), dev)
+            self._reserve(grow, dev)
+        self._prepare(x, dev)
+        self.ntotal += n
+
+    def _prepare(self, x, dev):
+        """rows x into the device blob at row ntotal"""
+        on_dev = isinstance(x, torch.Tensor) and x.is_cuda
+        n = x.shape[0]
         lib = _lib.load()
         # host rows are streamed in chunks of <= 1 GiB so that no second full copy of the database sits in HBM
         step = n if on_dev else max(1, (1 << 30) // (self.dp * 4))
@@ -1155,12 +1279,25 @@ class FlatIndex:
                 _lib.check(lib.anyloc_index_add(_lib.ptr(self._blob), self._blob.numel(), self.capacity,
                                                 self.ntotal + i, _lib.ptr(rows), rows.shape[0], self.dp,
                                                 int(self.norm_descs), _lib.stream_ptr()), "anyloc_index_add")
-        self.ntotal += n
+
+    def _plan(self, n, grow, dev, release_cache=True):
+        """_add_plan for n more host rows on `dev`"""
+        lib = _lib.load()
+        norm = int(self.norm_descs)
+        with torch.cuda.device(dev):
+            budget = _device_budget(dev, release_cache=release_cache)
+        held = self._blob.numel() if self._blob is not None else 0
+        return _add_plan(self.ntotal, n, self.capacity, held, grow, self.dp, _SEARCH_Q_CHUNK, budget, _STAGE_BYTES,
+                         lambda m: lib.anyloc_index_bytes(m, self.dp, norm),
+                         lambda m, q: lib.anyloc_index_search_workspace_bytes(m, q, self.dp, norm))
 
     def add_at(self, x: torch.Tensor, row_offset: int):
         """Prepare device rows `x` into rows [row_offset, row_offset + len(x)) of the (already reserved) index -- for
         callers that receive the database out of order, e.g. chunk by chunk from an all-gather (dist.py).  `ntotal`
         becomes the highest row written; the caller must fill every row below it before searching."""
+        if self._stream is not None:
+            raise ValueError("add_at on an index that streams host rows: reserve the capacity and add device rows, or "
+                             "use add()")
         n = x.shape[0]
         if self._blob is None or row_offset < 0 or row_offset + n > self.capacity:
             raise ValueError(f"rows [{row_offset}, {row_offset + n}) outside the reserved capacity {self.capacity}")
@@ -1173,14 +1310,24 @@ class FlatIndex:
                        "anyloc_index_add")
         self.ntotal = max(self.ntotal, row_offset + n)
 
-    def search(self, qu: Union[np.ndarray, torch.Tensor], k: int, n_q_chunk: int = 4096):
+    def search(self, qu: Union[np.ndarray, torch.Tensor], k: int, n_q_chunk: int = _SEARCH_Q_CHUNK):
+        """-> (dist, idx) [n_q, k], on the device for device queries, else on the host.  The queries are searched
+        n_q_chunk at a time.  The decision to stream (add) budgets the workspace of the default chunk.  A larger
+        n_q_chunk, and the device copy of the queries (n_q x d x 4 bytes) with the outputs, come out of the 1 GiB margin
+        of that decision; a streamed search of many queries may need a smaller n_q_chunk or fewer queries per call.
+        A streamed index answers k <= 4096 (the running k best are merged in shared memory)."""
         if self.ntotal == 0:
             raise ValueError("search on an empty index")
+        if self._stream is not None and k > _STREAM_K_MAX:
+            raise ValueError(f"k={k}: an index that streams host rows answers k <= {_STREAM_K_MAX}")
         on_dev = isinstance(qu, torch.Tensor) and qu.is_cuda
         dev = self._dev
         q = _as_device_f32(qu, dev)
         if self.dp != self.d:
             q = torch.nn.functional.pad(q, (0, self.dp - self.d))
+        if self._stream is not None:
+            dist, idx = self._search_streamed(q, k, n_q_chunk)
+            return (dist, idx) if on_dev else (dist.cpu(), idx.cpu())
         lib = _lib.load()
         n_q = q.shape[0]
         dist = torch.empty(n_q, k, device=dev, dtype=torch.float32)
@@ -1197,15 +1344,93 @@ class FlatIndex:
                 _lib.check(rc, "anyloc_index_search")
         return (dist, idx) if on_dev else (dist.cpu(), idx.cpu())
 
+    def _gather(self, dst, r0, m):
+        """rows [r0, r0 + m) of the host copy -> dst[:m, :d]"""
+        for first, rows in self._stream["host"]:
+            lo, hi = max(r0, first), min(r0 + m, first + rows.shape[0])
+            if lo < hi:
+                dst[lo - r0:hi - r0, :self.d].copy_(rows[lo - first:hi - first])
+
+    def _search_streamed(self, q, k, n_q_chunk):
+        """The k best of every query over the pieces of _search_pieces, in row order.  Database pieces are the outer
+        loop and query chunks the inner one, so each host row crosses the link once per search.  A host piece is
+        gathered into one of two pinned staging buffers and copied to the device on a side stream while the device
+        prepares and searches the piece before it."""
+        lib = _lib.load()
+        dev, dp, norm, metric = self._dev, self.dp, int(self.norm_descs), _lib.METRIC[self.method]
+        P, n_q = self._stream["P"], q.shape[0]
+        pieces = _search_pieces(self.ntotal, min(self.ntotal, self.capacity), P)
+        host_pieces = [p for p in pieces if not p[2]]
+        pad = float("inf") if self.method == "l2" else -float("inf")
+        with torch.cuda.device(dev):
+            dist = torch.full((n_q, k), pad, device=dev, dtype=torch.float32)     # the empty running list
+            idx = torch.full((n_q, k), -1, device=dev, dtype=torch.int64)
+            ws = _lib.workspaces.get(dev, lib.anyloc_index_search_workspace_bytes(
+                min(P, self.ntotal), min(n_q_chunk, n_q), dp, norm), "topk")
+            cs = torch.cuda.current_stream()
+            if host_pieces:
+                cap = max(m for _, m, _ in host_pieces)
+                blob = torch.empty(lib.anyloc_index_bytes(cap, dp, norm), dtype=torch.uint8, device=dev)
+                raw = [torch.empty(cap, dp, device=dev) for _ in range(2)]
+                host = [torch.empty(cap, dp, pin_memory=True) for _ in range(2)]
+                if dp != self.d:
+                    for h in host:
+                        h[:, self.d:] = 0
+                xs = torch.cuda.Stream()
+                copied, freed = [None, None], [None, None]
+                todo, staged = iter(host_pieces), []
+
+                def stage():
+                    """gather the next host piece into a staging buffer and queue its copy to the device"""
+                    p = next(todo, None)
+                    if p is None:
+                        return
+                    s = len(staged) & 1
+                    if copied[s] is not None:
+                        copied[s].synchronize()                     # the staging buffer's previous copy is done
+                    self._gather(host[s], p[0], p[1])
+                    with torch.cuda.stream(xs):
+                        if freed[s] is not None:
+                            xs.wait_event(freed[s])
+                        raw[s][:p[1]].copy_(host[s][:p[1]], non_blocking=True)
+                        copied[s] = torch.cuda.Event()
+                        copied[s].record(xs)
+                    staged.append((s, copied[s]))
+
+                if not pieces[0][2]:
+                    stage()
+            for j, (r0, m, resident) in enumerate(pieces):
+                if resident:
+                    src, src_cap, first = self._blob, self.capacity, r0
+                else:
+                    s, ev = staged[j - (len(pieces) - len(host_pieces))]
+                    cs.wait_event(ev)
+                    _lib.check(lib.anyloc_index_init(_lib.ptr(blob), blob.numel(), cap, dp, norm, _lib.stream_ptr()),
+                               "anyloc_index_init")
+                    _lib.check(lib.anyloc_index_add(_lib.ptr(blob), blob.numel(), cap, 0, _lib.ptr(raw[s]), m, dp,
+                                                    norm, _lib.stream_ptr()), "anyloc_index_add")
+                    freed[s] = torch.cuda.Event()
+                    freed[s].record(cs)
+                    src, src_cap, first = blob, cap, 0
+                for i in range(0, n_q, n_q_chunk):
+                    c = min(n_q_chunk, n_q - i)
+                    _lib.check(lib.anyloc_index_search_continue(
+                        _lib.ptr(src), src.numel(), src_cap, first, m, r0, self.ntotal, _lib.ptr(q[i:i + c]), c, dp, k,
+                        metric, norm, _lib.ptr(dist[i:i + c]), _lib.ptr(idx[i:i + c]), _lib.ptr(ws), ws.numel(),
+                        _lib.stream_ptr()), "anyloc_index_search_continue")
+                if host_pieces and (not resident or j + 1 == len(pieces) - len(host_pieces)):
+                    stage()                 # the gather of the next host piece overlaps the work just queued
+        return dist, idx
+
 
 def top_k_search(db: torch.Tensor, qu: torch.Tensor, k: int, method: str = "cosine",
                  norm_descs: bool = True) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact k-nearest search on the GPU (the `faiss.IndexFlatIP/L2` `add` + `search` of get_top_k_recall,
-    utilities.py:435-450).  Device tensors in, device tensors out."""
+    utilities.py:435-450).  Device tensors out; a host database larger than the device streams (FlatIndex)."""
     if method not in _lib.METRIC:
         raise NotImplementedError(f"Method: {method}")
-    dev = _lib.require_cuda(db.device)
-    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0], device=dev)
+    dev = _lib.require_cuda(db.device if db.is_cuda else None)
+    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if db.is_cuda else 0, device=dev)
     index.add(db)
     return index.search(qu.to(dev), k)
 
@@ -1225,7 +1450,8 @@ def get_top_k_recall(top_k: List[int], db: torch.Tensor, qu: torch.Tensor, gt_po
         qu = qu.unsqueeze(0)
     on_dev = db.is_cuda
     dev = _lib.require_cuda(db.device if on_dev else None)
-    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0], device=dev)
+    # host rows: add() reserves the index once it knows it fits, and streams the search when it does not
+    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if on_dev else 0, device=dev)
     index.add(db)                                   # host rows are streamed in <= 1 GiB chunks
     distances, indices = index.search(_as_device_f32(qu, dev), max(top_k))
     idx_host = indices.cpu().numpy()

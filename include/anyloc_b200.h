@@ -210,6 +210,18 @@ size_t anyloc_index_search_workspace_bytes(int64_t n_db, int n_q, int Dv, int no
 int anyloc_index_search(const void* index, size_t index_bytes, int64_t capacity, int64_t n_db, const float* qu,
                         int n_q, int Dv, int k, int metric, int normalize, float* dist, int64_t* idx, void* ws,
                         size_t ws_bytes, void* stream);
+/* Continuation form, for a database searched piece by piece (e.g. streamed from host memory): rows
+ * [first, first + n_rows) of the blob are the global rows [row0, row0 + n_rows) of a database of n_total rows.  Their
+ * k best are merged, in place and on the device, into the running list dist / idx [n_q, k] (global indices; score
+ * descending, lowest index first).  A fresh list is -1 / -inf (IP) or -1 / +inf (L2) everywhere.  The route (coarse or
+ * exact, see above) is chosen from n_total, not n_rows, and each route's score of a (query, row) pair does not depend
+ * on where the row sits, so pieces fed in row order give what anyloc_index_search over the whole database gives --
+ * except where the coarse route's 3-term fallback fires (it answers per piece).  k <= 4096.  Workspace:
+ * anyloc_index_search_workspace_bytes(n_rows, n_q, Dv, normalize). */
+int anyloc_index_search_continue(const void* index, size_t index_bytes, int64_t capacity, int64_t first,
+                                 int64_t n_rows, int64_t row0, int64_t n_total, const float* qu, int n_q, int Dv, int k,
+                                 int metric, int normalize, float* dist, int64_t* idx, void* ws, size_t ws_bytes,
+                                 void* stream);
 
 /* ------------------------------------------------------------- collective
  * The one data-path collective of the pipeline (BASELINE config 4): all-gather of the [n_loc, Dv] fp32 descriptors of
