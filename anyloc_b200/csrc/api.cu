@@ -54,12 +54,9 @@ int device_sm_count() {
 int gemm_simt_launch(const void*, const void*, int, const void*, const void*, int, int, int, int,
                      const EpiParams&, bool f16, cudaStream_t);
 int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int, int, int, int,
-                   const EpiParams&, bool f16, cudaStream_t);
+                   const EpiParams&, int fmt, cudaStream_t);
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
-                       int ldb, int M, int N, int K, const EpiParams& ep, bool f16);
-int gemm_tc_bf16_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
-int gemm_tc_f16x1_launch(const void*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
-int gemm_tc_fp8_launch(const void*, const float*, int, const void*, int, int, int, int, const EpiParams&, cudaStream_t);
+                       int ldb, int M, int N, int K, const EpiParams& ep, int fmt);
 // vit_ops.cu / attention.cu
 int launch_split(const float*, float*, float*, size_t, cudaStream_t);
 int launch_split_f16(const float*, void*, void*, size_t, float, cudaStream_t);
@@ -83,49 +80,39 @@ int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, i
 int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
                    cudaStream_t);
 
-// fmt: ANYLOC_PAIR_* of the operands.  Single bf16 and single fp16 are tensor-core-only formats: they run the wgmma
-// kernel at every M (no SIMT route, so a row's result never depends on how many rows share the call) and refuse the
-// SIMT engine.
+// fmt: ANYLOC_PAIR_* of the operands.  The single formats run on the tensor cores only: they run the wgmma kernel at
+// every M (no SIMT route, so a row's result never depends on how many rows share the call) and refuse the SIMT
+// engine.  Single e4m3's a_lo holds A's fp32 row scales.
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                          int ldb, int M, int N, int K, const EpiParams& ep, int engine, int fmt, cudaStream_t st) {
   if (M == 0 || N == 0) return ANYLOC_OK;
-  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1) {
-    if (engine == ANYLOC_GEMM_SIMT || a_lo || b_lo ||
-        !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, true)) {
-      set_error("gemm: the %s format runs on the tensor-core engine only, with 16-byte aligned operands, "
-                "K, lda and ldb multiples of 8 and no lo operands (M=%d N=%d K=%d lda=%d ldb=%d engine=%d)",
-                fmt == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16", M, N, K, lda, ldb, engine);
+  const FormatInfo& f = format_info(fmt);
+  const double flops = 2.0 * M * N * K;
+  if (f.tc_only) {
+    const bool a_lo_ok = f.row_scales ? a_lo && (reinterpret_cast<uintptr_t>(a_lo) & 3) == 0 : !a_lo;
+    if (engine == ANYLOC_GEMM_SIMT || !a_lo_ok || b_lo ||
+        !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, fmt)) {
+      set_error("gemm: the %s format runs on the tensor-core engine only, with 16-byte aligned operands, K, lda and "
+                "ldb multiples of %d%s (M=%d N=%d K=%d lda=%d ldb=%d engine=%d)", f.name, 16 / f.esz,
+                f.row_scales ? ", A's row scales and no B lo operand" : " and no lo operands", M, N, K, lda, ldb,
+                engine);
       return ANYLOC_ERR_UNSUPPORTED;
     }
-    ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
-    if (fmt == ANYLOC_PAIR_F16X1) return gemm_tc_f16x1_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
-    return gemm_tc_bf16_launch(a_hi, lda, b_hi, ldb, M, N, K, ep, st);
+    ProfScope ps(PC_GEMM_TC, st, flops);
+    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, nullptr, ldb, M, N, K, ep, fmt, st);
   }
-  if (fmt == ANYLOC_PAIR_FP8) {     // a_lo: A's fp32 row scales
-    if (engine == ANYLOC_GEMM_SIMT || !a_lo || b_lo || (reinterpret_cast<uintptr_t>(a_lo) & 3) || K % 16 ||
-        lda % 16 || ldb % 16 || !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, true)) {
-      set_error("gemm: the single-e4m3 format runs on the tensor-core engine only, with 16-byte aligned operands, "
-                "K, lda and ldb multiples of 16, A's row scales and no B lo operand (M=%d N=%d K=%d lda=%d ldb=%d "
-                "engine=%d)", M, N, K, lda, ldb, engine);
-      return ANYLOC_ERR_UNSUPPORTED;
-    }
-    ProfScope ps(PC_GEMM_TC, st, 2.0 * M * N * K);
-    return gemm_tc_fp8_launch(a_hi, (const float*)a_lo, lda, b_hi, ldb, M, N, K, ep, st);
-  }
-  const bool f16 = fmt == ANYLOC_PAIR_F16;
-  bool tc_ok = gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16);
+  bool tc_ok = gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt);
   if (engine == ANYLOC_GEMM_TC3 && !tc_ok) {
     set_error("gemm: tensor-core engine does not support this shape/alignment (M=%d N=%d K=%d lda=%d ldb=%d f16=%d)",
-              M, N, K, lda, ldb, (int)f16);
+              M, N, K, lda, ldb, (int)(fmt == ANYLOC_PAIR_F16));
     return ANYLOC_ERR_UNSUPPORTED;
   }
-  const double flops = 2.0 * M * N * K;
   if (engine == ANYLOC_GEMM_TC3 || (engine == ANYLOC_GEMM_AUTO && tc_ok && M >= 32)) {
     ProfScope ps(PC_GEMM_TC, st, flops);
-    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16, st);
+    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt, st);
   }
   ProfScope ps(PC_GEMM_SIMT, st, flops);
-  return gemm_simt_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16, st);
+  return gemm_simt_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt == ANYLOC_PAIR_F16, st);
 }
 
 }  // namespace anyloc
@@ -174,27 +161,23 @@ extern "C" int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const
   ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_F16X1 && out_dtype != ANYLOC_PAIR_FP8,
                  "gemm_nt: bad out_dtype %d", out_dtype);
   ANYLOC_REQUIRE(epilogue >= ANYLOC_EPI_BIAS && epilogue <= ANYLOC_EPI_LS_RESID, "gemm_nt: bad epilogue %d", epilogue);
-  const bool bf16 = in_dtype == ANYLOC_PAIR_BF16, fp8 = in_dtype == ANYLOC_PAIR_FP8;
-  const bool h1 = in_dtype == ANYLOC_PAIR_F16X1;
-  ANYLOC_REQUIRE((bf16 || fp8) == (out_dtype == ANYLOC_PAIR_BF16), "gemm_nt: single bf16 is the output format of the "
-                 "single bf16 and e4m3 inputs, and of no other (in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
-  ANYLOC_REQUIRE(h1 == (out_dtype == ANYLOC_PAIR_F16X1), "gemm_nt: single fp16 is the output format of the single "
-                 "fp16 inputs, and of no other (in_dtype=%d out_dtype=%d)", in_dtype, out_dtype);
-  if (fp8)
-    ANYLOC_REQUIRE(a_lo && !b_lo && !out_lo, "gemm_nt: e4m3 inputs take A's row scales in a_lo, no b_lo and no out_lo");
-  else if (bf16)
-    ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-bf16 format has no lo arrays (a_lo, b_lo, out_lo "
-                   "must be NULL)");
-  else if (h1)
-    ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the single-fp16 format has no lo arrays (a_lo, b_lo, out_lo "
-                   "must be NULL)");
+  const FormatInfo& f = format_info(in_dtype);
+  ANYLOC_REQUIRE(f.lo ? format_info(out_dtype).lo : out_dtype == f.out, "gemm_nt: %s inputs write %s outputs "
+                 "(in_dtype=%d out_dtype=%d)", f.name, f.lo ? "tf32-pair or fp16-pair" : format_info(f.out).name,
+                 in_dtype, out_dtype);
+  if (f.row_scales)
+    ANYLOC_REQUIRE(a_lo && !b_lo && !out_lo, "gemm_nt: %s inputs take A's row scales in a_lo, no b_lo and no out_lo",
+                   f.name);
+  else if (!f.lo)
+    ANYLOC_REQUIRE(!a_lo && !b_lo && !out_lo, "gemm_nt: the %s format has no lo arrays (a_lo, b_lo, out_lo must be "
+                   "NULL)", f.name);
   else if (epilogue == ANYLOC_EPI_BIAS_SPLIT || epilogue == ANYLOC_EPI_GELU_SPLIT || epilogue == ANYLOC_EPI_SWIGLU_SPLIT)
     ANYLOC_REQUIRE(out_lo, "gemm_nt: split epilogue needs out_lo");
   if (epilogue == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_REQUIRE(N % 2 == 0, "gemm_nt: swiglu needs even N");
   if (epilogue == ANYLOC_EPI_LS_RESID) ANYLOC_REQUIRE(gamma && resid, "gemm_nt: LS_RESID needs gamma and resid");
   EpiParams ep{epilogue, bias, gamma, resid, (float*)out, (float*)out_lo, ldo};
   ep.alpha = alpha;
-  ep.out_f16 = out_dtype == ANYLOC_PAIR_F16;
+  ep.out_fmt = out_dtype;
   return gemm_dispatch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, engine, in_dtype, (cudaStream_t)stream);
 }
 
@@ -206,15 +189,15 @@ extern "C" int anyloc_gemm_nt_gated(const void* a_hi, const void* a_lo, int lda,
   ep.alpha = alpha;
   ep.gate = gate;
   cudaStream_t st = (cudaStream_t)stream;
-  const bool f16 = in_dtype == ANYLOC_PAIR_F16;
+  const int fmt = in_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32;
   if (gate) {      // conditional fallback: tensor-core engine only (its kernels test the device flag), nothing recorded
-    if (!gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16)) {
+    if (!gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt)) {
       set_error("gemm_nt_gated: shape outside the tensor-core engine's contract");
       return ANYLOC_ERR_UNSUPPORTED;
     }
-    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, f16, st);
+    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt, st);
   }
-  return gemm_dispatch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, ANYLOC_GEMM_AUTO, f16, st);
+  return gemm_dispatch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, ANYLOC_GEMM_AUTO, fmt, st);
 }
 
 extern "C" int anyloc_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stream) {
@@ -237,25 +220,22 @@ extern "C" int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream
 
 extern "C" int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M, int D,
                                       float eps, void* y_hi, void* y_lo, int out_dtype, void* stream) {
-  const bool bf16 = out_dtype == ANYLOC_PAIR_BF16, h1 = out_dtype == ANYLOC_PAIR_F16X1;
-  ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || bf16 || h1), "layernorm: null pointer");
-  ANYLOC_REQUIRE(!(bf16 && y_lo), "layernorm: the single-bf16 output has no lo array (y_lo must be NULL)");
-  ANYLOC_REQUIRE(!(h1 && y_lo), "layernorm: the single-fp16 output has no lo array (y_lo must be NULL)");
+  const FormatInfo& f = format_info(out_dtype);
+  const bool has_lo = f.lo || f.row_scales;      // y_lo: the lo array, or e4m3's row scales
+  ANYLOC_REQUIRE(x && w && b && y_hi && (y_lo || !has_lo), "layernorm: null pointer");
+  ANYLOC_REQUIRE(has_lo || !y_lo, "layernorm: the %s output has no lo array (y_lo must be NULL)", f.name);
   ANYLOC_REQUIRE(M >= 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm: M=%d D=%d (M >= 0, D a multiple of 4 in "
                  "[4, 2048])", M, D);
-  // float4 loads of x, w and b; y_hi is stored 4 elements at a time (16, 8 or 4 bytes); fp8's y_lo holds fp32 scales
-  const uintptr_t lo_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
-  const uintptr_t hi_align = out_dtype == ANYLOC_PAIR_FP8 ? 3 : bf16 || h1 || out_dtype == ANYLOC_PAIR_F16 ? 7 : 15;
+  // float4 loads of x, w and b; y_hi and y_lo are stored 4 elements at a time (16, 8 or 4 bytes); e4m3's y_lo holds
+  // fp32 scales
+  const uintptr_t hi_align = 4 * f.esz - 1, lo_align = f.row_scales ? 3 : hi_align;
   ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(b)) &
                   15) == 0 && (reinterpret_cast<uintptr_t>(y_hi) & hi_align) == 0 &&
                  (reinterpret_cast<uintptr_t>(y_lo) & lo_align) == 0,
                  "layernorm: x, w and b must be 16-byte aligned, y_hi and y_lo aligned to 4 of their elements (fp8: "
                  "y_hi 4-byte, y_lo 4-byte)");
   if (M == 0) return ANYLOC_OK;
-  return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo,
-                          bf16 ? ANYLOC_PAIR_BF16 : h1 ? ANYLOC_PAIR_F16X1 : out_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_FP8
-                          : out_dtype == ANYLOC_PAIR_F16 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32,
-                          (cudaStream_t)stream);
+  return launch_layernorm(x, w, b, M, D, eps, y_hi, y_lo, out_dtype, (cudaStream_t)stream);
 }
 
 extern "C" float anyloc_fp8_scale(float amax) { return pow2f(fp8_scale_exp(amax)); }
@@ -297,13 +277,13 @@ static int attention_dispatch(const float* qkv_hi, const float* qkv_lo, int B, i
 
 extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                                 void* o_hi, void* o_lo, int out_dtype, int engine, void* stream) {
-  if (out_dtype == ANYLOC_PAIR_BF16 || out_dtype == ANYLOC_PAIR_F16X1) {   // single in and out: the qkv epilogue's
-    const char* name = out_dtype == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16";           // output format
+  const FormatInfo& f = format_info(out_dtype);
+  if (!f.lo && f.out == out_dtype) {     // single in and out: a format the qkv epilogue writes
     ANYLOC_REQUIRE(qkv_hi && o_hi, "attention: null pointer");
-    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", name);
+    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", f.name);
     ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
     if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0) {
-      set_error("attention: the %s format runs on the tensor-core engine only, with a 16-byte aligned qkv", name);
+      set_error("attention: the %s format runs on the tensor-core engine only, with a 16-byte aligned qkv", f.name);
       return ANYLOC_ERR_UNSUPPORTED;
     }
     if (B == 0 || T == 0) return ANYLOC_OK;
@@ -339,11 +319,11 @@ extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, i
                                        void* stream) {
   ANYLOC_REQUIRE(fmt == ANYLOC_PAIR_TF32 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 ||
                  fmt == ANYLOC_PAIR_F16X1, "attention_varlen: bad fmt %d", fmt);
-  const bool single = fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1;
+  const FormatInfo& f = format_info(fmt);
   ANYLOC_REQUIRE(qkv_hi && o_hi && row0 && len, "attention_varlen: null pointer");
-  if (single)
+  if (!f.lo)
     ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention_varlen: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)",
-                   fmt == ANYLOC_PAIR_BF16 ? "single-bf16" : "single-fp16");
+                   f.name);
   else
     ANYLOC_REQUIRE(qkv_lo && o_lo, "attention_varlen: the pair formats need qkv_lo and o_lo");
   ANYLOC_REQUIRE(n >= 1 && n <= ANYLOC_VIT_VARLEN_MAX_B, "attention_varlen: n=%d out of range [1,%d]", n,
@@ -392,48 +372,40 @@ struct VitBuffers {
   void* h8;         // single e4m3: the FFN hidden layer quantised [M, H] and its row scales [M] (else null)
   float* h8_s;
 };
-// n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  The single-bf16 format carves no
-// lo buffers and 2-byte GEMM inputs: pa [n_patch, Kp], y [M, D], qkv [M, 3D] (which also holds the fp32 [M, D] output
-// of a lone q/k/v tap), h [M, hidden] as bf16.
-// The single-fp16 format carves the same buffers as single bf16, of fp16.
-// The single-e4m3 format carves the bf16 patch rows as above, e4m3 LayerNorm rows y [M, D] with their row scales
-// [M], the bf16 qkv [M, 3D], the bf16 hidden layer h [M, H] (which also holds the attention's bf16 output [M, D]) and
-// the e4m3 hidden layer h8 [M, H] with its row scales [M].
+// n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  Each buffer is sized by the format
+// that fills it (format_info): the patch rows pa [n_patch, Kp] in the patch embedding's format, the LayerNorm rows y
+// [M, D] in pair_dtype, q, k, v [M, 3D] (which also hold the fp32 [M, D] output of a lone q/k/v tap) and the hidden
+// layer h [M, H] in the SPLIT output format; lo arrays where the format has them.  The pair formats' buffers hold fp32
+// words, so that either pair format fits (the SIMT attention of the fp16-pair precision takes tf32 pairs).  Single
+// e4m3 adds the LayerNorm rows' scales [M] in y_lo and the e4m3 hidden layer h8 [M, H] with its row scales [M], and its
+// attention writes its bf16 output [M, D] into h.
 size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
                  VitBuffers* out) {
-  const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch);
-  const bool bf16 = c->pair_dtype == ANYLOC_PAIR_BF16 || c->pair_dtype == ANYLOC_PAIR_F16X1;   // one 2-byte array
-  const bool fp8 = c->pair_dtype == ANYLOC_PAIR_FP8;
+  const int D = c->embed_dim, Kp = anyloc_vit_patch_k(c->patch), H = c->ffn_hidden;
+  const FormatInfo& f = format_info(c->pair_dtype);
+  const FormatInfo &pf = format_info(f.patch), &of = format_info(f.out);
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  // n elements of fi's arrays: hi, and lo (or null)
+  auto take = [&](const FormatInfo& fi, size_t n, float** hi, float** lo) {
+    const size_t esz = fi.lo ? sizeof(float) : fi.esz;
+    *hi = (float*)w.take<uint8_t>(n * esz);
+    *lo = fi.lo ? (float*)w.take<uint8_t>(n * esz) : nullptr;
+  };
   VitBuffers b;
-  b.h8 = nullptr; b.h8_s = nullptr;
-  if (fp8) {
-    b.pa_hi = (float*)w.take<uint16_t>(n_patch * Kp); b.pa_lo = nullptr;
-    b.ptmp = w.take<float>(n_patch * D);
-    b.x = w.take<float>(M * D);
-    b.y_hi = (float*)w.take<uint8_t>(M * D); b.y_lo = w.take<float>(M);
-    b.qkv = (float*)w.take<uint16_t>(M * 3 * D); b.qkv_lo = nullptr;
-    b.h_hi = (float*)w.take<uint16_t>(M * c->ffn_hidden); b.h_lo = nullptr;
-    b.h8 = w.take<uint8_t>(M * c->ffn_hidden); b.h8_s = w.take<float>(M);
-  } else if (bf16) {
-    b.pa_hi = (float*)w.take<uint16_t>(n_patch * Kp); b.pa_lo = nullptr;
-    b.ptmp = w.take<float>(n_patch * D);
-    b.x = w.take<float>(M * D);
-    b.y_hi = (float*)w.take<uint16_t>(M * D); b.y_lo = nullptr;
-    b.qkv = (float*)w.take<uint16_t>(M * 3 * D); b.qkv_lo = nullptr;
-    b.h_hi = (float*)w.take<uint16_t>(M * c->ffn_hidden); b.h_lo = nullptr;
-  } else {
-    b.pa_hi = w.take<float>(n_patch * Kp); b.pa_lo = w.take<float>(n_patch * Kp);
-    b.ptmp = w.take<float>(n_patch * D);
-    b.x = w.take<float>(M * D);
-    b.y_hi = w.take<float>(M * D); b.y_lo = w.take<float>(M * D);
-    b.qkv = w.take<float>(M * 3 * D); b.qkv_lo = w.take<float>(M * 3 * D);
-    b.h_hi = w.take<float>(M * c->ffn_hidden); b.h_lo = w.take<float>(M * c->ffn_hidden);
-  }
+  take(pf, n_patch * Kp, &b.pa_hi, &b.pa_lo);
+  b.ptmp = w.take<float>(n_patch * D);
+  b.x = w.take<float>(M * D);
+  take(f, M * D, &b.y_hi, &b.y_lo);
+  if (f.row_scales) b.y_lo = w.take<float>(M);
+  take(of, M * 3 * D, &b.qkv, &b.qkv_lo);
+  take(of, M * H, &b.h_hi, &b.h_lo);
+  b.h8 = f.row_scales ? w.take<uint8_t>(M * H) : nullptr;
+  b.h8_s = f.row_scales ? w.take<float>(M) : nullptr;
   b.qkv32 = qkv32 ? w.take<float>(M * 3 * D) : nullptr;
   if (out) *out = b;
   if (ws && (!b.pa_hi || !b.ptmp || !b.x || !b.y_hi || !b.qkv || !b.h_hi || (qkv32 && !b.qkv32) ||
-             (fp8 && (!b.y_lo || !b.h8 || !b.h8_s)) || (!bf16 && !fp8 && (!b.pa_lo || !b.y_lo || !b.qkv_lo || !b.h_lo))))
+             (f.row_scales && (!b.y_lo || !b.h8 || !b.h8_s)) ||
+             (f.lo && (!b.pa_lo || !b.y_lo || !b.qkv_lo || !b.h_lo))))
     return 0;
   return w.off;
 }
@@ -467,28 +439,23 @@ bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeight
   }
   return true;
 }
-// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for single-bf16, single-fp16 or
-// e4m3 weights with a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for those formats on the SIMT engine
+// The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for a single format's weights with
+// a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for a single format on the SIMT engine
 int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int engine) {
-  const bool fp8 = cfg->pair_dtype == ANYLOC_PAIR_FP8, h1 = cfg->pair_dtype == ANYLOC_PAIR_F16X1;
-  if (cfg->pair_dtype != ANYLOC_PAIR_BF16 && !fp8 && !h1) return ANYLOC_OK;
+  const FormatInfo& f = format_info(cfg->pair_dtype);
+  if (!f.tc_only) return ANYLOC_OK;
   bool lo = w->patch_w_lo != nullptr;
   for (int l = 0; l < cfg->depth && w->blocks; ++l) {
     const AnylocVitBlock& b = w->blocks[l];
     lo = lo || b.qkv_w_lo || b.proj_w_lo || b.in_w_lo || b.out_w_lo;
   }
   if (lo) {
-    set_error(fp8 ? "%s: pair_dtype ANYLOC_PAIR_FP8 takes e4m3 block weights and bf16 patch weights; every *_w_lo must "
-                    "be NULL"
-              : h1  ? "%s: pair_dtype ANYLOC_PAIR_F16X1 takes single fp16 weights; every *_w_lo must be NULL"
-                    : "%s: pair_dtype ANYLOC_PAIR_BF16 takes single bf16 weights; every *_w_lo must be NULL", fn);
+    set_error("%s: pair_dtype %s takes %s block weights and %s patch weights; every *_w_lo must be NULL", fn, f.id,
+              f.name, format_info(f.patch).name);
     return ANYLOC_ERR_ARG;
   }
   if (engine == ANYLOC_GEMM_SIMT) {
-    set_error(fp8 ? "%s: the single-e4m3 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)"
-              : h1  ? "%s: the single-fp16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)"
-                    : "%s: the single-bf16 format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)",
-              fn);
+    set_error("%s: the %s format runs on the tensor-core engine only (gemm_engine auto or tc3, not simt)", fn, f.name);
     return ANYLOC_ERR_UNSUPPORTED;
   }
   return ANYLOC_OK;
@@ -545,23 +512,21 @@ static int facet_out(const VitSeqs& sq, int M, const float* src, int64_t ld, int
   return launch_facet_out(src, sq.B, sq.T, ld, 0, D, tp.use_cls, tp.norm_descs, out, st);
 }
 
-// the fp32 qkv rows of layer l in bf.qkv32 -> the facets of l the plan asks for and, when `pairs`, the attention's
-// operands in bf.qkv / bf.qkv_lo (single bf16 in bf.qkv for the bf16 and e4m3 formats, single fp16 for the single-fp16
-// format, else fp16 pairs when f16_attn, else tf32 pairs)
+// the fp32 qkv rows of layer l in bf.qkv32 -> the facets of l the plan asks for and, unless attn_fmt is FMT_NONE, the
+// attention's operands in bf.qkv / bf.qkv_lo in the format attn_fmt
 static int qkv_tap(const AnylocVitCfg* c, const VitBuffers& bf, int M, const VitSeqs& sq, const TapPlan& tp, int l,
-                   bool pairs, bool f16_attn, cudaStream_t st) {
+                   int attn_fmt, cudaStream_t st) {
   const int D = c->embed_dim, m = tp.mask[l];
   const QkvTapOuts o{{(m & 1) ? tp.out[l][0] : nullptr, (m & 2) ? tp.out[l][1] : nullptr,
                       (m & 4) ? tp.out[l][2] : nullptr}};
-  const bool single = c->pair_dtype == ANYLOC_PAIR_BF16 || c->pair_dtype == ANYLOC_PAIR_FP8;   // bf16 attention
-  const bool h1 = c->pair_dtype == ANYLOC_PAIR_F16X1;
-  const int pair = pairs ? (single ? 3 : h1 ? 4 : f16_attn ? 2 : 1) : 0;
+  const bool pairs = attn_fmt != FMT_NONE;
+  const FormatInfo& f = format_info(attn_fmt);
   const double rows_out = (double)M - (tp.use_cls ? 0 : sq.B);
-  const double bytes = 12.0 * M * D + (pair ? (pair >= 3 ? 6.0 : pair == 2 ? 12.0 : 24.0) * M * D : 0.0) +
+  const double bytes = 12.0 * M * D + (pairs ? 3.0 * f.esz * (f.lo ? 2 : 1) * M * D : 0.0) +
                        4.0 * rows_out * D * popcount3(m);
   ProfScope ps(PC_VIT_MISC, st, bytes);
-  return launch_qkv_tap(bf.qkv32, M, sq.T, sq.img, D, pair, pairs ? bf.qkv : nullptr, pairs ? bf.qkv_lo : nullptr, o,
-                        tp.use_cls, tp.norm_descs, st);
+  return launch_qkv_tap(bf.qkv32, M, sq.T, sq.img, D, attn_fmt, pairs ? bf.qkv : nullptr, pairs ? bf.qkv_lo : nullptr,
+                        o, tp.use_cls, tp.norm_descs, st);
 }
 
 // One transformer block over the M token rows in bf.x, in place.  With tp (layer l has q/k/v taps) the qkv GEMM
@@ -570,43 +535,41 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
                      int engine, cudaStream_t st, const TapPlan* tp = nullptr, int l = 0) {
   const int D = c->embed_dim, Hf = c->ffn_hidden;
   const int fmt = c->pair_dtype;
-  const bool f16 = fmt == ANYLOC_PAIR_F16, bf16 = fmt == ANYLOC_PAIR_BF16, fp8 = fmt == ANYLOC_PAIR_FP8;
-  const bool h1 = fmt == ANYLOC_PAIR_F16X1;
+  const FormatInfo& f = format_info(fmt);
   int rc;
-  const double ln_bytes = (fp8 ? 5.0 : bf16 || h1 ? 6.0 : f16 ? 8.0 : 12.0) * M * D;
+  const double ln_bytes = (4.0 + f.esz * (f.lo ? 2 : 1)) * M * D;
   { ProfScope ps(PC_LAYERNORM, st, ln_bytes);
     if ((rc = launch_layernorm(bf.x, wb.ln1_w, wb.ln1_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
-  // q, k and v leave the qkv GEMM row-major through the plain split epilogue; for the tensor-core attention in the
-  // fp16-pair precision they are fp16 pairs of 8*x, the attention kernel's operand format
-  const bool f16_attn = engine != ANYLOC_GEMM_SIMT && f16;
+  // q, k and v leave the qkv GEMM row-major through the plain split epilogue, in the attention's operand format: the
+  // SPLIT output format, except that the SIMT attention of the fp16-pair precision takes tf32 pairs
+  const int attn_fmt = fmt == ANYLOC_PAIR_F16 && engine == ANYLOC_GEMM_SIMT ? ANYLOC_PAIR_TF32 : f.out;
   if (tp) {
     EpiParams e_qkv{ANYLOC_EPI_BIAS, wb.qkv_b, nullptr, nullptr, bf.qkv32, nullptr, 3 * D};
     e_qkv.alpha = wb.qkv_alpha;
     if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, fmt, st))) return rc;
-    if ((rc = qkv_tap(c, bf, M, sq, *tp, l, true, f16_attn, st))) return rc;
+    if ((rc = qkv_tap(c, bf, M, sq, *tp, l, attn_fmt, st))) return rc;
   } else {
     EpiParams e_qkv{ANYLOC_EPI_BIAS_SPLIT, wb.qkv_b, nullptr, nullptr, bf.qkv, bf.qkv_lo, 3 * D};
-    e_qkv.out_f16 = f16_attn;
+    e_qkv.out_fmt = attn_fmt;
     e_qkv.alpha = wb.qkv_alpha;
     if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, engine, fmt, st))) return rc;
   }
-  // single e4m3: the qkv epilogue wrote single bf16 and the bf16 attention runs; its output (in h) is quantised to the
-  // proj GEMM's e4m3 rows
-  float* o_hi = fp8 ? bf.h_hi : bf.y_hi;
-  const int attn_fmt = fp8 ? ANYLOC_PAIR_BF16 : fmt;
+  // single e4m3: the bf16 attention output goes to h and is quantised to the proj GEMM's e4m3 rows and their scales
+  float* o_hi = f.row_scales ? bf.h_hi : bf.y_hi;
+  float* o_lo = format_info(attn_fmt).lo ? bf.y_lo : nullptr;
   if (sq.tab) {
     ProfScope ps(PC_ATTENTION, st, sq.attn_flops);
-    if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, o_hi,
-                                         fp8 ? nullptr : bf.y_lo, attn_fmt, st)))
+    if ((rc = attention_tc_varlen_launch(bf.qkv, bf.qkv_lo, *sq.tab, sq.n_tiles, D, c->num_heads, o_hi, o_lo, attn_fmt,
+                                         st)))
       return rc;
-  } else if (bf16 || fp8 || h1) {
+  } else if (f.tc_only) {
     ProfScope ps(PC_ATTENTION, st, 4.0 * sq.B * (double)sq.T * sq.T * D);
     if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, o_hi, nullptr, attn_fmt, st))) return rc;
-  } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo, f16, engine,
-                                      st, f16_attn))) {
+  } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo,
+                                      fmt == ANYLOC_PAIR_F16, engine, st, attn_fmt == ANYLOC_PAIR_F16))) {
     return rc;
   }
-  if (fp8) {
+  if (f.row_scales) {
     ProfScope ps(PC_VIT_MISC, st, 3.0 * M * D);
     if ((rc = launch_quantize_fp8_rows(bf.h_hi, M, D, bf.y_hi, bf.y_lo, st))) return rc;
   }
@@ -617,17 +580,17 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
     if ((rc = launch_layernorm(bf.x, wb.ln2_w, wb.ln2_b, M, D, 1e-6f, bf.y_hi, bf.y_lo, fmt, st))) return rc; }
   EpiParams e_in{c->ffn_kind == ANYLOC_FFN_MLP ? ANYLOC_EPI_GELU_SPLIT : ANYLOC_EPI_SWIGLU_SPLIT, wb.in_b, nullptr,
                  nullptr, bf.h_hi, bf.h_lo, Hf};
-  e_in.alpha = wb.in_alpha; e_in.out_f16 = f16;
+  e_in.alpha = wb.in_alpha; e_in.out_fmt = f.out;
   const int n_in = c->ffn_kind == ANYLOC_FFN_MLP ? Hf : 2 * Hf;
   if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.in_w_hi, wb.in_w_lo, D, M, n_in, D, e_in, engine, fmt, st))) return rc;
-  if (fp8) {
+  if (f.row_scales) {
     ProfScope ps(PC_VIT_MISC, st, 3.0 * M * Hf);
     if ((rc = launch_quantize_fp8_rows(bf.h_hi, M, Hf, bf.h8, bf.h8_s, st))) return rc;
   }
   EpiParams e_out{ANYLOC_EPI_LS_RESID, wb.out_b, wb.ls2, bf.x, bf.x, nullptr, D};
   e_out.alpha = wb.out_alpha;
-  return gemm_dispatch(fp8 ? bf.h8 : bf.h_hi, fp8 ? bf.h8_s : bf.h_lo, Hf, wb.out_w_hi, wb.out_w_lo, Hf, M, D, Hf,
-                       e_out, engine, fmt, st);
+  return gemm_dispatch(f.row_scales ? bf.h8 : bf.h_hi, f.row_scales ? bf.h8_s : bf.h_lo, Hf, wb.out_w_hi,
+                       wb.out_w_lo, Hf, M, D, Hf, e_out, engine, fmt, st);
 }
 
 // Blocks 0..l_max over the M assembled token rows in bf.x, each run once, writing every tap of the plan:
@@ -639,8 +602,7 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
 static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const VitBuffers& bf, int M, const VitSeqs& sq,
                      const TapPlan& tp, int gemm_engine, cudaStream_t st) {
   const int D = cfg->embed_dim, fmt = cfg->pair_dtype;
-  const size_t wsz = fmt == ANYLOC_PAIR_FP8 ? 1
-                     : fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16X1 ? 2 : 4;
+  const size_t wsz = format_info(fmt).esz;
   int rc;
   for (int l = 0; l <= tp.l_max; ++l) {
     const AnylocVitBlock& wb = w->blocks[l];
@@ -664,18 +626,12 @@ static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const V
       if ((rc = gemm_dispatch(bf.y_hi, bf.y_lo, D, wb.qkv_w_hi, wb.qkv_w_lo, D, M, 3 * D, D, e_qkv, gemm_engine, fmt,
                               st)))
         return rc;
-      return qkv_tap(cfg, bf, M, sq, tp, l, false, false, st);
+      return qkv_tap(cfg, bf, M, sq, tp, l, FMT_NONE, st);
     }
     if ((rc = vit_block(cfg, wb, bf, M, sq, gemm_engine, st, qkv ? &tp : nullptr, l))) return rc;
     if (token && (rc = facet_out(sq, M, bf.x, D, D, tp, tp.out[l][ANYLOC_FACET_TOKEN], st))) return rc;
   }
   return ANYLOC_OK;
-}
-
-// the patch embedding's operand format: the single-e4m3 format keeps the bf16 im2col and GEMM (K = 3 14 14, a small
-// share of the FLOPs)
-static int patch_format(const AnylocVitCfg* cfg) {
-  return cfg->pair_dtype == ANYLOC_PAIR_FP8 ? ANYLOC_PAIR_BF16 : cfg->pair_dtype;
 }
 
 static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B,
@@ -701,7 +657,7 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
               vit_carve(cfg, (size_t)B * N, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  const int fmt = patch_format(cfg);
+  const int fmt = format_info(cfg->pair_dtype).patch;
   if ((rc = launch_im2col(img, B, H, W, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};
   e_pe.alpha = w->patch_alpha;
@@ -821,7 +777,7 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
               vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, nullptr, 0, nullptr) + 4096);
     return ANYLOC_ERR_WORKSPACE;
   }
-  const int fmt = patch_format(cfg);
+  const int fmt = format_info(cfg->pair_dtype).patch;
   for (int i = 0; i < B; ++i) p.img.ptr[i] = img[i];
   if ((rc = launch_im2col_varlen(p.img, p.n_patch, P, Kp, bf.pa_hi, bf.pa_lo, fmt, st))) return rc;
   EpiParams e_pe{ANYLOC_EPI_BIAS, w->patch_b, nullptr, nullptr, bf.ptmp, nullptr, D};

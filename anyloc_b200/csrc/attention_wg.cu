@@ -1,10 +1,12 @@
-// wgmma flash attention, softmax(Q K^T / 8) V per head (head_dim 64), for the two 2-byte formats:
-//   BF16 = false: q, k, v are fp16 pairs (hi, lo) of 8*x in the row-major qkv buffer [B*T, 3D] (q | k | v thirds, written
-//                 by the qkv GEMM's split epilogue); both products are 3-term  X.Y ~= X_hi.Y_hi + X_lo.Y_hi + X_hi.Y_lo;
-//                 output fp16 pairs of 8*o.
-//   BF16 = true : q, k, v are one bf16 array bf16_rn(x); one term per product, P rounded once to bf16; one bf16 output.
-//   H1 = true   : q, k, v are one fp16 array, the hi half of the fp16 pairs of 8*x; one term per product, the pairs'
-//                 scales (1/64 in the logit scale, P = 1024 p rounded once to its hi half); output the hi of 8*o.
+// wgmma flash attention, softmax(Q K^T / 8) V per head (head_dim 64), for the 2-byte formats FMT:
+//   ANYLOC_PAIR_F16  : q, k, v are fp16 pairs (hi, lo) of 8*x in the row-major qkv buffer [B*T, 3D] (q | k | v thirds,
+//                      written by the qkv GEMM's split epilogue); both products are 3-term
+//                      X.Y ~= X_hi.Y_hi + X_lo.Y_hi + X_hi.Y_lo; output fp16 pairs of 8*o.
+//   ANYLOC_PAIR_BF16 : q, k, v are one bf16 array bf16_rn(x); one term per product, P rounded once to bf16; one bf16
+//                      output.
+//   ANYLOC_PAIR_F16X1: q, k, v are one fp16 array, the hi half of the fp16 pairs of 8*x; one term per product, the
+//                      pairs' scales (1/64 in the logit scale, P = 1024 p rounded once to its hi half); output the hi of
+//                      8*o.
 // The arithmetic is that of the mma.sync kernel it replaced (attention_tc.cu keeps it for tf32 pairs): P = 1024 p split
 // into fp16 pairs, 1/kActScale^2 and log2(e) folded into the logit scale, ex2.approx, and each 64-key block's P.V
 // accumulated from zero by the tensor core and then added to the running output with round-to-nearest fp32 adds.
@@ -38,8 +40,8 @@ __device__ __forceinline__ float ex2(float x) {
 constexpr int BQ = 128, BKV = 64, HD = 64, THREADS = 384, STAGES = 4;
 constexpr int TILE_BYTES = 64 * 128;            // one 64-row x 64-column (128 B) box
 
-template <bool BF16, bool H1 = false> struct Cfg {
-  static constexpr int NT = BF16 || H1 ? 1 : 2;  // arrays per operand: (hi, lo), one bf16 or one fp16
+template <int FMT> struct Cfg {
+  static constexpr int NT = Fmt<FMT>::LO ? 2 : 1;   // arrays per operand: (hi, lo), or one
   static constexpr int Q_BYTES = NT * 2 * TILE_BYTES;                   // 128 rows
   static constexpr int K_OFF = 0, V_OFF = NT * TILE_BYTES;              // inside a stage; lo at + TILE_BYTES
   static constexpr int STAGE_BYTES = 2 * NT * TILE_BYTES;
@@ -47,12 +49,13 @@ template <bool BF16, bool H1 = false> struct Cfg {
   static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024 /*align*/;
 };
 
-template <bool BF16, bool VARLEN, bool H1 = false>
+template <int FMT, bool VARLEN>
 __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const CUtensorMap* tm_lo, int T, int D,
                                                  void* __restrict__ o_hi_, void* __restrict__ o_lo_,
                                                  const VarlenAttnTable* tab) {
-  using C = Cfg<BF16, H1>;
-  constexpr bool PAIRS = !BF16 && !H1;          // three terms per product
+  using C = Cfg<FMT>;
+  using F = Fmt<FMT>;
+  constexpr bool PAIRS = F::LO;                 // three terms per product
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);    // [STAGES]
@@ -113,7 +116,7 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
   const int cw = wg - 1;
   if (qt * BQ + cw * 64 >= T) return;           // no rows below T: not counted by the empty barriers
   const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31, g = lane >> 2, t4 = lane & 3;
-  constexpr bool SCALED = !BF16;                // fp16 pairs carry s = kActScale and P is scaled into fp16's range
+  constexpr bool SCALED = F::SCALED;            // fp16 operands carry s = kActScale and P is scaled into fp16's range
   const float P_SCALE = SCALED ? 1024.0f : 1.0f;
   // S holds (s q).(s k), s = kActScale for fp16 pairs: fold 1/s^2 into the 1/sqrt(64) * log2(e) scale
   const float kScale = 0.125f * 1.4426950408889634f * (SCALED ? 1.0f / (kActScale * kActScale) : 1.0f);
@@ -131,10 +134,10 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const uint64_t adv = (uint64_t)((k * 32) >> 4);          // +32 B per k16 step inside the 128 B row
-      wgmma_m64n64_ss<BF16>(s, dq_hi + adv, dk_hi + adv, k != 0 ? 1u : 0u);
+      wgmma_m64n64_ss<FMT>(s, dq_hi + adv, dk_hi + adv, k != 0 ? 1u : 0u);
       if constexpr (PAIRS) {
-        wgmma_m64n64_ss<false>(s, dq_lo + adv, dk_hi + adv, 1u);
-        wgmma_m64n64_ss<false>(s, dq_hi + adv, dk_lo + adv, 1u);
+        wgmma_m64n64_ss<FMT>(s, dq_lo + adv, dk_hi + adv, 1u);
+        wgmma_m64n64_ss<FMT>(s, dq_hi + adv, dk_lo + adv, 1u);
       }
     }
     wgmma_commit();
@@ -187,10 +190,7 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
     for (int ks = 0; ks < 4; ++ks) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const float a = p[8 * ks + 2 * i], b = p[8 * ks + 2 * i + 1];
-        if constexpr (BF16) ph[ks][i] = pack_bf16x2(a, b);
-        else if constexpr (H1) ph[ks][i] = pack_f16x2_hi(a * P_SCALE, b * P_SCALE);
-        else split_f16x2(a * P_SCALE, b * P_SCALE, ph[ks][i], pl[ks][i]);
+        F::pack2(p[8 * ks + 2 * i] * P_SCALE, p[8 * ks + 2 * i + 1] * P_SCALE, ph[ks][i], pl[ks][i]);
       }
     }
     // ---- O_j = P V (3-term), accumulated from zero, then o = alpha o + O_j (round-to-nearest)
@@ -220,10 +220,10 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
       const uint64_t adv = (uint64_t)((ks * 2048) >> 4);       // 16 keys = two 8-row atoms
-      wgmma_m64n64_rs_tb<BF16>(pv, ph[ks], dv_hi + adv, ks != 0 ? 1u : 0u);
+      wgmma_m64n64_rs_tb<FMT>(pv, ph[ks], dv_hi + adv, ks != 0 ? 1u : 0u);
       if constexpr (PAIRS) {
-        wgmma_m64n64_rs_tb<false>(pv, pl[ks], dv_hi + adv, 1u);
-        wgmma_m64n64_rs_tb<false>(pv, ph[ks], dv_lo + adv, 1u);
+        wgmma_m64n64_rs_tb<FMT>(pv, pl[ks], dv_hi + adv, 1u);
+        wgmma_m64n64_rs_tb<FMT>(pv, ph[ks], dv_lo + adv, 1u);
       }
     }
     wgmma_commit();
@@ -263,52 +263,62 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
     const size_t off = (out0 + q) * (size_t)D + (size_t)h * HD + 2 * t4;
 #pragma unroll
     for (int nd = 0; nd < 8; ++nd) {
-      const float a = o[4 * nd + 2 * half] * inv, c = o[4 * nd + 2 * half + 1] * inv;
-      if constexpr (BF16) {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(o_hi_) + off + nd * 8) = pack_bf16x2(a, c);
-      } else if constexpr (H1) {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_hi_) + off + nd * 8) = pack_f16x2_hi(a, c);
-      } else {
-        uint32_t hh, ll;
-        split_f16x2(a, c, hh, ll);
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_hi_) + off + nd * 8) = hh;
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(o_lo_) + off + nd * 8) = ll;
-      }
+      uint32_t hh, ll;           // o is already scaled: the words of the values as they are
+      F::pack2(o[4 * nd + 2 * half] * inv, o[4 * nd + 2 * half + 1] * inv, hh, ll);
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<typename F::T*>(o_hi_) + off + nd * 8) = hh;
+      if constexpr (F::LO) *reinterpret_cast<uint32_t*>(reinterpret_cast<typename F::T*>(o_lo_) + off + nd * 8) = ll;
     }
   }
 }
 
 // B images of T tokens each: grid (128-query tiles, heads, B); maps over (3D columns, T rows, B images)
-template <bool BF16, bool H1 = false>
+template <int FMT>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_wg_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, int T, int D,
                     void* __restrict__ o_hi, void* __restrict__ o_lo) {
-  attention_wg_cta<BF16, false, H1>(&tm_hi, &tm_lo, T, D, o_hi, o_lo, nullptr);
+  attention_wg_cta<FMT, false>(&tm_hi, &tm_lo, T, D, o_hi, o_lo, nullptr);
 }
 
 // Images of different lengths packed row after row: grid (sum of every image's 128-query tiles, heads); maps over
 // (3D columns, all packed rows, 1).  The host lists the images longest first, so the CTAs with the longest key loops
 // start first and short images fill the tail.
-template <bool BF16, bool H1 = false>
+template <int FMT>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_wg_varlen_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
                            const __grid_constant__ VarlenAttnTable tab, int D, void* __restrict__ o_hi,
                            void* __restrict__ o_lo) {
-  attention_wg_cta<BF16, true, H1>(&tm_hi, &tm_lo, 0, D, o_hi, o_lo, &tab);
+  attention_wg_cta<FMT, true>(&tm_hi, &tm_lo, 0, D, o_hi, o_lo, &tab);
 }
 
-template <bool BF16, bool H1 = false>
-static int set_smem_attrs() {
-  static unsigned long long seen = 0;
-  if (first_use_on_this_device(&seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_wg_kernel<BF16, H1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<BF16, H1>::SMEM_BYTES));
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_wg_varlen_kernel<BF16, H1>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BF16, H1>::SMEM_BYTES));
-  }
-  return ANYLOC_OK;
+// Launches the padded (tab == nullptr: B images of T tokens) or the packed kernel of fmt over the maps of qkv_{hi,lo}
+static int launch(const void* qkv_hi, const void* qkv_lo, int imgs, int rows, int T, const VarlenAttnTable* tab,
+                  dim3 grid, int D, void* o_hi, void* o_lo, int fmt, cudaStream_t st) {
+  CUtensorMap m_hi, m_lo;
+  int rc;
+  if ((rc = tc::make_map_3d16(&m_hi, qkv_hi, imgs, rows, 3 * D, 64, fmt))) return rc;
+  if ((rc = tc::make_map_3d16(&m_lo, format_info(fmt).lo ? qkv_lo : qkv_hi, imgs, rows, 3 * D, 64, fmt))) return rc;
+  return fmt_switch(fmt, [&](auto c) {
+    constexpr int FMT = decltype(c)::value;
+    if constexpr (sizeof(typename Fmt<FMT>::T) != 2) {
+      set_error("attention_wg: format %d is not a 2-byte format", fmt);
+      return (int)ANYLOC_ERR_ARG;
+    } else {
+      static unsigned long long seen = 0;
+      if (first_use_on_this_device(&seen)) {
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_wg_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               Cfg<FMT>::SMEM_BYTES));
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(attention_wg_varlen_kernel<FMT>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<FMT>::SMEM_BYTES));
+      }
+      if (tab)
+        attention_wg_varlen_kernel<FMT><<<grid, THREADS, Cfg<FMT>::SMEM_BYTES, st>>>(m_hi, m_lo, *tab, D, o_hi, o_lo);
+      else
+        attention_wg_kernel<FMT><<<grid, THREADS, Cfg<FMT>::SMEM_BYTES, st>>>(m_hi, m_lo, T, D, o_hi, o_lo);
+      ANYLOC_CHECK_LAUNCH();
+      return (int)ANYLOC_OK;
+    }
+  });
 }
-
 
 }  // namespace awg
 
@@ -318,24 +328,7 @@ static int set_smem_attrs() {
 int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
                         int fmt, cudaStream_t st) {
   using namespace awg;
-  const bool bf16 = fmt == ANYLOC_PAIR_BF16, single = bf16 || fmt == ANYLOC_PAIR_F16X1;
-  CUtensorMap m_hi, m_lo;
-  int rc;
-  if ((rc = tc::make_map_3d16(&m_hi, qkv_hi, B, T, 3 * D, 64, bf16))) return rc;
-  if ((rc = tc::make_map_3d16(&m_lo, single ? qkv_hi : qkv_lo, B, T, 3 * D, 64, bf16))) return rc;
-  const dim3 grid(cdiv(T, BQ), heads, B);
-  if (bf16) {
-    if ((rc = set_smem_attrs<true>())) return rc;
-    attention_wg_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(m_hi, m_lo, T, D, o_hi, o_lo);
-  } else if (single) {
-    if ((rc = set_smem_attrs<false, true>())) return rc;
-    attention_wg_kernel<false, true><<<grid, THREADS, Cfg<false, true>::SMEM_BYTES, st>>>(m_hi, m_lo, T, D, o_hi, o_lo);
-  } else {
-    if ((rc = set_smem_attrs<false>())) return rc;
-    attention_wg_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(m_hi, m_lo, T, D, o_hi, o_lo);
-  }
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  return launch(qkv_hi, qkv_lo, B, T, T, nullptr, dim3(cdiv(T, BQ), heads, B), D, o_hi, o_lo, fmt, st);
 }
 
 // the same over images of different lengths packed into one [rows, 3D] qkv buffer, rows = the end of the last image;
@@ -343,7 +336,6 @@ int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, in
 int attention_wg_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int D, int heads,
                                void* o_hi, void* o_lo, int fmt, cudaStream_t st) {
   using namespace awg;
-  const bool bf16 = fmt == ANYLOC_PAIR_BF16, single = bf16 || fmt == ANYLOC_PAIR_F16X1;
   VarlenAttnTable t = tab;
   int tiles = 0, rows = 0;
   for (int k = 0; k < t.n; ++k) {
@@ -351,24 +343,7 @@ int attention_wg_varlen_launch(const void* qkv_hi, const void* qkv_lo, const Var
     tiles += cdiv(t.len[k], BQ);
     if (t.row0[k] + t.len[k] > rows) rows = t.row0[k] + t.len[k];
   }
-  CUtensorMap m_hi, m_lo;
-  int rc;
-  if ((rc = tc::make_map_3d16(&m_hi, qkv_hi, 1, rows, 3 * D, 64, bf16))) return rc;
-  if ((rc = tc::make_map_3d16(&m_lo, single ? qkv_hi : qkv_lo, 1, rows, 3 * D, 64, bf16))) return rc;
-  const dim3 grid(tiles, heads);
-  if (bf16) {
-    if ((rc = set_smem_attrs<true>())) return rc;
-    attention_wg_varlen_kernel<true><<<grid, THREADS, Cfg<true>::SMEM_BYTES, st>>>(m_hi, m_lo, t, D, o_hi, o_lo);
-  } else if (single) {
-    if ((rc = set_smem_attrs<false, true>())) return rc;
-    attention_wg_varlen_kernel<false, true><<<grid, THREADS, Cfg<false, true>::SMEM_BYTES, st>>>(m_hi, m_lo, t, D, o_hi,
-                                                                                                o_lo);
-  } else {
-    if ((rc = set_smem_attrs<false>())) return rc;
-    attention_wg_varlen_kernel<false><<<grid, THREADS, Cfg<false>::SMEM_BYTES, st>>>(m_hi, m_lo, t, D, o_hi, o_lo);
-  }
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  return launch(qkv_hi, qkv_lo, 1, rows, 0, &t, dim3(tiles, heads), D, o_hi, o_lo, fmt, st);
 }
 
 }  // namespace anyloc

@@ -1,6 +1,6 @@
 // Shared GEMM epilogue (used by the SIMT and the tensor-core GEMM kernels).
 #pragma once
-#include "common.cuh"
+#include "formats.cuh"
 
 namespace anyloc {
 
@@ -13,26 +13,25 @@ struct EpiParams {
   float* out_lo;        // [M,ldo] (SPLIT modes)
   int ldo;
   float alpha = 1.0f;   // accumulator scale (1/(s_A*s_B) for fp16-pair inputs, else 1)
-  int out_f16 = 0;      // SPLIT outputs as fp16 pairs of kActScale*v (out/out_lo then point to __half)
+  int out_fmt = ANYLOC_PAIR_TF32;   // SPLIT output format (ANYLOC_PAIR_*): the pair GEMMs write tf32 or fp16 pairs by it
+                                    // at run time; the single formats write Fmt<FMT>::OUT
   const int* gate = nullptr;   // device flag (nullable): tensor-core GEMM kernels return immediately when *gate == 0 (conditional fallbacks without a host sync)
   const float* row_scale = nullptr;   // [M] e4m3 A operand's row scales (single e4m3 GEMM only): acc of row m times row_scale[m]
 };
 
-// SPLIT output format of a GEMM instantiation: the pair formats (chosen at run time by out_f16), or one array of the
-// tensor-core GEMM's single-bf16 / single-fp16 instantiations (out = bf16_rn(v), or the hi of split_f16(kActScale v))
-enum SingleOut { SGL_PAIRS = 0, SGL_BF16 = 1, SGL_F16X1 = 2 };
-template <int SGL = SGL_PAIRS>
+// SPLIT output v of element o in the format OUT
+template <int OUT>
+__device__ __forceinline__ void split_put1(const EpiParams& p, size_t o, float v) {
+  typedef typename Fmt<OUT>::T T;
+  put1<OUT>(reinterpret_cast<T*>(p.out), reinterpret_cast<T*>(p.out_lo), o, v);
+}
+// SPLIT output of a GEMM on FMT inputs (the SIMT engine's pair GEMMs take the default): Fmt<FMT>::OUT, or for the pair
+// inputs the pair format ep.out_fmt names, chosen at run time
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epi_store_split(const EpiParams& p, size_t o, float v) {
-  if (SGL == SGL_BF16) {
-    reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16_rn(v);
-  } else if (SGL == SGL_F16X1) {
-    reinterpret_cast<__half*>(p.out)[o] = f16_hi(v * kActScale);
-  } else if (p.out_f16) {
-    __half h, l; split_f16(v * kActScale, h, l);
-    reinterpret_cast<__half*>(p.out)[o] = h; reinterpret_cast<__half*>(p.out_lo)[o] = l;
-  } else {
-    float h, l; split_tf32(v, h, l); p.out[o] = h; p.out_lo[o] = l;
-  }
+  if constexpr (!Fmt<FMT>::LO) split_put1<Fmt<FMT>::OUT>(p, o, v);
+  else if (p.out_fmt != ANYLOC_PAIR_TF32) split_put1<ANYLOC_PAIR_F16>(p, o, v);
+  else split_put1<ANYLOC_PAIR_TF32>(p, o, v);
 }
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
@@ -51,24 +50,24 @@ __device__ __forceinline__ float silu_fast(float x) {
 
 // Apply the epilogue to one accumulator element (m, n).  For SWIGLU the caller passes the PAIR
 // (acc0 at column n even, acc1 at column n+1) and the result lands in column n/2.
-template <int SGL = SGL_PAIRS>
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epi_store1(const EpiParams& p, int m, int n, float acc) {
   float v = acc * p.alpha + (p.bias ? __ldg(p.bias + n) : 0.f);
   size_t o = (size_t)m * p.ldo + n;
   switch (p.mode) {
     case ANYLOC_EPI_BIAS: p.out[o] = v; break;
-    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split<SGL>(p, o, v); break;
-    case ANYLOC_EPI_GELU_SPLIT: epi_store_split<SGL>(p, o, gelu_erf(v)); break;
+    case ANYLOC_EPI_BIAS_SPLIT: epi_store_split<FMT>(p, o, v); break;
+    case ANYLOC_EPI_GELU_SPLIT: epi_store_split<FMT>(p, o, gelu_erf(v)); break;
     case ANYLOC_EPI_LS_RESID: p.out[o] = p.resid[o] + __ldg(p.gamma + n) * v; break;
     default: break;
   }
 }
-template <int SGL = SGL_PAIRS>
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epi_store_pair(const EpiParams& p, int m, int n_even, float acc0, float acc1) {
   // SWIGLU: columns (n_even, n_even+1) = (x1_j, x2_j), j = n_even/2
   float x1 = acc0 * p.alpha + (p.bias ? __ldg(p.bias + n_even) : 0.f);
   float x2 = acc1 * p.alpha + (p.bias ? __ldg(p.bias + n_even + 1) : 0.f);
-  epi_store_split<SGL>(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
+  epi_store_split<FMT>(p, (size_t)m * p.ldo + (n_even >> 1), silu(x1) * x2);
 }
 
 }  // namespace anyloc

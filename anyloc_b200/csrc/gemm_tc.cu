@@ -14,15 +14,11 @@
 //                 the last chunk: bias / GELU / SwiGLU / LayerScale+residual / pair split, staged in shared memory
 //                 subtile by subtile and stored with TMA (epilogue_staged), so the stores drain behind the next
 //                 tile's mainloop.  The hi-only coarse passes, and outputs TMA cannot store, are stored from registers.
-// A third operand format, single bf16 (ANYLOC_PAIR_BF16: one bf16 array of bf16_rn(x), no lo, no scale), runs one
-// wgmma.f32.bf16.bf16 per k-step through the same pipeline with hi-only stages and the staged epilogue
-// (gemm_tc_bf16_launch): a third of the 3-term MMAs, not fp32-equivalent.
-// A fourth, single e4m3 (ANYLOC_PAIR_FP8: A = e4m3 rows with one power-of-two scale per row, B = one e4m3 matrix),
-// runs one wgmma.f32.e4m3.e4m3 per 32-element k-step on UINT8 tensor maps (128-element k-blocks) with the bf16 pass's
-// stages and staged epilogue; the accumulator of row m is multiplied by A's row scale before the epilogue, and the
-// SPLIT outputs are one bf16 array (gemm_tc_fp8_launch).
-// A fifth, single fp16 (ANYLOC_PAIR_F16X1: the hi array of the fp16 pairs alone), runs the fp16 wgmma once per k-step
-// with the bf16 pass's stages and a staged epilogue that writes the hi of the fp16 pair (gemm_tc_f16x1_launch).
+// The single formats (formats.cuh) run one wgmma per k-step through the same pipeline with hi-only stages and the staged
+// epilogue, a third of the 3-term MMAs, not fp32-equivalent: single bf16 (ANYLOC_PAIR_BF16), single fp16
+// (ANYLOC_PAIR_F16X1, the hi array of the fp16 pairs alone), and single e4m3 (ANYLOC_PAIR_FP8: A = e4m3 rows with one
+// power-of-two scale per row, B = one e4m3 matrix; 128-element k-blocks on UINT8 tensor maps, the accumulator of row m
+// multiplied by A's row scale before the epilogue).  Their SPLIT outputs are one array in Fmt<FMT>::OUT.
 // Tiles are rastered in bands of BAND_N column blocks, n-fastest inside a band: the resident CTAs share a few A row
 // panels and one band of B that stays in L2 while the outputs stream through.
 #include <cuda.h>
@@ -44,7 +40,7 @@ constexpr int STG_BYTES = 8192;            // one epilogue staging buffer (see e
 // LO = true : stages hold {A_hi, A_lo, B_hi, B_lo} (3-term split, 64 KB).  LO = false: hi-only single pass (coarse
 // scores): {A_hi, B_hi} = 32 KB per stage -> twice the pipeline depth in the same shared memory.
 // LOM (lo operands present): bit 0 = A_lo, bit 1 = B_lo; a compile-time mask keeps the wgmma sequence branch-free.
-// STG: the staged epilogue is compiled in -- the 3-term passes and the single-bf16 pass (hi-only, so 6 stages of 32 KB
+// STG: the staged epilogue is compiled in -- the 3-term passes and the single formats (hi-only, so 6 stages of 32 KB
 // plus 4 x 8 KB staging = 231 424 B of H100's 232 448 B opt-in), not the hi-only coarse passes (below).
 template <bool LO, bool STG = LO> struct Cfg {
   static constexpr int STAGE_BYTES = (LO ? 2 : 1) * (A_BYTES + B_BYTES);
@@ -81,37 +77,31 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   n_blk = band * band_n + (r - m_blk * w);
 }
 
-template <int SGL = SGL_PAIRS>
+// SPLIT outputs of elements o, o + 1 (o even) in the format OUT; and as epi_store_split chooses it
+template <int OUT>
+__device__ __forceinline__ void split_put2(const EpiParams& ep, size_t o, float a, float b) {
+  typedef typename Fmt<OUT>::T T;
+  put2<OUT>(reinterpret_cast<T*>(ep.out), reinterpret_cast<T*>(ep.out_lo), o, a, b);
+}
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, float a, float b) {
-  if (SGL == SGL_BF16) {        // single bf16
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + o) = pack_bf16x2(a, b);
-  } else if (SGL == SGL_F16X1) {     // single fp16: the hi of the fp16 pair of kActScale*x
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(ep.out) + o) = pack_f16x2_hi(a * kActScale, b * kActScale);
-  } else if (ep.out_f16) {      // fp16 pair of kActScale*x
-    uint32_t h, l;
-    split_f16x2(a * kActScale, b * kActScale, h, l);
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(ep.out) + o) = h;
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(ep.out_lo) + o) = l;
-  } else {
-    float2 h, l;
-    split_tf32(a, h.x, l.x); split_tf32(b, h.y, l.y);
-    *reinterpret_cast<float2*>(ep.out + o) = h;
-    *reinterpret_cast<float2*>(ep.out_lo + o) = l;
-  }
+  if constexpr (!Fmt<FMT>::LO) split_put2<Fmt<FMT>::OUT>(ep, o, a, b);
+  else if (ep.out_fmt != ANYLOC_PAIR_TF32) split_put2<ANYLOC_PAIR_F16>(ep, o, a, b);
+  else split_put2<ANYLOC_PAIR_TF32>(ep, o, a, b);
 }
 
 // epilogue of two adjacent accumulator columns (n even, n+1) of row m
-template <int SGL = SGL_PAIRS>
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int N, float v0, float v1) {
   const int mode = ep.mode;
   if (mode < 0) return;                    // diagnostic: discard (ANYLOC_GEMM_DEBUG_SKIP_EPI)
   if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {   // (x1_j, x2_j) = columns (2j, 2j+1); N is even
-    epi_store_pair<SGL>(ep, m, n, v0, v1);
+    epi_store_pair<FMT>(ep, m, n, v0, v1);
     return;
   }
   if (n + 1 >= N || (ep.ldo & 1)) {
-    epi_store1<SGL>(ep, m, n, v0);
-    if (n + 1 < N) epi_store1<SGL>(ep, m, n + 1, v1);
+    epi_store1<FMT>(ep, m, n, v0);
+    if (n + 1 < N) epi_store1<FMT>(ep, m, n + 1, v1);
     return;
   }
   const float al = ep.alpha;
@@ -126,23 +116,23 @@ __device__ __forceinline__ void epi_pair(const EpiParams& ep, int m, int n, int 
     const float2 r = *reinterpret_cast<const float2*>(ep.resid + o);
     *reinterpret_cast<float2*>(ep.out + o) = make_float2(r.x + g.x * x0, r.y + g.y * x1);
   } else if (mode == ANYLOC_EPI_GELU_SPLIT) {
-    store_split2<SGL>(ep, o, gelu_erf(x0), gelu_erf(x1));
+    store_split2<FMT>(ep, o, gelu_erf(x0), gelu_erf(x1));
   } else {                                 // BIAS_SPLIT
-    store_split2<SGL>(ep, o, x0, x1);
+    store_split2<FMT>(ep, o, x0, x1);
   }
 }
 
 // Register epilogue of the 3-term passes that do not stage (gated launches, outputs TMA cannot store: see
 // make_epi_maps) of one consumer thread's part of a 64 x 128 sub-tile: rows r0 and r0 + 8, column pairs nq + 8j (j < 16), accumulators in the wgmma layout,
 // applied and stored pair by pair.
-template <int SGL = SGL_PAIRS>
+template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epilogue_pairs(const EpiParams& ep, int r0, int nq, int M, int N, const float* sum) {
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int n = nq + j * 8;
     if (n >= N) continue;
-    if (r0 < M) epi_pair<SGL>(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
-    if (r0 + 8 < M) epi_pair<SGL>(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
+    if (r0 < M) epi_pair<FMT>(ep, r0, n, N, sum[4 * j], sum[4 * j + 1]);
+    if (r0 + 8 < M) epi_pair<FMT>(ep, r0 + 8, n, N, sum[4 * j + 2], sum[4 * j + 3]);
   }
 }
 
@@ -206,28 +196,36 @@ __device__ __forceinline__ void epilogue_regs_batched(const EpiParams& ep, int r
 }
 
 // ------------------------------------------------------------------ staged epilogue
-// Output formats of the staged path.  A subtile is 64 rows x COLS output columns; one 8 KB staging buffer holds it:
-// 64 x 32 fp32, the hi and lo halves (4 KB each) of 64 x 32 fp16 or 64 x 16 fp32 pairs, or 64 x 64 single bf16 or
-// single fp16.
-enum StageKind { STG_F32 = 0, STG_F16_PAIR = 1, STG_TF32_PAIR = 2, STG_BF16 = 3, STG_F16 = 4 };
+// Output formats of the staged path: the SPLIT output format OUT (ANYLOC_PAIR_*), or OUT_F32 (BIAS / LS_RESID).  A
+// subtile is 64 rows x COLS output columns; one 8 KB staging buffer holds it: 64 x 32 fp32, the hi and lo halves (4 KB
+// each) of 64 x 32 fp16 or 64 x 16 fp32 pairs, or 64 x 64 single bf16 or single fp16.
+constexpr int OUT_F32 = -1;
 constexpr int STG_HALF = STG_BYTES / 2;    // offset of the lo array (pair formats)
 constexpr int STG_ROWS = 64;               // TMA box rows of the output maps: one consumer warpgroup's rows
 
-template <int KIND>
+template <int OUT> constexpr bool stage_lo() {
+  if constexpr (OUT == OUT_F32) return false;
+  else return Fmt<OUT>::LO;
+}
+template <int OUT> constexpr int stage_esz() {
+  if constexpr (OUT == OUT_F32) return 4;
+  else return (int)sizeof(typename Fmt<OUT>::T);
+}
+template <int OUT>
 struct StageFmt {
-  static constexpr bool SINGLE16 = KIND == STG_BF16 || KIND == STG_F16;   // one 2-byte array
-  static constexpr int ESZ = KIND == STG_F16_PAIR || SINGLE16 ? 2 : 4;
-  static constexpr int COLS = KIND == STG_TF32_PAIR ? 16 : SINGLE16 ? 64 : 32;   // output columns per subtile
-  static constexpr int ROW_BYTES = COLS * ESZ;                       // 128 (fp32) or 64 bytes per row of one array
+  static constexpr bool LO = stage_lo<OUT>();                        // a lo array in the buffer's second half
+  static constexpr int ESZ = stage_esz<OUT>();
+  static constexpr int ROW_BYTES = STG_BYTES / STG_ROWS / (LO ? 2 : 1);   // 128 or 64 bytes per row of one array
+  static constexpr int COLS = ROW_BYTES / ESZ;                       // output columns per subtile
   static constexpr uint32_t SWZ = ROW_BYTES == 128 ? 7 : 3;          // TMA SWIZZLE_128B / SWIZZLE_64B
 };
 
 // Byte offset of byte b of staging row `row`, placed as TMA's SWIZZLE_128B / _64B expects it: the 16-byte chunk index
 // XOR offset bits 7.. .  The 8 rows that one warp's store instruction covers land in distinct banks.
-template <int KIND>
+template <int OUT>
 __device__ __forceinline__ uint32_t stg_off(int row, int b) {
-  const uint32_t o = (uint32_t)(row * StageFmt<KIND>::ROW_BYTES + b);
-  return o ^ (((o >> 7) & StageFmt<KIND>::SWZ) << 4);
+  const uint32_t o = (uint32_t)(row * StageFmt<OUT>::ROW_BYTES + b);
+  return o ^ (((o >> 7) & StageFmt<OUT>::SWZ) << 4);
 }
 
 // bias / gamma of columns (n, n+1); columns at or past N (which TMA clips) read nothing
@@ -249,12 +247,12 @@ __device__ __forceinline__ void resid_load(const CUtensorMap* tm, uint8_t* buf, 
 // clips the M and N tails.  The stores drain while the warpgroup works on the next subtile and the next tile's
 // mainloop.  Two buffers alternate (running subtile count `cnt`); a buffer is rewritten only once the store issued
 // from it has read it (waited before the barrier of the subtile in between).  Same arithmetic as epi_pair.
-template <int KIND, bool SWIGLU, bool RESID>
+template <int OUT, bool SWIGLU, bool RESID>
 __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUtensorMap* tm_out, const CUtensorMap* tm_lo,
                                                 const CUtensorMap* tm_resid, uint8_t* stg, uint64_t* rbar,
                                                 uint32_t& rphase, uint32_t& cnt, int wg, int t, int m0, int n0, int N,
                                                 const float* sum) {
-  using F = StageFmt<KIND>;
+  using F = StageFmt<OUT>;
   constexpr int ACC = SWIGLU ? 2 * F::COLS : F::COLS;    // accumulator columns per subtile
   constexpr int JS = ACC / 8;                             // 8-column accumulator groups per subtile
   const int lane = t & 31, q = lane & 3, row = (t >> 5) * 16 + (lane >> 2);
@@ -279,28 +277,18 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
       for (int h = 0; h < 2; ++h) {
         const int r = row + 8 * h;
         const float x0 = sum[4 * j + 2 * h] * al + bb.x, x1 = sum[4 * j + 2 * h + 1] * al + bb.y;
-        if (SWIGLU) {                      // (x1_j, x2_j) = columns (n, n+1) -> output column n/2
+        if constexpr (SWIGLU) {            // (x1_j, x2_j) = columns (n, n+1) -> output column n/2
+          typedef typename Fmt<OUT>::T E;
           const float v = silu(x0) * x1;
-          const uint32_t o = stg_off<KIND>(r, (4 * jj + q) * F::ESZ);
-          if (KIND == STG_BF16) {
-            *reinterpret_cast<__nv_bfloat16*>(buf + o) = __float2bfloat16_rn(v);
-          } else if (KIND == STG_F16) {
-            *reinterpret_cast<__half*>(buf + o) = f16_hi(v * kActScale);
-          } else if (KIND == STG_F16_PAIR) {
-            __half hi, lo;
-            split_f16(v * kActScale, hi, lo);
-            *reinterpret_cast<__half*>(buf + o) = hi;
-            *reinterpret_cast<__half*>(buf + STG_HALF + o) = lo;
-          } else {
-            float hi, lo;
-            split_tf32(v, hi, lo);
-            *reinterpret_cast<float*>(buf + o) = hi;
-            *reinterpret_cast<float*>(buf + STG_HALF + o) = lo;
-          }
+          const uint32_t o = stg_off<OUT>(r, (4 * jj + q) * F::ESZ);
+          E hi, lo;
+          Fmt<OUT>::split1(v, hi, lo);
+          *reinterpret_cast<E*>(buf + o) = hi;
+          if constexpr (F::LO) *reinterpret_cast<E*>(buf + STG_HALF + o) = lo;
           continue;
         }
-        const uint32_t o = stg_off<KIND>(r, (8 * jj + 2 * q) * F::ESZ);
-        if (KIND == STG_F32) {
+        const uint32_t o = stg_off<OUT>(r, (8 * jj + 2 * q) * F::ESZ);
+        if constexpr (OUT == OUT_F32) {
           float2* p = reinterpret_cast<float2*>(buf + o);
           if (RESID) {
             const float2 rr = *p;
@@ -309,22 +297,12 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
             *p = make_float2(x0, x1);
           }
         } else {
+          typedef typename Fmt<OUT>::W2 W;
           const float y0 = gelu ? gelu_erf(x0) : x0, y1 = gelu ? gelu_erf(x1) : x1;
-          if (KIND == STG_BF16) {
-            *reinterpret_cast<uint32_t*>(buf + o) = pack_bf16x2(y0, y1);
-          } else if (KIND == STG_F16) {
-            *reinterpret_cast<uint32_t*>(buf + o) = pack_f16x2_hi(y0 * kActScale, y1 * kActScale);
-          } else if (KIND == STG_F16_PAIR) {
-            uint32_t hi, lo;
-            split_f16x2(y0 * kActScale, y1 * kActScale, hi, lo);
-            *reinterpret_cast<uint32_t*>(buf + o) = hi;
-            *reinterpret_cast<uint32_t*>(buf + STG_HALF + o) = lo;
-          } else {
-            float2 hi, lo;
-            split_tf32(y0, hi.x, lo.x); split_tf32(y1, hi.y, lo.y);
-            *reinterpret_cast<float2*>(buf + o) = hi;
-            *reinterpret_cast<float2*>(buf + STG_HALF + o) = lo;
-          }
+          W hi, lo;
+          Fmt<OUT>::split2(y0, y1, hi, lo);
+          *reinterpret_cast<W*>(buf + o) = hi;
+          if constexpr (F::LO) *reinterpret_cast<W*>(buf + STG_HALF + o) = lo;
         }
       }
     }
@@ -334,7 +312,7 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
     else named_bar_sync<2>(128);
     if (t == 0) {
       tma_store_2d(tm_out, smem_u32(buf), oc0, m0);
-      if (KIND != STG_F32 && !F::SINGLE16) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
+      if (F::LO) tma_store_2d(tm_lo, smem_u32(buf + STG_HALF), oc0, m0);
       bulk_commit();
       if (RESID && s + 2 < BN / ACC && oc0 + 2 * F::COLS < n_out) {
         // residual of subtile s + 2 into this buffer, once the store has read it
@@ -346,18 +324,13 @@ __device__ __forceinline__ void epilogue_staged(const EpiParams& ep, const CUten
   }
 }
 
-// F16 = false: operands are fp32 words read as tf32 (32 elements per 128 B k-block, wgmma K=8)
-// F16 = true : operands are fp16            (64 elements per 128 B k-block, wgmma K=16, 2x rate)
-// BF16 = true (with F16 and LOM = 0): single bf16 operands, same layout and rate as fp16, one wgmma per k-step; the
-//             staged epilogue writes single bf16 SPLIT outputs (STG_BF16).
+// FMT: the operand format (ANYLOC_PAIR_*); every k-block is 128 bytes of K: 32 tf32, 64 fp16 or bf16, 128 e4m3
+// elements.  LOM != 0 (lo operands) for the pair formats only.  The single formats run one wgmma per k-step and write
+// their SPLIT outputs in Fmt<FMT>::OUT; single e4m3 takes A's row scales in ep.row_scale.
 // ep.gate (nullable): the kernel returns at once when *gate == 0 (conditional fallbacks without a host sync).
 // staged != 0: the epilogue goes through shared memory and TMA stores (tm_out, tm_out_lo for the pair formats,
 // tm_resid for LS_RESID: (n_out, M) maps with 64-row boxes); 0: stored pair by pair from registers.
-// FP8 = true (with F16 and LOM = 0): single e4m3 operands (128 elements per 128 B k-block, wgmma K=32), A's row
-//             scales in ep.row_scale; SPLIT outputs as BF16.
-// F16X1 = true (with F16 and LOM = 0): single fp16 operands (the hi halves of fp16 pairs), the fp16 pairs' k-steps and
-//             alpha, one wgmma per k-step; the staged epilogue writes single fp16 SPLIT outputs (STG_F16).
-template <bool F16, int LOM, bool BF16 = false, bool FP8 = false, bool F16X1 = false>
+template <int FMT, int LOM>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
@@ -365,12 +338,8 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                 const __grid_constant__ CUtensorMap tm_resid, int staged,
                 int M, int N, int K, int band_n, int chunk_kb, EpiParams ep) {
   constexpr bool LO = LOM != 0, has_a_lo = (LOM & 1) != 0, has_b_lo = (LOM & 2) != 0;
-  static_assert(!BF16 || (F16 && LOM == 0), "bf16 is a single-operand 2-byte format");
-  static_assert(!FP8 || (F16 && LOM == 0 && !BF16), "e4m3 is a single-operand 1-byte format");
-  static_assert(!F16X1 || (F16 && LOM == 0 && !BF16 && !FP8), "single fp16 is a single-operand 2-byte format");
-  constexpr bool OUT_BF16 = BF16 || FP8;     // SPLIT outputs: one bf16 array
-  constexpr int SGL = OUT_BF16 ? SGL_BF16 : F16X1 ? SGL_F16X1 : SGL_PAIRS;
-  using C = Cfg<LO, LO || OUT_BF16 || F16X1>;
+  static_assert(LOM == 0 || Fmt<FMT>::LO, "lo operands belong to the pair formats");
+  using C = Cfg<LO, LO || !Fmt<FMT>::LO>;
   if (ep.gate != nullptr && *reinterpret_cast<const volatile int*>(ep.gate) == 0) return;   // uniform over the grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -381,7 +350,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   const int wg = threadIdx.x >> 7;
   const int num_m = (M + BM - 1) / BM, num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
-  constexpr int BKE = FP8 ? 128 : F16 ? 64 : 32;         // elements per k-block (128 bytes)
+  constexpr int BKE = 128 / (int)sizeof(typename Fmt<FMT>::T);   // elements per k-block (128 bytes)
   const int num_k = (K + BKE - 1) / BKE;
 
   if (threadIdx.x == 0) {
@@ -443,7 +412,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
         bulk_wait_read<0>();
         for (int i = 0; i < 2; ++i) {
           const uint32_t b = (stg_cnt + i) & 1;
-          const int oc = n0 + i * StageFmt<STG_F32>::COLS;
+          const int oc = n0 + i * StageFmt<OUT_F32>::COLS;
           if (oc < N) resid_load(&tm_resid, stg + b * STG_BYTES, rbar + b, oc, m0);
         }
       }
@@ -456,11 +425,9 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k) {
           const uint64_t adv = (uint64_t)((k * 32) >> 4);      // +32 B per k-step inside the atom (both types)
-          if constexpr (FP8) wgmma_m64n128_e4m3(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
-          else if constexpr (BF16) wgmma_m64n128_bf16(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
-          else wgmma_m64n128<F16>(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
-          if (has_a_lo) wgmma_m64n128<F16>(acc, a_lo + adv, b_hi + adv, 1u);
-          if (has_b_lo) wgmma_m64n128<F16>(acc, a_hi + adv, b_lo + adv, 1u);
+          wgmma_m64n128<FMT>(acc, a_hi + adv, b_hi + adv, (kb != kb0 || k != 0) ? 1u : 0u);
+          if (has_a_lo) wgmma_m64n128<FMT>(acc, a_lo + adv, b_hi + adv, 1u);
+          if (has_b_lo) wgmma_m64n128<FMT>(acc, a_hi + adv, b_lo + adv, 1u);
         }
         wgmma_commit();
         // the previous k-block's wgmmas have retired once at most this one is in flight: free its stage
@@ -477,7 +444,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
     }
     if (t == 0) mbar_arrive(smem_u32(empty_bar + prev_stage));
     if (mode < 0 || m0 >= M) continue;       // discard (ANYLOC_GEMM_DEBUG_SKIP_EPI) / no rows for this warpgroup
-    if constexpr (FP8) {                     // dequantise A: row m's sums times its power-of-two scale (exact)
+    if constexpr (FMT == ANYLOC_PAIR_FP8) {  // dequantise A: row m's sums times its power-of-two scale (exact)
       const int r = m0 + warp * 16 + (lane >> 2);
       const float s0 = r < M ? __ldg(ep.row_scale + r) : 0.f, s1 = r + 8 < M ? __ldg(ep.row_scale + r + 8) : 0.f;
 #pragma unroll
@@ -488,26 +455,23 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       continue;
     }
     if (!staged) {
-      epilogue_pairs<SGL>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
+      epilogue_pairs<FMT>(ep, m0 + warp * 16 + (lane >> 2), n0 + 2 * (lane & 3), M, N, sum);
       continue;
     }
-#define ANYLOC_EPI_STAGED(KIND_, SWIGLU_, RESID_)                                                                   \
-  epilogue_staged<KIND_, SWIGLU_, RESID_>(ep, &tm_out, &tm_out_lo, &tm_resid, stg, rbar, rphase, stg_cnt, wg, t, m0, \
-                                          n0, N, sum)
-    if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(STG_F32, false, false);
-    else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(STG_F32, false, true);
-    else if (OUT_BF16) {                     // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> single bf16
-      if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_BF16, true, false);
-      else ANYLOC_EPI_STAGED(STG_BF16, false, false);
-    } else if (F16X1) {                      // -> single fp16
-      if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(STG_F16, true, false);
-      else ANYLOC_EPI_STAGED(STG_F16, false, false);
-    } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {
-      if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, true, false);
-      else ANYLOC_EPI_STAGED(STG_TF32_PAIR, true, false);
+#define ANYLOC_EPI_STAGED(OUT_, SWIGLU_, RESID_)                                                                    \
+  epilogue_staged<OUT_, SWIGLU_, RESID_>(ep, &tm_out, &tm_out_lo, &tm_resid, stg, rbar, rphase, stg_cnt, wg, t, m0,  \
+                                         n0, N, sum)
+    if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(OUT_F32, false, false);
+    else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(OUT_F32, false, true);
+    else if constexpr (!Fmt<FMT>::LO) {      // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> the single output format
+      if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(Fmt<FMT>::OUT, true, false);
+      else ANYLOC_EPI_STAGED(Fmt<FMT>::OUT, false, false);
+    } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {    // -> tf32 or fp16 pairs, as ep.out_fmt says
+      if (ep.out_fmt != ANYLOC_PAIR_TF32) ANYLOC_EPI_STAGED(ANYLOC_PAIR_F16, true, false);
+      else ANYLOC_EPI_STAGED(ANYLOC_PAIR_TF32, true, false);
     } else {                                 // BIAS_SPLIT / GELU_SPLIT
-      if (ep.out_f16) ANYLOC_EPI_STAGED(STG_F16_PAIR, false, false);
-      else ANYLOC_EPI_STAGED(STG_TF32_PAIR, false, false);
+      if (ep.out_fmt != ANYLOC_PAIR_TF32) ANYLOC_EPI_STAGED(ANYLOC_PAIR_F16, false, false);
+      else ANYLOC_EPI_STAGED(ANYLOC_PAIR_TF32, false, false);
     }
 #undef ANYLOC_EPI_STAGED
   }
@@ -532,49 +496,56 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16, bool fp8) {
+// tensor-map element type of fmt's arrays (the tf32 pairs' are fp32 words)
+static CUtensorMapDataType map_dtype(int fmt) {
+  switch (fmt) {
+    case ANYLOC_PAIR_FP8: return CU_TENSOR_MAP_DATA_TYPE_UINT8;
+    case ANYLOC_PAIR_BF16: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    case ANYLOC_PAIR_F16: case ANYLOC_PAIR_F16X1: return CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    default: return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  }
+}
+
+int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, int fmt) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
-  const int esz = fp8 ? 1 : f16 ? 2 : 4;
+  const int esz = format_info(fmt).esz;
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esz), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                 : f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  CUresult r = enc(map, dt, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  CUresult r = enc(map, map_dtype(fmt), 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("gemm_tc: cuTensorMapEncodeTiled failed (%d) rows=%d K=%d ld=%d", (int)r, rows, K, ld); return ANYLOC_ERR_CUDA; }
   return ANYLOC_OK;
 }
 
-int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, bool bf16) {
+int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, int fmt) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("tensor map: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
   cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)imgs};
   cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)rows * cols * 2};
   cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)ptr, dims,
+  CUresult r = enc(map, map_dtype(fmt), 3, (void*)ptr, dims,
                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("tensor map: cuTensorMapEncodeTiled failed (%d) imgs=%d rows=%d cols=%d", (int)r, imgs, rows, cols); return ANYLOC_ERR_CUDA; }
   return ANYLOC_OK;
 }
 
-// output map of the staged epilogue: [rows, cols] of esz-byte elements, row pitch ld, boxes of 64 rows x box_cols
-// swizzled as stg_off places them.  TMA clips the boxes at rows and cols, so the ld padding is never written.
-static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int esz, int box_cols,
-                        bool bf16 = false) {
+// output map of the staged epilogue: [rows, cols] of fmt's elements (ANYLOC_PAIR_TF32: fp32), row pitch ld, boxes of
+// 64 rows x box_cols swizzled as stg_off places them.  TMA clips the boxes at rows and cols, so the ld padding is never
+// written.
+static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int fmt, int box_cols) {
+  const int esz = format_info(fmt).esz;
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("gemm_tc: cuTensorMapEncodeTiled unavailable"); return ANYLOC_ERR_CUDA; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)STG_ROWS};
   cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                 : esz == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  CUresult r = enc(map, dt, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(map, map_dtype(fmt), 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    box_cols * esz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("gemm_tc: cuTensorMapEncodeTiled failed (%d) for the output: rows=%d cols=%d ld=%d", (int)r, rows, cols, ld); return ANYLOC_ERR_CUDA; }
@@ -586,32 +557,33 @@ static int make_out_map(CUtensorMap* map, const void* ptr, int rows, int cols, i
 // gemm_tc_supported).  The row-length condition is conservative: in one H100 run of the staged-path test without it,
 // a 68-column fp16 output (136 bytes per row) came back with its ldo padding columns 68..71 written, as if the store
 // clipped columns only to 16-byte units.  Not reproduced since (the condition keeps such shapes off the staged path).
-// sgl (SGL_BF16 / SGL_F16X1): the SPLIT outputs are one bf16 or fp16 array (64-column boxes, no lo map).
-static int make_epi_maps(const EpiParams& ep, int M, int N, CUtensorMap* m_out, CUtensorMap* m_lo, CUtensorMap* m_resid,
-                         bool* staged, int sgl) {
+// out: the SPLIT output format (ANYLOC_PAIR_*).
+static int make_epi_maps(const EpiParams& ep, int out, int M, int N, CUtensorMap* m_out, CUtensorMap* m_lo,
+                         CUtensorMap* m_resid, bool* staged) {
   memset(m_out, 0, sizeof(*m_out)); memset(m_lo, 0, sizeof(*m_lo)); memset(m_resid, 0, sizeof(*m_resid));
   const bool split = ep.mode == ANYLOC_EPI_BIAS_SPLIT || ep.mode == ANYLOC_EPI_GELU_SPLIT ||
                      ep.mode == ANYLOC_EPI_SWIGLU_SPLIT;
-  const bool single = sgl != SGL_PAIRS;
-  const int esz = split && (ep.out_f16 || single) ? 2 : 4;
+  const int fmt = split ? out : ANYLOC_PAIR_TF32;      // BIAS / LS_RESID: fp32
+  const FormatInfo& f = format_info(fmt);
+  const int esz = f.esz;
   const int n_out = ep.mode == ANYLOC_EPI_SWIGLU_SPLIT ? N / 2 : N;
   *staged = ep.mode >= 0 && ((long long)ep.ldo * esz) % 16 == 0 && ((long long)n_out * esz) % 16 == 0;
   if (!*staged) return ANYLOC_OK;
-  const int cols = split && single ? StageFmt<STG_BF16>::COLS
-                   : split && !ep.out_f16 ? StageFmt<STG_TF32_PAIR>::COLS : StageFmt<STG_F32>::COLS;
+  const bool lo = split && f.lo;
+  const int cols = STG_BYTES / STG_ROWS / (lo ? 2 : 1) / esz;     // StageFmt<out or OUT_F32>::COLS
   int rc;
-  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, esz, cols, split && sgl == SGL_BF16))) return rc;
-  if (split && !single && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, esz, cols))) return rc;
-  if (ep.mode == ANYLOC_EPI_LS_RESID && (rc = make_out_map(m_resid, ep.resid, M, n_out, ep.ldo, esz, cols))) return rc;
+  if ((rc = make_out_map(m_out, ep.out, M, n_out, ep.ldo, fmt, cols))) return rc;
+  if (lo && (rc = make_out_map(m_lo, ep.out_lo, M, n_out, ep.ldo, fmt, cols))) return rc;
+  if (ep.mode == ANYLOC_EPI_LS_RESID && (rc = make_out_map(m_resid, ep.resid, M, n_out, ep.ldo, fmt, cols))) return rc;
   return ANYLOC_OK;
 }
 
 }  // namespace tc
 
 bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb,
-                       int M, int N, int K, const EpiParams& ep, bool f16) {
+                       int M, int N, int K, const EpiParams& ep, int fmt) {
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  const int q = f16 ? 8 : 4;                 // elements per 16 bytes
+  const int q = 16 / format_info(fmt).esz;   // elements per 16 bytes
   if (M < 1 || N < 1 || K < q) return false;
   if ((K % q) || (lda % q) || (ldb % q)) return false;
   if (!al16(a_hi) || !al16(b_hi) || (a_lo && !al16(a_lo)) || (b_lo && !al16(b_lo))) return false;
@@ -624,37 +596,37 @@ bool gemm_tc_supported(const void* a_hi, const void* a_lo, int lda, const void* 
 // epilogue of this host thread's last launch (anyloc_gemm_tc_last_staged)
 static thread_local int g_last_staged = -1;
 
-template <bool F16, int LOM, bool BF16 = false, bool FP8 = false, bool F16X1 = false>
+template <int FMT, int LOM>
 static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
                        int N, int K, const EpiParams& ep, int chunk, cudaStream_t st) {
   using namespace tc;
   constexpr bool LO = LOM != 0;
-  using CF = Cfg<LO, LO || BF16 || FP8 || F16X1>;
+  using CF = Cfg<LO, LO || !Fmt<FMT>::LO>;
+  static_assert(CF::SMEM_BYTES_STAGED <= 232448, "GEMM over H100's shared-memory opt-in");
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   int rc;
-  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, F16, BF16, FP8))) return rc;
-  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, F16, BF16, FP8))) return rc;
-  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, F16, BF16, FP8))) return rc;
-  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, F16, BF16, FP8))) return rc;
+  if ((rc = make_map(&ma_hi, a_hi, M, K, lda, BM, FMT))) return rc;
+  if ((rc = make_map(&ma_lo, a_lo ? a_lo : a_hi, M, K, lda, BM, FMT))) return rc;
+  if ((rc = make_map(&mb_hi, b_hi, N, K, ldb, BN, FMT))) return rc;
+  if ((rc = make_map(&mb_lo, b_lo ? b_lo : b_hi, N, K, ldb, BN, FMT))) return rc;
   CUtensorMap mo, mo_lo, mr;
   bool staged = false;
   memset(&mo, 0, sizeof(mo)); memset(&mo_lo, 0, sizeof(mo_lo)); memset(&mr, 0, sizeof(mr));
   // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
   // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
   // for more would make the SM switch its shared-memory configuration back and forth).
-  constexpr int SGL = BF16 || FP8 ? SGL_BF16 : F16X1 ? SGL_F16X1 : SGL_PAIRS;
-  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, M, N, &mo, &mo_lo, &mr, &staged, SGL))) return rc;
+  const int out = Fmt<FMT>::LO ? (ep.out_fmt != ANYLOC_PAIR_TF32 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32) : Fmt<FMT>::OUT;
+  if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, out, M, N, &mo, &mo_lo, &mr, &staged))) return rc;
   const int smem = staged ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES;
   g_last_staged = staged ? 1 : 0;
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen)) {
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<F16, LOM, BF16, FP8, F16X1>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc3_kernel<FMT, LOM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            CF::STAGED ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES));
   }
   const int tiles = cdiv(M, BM) * cdiv(N, BN);
   const int grid = std::min(tiles, device_sm_count());
-  gemm_tc3_kernel<F16, LOM, BF16, FP8, F16X1><<<grid, THREADS, smem, st>>>(
+  gemm_tc3_kernel<FMT, LOM><<<grid, THREADS, smem, st>>>(
       ma_hi, ma_lo, mb_hi, mb_lo, mo, mo_lo, mr, staged ? 1 : 0, M, N, K, std::min(BAND_N, cdiv(N, BN)), chunk, ep);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
@@ -667,58 +639,49 @@ static int gemm_chunk_env() {
   return chunk_env;
 }
 
+// C = A . B^T + epilogue of fmt operands.  The pair formats take lo operands (a_lo, b_lo nullable); the single formats
+// take none, except single e4m3, whose a_lo holds A's fp32 row scales [M].  The single bf16 and fp16 GEMMs accumulate
+// in the fp16 pairs' round-to-nearest chunks (CHUNK_KB_F16), single e4m3 promotes every CHUNK_KB_FP8 k-blocks.  The
+// single formats have their own instantiations, so the hi-only coarse passes (<F16 | TF32, 0>) keep their register
+// epilogue and shared memory.
 int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo, int ldb, int M,
-                   int N, int K, const EpiParams& ep_in, bool f16, cudaStream_t st) {
+                   int N, int K, const EpiParams& ep_in, int fmt, cudaStream_t st) {
   const int chunk_env = gemm_chunk_env();
+  EpiParams ep = ep_in;
+  switch (fmt) {
+    case ANYLOC_PAIR_BF16:
+      return launch_impl<ANYLOC_PAIR_BF16, 0>(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
+    case ANYLOC_PAIR_F16X1:
+      return launch_impl<ANYLOC_PAIR_F16X1, 0>(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16,
+                                               st);
+    case ANYLOC_PAIR_FP8:
+      ep.row_scale = static_cast<const float*>(a_lo);
+      return launch_impl<ANYLOC_PAIR_FP8, 0>(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep,
+                                             chunk_env > 0 ? chunk_env : tc::CHUNK_KB_FP8, st);
+    default: break;
+  }
   // diagnostic only (tools/, never set by the product): bit m set -> GEMMs with epilogue mode m discard their result,
   // which exposes how much of a GEMM's time is its epilogue
   static int skip_epi = -1;
   if (skip_epi < 0) { const char* e = getenv("ANYLOC_GEMM_DEBUG_SKIP_EPI"); skip_epi = e ? atoi(e) : 0; }
-  EpiParams ep = ep_in;
   if (skip_epi && ((skip_epi >> ep_in.mode) & 1)) ep.mode = -1;
+  const bool f16 = fmt == ANYLOC_PAIR_F16;
   const int lom = (a_lo ? 1 : 0) | (b_lo ? 2 : 0);
   // hi-only fp16 pass = the retrieval's coarse scores, whose error bound allows long chunks
   const int chunk = lom == 0 ? (f16 ? tc::CHUNK_KB_COARSE : tc::CHUNK_KB_TF32)
                              : chunk_env > 0 ? chunk_env : (f16 ? tc::CHUNK_KB_F16 : tc::CHUNK_KB_TF32);
-#define ANYLOC_GEMM_LAUNCH(F16_, LOM_) launch_impl<F16_, LOM_>(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, chunk, st)
+#define ANYLOC_GEMM_LAUNCH(FMT_, LOM_) launch_impl<FMT_, LOM_>(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, chunk, st)
   switch (lom + (f16 ? 4 : 0)) {
-    case 0: return ANYLOC_GEMM_LAUNCH(false, 0);
-    case 1: return ANYLOC_GEMM_LAUNCH(false, 1);
-    case 2: return ANYLOC_GEMM_LAUNCH(false, 2);
-    case 3: return ANYLOC_GEMM_LAUNCH(false, 3);
-    case 4: return ANYLOC_GEMM_LAUNCH(true, 0);
-    case 5: return ANYLOC_GEMM_LAUNCH(true, 1);
-    case 6: return ANYLOC_GEMM_LAUNCH(true, 2);
-    default: return ANYLOC_GEMM_LAUNCH(true, 3);
+    case 0: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_TF32, 0);
+    case 1: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_TF32, 1);
+    case 2: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_TF32, 2);
+    case 3: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_TF32, 3);
+    case 4: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_F16, 0);
+    case 5: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_F16, 1);
+    case 6: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_F16, 2);
+    default: return ANYLOC_GEMM_LAUNCH(ANYLOC_PAIR_F16, 3);
   }
 #undef ANYLOC_GEMM_LAUNCH
-}
-
-// single-bf16 GEMM (ANYLOC_PAIR_BF16): one bf16 operand per side, one wgmma per k-step, fp32 accumulation in
-// round-to-nearest chunks as the fp16 pairs, staged epilogue; SPLIT outputs are one bf16 array
-int gemm_tc_bf16_launch(const void* a, int lda, const void* b, int ldb, int M, int N, int K, const EpiParams& ep,
-                        cudaStream_t st) {
-  static_assert(tc::Cfg<false, true>::SMEM_BYTES_STAGED <= 232448, "bf16 GEMM over H100's shared-memory opt-in");
-  return launch_impl<true, 0, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
-}
-
-// single-fp16 GEMM (ANYLOC_PAIR_F16X1): the hi halves of fp16 pairs, one wgmma per k-step, the fp16 pairs' chunks and
-// alpha, staged epilogue; SPLIT outputs are one fp16 array (the hi of the fp16 pair of kActScale v).  Its own
-// instantiation, so the hi-only coarse pass (gemm_tc3_kernel<true, 0>) keeps its register epilogue and shared memory.
-int gemm_tc_f16x1_launch(const void* a, int lda, const void* b, int ldb, int M, int N, int K, const EpiParams& ep,
-                         cudaStream_t st) {
-  return launch_impl<true, 0, false, false, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep, tc::CHUNK_KB_F16, st);
-}
-
-// single-e4m3 GEMM (ANYLOC_PAIR_FP8): e4m3 A rows with their scales a_scale [M], one e4m3 B, one wgmma per 32-element
-// k-step, the partial sums promoted every CHUNK_KB_FP8 k-blocks, staged epilogue; SPLIT outputs are one bf16 array
-int gemm_tc_fp8_launch(const void* a, const float* a_scale, int lda, const void* b, int ldb, int M, int N, int K,
-                       const EpiParams& ep_in, cudaStream_t st) {
-  EpiParams ep = ep_in;
-  ep.row_scale = a_scale;
-  const int chunk_env = gemm_chunk_env();
-  return launch_impl<true, 0, false, true>(a, nullptr, lda, b, nullptr, ldb, M, N, K, ep,
-                                           chunk_env > 0 ? chunk_env : tc::CHUNK_KB_FP8, st);
 }
 
 }  // namespace anyloc

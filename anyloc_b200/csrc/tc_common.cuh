@@ -1,7 +1,7 @@
 // wgmma / TMA / mbarrier building blocks shared by the tensor-core kernels of this library (sm_90a).
 #pragma once
 #include <cuda.h>
-#include "common.cuh"
+#include "formats.cuh"
 
 namespace anyloc {
 namespace tc {
@@ -81,86 +81,39 @@ __device__ __forceinline__ void fence_regs(float* d) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[64 x 128] (+)= A[64 x K] . B[128 x K]^T, both K-major in shared memory; K = 16 (f16) or 8 (tf32) per instruction.
+#define ANYLOC_WG_D64                                                                                               \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),       \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),        \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),       \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),       \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),       \
+      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),       \
+      "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),       \
+      "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define ANYLOC_WG_D64_STR                                                                                           \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "  \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define ANYLOC_WG_M64N128(SHAPE_TYPES, TAIL)                                                                        \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                 \
+               "wgmma.mma_async.sync.aligned.m64n128" SHAPE_TYPES " " ANYLOC_WG_D64_STR ", %64, %65, p, 1, 1" TAIL     \
+               ";\n\t}"                                                                                              \
+               : ANYLOC_WG_D64 : "l"(adesc), "l"(bdesc), "r"(scale_d))
+
+// D[64 x 128] (+)= A[64 x K] . B[128 x K]^T of FMT operands, both K-major in shared memory; 32 bytes of K per
+// instruction: K = 8 (tf32), 16 (fp16, bf16) or 32 (e4m3).
 // Accumulator layout (per warpgroup thread t, warp w = t / 32, lane l): d[4j + {0,1}] = row 16w + l/4, columns
 // 8j + 2(l%4) + {0,1}; d[4j + {2,3}] = row 16w + l/4 + 8, same columns.
-template <bool F16>
+template <int FMT>
 __device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (F16)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-        "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
-        "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-        "%64, %65, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(scale_d));
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-        "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
-        "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-        "%64, %65, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(scale_d));
+  if constexpr (FMT == ANYLOC_PAIR_TF32) ANYLOC_WG_M64N128("k8.f32.tf32.tf32", "");
+  else if constexpr (FMT == ANYLOC_PAIR_FP8) ANYLOC_WG_M64N128("k32.f32.e4m3.e4m3", "");
+  else if constexpr (FMT == ANYLOC_PAIR_BF16) ANYLOC_WG_M64N128("k16.f32.bf16.bf16", ", 0, 0");
+  else ANYLOC_WG_M64N128("k16.f32.f16.f16", ", 0, 0");     // fp16 pairs, single fp16
 }
-
-// The same product with bf16 operands (single bf16 format): K = 16 per instruction, fp16's rate and layout.
-__device__ __forceinline__ void wgmma_m64n128_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
-      "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(scale_d));
-}
-
-// The same product with e4m3 operands (single e4m3 format): K = 32 per instruction (32 bytes, as the 16-bit k-steps).
-__device__ __forceinline__ void wgmma_m64n128_e4m3(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
-      "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(scale_d));
-}
+#undef ANYLOC_WG_M64N128
+#undef ANYLOC_WG_D64
+#undef ANYLOC_WG_D64_STR
 
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
@@ -194,12 +147,12 @@ __device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
   "%24, %25, %26, %27, %28, %29, %30, %31}"
 
-// D[64 x 64] (+)= A[64 x 16] . B[64 x 16]^T, A and B K-major in shared memory (SS form); 16-bit operands, fp16 or bf16.
+// D[64 x 64] (+)= A[64 x 16] . B[64 x 16]^T, A and B K-major in shared memory (SS form); the 16-bit operands of FMT.
 // Accumulator layout as wgmma_m64n128's: d[4j + {0,1}] = row 16w + l/4, columns 8j + 2(l%4) + {0,1}; d[4j + {2,3}] =
 // row 16w + l/4 + 8.
-template <bool BF16>
+template <int FMT>
 __device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (BF16)
+  if constexpr (FMT == ANYLOC_PAIR_BF16)
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR ", %32, %33, p, 1, 1, 0, 0;\n\t}"
                  : ANYLOC_WG_D32 : "l"(adesc), "l"(bdesc), "r"(scale_d));
@@ -210,12 +163,12 @@ __device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t adesc, uint64
 }
 
 // D[64 x 64] (+)= A[64 x 16] . B[16 x 64], A from registers (RS form), B MN-major in shared memory (transposed B, 16-bit
-// types only).  The A fragment of warp w is mma.sync m16n8k16's for rows [16w, 16w + 16): a[0] = (row l/4, k 2(l%4) +
-// {0,1}), a[1] = row + 8, a[2] = k + 8, a[3] = both -- which is the accumulator layout of a 16-bit wgmma, two n8
-// column groups per k16 step.
-template <bool BF16>
+// types only), the operands of FMT.  The A fragment of warp w is mma.sync m16n8k16's for rows [16w, 16w + 16): a[0] =
+// (row l/4, k 2(l%4) + {0,1}), a[1] = row + 8, a[2] = k + 8, a[3] = both -- which is the accumulator layout of a 16-bit
+// wgmma, two n8 column groups per k16 step.
+template <int FMT>
 __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (BF16)
+  if constexpr (FMT == ANYLOC_PAIR_BF16)
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR
                  ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
@@ -229,13 +182,12 @@ __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t* a, 
 #undef ANYLOC_WG_D32
 #undef ANYLOC_WG_D32_STR
 
-// host: 2-D tiled tensor map over a row-major [rows, K] matrix (row pitch ld elements), box = 128 bytes of K x box_rows
-// rows, 128B swizzle (defined in gemm_tc.cu); elements are fp32, fp16 (f16), bf16 (f16 and bf16) or e4m3 bytes (fp8)
-int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, bool f16, bool bf16 = false,
-             bool fp8 = false);
-// host: 3-D tiled tensor map over imgs row-major [rows, cols] matrices of 2-byte elements (fp16, or bf16) laid end to
-// end, box = 64 columns (128 B) x box_rows rows x 1 matrix, 128B swizzle; boxes past `rows` of a matrix read zeros
-int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, bool bf16);
+// host: 2-D tiled tensor map over a row-major [rows, K] matrix of fmt's elements (row pitch ld elements), box = 128
+// bytes of K x box_rows rows, 128B swizzle (defined in gemm_tc.cu)
+int make_map(CUtensorMap* map, const void* ptr, int rows, int K, int ld, int box_rows, int fmt);
+// host: 3-D tiled tensor map over imgs row-major [rows, cols] matrices of fmt's 2-byte elements laid end to end, box =
+// 64 columns (128 B) x box_rows rows x 1 matrix, 128B swizzle; boxes past `rows` of a matrix read zeros
+int make_map_3d16(CUtensorMap* map, const void* ptr, int imgs, int rows, int cols, int box_rows, int fmt);
 
 }  // namespace tc
 }  // namespace anyloc

@@ -6,7 +6,7 @@
 // forward continues through.
 #include <string.h>
 #include <algorithm>
-#include "common.cuh"
+#include "formats.cuh"
 
 namespace anyloc {
 
@@ -25,8 +25,6 @@ __global__ void split_f16_kernel(const float* __restrict__ x, __half* __restrict
   for (; i < n; i += stride) { __half h, l; split_f16(x[i] * scale, h, l); hi[i] = h; lo[i] = l; }
 }
 
-// GEMM-input formats of the row kernels: FMT = ANYLOC_PAIR_TF32 (tf32 pairs), _F16 (fp16 pairs of kActScale*x), _BF16
-// (one bf16 array bf16_rn(x); the lo pointer is unused) or _F16X1 (the hi array of _F16 alone; lo unused)
 // x -> bf16_rn(x) (single bf16 format)
 __global__ void split_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -34,33 +32,13 @@ __global__ void split_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __
   for (; i < n; i += stride) y[i] = __float2bfloat16_rn(x[i]);
 }
 
-template <int FMT> struct PairOut;
-template <> struct PairOut<ANYLOC_PAIR_TF32> {
-  typedef float T;
-  static __device__ __forceinline__ void put(float* hi, float* lo, size_t i, float v) { float h, l; split_tf32(v, h, l); hi[i] = h; lo[i] = l; }
-};
-template <> struct PairOut<ANYLOC_PAIR_F16> {
-  typedef __half T;
-  static __device__ __forceinline__ void put(__half* hi, __half* lo, size_t i, float v) { __half h, l; split_f16(v * kActScale, h, l); hi[i] = h; lo[i] = l; }
-};
-template <> struct PairOut<ANYLOC_PAIR_BF16> {
-  typedef __nv_bfloat16 T;
-  static __device__ __forceinline__ void put(__nv_bfloat16* hi, __nv_bfloat16*, size_t i, float v) { hi[i] = __float2bfloat16_rn(v); }
-};
-template <> struct PairOut<ANYLOC_PAIR_F16X1> {    // the hi half of PairOut<ANYLOC_PAIR_F16>'s pair; lo unused
-  typedef __half T;
-  static __device__ __forceinline__ void put(__half* hi, __half*, size_t i, float v) { hi[i] = f16_hi(v * kActScale); }
-};
-template <> struct PairOut<ANYLOC_PAIR_FP8> {     // LayerNorm only: e4m3 rows, y_lo holds the fp32 row scales
-  typedef uint8_t T;
-};
-
+// The row kernels write their rows in the GEMM-input format FMT (formats.cuh); the single formats' lo pointer is unused.
 // patch pi of image b of img [B,3,H,W] -> patch row `row` of (hi,lo), column order (c, ky, kx) like conv
 // weight.flatten(1)
 template <int FMT>
 __device__ __forceinline__ void im2col_row(const float* __restrict__ img, int b, int H, int W, int P, int Kp, size_t row,
-                                           int pi, typename PairOut<FMT>::T* __restrict__ hi,
-                                           typename PairOut<FMT>::T* __restrict__ lo) {
+                                           int pi, typename Fmt<FMT>::T* __restrict__ hi,
+                                           typename Fmt<FMT>::T* __restrict__ lo) {
   const int gw = W / P;
   const int py = pi / gw, px = pi % gw;
   const int Kreal = 3 * P * P;
@@ -70,14 +48,14 @@ __device__ __forceinline__ void im2col_row(const float* __restrict__ img, int b,
       int ch = c / (P * P), rem = c % (P * P), ky = rem / P, kx = rem % P;
       v = __ldg(img + (((size_t)b * 3 + ch) * H + (py * P + ky)) * W + (px * P + kx));
     }
-    PairOut<FMT>::put(hi, lo, row * Kp + c, v);
+    put1<FMT>(hi, lo, row * Kp + c, v);
   }
 }
 
 // img [B,3,H,W] -> patches (hi,lo) [B*gh*gw, Kp]
 template <int FMT>
 __global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H, int W, int P, int Kp,
-                                    typename PairOut<FMT>::T* __restrict__ hi, typename PairOut<FMT>::T* __restrict__ lo) {
+                                    typename Fmt<FMT>::T* __restrict__ hi, typename Fmt<FMT>::T* __restrict__ lo) {
   const int gh = H / P, gw = W / P;
   const size_t row = blockIdx.x;               // patch index
   const int b = (int)(row / (gh * gw)), pi = (int)(row % (gh * gw));
@@ -87,8 +65,8 @@ __global__ void im2col_split_kernel(const float* __restrict__ img, int B, int H,
 // images of different sizes, one block per patch row of the packed [sum gh_i*gw_i, Kp] output
 template <int FMT>
 __global__ void im2col_split_varlen_kernel(const __grid_constant__ VarlenImgTable tab, int P, int Kp,
-                                           typename PairOut<FMT>::T* __restrict__ hi,
-                                           typename PairOut<FMT>::T* __restrict__ lo) {
+                                           typename Fmt<FMT>::T* __restrict__ hi,
+                                           typename Fmt<FMT>::T* __restrict__ lo) {
   const int skip = 1 + tab.nreg, row = blockIdx.x, i = varlen_image_of(tab, row, skip);
   im2col_row<FMT>(tab.ptr[i], 0, tab.gh[i] * P, tab.gw[i] * P, P, Kp, row, row - (tab.tok0[i] - skip * i), hi, lo);
 }
@@ -133,7 +111,7 @@ template <int MAXV, int FMT>   // float4 per lane
 __global__ void __launch_bounds__(256)
 layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
                        const float* __restrict__ b, int M, int D, float eps,
-                       typename PairOut<FMT>::T* __restrict__ y_hi, typename PairOut<FMT>::T* __restrict__ y_lo) {
+                       typename Fmt<FMT>::T* __restrict__ y_hi, typename Fmt<FMT>::T* __restrict__ y_lo) {
   const int lane = threadIdx.x & 31;
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (row >= M) return;
@@ -189,23 +167,7 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
       float4 ww = __ldg(w4 + d), bb = __ldg(b4 + d);
       const float y0 = (v[i].x - mean) * rstd * ww.x + bb.x, y1 = (v[i].y - mean) * rstd * ww.y + bb.y;
       const float y2 = (v[i].z - mean) * rstd * ww.z + bb.z, y3 = (v[i].w - mean) * rstd * ww.w + bb.w;
-      if constexpr (FMT == ANYLOC_PAIR_BF16) {
-        reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] = make_uint2(pack_bf16x2(y0, y1), pack_bf16x2(y2, y3));
-      } else if constexpr (FMT == ANYLOC_PAIR_F16X1) {
-        reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] =
-            make_uint2(pack_f16x2_hi(y0 * kActScale, y1 * kActScale), pack_f16x2_hi(y2 * kActScale, y3 * kActScale));
-      } else if constexpr (FMT == ANYLOC_PAIR_F16) {
-        uint2 h, l;
-        split_f16x2(y0 * kActScale, y1 * kActScale, h.x, l.x);
-        split_f16x2(y2 * kActScale, y3 * kActScale, h.y, l.y);
-        reinterpret_cast<uint2*>(y_hi + (size_t)row * D)[d] = h;
-        reinterpret_cast<uint2*>(y_lo + (size_t)row * D)[d] = l;
-      } else {
-        float4 h, l;
-        split_tf32(y0, h.x, l.x); split_tf32(y1, h.y, l.y); split_tf32(y2, h.z, l.z); split_tf32(y3, h.w, l.w);
-        reinterpret_cast<float4*>(y_hi + (size_t)row * D)[d] = h;
-        reinterpret_cast<float4*>(y_lo + (size_t)row * D)[d] = l;
-      }
+      Fmt<FMT>::put4(y_hi + (size_t)row * D, y_lo + (size_t)row * D, d, y0, y1, y2, y3);
     }
   }
   }
@@ -302,12 +264,23 @@ __device__ __forceinline__ void facet_row(int lane, const float* __restrict__ x,
   }
 }
 
+// one third's float4s v (lane, lane + 32, ...) -> its operands in the format FMT from element off of hi (and lo)
+template <int FMT, int MAXV>
+__device__ __forceinline__ void qkv_tap_put(int lane, int D4, const float4 (&v)[MAXV], void* hi, void* lo, int f, int D) {
+  typename Fmt<FMT>::T* h = reinterpret_cast<typename Fmt<FMT>::T*>(hi) + (size_t)f * D;
+  typename Fmt<FMT>::T* l = reinterpret_cast<typename Fmt<FMT>::T*>(lo) + (size_t)f * D;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    const int d = lane + i * 32;
+    if (d < D4) Fmt<FMT>::put4(h, l, d, v[i].x, v[i].y, v[i].z, v[i].w);
+  }
+}
+
 // One fp32 row [q | k | v] of a tapped layer's qkv GEMM (3D columns, one warp, each element read once) -> the
-// attention's operand pairs of the row, in the format the qkv GEMM's split epilogue writes (pair: 0 none, 1 tf32
-// pairs, 2 fp16 pairs of kActScale*x; epi_store_split's split; 3 single bf16, lo unused; 4 single fp16, the hi of
-// pair 2's fp16 pair, lo unused), and the rows of the requested facets (out[f] != null), through facet_row's arithmetic.
+// attention's operands of the row in the format fmt (ANYLOC_PAIR_* but e4m3, or FMT_NONE for none), as the qkv GEMM's
+// split epilogue writes them, and the rows of the requested facets (out[f] != null), through facet_row's arithmetic.
 template <int MAXV>     // float4 per lane and third: D <= 128 * MAXV
-__device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int pair, void* hi,
+__device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int fmt, void* hi,
                                             void* lo, const QkvTapOuts& o, int64_t orow, int do_norm) {
   const int D4 = D >> 2;
 #pragma unroll 1
@@ -317,48 +290,10 @@ __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < MAXV; ++i)
       if (lane + i * 32 < D4) v[i] = xr[lane + i * 32];
-    if (pair == 3) {
-      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(hi) + (size_t)f * D);
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int d = lane + i * 32;
-        if (d < D4) h2[d] = make_uint2(pack_bf16x2(v[i].x, v[i].y), pack_bf16x2(v[i].z, v[i].w));
-      }
-    } else if (pair == 4) {
-      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int d = lane + i * 32;
-        if (d < D4)
-          h2[d] = make_uint2(pack_f16x2_hi(v[i].x * kActScale, v[i].y * kActScale),
-                             pack_f16x2_hi(v[i].z * kActScale, v[i].w * kActScale));
-      }
-    } else if (pair == 2) {
-      uint2* h2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(hi) + (size_t)f * D);
-      uint2* l2 = reinterpret_cast<uint2*>(reinterpret_cast<__half*>(lo) + (size_t)f * D);
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int d = lane + i * 32;
-        if (d < D4) {
-          uint2 h, l;
-          split_f16x2(v[i].x * kActScale, v[i].y * kActScale, h.x, l.x);
-          split_f16x2(v[i].z * kActScale, v[i].w * kActScale, h.y, l.y);
-          h2[d] = h; l2[d] = l;
-        }
-      }
-    } else if (pair == 1) {
-      float4* h4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(hi) + (size_t)f * D);
-      float4* l4 = reinterpret_cast<float4*>(reinterpret_cast<float*>(lo) + (size_t)f * D);
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int d = lane + i * 32;
-        if (d < D4) {
-          float4 h, l;
-          split_tf32(v[i].x, h.x, l.x); split_tf32(v[i].y, h.y, l.y); split_tf32(v[i].z, h.z, l.z); split_tf32(v[i].w, h.w, l.w);
-          h4[d] = h; l4[d] = l;
-        }
-      }
-    }
+    if (fmt == ANYLOC_PAIR_BF16) qkv_tap_put<ANYLOC_PAIR_BF16, MAXV>(lane, D4, v, hi, lo, f, D);
+    else if (fmt == ANYLOC_PAIR_F16X1) qkv_tap_put<ANYLOC_PAIR_F16X1, MAXV>(lane, D4, v, hi, lo, f, D);
+    else if (fmt == ANYLOC_PAIR_F16) qkv_tap_put<ANYLOC_PAIR_F16, MAXV>(lane, D4, v, hi, lo, f, D);
+    else if (fmt == ANYLOC_PAIR_TF32) qkv_tap_put<ANYLOC_PAIR_TF32, MAXV>(lane, D4, v, hi, lo, f, D);
     float* out = f == 0 ? o.out[0] : f == 1 ? o.out[1] : o.out[2];     // (not o.out[f]: no local-memory copy)
     if (out == nullptr || orow < 0) continue;
     float4* yr = reinterpret_cast<float4*>(out + orow * D);
@@ -376,30 +311,30 @@ __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ 
 // B images of T tokens: token row r -> output row r (use_cls) or r - b - 1 (its cls row has none)
 template <int MAXV>
 __global__ void __launch_bounds__(256)
-qkv_tap_kernel(const float* __restrict__ src, int M, int T, int D, int pair, void* hi, void* lo, const QkvTapOuts o,
+qkv_tap_kernel(const float* __restrict__ src, int M, int T, int D, int fmt, void* hi, void* lo, const QkvTapOuts o,
                int use_cls, int do_norm) {
   const int lane = threadIdx.x & 31;
   const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (row >= M) return;
   const int b = row / T, t = row - b * T;
   const int64_t orow = use_cls ? row : (t == 0 ? -1 : row - b - 1);
-  const size_t e = (size_t)row * 3 * D * (pair >= 2 ? 2 : 4);     // byte offset of the row's pairs
-  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
+  const size_t e = (size_t)row * 3 * D * (fmt == ANYLOC_PAIR_TF32 ? 4 : 2);     // byte offset of the row's operands
+  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, fmt, fmt != FMT_NONE ? (char*)hi + e : nullptr,
                     lo ? (char*)lo + e : nullptr, o, orow, do_norm);
 }
 
 // images of different sizes packed row after row: image i's tokens from tab.tok0[i]
 template <int MAXV>
 __global__ void __launch_bounds__(256)
-qkv_tap_varlen_kernel(const float* __restrict__ src, const __grid_constant__ VarlenImgTable tab, int M, int D, int pair,
+qkv_tap_varlen_kernel(const float* __restrict__ src, const __grid_constant__ VarlenImgTable tab, int M, int D, int fmt,
                       void* hi, void* lo, const QkvTapOuts o, int use_cls, int do_norm) {
   const int lane = threadIdx.x & 31;
   const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (row >= M) return;
   const int i = varlen_image_of(tab, row, 0);
   const int64_t orow = use_cls ? row : (row == tab.tok0[i] ? -1 : row - i - 1);
-  const size_t e = (size_t)row * 3 * D * (pair >= 2 ? 2 : 4);
-  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, pair, pair ? (char*)hi + e : nullptr,
+  const size_t e = (size_t)row * 3 * D * (fmt == ANYLOC_PAIR_TF32 ? 4 : 2);
+  qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, fmt, fmt != FMT_NONE ? (char*)hi + e : nullptr,
                     lo ? (char*)lo + e : nullptr, o, orow, do_norm);
 }
 
@@ -448,18 +383,21 @@ int launch_split_bf16(const float* x, void* y, size_t n, cudaStream_t st) {
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-// fmt: ANYLOC_PAIR_* of the patch rows (bf16 and single fp16: lo unused)
+// fmt: ANYLOC_PAIR_* of the patch rows (not e4m3)
 int launch_im2col(const float* img, int B, int H, int W, int P, int Kp, void* hi, void* lo, int fmt, cudaStream_t st) {
   const int n = B * (H / P) * (W / P);
-  if (fmt == ANYLOC_PAIR_BF16)
-    im2col_split_kernel<ANYLOC_PAIR_BF16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__nv_bfloat16*)hi, nullptr);
-  else if (fmt == ANYLOC_PAIR_F16X1)
-    im2col_split_kernel<ANYLOC_PAIR_F16X1><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, nullptr);
-  else if (fmt == ANYLOC_PAIR_F16)
-    im2col_split_kernel<ANYLOC_PAIR_F16><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (__half*)hi, (__half*)lo);
-  else im2col_split_kernel<ANYLOC_PAIR_TF32><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (float*)hi, (float*)lo);
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  return fmt_switch(fmt, [&](auto c) {
+    constexpr int FMT = decltype(c)::value;
+    typedef typename Fmt<FMT>::T T;
+    if constexpr (FMT == ANYLOC_PAIR_FP8) {
+      set_error("im2col: no e4m3 patch rows");
+      return (int)ANYLOC_ERR_ARG;
+    } else {
+      im2col_split_kernel<FMT><<<n, 128, 0, st>>>(img, B, H, W, P, Kp, (T*)hi, (T*)lo);
+      ANYLOC_CHECK_LAUNCH();
+      return (int)ANYLOC_OK;
+    }
+  });
 }
 int launch_assemble(const float* patch, const float* cls, const float* reg, const float* pos, int B, int N, int R, int D,
                     float* x, cudaStream_t st) {
@@ -467,24 +405,18 @@ int launch_assemble(const float* patch, const float* cls, const float* reg, cons
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-template <int FMT>
-static void ln_launch(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi, void* y_lo,
-                      cudaStream_t st) {
-  typedef typename PairOut<FMT>::T T;
-  int blocks = cdiv(M, 8);
-  if (D <= 512) layernorm_split_kernel<4, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
-  else if (D <= 1024) layernorm_split_kernel<8, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
-  else layernorm_split_kernel<16, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
-}
-// fmt: ANYLOC_PAIR_* of the output (bf16 and single fp16: y_lo unused; fp8: y_lo = the fp32 row scales [M])
+// fmt: ANYLOC_PAIR_* of the output (fp8: y_lo = the fp32 row scales [M])
 int launch_layernorm(const float* x, const float* w, const float* b, int M, int D, float eps, void* y_hi,
                      void* y_lo, int fmt, cudaStream_t st) {
   ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "layernorm: D=%d unsupported (multiple of 4, <= 2048)", D);
-  if (fmt == ANYLOC_PAIR_FP8) ln_launch<ANYLOC_PAIR_FP8>(x, w, b, M, D, eps, y_hi, y_lo, st);
-  else if (fmt == ANYLOC_PAIR_BF16) ln_launch<ANYLOC_PAIR_BF16>(x, w, b, M, D, eps, y_hi, nullptr, st);
-  else if (fmt == ANYLOC_PAIR_F16X1) ln_launch<ANYLOC_PAIR_F16X1>(x, w, b, M, D, eps, y_hi, nullptr, st);
-  else if (fmt == ANYLOC_PAIR_F16) ln_launch<ANYLOC_PAIR_F16>(x, w, b, M, D, eps, y_hi, y_lo, st);
-  else ln_launch<ANYLOC_PAIR_TF32>(x, w, b, M, D, eps, y_hi, y_lo, st);
+  fmt_switch(fmt, [&](auto c) {
+    constexpr int FMT = decltype(c)::value;
+    typedef typename Fmt<FMT>::T T;
+    const int blocks = cdiv(M, 8);
+    if (D <= 512) layernorm_split_kernel<4, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+    else if (D <= 1024) layernorm_split_kernel<8, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+    else layernorm_split_kernel<16, FMT><<<blocks, 256, 0, st>>>(x, w, b, M, D, eps, (T*)y_hi, (T*)y_lo);
+  });
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
@@ -530,15 +462,18 @@ int launch_facet_out(const float* src, int B, int T, int64_t ld, int col0, int D
 // packed batches of differently sized images: tab.ptr holds the images (im2col) or the positional tables (assembly)
 int launch_im2col_varlen(const VarlenImgTable& tab, int n_patches, int P, int Kp, void* hi, void* lo, int fmt,
                          cudaStream_t st) {
-  if (fmt == ANYLOC_PAIR_BF16)
-    im2col_split_varlen_kernel<ANYLOC_PAIR_BF16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__nv_bfloat16*)hi, nullptr);
-  else if (fmt == ANYLOC_PAIR_F16X1)
-    im2col_split_varlen_kernel<ANYLOC_PAIR_F16X1><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, nullptr);
-  else if (fmt == ANYLOC_PAIR_F16)
-    im2col_split_varlen_kernel<ANYLOC_PAIR_F16><<<n_patches, 128, 0, st>>>(tab, P, Kp, (__half*)hi, (__half*)lo);
-  else im2col_split_varlen_kernel<ANYLOC_PAIR_TF32><<<n_patches, 128, 0, st>>>(tab, P, Kp, (float*)hi, (float*)lo);
-  ANYLOC_CHECK_LAUNCH();
-  return ANYLOC_OK;
+  return fmt_switch(fmt, [&](auto c) {
+    constexpr int FMT = decltype(c)::value;
+    typedef typename Fmt<FMT>::T T;
+    if constexpr (FMT == ANYLOC_PAIR_FP8) {
+      set_error("im2col: no e4m3 patch rows");
+      return (int)ANYLOC_ERR_ARG;
+    } else {
+      im2col_split_varlen_kernel<FMT><<<n_patches, 128, 0, st>>>(tab, P, Kp, (T*)hi, (T*)lo);
+      ANYLOC_CHECK_LAUNCH();
+      return (int)ANYLOC_OK;
+    }
+  });
 }
 int launch_assemble_varlen(const float* patch, const float* cls, const float* reg, const VarlenImgTable& tab,
                            int n_tokens, int D, float* x, cudaStream_t st) {
@@ -552,21 +487,20 @@ int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int row
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
-// the fp32 qkv rows [M, 3D] of a tapped layer -> pairs (hi, lo; null: none; pair 3 / 4: single bf16 / fp16 in hi) and
-// facet rows; tab: packed images, else
-// B images of T tokens
+// the fp32 qkv rows [M, 3D] of a tapped layer -> the attention's operands in the format fmt (or FMT_NONE) and facet
+// rows; tab: packed images, else B images of T tokens
 template <int MAXV>
-static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi,
+static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int fmt, void* hi,
                            void* lo, const QkvTapOuts& o, int use_cls, int do_norm, cudaStream_t st) {
-  if (tab) qkv_tap_varlen_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, pair, hi, lo, o, use_cls, do_norm);
-  else qkv_tap_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, M, T, D, pair, hi, lo, o, use_cls, do_norm);
+  if (tab) qkv_tap_varlen_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, fmt, hi, lo, o, use_cls, do_norm);
+  else qkv_tap_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, M, T, D, fmt, hi, lo, o, use_cls, do_norm);
 }
-int launch_qkv_tap(const float* src, int M, int T, const VarlenImgTable* tab, int D, int pair, void* hi, void* lo,
+int launch_qkv_tap(const float* src, int M, int T, const VarlenImgTable* tab, int D, int fmt, void* hi, void* lo,
                    const QkvTapOuts& o, int use_cls, int do_norm, cudaStream_t st) {
   ANYLOC_REQUIRE(D % 4 == 0 && D <= 2048, "qkv_tap: D=%d unsupported (multiple of 4, <= 2048)", D);
-  if (D <= 512) qkv_tap_launch<4>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
-  else if (D <= 1024) qkv_tap_launch<8>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
-  else qkv_tap_launch<16>(src, M, T, tab, D, pair, hi, lo, o, use_cls, do_norm, st);
+  if (D <= 512) qkv_tap_launch<4>(src, M, T, tab, D, fmt, hi, lo, o, use_cls, do_norm, st);
+  else if (D <= 1024) qkv_tap_launch<8>(src, M, T, tab, D, fmt, hi, lo, o, use_cls, do_norm, st);
+  else qkv_tap_launch<16>(src, M, T, tab, D, fmt, hi, lo, o, use_cls, do_norm, st);
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }

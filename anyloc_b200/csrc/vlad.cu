@@ -791,10 +791,10 @@ using namespace anyloc;
 
 namespace anyloc {
 // GEMM engines (gemm_tc.cu)
-int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int, int, int, int, const EpiParams&, bool,
+int gemm_tc_launch(const void*, const void*, int, const void*, const void*, int, int, int, int, const EpiParams&, int,
                    cudaStream_t);
 bool gemm_tc_supported(const void*, const void*, int, const void*, const void*, int, int, int, int, const EpiParams&,
-                       bool);
+                       int);
 }  // namespace anyloc
 
 namespace {
@@ -817,9 +817,9 @@ int launch_assign(const float* feats, const int32_t* n_valid, int N_per_img, int
   }
   EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, K};
   const bool fast = ab.coarse != nullptr && D <= 2048 && R >= 256 && R < (1ll << 31) &&
-                    gemm_tc_supported(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, false);
+                    gemm_tc_supported(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, ANYLOC_PAIR_TF32);
   if (fast) {
-    int rc = gemm_tc_launch(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, false, st);
+    int rc = gemm_tc_launch(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, ANYLOC_PAIR_TF32, st);
     if (rc) return rc;
     const int blocks = (int)((R + 7) / 8);
     if (D <= 512)
