@@ -21,6 +21,7 @@ ENGINE = {"auto": 0, "simt": 1, "tc3": 2}
 PAIR = {"tf32": 0, "f16": 1, "bf16": 2, "fp8": 3, "f16x1": 4}
 ACT_SCALE = 8.0     # kActScale in csrc/common.cuh
 VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_extract_varlen call
+PREPROCESS_VARLEN_BATCH = 64    # ANYLOC_PREPROCESS_VARLEN_BATCH: images per launch of anyloc_preprocess_u8_varlen
 ERR = {"arg": -1, "cuda": -2, "workspace": -3, "unsupported": -4}
 
 
@@ -72,6 +73,9 @@ _SIGS = {
                              [C.c_void_p, C.c_void_p]),
     "anyloc_preprocess_resize_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 10 + [C.POINTER(C.c_float)] * 2 +
                                     [C.c_void_p, C.c_void_p]),
+    "anyloc_preprocess_u8_varlen": (C.c_int, [C.c_int, C.POINTER(C.c_void_p)] + [C.POINTER(C.c_int)] * 4 + [C.c_int] +
+                                    [C.POINTER(C.c_int)] * 4 + [C.POINTER(C.c_float)] * 2 +
+                                    [C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "anyloc_pool": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     "anyloc_vlad_residuals": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_void_p]),
     "anyloc_vlad_from_residuals_workspace_bytes": (C.c_size_t, [C.c_int] * 2),

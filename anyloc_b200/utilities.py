@@ -230,16 +230,138 @@ def center_crop_box(h: int, w: int, patch: int = 14) -> Tuple[int, int, int, int
 _INTERP = {"bilinear": 0, "bicubic": 1}
 
 
-def preprocess_images(imgs: Union[np.ndarray, torch.Tensor], mean=IMAGENET_MEAN, std=IMAGENET_STD,
+def max_side_size(h: int, w: int, max_side: int) -> Tuple[int, int]:
+    """The size the reference demo resizes an h x w photo to (demo/anyloc_vlad_generate.py:165-173): when the longer
+    side is over `max_side` it becomes `max_side` and the other side keeps the aspect ratio, rounded down; otherwise
+    (h, w) unchanged."""
+    if max(h, w) > max_side:
+        if h == max(h, w):
+            w = int(w * max_side / h)
+            h = max_side
+        else:
+            h = int(h * max_side / w)
+            w = max_side
+    return h, w
+
+
+def _resized_size(H, W, resize, max_side):
+    """-> (hr, wr, resized): the size an H x W image is resized to before the centre crop, and whether it is resized"""
+    if max_side is not None:
+        hr, wr = max_side_size(H, W, int(max_side))
+        return hr, wr, (hr, wr) != (H, W)
+    if resize is not None:
+        return int(resize[0]), int(resize[1]), True
+    return H, W, False
+
+
+def _list_geometry(shapes, patch, resize, max_side):
+    """Per (H, W) of a list: (hr, wr, resized, top, left, hc, wc); ValueError for an image smaller than one patch after
+    the resize.  Pure: no device work."""
+    geo = []
+    for k, (H, W) in enumerate(shapes):
+        hr, wr, resized = _resized_size(H, W, resize, max_side)
+        top, left, hc, wc = center_crop_box(hr, wr, patch) if hr > 0 and wr > 0 else (0, 0, 0, 0)
+        if hc == 0 or wc == 0:
+            raise ValueError(f"image {k} ({H}x{W}, resized to {hr}x{wr}) is smaller than one {patch}x{patch} patch")
+        geo.append((hr, wr, resized, top, left, hc, wc))
+    return geo
+
+
+def _check_resize_args(resize, max_side, interpolation):
+    if interpolation not in _INTERP:
+        raise ValueError(f"interpolation must be one of {sorted(_INTERP)}, got {interpolation!r}")
+    if resize is not None and max_side is not None:
+        raise ValueError("give resize=(h, w) or max_side, not both")
+    if max_side is not None and int(max_side) < 1:
+        raise ValueError(f"max_side must be positive, got {max_side!r}")
+
+
+def _preprocess_list(items, mean, std, patch, device, resize, interpolation, max_side):
+    """preprocess_images on a list / tuple of [H_i,W_i,3] uint8 images (see there)"""
+    _check_resize_args(resize, max_side, interpolation)
+    if len(items) == 0:
+        raise ValueError("preprocess_images got an empty list")
+    imgs = []
+    for k, x in enumerate(items):
+        if type(x) == np.ndarray:
+            x = torch.from_numpy(x)
+        if not isinstance(x, torch.Tensor):
+            raise TypeError(f"preprocess_images: item {k} is a {type(x).__name__}, expected a uint8 array or tensor")
+        if x.dtype != torch.uint8:
+            raise TypeError(f"preprocess_images expects uint8 pixels, got {x.dtype} (item {k})")
+        if x.dim() != 3 or x.shape[-1] != 3:
+            raise ValueError(f"preprocess_images expects list items [H,W,3], got {tuple(x.shape)} (item {k})")
+        if x.shape[0] == 0 or x.shape[1] == 0:
+            raise ValueError(f"preprocess_images: item {k} is empty ({tuple(x.shape)})")
+        imgs.append(x)
+    geo = _list_geometry([(x.shape[0], x.shape[1]) for x in imgs], patch, resize, max_side)
+    on_dev = {x.device for x in imgs if x.is_cuda}
+    if len(on_dev) > 1:
+        raise ValueError(f"preprocess_images: the list's device images are on several devices {sorted(map(str, on_dev))}")
+    dev = _lib.require_cuda(on_dev.pop() if on_dev else (torch.device(device) if device is not None else None))
+    with torch.cuda.device(dev):
+        # host images: gathered into one pinned buffer, one copy; device images: read in place
+        src = [x.contiguous() if x.is_cuda else None for x in imgs]
+        host = [k for k, x in enumerate(imgs) if not x.is_cuda]
+        if host:
+            staging = torch.empty(sum(imgs[k].numel() for k in host), dtype=torch.uint8, pin_memory=True)
+            views, o = {}, 0
+            for k in host:
+                n = imgs[k].numel()
+                staging[o:o + n].view(imgs[k].shape).copy_(imgs[k])
+                views[k], o = (o, n), o + n
+            dbuf = staging.to(dev, non_blocking=True)
+            for k, (o, n) in views.items():
+                src[k] = dbuf[o:o + n]
+        sizes = [3 * g[5] * g[6] for g in geo]
+        offs = np.concatenate(([0], np.cumsum(sizes)[:-1])).astype(np.int64)
+        flat = torch.empty(int(sum(sizes)), device=dev, dtype=torch.float32)
+        m3 = (C.c_float * 3)(*[float(v) for v in mean])
+        s3 = (C.c_float * 3)(*[float(v) for v in std])
+        for resized in (False, True):
+            idx = [k for k, g in enumerate(geo) if g[2] == resized]
+            if not idx:
+                continue
+            n = len(idx)
+
+            def ints(col):
+                return (C.c_int * n)(*[int(col(k)) for k in idx])
+            rc = _lib.load().anyloc_preprocess_u8_varlen(
+                n, (C.c_void_p * n)(*[src[k].data_ptr() for k in idx]), ints(lambda k: imgs[k].shape[0]),
+                ints(lambda k: imgs[k].shape[1]), ints(lambda k: geo[k][0]), ints(lambda k: geo[k][1]),
+                _INTERP[interpolation] if resized else -1, ints(lambda k: geo[k][3]), ints(lambda k: geo[k][4]),
+                ints(lambda k: geo[k][5]), ints(lambda k: geo[k][6]), m3, s3, _lib.ptr(flat),
+                (C.c_int64 * n)(*[int(offs[k]) for k in idx]), _lib.stream_ptr())
+            _lib.check(rc, "anyloc_preprocess_u8_varlen")
+    if resize is not None:
+        return flat.view(len(geo), 3, geo[0][5], geo[0][6])
+    return [flat[o:o + s].view(3, g[5], g[6]) for o, s, g in zip(offs.tolist(), sizes, geo)]
+
+
+def preprocess_images(imgs: Union[np.ndarray, torch.Tensor, list, tuple], mean=IMAGENET_MEAN, std=IMAGENET_STD,
                       patch: int = 14, device: Union[str, torch.device, None] = None,
-                      resize: Union[Tuple[int, int], None] = None, interpolation: str = "bilinear") -> torch.Tensor:
+                      resize: Union[Tuple[int, int], None] = None, interpolation: str = "bilinear",
+                      max_side: Union[int, None] = None):
     """uint8 RGB images [B,H,W,3] (or one [H,W,3]) -> the extractor's input [B,3,H',W'] on the GPU: the reference's
     `base_transform` (ToTensor + Normalize, dvgl_benchmark/datasets_ws.py:20-23), optionally the dataset loader's
     `T.functional.resize(img, resize)` (:233-235, `resize=(480, 640)` is the reference default, configs.py:141; or the
     demo's bicubic down-scaling, demo/anyloc_vlad_generate.py:165-177) and the centre crop to a multiple of the patch
     size (scripts/dino_v2_vlad.py:174-176) in ONE kernel.  Without `resize` the result is bit-identical to the
     torchvision pipeline; with it, antialiased bilinear / bicubic resampling as torchvision applies to tensors (fp32
-    rounding differences only).  A quarter of the host->device bytes of sending normalised fp32 images."""
+    rounding differences only).  A quarter of the host->device bytes of sending normalised fp32 images.
+
+    `max_side` applies the demo's rule instead of a fixed `resize`: an image whose longer side is over `max_side` is
+    resized to the size `max_side_size` gives (demo/anyloc_vlad_generate.py:165-177, `max_side=1024`,
+    `interpolation="bicubic"` there), any other is only normalised and cropped.
+
+    `imgs` may also be a list or tuple of differently sized [H_i,W_i,3] uint8 arrays or tensors, on the host or the
+    device (host images are gathered into one pinned buffer and copied once; device images are read in place), all
+    pre-processed in one launch per 64 images (two groups when `max_side` resizes some images and not others).  With
+    `resize` every item has the same size and the result is one [B,3,h,w] tensor; otherwise it is a list of [3,h_i,w_i]
+    views of one allocation, which DinoV2ExtractFeatures and DinoV2MultiExtractFeatures take as a list input.  Each
+    item is bit-identical to this function on that image alone."""
+    if isinstance(imgs, (list, tuple)):
+        return _preprocess_list(imgs, mean, std, patch, device, resize, interpolation, max_side)
     if type(imgs) == np.ndarray:
         imgs = torch.from_numpy(imgs)
     if imgs.dtype != torch.uint8:
@@ -248,12 +370,11 @@ def preprocess_images(imgs: Union[np.ndarray, torch.Tensor], mean=IMAGENET_MEAN,
         imgs = imgs[None]
     if imgs.dim() != 4 or imgs.shape[-1] != 3:
         raise ValueError(f"preprocess_images expects [B,H,W,3], got {tuple(imgs.shape)}")
-    if interpolation not in _INTERP:
-        raise ValueError(f"interpolation must be one of {sorted(_INTERP)}, got {interpolation!r}")
+    _check_resize_args(resize, max_side, interpolation)
     dev = _lib.require_cuda(imgs.device if imgs.is_cuda else (torch.device(device) if device is not None else None))
     x = imgs.to(dev, non_blocking=True).contiguous()
     B, H, W, _ = x.shape
-    hr, wr = (H, W) if resize is None else (int(resize[0]), int(resize[1]))
+    hr, wr, resized = _resized_size(H, W, resize, max_side)
     top, left, hc, wc = center_crop_box(hr, wr, patch)
     if hc == 0 or wc == 0:
         raise ValueError(f"image {hr}x{wr} is smaller than one {patch}x{patch} patch")
@@ -261,7 +382,7 @@ def preprocess_images(imgs: Union[np.ndarray, torch.Tensor], mean=IMAGENET_MEAN,
     m3 = (C.c_float * 3)(*[float(v) for v in mean])
     s3 = (C.c_float * 3)(*[float(v) for v in std])
     with torch.cuda.device(dev):
-        if resize is None:
+        if not resized:
             _lib.check(_lib.load().anyloc_preprocess_u8(_lib.ptr(x), B, H, W, top, left, hc, wc, m3, s3, _lib.ptr(out),
                                                         _lib.stream_ptr()), "anyloc_preprocess_u8")
         else:

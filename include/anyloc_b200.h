@@ -475,6 +475,25 @@ int anyloc_preprocess_u8(const uint8_t* img, int B, int H, int W, int top, int l
 int anyloc_preprocess_resize_u8(const uint8_t* img, int B, int H, int W, int Hr, int Wr, int interpolation, int top,
                                 int left, int Hc, int Wc, const float* mean3, const float* std3, float* out,
                                 void* stream);
+/* A list of n differently sized photos, the two ways they reach AnyLoc: the demo's "your own images" path
+ * (demo/anyloc_vlad_generate.py:160-185: each photo normalised, bicubic-resized to a 1024 long side with the aspect
+ * ratio kept when larger, centre-cropped to multiples of 14, so every photo keeps its own size) and the dataset loader
+ * (dvgl_benchmark/datasets_ws.py:222-239: every photo resized to 480x640 whatever its source size).
+ * Image i: imgs[i] a DEVICE pointer to uint8 [H[i], W[i], 3]; with interpolation 0 (bilinear) or 1 (bicubic) it is
+ * resized to Hr[i] x Wr[i] and the window [top[i], +Hc[i]) x [left[i], +Wc[i]) of the resized image is written, each
+ * image bit-identical to anyloc_preprocess_resize_u8 on that image alone; with interpolation -1 there is no resize (Hr,
+ * Wr may be NULL), the window is taken from the source image, and each image is bit-identical to anyloc_preprocess_u8.
+ * Its output [3, Hc[i], Wc[i]] fp32 starts at out + out_offset[i] (floats).  imgs, H, W, Hr, Wr, top, left, Hc, Wc,
+ * out_offset, mean3 and std3 are HOST arrays.  Up to ANYLOC_PREPROCESS_VARLEN_BATCH images per launch; a longer list
+ * takes consecutive launches on the stream.  ANYLOC_ERR_ARG for a null pointer, an unknown interpolation, a crop
+ * outside the (resized) image, a zero std, a negative offset, a horizontal down-scaling beyond the 64-tap window or a
+ * launch over the grid limit -- all checked before the first launch, so a refusal writes nothing.  Never synchronises
+ * with the host.  n = 0 launches nothing. */
+#define ANYLOC_PREPROCESS_VARLEN_BATCH 64
+int anyloc_preprocess_u8_varlen(int n, const uint8_t* const* imgs, const int* H, const int* W, const int* Hr,
+                                const int* Wr, int interpolation, const int* top, const int* left, const int* Hc,
+                                const int* Wc, const float* mean3, const float* std3, float* out,
+                                const int64_t* out_offset, void* stream);
 
 #ifdef __cplusplus
 }
