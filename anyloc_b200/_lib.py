@@ -106,6 +106,21 @@ _SIGS = {
                             [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_index_search_continue": (C.c_int, [C.c_void_p, C.c_size_t] + [C.c_int64] * 5 + [C.c_void_p] +
                                      [C.c_int] * 5 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_index_split_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "anyloc_index_split_init": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_int, C.c_void_p]),
+    "anyloc_index_split_copy": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_size_t, C.c_int64,
+                                          C.c_int64, C.c_int, C.c_void_p]),
+    "anyloc_index_split_add": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int,
+                                         C.c_int, C.c_void_p]),
+    "anyloc_index_split_search_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "anyloc_index_split_stage_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "anyloc_index_split_search": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_void_p] + [C.c_int] * 3 +
+                                  [C.c_void_p, C.c_size_t, C.POINTER(C.c_int64), C.c_void_p]),
+    "anyloc_index_split_rescore": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_int64] + [C.c_int] * 3 +
+                                   [C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
+    "anyloc_index_split_piece": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_void_p, C.c_size_t, C.c_int64,
+                                           C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p]),
     "anyloc_allgather_desc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
     "anyloc_vit_patch_k": (C.c_int, [C.c_int]),
     "anyloc_vit_workspace_bytes": (C.c_size_t, [C.POINTER(VitCfg), C.c_int, C.c_int, C.c_int]),

@@ -505,17 +505,19 @@ using namespace anyloc;
 // path) or tf32 pairs of y (rows of unknown range).
 static bool index_uses_f16(int Dv, int normalize) { return normalize && (Dv % 8) == 0; }
 struct IndexView { void* hi; void* lo; float* sq; float* dn; int* hdr; bool f16; size_t pair_bytes_per_row; };
-static bool carve_index(void* blob, size_t bytes, int64_t capacity, int Dv, int normalize, IndexView* v) {
+// split: the device blob of a split index (fp16 pairs; lo lives in host memory), hi | sq | dn | header
+static bool carve_index(void* blob, size_t bytes, int64_t capacity, int Dv, int normalize, IndexView* v,
+                        bool split = false) {
   v->f16 = index_uses_f16(Dv, normalize);
   const size_t esz = v->f16 ? 2 : 4;
   v->pair_bytes_per_row = (size_t)Dv * esz;
   Workspace w(blob, bytes);
   v->hi = w.take<char>((size_t)capacity * Dv * esz);
-  v->lo = w.take<char>((size_t)capacity * Dv * esz);
+  v->lo = split ? nullptr : w.take<char>((size_t)capacity * Dv * esz);
   v->sq = w.take<float>((size_t)capacity);
   v->dn = w.take<float>((size_t)capacity);
   v->hdr = w.take<int>(64);
-  return v->hi && v->lo && v->sq && v->dn && v->hdr;
+  return v->hi && (split || v->lo) && v->sq && v->dn && v->hdr;
 }
 
 extern "C" size_t anyloc_index_bytes(int64_t capacity, int Dv, int normalize) {
@@ -585,6 +587,20 @@ extern "C" size_t anyloc_index_search_workspace_bytes(int64_t n_db, int n_q, int
          align_up((size_t)n_q * 4, 256) + 256 + 1024;
 }
 
+struct SearchWs { void* qu_hi; void* qu_lo; float* qq; float* dnq; float* scores; int32_t* cand; int32_t* cand_n; int* flags; };
+static bool carve_search(void* ws, size_t ws_bytes, int64_t n_db, int n_q, int Dv, size_t esz, SearchWs* s) {
+  Workspace w(ws, ws_bytes);
+  s->qu_hi = w.take<char>((size_t)n_q * Dv * esz);
+  s->qu_lo = w.take<char>((size_t)n_q * Dv * esz);
+  s->qq = w.take<float>(n_q);
+  s->dnq = w.take<float>(n_q);
+  s->scores = w.take<float>((size_t)n_q * (size_t)n_db);
+  s->cand = w.take<int32_t>((size_t)n_q * CAND_MAX);
+  s->cand_n = w.take<int32_t>(n_q);
+  s->flags = w.take<int>(64);
+  return s->qu_hi && s->qu_lo && s->qq && s->dnq && s->scores && s->cand && s->cand_n && s->flags;
+}
+
 // The search of rows [first, first + n_db) of a carved index.  Resident (MERGE = false, first = row0 = 0, n_total = n_db):
 // the k best are written to dist / idx.  Continuation (MERGE): those rows are global rows [row0, row0 + n_db) of a
 // database of n_total rows, and their k best are merged into the running list dist / idx.  The route follows n_total,
@@ -603,20 +619,16 @@ static int search_rows(const IndexView& v0, int64_t first, int64_t n_db, int64_t
   } else {
     (void)first; (void)row0; (void)n_total;
   }
-  Workspace w(ws, ws_bytes);
-  void* qu_hi = w.take<char>((size_t)n_q * Dv * esz);
-  void* qu_lo = w.take<char>((size_t)n_q * Dv * esz);
-  float* qq = w.take<float>(n_q);
-  float* dnq = w.take<float>(n_q);
-  float* scores = w.take<float>((size_t)n_q * (size_t)n_db);
-  int32_t* cand = w.take<int32_t>((size_t)n_q * CAND_MAX);
-  int32_t* cand_n = w.take<int32_t>(n_q);
-  int* flags = w.take<int>(64);
-  if (!qu_hi || !qu_lo || !qq || !dnq || !scores || !cand || !cand_n || !flags) {
+  SearchWs s;
+  if (!carve_search(ws, ws_bytes, n_db, n_q, Dv, esz, &s)) {
     set_error("index_search: workspace too small (%zu given, %zu needed)", ws_bytes,
               anyloc_index_search_workspace_bytes(n_db, n_q, Dv, normalize));
     return ANYLOC_ERR_WORKSPACE;
   }
+  void *qu_hi = s.qu_hi, *qu_lo = s.qu_lo;
+  float *qq = s.qq, *dnq = s.dnq, *scores = s.scores;
+  int32_t *cand = s.cand, *cand_n = s.cand_n;
+  int* flags = s.flags;
   int rc;
   {
     ProfScope ps(PC_TOPK, st, (v.f16 ? 8.0 : 12.0) * (double)n_q * Dv);
@@ -700,6 +712,297 @@ extern "C" int anyloc_index_search_continue(const void* index, size_t index_byte
   }
   return search_rows<true>(v, first, n_rows, row0, n_total, qu, n_q, Dv, k, metric, normalize, dist, idx, ws, ws_bytes,
                            (cudaStream_t)stream);
+}
+
+// ---- split index: an fp16-pair index (normalize = 1, Dv % 8 == 0) whose lo halves live in caller-owned page-locked
+// host memory, lo [capacity, Dv] fp16, and whose device blob is hi | sq | dn | header (carve_index(split = true)).  Every
+// value is the one the resident index holds (the same kernel writes them); only where lo lives differs.
+static bool split_carve(const void* blob, size_t bytes, int64_t capacity, int Dv, IndexView* v) {
+  return carve_index(const_cast<void*>(blob), bytes, capacity, Dv, 1, v, true);
+}
+
+// the device address of the host lo array (page-locked memory is mapped into the unified address space)
+static __half* split_lo(const void* lo, const char* what) {
+  cudaPointerAttributes a;
+  if (!lo || cudaPointerGetAttributes(&a, lo) != cudaSuccess || a.type != cudaMemoryTypeHost || !a.devicePointer) {
+    cudaGetLastError();
+    set_error("%s: lo must be page-locked host memory (cudaHostAlloc, torch pin_memory)", what);
+    return nullptr;
+  }
+  return (__half*)a.devicePointer;
+}
+
+extern "C" size_t anyloc_index_split_bytes(int64_t capacity, int Dv) {
+  return align_up((size_t)capacity * Dv * 2, 256) + 2 * align_up((size_t)capacity * 4, 256) + 256 + 256;
+}
+
+extern "C" int anyloc_index_split_init(void* index, size_t index_bytes, int64_t capacity, int Dv, void* stream) {
+  ANYLOC_REQUIRE(index && capacity >= 0 && Dv > 0 && Dv % 8 == 0,
+                 "index_split_init: bad arguments (capacity=%lld, Dv=%d must be a positive multiple of 8)",
+                 (long long)capacity, Dv);
+  IndexView v;
+  if (!split_carve(index, index_bytes, capacity, Dv, &v)) { set_error("index_split_init: blob too small"); return ANYLOC_ERR_WORKSPACE; }
+  ANYLOC_CHECK_CUDA(cudaMemsetAsync(v.hdr, 0, 256, (cudaStream_t)stream));
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_index_split_copy(void* dst, size_t dst_bytes, int64_t dst_capacity, const void* src,
+                                       size_t src_bytes, int64_t src_capacity, int64_t n_rows, int Dv, void* stream) {
+  ANYLOC_REQUIRE(dst && src && n_rows >= 0 && n_rows <= src_capacity && n_rows <= dst_capacity && Dv > 0 && Dv % 8 == 0,
+                 "index_split_copy: bad arguments");
+  IndexView d, s;
+  if (!split_carve(dst, dst_bytes, dst_capacity, Dv, &d) || !split_carve(src, src_bytes, src_capacity, Dv, &s)) {
+    set_error("index_split_copy: blob too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.hi, s.hi, (size_t)n_rows * d.pair_bytes_per_row, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.sq, s.sq, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.dn, s.dn, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.hdr, s.hdr, 256, cudaMemcpyDeviceToDevice, st));
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_index_split_add(void* index, size_t index_bytes, int64_t capacity, void* lo, int64_t row_offset,
+                                      const float* rows, int n_rows, int Dv, void* stream) {
+  ANYLOC_REQUIRE(index && (rows || n_rows == 0), "index_split_add: null pointer");
+  ANYLOC_REQUIRE(n_rows >= 0 && Dv > 0 && Dv % 8 == 0 && row_offset >= 0 && row_offset + n_rows <= capacity,
+                 "index_split_add: bad dims n_rows=%d Dv=%d (a multiple of 8) offset=%lld capacity=%lld", n_rows, Dv,
+                 (long long)row_offset, (long long)capacity);
+  IndexView v;
+  if (!split_carve(index, index_bytes, capacity, Dv, &v)) {
+    set_error("index_split_add: blob too small (%zu given, %zu needed)", index_bytes, anyloc_index_split_bytes(capacity, Dv));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  __half* lo_d = split_lo(lo, "index_split_add");
+  if (!lo_d) return ANYLOC_ERR_ARG;
+  if (n_rows == 0) return ANYLOC_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope ps(PC_TOPK, st, 8.0 * (double)n_rows * Dv);
+  const size_t off = (size_t)row_offset * Dv;
+  ANYLOC_CHECK_CUDA(launch_normalize_rows<true>(rows, n_rows, Dv, 1, (__half*)v.hi + off, lo_d + off, v.sq + row_offset,
+                                                v.dn + row_offset, v.hdr, st));
+  count_launch();
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_index_split_piece(void* dst, size_t dst_bytes, int64_t dst_capacity, const void* index,
+                                        size_t index_bytes, int64_t capacity, const void* lo, int64_t first,
+                                        int64_t n_rows, int Dv, void* stream) {
+  ANYLOC_REQUIRE(dst && index && first >= 0 && n_rows >= 0 && first + n_rows <= capacity && n_rows <= dst_capacity &&
+                 Dv > 0 && Dv % 8 == 0, "index_split_piece: bad arguments first=%lld n_rows=%lld capacity=%lld "
+                 "dst_capacity=%lld Dv=%d", (long long)first, (long long)n_rows, (long long)capacity,
+                 (long long)dst_capacity, Dv);
+  IndexView d, s;
+  if (!carve_index(dst, dst_bytes, dst_capacity, Dv, 1, &d) || !split_carve(index, index_bytes, capacity, Dv, &s)) {
+    set_error("index_split_piece: blob too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  const __half* lo_d = split_lo(lo, "index_split_piece");
+  if (!lo_d) return ANYLOC_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t pb = (size_t)n_rows * d.pair_bytes_per_row;
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.hi, (const __half*)s.hi + (size_t)first * Dv, pb, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.lo, lo_d + (size_t)first * Dv, pb, cudaMemcpyDefault, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.sq, s.sq + first, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.dn, s.dn + first, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, st));
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(d.hdr, s.hdr, 256, cudaMemcpyDeviceToDevice, st));
+  return ANYLOC_OK;
+}
+
+// The coarse route of a split index.  The candidates' lo rows reach the unchanged topk_rescore_kernel through a staging
+// blob: the chunk's candidate rows are de-duplicated on the device and given staging slots in ascending row order (so
+// the rescore's (score desc, index asc) order over slots is its order over rows), their hi (HBM) and lo (host memory)
+// rows are gathered into the slots, the lists are remapped to slots, and the k best are mapped back to rows.
+namespace anyloc {
+// every candidate row of the chunk: slot[row] = 1; cnt[1] += the candidates of the query
+__global__ void __launch_bounds__(256)
+split_mark_kernel(const int32_t* __restrict__ cand, const int32_t* __restrict__ cand_n, int32_t* __restrict__ slot,
+                  int* __restrict__ cnt) {
+  const int q = blockIdx.x, n = cand_n[q];
+  for (int c = threadIdx.x; c < n; c += blockDim.x) slot[cand[(size_t)q * CAND_MAX + c]] = 1;
+  if (threadIdx.x == 0 && n) atomicAdd(cnt + 1, n);
+}
+
+// one CTA: each marked row gets slot[row] = its rank among the marked rows, row_of[rank] = row; cnt[0] = their count
+__global__ void __launch_bounds__(1024)
+split_scan_kernel(int32_t* __restrict__ slot, int n_db, int32_t* __restrict__ row_of, int* __restrict__ cnt) {
+  __shared__ int wsum[32];
+  const int per = (n_db + blockDim.x - 1) / blockDim.x;
+  const int b = min(n_db, (int)threadIdx.x * per), e = min(n_db, b + per);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int own = 0;
+  for (int j = b; j < e; ++j) own += slot[j];
+  int x = own;                                           // inclusive scan over the block, warp by warp
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    int t = lane < (int)(blockDim.x >> 5) ? wsum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
+    wsum[lane] = t;
+  }
+  __syncthreads();
+  int r = x - own + (w ? wsum[w - 1] : 0);
+  for (int j = b; j < e; ++j)
+    if (slot[j]) { row_of[r] = j; slot[j] = r++; }
+  if (threadIdx.x == blockDim.x - 1) cnt[0] = r;
+}
+
+// staging slot blockIdx.x <- database row row_of[slot]: hi from the device blob, lo from host memory through its
+// unified address.  16-byte loads, 4 per thread and array issued before any store, so that ~1000 resident CTAs keep
+// thousands of host reads in flight.
+__global__ void __launch_bounds__(256)
+split_gather_kernel(const uint4* __restrict__ hi, const uint4* __restrict__ lo, const int32_t* __restrict__ row_of,
+                    int n16, uint4* __restrict__ st_hi, uint4* __restrict__ st_lo) {
+  const size_t src = (size_t)row_of[blockIdx.x] * n16, dst = (size_t)blockIdx.x * n16;
+  for (int t0 = threadIdx.x; t0 < n16; t0 += 4 * blockDim.x) {
+    uint4 l[4], h[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = t0 + u * blockDim.x;
+      if (t < n16) { l[u] = __ldg(lo + src + t); h[u] = __ldg(hi + src + t); }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = t0 + u * blockDim.x;
+      if (t < n16) { st_lo[dst + t] = l[u]; st_hi[dst + t] = h[u]; }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+split_remap_kernel(int32_t* __restrict__ cand, const int32_t* __restrict__ cand_n, const int32_t* __restrict__ slot) {
+  const int q = blockIdx.x;
+  for (int c = threadIdx.x; c < cand_n[q]; c += blockDim.x) {
+    int32_t* p = cand + (size_t)q * CAND_MAX + c;
+    *p = slot[*p];
+  }
+}
+
+__global__ void __launch_bounds__(256)
+split_unmap_kernel(int64_t* __restrict__ idx, int64_t n, const int32_t* __restrict__ row_of) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && idx[i] >= 0) idx[i] = row_of[idx[i]];
+}
+}  // namespace anyloc
+
+// the search workspace, then slot [n_db] and row_of [n_q * CAND_MAX]
+struct SplitWs { SearchWs s; int32_t* slot; int32_t* row_of; };
+static bool carve_split_search(void* ws, size_t ws_bytes, int64_t n_db, int n_q, int Dv, SplitWs* w) {
+  const size_t head = anyloc_index_search_workspace_bytes(n_db, n_q, Dv, 1);
+  if (!carve_search(ws, ws_bytes, n_db, n_q, Dv, 2, &w->s) || ws_bytes < head) return false;
+  Workspace t((char*)ws + head, ws_bytes - head);
+  w->slot = t.take<int32_t>((size_t)n_db);
+  w->row_of = t.take<int32_t>((size_t)n_q * CAND_MAX);
+  return w->slot && w->row_of;
+}
+
+extern "C" size_t anyloc_index_split_search_workspace_bytes(int64_t n_db, int n_q, int Dv) {
+  return anyloc_index_search_workspace_bytes(n_db, n_q, Dv, 1) + align_up((size_t)n_db * 4, 256) +
+         align_up((size_t)n_q * CAND_MAX * 4, 256);
+}
+
+extern "C" size_t anyloc_index_split_stage_bytes(int64_t rows, int Dv) {
+  return 2 * align_up((size_t)rows * Dv * 2, 256);
+}
+
+extern "C" int anyloc_index_split_search(const void* index, size_t index_bytes, int64_t capacity, int64_t n_db,
+                                         const float* qu, int n_q, int Dv, int k, void* ws, size_t ws_bytes,
+                                         int64_t* counts, void* stream) {
+  ANYLOC_REQUIRE(index && qu && ws && counts, "index_split_search: null pointer");
+  counts[0] = -1; counts[1] = 0;
+  ANYLOC_REQUIRE(n_db > 0 && n_db <= capacity && n_db < (1ll << 31) && n_q >= 0 && Dv > 0 && Dv % 8 == 0 && k > 0,
+                 "index_split_search: bad dims n_db=%lld n_q=%d Dv=%d (a multiple of 8) k=%d", (long long)n_db, n_q,
+                 Dv, k);
+  IndexView v;
+  if (!split_carve(index, index_bytes, capacity, Dv, &v)) {
+    set_error("index_split_search: index blob too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  if (!(k <= COARSE_K_MAX && n_db >= 1024 && n_q >= 32)) return ANYLOC_OK;    // the resident search's route test
+  SplitWs w;
+  if (!carve_split_search(ws, ws_bytes, n_db, n_q, Dv, &w)) {
+    set_error("index_split_search: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_index_split_search_workspace_bytes(n_db, n_q, Dv));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  const SearchWs& s = w.s;
+  cudaStream_t st = (cudaStream_t)stream;
+  {
+    ProfScope ps(PC_TOPK, st, 8.0 * (double)n_q * Dv);
+    ANYLOC_CHECK_CUDA(launch_normalize_rows<true>(qu, n_q, Dv, 1, s.qu_hi, s.qu_lo, s.qq, s.dnq, nullptr, st));
+    count_launch();
+  }
+  ANYLOC_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 256, st));
+  int rc = anyloc_gemm_nt(s.qu_hi, nullptr, Dv, v.hi, nullptr, Dv, n_q, (int)n_db, Dv, ANYLOC_PAIR_F16,
+                          1.0f / (kRetrievalScale * kRetrievalScale), ANYLOC_EPI_BIAS, nullptr, nullptr, nullptr,
+                          s.scores, nullptr, (int)n_db, ANYLOC_PAIR_TF32, ANYLOC_GEMM_TC3, stream);
+  if (rc) return rc;
+  ProfScope ps(PC_TOPK, st, 8.0 * (double)n_q * (double)n_db);
+  topk_candidates_kernel<false><<<n_q, 1024, 0, st>>>(s.scores, (int)n_db, n_db, k, s.dnq, v.hdr, s.cand, s.cand_n,
+                                                      s.flags, nullptr);
+  ANYLOC_CHECK_LAUNCH();
+  // flags[0]: overflow (topk_candidates_kernel), flags[1]: unique candidate rows, flags[2]: candidate rows
+  ANYLOC_CHECK_CUDA(cudaMemsetAsync(w.slot, 0, (size_t)n_db * 4, st));
+  split_mark_kernel<<<n_q, 256, 0, st>>>(s.cand, s.cand_n, w.slot, s.flags + 1);
+  ANYLOC_CHECK_LAUNCH();
+  split_scan_kernel<<<1, 1024, 0, st>>>(w.slot, (int)n_db, w.row_of, s.flags + 1);
+  ANYLOC_CHECK_LAUNCH();
+  int f[3];
+  ANYLOC_CHECK_CUDA(cudaMemcpyAsync(f, s.flags, sizeof(f), cudaMemcpyDeviceToHost, st));
+  ANYLOC_CHECK_CUDA(cudaStreamSynchronize(st));
+  if (!f[0]) { counts[0] = f[1]; counts[1] = f[2]; }
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_index_split_rescore(const void* index, size_t index_bytes, int64_t capacity, const void* lo,
+                                          int64_t n_db, int n_q, int Dv, int k, void* ws, size_t ws_bytes,
+                                          int64_t n_unique, void* stage, size_t stage_bytes, float* dist, int64_t* idx,
+                                          void* stream) {
+  ANYLOC_REQUIRE(index && ws && dist && idx, "index_split_rescore: null pointer");
+  ANYLOC_REQUIRE(n_db > 0 && n_db <= capacity && n_db < (1ll << 31) && n_q >= 32 && Dv > 0 && Dv % 8 == 0 && k > 0 &&
+                 k <= COARSE_K_MAX && n_unique >= 0 && n_unique <= std::min<int64_t>(n_db, (int64_t)n_q * CAND_MAX),
+                 "index_split_rescore: bad dims n_db=%lld n_q=%d Dv=%d k=%d n_unique=%lld", (long long)n_db, n_q, Dv,
+                 k, (long long)n_unique);
+  IndexView v;
+  SplitWs w;
+  if (!split_carve(index, index_bytes, capacity, Dv, &v) || !carve_split_search(ws, ws_bytes, n_db, n_q, Dv, &w)) {
+    set_error("index_split_rescore: index blob or workspace too small");
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  const __half* lo_d = split_lo(lo, "index_split_rescore");
+  if (!lo_d) return ANYLOC_ERR_ARG;
+  const SearchWs& s = w.s;
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope ps(PC_TOPK, st, 4.0 * (double)n_unique * Dv);
+  const __half *db_hi = (const __half*)v.hi, *db_lo = lo_d;
+  if (stage) {
+    ANYLOC_REQUIRE(stage_bytes >= anyloc_index_split_stage_bytes(n_unique, Dv),
+                   "index_split_rescore: stage too small (%zu given, %zu needed)", stage_bytes,
+                   anyloc_index_split_stage_bytes(n_unique, Dv));
+    __half* st_hi = (__half*)stage;
+    __half* st_lo = (__half*)((char*)stage + align_up((size_t)n_unique * Dv * 2, 256));
+    if (n_unique) {
+      split_gather_kernel<<<(unsigned)n_unique, 256, 0, st>>>((const uint4*)v.hi, (const uint4*)lo_d, w.row_of, Dv / 8,
+                                                              (uint4*)st_hi, (uint4*)st_lo);
+      ANYLOC_CHECK_LAUNCH();
+    }
+    split_remap_kernel<<<n_q, 256, 0, st>>>(s.cand, s.cand_n, w.slot);
+    ANYLOC_CHECK_LAUNCH();
+    db_hi = st_hi; db_lo = st_lo;
+  }
+  topk_rescore_kernel<false><<<n_q, 256, 0, st>>>(db_hi, db_lo, (const __half*)s.qu_hi, (const __half*)s.qu_lo, Dv, k,
+                                                  s.cand, s.cand_n, s.flags, dist, idx, 0);
+  ANYLOC_CHECK_LAUNCH();
+  if (stage) {
+    const int64_t n = (int64_t)n_q * k;
+    split_unmap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(idx, n, w.row_of);
+    ANYLOC_CHECK_LAUNCH();
+  }
+  return ANYLOC_OK;
 }
 
 // One-shot form (get_top_k_recall builds the index and searches it once, utilities.py:449-450): a temporary index in

@@ -1215,6 +1215,17 @@ def pool_descriptors(patch_descs: torch.Tensor, method: str = "gem", gem_p: floa
 # ------------------------------------------------------------------ retrieval
 _SEARCH_Q_CHUNK = 4096      # queries per anyloc_index_search call: bounds the [n_q, n_db] score matrix
 _STREAM_K_MAX = 4096        # anyloc_index_search_continue merges the running k best in shared memory
+_COARSE_K_MAX = 64          # the coarse route's largest k (COARSE_K_MAX in csrc/topk.cu)
+PLACEMENTS = ("device", "split")
+
+
+def resolve_placement(placement=None):
+    """The index placement of top_k_search / get_top_k_recall: the argument, else $ANYLOC_B200_INDEX_PLACEMENT, else
+    "device".  ValueError on an unknown name."""
+    placement = placement or os.environ.get("ANYLOC_B200_INDEX_PLACEMENT", "device")
+    if placement not in PLACEMENTS:
+        raise ValueError(f"placement must be 'device' or 'split', got {placement!r}")
+    return placement
 
 
 def _stream_fixed_bytes(P, row, index_bytes, ws_bytes):
@@ -1295,6 +1306,40 @@ TOPK_KERNEL_DESCRIPTION = ("retrieval: gemm_tc3_kernel<true, 0> (wgmma, hi-only:
                            "(hi,lo) pairs + k-best); 3-term GEMM + topk_select2_kernel as the device-gated fallback")
 
 
+class _PinnedRows:
+    """[n, d] fp16 rows in host memory page-locked to the byte: a plain host allocation registered with
+    cudaHostRegister (torch's pinned allocator rounds each request up to a power of two and keeps freed blocks locked
+    in its cache).  `done` is an event after the last device work that uses the rows; release() waits for it, then
+    unlocks them."""
+
+    def __init__(self, n, d):
+        self.t = torch.empty(n, d, dtype=torch.float16)
+        self.nbytes, self.done = self.t.numel() * 2, None
+        if self.nbytes:
+            torch.cuda.check_error(torch.cuda.cudart().cudaHostRegister(self.t.data_ptr(), self.nbytes, 0))
+
+    def ptr(self):
+        return C.c_void_p(self.t.data_ptr())
+
+    def used(self):
+        """record the device work queued so far on the current stream as the last use"""
+        self.done = torch.cuda.Event()
+        self.done.record()
+
+    def release(self):
+        if self.nbytes:
+            if self.done is not None:
+                self.done.synchronize()
+            torch.cuda.check_error(torch.cuda.cudart().cudaHostUnregister(self.t.data_ptr()))
+            self.nbytes = 0
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:       # at interpreter exit the CUDA runtime may already be gone, and the lock with it
+            pass
+
+
 class FlatIndex:
     """GPU stand-in for `faiss.IndexFlatIP` / `IndexFlatL2` as get_top_k_recall drives them (utilities.py:439-450):
     `add(db)` normalises the rows (when `norm_descs`) and stores them once as the operand pairs of the score GEMM
@@ -1308,15 +1353,35 @@ class FlatIndex:
     holds, stay prepared on the device.  The answer is the resident search's, bit for bit, except in a query batch where
     the coarse route's 3-term fallback fires (DESIGN §4.5).  A streamed index answers k <= 4096.  Device rows never make
     an index stream; device rows added to an index that already streams join its host copy once its device blob is
-    full, as host rows do."""
+    full, as host rows do.
 
-    def __init__(self, d: int, method: str = "cosine", norm_descs: bool = True, capacity: int = 0, device=None):
+    placement="split" keeps the low fp16 halves of the rows (half the index) in page-locked host memory and the rest on
+    the device, so an index up to about twice the device memory is searched without streaming.  It needs an fp16-pair
+    inner-product index: method="cosine", norm_descs=True and d % 8 == 0.  The answer is the resident index's, bit for
+    bit.  The coarse route reads the lo rows of each query's candidates only; every other search (k > 64, fewer than
+    32 queries, fewer than 1024 rows, a batch whose candidate lists overflow) copies every lo row to the device once.
+    A split index answers k <= 4096 and never streams.  Growing it holds the old and the new device part at once, so
+    rows added in chunks without a reserved `capacity` fill at most about half the device; reserve the capacity to fill
+    it.  When the doubled device part does not fit, the largest one that does is taken; when not even the rows fit,
+    add raises MemoryError."""
+
+    def __init__(self, d: int, method: str = "cosine", norm_descs: bool = True, capacity: int = 0, device=None, *,
+                 placement: str = "device"):
         if method not in _lib.METRIC:
             raise NotImplementedError(f"Method: {method}")
+        if placement not in PLACEMENTS:
+            raise ValueError(f"placement must be 'device' or 'split', got {placement!r}")
+        if placement == "split" and not (method == "cosine" and norm_descs and int(d) % 8 == 0):
+            raise ValueError("placement='split' holds an fp16-pair inner-product index: it needs method='cosine', "
+                             f"norm_descs=True and d % 8 == 0 (got method={method!r}, norm_descs={norm_descs}, d={d})")
         self.d, self.method, self.norm_descs = int(d), method, bool(norm_descs)
         self.dp = self.d + (-self.d) % 4            # zero columns change neither norms nor scores
         self.ntotal, self.capacity = 0, 0
         self._blob, self._dev = None, (torch.device(device) if device is not None else None)
+        self._split = placement == "split"
+        self._lo = None                             # split: the lo halves, _PinnedRows [capacity, d]
+        self._xs = None                             # split: the side stream of the exact route
+        self._split_counts = []                     # split: (unique, all) candidate rows of each coarse query chunk
         # streamed index: {"P": rows per piece, "host": [(first row, fp32 rows [m, d] on the host), ...]}; the device
         # blob then holds rows [0, capacity) and the host copy rows [capacity, ntotal)
         self._stream = None
@@ -1324,6 +1389,8 @@ class FlatIndex:
             self._reserve(int(capacity), _lib.require_cuda(self._dev))
 
     def _reserve(self, capacity, dev):
+        if self._split:
+            return self._reserve_split(capacity, dev)
         lib = _lib.load()
         norm = int(self.norm_descs)
         blob = torch.empty(lib.anyloc_index_bytes(capacity, self.dp, norm), dtype=torch.uint8, device=dev)
@@ -1336,6 +1403,37 @@ class FlatIndex:
                                                  _lib.stream_ptr()), "anyloc_index_copy")
         self._blob, self.capacity, self._dev = blob, capacity, dev
 
+    def _reserve_split(self, capacity, dev, need=0):
+        """a device part of `capacity` rows, or, when that does not fit, of the most rows that fit if those are at
+        least `need`"""
+        lib = _lib.load()
+        nbytes = lib.anyloc_index_split_bytes(capacity, self.dp)
+        with torch.cuda.device(dev):
+            budget = _device_budget(dev)
+        if nbytes > budget and need:
+            fit = max(0, budget - 2048) // (2 * self.dp + 8)     # 2048: the header and the sections' alignment
+            if need <= fit < capacity:
+                capacity, nbytes = fit, lib.anyloc_index_split_bytes(fit, self.dp)
+        if nbytes > budget:
+            raise MemoryError(f"placement='split': the device part of a {capacity}-row index of dimension {self.d} "
+                              f"({nbytes / 2**30:.2f} GiB: the fp16 hi halves, |y|^2 and dn) does not fit the "
+                              f"{budget / 2**30:.2f} GiB free on {dev}; a split index does not stream")
+        blob = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        lo = _PinnedRows(capacity, self.dp)
+        with torch.cuda.device(dev):
+            _lib.check(lib.anyloc_index_split_init(_lib.ptr(blob), blob.numel(), capacity, self.dp, _lib.stream_ptr()),
+                       "anyloc_index_split_init")
+            if self.ntotal:
+                _lib.check(lib.anyloc_index_split_copy(_lib.ptr(blob), blob.numel(), capacity, _lib.ptr(self._blob),
+                                                       self._blob.numel(), self.capacity, self.ntotal, self.dp,
+                                                       _lib.stream_ptr()), "anyloc_index_split_copy")
+                if self._lo.done is not None:
+                    self._lo.done.synchronize()                 # the old lo rows are final once the adds are done
+                lo.t[:self.ntotal].copy_(self._lo.t[:self.ntotal])
+        if self._lo is not None:
+            self._lo.release()
+        self._blob, self._lo, self.capacity, self._dev = blob, lo, capacity, dev
+
     def reset(self):
         """faiss `index.reset()`: forget the rows, keep the allocation (a streamed index drops its host copy and
         chooses again at the next add)."""
@@ -1347,6 +1445,10 @@ class FlatIndex:
 
     def _reserve_header_only(self):
         with torch.cuda.device(self._dev):
+            if self._split:
+                _lib.check(_lib.load().anyloc_index_split_init(_lib.ptr(self._blob), self._blob.numel(), self.capacity,
+                                                               self.dp, _lib.stream_ptr()), "anyloc_index_split_init")
+                return
             _lib.check(_lib.load().anyloc_index_init(_lib.ptr(self._blob), self._blob.numel(), self.capacity, self.dp,
                                                      int(self.norm_descs), _lib.stream_ptr()), "anyloc_index_init")
 
@@ -1357,7 +1459,7 @@ class FlatIndex:
         if x.shape[1] != self.d:
             raise ValueError(f"index dimension {self.d}, got rows of {x.shape[1]}")
         grow = max(self.ntotal + n, 2 * self.capacity if self.ntotal else 0)
-        if self._stream is None and not on_dev and n:
+        if self._stream is None and not on_dev and n and not self._split:
             # first against the free memory as it is; torch's cache is emptied only when that is not enough
             plan = self._plan(n, grow, dev, release_cache=False)
             if plan[0] != "resident":
@@ -1381,7 +1483,10 @@ class FlatIndex:
             self.ntotal += n
             return
         if self.ntotal + n > self.capacity:
-            self._reserve(grow, dev)
+            if self._split:
+                self._reserve_split(grow, dev, need=self.ntotal + n)
+            else:
+                self._reserve(grow, dev)
         self._prepare(x, dev)
         self.ntotal += n
 
@@ -1397,6 +1502,13 @@ class FlatIndex:
                 rows = _as_device_f32(x[i:i + step], dev)
                 if self.dp != self.d:
                     rows = torch.nn.functional.pad(rows, (0, self.dp - self.d))
+                if self._split:
+                    _lib.check(lib.anyloc_index_split_add(_lib.ptr(self._blob), self._blob.numel(), self.capacity,
+                                                          self._lo.ptr(), self.ntotal + i, _lib.ptr(rows),
+                                                          rows.shape[0], self.dp, _lib.stream_ptr()),
+                               "anyloc_index_split_add")
+                    self._lo.used()
+                    continue
                 _lib.check(lib.anyloc_index_add(_lib.ptr(self._blob), self._blob.numel(), self.capacity,
                                                 self.ntotal + i, _lib.ptr(rows), rows.shape[0], self.dp,
                                                 int(self.norm_descs), _lib.stream_ptr()), "anyloc_index_add")
@@ -1419,6 +1531,8 @@ class FlatIndex:
         if self._stream is not None:
             raise ValueError("add_at on an index that streams host rows: reserve the capacity and add device rows, or "
                              "use add()")
+        if self._split:
+            raise ValueError("add_at on an index with placement='split': use add()")
         n = x.shape[0]
         if self._blob is None or row_offset < 0 or row_offset + n > self.capacity:
             raise ValueError(f"rows [{row_offset}, {row_offset + n}) outside the reserved capacity {self.capacity}")
@@ -1441,13 +1555,15 @@ class FlatIndex:
             raise ValueError("search on an empty index")
         if self._stream is not None and k > _STREAM_K_MAX:
             raise ValueError(f"k={k}: an index that streams host rows answers k <= {_STREAM_K_MAX}")
+        if self._split and k > _STREAM_K_MAX:
+            raise ValueError(f"k={k}: an index with placement='split' answers k <= {_STREAM_K_MAX}")
         on_dev = isinstance(qu, torch.Tensor) and qu.is_cuda
         dev = self._dev
         q = _as_device_f32(qu, dev)
         if self.dp != self.d:
             q = torch.nn.functional.pad(q, (0, self.dp - self.d))
-        if self._stream is not None:
-            dist, idx = self._search_streamed(q, k, n_q_chunk)
+        if self._stream is not None or self._split:
+            dist, idx = (self._search_split if self._split else self._search_streamed)(q, k, n_q_chunk)
             return (dist, idx) if on_dev else (dist.cpu(), idx.cpu())
         lib = _lib.load()
         n_q = q.shape[0]
@@ -1543,15 +1659,105 @@ class FlatIndex:
                     stage()                 # the gather of the next host piece overlaps the work just queued
         return dist, idx
 
+    def _search_split(self, q, k, n_q_chunk):
+        """Each query chunk tries the coarse route (anyloc_index_split_search).  Its unique candidate rows are gathered
+        into a device stage of exactly their size and re-scored there (anyloc_index_split_rescore); when the stage does
+        not fit the free device memory, the re-scoring reads lo from host memory instead.  The chunks the coarse route
+        leaves go through the exact route over pieces, together, so every lo row crosses the link once per search.
+        Returns after the device work is done: that work reads the index's host memory."""
+        lib = _lib.load()
+        dev, dp, n_q = self._dev, self.dp, q.shape[0]
+        dist = torch.empty(n_q, k, device=dev, dtype=torch.float32)
+        idx = torch.empty(n_q, k, device=dev, dtype=torch.int64)
+        counts, exact = (C.c_int64 * 2)(), []
+        self._split_counts = []
+        blob = (_lib.ptr(self._blob), self._blob.numel(), self.capacity)
+        with torch.cuda.device(dev):
+            for i in range(0, n_q, n_q_chunk):
+                m = min(n_q_chunk, n_q - i)
+                ws = _lib.workspaces.get(dev, lib.anyloc_index_split_search_workspace_bytes(self.ntotal, m, dp), "topk")
+                _lib.check(lib.anyloc_index_split_search(*blob, self.ntotal, _lib.ptr(q[i:i + m]), m, dp, k,
+                                                         _lib.ptr(ws), ws.numel(), counts, _lib.stream_ptr()),
+                           "anyloc_index_split_search")
+                if counts[0] < 0:
+                    exact.append((i, m))
+                    continue
+                self._split_counts.append((counts[0], counts[1]))
+                nbytes = lib.anyloc_index_split_stage_bytes(counts[0], dp)
+                stage = self._split_stage(nbytes, dev)
+                _lib.check(lib.anyloc_index_split_rescore(
+                    *blob, self._lo.ptr(), self.ntotal, m, dp, k, _lib.ptr(ws), ws.numel(), counts[0],
+                    _lib.ptr(stage), nbytes if stage is not None else 0, _lib.ptr(dist[i:i + m]),
+                    _lib.ptr(idx[i:i + m]), _lib.stream_ptr()), "anyloc_index_split_rescore")
+            if exact:
+                self._search_split_exact(q, k, exact, dist, idx)
+            torch.cuda.current_stream().synchronize()
+        return dist, idx
+
+    @staticmethod
+    def _split_stage(nbytes, dev):
+        """a device stage of nbytes, or None when it does not fit the free memory (torch's cache emptied only if needed)"""
+        for release in (False, True):
+            if nbytes <= _device_budget(dev, release_cache=release):
+                return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        return None
+
+    def _search_split_exact(self, q, k, chunks, dist, idx):
+        """The query chunks `chunks` [(first query, queries)] by the exact route: the index is rebuilt piece by piece as
+        ordinary index blobs (anyloc_index_split_piece, on a side stream, two blobs so that the copy of piece j+1
+        overlaps the search of piece j) and searched by anyloc_index_search_continue.  It asks for at least 65 best,
+        which takes the exact route on every batch: the 3-term product the resident index's overflow fallback uses,
+        in the same (score, index) order, so the first k columns are the resident answer."""
+        lib = _lib.load()
+        dev, dp, n = self._dev, self.dp, self.ntotal
+        ke = max(k, _COARSE_K_MAX + 1)
+        ib = lambda p: lib.anyloc_index_bytes(p, dp, 1)
+        wb = lambda p: lib.anyloc_index_search_workspace_bytes(p, max(m for _, m in chunks), dp, 1)
+        fixed = lambda p: 2 * ib(p) + wb(p)
+        P = _piece_rows(n, dp, _device_budget(dev, release_cache=False), _STAGE_BYTES, fixed)
+        if P < min(n, _STAGE_BYTES // (4 * dp)):      # fewer rows than a full piece: empty torch's cache and plan again
+            P = _piece_rows(n, dp, _device_budget(dev), _STAGE_BYTES, fixed)
+        run = [(torch.full((m, ke), -float("inf"), device=dev), torch.full((m, ke), -1, device=dev, dtype=torch.int64))
+               for _, m in chunks]
+        blobs = [torch.empty(ib(P), dtype=torch.uint8, device=dev) for _ in range(2)]
+        ws = _lib.workspaces.get(dev, wb(P), "topk")
+        if self._xs is None or self._xs.device != dev:
+            self._xs = torch.cuda.Stream(dev)
+        cs, xs = torch.cuda.current_stream(), self._xs
+        xs.wait_stream(cs)
+        freed = [None, None]
+        for j, r0 in enumerate(range(0, n, P)):
+            m, s = min(P, n - r0), j & 1
+            with torch.cuda.stream(xs):
+                if freed[s] is not None:
+                    xs.wait_event(freed[s])             # the search of piece j-2 is done with this blob
+                _lib.check(lib.anyloc_index_split_piece(
+                    _lib.ptr(blobs[s]), blobs[s].numel(), P, _lib.ptr(self._blob), self._blob.numel(), self.capacity,
+                    self._lo.ptr(), r0, m, dp, _lib.stream_ptr()), "anyloc_index_split_piece")
+                ready = torch.cuda.Event()
+                ready.record(xs)
+            cs.wait_event(ready)
+            for (i, c), (d, x) in zip(chunks, run):
+                _lib.check(lib.anyloc_index_search_continue(
+                    _lib.ptr(blobs[s]), blobs[s].numel(), P, 0, m, r0, n, _lib.ptr(q[i:i + c]), c, dp, ke, 0, 1,
+                    _lib.ptr(d), _lib.ptr(x), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_index_search_continue")
+            freed[s] = torch.cuda.Event()
+            freed[s].record(cs)
+        for (i, c), (d, x) in zip(chunks, run):
+            dist[i:i + c], idx[i:i + c] = d[:, :k], x[:, :k]
+
 
 def top_k_search(db: torch.Tensor, qu: torch.Tensor, k: int, method: str = "cosine",
-                 norm_descs: bool = True) -> Tuple[torch.Tensor, torch.Tensor]:
+                 norm_descs: bool = True, *, placement: str = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact k-nearest search on the GPU (the `faiss.IndexFlatIP/L2` `add` + `search` of get_top_k_recall,
-    utilities.py:435-450).  Device tensors out; a host database larger than the device streams (FlatIndex)."""
+    utilities.py:435-450).  Device tensors out; a host database larger than the device streams (FlatIndex).
+    `placement` (else $ANYLOC_B200_INDEX_PLACEMENT, else "device") is FlatIndex's."""
     if method not in _lib.METRIC:
         raise NotImplementedError(f"Method: {method}")
+    placement = resolve_placement(placement)
     dev = _lib.require_cuda(db.device if db.is_cuda else None)
-    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if db.is_cuda else 0, device=dev)
+    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if db.is_cuda else 0, device=dev,
+                      placement=placement)
     index.add(db)
     return index.search(qu.to(dev), k)
 
@@ -1561,9 +1767,12 @@ def get_top_k_recall(top_k: List[int], db: torch.Tensor, qu: torch.Tensor, gt_po
                      use_percentage: bool = True, sub_sample_db: int = 1, sub_sample_qu: int = 1) \
         -> Tuple[np.ndarray, np.ndarray, dict]:
     """utilities.py:390-469.  `use_gpu` is accepted for signature compatibility; the search always
-    runs on the GPU.  Host tensors in -> host tensors out (like faiss with torch_utils)."""
+    runs on the GPU.  Host tensors in -> host tensors out (like faiss with torch_utils).  The signature is the
+    reference's, so the index placement comes from $ANYLOC_B200_INDEX_PLACEMENT ("device" when unset; "split":
+    FlatIndex's placement="split")."""
     if method not in _lib.METRIC:
         raise NotImplementedError(f"Method: {method}")
+    placement = resolve_placement()
     as_numpy = type(db) == np.ndarray
     if as_numpy:
         db, qu = torch.from_numpy(db), torch.from_numpy(np.asarray(qu))
@@ -1572,7 +1781,8 @@ def get_top_k_recall(top_k: List[int], db: torch.Tensor, qu: torch.Tensor, gt_po
     on_dev = db.is_cuda
     dev = _lib.require_cuda(db.device if on_dev else None)
     # host rows: add() reserves the index once it knows it fits, and streams the search when it does not
-    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if on_dev else 0, device=dev)
+    index = FlatIndex(db.shape[1], method, norm_descs, capacity=db.shape[0] if on_dev else 0, device=dev,
+                      placement=placement)
     index.add(db)                                   # host rows are streamed in <= 1 GiB chunks
     distances, indices = index.search(_as_device_f32(qu, dev), max(top_k))
     idx_host = indices.cpu().numpy()

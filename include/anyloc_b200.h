@@ -222,6 +222,42 @@ int anyloc_index_search_continue(const void* index, size_t index_bytes, int64_t 
                                  int64_t n_rows, int64_t row0, int64_t n_total, const float* qu, int n_q, int Dv, int k,
                                  int metric, int normalize, float* dist, int64_t* idx, void* ws, size_t ws_bytes,
                                  void* stream);
+/* Split index: an fp16-pair inner-product index (normalize = 1, Dv % 8 == 0) whose lo halves stay in caller-owned
+ * page-locked host memory, lo [capacity, Dv] fp16 (cudaHostAlloc or cudaHostRegister; the kernels reach it through its
+ * unified address).
+ * The device blob (anyloc_index_split_bytes for `capacity` rows) holds hi, |y|^2, dn and the header: about half of
+ * anyloc_index_bytes.  Every stored value equals the resident index's, so searches return its (dist, idx) bit for bit.
+ * anyloc_index_split_init / _copy / _add are anyloc_index_init / _copy / _add on this layout; _copy moves the device
+ * part only (the caller copies lo rows [0, n_rows) to the new host array), _add writes lo into `lo` over the link. */
+size_t anyloc_index_split_bytes(int64_t capacity, int Dv);
+int anyloc_index_split_init(void* index, size_t index_bytes, int64_t capacity, int Dv, void* stream);
+int anyloc_index_split_copy(void* dst, size_t dst_bytes, int64_t dst_capacity, const void* src, size_t src_bytes,
+                            int64_t src_capacity, int64_t n_rows, int Dv, void* stream);
+int anyloc_index_split_add(void* index, size_t index_bytes, int64_t capacity, void* lo, int64_t row_offset,
+                           const float* rows, int n_rows, int Dv, void* stream);
+/* The coarse route of a search over the first n_db rows, in two calls on one workspace
+ * (anyloc_index_split_search_workspace_bytes).  anyloc_index_split_search: the hi-only pass and the candidate lists on
+ * the device, the candidate rows de-duplicated and numbered in ascending row order, then ONE host synchronisation.
+ * counts[0] = the unique candidate rows, counts[1] = the candidate rows summed over the queries.  counts[0] = -1: the
+ * coarse route does not answer this batch (k > 64, n_db < 1024, n_q < 32, or a candidate list overflowed); answer it
+ * by the exact route over pieces (anyloc_index_split_piece + anyloc_index_search_continue with n_total = n_db and
+ * k > 64, whose first k columns are the resident answer: the same 3-term product and the same (score, index) order).
+ * Otherwise anyloc_index_split_rescore writes the resident search's dist / idx [n_q, k].  With a stage of
+ * anyloc_index_split_stage_bytes(counts[0], Dv) device bytes it gathers the unique rows' hi and lo (lo from host memory)
+ * into the stage first and re-scores from there; with stage = NULL the re-scoring reads each candidate's lo row from
+ * host memory directly, once per query that has it. */
+size_t anyloc_index_split_search_workspace_bytes(int64_t n_db, int n_q, int Dv);
+size_t anyloc_index_split_stage_bytes(int64_t rows, int Dv);
+int anyloc_index_split_search(const void* index, size_t index_bytes, int64_t capacity, int64_t n_db, const float* qu,
+                              int n_q, int Dv, int k, void* ws, size_t ws_bytes, int64_t* counts, void* stream);
+int anyloc_index_split_rescore(const void* index, size_t index_bytes, int64_t capacity, const void* lo, int64_t n_db,
+                               int n_q, int Dv, int k, void* ws, size_t ws_bytes, int64_t n_unique, void* stage,
+                               size_t stage_bytes, float* dist, int64_t* idx, void* stream);
+/* Rows [first, first + n_rows) of a split index as rows [0, n_rows) of an ordinary index blob (anyloc_index_bytes(
+ * dst_capacity, Dv, 1)): hi, |y|^2 and dn copied on the device, lo copied from the host, the header (DN of the whole
+ * index, a valid bound for the piece).  Asynchronous on `stream`; no init of `dst` is needed. */
+int anyloc_index_split_piece(void* dst, size_t dst_bytes, int64_t dst_capacity, const void* index, size_t index_bytes,
+                             int64_t capacity, const void* lo, int64_t first, int64_t n_rows, int Dv, void* stream);
 
 /* ------------------------------------------------------------- collective
  * The one data-path collective of the pipeline (BASELINE config 4): all-gather of the [n_loc, Dv] fp32 descriptors of
