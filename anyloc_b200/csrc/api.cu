@@ -79,6 +79,12 @@ int launch_assemble_varlen(const float*, const float*, const float*, const Varle
 int launch_facet_out_varlen(const float*, const VarlenImgTable&, int, int64_t, int, int, int, int, float*, cudaStream_t);
 int launch_qkv_tap(const float*, int, int, const VarlenImgTable*, int, int, void*, void*, const QkvTapOuts&, int, int,
                    cudaStream_t);
+// pca.cu
+size_t pca_colsum_workspace_bytes(int64_t, int);
+int pca_colsum_launch(const float*, int64_t, int64_t, int, double*, double*, cudaStream_t);
+int pca_atb_launch(int, const float*, int64_t, const double*, const double*, int64_t, int64_t, int, int, double*,
+                   int64_t, cudaStream_t);
+int pca_mirror_launch(double*, int, int64_t, cudaStream_t);
 
 // fmt: ANYLOC_PAIR_* of the operands.  The single formats run on the tensor cores only: they run the wgmma kernel at
 // every M (no SIMT route, so a row's result never depends on how many rows share the call) and refuse the SIMT
@@ -360,6 +366,51 @@ extern "C" int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int
                  "l2_normalize_rows: x and y must be 16-byte aligned (float4 access)");
   if (rows == 0) return ANYLOC_OK;
   return launch_l2norm(x, rows, D, ld_in, y, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------ streamed PCA fit (pca.cu)
+extern "C" size_t anyloc_pca_colsum_workspace_bytes(int64_t rows, int cols) {
+  return pca_colsum_workspace_bytes(rows, cols);
+}
+
+extern "C" int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int cols, double* sum, void* ws,
+                                 size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(x && sum && ws, "pca_colsum: null pointer");
+  ANYLOC_REQUIRE(rows >= 0 && cols >= 0 && ld >= cols, "pca_colsum: rows=%lld cols=%d ld=%lld (rows >= 0, cols >= 0, "
+                 "ld >= cols)", (long long)rows, cols, (long long)ld);
+  if (ws_bytes < pca_colsum_workspace_bytes(rows, cols)) {
+    set_error("pca_colsum: workspace too small (%zu given, %zu needed)", ws_bytes,
+              pca_colsum_workspace_bytes(rows, cols));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  return pca_colsum_launch(x, ld, rows, cols, sum, (double*)ws, (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64_t rows, int cols, const double* mu,
+                                     const double* u, int64_t ld_u, int k, double* out, int64_t ld_out, void* stream) {
+  ANYLOC_REQUIRE(mode == ANYLOC_PCA_COV || mode == ANYLOC_PCA_GRAM || mode == ANYLOC_PCA_VT,
+                 "pca_accumulate: unknown mode %d", mode);
+  ANYLOC_REQUIRE(x && mu && out && (mode != ANYLOC_PCA_VT || u || k == 0), "pca_accumulate: null pointer");
+  ANYLOC_REQUIRE(rows >= 0 && cols >= 0 && ld >= cols, "pca_accumulate: rows=%lld cols=%d ld=%lld (rows >= 0, "
+                 "cols >= 0, ld >= cols)", (long long)rows, cols, (long long)ld);
+  // out [M, N] += sum over K of A(kk, i) B(kk, j)
+  int64_t M = cols, N = cols, K = rows;
+  if (mode == ANYLOC_PCA_GRAM) {
+    M = N = rows;
+    K = cols;
+  } else if (mode == ANYLOC_PCA_VT) {
+    ANYLOC_REQUIRE(k >= 0 && ld_u >= k, "pca_accumulate: k=%d ld_u=%lld (k >= 0, ld_u >= k)", k, (long long)ld_u);
+    M = k;
+  }
+  ANYLOC_REQUIRE(M <= (1 << 20) && ld_out >= N, "pca_accumulate: output [%lld, %lld] with ld_out=%lld (at most 2^20 "
+                 "rows, ld_out >= columns)", (long long)M, (long long)N, (long long)ld_out);
+  return pca_atb_launch(mode, x, ld, mu, u, ld_u, K, (int)M, (int)N, out, ld_out, (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream) {
+  ANYLOC_REQUIRE(a && m >= 0 && m <= 65535 * 32 && ld >= m, "pca_mirror: a=%p m=%d ld=%lld (0 <= m <= 65535*32, "
+                 "ld >= m)", (void*)a, m, (long long)ld);
+  return pca_mirror_launch(a, m, ld, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------ ViT forward

@@ -166,6 +166,10 @@ class _PcaDev:
             ev, v = ev.flip(0).clamp_min(0), v.flip(1)
             s = ev.sqrt()
             vt = v[:, :k].T.contiguous()
+        return self._set_components(vt, s, n)
+
+    def _set_components(self, vt, s, n):
+        k = self.n_components
         sign = torch.sign(torch.gather(vt, 1, vt.abs().argmax(dim=1, keepdim=True)))
         sign[sign == 0] = 1
         self.components_ = (vt * sign).float().contiguous()
@@ -173,6 +177,50 @@ class _PcaDev:
         self.explained_variance_ = (s[:k] ** 2 / (n - 1)).float()
         self.all_singular_values_ = s
         return self
+
+    def fit_streamed(self, rows, plan, dev):
+        """fit() on rows (a _PcaRows) fed to the device piece by piece (_pca_plan, _pca_boxes), so that only the m x m
+        fp64 matrix, its eigen-decomposition and k x d vectors live there.  Covariance route (n > d): one pass over row
+        pieces for the mean, one accumulating C = Xc^T Xc.  Gram route (n <= d): one pass over column slabs of all n
+        rows, each giving its columns' mean and its part of G = Xc Xc^T, then a second one for vt = u[:, :k]^T Xc / s.
+        The sums are anyloc_pca_colsum / anyloc_pca_accumulate, fp64 on the FP64 tensor cores, centring in registers."""
+        n, d = rows.shape
+        k = self.n_components
+        if not 0 <= k <= min(n, d):
+            raise ValueError(f"n_components={k} must be between 0 and min(n_samples, n_features)={min(n, d)} with "
+                             "svd_solver='full'")
+        m = min(n, d)
+        boxes = _pca_boxes(n, d, plan)
+        with torch.cuda.device(dev):
+            mu = torch.zeros(d, dtype=torch.float64, device=dev)
+            a = torch.zeros(m, m, dtype=torch.float64, device=dev)
+            if n > d:
+                for x in _pca_staged(rows, boxes, dev):
+                    _pca_colsum(x, mu)
+                mu /= n
+                for x in _pca_staged(rows, boxes, dev):
+                    _pca_accumulate("cov", x, mu, a)
+            else:
+                for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                    _pca_colsum(x, mu[c0:c1])
+                    mu[c0:c1] /= n
+                    _pca_accumulate("gram", x, mu[c0:c1], a)
+            _lib.check(_lib.load().anyloc_pca_mirror(_lib.ptr(a), m, m, _lib.stream_ptr()), "anyloc_pca_mirror")
+            ev, vec = torch.linalg.eigh(a)
+            del a
+            ev, vec = ev.flip(0).clamp_min(0), vec.flip(1)
+            s = ev.sqrt()
+            if n <= d:
+                u = vec[:, :k].contiguous()
+                del vec
+                vt = torch.zeros(k, d, dtype=torch.float64, device=dev)
+                for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                    _pca_accumulate("vt", x, mu[c0:c1], vt[:, c0:c1], u)
+                vt /= s[:k, None].clamp_min(1e-300)
+            else:
+                vt = vec[:, :k].T.contiguous()
+            self.mean_ = mu.float()
+            return self._set_components(vt, s, n)
 
     def transform(self, x):
         y = _gemm_nt_dev(x - self.mean_, self.components_)
@@ -189,10 +237,20 @@ def reduce_pca(train_descs: np.ndarray, test_descs: np.ndarray, lower_dim: int, 
     """PCA projection fitted on the training set (utilities.py:522-586; scripts/dino_v2_vlad.py:357-369 reduces the
     database / query VLADs with it).  Same arguments and return types (numpy in -> numpy out, torch tensors accepted);
     the arithmetic runs on the GPU -- see _PcaDev.  `svd_solver` is accepted for signature compatibility: the result
-    is the exact ("full") decomposition."""
+    is the exact ("full") decomposition.
+
+    When the in-memory fit would not fit the device (_pca_plan), the rows stream through it instead
+    (_reduce_pca_streamed); when not even the m x m matrix (m = min(n_samples, n_features)) and its eigen-decomposition
+    fit, MemoryError."""
     assert 0 <= low_factor <= 1
     as_np = type(train_descs) == np.ndarray
     dev = _lib.require_cuda(None)
+    (n, d), n_te = train_descs.shape, test_descs.shape[0]
+    n_fit, n_held = (n + n_te, n + n_te) if low_factor != 0.0 and n < d else (n, n_te)     # fallback: cat(tr, te)
+    plan = _pca_plan(n_fit, d, n_held, _device_budget(dev), _STAGE_BYTES)       # the first fit's
+    if plan is not None:
+        tr, te = _reduce_pca_streamed(train_descs, test_descs, lower_dim, low_factor, fallback, whitening, plan, dev)
+        return (tr.numpy(), te.numpy()) if as_np else (tr, te)
     tr, te = _as_device_f32(train_descs, dev), _as_device_f32(test_descs, dev)
 
     def ret(a, b):
@@ -213,6 +271,153 @@ def reduce_pca(train_descs: np.ndarray, test_descs: np.ndarray, lower_dim: int, 
     pca = _PcaDev(tr.shape[1]).fit(tr)
     basis = torch.cat((pca.components_[:n_top], pca.components_[-n_low:])).contiguous()
     return ret(_gemm_nt_dev(tr - pca.mean_, basis), _gemm_nt_dev(te - pca.mean_, basis))
+
+
+class _PcaRows:
+    """The rows of one or more [n_i, d] matrices stacked -- reduce_pca's training rows, or its training and test rows
+    for the `fallback` pre-reduction -- as numpy arrays or tensors of any dtype and strides, on the host or a device.
+    Read box by box; no input is ever copied whole, converted whole or pinned."""
+
+    def __init__(self, parts):
+        self.parts = [torch.from_numpy(p) if type(p) == np.ndarray else p.detach() for p in parts]
+        self.shape = (sum(p.shape[0] for p in self.parts), self.parts[0].shape[1])
+        self.is_cuda = all(p.is_cuda for p in self.parts)
+
+    def _slices(self, r0, r1, c0, c1):
+        o = 0
+        for p in self.parts:
+            a, b = max(r0 - o, 0), min(r1 - o, p.shape[0])
+            if a < b:
+                yield p[a:b, c0:c1]
+            o += p.shape[0]
+
+    def gather(self, dst, box):
+        """rows[r0:r1, c0:c1] -> the host fp32 matrix dst"""
+        o = 0
+        for s in self._slices(*box):
+            dst[o:o + s.shape[0]].copy_(s)
+            o += s.shape[0]
+
+    def on_device(self, box, dev):
+        """rows[r0:r1, c0:c1] as a device fp32 matrix with unit column stride: a view of the input where it is one
+        already, else a converted copy of the box"""
+        s = list(self._slices(*box))
+        if (len(s) == 1 and s[0].device == dev and s[0].dtype == torch.float32 and s[0].stride(1) == 1 and
+                s[0].stride(0) >= s[0].shape[1]):
+            return s[0]
+        return torch.cat([t.to(device=dev, dtype=torch.float32) for t in s]).contiguous()
+
+
+def _pca_staged(rows, boxes, dev):
+    """Yield rows[r0:r1, c0:c1] for each box in order, as a device fp32 matrix with unit column stride.  Device rows are
+    read in place.  Host rows are gathered into one of two pinned stages and copied to the device on a side stream;
+    box j+1 is gathered and its copy queued when the caller resumes the generator, i.e. once it has queued its work on
+    box j, so the gather and the copy overlap that work."""
+    if rows.is_cuda:
+        for b in boxes:
+            yield rows.on_device(b, dev)
+        return
+    if not boxes:
+        return
+    cap = max((r1 - r0) * (c1 - c0) for r0, r1, c0, c1 in boxes)
+    host = [torch.empty(cap, pin_memory=True) for _ in range(min(2, len(boxes)))]
+    raw = [torch.empty(cap, device=dev) for _ in host]
+    cs, xs = torch.cuda.current_stream(), torch.cuda.Stream()
+    copied, freed = [None, None], [None, None]
+
+    def stage(j):
+        r0, r1, c0, c1 = boxes[j]
+        s, size = j & 1, (r1 - r0) * (c1 - c0)
+        if copied[s] is not None:
+            copied[s].synchronize()                    # the stage's previous copy is done
+        rows.gather(host[s][:size].view(r1 - r0, c1 - c0), boxes[j])
+        with torch.cuda.stream(xs):
+            if freed[s] is not None:
+                xs.wait_event(freed[s])                # the caller's work on the box before is done with raw[s]
+            raw[s][:size].copy_(host[s][:size], non_blocking=True)
+            copied[s] = torch.cuda.Event()
+            copied[s].record(xs)
+
+    stage(0)
+    for j, (r0, r1, c0, c1) in enumerate(boxes):
+        s = j & 1
+        cs.wait_event(copied[s])
+        yield raw[s][:(r1 - r0) * (c1 - c0)].view(r1 - r0, c1 - c0)
+        freed[s] = torch.cuda.Event()
+        freed[s].record(cs)
+        if j + 1 < len(boxes):
+            stage(j + 1)
+
+
+def _pca_colsum(x, out):
+    """out[c] += sum_r x[r, c] (fp64) for a device fp32 matrix x with unit column stride"""
+    lib = _lib.load()
+    rows, cols = x.shape
+    ws = _lib.workspaces.get(x.device, lib.anyloc_pca_colsum_workspace_bytes(rows, cols), "pca")
+    _lib.check(lib.anyloc_pca_colsum(C.c_void_p(x.data_ptr()), x.stride(0), rows, cols, C.c_void_p(out.data_ptr()),
+                                     _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_pca_colsum")
+
+
+def _pca_accumulate(mode, x, mu, out, u=None):
+    """anyloc_pca_accumulate(ANYLOC_PCA_<mode>) of the device fp32 matrix x (unit column stride) centred by mu into the
+    fp64 view out (unit column stride)"""
+    rows, cols = x.shape
+    k, ld_u = (u.shape[1], u.stride(0)) if u is not None else (0, 0)
+    _lib.check(_lib.load().anyloc_pca_accumulate(
+        _lib.PCA[mode], C.c_void_p(x.data_ptr()), x.stride(0), rows, cols, C.c_void_p(mu.data_ptr()), _lib.ptr(u),
+        ld_u, k, C.c_void_p(out.data_ptr()), out.stride(0), _lib.stream_ptr()), "anyloc_pca_accumulate")
+
+
+def _pca_project_streamed(rows, project, k, dev):
+    """project(x) (device rows -> [rows, k] fp32) of every row of `rows`, fed in row pieces of at most one staging
+    buffer -> host fp32 [n, k]"""
+    n, d = rows.shape
+    out = torch.empty(n, k)
+    boxes = _pca_boxes(n, d, ("cov", max(1, min(n, _STAGE_BYTES // (4 * d)))))
+    with torch.cuda.device(dev):
+        for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+            out[r0:r1].copy_(project(x))
+    return out
+
+
+def _pca_fit_any(rows, k, dev):
+    """_PcaDev(k) fitted on `rows` (a _PcaRows): in memory when that fits the device, else streamed"""
+    n, d = rows.shape
+    plan = _pca_plan(n, d, 0, _device_budget(dev), _STAGE_BYTES)
+    if plan is None:
+        return _PcaDev(k).fit(torch.cat([_as_device_f32(p, dev) for p in rows.parts]))
+    return _PcaDev(k).fit_streamed(rows, plan, dev)
+
+
+def _reduce_pca_streamed(train_descs, test_descs, lower_dim, low_factor, fallback, whitening, plan, dev):
+    """reduce_pca for rows the in-memory route cannot hold: the same steps (fallback pre-reduction, fit, whitening,
+    top / bottom basis).  The first fit is streamed by `plan` (_PcaDev.fit_streamed); the fit after the fallback
+    pre-reduction, on its far smaller rows, is streamed only when it has to be.  Every projection streams in row pieces
+    straight into host fp32 outputs -> (tr, te) host tensors"""
+    tr, te = _PcaRows([train_descs]), _PcaRows([test_descs])
+    if low_factor == 0.0:
+        pca = _PcaDev(lower_dim, whiten=whitening).fit_streamed(tr, plan, dev)
+        return (_pca_project_streamed(tr, pca.transform, lower_dim, dev),
+                _pca_project_streamed(te, pca.transform, lower_dim, dev))
+    n_samples, n_components = tr.shape
+    if n_samples < n_components:
+        print(f"Too few samples, fallback to {fallback}d first")
+        pca = _PcaDev(fallback).fit_streamed(_PcaRows(tr.parts + te.parts), plan, dev)
+        tr = _PcaRows([_pca_project_streamed(tr, pca.transform, fallback, dev)])
+        te = _PcaRows([_pca_project_streamed(te, pca.transform, fallback, dev)])
+    n_low = int(low_factor * lower_dim)
+    n_top = lower_dim - n_low
+    print(f"Up: {n_top}, Down: {n_low}")
+    if n_samples < n_components:
+        pca = _pca_fit_any(tr, tr.shape[1], dev)
+    else:
+        pca = _PcaDev(n_components).fit_streamed(tr, plan, dev)
+    basis = torch.cat((pca.components_[:n_top], pca.components_[-n_low:])).contiguous()
+
+    def project(x):
+        return _gemm_nt_dev(x - pca.mean_, basis)
+    return (_pca_project_streamed(tr, project, basis.shape[0], dev),
+            _pca_project_streamed(te, project, basis.shape[0], dev))
 
 
 # ------------------------------------------------------------------ image pre-processing (extension)
@@ -659,6 +864,54 @@ def _kmeans_plan(R, D, chunks, rows_per, budget, copies, ws_bytes, stage_bytes):
     rr = chunks * P
     fixed = ws_bytes(rr) + 4 * R + (1 + copies) * rr * row      # two transfer buffers, plus the normalised round
     return P, int(max(0, min(n_rounds, (budget - fixed) // (rr * row))))
+
+
+# device bytes of torch.linalg.eigh (cuSOLVER syevd) on an m x m fp64 matrix, in 8 m^2 units: the matrix, the
+# eigenvectors and the workspace, which cusolverDnXsyevd_bufferSize puts at 4.0 matrices (CUDA 12.8's cuSOLVER on an
+# H100, m = 10 000 to 26 733)
+_PCA_EIGH_MATRICES = 6
+# the largest m that workspace query accepts there; from m = 26 734 on it returns CUSOLVER_STATUS_INVALID_VALUE
+_PCA_EIGH_MAX_M = 26_733
+
+
+def _pca_in_memory_bytes(n, d, n_held):
+    """Peak device bytes of reduce_pca's in-memory route (_PcaDev) on n rows of dimension d, beside n_held more rows
+    it holds: the fp32 rows and their centred fp32 and fp64 copies (16 n d), the other rows (4 n_held d), and the m x m
+    fp64 matrix, m = min(n, d), with what eigh needs for it."""
+    m = min(n, d)
+    return 16 * n * d + 4 * n_held * d + 8 * _PCA_EIGH_MATRICES * m * m
+
+
+def _pca_plan(n, d, n_held, budget, stage_bytes):
+    """Where reduce_pca fits n rows of dimension d, beside n_held more rows, given `budget` free device bytes.
+    -> None: in memory, when _pca_in_memory_bytes fits.  Else streamed (_PcaDev.fit_streamed): ("cov", P) for n > d,
+    the rows fed in pieces of P rows; ("gram", W) for n <= d, the columns fed in slabs of W columns of all n rows.  A
+    piece fills at most one `stage_bytes` staging buffer, and two device copies of it fit beside the m x m matrix.
+    MemoryError when not even the m x m matrix and its eigh fit, or m is beyond _PCA_EIGH_MAX_M: reduce_pca has no
+    top-k eigensolver."""
+    if _pca_in_memory_bytes(n, d, n_held) <= budget:
+        return None
+    m = min(n, d)
+    eig = 8 * _PCA_EIGH_MATRICES * m * m
+    if m > _PCA_EIGH_MAX_M:
+        raise MemoryError(f"reduce_pca: m = min(n_samples, n_features) = {m} is beyond the {_PCA_EIGH_MAX_M} x "
+                          f"{_PCA_EIGH_MAX_M} fp64 matrices the eigensolver (torch.linalg.eigh, cuSOLVER syevd) takes")
+    if eig > budget:
+        raise MemoryError(f"reduce_pca: the {m} x {m} fp64 Gram / covariance matrix (m = min(n_samples, n_features)) "
+                          f"and its eigen-decomposition need {eig} bytes of device memory, {budget} are free")
+    spare = (budget - 8 * m * m) // 2               # per device copy of a piece, beside the accumulating matrix
+    if n > d:
+        return "cov", int(max(1, min(n, stage_bytes // (4 * d), spare // (4 * d))))
+    return "gram", int(max(1, min(d, stage_bytes // (4 * n), spare // (4 * n))))
+
+
+def _pca_boxes(n, d, plan):
+    """The pieces (r0, r1, c0, c1) of rows [n, d] a streamed PCA pass reads, in order: pieces of P rows over all
+    columns ("cov", P), or slabs of P columns over all rows ("gram", P)"""
+    route, P = plan
+    if route == "cov":
+        return [(r0, min(n, r0 + P), 0, d) for r0 in range(0, n, P)]
+    return [(0, n, c0, min(d, c0 + P)) for c0 in range(0, d, P)]
 
 
 def _host_fit_plan(X, dev, K, copies):

@@ -484,6 +484,36 @@ int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const
  * ld_in < D, or x or y not 16-byte aligned.  rows = 0 launches nothing. */
 int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y, void* stream);
 
+/* ------------------------------------------------------------------ streamed PCA fit
+ * The fit of reduce_pca (utilities.py:522-586, sklearn PCA(svd_solver="full")) for rows that do not fit on the device:
+ * the rows are fed in pieces and every sum lands in a caller-owned fp64 output that persists across calls.  x is fp32
+ * [rows, cols], rows ld elements apart (ld >= cols); mu is fp64 [cols].  Each call sums in a fixed order, so the same
+ * pieces give the same bits on every run.  Null pointers, negative sizes or ld < the row length return ANYLOC_ERR_ARG
+ * before anything is launched; zero-sized calls launch nothing.
+ *
+ * anyloc_pca_colsum (utilities.py:522-586, the mean pass): sum[c] += sum_r x[r, c], in fp64.  Workspace
+ * anyloc_pca_colsum_workspace_bytes(rows, cols); a short one returns ANYLOC_ERR_WORKSPACE. */
+size_t anyloc_pca_colsum_workspace_bytes(int64_t rows, int cols);
+int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int cols, double* sum, void* ws, size_t ws_bytes,
+                      void* stream);
+/* anyloc_pca_accumulate (utilities.py:522-586, the Gram / covariance matrix and vt): a centred A^T.B over the rows of
+ * one piece on the FP64 tensor cores, each x element centred as (double)x - mu in registers.  out has ld_out >= its
+ * columns; only its [out rows, out columns] elements are read and written.
+ *   ANYLOC_PCA_COV  (n > d): out[cols, cols] += (x - mu)^T (x - mu), over a block of rows.  Lower-triangle 64x64 tiles
+ *                   only; anyloc_pca_mirror completes the matrix.  u NULL, k unused.
+ *   ANYLOC_PCA_GRAM (n <= d): out[rows, rows] += (x - mu)(x - mu)^T, over a slab of columns (x = those columns of all
+ *                   rows, mu their means).  Lower-triangle tiles only, as above.  u NULL, k unused.
+ *   ANYLOC_PCA_VT   out[k, cols] += u^T (x - mu), u fp64 [rows, k] (ld_u >= k; NULL only with k = 0), not centred: the Gram route's
+ *                   vt = u[:, :k]^T Xc / s for one slab of columns (the caller divides by s). */
+#define ANYLOC_PCA_COV 0
+#define ANYLOC_PCA_GRAM 1
+#define ANYLOC_PCA_VT 2
+int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64_t rows, int cols, const double* mu,
+                          const double* u, int64_t ld_u, int k, double* out, int64_t ld_out, void* stream);
+/* anyloc_pca_mirror (utilities.py:522-586): a[i, j] = a[j, i] for j > i < m, after the last triangle accumulate, so
+ * the matrix handed to the eigensolver is exactly symmetric. */
+int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream);
+
 /* ------------------------------------------------------------------ sibling aggregators
  * The pooling the reference's other DINOv2 scripts apply to the same patch features [B,N,D] -> [B,D]:
  *   ANYLOC_POOL_AVG  torch.mean(ret, dim=1)        scripts/dino_v2_gp.py:130-131
