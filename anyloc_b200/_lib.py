@@ -23,7 +23,7 @@ ACT_SCALE = 8.0     # kActScale in csrc/common.cuh
 VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_extract_varlen call
 PREPROCESS_VARLEN_BATCH = 64    # ANYLOC_PREPROCESS_VARLEN_BATCH: images per launch of anyloc_preprocess_u8_varlen
 ERR = {"arg": -1, "cuda": -2, "workspace": -3, "unsupported": -4}
-PCA = {"cov": 0, "gram": 1, "vt": 2}        # ANYLOC_PCA_*: the layouts of anyloc_pca_accumulate
+PCA = {"cov": 0, "gram": 1, "vt": 2, "sketch": 3}        # ANYLOC_PCA_*: the layouts of anyloc_pca_accumulate
 
 
 class AnylocError(RuntimeError):

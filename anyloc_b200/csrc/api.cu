@@ -388,9 +388,10 @@ extern "C" int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int c
 
 extern "C" int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64_t rows, int cols, const double* mu,
                                      const double* u, int64_t ld_u, int k, double* out, int64_t ld_out, void* stream) {
-  ANYLOC_REQUIRE(mode == ANYLOC_PCA_COV || mode == ANYLOC_PCA_GRAM || mode == ANYLOC_PCA_VT,
-                 "pca_accumulate: unknown mode %d", mode);
-  ANYLOC_REQUIRE(x && mu && out && (mode != ANYLOC_PCA_VT || u || k == 0), "pca_accumulate: null pointer");
+  ANYLOC_REQUIRE(mode == ANYLOC_PCA_COV || mode == ANYLOC_PCA_GRAM || mode == ANYLOC_PCA_VT ||
+                 mode == ANYLOC_PCA_SKETCH, "pca_accumulate: unknown mode %d", mode);
+  const bool uses_u = mode == ANYLOC_PCA_VT || mode == ANYLOC_PCA_SKETCH;
+  ANYLOC_REQUIRE(x && mu && out && (!uses_u || u || k == 0), "pca_accumulate: null pointer");
   ANYLOC_REQUIRE(rows >= 0 && cols >= 0 && ld >= cols, "pca_accumulate: rows=%lld cols=%d ld=%lld (rows >= 0, "
                  "cols >= 0, ld >= cols)", (long long)rows, cols, (long long)ld);
   // out [M, N] += sum over K of A(kk, i) B(kk, j)
@@ -398,9 +399,15 @@ extern "C" int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64
   if (mode == ANYLOC_PCA_GRAM) {
     M = N = rows;
     K = cols;
-  } else if (mode == ANYLOC_PCA_VT) {
+  } else if (uses_u) {
     ANYLOC_REQUIRE(k >= 0 && ld_u >= k, "pca_accumulate: k=%d ld_u=%lld (k >= 0, ld_u >= k)", k, (long long)ld_u);
-    M = k;
+    if (mode == ANYLOC_PCA_VT) {
+      M = k;
+    } else {
+      M = rows;
+      N = k;
+      K = cols;
+    }
   }
   ANYLOC_REQUIRE(M <= (1 << 20) && ld_out >= N, "pca_accumulate: output [%lld, %lld] with ld_out=%lld (at most 2^20 "
                  "rows, ld_out >= columns)", (long long)M, (long long)N, (long long)ld_out);

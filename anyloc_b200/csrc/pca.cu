@@ -1,6 +1,7 @@
 // Streamed PCA fit of reduce_pca (utilities.py:522-586) for rows that do not fit on the device: the fp64 column sums
 // of the mean pass and the centred A^T.B products of the Gram / covariance matrix and of vt, accumulated piece by
-// piece into caller-owned fp64 outputs.  The rows arrive as fp32 and are centred in fp64 registers on the way to
+// piece into caller-owned fp64 outputs; and the two products of the randomized fit's power iterations, (X - mu).W
+// (sketch) and W^T.(X - mu) (vt).  The rows arrive as fp32 and are centred in fp64 registers on the way to
 // shared memory; no centred or fp64 copy of them is ever written.  The products run on the FP64 tensor cores
 // (mma.sync m16n8k4 .f64, DMMA: wgmma has no fp64 shape).
 #include <algorithm>
@@ -85,13 +86,15 @@ __device__ __forceinline__ void store_tile(double (*s)[PCA_LDS], const double (&
 //   ANYLOC_PCA_COV : A = B = x - mu (MN-major, rows [K, M]);  lower-triangle tiles only (out [M, M]).
 //   ANYLOC_PCA_GRAM: A = B = (x - mu)^T (K-major, x [M, K]);  lower-triangle tiles only (out [M, M]).
 //   ANYLOC_PCA_VT  : A = u (fp64 [K, M], not centred), B = x - mu (x [K, N]); every tile (out [M, N]).
+//   ANYLOC_PCA_SKETCH: A = (x - mu)^T (K-major, x [M, K]), B = u (fp64 [K, N], not centred); every tile (out [M, N]).
 template <int MODE>
 __global__ void __launch_bounds__(PCA_THREADS) pca_atb_kernel(const float* __restrict__ x, int64_t ldx,
                                                               const double* __restrict__ mu,
                                                               const double* __restrict__ u, int64_t ldu, int64_t K,
                                                               int M, int N, double* __restrict__ out, int64_t ldo) {
-  constexpr bool TRI = MODE != ANYLOC_PCA_VT;
-  constexpr bool KMAJOR = MODE == ANYLOC_PCA_GRAM;
+  constexpr bool TRI = MODE == ANYLOC_PCA_COV || MODE == ANYLOC_PCA_GRAM;
+  constexpr bool A_KMAJOR = MODE == ANYLOC_PCA_GRAM || MODE == ANYLOC_PCA_SKETCH;
+  constexpr bool B_KMAJOR = MODE == ANYLOC_PCA_GRAM;
   __shared__ double As[PCA_BK][PCA_LDS];
   __shared__ double Bs[PCA_BK][PCA_LDS];
 
@@ -118,10 +121,12 @@ __global__ void __launch_bounds__(PCA_THREADS) pca_atb_kernel(const float* __res
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.0;
 
-  using ALoader = TileLoader<KMAJOR, typename std::conditional<MODE == ANYLOC_PCA_VT, double, float>::type>;
+  using ALoader = TileLoader<A_KMAJOR, typename std::conditional<MODE == ANYLOC_PCA_VT, double, float>::type>;
+  using BLoader = TileLoader<B_KMAJOR, typename std::conditional<MODE == ANYLOC_PCA_SKETCH, double, float>::type>;
   const ALoader la = MODE == ANYLOC_PCA_VT ? ALoader((const typename ALoader::Elem*)u, ldu, nullptr, m0, M)
                                            : ALoader((const typename ALoader::Elem*)x, ldx, mu, m0, M);
-  const TileLoader<KMAJOR, float> lb(x, ldx, mu, n0, N);
+  const BLoader lb = MODE == ANYLOC_PCA_SKETCH ? BLoader((const typename BLoader::Elem*)u, ldu, nullptr, n0, N)
+                                               : BLoader((const typename BLoader::Elem*)x, ldx, mu, n0, N);
   double va[8], vb[8];
   auto load = [&](int64_t k0) {
     la.load(va, k0, K);
@@ -130,8 +135,8 @@ __global__ void __launch_bounds__(PCA_THREADS) pca_atb_kernel(const float* __res
   const int64_t nk = (K + PCA_BK - 1) / PCA_BK;
   load(0);
   for (int64_t kt = 0; kt < nk; ++kt) {
-    store_tile<KMAJOR>(As, va);
-    store_tile<KMAJOR>(Bs, vb);
+    store_tile<A_KMAJOR>(As, va);
+    store_tile<B_KMAJOR>(Bs, vb);
     __syncthreads();
     if (kt + 1 < nk) load((kt + 1) * PCA_BK);     // the next tile's global loads fly under this tile's DMMAs
 #pragma unroll
@@ -234,6 +239,9 @@ int pca_atb_launch(int mode, const float* x, int64_t ldx, const double* mu, cons
   if (mode == ANYLOC_PCA_VT) {
     pca_atb_kernel<ANYLOC_PCA_VT><<<dim3((unsigned)tn, (unsigned)tm), PCA_THREADS, 0, st>>>(x, ldx, mu, u, ldu, K, M,
                                                                                            N, out, ldo);
+  } else if (mode == ANYLOC_PCA_SKETCH) {
+    pca_atb_kernel<ANYLOC_PCA_SKETCH><<<dim3((unsigned)tn, (unsigned)tm), PCA_THREADS, 0, st>>>(x, ldx, mu, u, ldu, K,
+                                                                                               M, N, out, ldo);
   } else {
     const unsigned tiles = (unsigned)(tm * (tm + 1) / 2);
     if (mode == ANYLOC_PCA_COV)

@@ -9,6 +9,7 @@ Put `<repo>/anyloc_b200/dropin` first on PYTHONPATH to make `from utilities impo
 reference's scripts (scripts/dino_v2_vlad.py:37-38,50) resolve here (see INTEGRATION.md).
 """
 import ctypes as C
+import math
 import os
 import random
 from typing import List, Literal, Tuple, Union
@@ -139,6 +140,40 @@ def _gemm_nt_dev(a, b, bias=None):
     return out
 
 
+def _flip_signs(vt):
+    """The signs of sklearn's `svd_flip(u_based_decision=False)`: each row of vt times the sign of its largest-magnitude
+    element (+1 for a zero row) -> [k, 1]"""
+    sign = torch.sign(torch.gather(vt, 1, vt.abs().argmax(dim=1, keepdim=True)))
+    sign[sign == 0] = 1
+    return sign
+
+
+def _lu_pl(y):
+    """P L of the partial-pivoting LU y = P L U, the normaliser `scipy.linalg.lu(y, permute_l=True)[0]` that sklearn's
+    randomized range finder applies after each half-step: [m, min(m, w)] for y [m, w].  P is applied as a row
+    permutation, never formed."""
+    if y.is_cuda:
+        # torch's default backend runs MAGMA's batched getrf on one tall matrix: slower than cuSOLVER, and it prints
+        # a warning on every call
+        prev = torch.backends.cuda.preferred_linalg_library()
+        torch.backends.cuda.preferred_linalg_library("cusolver")
+        try:
+            lu, piv = torch.linalg.lu_factor(y)
+        finally:
+            torch.backends.cuda.preferred_linalg_library(prev)
+    else:
+        lu, piv = torch.linalg.lu_factor(y)
+    m, r = lu.shape[0], min(lu.shape)
+    lo = lu[:, :r].tril(-1)
+    lo.diagonal().fill_(1.0)
+    perm = np.arange(m)
+    for i, p in enumerate(piv.cpu().numpy() - 1):     # LAPACK's row interchanges, in order: y[perm] = L U
+        perm[[i, p]] = perm[[p, i]]
+    out = torch.empty(m, r, dtype=y.dtype, device=y.device)
+    out[torch.from_numpy(perm).to(y.device)] = lo
+    return out
+
+
 class _PcaDev:
     """`sklearn.decomposition.PCA(k, svd_solver="full", whiten=...)` as reduce_pca uses it (utilities.py:560-586), on
     the GPU: the fit is a one-off fp64 eigen-decomposition of the smaller Gram / covariance matrix (torch.linalg.eigh,
@@ -170,8 +205,7 @@ class _PcaDev:
 
     def _set_components(self, vt, s, n):
         k = self.n_components
-        sign = torch.sign(torch.gather(vt, 1, vt.abs().argmax(dim=1, keepdim=True)))
-        sign[sign == 0] = 1
+        sign = _flip_signs(vt)
         self.components_ = (vt * sign).float().contiguous()
         self.singular_values_ = s[:k].float()
         self.explained_variance_ = (s[:k] ** 2 / (n - 1)).float()
@@ -222,6 +256,57 @@ class _PcaDev:
             self.mean_ = mu.float()
             return self._set_components(vt, s, n)
 
+    def fit_randomized(self, rows, w, P, dev):
+        """`sklearn.decomposition.PCA(k, svd_solver="randomized")`'s fit with its default parameters (_randomized_svd:
+        n_oversamples=10, n_iter="auto", LU-normalised power iterations, transpose="auto"), step for step, on rows (a
+        _PcaRows) read in row pieces of P.  w is the test matrix (_pca_test_matrix).  With A = Xc, or Xc^T when
+        n < d: n_iter times Q = PL(A Q), Q = PL(A^T Q); then Q = qr(A Q), B = Q^T A = U^ S Vt, U = Q U^.  Every product
+        with A is one pass over the rows (anyloc_pca_accumulate "sketch": Xc W, "vt": W^T Xc), fp64 on the FP64 tensor
+        cores; LU, QR and SVD are fp64 torch.linalg (cuSOLVER) on the [max(n, d), l] and [min(n, d), l] matrices.
+        Also sets fit_rows_: what sklearn's fit_transform returns for the rows, U S (U sqrt(n - 1) when whitening)."""
+        n, d = rows.shape
+        k = self.n_components
+        if not 1 <= k <= min(n, d):
+            raise ValueError(f"n_components={k} must be between 1 and min(n_samples, n_features)={min(n, d)} with "
+                             "svd_solver='randomized'")
+        _, n_iter, transpose = _pca_randomized_params(n, d, k)
+        boxes = _pca_boxes(n, d, ("cov", P))
+        with torch.cuda.device(dev):
+            mu = torch.zeros(d, dtype=torch.float64, device=dev)
+            for x in _pca_staged(rows, boxes, dev):
+                _pca_colsum(x, mu)
+            mu /= n
+
+            def xw(q):                                  # Xc q: [n, width]
+                q, out = q.contiguous(), torch.zeros(n, q.shape[1], dtype=torch.float64, device=dev)
+                for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                    _pca_accumulate("sketch", x, mu, out[r0:r1], q)
+                return out
+
+            def xtw(q):                                 # Xc^T q: [d, width], summed over the row pieces
+                q, out = q.contiguous(), torch.zeros(q.shape[1], d, dtype=torch.float64, device=dev)
+                for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                    _pca_accumulate("vt", x, mu, out, q[r0:r1])
+                return out.T
+            a, at = (xtw, xw) if transpose else (xw, xtw)
+            q = torch.from_numpy(w).to(device=dev, dtype=torch.float64)
+            for _ in range(n_iter):
+                q = _lu_pl(a(q))
+                q = _lu_pl(at(q))
+            q = torch.linalg.qr(a(q)).Q
+            # the SVD of B = Q^T A [l, min(n, d)] through the QR of B^T = Q2 R: B = R^T Q2^T, R^T = U^ S W^T
+            q2, r = torch.linalg.qr(at(q))
+            uh, s, wt = torch.linalg.svd(r.T)
+            vt = wt @ q2.T
+            uq = q @ uh
+            del q, q2
+            u_rows, vt = (vt[:k].T, uq[:, :k].T) if transpose else (uq[:, :k], vt[:k])
+            sign = _flip_signs(vt)
+            scale = math.sqrt(n - 1) if self.whiten else s[:k]
+            self.fit_rows_ = (u_rows * (sign.T * scale)).float()
+            self.mean_ = mu.float()
+            return self._set_components(vt.contiguous(), s, n)
+
     def transform(self, x):
         y = _gemm_nt_dev(x - self.mean_, self.components_)
         if self.whiten:
@@ -236,8 +321,9 @@ def reduce_pca(train_descs: np.ndarray, test_descs: np.ndarray, lower_dim: int, 
         -> Tuple[np.ndarray, np.ndarray]:
     """PCA projection fitted on the training set (utilities.py:522-586; scripts/dino_v2_vlad.py:357-369 reduces the
     database / query VLADs with it).  Same arguments and return types (numpy in -> numpy out, torch tensors accepted);
-    the arithmetic runs on the GPU -- see _PcaDev.  `svd_solver` is accepted for signature compatibility: the result
-    is the exact ("full") decomposition.
+    the arithmetic runs on the GPU -- see _PcaDev.  svd_solver="randomized" is sklearn's randomized PCA with its
+    defaults, step for step and from the same draw of numpy's global generator (_reduce_pca_randomized); it has no
+    limit on min(n_samples, n_features).  Every other `svd_solver` gives the exact ("full") decomposition.
 
     When the in-memory fit would not fit the device (_pca_plan), the rows stream through it instead
     (_reduce_pca_streamed); when not even the m x m matrix (m = min(n_samples, n_features)) and its eigen-decomposition
@@ -246,6 +332,15 @@ def reduce_pca(train_descs: np.ndarray, test_descs: np.ndarray, lower_dim: int, 
     as_np = type(train_descs) == np.ndarray
     dev = _lib.require_cuda(None)
     (n, d), n_te = train_descs.shape, test_descs.shape[0]
+    if svd_solver == "randomized" and (low_factor == 0.0 or n < d):
+        tr, te = _reduce_pca_randomized(train_descs, test_descs, lower_dim, low_factor, fallback, whitening, dev)
+        return (tr.numpy(), te.numpy()) if as_np else (tr, te)
+    if svd_solver == "randomized":
+        # a randomized fit of all min(n, d) components spans the whole space, i.e. is the exact fit; sklearn's still
+        # draws its test matrix from numpy's global generator, so draw it too and leave that generator where it does
+        out = reduce_pca(train_descs, test_descs, lower_dim, low_factor, fallback, "full", whitening)
+        _pca_skip_test_matrix(n, d, d)
+        return out
     n_fit, n_held = (n + n_te, n + n_te) if low_factor != 0.0 and n < d else (n, n_te)     # fallback: cat(tr, te)
     plan = _pca_plan(n_fit, d, n_held, _device_budget(dev), _STAGE_BYTES)       # the first fit's
     if plan is not None:
@@ -418,6 +513,79 @@ def _reduce_pca_streamed(train_descs, test_descs, lower_dim, low_factor, fallbac
         return _gemm_nt_dev(x - pca.mean_, basis)
     return (_pca_project_streamed(tr, project, basis.shape[0], dev),
             _pca_project_streamed(te, project, basis.shape[0], dev))
+
+
+def _pca_randomized_params(n, d, k):
+    """(l, n_iter, transpose) of sklearn's PCA(k, svd_solver="randomized") on n x d rows with its defaults: l = k + 10
+    test vectors (n_oversamples), n_iter = 7 power iterations when k < 0.1 min(n, d), else 4 (iterated_power="auto"),
+    and the transpose A = Xc^T when n < d (_randomized_svd's transpose="auto")"""
+    return k + 10, 7 if k < 0.1 * min(n, d) else 4, n < d
+
+
+def _pca_test_matrix(n, d, k, f32):
+    """The Gaussian test matrix of sklearn's _randomized_range_finder, [min(n, d), l] (A.shape[1] of the possibly
+    transposed A), drawn as it draws it: np.random.normal from numpy's global generator, rounded to fp32 for fp32 rows"""
+    w = np.random.normal(size=(min(n, d), _pca_randomized_params(n, d, k)[0]))
+    return w.astype(np.float32) if f32 else w
+
+
+def _pca_skip_test_matrix(n, d, k, chunk=1 << 22):
+    """Advance numpy's global generator past _pca_test_matrix(n, d, k) without holding it: the legacy Gaussian sampler
+    yields the same sequence, and ends in the same state, whether the values are drawn at once or in pieces"""
+    total = min(n, d) * _pca_randomized_params(n, d, k)[0]
+    for i in range(0, total, chunk):
+        np.random.normal(size=min(chunk, total - i))
+
+
+def _pca_fit_randomized(rows, k, dev, whiten=False):
+    """_PcaDev(k, whiten).fit_randomized on `rows` (a _PcaRows).  Device fp32 rows with unit column stride are read in
+    place.  Other rows are uploaded once as fp32 when they fit the device beside the fit's matrices
+    (_pca_randomized_plan), else every pass streams them in row pieces through the pinned stages."""
+    n, d = rows.shape
+    if not 1 <= k <= min(n, d):
+        raise ValueError(f"n_components={k} must be between 1 and min(n_samples, n_features)={min(n, d)} with "
+                         "svd_solver='randomized'")
+    f32 = all(q.dtype == torch.float32 for q in rows.parts)
+    p = rows.parts[0]
+    P = min(n, _PCA_PIECE_MAX_ROWS)
+    if not (len(rows.parts) == 1 and p.device == dev and p.dtype == torch.float32 and p.stride(1) == 1 and
+            p.stride(0) >= d):
+        plan = _pca_randomized_plan(n, d, _pca_randomized_params(n, d, k)[0], _device_budget(dev), _STAGE_BYTES)
+        if plan is None:
+            x = torch.empty(n, d, device=dev)
+            boxes = _pca_boxes(n, d, ("cov", max(1, min(n, _STAGE_BYTES // (4 * d)))))
+            with torch.cuda.device(dev):
+                for (r0, r1, _, _), piece in zip(boxes, _pca_staged(rows, boxes, dev)):
+                    x[r0:r1].copy_(piece)
+            rows = _PcaRows([x])
+        else:
+            P = plan
+    w = _pca_test_matrix(n, d, k, f32)
+    return _PcaDev(k, whiten=whiten).fit_randomized(rows, w, P, dev)
+
+
+def _reduce_pca_randomized(train_descs, test_descs, lower_dim, low_factor, fallback, whitening, dev):
+    """reduce_pca(svd_solver="randomized") for low_factor == 0 and for the low_factor branch's `fallback`
+    pre-reduction (n_samples < n_features), whose fits are sklearn's randomized ones (_pca_fit_randomized).  As sklearn's
+    fit_transform, a fit's own rows come back as U S from the fit; other rows are projected in row pieces straight into
+    host fp32 outputs.  The low_factor branch's fit of the full basis on the pre-reduced rows is the exact one
+    (_pca_fit_any), as in reduce_pca -> (tr, te) host tensors"""
+    tr, te = _PcaRows([train_descs]), _PcaRows([test_descs])
+    if low_factor == 0.0:
+        pca = _pca_fit_randomized(tr, lower_dim, dev, whiten=whitening)
+        return pca.fit_rows_.cpu(), _pca_project_streamed(te, pca.transform, lower_dim, dev)
+    n = tr.shape[0]
+    print(f"Too few samples, fallback to {fallback}d first")
+    both = _pca_fit_randomized(_PcaRows(tr.parts + te.parts), fallback, dev).fit_rows_
+    tr, te = both[:n].contiguous(), both[n:].contiguous()
+    n_low = int(low_factor * lower_dim)
+    n_top = lower_dim - n_low
+    print(f"Up: {n_top}, Down: {n_low}")
+    pca = _pca_fit_any(_PcaRows([tr]), fallback, dev)
+    _pca_skip_test_matrix(n, fallback, fallback)            # as in reduce_pca: the full basis is the exact fit
+    basis = torch.cat((pca.components_[:n_top], pca.components_[-n_low:])).contiguous()
+    with torch.cuda.device(dev):
+        return _gemm_nt_dev(tr - pca.mean_, basis).cpu(), _gemm_nt_dev(te - pca.mean_, basis).cpu()
 
 
 # ------------------------------------------------------------------ image pre-processing (extension)
@@ -895,14 +1063,43 @@ def _pca_plan(n, d, n_held, budget, stage_bytes):
     eig = 8 * _PCA_EIGH_MATRICES * m * m
     if m > _PCA_EIGH_MAX_M:
         raise MemoryError(f"reduce_pca: m = min(n_samples, n_features) = {m} is beyond the {_PCA_EIGH_MAX_M} x "
-                          f"{_PCA_EIGH_MAX_M} fp64 matrices the eigensolver (torch.linalg.eigh, cuSOLVER syevd) takes")
+                          f"{_PCA_EIGH_MAX_M} fp64 matrices the eigensolver (torch.linalg.eigh, cuSOLVER syevd) takes; "
+                          "svd_solver='randomized' has no such limit")
     if eig > budget:
         raise MemoryError(f"reduce_pca: the {m} x {m} fp64 Gram / covariance matrix (m = min(n_samples, n_features)) "
-                          f"and its eigen-decomposition need {eig} bytes of device memory, {budget} are free")
+                          f"and its eigen-decomposition need {eig} bytes of device memory, {budget} are free; "
+                          "svd_solver='randomized' needs far less")
     spare = (budget - 8 * m * m) // 2               # per device copy of a piece, beside the accumulating matrix
     if n > d:
         return "cov", int(max(1, min(n, stage_bytes // (4 * d), spare // (4 * d))))
     return "gram", int(max(1, min(d, stage_bytes // (4 * n), spare // (4 * n))))
+
+
+_PCA_PIECE_MAX_ROWS = 1 << 20      # anyloc_pca_accumulate's "sketch" output has at most 2^20 rows
+
+
+def _pca_randomized_bytes(n, d, l):
+    """Peak device bytes of the randomized fit's matrices (_PcaDev.fit_randomized) beside its rows, l = k + 10: three
+    fp64 [max(n, d), l] and three fp64 [min(n, d), l] (a pass's product, its LU factor and P L beside the basis the
+    product came from; at the end Q, U = Q U^, B^T, its QR and vt), and the fp32 fit rows and components"""
+    return 8 * l * (3 * max(n, d) + 3 * min(n, d)) + 4 * l * (n + d)
+
+
+def _pca_randomized_plan(n, d, l, budget, stage_bytes):
+    """Where reduce_pca's randomized fit (l = k + 10 test vectors) reads n rows of dimension d that are not device fp32
+    already, given `budget` free device bytes.  -> None: uploaded once as fp32 [n, d], when that fits beside the fit's
+    matrices (_pca_randomized_bytes) and, during the upload, beside two staging copies.  Else P: every pass streams the
+    rows in pieces of P rows, a piece filling at most one `stage_bytes` staging buffer with two device copies beside the
+    matrices.  MemoryError when not even the matrices and two one-row pieces fit."""
+    mats = _pca_randomized_bytes(n, d, l)
+    piece = 4 * d * max(1, min(n, stage_bytes // (4 * d)))
+    if 4 * n * d + max(mats, 2 * piece) <= budget:
+        return None
+    if mats + 8 * d > budget:
+        raise MemoryError(f"reduce_pca(svd_solver='randomized'): the fp64 [{max(n, d)}, {l}] and [{min(n, d)}, {l}] "
+                          f"matrices of the randomized fit and their factorisations need {mats} bytes of device memory "
+                          f"and a piece of one row {8 * d} more, {budget} are free")
+    return int(max(1, min(n, _PCA_PIECE_MAX_ROWS, stage_bytes // (4 * d), (budget - mats) // (8 * d))))
 
 
 def _pca_boxes(n, d, plan):

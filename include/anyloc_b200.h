@@ -485,7 +485,8 @@ int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const
 int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in, float* y, void* stream);
 
 /* ------------------------------------------------------------------ streamed PCA fit
- * The fit of reduce_pca (utilities.py:522-586, sklearn PCA(svd_solver="full")) for rows that do not fit on the device:
+ * The fit of reduce_pca (utilities.py:522-586, sklearn PCA(svd_solver="full")) for rows that do not fit on the device,
+ * and the row passes of its randomized fit (svd_solver="randomized"):
  * the rows are fed in pieces and every sum lands in a caller-owned fp64 output that persists across calls.  x is fp32
  * [rows, cols], rows ld elements apart (ld >= cols); mu is fp64 [cols].  Each call sums in a fixed order, so the same
  * pieces give the same bits on every run.  Null pointers, negative sizes or ld < the row length return ANYLOC_ERR_ARG
@@ -504,10 +505,14 @@ int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int cols, double
  *   ANYLOC_PCA_GRAM (n <= d): out[rows, rows] += (x - mu)(x - mu)^T, over a slab of columns (x = those columns of all
  *                   rows, mu their means).  Lower-triangle tiles only, as above.  u NULL, k unused.
  *   ANYLOC_PCA_VT   out[k, cols] += u^T (x - mu), u fp64 [rows, k] (ld_u >= k; NULL only with k = 0), not centred: the Gram route's
- *                   vt = u[:, :k]^T Xc / s for one slab of columns (the caller divides by s). */
+ *                   vt = u[:, :k]^T Xc / s for one slab of columns (the caller divides by s), and the randomized fit's
+ *                   W^T Xc over a block of rows.
+ *   ANYLOC_PCA_SKETCH out[rows, k] += (x - mu) u, u fp64 [cols, k] (ld_u >= k; NULL only with k = 0), not centred: the
+ *                   randomized fit's Xc W for a block of rows, contracting over the columns.  Every tile; rows <= 2^20. */
 #define ANYLOC_PCA_COV 0
 #define ANYLOC_PCA_GRAM 1
 #define ANYLOC_PCA_VT 2
+#define ANYLOC_PCA_SKETCH 3
 int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64_t rows, int cols, const double* mu,
                           const double* u, int64_t ld_u, int k, double* out, int64_t ld_out, void* stream);
 /* anyloc_pca_mirror (utilities.py:522-586): a[i, j] = a[j, i] for j > i < m, after the last triangle accumulate, so
