@@ -24,6 +24,8 @@ VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_ext
 PREPROCESS_VARLEN_BATCH = 64    # ANYLOC_PREPROCESS_VARLEN_BATCH: images per launch of anyloc_preprocess_u8_varlen
 ERR = {"arg": -1, "cuda": -2, "workspace": -3, "unsupported": -4}
 PCA = {"cov": 0, "gram": 1, "vt": 2, "sketch": 3}        # ANYLOC_PCA_*: the layouts of anyloc_pca_accumulate
+VLAD_ROUTE_SORTED = 2       # ANYLOC_VLAD_ROUTE_SORTED: anyloc_vlad_generate_route's answer where generate refuses
+KMEANS_SMEM_BYTES = 220 * 1024      # anyloc_kmeans_update's shared memory: (K * 128 + K) * 4 bytes must fit
 
 
 class AnylocError(RuntimeError):
@@ -68,6 +70,10 @@ _SIGS = {
     "anyloc_vlad_prepare": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_vlad_generate_prepared": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t] +
                                       [C.c_int] * 7 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_vlad_generate_route": (C.c_int, [C.c_int] * 4),
+    "anyloc_vlad_sorted_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "anyloc_vlad_generate_sorted": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t] +
+                                    [C.c_int] * 7 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_vlad_generate_soft": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_float] +
                                   [C.c_int] * 2 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_preprocess_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.POINTER(C.c_float)] * 2 +
@@ -93,6 +99,10 @@ _SIGS = {
                                                  C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_kmeans_finalize": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_size_t, C.c_void_p]),
+    "anyloc_kmeans_accumulate_round_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64] +
+                                             [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_kmeans_update_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_int] * 3 +
+                                   [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_topk_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
     "anyloc_topk": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 6 +
                     [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -12,6 +12,8 @@
 //   accumulate3 : CTA per (128-column slice, image): rows sorted by label, sum_{label=k}(x^ - c_k) in registers, then
 //                 the intra + global L2 normalisation in the same kernel.  Images of more rows than its shared memory
 //                 holds take accumulate2 (shared-memory accumulators) + the normalise launch.
+//   sorted      : (anyloc_vlad_generate_sorted, the shapes neither holds) accumulate3's order with its per-image tables
+//                 in the workspace: sort, accumulate, combine and normalise launches.
 // (The FFMA assignment kernel serves D > 2048, calls of fewer than 256 rows and workspaces without room for the
 // coarse scores, at any K.)
 #include <algorithm>
@@ -719,6 +721,187 @@ vlad_normalize_kernel(float* __restrict__ vlad, const float* __restrict__ partia
   }
 }
 
+// ------------------------------------------------------------------ sorted route (any K, any N)
+// accumulate3's summation order with its per-image tables in the workspace instead of shared memory, so no (N, K) is
+// out of reach.  vlad_sort_kernel (CTA per image) builds the stable label order of the rows, the tasks of <= 64 rows
+// of one cluster and the slot bases of multi-task clusters exactly as accumulate3's prologue does;
+// vlad_sorted_accumulate_kernel sums each task in registers with accumulate3's loop; vlad_sorted_combine_kernel adds
+// the slots of multi-task clusters in task order; vlad_normalize_kernel then applies the factors of vlad_norm_factors.
+// Every sum has accumulate3's order, so the descriptors are bitwise those of accumulate3 wherever it runs.
+constexpr int SORTED_TASKS_PER_CTA = 64;
+static inline int sorted_max_slots(int N) { return 2 * (N / ACC3_SEG) + 2; }
+struct SortedTables {
+  int64_t* ooff;     // [B,N] row offsets n * D in label order (stable)
+  float* inv_s;      // [B,N] 1/|x| in the same order
+  int* cntw;         // [B,ACC3_WARPS,K] per-warp histograms, then placement cursors
+  int* start;        // [B,K+1] first sorted position of cluster k
+  int* tstart;       // [B,K+1] first task of cluster k
+  int* sbase;        // [B,K+1] first slot of a multi-task cluster
+  int* task_k;       // [B,max_tasks] cluster of each task
+  float* slots;      // [B,max_slots,D] partial sums of multi-task clusters
+};
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sort_kernel(const int32_t* __restrict__ labels, const float* __restrict__ inv_norm, int N, int D, int K,
+                 int norm_descs, SortedTables tb) {
+  const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int maxT = acc3_max_tasks_dev(N, K);
+  const int32_t* lab = labels + (size_t)b * N;
+  int64_t* ooff = tb.ooff + (size_t)b * N;
+  float* inv_s = tb.inv_s + (size_t)b * N;
+  int* cntw = tb.cntw + (size_t)b * ACC3_WARPS * K;
+  int* start = tb.start + (size_t)b * (K + 1);
+  int* tstart = tb.tstart + (size_t)b * (K + 1);
+  int* sbase = tb.sbase + (size_t)b * (K + 1);
+  int* task_k = tb.task_k + (size_t)b * maxT;
+  for (int i = t; i < ACC3_WARPS * K; i += blockDim.x) cntw[i] = 0;
+  __syncthreads();
+  const int chunk = (((N + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
+  const int r0 = min(N, w * chunk), r1 = min(N, r0 + chunk);
+  for (int n = r0 + lane; n < r1; n += 32) { const int l = lab[n]; if (l >= 0) atomicAdd(&cntw[w * K + l], 1); }
+  __syncthreads();
+  for (int k = t; k < K; k += blockDim.x) {
+    int tot = 0;
+    for (int ww = 0; ww < ACC3_WARPS; ++ww) { const int c = cntw[ww * K + k]; cntw[ww * K + k] = tot; tot += c; }
+    start[k] = tot;
+  }
+  __syncthreads();
+  if (w == 0) {
+    int run_r = 0, run_t = 0, run_s = 0;
+    for (int k0 = 0; k0 < K; k0 += 32) {
+      const int k = k0 + lane;
+      const int c = k < K ? start[k] : 0;
+      const int nt = k < K ? max(1, (c + ACC3_SEG - 1) / ACC3_SEG) : 0;
+      const int ns = nt > 1 ? nt : 0;
+      int ir = c, it = nt, is = ns;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int yr = __shfl_up_sync(0xffffffffu, ir, o), yt = __shfl_up_sync(0xffffffffu, it, o),
+                  ys = __shfl_up_sync(0xffffffffu, is, o);
+        if (lane >= o) { ir += yr; it += yt; is += ys; }
+      }
+      if (k < K) { start[k] = run_r + ir - c; tstart[k] = run_t + it - nt; sbase[k] = run_s + is - ns; }
+      run_r += __shfl_sync(0xffffffffu, ir, 31);
+      run_t += __shfl_sync(0xffffffffu, it, 31);
+      run_s += __shfl_sync(0xffffffffu, is, 31);
+    }
+    if (lane == 0) { start[K] = run_r; tstart[K] = run_t; sbase[K] = run_s; }
+  }
+  __syncthreads();
+  for (int k = t; k < K; k += blockDim.x)
+    for (int q = tstart[k]; q < tstart[k + 1]; ++q) task_k[q] = k;
+  for (int n0 = r0; n0 < r1; n0 += 32) {
+    const int n = n0 + lane;
+    const int l = n < r1 ? lab[n] : -1;
+    const bool active = l >= 0;
+    const unsigned am = __ballot_sync(0xffffffffu, active);
+    unsigned peers = 0; int rank = 0;
+    if (active) {
+      peers = __match_any_sync(am, l);
+      rank = __popc(peers & ((1u << lane) - 1u));
+      const int pos = start[l] + cntw[w * K + l] + rank;
+      ooff[pos] = (int64_t)n * D;
+      inv_s[pos] = norm_descs ? inv_norm[(size_t)b * N + n] : 1.0f;
+    }
+    __syncwarp();
+    if (active && rank == 0) cntw[w * K + l] += __popc(peers);
+    __syncwarp();
+  }
+}
+
+// CTA = (128-column slice, image, range of SORTED_TASKS_PER_CTA tasks); warps grab the range's tasks dynamically.  A
+// single-task cluster's sum goes straight to the descriptor with its sum of squares; a multi-task cluster's to its
+// slot.  The loop body is accumulate3's, term for term.
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sorted_accumulate_kernel(const float* __restrict__ x, const float* __restrict__ centers, int N, int D, int K,
+                              SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  __shared__ int next_task;
+  const int b = blockIdx.y, slice = blockIdx.x, nslices = gridDim.x, lane = threadIdx.x & 31;
+  const int maxT = acc3_max_tasks_dev(N, K), maxS = 2 * (N / ACC3_SEG) + 2;
+  const int* start = tb.start + (size_t)b * (K + 1);
+  const int* tstart = tb.tstart + (size_t)b * (K + 1);
+  const int* sbase = tb.sbase + (size_t)b * (K + 1);
+  const int* task_k = tb.task_k + (size_t)b * maxT;
+  const int64_t* ooff = tb.ooff + (size_t)b * N;
+  const float* inv_s = tb.inv_s + (size_t)b * N;
+  const int q0 = blockIdx.z * SORTED_TASKS_PER_CTA, q1 = min(tstart[K], q0 + SORTED_TASKS_PER_CTA);
+  if (q0 >= q1) return;
+  if (threadIdx.x == 0) next_task = q0;
+  __syncthreads();
+  const int col = slice * 128 + lane * 4;
+  const bool colok = col < D;
+  const float* xb = x + (size_t)b * N * D + col;
+  auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
+  int q = grab();
+  while (q < q1) {
+    const int qn = grab();
+    const int k = task_k[q];
+    const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
+    const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
+    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (colok) {
+      constexpr int U = 8;
+      int i = s;
+      for (; i + U <= e; i += U) {
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const float sc = inv_s[i + u];
+          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+        }
+      }
+      if (i < e) {
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          if (i + u < e) {
+            const float sc = inv_s[i + u];
+            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+          }
+        }
+      }
+    }
+    if (nt == 1) {
+      if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
+      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+      if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
+    } else if (colok) {
+      *reinterpret_cast<float4*>(tb.slots + ((size_t)b * maxS + sbase[k] + seg) * D + col) = a;
+    }
+    q = qn;
+  }
+}
+
+// CTA = (128-column slice, image): clusters of several tasks, their slots added in task order (accumulate3's combine)
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sorted_combine_kernel(int N, int D, int K, SortedTables tb, float* __restrict__ vlad,
+                           float* __restrict__ partial_ss) {
+  const int b = blockIdx.y, slice = blockIdx.x, nslices = gridDim.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int maxS = 2 * (N / ACC3_SEG) + 2;
+  const int* tstart = tb.tstart + (size_t)b * (K + 1);
+  const int* sbase = tb.sbase + (size_t)b * (K + 1);
+  const int col = slice * 128 + lane * 4;
+  const bool colok = col < D;
+  for (int k = w; k < K; k += ACC3_WARPS) {
+    const int nt = tstart[k + 1] - tstart[k];
+    if (nt <= 1) continue;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int q = 0; q < nt; ++q) {
+      const float4 p = colok ? *reinterpret_cast<const float4*>(tb.slots + ((size_t)b * maxS + sbase[k] + q) * D + col)
+                             : make_float4(0.f, 0.f, 0.f, 0.f);
+      a.x += p.x; a.y += p.y; a.z += p.z; a.w += p.w;
+    }
+    if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
+    const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+    if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
+  }
+}
+
 // ------------------------------------------------------------------ k-means update
 // Deterministic: every (column slice, row chunk) CTA writes ITS partial sums / counts, the finalize kernel adds the
 // chunks in chunk order -- no floating-point atomics, so a fitted vocabulary is bit-reproducible for a fixed seed
@@ -752,6 +935,36 @@ __global__ void kmeans_accumulate_kernel(const float* __restrict__ x, const int3
     if (colok) ps[(size_t)k * D + col] = acc[k * ACC_COLS + t];
   if (blockIdx.x == 0)
     for (int k = t; k < K; k += ACC_COLS) pcounts[(size_t)blockIdx.y * K + k] = cnt[k];
+}
+
+// The same partials for any K: grid (D/128 slices, row-chunks, cluster tiles); a CTA keeps the 128-column sums of the
+// k_tile clusters [k0, k0 + k_tile) in shared memory and adds only the rows labelled inside its tile, in row order --
+// every (cluster, column) sum is kmeans_accumulate_kernel's sequential sum, so the partials are bitwise equal.
+__global__ void kmeans_accumulate_tiled_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                                               int64_t R, int64_t piece, int D, int K, int k_tile, int resume,
+                                               float* __restrict__ psums /* [chunks,K,D] */,
+                                               float* __restrict__ pcounts /* [chunks,K] */) {
+  extern __shared__ float acc[];                          // [k_tile][128] sums, then [k_tile] counts
+  const int t = threadIdx.x, col = blockIdx.x * ACC_COLS + t;
+  const bool colok = col < D;
+  const int k0 = blockIdx.z * k_tile, kt = min(k_tile, K - k0);
+  float* ps = psums + (size_t)blockIdx.y * K * D + (size_t)k0 * D;
+  for (int k = 0; k < kt; ++k) acc[k * ACC_COLS + t] = resume && colok ? ps[(size_t)k * D + col] : 0.f;
+  float* cnt = acc + (size_t)k_tile * ACC_COLS;
+  for (int k = t; k < kt; k += ACC_COLS) cnt[k] = resume && blockIdx.x == 0 ? pcounts[(size_t)blockIdx.y * K + k0 + k] : 0.f;
+  __syncthreads();
+  int64_t r0 = (int64_t)blockIdx.y * piece, r1 = min(R, r0 + piece);
+  for (int64_t r = r0; r < r1; ++r) {
+    const int l = labels[r] - k0;
+    if (l < 0 || l >= kt) continue;
+    if (colok) acc[l * ACC_COLS + t] += __ldg(x + r * D + col);
+    if (blockIdx.x == 0 && t == 0) cnt[l] += 1.f;
+  }
+  __syncthreads();
+  for (int k = 0; k < kt; ++k)
+    if (colok) ps[(size_t)k * D + col] = acc[k * ACC_COLS + t];
+  if (blockIdx.x == 0)
+    for (int k = t; k < kt; k += ACC_COLS) pcounts[(size_t)blockIdx.y * K + k0 + k] = cnt[k];
 }
 
 __global__ void __launch_bounds__(256)
@@ -928,6 +1141,20 @@ extern "C" int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_
   return ANYLOC_OK;
 }
 
+// accumulate2's row-splitting warps: as many as shared memory allows ((1 + warps) * K * 128 floats), at most 4 when
+// two CTAs then fit per SM, else what fits in one (signed: K > 200 leaves none)
+static int acc2_warps(int K) {
+  return (int)std::min<long long>(4, (long long)((200 * 1024) / ((size_t)K * 128 * 4)) - 1);
+}
+
+// The one predicate that picks the hard-VLAD accumulation: accumulate3 when its shared memory fits 100 KB, else
+// accumulate2 when one row-splitting warp fits, else the sorted route (anyloc_vlad_generate_sorted), which
+// vlad_generate_impl refuses.
+static int vlad_route(int N, int D, int K) {
+  if (acc3_smem_bytes(N, K) <= 100 * 1024 && (int64_t)N * D < (1ll << 31)) return ANYLOC_VLAD_ROUTE_ACC3;
+  return acc2_warps(K) >= 1 ? ANYLOC_VLAD_ROUTE_ACC2 : ANYLOC_VLAD_ROUTE_SORTED;
+}
+
 static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const float* centers, void* prepared,
                               size_t prepared_bytes, int B, int N, int D, int K, int dist_mode, int norm_descs,
                               int intra_norm, float* vlad, int32_t* labels_out, void* ws, size_t ws_bytes, void* stream) {
@@ -942,7 +1169,7 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   const size_t R = (size_t)B * N;
   const int nslices = cdiv(D, ACC_COLS);
   const size_t smem3 = acc3_smem_bytes(N, K);
-  const bool fits3 = smem3 <= 100 * 1024 && (int64_t)N * D < (1ll << 31);
+  const bool fits3 = vlad_route(N, D, K) == ANYLOC_VLAD_ROUTE_ACC3;
   HardBufs hb;
   if (!carve_hard(ws, ws_bytes, B, N, D, K, fits3, &hb)) {
     set_error("vlad_generate: workspace too small (%zu bytes given)", ws_bytes);
@@ -950,9 +1177,8 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   }
   AssignBufs& ab = hb.ab;
   const bool acc3 = ab.done != nullptr;             // fits3 and room for the tickets
-  // else accumulate2 with as many row-splitting warps as shared memory allows ((1 + warps) * K * 128 floats), at most
-  // 4 row-splitting warps when two CTAs then fit per SM, else what fits in one (signed: K > 400 leaves none)
-  const int warps = (int)std::min<long long>(4, (long long)((200 * 1024) / ((size_t)K * 128 * 4)) - 1);
+  // else accumulate2; shapes neither serves belong to anyloc_vlad_generate_sorted
+  const int warps = acc2_warps(K);
   ANYLOC_REQUIRE(acc3 || warps >= 1, "vlad_generate: K=%d N=%d needs %zu B shared memory (accumulate3 has 100 KB)", K,
                  N, smem3);
   // a prepared vocabulary replaces the per-call centre prep on every route
@@ -1006,6 +1232,81 @@ extern "C" int anyloc_vlad_generate_prepared(const float* feats, const int32_t* 
   ANYLOC_REQUIRE(prepared, "vlad_generate_prepared: null prepared blob");
   return vlad_generate_impl(feats, n_valid, centers, prepared, prepared_bytes, B, N, D, K, dist_mode, norm_descs,
                             intra_norm, vlad, labels_out, ws, ws_bytes, stream);
+}
+
+extern "C" int anyloc_vlad_generate_route(int B, int N, int D, int K) {
+  ANYLOC_REQUIRE(B >= 0 && N >= 0 && D > 0 && K > 0, "vlad_generate_route: bad dims");
+  return vlad_route(N, D, K);
+}
+
+// The sorted route's workspace: carve_hard's buffers without the tickets, then the per-image tables.  With
+// ws == nullptr a dry run; returns the bytes taken, 0 when the workspace is too small.
+static size_t carve_sorted(void* ws, size_t ws_bytes, int B, int N, int D, int K, HardBufs* hb, SortedTables* tb) {
+  const size_t off = carve_hard(ws, ws_bytes, B, N, D, K, false, hb);
+  if (!off) return 0;
+  Workspace w(ws ? (void*)((char*)ws + off) : (void*)256, ws ? ws_bytes - off : (size_t)-1 / 2);
+  const size_t R = (size_t)B * N, K1 = (size_t)B * (K + 1);
+  tb->ooff = w.take<int64_t>(R);
+  tb->inv_s = w.take<float>(R);
+  tb->cntw = w.take<int>((size_t)B * ACC3_WARPS * K);
+  tb->start = w.take<int>(K1);
+  tb->tstart = w.take<int>(K1);
+  tb->sbase = w.take<int>(K1);
+  tb->task_k = w.take<int>((size_t)B * acc3_max_tasks(N, K));
+  tb->slots = w.take<float>((size_t)B * sorted_max_slots(N) * D);
+  const bool ok = tb->ooff && tb->inv_s && tb->cntw && tb->start && tb->tstart && tb->sbase && tb->task_k && tb->slots;
+  return ok ? off + w.off : 0;
+}
+
+extern "C" size_t anyloc_vlad_sorted_workspace_bytes(int B, int N, int D, int K) {
+  HardBufs hb;
+  SortedTables tb;
+  return carve_sorted(nullptr, 0, B, N, D, K, &hb, &tb);
+}
+
+extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_valid, const float* centers,
+                                           void* prepared, size_t prepared_bytes, int B, int N, int D, int K,
+                                           int dist_mode, int norm_descs, int intra_norm, float* vlad,
+                                           int32_t* labels_out, void* ws, size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(feats && centers && prepared && vlad && ws, "vlad_generate_sorted: null pointer");
+  ANYLOC_REQUIRE(B >= 0 && N >= 0 && D > 0 && K > 0, "vlad_generate_sorted: bad dims");
+  ANYLOC_REQUIRE(D % 4 == 0, "vlad_generate_sorted: D=%d must be a multiple of 4", D);
+  ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
+                 "vlad_generate_sorted: unknown dist_mode %d", dist_mode);
+  const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
+  ANYLOC_REQUIRE(B <= 65535 && ztasks <= 65535, "vlad_generate_sorted: B=%d N=%d K=%d exceed the launch grid", B, N, K);
+  if (B == 0) return ANYLOC_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
+  HardBufs hb;
+  SortedTables tb;
+  if (!carve_sorted(ws, ws_bytes, B, N, D, K, &hb, &tb)) {
+    set_error("vlad_generate_sorted: workspace too small (%zu bytes given, %zu needed)", ws_bytes,
+              anyloc_vlad_sorted_workspace_bytes(B, N, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  AssignBufs& ab = hb.ab;
+  PreparedView pv;
+  const bool use_prep = carve_prepared(prepared, prepared_bytes, D, K, &pv);
+  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
+  const size_t R = (size_t)B * N;
+  const int nslices = cdiv(D, ACC_COLS);
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
+  int rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st,
+                         use_prep);
+  if (rc) return rc;
+  vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, N, D, K, norm_descs, tb);
+  ANYLOC_CHECK_LAUNCH();
+  vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, tb,
+                                                                                      vlad, hb.partial);
+  ANYLOC_CHECK_LAUNCH();
+  vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, hb.partial);
+  ANYLOC_CHECK_LAUNCH();
+  rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
+  if (rc) return rc;
+  if (labels_out)
+    ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, hb.labels, R * 4, cudaMemcpyDeviceToDevice, st));
+  return ANYLOC_OK;
 }
 
 // Centres for F.cosine_similarity: c / max(|c|, 1e-8)
@@ -1164,6 +1465,51 @@ extern "C" int anyloc_kmeans_update(const float* x, const int32_t* labels, const
   int64_t rows_per;
   int rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
   if (!rc) rc = anyloc_kmeans_accumulate_round(x, labels, R, R, rows_per, D, K, 0, ws, ws_bytes, stream);
+  if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
+  return rc;
+}
+
+// clusters per CTA of kmeans_accumulate_tiled_kernel: (k_tile * 128 + k_tile) * 4 bytes within the same 220 KB
+constexpr int KMEANS_MAX_TILE = 220 * 1024 / ((ACC_COLS + 1) * 4);
+
+extern "C" int anyloc_kmeans_accumulate_round_tiled(const float* x, const int32_t* labels, int64_t R, int64_t round_rows,
+                                                    int64_t piece_rows, int D, int K, int k_tile, int resume, void* ws,
+                                                    size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(x && labels && ws, "kmeans_accumulate_round_tiled: null pointer");
+  ANYLOC_REQUIRE(R >= 0 && D > 0 && K > 0 && piece_rows >= 0 && round_rows >= 0,
+                 "kmeans_accumulate_round_tiled: bad dims R=%lld D=%d K=%d", (long long)R, D, K);
+  ANYLOC_REQUIRE(k_tile >= 0 && k_tile <= KMEANS_MAX_TILE, "kmeans_accumulate_round_tiled: k_tile=%d not in [0, %d]",
+                 k_tile, KMEANS_MAX_TILE);
+  KmeansBufs b;
+  if (!take_kmeans_bufs(ws, ws_bytes, R, D, K, &b)) {
+    set_error("kmeans_accumulate_round_tiled: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_kmeans_round_workspace_bytes(R, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  ANYLOC_REQUIRE(round_rows <= (int64_t)b.chunks * piece_rows,
+                 "kmeans_accumulate_round_tiled: %lld rows do not fit %d pieces of %lld", (long long)round_rows,
+                 b.chunks, (long long)piece_rows);
+  const int tile = std::min(K, k_tile == 0 ? KMEANS_MAX_TILE : k_tile);
+  const int ntiles = cdiv(K, tile);
+  ANYLOC_REQUIRE(ntiles <= 65535, "kmeans_accumulate_round_tiled: K=%d needs %d tiles of %d", K, ntiles, tile);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t smem = ((size_t)tile * ACC_COLS + tile) * 4;
+  ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(kmeans_accumulate_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+  kmeans_accumulate_tiled_kernel<<<dim3(cdiv(D, ACC_COLS), b.chunks, ntiles), ACC_COLS, smem, st>>>(
+      x, labels, round_rows, piece_rows, D, K, tile, resume, b.psums, b.pcounts);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+
+extern "C" int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels, const float* old_centers, int64_t R,
+                                          int D, int K, int k_tile, float* new_centers, float* err_out, void* ws,
+                                          size_t ws_bytes, void* stream) {
+  ANYLOC_REQUIRE(x && labels && old_centers && new_centers && err_out && ws, "kmeans_update_tiled: null pointer");
+  int chunks;
+  int64_t rows_per;
+  int rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
+  if (!rc) rc = anyloc_kmeans_accumulate_round_tiled(x, labels, R, R, rows_per, D, K, k_tile, 0, ws, ws_bytes, stream);
   if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
   return rc;
 }

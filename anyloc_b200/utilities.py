@@ -1030,8 +1030,33 @@ def _kmeans_plan(R, D, chunks, rows_per, budget, copies, ws_bytes, stage_bytes):
     P = max(1, min(rows_per, stage_bytes // (chunks * row)))
     n_rounds = -(-rows_per // P)
     rr = chunks * P
-    fixed = ws_bytes(rr) + 4 * R + (1 + copies) * rr * row      # two transfer buffers, plus the normalised round
+    fixed = _kmeans_stream_bytes(R, D, chunks, P, copies, ws_bytes)
     return P, int(max(0, min(n_rounds, (budget - fixed) // (rr * row))))
+
+
+def _kmeans_stream_bytes(R, D, chunks, P, copies, ws_bytes):
+    """Device bytes of a streamed fit with no round resident: the workspaces and labels of one round of chunks * P
+    rows, the labels of all R rows, two transfer buffers and the normalised round"""
+    rr = chunks * P
+    return ws_bytes(rr) + 4 * R + (1 + copies) * rr * 4 * D
+
+
+def _kmeans_fit_plan(R, D, chunks, rows_per, budget, free, copies, ws_bytes, stage_bytes):
+    """_kmeans_plan, with MemoryError naming the bytes when the streamed fit does not fit the `free` device bytes
+    even with no round resident (the partial sums alone are chunks * K * D * 4 bytes: 403 MB at K = 1024, D = 1536)"""
+    plan = _kmeans_plan(R, D, chunks, rows_per, budget, copies, ws_bytes, stage_bytes)
+    if plan is not None:
+        need = _kmeans_stream_bytes(R, D, chunks, plan[0], copies, ws_bytes)
+        if need > free:
+            raise MemoryError(f"VLAD.fit: the streamed k-means fit of {R} x {D} rows needs {need} bytes of device "
+                              f"memory (workspaces, labels and round buffers), {free} are free")
+    return plan
+
+
+def _kmeans_tiled(K):
+    """whether the k-means update takes the cluster-tiled kernels: anyloc_kmeans_update keeps (K * 128 + K) * 4 bytes
+    of partial sums in shared memory and refuses K beyond them"""
+    return (K * 128 + K) * 4 > _lib.KMEANS_SMEM_BYTES
 
 
 # device bytes of torch.linalg.eigh (cuSOLVER syevd) on an m x m fp64 matrix, in 8 m^2 units: the matrix, the
@@ -1119,11 +1144,13 @@ def _host_fit_plan(X, dev, K, copies):
     R, D = X.shape
     with torch.cuda.device(dev):
         chunks, rows_per = _kmeans_partition(R, D)
+        upd = lib.anyloc_kmeans_round_workspace_bytes(R, D, K)     # chunks * K * D partial sums, whatever the round
 
         def ws_bytes(n):
-            return (lib.anyloc_vlad_workspace_bytes(1, n, D, K) + lib.anyloc_kmeans_round_workspace_bytes(n, D, K) +
-                    4 * n)
-        return _kmeans_plan(R, D, chunks, rows_per, _device_budget(dev), copies, ws_bytes, _STAGE_BYTES)
+            return lib.anyloc_vlad_workspace_bytes(1, n, D, K) + upd + 4 * n
+        budget = _device_budget(dev)
+        return _kmeans_fit_plan(R, D, chunks, rows_per, budget, torch.cuda.mem_get_info(dev)[0], copies, ws_bytes,
+                                _STAGE_BYTES)
 
 
 def _kmeans_partition(R, D):
@@ -1167,9 +1194,14 @@ class _KMeans:
         err = torch.zeros(1, device=x.device)
         with torch.cuda.device(x.device):
             ws = _lib.workspaces.get(x.device, lib.anyloc_kmeans_workspace_bytes(n, D, K), "kmeans_upd")
-            _lib.check(lib.anyloc_kmeans_update(_lib.ptr(x), _lib.ptr(labels), _lib.ptr(c), n, D, K,
-                                                _lib.ptr(new_c), _lib.ptr(err), _lib.ptr(ws), ws.numel(),
-                                                _lib.stream_ptr()), "anyloc_kmeans_update")
+            if _kmeans_tiled(K):
+                _lib.check(lib.anyloc_kmeans_update_tiled(_lib.ptr(x), _lib.ptr(labels), _lib.ptr(c), n, D, K, 0,
+                                                          _lib.ptr(new_c), _lib.ptr(err), _lib.ptr(ws), ws.numel(),
+                                                          _lib.stream_ptr()), "anyloc_kmeans_update_tiled")
+            else:
+                _lib.check(lib.anyloc_kmeans_update(_lib.ptr(x), _lib.ptr(labels), _lib.ptr(c), n, D, K,
+                                                    _lib.ptr(new_c), _lib.ptr(err), _lib.ptr(ws), ws.numel(),
+                                                    _lib.stream_ptr()), "anyloc_kmeans_update")
         return new_c, err              # err stays on the device: fit_predict reads it one iteration late
 
     def predict(self, X):
@@ -1241,6 +1273,7 @@ class _KMeans:
         X = X.detach()
         R, D = X.shape
         K = self.n_clusters
+        tiled = _kmeans_tiled(K)
         with torch.cuda.device(dev):
             chunks, rows_per = _kmeans_partition(R, D)
             rounds = _stream_rounds(R, chunks, rows_per, P)
@@ -1297,9 +1330,15 @@ class _KMeans:
                         if j < resident:
                             kept[offs[j]:offs[j + 1]].copy_(x)
                     labels_r.append(self._assign(x, c))
-                    _lib.check(lib.anyloc_kmeans_accumulate_round(_lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j],
-                                                                  piece[j], D, K, int(j > 0), _lib.ptr(ws), ws.numel(),
-                                                                  _lib.stream_ptr()), "anyloc_kmeans_accumulate_round")
+                    if tiled:
+                        _lib.check(lib.anyloc_kmeans_accumulate_round_tiled(
+                            _lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j], piece[j], D, K, 0, int(j > 0),
+                            _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_kmeans_accumulate_round_tiled")
+                    else:
+                        _lib.check(lib.anyloc_kmeans_accumulate_round(_lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j],
+                                                                      piece[j], D, K, int(j > 0), _lib.ptr(ws),
+                                                                      ws.numel(), _lib.stream_ptr()),
+                                   "anyloc_kmeans_accumulate_round")
                     if it == 0 or j >= resident:
                         freed[s] = torch.cuda.Event()
                         freed[s].record(cs)
@@ -1472,15 +1511,19 @@ class VLAD:
                                                    _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
             _lib.check(rc, "anyloc_vlad_generate_soft")
             return out, assign
+        # the sorted route only for shapes the shared-memory accumulations refuse: every other shape keeps its bits
+        sorted_route = lib.anyloc_vlad_generate_route(B, N, D, K) == _lib.VLAD_ROUTE_SORTED
+        generate, name, ws_bytes = ((lib.anyloc_vlad_generate_sorted, "anyloc_vlad_generate_sorted",
+                                     lib.anyloc_vlad_sorted_workspace_bytes) if sorted_route else
+                                    (lib.anyloc_vlad_generate_prepared, "anyloc_vlad_generate_prepared",
+                                     lib.anyloc_vlad_workspace_bytes))
         with torch.cuda.device(dev):
-            ws = _lib.workspaces.get(dev, lib.anyloc_vlad_workspace_bytes(B, N, D, K), "vlad")
+            ws = _lib.workspaces.get(dev, ws_bytes(B, N, D, K), "vlad")
             prep = self._prepared_on(dev, centers)
-            rc = lib.anyloc_vlad_generate_prepared(_lib.ptr(feats), _lib.ptr(n_valid), _lib.ptr(centers), _lib.ptr(prep),
-                                                   prep.numel(), B, N, D, K, _lib.DIST[self.mode],
-                                                   int(bool(self.norm_descs)), int(bool(self.intra_norm)),
-                                                   _lib.ptr(out), _lib.ptr(labels), _lib.ptr(ws), ws.numel(),
-                                                   _lib.stream_ptr())
-        _lib.check(rc, "anyloc_vlad_generate_prepared")
+            rc = generate(_lib.ptr(feats), _lib.ptr(n_valid), _lib.ptr(centers), _lib.ptr(prep), prep.numel(), B, N, D,
+                          K, _lib.DIST[self.mode], int(bool(self.norm_descs)), int(bool(self.intra_norm)),
+                          _lib.ptr(out), _lib.ptr(labels), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
+        _lib.check(rc, name)
         return out, labels
 
     # -- per-image cache (utilities.py:843-852 labels, :864-878 soft assignment, :951-970 residuals)

@@ -131,6 +131,23 @@ int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_mode, void*
 int anyloc_vlad_generate_prepared(const float* feats, const int32_t* n_valid, const float* centers, void* prepared,
                                   size_t prepared_bytes, int B, int N, int D, int K, int dist_mode, int norm_descs,
                                   int intra_norm, float* vlad, int32_t* labels, void* ws, size_t ws_bytes, void* stream);
+/* Hard VLAD at any vocabulary size (the reference's VLAD takes any num_clusters, utilities.py:657-662, :819-926;
+ * scripts/dino_v2_vlad_ablations.sh lists num_clusters up to 256).  anyloc_vlad_generate(_prepared) accumulates in
+ * shared memory and refuses shapes outside it; anyloc_vlad_generate_route(B, N, D, K) names the accumulation a shape
+ * takes there: ANYLOC_VLAD_ROUTE_ACC3 / _ACC2, or ANYLOC_VLAD_ROUTE_SORTED where it refuses.
+ * anyloc_vlad_generate_sorted takes the arguments of anyloc_vlad_generate_prepared (same assignment, labels_out and
+ * results' meaning) and accepts every shape with D % 4 == 0: the per-image label sort, task table and multi-task
+ * partial sums live in the workspace (anyloc_vlad_sorted_workspace_bytes), and every sum is taken in the order of
+ * ACC3, so where ACC3 runs both give bitwise equal descriptors and labels.  Each image's descriptor is independent of
+ * the other images of the batch.  No floating-point atomics. */
+#define ANYLOC_VLAD_ROUTE_ACC3 0
+#define ANYLOC_VLAD_ROUTE_ACC2 1
+#define ANYLOC_VLAD_ROUTE_SORTED 2
+int anyloc_vlad_generate_route(int B, int N, int D, int K);
+size_t anyloc_vlad_sorted_workspace_bytes(int B, int N, int D, int K);
+int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_valid, const float* centers, void* prepared,
+                                size_t prepared_bytes, int B, int N, int D, int K, int dist_mode, int norm_descs,
+                                int intra_norm, float* vlad, int32_t* labels, void* ws, size_t ws_bytes, void* stream);
 /* Soft assignment (vlad_mode="soft", utilities.py:862-887):
  *   a[q,k] = softmax_k(soft_temp * cos(x_q, c_k))      (F.cosine_similarity :870-875, norms clamped at 1e-8)
  *   V_k    = sum_q a[q,k] * sum_c (x^_q - c_c)          (the reference weights the residuals to ALL centres by
@@ -177,6 +194,18 @@ int anyloc_kmeans_accumulate_round(const float* x, const int32_t* labels, int64_
                                    void* stream);
 int anyloc_kmeans_finalize(const float* old_centers, int64_t R, int D, int K, float* new_centers, float* err_out,
                            void* ws, size_t ws_bytes, void* stream);
+/* The update and the round at any K (VLAD.fit with any num_clusters, utilities.py:749-791).  anyloc_kmeans_update and
+ * anyloc_kmeans_accumulate_round keep K clusters' 128-column sums in 220 KB of shared memory, so they refuse
+ * (K * 128 + K) * 4 > 220 KB (K >= 437).  The _tiled entries split the clusters into tiles of k_tile (0: the largest
+ * that fits, 436); each tile reads its chunk's rows in order and adds those labelled inside it, so the partial sums,
+ * centres, counts and err_out are bitwise those of the untiled entries wherever those run.  Same partition, workspace
+ * (anyloc_kmeans_round_workspace_bytes), resume semantics and anyloc_kmeans_finalize. */
+int anyloc_kmeans_accumulate_round_tiled(const float* x, const int32_t* labels, int64_t R, int64_t round_rows,
+                                         int64_t piece_rows, int D, int K, int k_tile, int resume, void* ws,
+                                         size_t ws_bytes, void* stream);
+int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels, const float* old_centers, int64_t R, int D,
+                               int K, int k_tile, float* new_centers, float* err_out, void* ws, size_t ws_bytes,
+                               void* stream);
 
 /* ------------------------------------------------------------- retrieval
  * Replaces the faiss part of get_top_k_recall (utilities.py:435-450): optional row
