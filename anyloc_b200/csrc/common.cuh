@@ -118,7 +118,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
 // with one power-of-two scale s, x ~ q s.  s = 2^k with k the smallest integer that puts max|x| / s <= 448 (e4m3's
 // largest finite value), at least -126 so that s and 1/s are normal fp32 numbers; s = 1 for an all-zero (or NaN) row.
 // Scaling by a power of two is exact, so e4m3_rn is the only rounding.  448 = 0.875 2^9: with max|x| = m 2^e, m in
-// [0.5, 1), k = e - 9, or e - 8 when m > 0.875.
+// [0.5, 1), k = e - 9, or e - 8 when m > 0.875.  Activation rows that hold an Inf get a NaN scale (fp8_row_scale).
 __host__ __device__ inline int fp8_scale_exp(float amax) {
   if (!(amax > 0.f) || amax > 3.402823466e38f) return 0;
   int e;
@@ -131,6 +131,16 @@ __host__ __device__ inline float pow2f(int k) {
   union { uint32_t u; float f; } v;
   v.u = (uint32_t)(127 + k) << 23;
   return v.f;
+}
+// The scale s and its inverse of a row of e4m3 activations whose max |x| (NaNs dropped, as fmaxf drops them) is amax.
+// A row that holds an Inf gets s = 1/s = NaN: q = e4m3_rn(x / s) is then NaN throughout, where satfinite would have
+// clamped the Inf to +-448 and left a finite, wrong row, and the GEMM's dequantisation by s makes the consumer's output
+// row NaN.
+__device__ __forceinline__ void fp8_row_scale(float amax, float& s, float& inv) {
+  const int k = fp8_scale_exp(amax);
+  const bool inf = !(amax <= 3.402823466e38f);
+  s = inf ? __int_as_float(0x7fffffff) : pow2f(k);
+  inv = inf ? __int_as_float(0x7fffffff) : pow2f(-k);
 }
 // e4m3_rn of two values (satfinite: beyond +-448 clamps, NaN stays NaN) -> `a` in the low byte, `b` in the high byte
 __device__ __forceinline__ uint32_t pack_e4m3x2(float a, float b) {

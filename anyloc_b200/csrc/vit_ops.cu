@@ -149,8 +149,8 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
         amax = fmaxf(fmaxf(amax, fmaxf(fabsf(v[i].x), fabsf(v[i].y))), fmaxf(fabsf(v[i].z), fabsf(v[i].w)));
       }
     }
-    const int k = fp8_scale_exp(warp_max(amax));
-    const float inv = pow2f(-k);
+    float s, inv;
+    fp8_row_scale(warp_max(amax), s, inv);
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) {
       int d = lane + i * 32;
@@ -158,7 +158,7 @@ layernorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w,
         reinterpret_cast<uint32_t*>(y_hi + (size_t)row * D)[d] =
             pack_e4m3x4(v[i].x * inv, v[i].y * inv, v[i].z * inv, v[i].w * inv);
     }
-    if (lane == 0) reinterpret_cast<float*>(y_lo)[row] = pow2f(k);
+    if (lane == 0) reinterpret_cast<float*>(y_lo)[row] = s;
   } else {
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
@@ -192,15 +192,15 @@ quantize_fp8_rows_kernel(const __nv_bfloat16* __restrict__ x, int M, int K, uint
     amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(lo(u.x)), fabsf(hi(u.x))), fmaxf(fabsf(lo(u.y)), fabsf(hi(u.y)))),
                              fmaxf(fmaxf(fabsf(lo(u.z)), fabsf(hi(u.z))), fmaxf(fabsf(lo(u.w)), fabsf(hi(u.w))))));
   }
-  const int k = fp8_scale_exp(warp_max(amax));
-  const float inv = pow2f(-k);
+  float s, inv;
+  fp8_row_scale(warp_max(amax), s, inv);
   uint2* qr = reinterpret_cast<uint2*>(q + (size_t)row * K);
   for (int i = lane; i < K8; i += 32) {
     const uint4 u = xr[i];
     qr[i] = make_uint2(pack_e4m3x4(lo(u.x) * inv, hi(u.x) * inv, lo(u.y) * inv, hi(u.y) * inv),
                        pack_e4m3x4(lo(u.z) * inv, hi(u.z) * inv, lo(u.w) * inv, hi(u.w) * inv));
   }
-  if (lane == 0) scale[row] = pow2f(k);
+  if (lane == 0) scale[row] = s;
 }
 
 // max |x| of a tensor into *amax (an fp32 bit pattern: non-negative floats order as integers; NaN above every other)

@@ -480,7 +480,10 @@ int anyloc_layernorm_split(const float* x, const float* w, const float* b, int M
 /* The scale rule of ANYLOC_PAIR_FP8: the power of two s for a row or matrix whose largest magnitude is amax (host). */
 float anyloc_fp8_scale(float amax);
 /* bf16 rows x [M, K] -> e4m3 rows q [M, K] and their fp32 scales [M] (ANYLOC_PAIR_FP8's A operand).  K a multiple of 8;
- * x 16-byte, q 8-byte aligned. */
+ * x 16-byte, q 8-byte aligned.  Non-finite elements: a NaN becomes an e4m3 NaN and the row's scale is that of its
+ * finite elements; a row that holds an Inf gets NaN bytes and a NaN scale, so the GEMM that consumes it writes a NaN
+ * output row (e4m3 has no Inf, and saturating it to +-448 would leave the row finite and wrong).  The e4m3 LayerNorm
+ * (anyloc_layernorm_split) does the same for a row whose output overflows fp32. */
 int anyloc_quantize_fp8_rows(const void* x, int M, int K, void* q, float* scales, void* stream);
 /* fp32 x [n] -> e4m3 q [n] = e4m3_rn(x / s) with one scale s, returned in *scale_host (a weight matrix of
  * ANYLOC_PAIR_FP8: its GEMM's alpha is s).  Synchronises the stream (the scale is chosen on the host); a NaN or Inf

@@ -57,14 +57,15 @@ def dptr(t, offset_elems=0):
 
 
 def gemm_nt(L, a_hi, a_lo, b_hi, b_lo, M, N, K, *, pair="tf32", alpha=1.0, epi="bias", bias=None, gamma=None,
-            resid=None, out, out_lo=None, ldo, lda=None, ldb=None, engine="tc3", out_off=0):
+            resid=None, out, out_lo=None, ldo, lda=None, ldb=None, engine="tc3", out_off=0, out_dtype=None):
     """anyloc_gemm_nt on raw buffers (lda/ldb default to K); returns the C ABI's return code.  out, out_lo and resid
-    are buffers whose element `out_off` is the output's (0, 0), with leading dimension ldo."""
+    are buffers whose element `out_off` is the output's (0, 0), with leading dimension ldo.  out_dtype defaults to the
+    input format (e4m3 inputs write bf16: out_dtype="bf16")."""
     import ctypes as C
     return L.load().anyloc_gemm_nt(
         dptr(a_hi), dptr(a_lo), K if lda is None else lda, dptr(b_hi), dptr(b_lo), K if ldb is None else ldb, M, N, K,
         L.PAIR[pair], C.c_float(alpha), L.EPI[epi], dptr(bias), dptr(gamma), dptr(resid, out_off),
-        dptr(out, out_off), dptr(out_lo, out_off), ldo, L.PAIR[pair], L.ENGINE[engine], L.stream_ptr())
+        dptr(out, out_off), dptr(out_lo, out_off), ldo, L.PAIR[out_dtype or pair], L.ENGINE[engine], L.stream_ptr())
 
 
 def gemm(L, a, b, epi="bias", bias=None, gamma=None, resid=None, engine="simt", pair="tf32"):
