@@ -120,6 +120,15 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
   const float P_SCALE = SCALED ? 1024.0f : 1.0f;
   // S holds (s q).(s k), s = kActScale for fp16 pairs: fold 1/s^2 into the 1/sqrt(64) * log2(e) scale
   const float kScale = 0.125f * 1.4426950408889634f * (SCALED ? 1.0f / (kActScale * kActScale) : 1.0f);
+  // The scaled logit of a live key.  fp16 operands cannot overflow the fp32 sum (|S| < 64 * 65504^2), so an infinite S
+  // means an operand overflowed fp16.  A key whose operand is +-Inf against a query of the opposite sign gives
+  // S = -Inf (single fp16 has no lo term to meet it; the pairs' lo term may have the same sign), and the softmax would
+  // drop that key with p = 0 while every output stays finite.  s * 0 turns such an S into NaN, which reaches the
+  // outputs and the fp16-range guard; for finite s it is a zero of s's sign, so the sum is s * kScale bit for bit.
+  auto logit = [&](float s) {
+    if constexpr (SCALED) return fmaf(s, kScale, s * 0.0f);
+    else return s * kScale;
+  };
 
   const uint32_t q_base = smem_u32(smem) + cw * TILE_BYTES;
   const uint64_t dq_hi = make_desc(q_base), dq_lo = make_desc(q_base + 2 * TILE_BYTES);
@@ -166,8 +175,8 @@ __device__ __forceinline__ void attention_wg_cta(const CUtensorMap* tm_hi, const
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const bool live = key + e < T;
-        p[4 * nt + e] = live ? p[4 * nt + e] * kScale : -INFINITY;
-        p[4 * nt + 2 + e] = live ? p[4 * nt + 2 + e] * kScale : -INFINITY;
+        p[4 * nt + e] = live ? logit(p[4 * nt + e]) : -INFINITY;
+        p[4 * nt + 2 + e] = live ? logit(p[4 * nt + 2 + e]) : -INFINITY;
         mx0 = fmaxf(mx0, p[4 * nt + e]); mx1 = fmaxf(mx1, p[4 * nt + 2 + e]);
       }
     }
