@@ -4,7 +4,8 @@
 //   gem     : m = mean_n x^p (|x|^p with use_abs);  out = sign(m) |m|^(1/p)   (the reference takes the complex
 //             root and restores the sign; with use_abs it is the plain real root)
 // One read of the features (HBM-bound, 4 B per element).  CTA = (128-column slice, image): 8 row groups x 32 lanes
-// x float4 columns, fixed-order shared-memory reduction across the row groups -> deterministic.
+// x float4 columns, fixed-order shared-memory reduction across the row groups -> deterministic.  An image with no
+// valid rows (n_valid[b] <= 0) is written NaN in every mode: torch's mean of an empty set, and max has no value.
 #include "common.cuh"
 
 namespace anyloc {
@@ -69,6 +70,7 @@ pool_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid, in
         const float root = powf(fabsf(m), 1.0f / p);
         r[i] = use_abs ? root : (m > 0.f ? root : (m < 0.f ? -root : (m == 0.f ? 0.f : m)));
       }
+      if (n <= 0) r[i] = __int_as_float(0x7fc00000);
     }
     *reinterpret_cast<float4*>(out + (size_t)b * D + col) = make_float4(r[0], r[1], r[2], r[3]);
   }
@@ -85,6 +87,8 @@ extern "C" int anyloc_pool(const float* feats, const int32_t* n_valid, int B, in
   ANYLOC_REQUIRE(B <= 65535, "pool: B=%d exceeds the grid limit", B);
   ANYLOC_REQUIRE(mode >= POOL_AVG && mode <= POOL_GEM, "pool: unknown mode %d", mode);
   ANYLOC_REQUIRE(mode != POOL_GEM || gem_p != 0.f, "pool: gem_p must be non-zero");
+  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(feats) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+                 "pool: feats and out must be 16-byte aligned (float4 access)");
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   dim3 grid(cdiv(D, 128), B);

@@ -266,6 +266,9 @@ extern "C" int anyloc_preprocess_u8(const uint8_t* img, int B, int H, int W, int
                  "preprocess_u8: crop [%d+%d, %d+%d] outside the %dx%d image", top, Hc, left, Wc, H, W);
   ANYLOC_REQUIRE(Hc <= 65535 && B <= 65535, "preprocess_u8: Hc=%d / B=%d exceed the grid limits", Hc, B);
   ANYLOC_REQUIRE(std3[0] != 0.f && std3[1] != 0.f && std3[2] != 0.f, "preprocess_u8: zero std");
+  // an even Wc keeps every row's pairs at even element offsets, which the kernel stores as float2
+  ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(out) & ((Wc & 1) ? 3 : 7)) == 0,
+                 "preprocess_u8: out must be 4-byte aligned, and 8-byte aligned when Wc is even (float2 stores)");
   if (B == 0) return ANYLOC_OK;
   dim3 grid(cdiv(cdiv(Wc, 2), 256), Hc, B);
   preprocess_u8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(img, H, W, top, left, Hc, Wc, mean3[0], mean3[1], mean3[2],
@@ -286,6 +289,7 @@ extern "C" int anyloc_preprocess_resize_u8(const uint8_t* img, int B, int H, int
                  "preprocess_resize_u8: crop [%d+%d, %d+%d] outside the resized %dx%d image", top, Hc, left, Wc, Hr, Wr);
   ANYLOC_REQUIRE(Hc <= 65535 && B <= 65535, "preprocess_resize_u8: Hc=%d / B=%d exceed the grid limits", Hc, B);
   ANYLOC_REQUIRE(std3[0] != 0.f && std3[1] != 0.f && std3[2] != 0.f, "preprocess_resize_u8: zero std");
+  ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "preprocess_resize_u8: out must be 4-byte aligned");
   const float taps = interpolation ? 4.0f : 2.0f;
   const float sxm = std::max((float)W / Wr, 1.0f), sym = std::max((float)H / Hr, 1.0f);
   ANYLOC_REQUIRE(taps * sxm + 2.0f <= AA_MAX_TAPS && taps * sym + 2.0f <= 1.0e9f,
@@ -313,6 +317,7 @@ extern "C" int anyloc_preprocess_u8_varlen(int n, const uint8_t* const* imgs, co
                      (!resize || (Hr && Wr)),
                  "preprocess_u8_varlen: null pointer");
   ANYLOC_REQUIRE(std3[0] != 0.f && std3[1] != 0.f && std3[2] != 0.f, "preprocess_u8_varlen: zero std");
+  ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "preprocess_u8_varlen: out must be 4-byte aligned");
   for (int i = 0; i < n; ++i) {
     const int hr = resize ? Hr[i] : H[i], wr = resize ? Wr[i] : W[i];
     ANYLOC_REQUIRE(imgs[i], "preprocess_u8_varlen: null pointer (image %d)", i);

@@ -975,9 +975,13 @@ class DinoV2MultiExtractFeatures(_GuardedExtractor):
 
 # ------------------------------------------------------------------ VLAD
 def _as_device_f32(x, device):
+    """x as a contiguous fp32 tensor on `device` whose data_ptr() is 16-byte aligned.  The kernels read rows with float4
+    loads, and a contiguous view at an odd storage offset (`buf[1:].view(B, N, D)`) passes `.contiguous()` unchanged, so
+    such a view is copied; every other tensor is returned as before."""
     if type(x) == np.ndarray:
         x = torch.from_numpy(x)
-    return x.detach().to(device=device, dtype=torch.float32).contiguous()
+    x = x.detach().to(device=device, dtype=torch.float32).contiguous()
+    return x if x.data_ptr() % 16 == 0 else x.clone()
 
 
 def _normalize_rows_dev(x):

@@ -556,7 +556,11 @@ int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream);
  *   ANYLOC_POOL_AVG  torch.mean(ret, dim=1)        scripts/dino_v2_gp.py:130-131
  *   ANYLOC_POOL_MAX  torch.max(ret, dim=1)[0]      scripts/dino_v2_gp.py:132-133
  *   ANYLOC_POOL_GEM  m = mean(x^p) (|x|^p with gem_use_abs); sign(m)|m|^(1/p)   scripts/dino_v2_gem.py:170-189
- * n_valid [B] nullable (ragged batches). */
+ * n_valid [B] nullable (ragged batches): image b pools its first min(N, n_valid[b]) rows and never reads the rest.  An
+ * image with n_valid[b] <= 0 is empty and is written NaN in every mode (torch's mean of an empty set; max has no value
+ * to give).  ANYLOC_ERR_ARG before anything is launched for a null pointer, B outside [0, 65535], N <= 0, D not a
+ * positive multiple of 4, an unknown mode, gem_p = 0 with ANYLOC_POOL_GEM, or feats or out not 16-byte aligned (float4
+ * access).  B = 0 launches nothing. */
 #define ANYLOC_POOL_AVG 0
 #define ANYLOC_POOL_MAX 1
 #define ANYLOC_POOL_GEM 2
@@ -567,14 +571,16 @@ int anyloc_pool(const float* feats, const int32_t* n_valid, int B, int N, int D,
  * Replaces `base_transform` (dvgl_benchmark/datasets_ws.py:20-23: T.ToTensor + T.Normalize) and the centre crop to a
  * multiple of the patch size (scripts/dino_v2_vlad.py:174-176) in one pass:
  *   out[b,c,y,x] = ((float)img[b,top+y,left+x,c] / 255 - mean[c]) / std[c]     (bit-identical to torchvision)
- * img [B,H,W,3] uint8 (device), mean3/std3 HOST arrays of 3 floats, out [B,3,Hc,Wc] fp32 (device). */
+ * img [B,H,W,3] uint8 (device), mean3/std3 HOST arrays of 3 floats, out [B,3,Hc,Wc] fp32 (device).  out must be 4-byte
+ * aligned, and 8-byte aligned when Wc is even (pairs of columns are stored as float2); ANYLOC_ERR_ARG otherwise, before
+ * anything is launched. */
 int anyloc_preprocess_u8(const uint8_t* img, int B, int H, int W, int top, int left, int Hc, int Wc,
                          const float* mean3, const float* std3, float* out, void* stream);
 /* The same with the dataset loader's resize in between (dvgl_benchmark/datasets_ws.py:222-239
  * `T.functional.resize(base_transform(img), [480, 640])`; demo/anyloc_vlad_generate.py:165-177 bicubic down-scaling of
  * over-sized images): ToTensor + Normalize, ANTIALIASED resize to Hr x Wr (interpolation 0 = bilinear, 1 = bicubic --
  * torchvision's tensor defaults, i.e. torch interpolate(align_corners=False, antialias=True)), then the crop window
- * [top, top+Hc) x [left, left+Wc) of the resized image.  out [B,3,Hc,Wc]. */
+ * [top, top+Hc) x [left, left+Wc) of the resized image.  out [B,3,Hc,Wc], 4-byte aligned (else ANYLOC_ERR_ARG). */
 int anyloc_preprocess_resize_u8(const uint8_t* img, int B, int H, int W, int Hr, int Wr, int interpolation, int top,
                                 int left, int Hc, int Wc, const float* mean3, const float* std3, float* out,
                                 void* stream);
@@ -589,8 +595,9 @@ int anyloc_preprocess_resize_u8(const uint8_t* img, int B, int H, int W, int Hr,
  * Its output [3, Hc[i], Wc[i]] fp32 starts at out + out_offset[i] (floats).  imgs, H, W, Hr, Wr, top, left, Hc, Wc,
  * out_offset, mean3 and std3 are HOST arrays.  Up to ANYLOC_PREPROCESS_VARLEN_BATCH images per launch; a longer list
  * takes consecutive launches on the stream.  ANYLOC_ERR_ARG for a null pointer, an unknown interpolation, a crop
- * outside the (resized) image, a zero std, a negative offset, a horizontal down-scaling beyond the 64-tap window or a
- * launch over the grid limit -- all checked before the first launch, so a refusal writes nothing.  Never synchronises
+ * outside the (resized) image, a zero std, a negative offset, an out that is not 4-byte aligned, a horizontal
+ * down-scaling beyond the 64-tap window or a launch over the grid limit -- all checked before the first launch, so a
+ * refusal writes nothing.  Never synchronises
  * with the host.  n = 0 launches nothing. */
 #define ANYLOC_PREPROCESS_VARLEN_BATCH 64
 int anyloc_preprocess_u8_varlen(int n, const uint8_t* const* imgs, const int* H, const int* W, const int* Hr,
