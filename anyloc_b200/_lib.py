@@ -76,6 +76,14 @@ _SIGS = {
                                     [C.c_int] * 7 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_vlad_generate_soft": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_float] +
                                   [C.c_int] * 2 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_vlad_varlen_workspace_bytes": (C.c_size_t, [C.c_int64] + [C.c_int] * 4),
+    "anyloc_vlad_generate_varlen": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                              C.c_void_p, C.c_size_t] + [C.c_int] * 5 +
+                                    [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_vlad_soft_varlen_workspace_bytes": (C.c_size_t, [C.c_int64] + [C.c_int] * 3),
+    "anyloc_vlad_generate_soft_varlen": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,
+                                                   C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int] +
+                                         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_preprocess_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.POINTER(C.c_float)] * 2 +
                              [C.c_void_p, C.c_void_p]),
     "anyloc_preprocess_resize_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 10 + [C.POINTER(C.c_float)] * 2 +
@@ -84,6 +92,8 @@ _SIGS = {
                                     [C.POINTER(C.c_int)] * 4 + [C.POINTER(C.c_float)] * 2 +
                                     [C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "anyloc_pool": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
+    "anyloc_pool_varlen": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                     C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     "anyloc_vlad_residuals": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_void_p]),
     "anyloc_vlad_from_residuals_workspace_bytes": (C.c_size_t, [C.c_int] * 2),
     "anyloc_vlad_from_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 4 +

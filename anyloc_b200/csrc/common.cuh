@@ -185,6 +185,26 @@ struct VarlenAttnTable {
 };
 static_assert(sizeof(VarlenAttnTable) <= 4096, "kernel parameter over 4 KB");
 
+// Where an aggregation kernel finds image b's rows.  A padded batch [B,N,D] keeps image b at rows b*N.., of which the
+// first min(N, n_valid[b]) count (all N without n_valid); a packed list [R,D] keeps it at rows row0[b] .. + len[b]
+// (device arrays, checked on the host by varlen_rows_check).  The kernels take either, so the padded instantiations
+// compile to the code they had before the packed ones existed.
+struct PaddedRows {
+  const int32_t* n_valid; int N;
+  __device__ __forceinline__ size_t first(int b) const { return (size_t)b * N; }
+  __device__ __forceinline__ int count(int b) const { return n_valid ? min(N, n_valid[b]) : N; }
+};
+struct PackedRows {
+  const int64_t* row0; const int32_t* len;
+  __device__ __forceinline__ size_t first(int b) const { return (size_t)row0[b]; }
+  __device__ __forceinline__ int count(int b) const { return len[b]; }
+};
+// The host side of a packed list's table: copies row0 / len [B] from the device (a synchronisation of `st`) and
+// checks that every len >= 0, row0 >= 0, row0 + len <= R and that no two images share a row (an empty image shares
+// none).  -> ANYLOC_OK with the largest len in *max_len, else ANYLOC_ERR_ARG / _CUDA naming `who`.
+int varlen_rows_check(const int64_t* row0, const int32_t* len, int B, int64_t R, cudaStream_t st, const char* who,
+                      int* max_len);
+
 // where the qkv tap kernel writes the q, k and v facet rows of one layer (null: that facet is not tapped)
 struct QkvTapOuts {
   float* out[3];

@@ -212,15 +212,17 @@ vlad_rescore_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_v
 // CTA = (image, 128-column slice); WARPS warps split the rows; lane owns 4 consecutive columns (float4).
 // Per-warp accumulators [K][128] in shared memory (no conflicts: a warp touches 512 contiguous bytes per row),
 // reduced across warps at the end in a fixed order -> deterministic.
-__global__ void __launch_bounds__(256, 2)
-vlad_accumulate2_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
-                        const float* __restrict__ inv_norm, const float* __restrict__ centers,
-                        int N, int D, int K, int norm_descs, int warps, float* __restrict__ vlad,
-                        float* __restrict__ partial_ss /* [B,K,nslices] */) {
+// Image b is rows.count(b) rows from rows.first(b) of x, labels and inv_norm (PaddedRows / PackedRows, common.cuh).
+template <class Rows>
+__device__ __forceinline__ void accumulate2_image(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                                                  const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                                                  Rows rows, int D, int K, int norm_descs, int warps,
+                                                  float* __restrict__ vlad, float* __restrict__ partial_ss) {
   extern __shared__ float sm[];
   float* cen = sm;                                        // [K][128]
   float* acc = sm + (size_t)K * 128;                      // [warps][K][128]
   const int b = blockIdx.y, slice = blockIdx.x, t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int N = rows.count(b);
   const int col = slice * 128 + lane * 4;
   const bool colok = col < D;                             // D % 4 == 0
   for (int i = t; i < K * 32; i += blockDim.x) {
@@ -232,9 +234,9 @@ vlad_accumulate2_kernel(const float* __restrict__ x, const int32_t* __restrict__
   __syncthreads();
   if (w < warps && colok) {
     float* my = acc + (size_t)w * K * 128 + lane * 4;
-    const float* xb = x + (size_t)b * N * D + col;
-    const int32_t* lb = labels + (size_t)b * N;
-    const float* ib = inv_norm + (size_t)b * N;
+    const float* xb = x + rows.first(b) * D + col;
+    const int32_t* lb = labels + rows.first(b);
+    const float* ib = inv_norm + rows.first(b);
     constexpr int U = 16;                                 // rows in flight per warp (latency hiding)
     for (int n0 = w; n0 < N; n0 += U * warps) {
       float4 v[U]; int lab[U]; float sc[U];
@@ -273,6 +275,23 @@ vlad_accumulate2_kernel(const float* __restrict__ x, const int32_t* __restrict__
     ss = warp_sum(ss);
     if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
   }
+}
+
+__global__ void __launch_bounds__(256, 2)
+vlad_accumulate2_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                        const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                        int N, int D, int K, int norm_descs, int warps, float* __restrict__ vlad,
+                        float* __restrict__ partial_ss /* [B,K,nslices] */) {
+  accumulate2_image(x, labels, inv_norm, centers, PaddedRows{nullptr, N}, D, K, norm_descs, warps, vlad, partial_ss);
+}
+
+// packed images: image b is rows [row0[b], row0[b] + len[b]) of x, labels and inv_norm
+__global__ void __launch_bounds__(256, 2)
+vlad_accumulate2_varlen_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                               const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                               const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int D, int K,
+                               int norm_descs, int warps, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  accumulate2_image(x, labels, inv_norm, centers, PackedRows{row0, len}, D, K, norm_descs, warps, vlad, partial_ss);
 }
 
 // ------------------------------------------------------------------ normalisation factors
@@ -545,6 +564,238 @@ vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__
   }
 }
 
+// accumulate3 on packed images: image b is rows [row0[b], row0[b] + len[b]) of x, labels and inv_norm, and N >= every
+// len[b] sizes the shared-memory layout.  A copy of accumulate3 that differs only in where it finds an image's rows
+// (rows.first / rows.count), so the padded kernel keeps its code.  The stable label order, the tasks and their sums
+// depend on the image's rows alone, not on N or on the row chunks of the histogram pass: an image's descriptor is
+// bitwise accumulate3's for the same rows.
+__global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
+vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                               const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                               const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D, int K,
+                               int norm_descs, int intra_norm, float* vlad, float* partial_ss, int32_t* done,
+                               int wait_all) {
+  const PackedRows rows{row0, len};
+  extern __shared__ __align__(16) int sm3[];
+  int* ooff = sm3;                                          // [N] n * D of the rows, sorted by label (stable)
+  int* lab = ooff + N;                                      // [N]
+  float* inv_s = reinterpret_cast<float*>(lab + N);         // [N] 1/|x| in the same sorted order
+  int* start = reinterpret_cast<int*>(inv_s + N);           // [K+1] first sorted position of cluster k
+  int* tstart = start + K + 1;                              // [K+1] first task of cluster k
+  int* sbase = tstart + K + 1;                              // [K+1] first partial-sum slot of a multi-task cluster
+  int* cntw = sbase + K + 1;                                // [ACC3_WARPS][K]
+  float* kss = reinterpret_cast<float*>(cntw + ACC3_WARPS * K);   // [K]
+  float* ksq = kss + K;                                     // [K]
+  int* task_k = reinterpret_cast<int*>(ksq + K);            // [max_tasks]
+  float* inv = reinterpret_cast<float*>(task_k + acc3_max_tasks_dev(N, K));   // [N] 1/|x| in row order (prologue only)
+  float* slots = reinterpret_cast<float*>(sm3) +
+                 (((size_t)4 * N + 3 * (size_t)(K + 1) + (size_t)ACC3_WARPS * K + 2 * (size_t)K + acc3_max_tasks_dev(N, K) + 3) & ~(size_t)3);
+  __shared__ int next_task, s_last;
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  // images in reverse order: the assignment pass streamed them in ascending order, so the last ones are the most
+  // likely to still sit in L2 when this kernel starts
+  const int b = (int)gridDim.y - 1 - (int)blockIdx.y, slice = blockIdx.x, nslices = gridDim.x;
+  const int nr = rows.count(b);
+  const int col = slice * 128 + lane * 4;
+  const bool colok = col < D;                               // D % 4 == 0
+  for (int n = t; n < nr; n += blockDim.x) {
+    lab[n] = labels[rows.first(b) + n];
+    inv[n] = norm_descs ? inv_norm[rows.first(b) + n] : 1.0f;
+  }
+  for (int i = t; i < ACC3_WARPS * K; i += blockDim.x) cntw[i] = 0;
+  if (t == 0) next_task = 0;
+  __syncthreads();
+  // per-warp histograms over contiguous row chunks
+  const int chunk = (((nr + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
+  const int r0 = min(nr, w * chunk), r1 = min(nr, r0 + chunk);
+  for (int n = r0 + lane; n < r1; n += 32) { const int l = lab[n]; if (l >= 0) atomicAdd(&cntw[w * K + l], 1); }
+  __syncthreads();
+  for (int k = t; k < K; k += blockDim.x) {                 // exclusive prefix over the warps, cluster totals
+    int tot = 0;
+    for (int ww = 0; ww < ACC3_WARPS; ++ww) { const int c = cntw[ww * K + k]; cntw[ww * K + k] = tot; tot += c; }
+    start[k] = tot;
+  }
+  __syncthreads();
+  if (w == 0) {                                             // exclusive scans: rows, tasks, partial-sum slots
+    int run_r = 0, run_t = 0, run_s = 0;
+    for (int k0 = 0; k0 < K; k0 += 32) {
+      const int k = k0 + lane;
+      const int c = k < K ? start[k] : 0;
+      const int nt = k < K ? max(1, (c + ACC3_SEG - 1) / ACC3_SEG) : 0;
+      const int ns = nt > 1 ? nt : 0;
+      int ir = c, it = nt, is = ns;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int yr = __shfl_up_sync(0xffffffffu, ir, o), yt = __shfl_up_sync(0xffffffffu, it, o),
+                  ys = __shfl_up_sync(0xffffffffu, is, o);
+        if (lane >= o) { ir += yr; it += yt; is += ys; }
+      }
+      if (k < K) { start[k] = run_r + ir - c; tstart[k] = run_t + it - nt; sbase[k] = run_s + is - ns; }
+      run_r += __shfl_sync(0xffffffffu, ir, 31);
+      run_t += __shfl_sync(0xffffffffu, it, 31);
+      run_s += __shfl_sync(0xffffffffu, is, 31);
+    }
+    if (lane == 0) { start[K] = run_r; tstart[K] = run_t; sbase[K] = run_s; }
+  }
+  __syncthreads();
+  for (int k = t; k < K; k += blockDim.x)                   // task table
+    for (int q = tstart[k]; q < tstart[k + 1]; ++q) task_k[q] = k;
+  for (int n0 = r0; n0 < r1; n0 += 32) {                    // stable placement
+    const int n = n0 + lane;
+    const int l = n < r1 ? lab[n] : -1;
+    const bool active = l >= 0;
+    const float iv = active ? inv[n] : 1.0f;
+    const unsigned am = __ballot_sync(0xffffffffu, active);
+    unsigned peers = 0; int rank = 0;
+    if (active) {
+      peers = __match_any_sync(am, l);
+      rank = __popc(peers & ((1u << lane) - 1u));
+      const int pos = start[l] + cntw[w * K + l] + rank;
+      ooff[pos] = n * D;
+      inv_s[pos] = iv;
+    }
+    __syncwarp();
+    if (active && rank == 0) cntw[w * K + l] += __popc(peers);
+    __syncwarp();
+  }
+  __syncthreads();
+  // tasks -> registers.  Every warp grabs its NEXT task one task early.
+  const float* xb = x + rows.first(b) * D + col;
+  const int ntasks = tstart[K];
+  auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
+  int q = grab();
+  while (q < ntasks) {
+    const int qn = grab();
+    const int k = task_k[q];
+    const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
+    const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
+    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (colok) {
+      // The in-flight bytes live in registers (8 x 16 B per lane = 4 KB per warp; 4 CTAs x 8 warps -> 128 KB per SM),
+      // so the loop is kept lean: row offsets and 1/|x| were laid out in sorted order by the placement pass.
+      constexpr int U = 8;
+      int i = s;
+      for (; i + U <= e; i += U) {
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const float sc = inv_s[i + u];
+          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+        }
+      }
+      if (i < e) {                                           // tail: < U rows, same order
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          if (i + u < e) {
+            const float sc = inv_s[i + u];
+            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+          }
+        }
+      }
+    }
+    if (nt == 1) {
+      if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
+      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+      if (lane == 0) kss[k] = ss;
+    } else {
+      *reinterpret_cast<float4*>(slots + (size_t)(sbase[k] + seg) * 128 + lane * 4) = a;
+    }
+    q = qn;
+  }
+  __syncthreads();
+  for (int k = w; k < K; k += ACC3_WARPS) {                 // clusters of several tasks: combine in task order
+    const int nt = tstart[k + 1] - tstart[k];
+    if (nt <= 1) continue;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int q = 0; q < nt; ++q) {
+      const float4 p = *reinterpret_cast<const float4*>(slots + (size_t)(sbase[k] + q) * 128 + lane * 4);
+      a.x += p.x; a.y += p.y; a.z += p.z; a.w += p.w;
+    }
+    if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
+    const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+    if (lane == 0) kss[k] = ss;
+  }
+  __syncthreads();
+  for (int k = t; k < K; k += blockDim.x) partial_ss[((size_t)b * K + k) * nslices + slice] = kss[k];
+  __syncthreads();
+  if (t == 0) {
+    __threadfence();      // cumulative: orders every write the barrier above made visible to this thread (the pattern of
+                          // cooperative-groups grid sync), instead of 256 per-thread fences
+    s_last = (atomicAdd(&done[b], 1) == nslices - 1);
+  }
+  __syncthreads();
+  if (wait_all) {
+    // Whole grid co-resident (checked on the host): every slice-CTA waits until all slices of its image have published
+    // their sums of squares, derives the SAME scales in the same order, and normalises ITS OWN 128-column slice -- the
+    // normalisation is spread over all CTAs of the image instead of serialising K*D elements behind the last one
+    // (measured tail of the last-CTA variant: 10 us of 41 at c2, 30-40 us of 130 at c5).
+    if (t == 0) {
+      const long long t0 = clock64();
+      for (;;) {
+        int v;
+        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(done + b) : "memory");
+        if (v >= nslices) break;
+        __nanosleep(64);
+        if (clock64() - t0 > 8000000000LL) __trap();      // never hang the GPU
+      }
+    }
+    __syncthreads();
+    const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
+    const int nq = K * 32;                                  // float4 elements of this slice
+    constexpr int UW = 8;
+    for (int i0 = t; i0 < nq; i0 += blockDim.x * UW) {
+      float4 v[UW];
+#pragma unroll
+      for (int u = 0; u < UW; ++u) {
+        const int i = i0 + u * blockDim.x, c4 = slice * 128 + (i & 31) * 4;
+        if (i < nq && c4 < D) v[u] = __ldcg(reinterpret_cast<const float4*>(vlad + ((size_t)b * K + (i >> 5)) * D + c4));
+      }
+#pragma unroll
+      for (int u = 0; u < UW; ++u) {
+        const int i = i0 + u * blockDim.x, c4 = slice * 128 + (i & 31) * 4;
+        if (i < nq && c4 < D) {
+          const float sc = kss[i >> 5];
+          v[u].x = (v[u].x * sc) * g; v[u].y = (v[u].y * sc) * g; v[u].z = (v[u].z * sc) * g; v[u].w = (v[u].w * sc) * g;
+          *reinterpret_cast<float4*>(vlad + ((size_t)b * K + (i >> 5)) * D + c4) = v[u];
+        }
+      }
+    }
+    return;
+  }
+  if (!s_last) return;
+  // ---- last CTA of this image: intra- and global normalisation (same factors as vlad_normalize_kernel)
+  __threadfence();
+  if (t == 0) done[b] = 0;
+  const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
+  float4* vb = reinterpret_cast<float4*>(vlad + (size_t)b * K * D);
+  const int D4 = D >> 2, total4 = K * D4;
+  constexpr int UN = 8;                                     // loads batched ahead of the stores (L2 latency chain)
+  for (int i0 = t; i0 < total4; i0 += blockDim.x * UN) {
+    float4 v[UN];
+#pragma unroll
+    for (int u = 0; u < UN; ++u) {
+      const int i = i0 + u * blockDim.x;
+      if (i < total4) v[u] = __ldcg(vb + i);
+    }
+#pragma unroll
+    for (int u = 0; u < UN; ++u) {
+      const int i = i0 + u * blockDim.x;
+      if (i < total4) {
+        const float sc = kss[i / D4];
+        // two separate multiplications like F.normalize(intra) then F.normalize(global)
+        v[u].x = (v[u].x * sc) * g; v[u].y = (v[u].y * sc) * g; v[u].z = (v[u].z * sc) * g; v[u].w = (v[u].w * sc) * g;
+        vb[i] = v[u];
+      }
+    }
+  }
+}
+
 // columns per slice: every VLAD path cuts D into 128-column slices (one thread per column in the kernels below)
 constexpr int ACC_COLS = 128;
 
@@ -634,20 +885,27 @@ vlad_soft_assign_kernel(const float* __restrict__ x, const int32_t* __restrict__
 // CTA = (128-column slice, image); thread = column; KC cluster accumulators in registers per pass.  Only the image's
 // first n_valid[b] rows are read: a padded row's weight is 0, but 0 * NaN would not be.
 constexpr int SOFT_KC = 32, SOFT_QT = 64;
-__global__ void __launch_bounds__(ACC_COLS)
-vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid,
-                            const float* __restrict__ assign, const float* __restrict__ inv_norm,
-                            const float* __restrict__ centers, int N_per_img, int D, int K, int norm_descs,
-                            float* __restrict__ vlad, float* __restrict__ partial_ss) {
+// the padded soft batch: image b's first min(N, max(0, n_valid[b])) rows of b*N.. (all N without n_valid)
+struct SoftPaddedRows {
+  const int32_t* n_valid; int N;
+  __device__ __forceinline__ size_t first(int b) const { return (size_t)b * N; }
+  __device__ __forceinline__ int count(int b) const { return n_valid ? min(N, max(0, n_valid[b])) : N; }
+};
+template <class Rows>
+__device__ __forceinline__ void soft_accumulate_image(const float* __restrict__ x, Rows rows,
+                                                      const float* __restrict__ assign,
+                                                      const float* __restrict__ inv_norm,
+                                                      const float* __restrict__ centers, int D, int K, int norm_descs,
+                                                      float* __restrict__ vlad, float* __restrict__ partial_ss) {
   __shared__ __align__(16) float a_tile[SOFT_QT][SOFT_KC];
   __shared__ float inv_tile[SOFT_QT];
   __shared__ float red[ACC_COLS / 32][SOFT_KC];
   const int t = threadIdx.x, slice = blockIdx.x, b = blockIdx.y, nslices = gridDim.x;
   const int col = slice * ACC_COLS + t;
   const bool colok = col < D;
-  const int N = n_valid ? min(N_per_img, max(0, n_valid[b])) : N_per_img;
-  const float* xb = x + (size_t)b * N_per_img * D;
-  const float* ab = assign + (size_t)b * N_per_img * K;
+  const int N = rows.count(b);
+  const float* xb = x + rows.first(b) * D;
+  const float* ab = assign + rows.first(b) * K;
   float csum = 0.f;
   if (colok) for (int c = 0; c < K; ++c) csum += __ldg(centers + (size_t)c * D + col);
   for (int k0 = 0; k0 < K; k0 += SOFT_KC) {
@@ -664,7 +922,7 @@ vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restri
         a_tile[q][j] = (q < qn && j < kc) ? __ldg(ab + (size_t)(q0 + q) * K + k0 + j) : 0.f;
       }
       for (int q = t; q < SOFT_QT; q += ACC_COLS)
-        inv_tile[q] = (q < qn) ? (norm_descs ? inv_norm[(size_t)b * N_per_img + q0 + q] : 1.0f) : 0.f;
+        inv_tile[q] = (q < qn) ? (norm_descs ? inv_norm[rows.first(b) + q0 + q] : 1.0f) : 0.f;
       __syncthreads();
       if (t < SOFT_KC) for (int q = 0; q < qn; ++q) wsum += a_tile[q][t];
       if (colok) {
@@ -704,6 +962,24 @@ vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restri
   }
 }
 
+__global__ void __launch_bounds__(ACC_COLS)
+vlad_soft_accumulate_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid,
+                            const float* __restrict__ assign, const float* __restrict__ inv_norm,
+                            const float* __restrict__ centers, int N_per_img, int D, int K, int norm_descs,
+                            float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  soft_accumulate_image(x, SoftPaddedRows{n_valid, N_per_img}, assign, inv_norm, centers, D, K, norm_descs, vlad,
+                        partial_ss);
+}
+
+// packed images: image b is rows [row0[b], row0[b] + len[b]) of x, assign [R,K] and inv_norm
+__global__ void __launch_bounds__(ACC_COLS)
+vlad_soft_accumulate_varlen_kernel(const float* __restrict__ x, const int64_t* __restrict__ row0,
+                                   const int32_t* __restrict__ len, const float* __restrict__ assign,
+                                   const float* __restrict__ inv_norm, const float* __restrict__ centers, int D, int K,
+                                   int norm_descs, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  soft_accumulate_image(x, PackedRows{row0, len}, assign, inv_norm, centers, D, K, norm_descs, vlad, partial_ss);
+}
+
 // ------------------------------------------------------------------ normalise
 __global__ void __launch_bounds__(256)
 vlad_normalize_kernel(float* __restrict__ vlad, const float* __restrict__ partial_ss, int D, int K,
@@ -741,12 +1017,14 @@ struct SortedTables {
   float* slots;      // [B,max_slots,D] partial sums of multi-task clusters
 };
 
-__global__ void __launch_bounds__(ACC3_WARPS * 32)
-vlad_sort_kernel(const int32_t* __restrict__ labels, const float* __restrict__ inv_norm, int N, int D, int K,
-                 int norm_descs, SortedTables tb) {
+// Image b is rows.count(b) <= N rows from rows.first(b) of labels and inv_norm; N sizes the tables.
+template <class Rows>
+__device__ __forceinline__ void sort_image(const int32_t* __restrict__ labels, const float* __restrict__ inv_norm,
+                                           Rows rows, int N, int D, int K, int norm_descs, SortedTables tb) {
   const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int nr = rows.count(b);
   const int maxT = acc3_max_tasks_dev(N, K);
-  const int32_t* lab = labels + (size_t)b * N;
+  const int32_t* lab = labels + rows.first(b);
   int64_t* ooff = tb.ooff + (size_t)b * N;
   float* inv_s = tb.inv_s + (size_t)b * N;
   int* cntw = tb.cntw + (size_t)b * ACC3_WARPS * K;
@@ -756,8 +1034,8 @@ vlad_sort_kernel(const int32_t* __restrict__ labels, const float* __restrict__ i
   int* task_k = tb.task_k + (size_t)b * maxT;
   for (int i = t; i < ACC3_WARPS * K; i += blockDim.x) cntw[i] = 0;
   __syncthreads();
-  const int chunk = (((N + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
-  const int r0 = min(N, w * chunk), r1 = min(N, r0 + chunk);
+  const int chunk = (((nr + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
+  const int r0 = min(nr, w * chunk), r1 = min(nr, r0 + chunk);
   for (int n = r0 + lane; n < r1; n += 32) { const int l = lab[n]; if (l >= 0) atomicAdd(&cntw[w * K + l], 1); }
   __syncthreads();
   for (int k = t; k < K; k += blockDim.x) {
@@ -801,12 +1079,25 @@ vlad_sort_kernel(const int32_t* __restrict__ labels, const float* __restrict__ i
       rank = __popc(peers & ((1u << lane) - 1u));
       const int pos = start[l] + cntw[w * K + l] + rank;
       ooff[pos] = (int64_t)n * D;
-      inv_s[pos] = norm_descs ? inv_norm[(size_t)b * N + n] : 1.0f;
+      inv_s[pos] = norm_descs ? inv_norm[rows.first(b) + n] : 1.0f;
     }
     __syncwarp();
     if (active && rank == 0) cntw[w * K + l] += __popc(peers);
     __syncwarp();
   }
+}
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sort_kernel(const int32_t* __restrict__ labels, const float* __restrict__ inv_norm, int N, int D, int K,
+                 int norm_descs, SortedTables tb) {
+  sort_image(labels, inv_norm, PaddedRows{nullptr, N}, N, D, K, norm_descs, tb);
+}
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sort_varlen_kernel(const int32_t* __restrict__ labels, const float* __restrict__ inv_norm,
+                        const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D, int K,
+                        int norm_descs, SortedTables tb) {
+  sort_image(labels, inv_norm, PackedRows{row0, len}, N, D, K, norm_descs, tb);
 }
 
 // CTA = (128-column slice, image, range of SORTED_TASKS_PER_CTA tasks); warps grab the range's tasks dynamically.  A
@@ -831,6 +1122,75 @@ vlad_sorted_accumulate_kernel(const float* __restrict__ x, const float* __restri
   const int col = slice * 128 + lane * 4;
   const bool colok = col < D;
   const float* xb = x + (size_t)b * N * D + col;
+  auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
+  int q = grab();
+  while (q < q1) {
+    const int qn = grab();
+    const int k = task_k[q];
+    const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
+    const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
+    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (colok) {
+      constexpr int U = 8;
+      int i = s;
+      for (; i + U <= e; i += U) {
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const float sc = inv_s[i + u];
+          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+        }
+      }
+      if (i < e) {
+        float4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          if (i + u < e) {
+            const float sc = inv_s[i + u];
+            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
+          }
+        }
+      }
+    }
+    if (nt == 1) {
+      if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
+      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+      if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
+    } else if (colok) {
+      *reinterpret_cast<float4*>(tb.slots + ((size_t)b * maxS + sbase[k] + seg) * D + col) = a;
+    }
+    q = qn;
+  }
+}
+
+// The same on packed images (image b's rows start at row0[b] of x; N sizes the tables): a copy that differs only in
+// the image's first row, so the padded kernel keeps its code.
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sorted_accumulate_varlen_kernel(const float* __restrict__ x, const float* __restrict__ centers,
+                                     const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D,
+                                     int K, SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  const PackedRows rows{row0, len};
+  __shared__ int next_task;
+  const int b = blockIdx.y, slice = blockIdx.x, nslices = gridDim.x, lane = threadIdx.x & 31;
+  const int maxT = acc3_max_tasks_dev(N, K), maxS = 2 * (N / ACC3_SEG) + 2;
+  const int* start = tb.start + (size_t)b * (K + 1);
+  const int* tstart = tb.tstart + (size_t)b * (K + 1);
+  const int* sbase = tb.sbase + (size_t)b * (K + 1);
+  const int* task_k = tb.task_k + (size_t)b * maxT;
+  const int64_t* ooff = tb.ooff + (size_t)b * N;
+  const float* inv_s = tb.inv_s + (size_t)b * N;
+  const int q0 = blockIdx.z * SORTED_TASKS_PER_CTA, q1 = min(tstart[K], q0 + SORTED_TASKS_PER_CTA);
+  if (q0 >= q1) return;
+  if (threadIdx.x == 0) next_task = q0;
+  __syncthreads();
+  const int col = slice * 128 + lane * 4;
+  const bool colok = col < D;
+  const float* xb = x + rows.first(b) * D + col;
   auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
   int q = grab();
   while (q < q1) {
@@ -1020,7 +1380,7 @@ struct AssignBufs {
 // FFMA kernel
 int launch_assign(const float* feats, const int32_t* n_valid, int N_per_img, int64_t R, int D, int K,
                   const float* centers, int dist_mode, const AssignBufs& ab, int32_t* labels, float* inv_norm,
-                  cudaStream_t st, bool prepared = false) {
+                  cudaStream_t st, bool prepared = false, int64_t R_route = -1) {
   if (prepared) {    // c^, tf32 copy, bias and norms already sit in ab (anyloc_vlad_prepare); only the tickets need zeroing
     if (ab.done) ANYLOC_CHECK_CUDA(cudaMemsetAsync(ab.done, 0, (size_t)ab.n_done * sizeof(int32_t), st));
   } else {
@@ -1029,7 +1389,8 @@ int launch_assign(const float* feats, const int32_t* n_valid, int N_per_img, int
     ANYLOC_CHECK_LAUNCH();
   }
   EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, K};
-  const bool fast = ab.coarse != nullptr && D <= 2048 && R >= 256 && R < (1ll << 31) &&
+  // R_route: the rows of the padded batch a packed list stands for, so both take the same kernels
+  const bool fast = ab.coarse != nullptr && D <= 2048 && (R_route < 0 ? R : R_route) >= 256 && R < (1ll << 31) &&
                     gemm_tc_supported(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, ANYLOC_PAIR_TF32);
   if (fast) {
     int rc = gemm_tc_launch(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K, D, ep, ANYLOC_PAIR_TF32, st);
@@ -1069,11 +1430,11 @@ bool take_assign_bufs(Workspace& w, int64_t R, int D, int K, AssignBufs* ab) {
 // The hard path's workspace: labels, 1/|x|, per-slice sums of squares, the assignment buffers and, with `tickets`,
 // the accumulate3 tickets.  It is a superset of the soft path's carve (1/|x|, sums of squares, c^ and the [R,K]
 // assignment in the coarse scores' place) and of anyloc_vlad_assign's, so anyloc_vlad_workspace_bytes sizes all
-// three.  With ws == nullptr it is a dry run; returns the bytes taken, 0 when the workspace is too small.
+// three.  R rows of features (B * N padded), B images.  With ws == nullptr it is a dry run; returns the bytes taken,
+// 0 when the workspace is too small.
 struct HardBufs { int32_t* labels; float *inv_norm, *partial; AssignBufs ab; };
-size_t carve_hard(void* ws, size_t ws_bytes, int B, int N, int D, int K, bool tickets, HardBufs* hb) {
+size_t carve_hard(void* ws, size_t ws_bytes, size_t R, int B, int D, int K, bool tickets, HardBufs* hb) {
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
-  const size_t R = (size_t)B * N;
   hb->labels = w.take<int32_t>(R);
   hb->inv_norm = w.take<float>(R);
   hb->partial = w.take<float>((size_t)B * K * cdiv(D, ACC_COLS));
@@ -1094,7 +1455,7 @@ int launch_normalize(float* vlad, const float* partial, int B, int D, int K, int
 
 extern "C" size_t anyloc_vlad_workspace_bytes(int B, int N, int D, int K) {
   HardBufs hb;
-  return carve_hard(nullptr, 0, B, N, D, K, true, &hb);
+  return carve_hard(nullptr, 0, (size_t)B * N, B, D, K, true, &hb);
 }
 
 extern "C" int anyloc_vlad_assign(const float* feats, const float* centers, int R, int D, int K,
@@ -1171,7 +1532,7 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   const size_t smem3 = acc3_smem_bytes(N, K);
   const bool fits3 = vlad_route(N, D, K) == ANYLOC_VLAD_ROUTE_ACC3;
   HardBufs hb;
-  if (!carve_hard(ws, ws_bytes, B, N, D, K, fits3, &hb)) {
+  if (!carve_hard(ws, ws_bytes, R, B, D, K, fits3, &hb)) {
     set_error("vlad_generate: workspace too small (%zu bytes given)", ws_bytes);
     return ANYLOC_ERR_WORKSPACE;
   }
@@ -1239,10 +1600,11 @@ extern "C" int anyloc_vlad_generate_route(int B, int N, int D, int K) {
   return vlad_route(N, D, K);
 }
 
-// The sorted route's workspace: carve_hard's buffers without the tickets, then the per-image tables.  With
-// ws == nullptr a dry run; returns the bytes taken, 0 when the workspace is too small.
-static size_t carve_sorted(void* ws, size_t ws_bytes, int B, int N, int D, int K, HardBufs* hb, SortedTables* tb) {
-  const size_t off = carve_hard(ws, ws_bytes, B, N, D, K, false, hb);
+// The sorted route's workspace: carve_hard's buffers for R feature rows without the tickets, then the per-image tables
+// of B images of up to N rows.  With ws == nullptr a dry run; returns the bytes taken, 0 when the workspace is too small.
+static size_t carve_sorted(void* ws, size_t ws_bytes, size_t R_feats, int B, int N, int D, int K, HardBufs* hb,
+                           SortedTables* tb) {
+  const size_t off = carve_hard(ws, ws_bytes, R_feats, B, D, K, false, hb);
   if (!off) return 0;
   Workspace w(ws ? (void*)((char*)ws + off) : (void*)256, ws ? ws_bytes - off : (size_t)-1 / 2);
   const size_t R = (size_t)B * N, K1 = (size_t)B * (K + 1);
@@ -1261,7 +1623,7 @@ static size_t carve_sorted(void* ws, size_t ws_bytes, int B, int N, int D, int K
 extern "C" size_t anyloc_vlad_sorted_workspace_bytes(int B, int N, int D, int K) {
   HardBufs hb;
   SortedTables tb;
-  return carve_sorted(nullptr, 0, B, N, D, K, &hb, &tb);
+  return carve_sorted(nullptr, 0, (size_t)B * N, B, N, D, K, &hb, &tb);
 }
 
 extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_valid, const float* centers,
@@ -1280,7 +1642,7 @@ extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
   HardBufs hb;
   SortedTables tb;
-  if (!carve_sorted(ws, ws_bytes, B, N, D, K, &hb, &tb)) {
+  if (!carve_sorted(ws, ws_bytes, (size_t)B * N, B, N, D, K, &hb, &tb)) {
     set_error("vlad_generate_sorted: workspace too small (%zu bytes given, %zu needed)", ws_bytes,
               anyloc_vlad_sorted_workspace_bytes(B, N, D, K));
     return ANYLOC_ERR_WORKSPACE;
@@ -1372,6 +1734,196 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   if (assign_out)
     ANYLOC_CHECK_CUDA(cudaMemcpyAsync(assign_out, assign, R * K * 4, cudaMemcpyDeviceToDevice, st));
   return ANYLOC_OK;
+}
+
+// ====================================================================================================================
+// Packed lists (anyloc_vlad_generate_varlen / _soft_varlen): image b is rows [row0[b], row0[b] + len[b]) of feats
+// [R,D].  The per-row passes (assignment, 1/|x|) run over all R rows with the padded path's kernels; the accumulations
+// take the *_varlen instantiations, which find an image's rows through the table and otherwise run the padded
+// kernels' code at the padded shape (N = the longest len), so each descriptor is bitwise the padded call's.
+// ====================================================================================================================
+namespace anyloc {
+// dst rows of image b = src rows of image b (width 32-bit words per row); CTA per image.  The per-row outputs
+// (labels, soft assignment) of the rows that belong to an image; the caller has filled the others.
+__global__ void __launch_bounds__(256)
+varlen_copy_rows_kernel(const uint32_t* __restrict__ src, const int64_t* __restrict__ row0,
+                        const int32_t* __restrict__ len, int width, uint32_t* __restrict__ dst) {
+  const int b = blockIdx.x;
+  const size_t off = (size_t)row0[b] * width, n = (size_t)len[b] * width;
+  for (size_t i = threadIdx.x; i < n; i += blockDim.x) dst[off + i] = src[off + i];
+}
+}  // namespace anyloc
+
+namespace {
+// the refusals every packed entry shares, before anything is read or launched
+int varlen_args(const char* who, const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B,
+                int D, int K, const float* vlad) {
+  ANYLOC_REQUIRE(B >= 0 && B <= 65535 && R >= 0 && R < (1ll << 31) && D > 0 && K > 0 && D % 4 == 0,
+                 "%s: bad dims B=%d R=%lld D=%d K=%d (B <= 65535, R < 2^31, D a multiple of 4)", who, B, (long long)R,
+                 D, K);
+  ANYLOC_REQUIRE(feats && row0 && len && vlad, "%s: null pointer", who);
+  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(feats) | reinterpret_cast<uintptr_t>(vlad)) & 15) == 0 &&
+                     (reinterpret_cast<uintptr_t>(row0) & 7) == 0 && (reinterpret_cast<uintptr_t>(len) & 3) == 0,
+                 "%s: feats and vlad must be 16-byte aligned (float4 access), row0 8-byte and len 4-byte", who);
+  return ANYLOC_OK;
+}
+
+// labels_out / assign_out [R, width]: fill (every byte `fill`), then each image's rows from the workspace copy
+int varlen_rows_out(const void* src, const int64_t* row0, const int32_t* len, int B, int64_t R, int width, int fill,
+                    void* dst, cudaStream_t st) {
+  ANYLOC_CHECK_CUDA(cudaMemsetAsync(dst, fill, (size_t)R * width * 4, st));
+  if (!src) return ANYLOC_OK;
+  varlen_copy_rows_kernel<<<B, 256, 0, st>>>((const uint32_t*)src, row0, len, width, (uint32_t*)dst);
+  ANYLOC_CHECK_LAUNCH();
+  return ANYLOC_OK;
+}
+}  // namespace
+
+extern "C" size_t anyloc_vlad_varlen_workspace_bytes(int64_t R, int B, int max_len, int D, int K) {
+  HardBufs hb;
+  SortedTables tb;
+  if (vlad_route(max_len, D, K) == ANYLOC_VLAD_ROUTE_SORTED)
+    return carve_sorted(nullptr, 0, (size_t)R, B, max_len, D, K, &hb, &tb);
+  return carve_hard(nullptr, 0, (size_t)R, B, D, K, true, &hb);
+}
+
+extern "C" int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len,
+                                           int B, const float* centers, void* prepared, size_t prepared_bytes, int D,
+                                           int K, int dist_mode, int norm_descs, int intra_norm, float* vlad,
+                                           int32_t* labels_out, void* ws, size_t ws_bytes, void* stream) {
+  int rc = varlen_args("vlad_generate_varlen", feats, R, row0, len, B, D, K, vlad);
+  if (rc) return rc;
+  ANYLOC_REQUIRE(centers && ws, "vlad_generate_varlen: null pointer");
+  ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
+                 "vlad_generate_varlen: unknown dist_mode %d", dist_mode);
+  if (B == 0) return ANYLOC_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int N = 0;                                        // the padded batch's row count: the longest image
+  rc = varlen_rows_check(row0, len, B, R, st, "vlad_generate_varlen", &N);
+  if (rc) return rc;
+  const int route = vlad_route(N, D, K);
+  const int nslices = cdiv(D, ACC_COLS);
+  const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
+  ANYLOC_REQUIRE(route != ANYLOC_VLAD_ROUTE_SORTED || ztasks <= 65535,
+                 "vlad_generate_varlen: N=%d K=%d exceed the launch grid", N, K);
+  HardBufs hb;
+  SortedTables tb;
+  const size_t got = route == ANYLOC_VLAD_ROUTE_SORTED
+                         ? carve_sorted(ws, ws_bytes, (size_t)R, B, N, D, K, &hb, &tb)
+                         : carve_hard(ws, ws_bytes, (size_t)R, B, D, K, route == ANYLOC_VLAD_ROUTE_ACC3, &hb);
+  if (!got || (route == ANYLOC_VLAD_ROUTE_ACC3 && !hb.ab.done)) {
+    set_error("vlad_generate_varlen: workspace too small (%zu bytes given, %zu needed)", ws_bytes,
+              anyloc_vlad_varlen_workspace_bytes(R, B, N, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  if (N == 0) {                                     // every image empty: zero descriptors, like the padded call
+    ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st));
+    return labels_out ? varlen_rows_out(nullptr, row0, len, B, R, 1, 0xff, labels_out, st) : ANYLOC_OK;
+  }
+  AssignBufs& ab = hb.ab;
+  PreparedView pv;
+  const bool use_prep = prepared && carve_prepared(prepared, prepared_bytes, D, K, &pv);
+  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)B * K * D + (double)K * D));
+  rc = launch_assign(feats, nullptr, 0, R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep,
+                     (int64_t)B * N);
+  if (rc) return rc;
+  if (route == ANYLOC_VLAD_ROUTE_ACC3) {
+    const size_t smem3 = acc3_smem_bytes(N, K);
+    static unsigned long long attr_seen = 0;
+    if (first_use_on_this_device(&attr_seen)) {
+      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             100 * 1024));
+    }
+    int occ = 0;
+    ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_varlen_kernel,
+                                                                    ACC3_WARPS * 32, smem3));
+    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
+    vlad_accumulate3_varlen_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
+        feats, hb.labels, hb.inv_norm, centers, row0, len, N, D, K, norm_descs, intra_norm, vlad, hb.partial, ab.done,
+        wait_all);
+    ANYLOC_CHECK_LAUNCH();
+  } else if (route == ANYLOC_VLAD_ROUTE_ACC2) {
+    const int warps = acc2_warps(K);
+    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)smem));
+    vlad_accumulate2_varlen_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, hb.labels, hb.inv_norm, centers, row0,
+                                                                        len, D, K, norm_descs, warps, vlad, hb.partial);
+    ANYLOC_CHECK_LAUNCH();
+    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
+    if (rc) return rc;
+  } else {
+    vlad_sort_varlen_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, row0, len, N, D, K, norm_descs, tb);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_accumulate_varlen_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(
+        feats, centers, row0, len, N, D, K, tb, vlad, hb.partial);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, hb.partial);
+    ANYLOC_CHECK_LAUNCH();
+    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
+    if (rc) return rc;
+  }
+  return labels_out ? varlen_rows_out(hb.labels, row0, len, B, R, 1, 0xff, labels_out, st) : ANYLOC_OK;
+}
+
+// inv_norm [R] | partial [B,K,nslices] | c^ [K,D] | assign [R,K]: anyloc_vlad_generate_soft's carve for R packed rows
+static size_t carve_soft_varlen(void* ws, size_t ws_bytes, int64_t R, int B, int D, int K, float** inv_norm,
+                                float** partial, float** chat, float** assign) {
+  Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  *inv_norm = w.take<float>((size_t)R);
+  *partial = w.take<float>((size_t)B * K * cdiv(D, ACC_COLS));
+  *chat = w.take<float>((size_t)K * D);
+  *assign = w.take<float>((size_t)R * K);
+  return *inv_norm && *partial && *chat && *assign ? w.off : 0;
+}
+
+extern "C" size_t anyloc_vlad_soft_varlen_workspace_bytes(int64_t R, int B, int D, int K) {
+  float *a, *b, *c, *d;
+  return carve_soft_varlen(nullptr, 0, R, B, D, K, &a, &b, &c, &d);
+}
+
+extern "C" int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len,
+                                                int B, const float* centers, int D, int K, float soft_temp,
+                                                int norm_descs, int intra_norm, float* vlad, float* assign_out,
+                                                void* ws, size_t ws_bytes, void* stream) {
+  int rc = varlen_args("vlad_generate_soft_varlen", feats, R, row0, len, B, D, K, vlad);
+  if (rc) return rc;
+  ANYLOC_REQUIRE(centers && ws, "vlad_generate_soft_varlen: null pointer");
+  ANYLOC_REQUIRE(K <= 2048, "vlad_generate_soft_varlen: K=%d > 2048", K);
+  if (B == 0) return ANYLOC_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int N = 0;
+  rc = varlen_rows_check(row0, len, B, R, st, "vlad_generate_soft_varlen", &N);
+  if (rc) return rc;
+  float *inv_norm, *partial, *chat, *assign;
+  if (!carve_soft_varlen(ws, ws_bytes, R, B, D, K, &inv_norm, &partial, &chat, &assign)) {
+    set_error("vlad_generate_soft_varlen: workspace too small (%zu bytes given, %zu needed)", ws_bytes,
+              anyloc_vlad_soft_varlen_workspace_bytes(R, B, D, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  if (N == 0) {
+    ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st));
+    return assign_out ? varlen_rows_out(nullptr, row0, len, B, R, K, 0, assign_out, st) : ANYLOC_OK;
+  }
+  const int nslices = cdiv(D, ACC_COLS);
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)B * K * D + (double)K * D));
+  vlad_soft_centre_prep_kernel<<<K, 256, 0, st>>>(centers, K, D, chat);
+  ANYLOC_CHECK_LAUNCH();
+  constexpr int ROWS = 2;
+  const size_t smem = (size_t)8 * ROWS * K * 4;
+  ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_soft_assign_kernel<ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+  int blocks = (int)std::min<int64_t>(((int64_t)(R + ROWS - 1) / ROWS + 7) / 8, (int64_t)device_sm_count() * 8);
+  vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, nullptr, 0, R, D, K, chat, soft_temp,
+                                                                       assign, inv_norm);
+  ANYLOC_CHECK_LAUNCH();
+  vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm, centers,
+                                                                           D, K, norm_descs, vlad, partial);
+  ANYLOC_CHECK_LAUNCH();
+  rc = launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  if (rc) return rc;
+  return assign_out ? varlen_rows_out(assign, row0, len, B, R, K, 0, assign_out, st) : ANYLOC_OK;
 }
 
 // The fixed row partition of the k-means update: at most 64 contiguous chunks, enough (column slice, chunk) CTAs to

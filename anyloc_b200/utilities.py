@@ -984,6 +984,53 @@ def _as_device_f32(x, device):
     return x if x.data_ptr() % 16 == 0 else x.clone()
 
 
+def _packed_rows(items):
+    """The [R, D] view of one buffer whose consecutive row ranges the items are, or None.  `ext(list)` and
+    `DinoV2MultiExtractFeatures(list)` return such views of their packed output, and the packed aggregations read them
+    in place.  Every item must be a 2-D fp32 tensor with unit column stride and rows D apart, on the storage of the
+    first one, starting where the previous item ends; the first row must be 16-byte aligned (float4 loads)."""
+    if not items or not all(isinstance(q, torch.Tensor) for q in items):
+        return None
+    first = items[0]
+    if first.dim() != 2 or first.dtype != torch.float32:
+        return None
+    D = first.shape[1]
+    storage, off = first.untyped_storage().data_ptr(), first.storage_offset()
+    for q in items:
+        if (q.dim() != 2 or q.dtype != torch.float32 or q.device != first.device or q.shape[1] != D
+                or q.untyped_storage().data_ptr() != storage or q.storage_offset() != off):
+            return None
+        if q.shape[0] > 0 and (q.stride(1) != 1 and D > 1 or q.stride(0) != D and q.shape[0] > 1):
+            return None
+        off += q.shape[0] * D
+    if first.data_ptr() % 16:
+        return None
+    R = sum(q.shape[0] for q in items)
+    return first.detach().as_strided((R, D), (D, 1), first.storage_offset())
+
+
+def _pack_list(items, device):
+    """A list of [n_i, D] feature sets -> (feats [R, D] contiguous fp32 on `device`, row0, lens): image i is rows
+    row0[i] .. row0[i] + lens[i] of feats.  Consecutive views of one buffer on `device` (_packed_rows) are passed as
+    that buffer, without a copy; anything else is packed once with one torch.cat (host items through
+    _as_device_f32)."""
+    lens = [int(q.shape[0]) for q in items]
+    row0 = [0] * len(items)
+    for i in range(1, len(items)):
+        row0[i] = row0[i - 1] + lens[i - 1]
+    feats = _packed_rows(items)
+    if feats is None or feats.device != torch.device(device):
+        feats = torch.cat([_as_device_f32(q, device) for q in items])
+        feats = feats if feats.data_ptr() % 16 == 0 else feats.clone()
+    return feats, row0, lens
+
+
+def _table_dev(row0, lens, dev):
+    """row0 [B] int64 and len [B] int32 on `dev` (the packed entries' table)"""
+    return (torch.tensor(row0, dtype=torch.int64).to(dev, non_blocking=True),
+            torch.tensor(lens, dtype=torch.int32).to(dev, non_blocking=True))
+
+
 def _normalize_rows_dev(x):
     """F.normalize(x) of a device matrix [R,D] (utilities.py:782-783)."""
     y = torch.empty_like(x)
@@ -1530,6 +1577,40 @@ class VLAD:
         _lib.check(rc, name)
         return out, labels
 
+    def _run_varlen(self, feats, row0, lens, dev, want_labels=False):
+        """feats [R,D] device fp32 holding image i at rows row0[i] .. + lens[i] -> ([B,K*D], labels [R] | None); each
+        descriptor is bitwise _run's on the padded batch [B, max(lens), D] with n_valid = lens (soft mode: the [R,K]
+        assignment in place of the labels).  One launch sequence whatever B is, and no padded copy."""
+        assert self.kmeans is not None
+        assert self.c_centers is not None
+        lib = _lib.load()
+        R, D = feats.shape
+        B, K = len(lens), self.num_clusters
+        centers = self._centers_on(dev)
+        if centers.shape != (K, D):
+            raise ValueError(f"cluster centres {tuple(centers.shape)} do not match K={K}, D={D}")
+        out = torch.empty(B, K * D, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            r0, ln = _table_dev(row0, lens, dev)
+            if self.vlad_mode == "soft":
+                assign = torch.empty(R, K, device=dev, dtype=torch.float32) if want_labels else None
+                ws = _lib.workspaces.get(dev, lib.anyloc_vlad_soft_varlen_workspace_bytes(R, B, D, K), "vlad")
+                rc = lib.anyloc_vlad_generate_soft_varlen(
+                    _lib.ptr(feats), R, _lib.ptr(r0), _lib.ptr(ln), B, _lib.ptr(centers), D, K, float(self.soft_temp),
+                    int(bool(self.norm_descs)), int(bool(self.intra_norm)), _lib.ptr(out), _lib.ptr(assign),
+                    _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
+                _lib.check(rc, "anyloc_vlad_generate_soft_varlen")
+                return out, assign
+            labels = torch.empty(R, device=dev, dtype=torch.int32) if want_labels else None
+            ws = _lib.workspaces.get(dev, lib.anyloc_vlad_varlen_workspace_bytes(R, B, max(lens), D, K), "vlad")
+            prep = self._prepared_on(dev, centers)
+            rc = lib.anyloc_vlad_generate_varlen(
+                _lib.ptr(feats), R, _lib.ptr(r0), _lib.ptr(ln), B, _lib.ptr(centers), _lib.ptr(prep), prep.numel(), D, K,
+                _lib.DIST[self.mode], int(bool(self.norm_descs)), int(bool(self.intra_norm)), _lib.ptr(out),
+                _lib.ptr(labels), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
+        _lib.check(rc, "anyloc_vlad_generate_varlen")
+        return out, labels
+
     # -- per-image cache (utilities.py:843-852 labels, :864-878 soft assignment, :951-970 residuals)
     def _cache_path(self, cache_id, suffix):
         return f"{self.cache_dir}/{cache_id}_{suffix}.pt"
@@ -1634,14 +1715,9 @@ class VLAD:
                 return torch.stack([])      # same failure as the reference on an empty list
             on_dev = all(isinstance(q, torch.Tensor) and q.is_cuda for q in multi_query)
             dev = _lib.require_cuda(multi_query[0].device if on_dev else None)
-            qs = [_as_device_f32(q, dev) for q in multi_query]
-            n_max = max(q.shape[0] for q in qs)
-            D = qs[0].shape[1]
-            feats = torch.zeros(len(qs), n_max, D, device=dev, dtype=torch.float32)
-            for i, q in enumerate(qs):
-                feats[i, :q.shape[0]] = q
-            n_valid = torch.tensor([q.shape[0] for q in qs], dtype=torch.int32, device=dev)
-            out, _ = self._run(feats, n_valid, dev)
+            # packed: the items' rows in one [R, D] buffer (ext(list)'s own, when the items are its views)
+            feats, row0, lens = _pack_list(multi_query, dev)
+            out, _ = self._run_varlen(feats, row0, lens, dev)
             return out if on_dev else out.cpu()
         was_np = type(multi_query) == np.ndarray
         on_dev = isinstance(multi_query, torch.Tensor) and multi_query.is_cuda
@@ -1690,13 +1766,20 @@ class VLAD:
 _POOL = {"average": 0, "avg": 0, "mean": 0, "max": 1, "gem": 2}
 
 
-def pool_descriptors(patch_descs: torch.Tensor, method: str = "gem", gem_p: float = 3.0,
+def pool_descriptors(patch_descs: Union[torch.Tensor, list], method: str = "gem", gem_p: float = 3.0,
                      gem_use_abs: bool = False) -> torch.Tensor:
     """Global descriptors [N, d_dim] from patch features [N, n_p, d_dim] the way the reference's other DINOv2
     scripts pool them: `get_gem_descriptors` (scripts/dino_v2_gem.py:170-189; `gem_p`, `gem_use_abs`) and the
-    "average" / "max" pooling of scripts/dino_v2_gp.py:130-135.  CPU in -> CPU out, CUDA in -> CUDA out."""
+    "average" / "max" pooling of scripts/dino_v2_gp.py:130-135.  CPU in -> CPU out, CUDA in -> CUDA out.
+
+    A list (or tuple) of [n_i, d_dim] feature sets of differently sized images, such as ext(list) returns, gives
+    [len(list), d_dim] from one launch: the items are read where they lie when they are consecutive views of one
+    buffer (ext(list)'s), else packed once.  Row i is bitwise what the [N, n_p, d_dim] call gives for item i zero-padded
+    to the longest item; an empty item gives NaN.  CUDA out when every item is a CUDA tensor, else CPU out."""
     if method not in _POOL:
         raise NotImplementedError(f"ID: {method}")          # scripts/dino_v2_gp.py:134-135
+    if isinstance(patch_descs, (list, tuple)):
+        return _pool_list(list(patch_descs), method, gem_p, gem_use_abs)
     assert len(patch_descs.shape) == len(("N", "n_p", "d_dim"))
     on_dev = patch_descs.is_cuda
     dev = _lib.require_cuda(patch_descs.device if on_dev else None)
@@ -1706,6 +1789,22 @@ def pool_descriptors(patch_descs: torch.Tensor, method: str = "gem", gem_p: floa
     with torch.cuda.device(dev):
         _lib.check(_lib.load().anyloc_pool(_lib.ptr(x), None, B, N, D, _POOL[method], float(gem_p),
                                            int(bool(gem_use_abs)), _lib.ptr(out), _lib.stream_ptr()), "anyloc_pool")
+    return out if on_dev else out.cpu()
+
+
+def _pool_list(items, method, gem_p, gem_use_abs):
+    if not items:
+        raise ValueError("pool_descriptors: an empty list has no feature dimension")
+    on_dev = all(isinstance(q, torch.Tensor) and q.is_cuda for q in items)
+    dev = _lib.require_cuda(items[0].device if on_dev else None)
+    feats, row0, lens = _pack_list(items, dev)
+    R, D = feats.shape
+    out = torch.empty(len(items), D, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        r0, ln = _table_dev(row0, lens, dev)
+        _lib.check(_lib.load().anyloc_pool_varlen(_lib.ptr(feats), R, _lib.ptr(r0), _lib.ptr(ln), len(items), D,
+                                                  _POOL[method], float(gem_p), int(bool(gem_use_abs)), _lib.ptr(out),
+                                                  _lib.stream_ptr()), "anyloc_pool_varlen")
     return out if on_dev else out.cpu()
 
 

@@ -156,6 +156,29 @@ int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_valid, cons
 int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_valid, const float* centers,
                               int B, int N, int D, int K, float soft_temp, int norm_descs, int intra_norm,
                               float* vlad, float* assign, void* ws, size_t ws_bytes, void* stream);
+/* Packed lists (VLAD.generate_multi of a list, whose items ext(list) returns as consecutive views of one buffer):
+ * feats [R,D] fp32 rows, image b = rows [row0[b], row0[b] + len[b]) with row0 [B] int64 and len [B] int32 DEVICE
+ * arrays, so one call serves any number of images without padding them to a common length.  Images may sit in any
+ * order with rows between them that belong to none; len = 0 is allowed (a zero descriptor, as for an empty padded
+ * image).  The call copies the table to the host (a synchronisation of `stream`) and returns ANYLOC_ERR_ARG, with
+ * nothing launched, for len < 0, row0 < 0, row0 + len > R, two images sharing a row, B outside [0, 65535], R >= 2^31,
+ * D not a multiple of 4, a null pointer, or feats / vlad not 16-byte, row0 not 8-byte or len not 4-byte aligned.
+ * anyloc_vlad_generate_varlen takes the accumulation anyloc_vlad_generate_route(B, max len, D, K) names -- the route
+ * of the padded batch [B, max len, D] -- and the descriptor of every image is bitwise the padded call's
+ * (anyloc_vlad_generate_prepared / _sorted with n_valid = len); prepared is optional (NULL: centre prep per call).
+ * labels [R] int32 (nullable): the padded call's label of each image row, -1 for rows of no image.  The soft form's
+ * assign [R,K] (nullable) likewise: each image row's probabilities, 0 for rows of no image.  Workspaces:
+ * anyloc_vlad_varlen_workspace_bytes(R, B, max len, D, K) and anyloc_vlad_soft_varlen_workspace_bytes(R, B, D, K). */
+size_t anyloc_vlad_varlen_workspace_bytes(int64_t R, int B, int max_len, int D, int K);
+int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B,
+                                const float* centers, void* prepared, size_t prepared_bytes, int D, int K, int dist_mode,
+                                int norm_descs, int intra_norm, float* vlad, int32_t* labels, void* ws, size_t ws_bytes,
+                                void* stream);
+size_t anyloc_vlad_soft_varlen_workspace_bytes(int64_t R, int B, int D, int K);
+int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B,
+                                     const float* centers, int D, int K, float soft_temp, int norm_descs,
+                                     int intra_norm, float* vlad, float* assign, void* ws, size_t ws_bytes,
+                                     void* stream);
 /* Residual tensor of VLAD.generate_res_vec (utilities.py:928-972): out[q,k,:] = x^_q - c_k for ALL (patch, centre)
  * pairs, [N,K,D] fp32 (x^ = F.normalize(x) when norm_descs).  The reference builds every descriptor from this tensor
  * and caches it per image (`<cache_id>_r.pt`); here it is only materialised when a caller asks for it. */
@@ -566,6 +589,12 @@ int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream);
 #define ANYLOC_POOL_GEM 2
 int anyloc_pool(const float* feats, const int32_t* n_valid, int B, int N, int D, int mode, float gem_p,
                 int gem_use_abs, float* out, void* stream);
+/* The same pooling of a packed list: feats [R,D], image b = rows [row0[b], row0[b] + len[b]) (row0 [B] int64, len [B]
+ * int32, device arrays; the table rules and refusals of anyloc_vlad_generate_varlen, out 16-byte aligned in vlad's
+ * place).  Each image's rows are read in pool's order, so out[b] is bitwise anyloc_pool's for the padded batch with
+ * n_valid = len; len = 0 gives NaN.  No workspace. */
+int anyloc_pool_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B, int D, int mode,
+                       float gem_p, int gem_use_abs, float* out, void* stream);
 
 /* ------------------------------------------------------------------ image pre-processing
  * Replaces `base_transform` (dvgl_benchmark/datasets_ws.py:20-23: T.ToTensor + T.Normalize) and the centre crop to a
