@@ -113,7 +113,14 @@ _SIGS = {
                                              [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_kmeans_update_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_int] * 3 +
                                    [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "anyloc_topk_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
+    "anyloc_vlad_assign_multi_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "anyloc_vlad_assign_multi": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                           C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+                                           C.c_void_p]),
+    "anyloc_kmeans_accumulate_round_multi": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int),
+                                                       C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int,
+                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_void_p]),
+    "anyloc_topk_workspace_bytes":(C.c_size_t, [C.c_int] * 4),
     "anyloc_topk": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 6 +
                     [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_index_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),

@@ -17,6 +17,7 @@
 // (The FFMA assignment kernel serves D > 2048, calls of fewer than 256 rows and workspaces without room for the
 // coarse scores, at any K.)
 #include <algorithm>
+#include <vector>
 #include "epilogue.cuh"
 
 namespace anyloc {
@@ -205,6 +206,100 @@ vlad_rescore_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_v
   if (lane == 0) {
     labels[row] = valid ? bestk : -1;
     if (inv_norm) inv_norm[row] = 1.0f / fmaxf(xn, 1e-12f);
+  }
+}
+
+// Several vocabularies' labels from one read of each row (anyloc_vlad_assign_multi).  load_row and rescore_row restate
+// vlad_rescore_kernel's row load and its per-row body operation for operation (the same loads, FMAs, reductions and
+// candidate order), so each vocabulary's label is the one that kernel computes; vlad_rescore_kernel keeps its own text
+// because calling the shared body from it changes its register allocation.
+// rescore_row: the label of one row (warp-wide); v holds the row's float4s, xn = |x|, crow its K coarse scores.
+template <int MAXV>
+__device__ __forceinline__ int rescore_row(const float4 (&v)[MAXV], float xn, int lane, int D, int K,
+                                           const float* __restrict__ crow, const float* __restrict__ chat,
+                                           const float* __restrict__ cbias, const float* __restrict__ cnorm) {
+  const int D4 = D >> 2;
+  // coarse maximum and the largest centre norm (lanes stride over k)
+  float smax = -INFINITY, cmax = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    smax = fmaxf(smax, crow[k]);
+    cmax = fmaxf(cmax, cnorm[k]);
+  }
+  smax = warp_max(smax); cmax = warp_max(cmax);
+  // |S~_k - S_k| <= (2^-10 + 2^-11) sum|x_i c_i| <= 1.5 * 2^-10 |x||c_k| < 2^-9 |x||c_k|  (truncated x, rounded c)
+  const float thresh = smax - 2.0f * (0.001953125f * xn * cmax) - 1e-30f;
+  float best = -INFINITY; int bestk = 0;
+  for (int k0 = 0; k0 < K; k0 += 32) {
+    const int k = k0 + lane;
+    const bool cand = k < K && crow[k] >= thresh;
+    unsigned mask = __ballot_sync(0xffffffffu, cand);
+    while (mask) {
+      // up to four candidates at a time (independent accumulators hide the L1/L2 latency of the centre rows)
+      int kk[4]; int n = 0;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        if (mask) { kk[q] = k0 + __ffs(mask) - 1; mask &= mask - 1; ++n; } else kk[q] = kk[0];
+      }
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        int d = lane + i * 32;
+        if (d < D4) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            float4 c = __ldg(reinterpret_cast<const float4*>(chat + (size_t)kk[q] * D) + d);
+            acc[q] = fmaf(v[i].x, c.x, acc[q]); acc[q] = fmaf(v[i].y, c.y, acc[q]);
+            acc[q] = fmaf(v[i].z, c.z, acc[q]); acc[q] = fmaf(v[i].w, c.w, acc[q]);
+          }
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float sc = warp_sum(acc[q]) + cbias[kk[q]];
+        if (q < n && sc > best) { best = sc; bestk = kk[q]; }   // ascending k, strict >: lowest index wins exact ties
+      }
+    }
+  }
+  return bestk;
+}
+
+template <int MAXV>      // float4 per lane: D <= 128 * MAXV
+__device__ __forceinline__ float load_row(const float* __restrict__ x, int64_t row, int D, int lane, float4 (&v)[MAXV]) {
+  const int D4 = D >> 2;
+  const float4* xr = reinterpret_cast<const float4*>(x + row * (int64_t)D);
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < MAXV; ++i) {
+    int d = lane + i * 32;
+    if (d < D4) { v[i] = __ldg(xr + d); ss += v[i].x * v[i].x + v[i].y * v[i].y + v[i].z * v[i].z + v[i].w * v[i].w; }
+  }
+  return sqrtf(warp_sum(ss));
+}
+
+// The coarse scores [R, ldc] hold the vocabularies side by side, segment s in columns [koff[s], koff[s] + k[s]) of the scores and rows of the prepared
+// centres.  Each segment's candidates, threshold and argmax are vlad_rescore_kernel's for that vocabulary alone.
+constexpr int ASSIGN_MULTI_SEGS = 32;      // segments per rescoring launch
+struct RescoreSegs {
+  int n;
+  int koff[ASSIGN_MULTI_SEGS], k[ASSIGN_MULTI_SEGS];
+  int32_t* labels[ASSIGN_MULTI_SEGS];      // the segment's labels of this launch's first row
+};
+
+template <int MAXV>
+__global__ void __launch_bounds__(256)
+vlad_rescore_multi_kernel(const float* __restrict__ x, int64_t R, int D, int ldc, const float* __restrict__ chat,
+                          const float* __restrict__ cbias, const float* __restrict__ cnorm,
+                          const float* __restrict__ coarse /*[R,ldc]*/, const RescoreSegs segs) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (row >= R) return;
+  float4 v[MAXV];
+  const float xn = load_row<MAXV>(x, row, D, lane, v);
+  for (int s = 0; s < segs.n; ++s) {
+    const int k0 = segs.koff[s];
+    const int bestk = rescore_row<MAXV>(v, xn, lane, D, segs.k[s], coarse + row * ldc + k0, chat + (size_t)k0 * D,
+                                        cbias + k0, cnorm + k0);
+    if (lane == 0) segs.labels[s][row] = bestk;
   }
 }
 
@@ -1327,6 +1422,54 @@ __global__ void kmeans_accumulate_tiled_kernel(const float* __restrict__ x, cons
     for (int k = t; k < kt; k += ACC_COLS) pcounts[(size_t)blockIdx.y * K + k0 + k] = cnt[k];
 }
 
+// The same partials for several vocabularies fitted on the same rows (anyloc_kmeans_accumulate_round_multi): a CTA
+// keeps every vocabulary's [K][128] sums and [K] counts in shared memory, reads each row's 128 columns once and adds
+// them to every vocabulary's cluster, in row order -- each vocabulary's sums are kmeans_accumulate_kernel's.
+constexpr int KMEANS_MULTI_SET = 32;       // vocabularies per launch
+struct AccumSet {
+  int n;
+  int k[KMEANS_MULTI_SET], off[KMEANS_MULTI_SET];      // off: the vocabulary's first shared-memory float
+  const int32_t* labels[KMEANS_MULTI_SET];
+  float *psums[KMEANS_MULTI_SET], *pcounts[KMEANS_MULTI_SET];
+};
+
+__global__ void kmeans_accumulate_multi_kernel(const float* __restrict__ x, int64_t R, int64_t piece, int D, int resume,
+                                               const AccumSet set) {
+  extern __shared__ float acc[];                          // per vocabulary: [K][128] sums, then [K] counts
+  const int t = threadIdx.x, col = blockIdx.x * ACC_COLS + t;
+  const bool colok = col < D;
+  for (int v = 0; v < set.n; ++v) {
+    const int K = set.k[v];
+    float* a = acc + set.off[v];
+    const float* ps = set.psums[v] + (size_t)blockIdx.y * K * D;
+    for (int k = 0; k < K; ++k) a[k * ACC_COLS + t] = resume && colok ? ps[(size_t)k * D + col] : 0.f;
+    for (int k = t; k < K; k += ACC_COLS)
+      a[K * ACC_COLS + k] = resume && blockIdx.x == 0 ? set.pcounts[v][(size_t)blockIdx.y * K + k] : 0.f;
+  }
+  __syncthreads();
+  int64_t r0 = (int64_t)blockIdx.y * piece, r1 = min(R, r0 + piece);
+  for (int64_t r = r0; r < r1; ++r) {
+    const float xv = colok ? __ldg(x + r * D + col) : 0.f;
+    for (int v = 0; v < set.n; ++v) {
+      const int l = set.labels[v][r];
+      if (l < 0) continue;
+      float* a = acc + set.off[v];
+      if (colok) a[l * ACC_COLS + t] += xv;
+      if (blockIdx.x == 0 && t == 0) a[set.k[v] * ACC_COLS + l] += 1.f;
+    }
+  }
+  __syncthreads();
+  for (int v = 0; v < set.n; ++v) {
+    const int K = set.k[v];
+    const float* a = acc + set.off[v];
+    float* ps = set.psums[v] + (size_t)blockIdx.y * K * D;
+    for (int k = 0; k < K; ++k)
+      if (colok) ps[(size_t)k * D + col] = a[k * ACC_COLS + t];
+    if (blockIdx.x == 0)
+      for (int k = t; k < K; k += ACC_COLS) set.pcounts[v][(size_t)blockIdx.y * K + k] = a[K * ACC_COLS + k];
+  }
+}
+
 __global__ void __launch_bounds__(256)
 kmeans_finalize_kernel(const float* __restrict__ psums, const float* __restrict__ pcounts, int chunks,
                        const float* __restrict__ old_c, int D, int K, float* __restrict__ new_c,
@@ -1468,6 +1611,119 @@ extern "C" int anyloc_vlad_assign(const float* feats, const float* centers, int 
   AssignBufs ab;
   if (!take_assign_bufs(w, R, D, K, &ab)) { set_error("vlad_assign: workspace too small"); return ANYLOC_ERR_WORKSPACE; }
   return launch_assign(feats, nullptr, R, R, D, K, centers, dist_mode, ab, labels, nullptr, (cudaStream_t)stream);
+}
+
+// anyloc_vlad_assign_multi: the rows of one coarse slice, bounding its [rows, sum K] scores to 2^26 floats (256 MB)
+constexpr int64_t ASSIGN_MULTI_COARSE = 1ll << 26;
+static int64_t assign_multi_slice(int64_t R, int64_t Ksum) {
+  return std::min<int64_t>(R, std::max<int64_t>(256, ASSIGN_MULTI_COARSE / Ksum / 256 * 256));
+}
+
+// the prepared centres of all vocabularies side by side ([sum K, D], tf32 copy, bias, norms) and, where the coarse
+// route can run at all (D <= 2048, R >= 256), one slice of coarse scores.  ws == nullptr: dry run.
+static size_t carve_assign_multi(void* ws, size_t ws_bytes, int64_t R, int D, int64_t Ksum, AssignBufs* ab) {
+  Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  ab->chat = w.take<float>((size_t)Ksum * D);
+  ab->chat_tf32 = w.take<float>((size_t)Ksum * D);
+  ab->cbias = w.take<float>(Ksum);
+  ab->cnorm = w.take<float>(Ksum);
+  ab->coarse = D <= 2048 && R >= 256 ? w.take<float>((size_t)assign_multi_slice(R, Ksum) * Ksum) : nullptr;
+  const bool ok = ab->chat && ab->chat_tf32 && ab->cbias && ab->cnorm && (ab->coarse || D > 2048 || R < 256);
+  return ok ? w.off : 0;
+}
+
+static int64_t assign_multi_ksum(int V, const int* K) {
+  int64_t s = 0;
+  for (int v = 0; v < V; ++v) s += K[v];
+  return s;
+}
+
+extern "C" size_t anyloc_vlad_assign_multi_workspace_bytes(int64_t R, int D, int V, const int* K) {
+  if (!K || V <= 0 || D <= 0) return 0;
+  const int64_t Ksum = assign_multi_ksum(V, K);
+  AssignBufs ab;
+  return Ksum > 0 ? carve_assign_multi(nullptr, 0, R, D, Ksum, &ab) : 0;
+}
+
+extern "C" int anyloc_vlad_assign_multi(const float* feats, int64_t R, int D, int V, const float* const* centers,
+                                        const int* K, int dist_mode, int32_t* labels, void* ws, size_t ws_bytes,
+                                        void* stream) {
+  ANYLOC_REQUIRE(feats && centers && K && labels && ws, "vlad_assign_multi: null pointer");
+  ANYLOC_REQUIRE(R >= 0 && R < (1ll << 31) && D > 0 && D % 4 == 0 && V > 0,
+                 "vlad_assign_multi: bad dims R=%lld D=%d V=%d", (long long)R, D, V);
+  ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
+                 "vlad_assign_multi: unknown dist_mode %d", dist_mode);
+  for (int v = 0; v < V; ++v)
+    ANYLOC_REQUIRE(K[v] > 0 && centers[v], "vlad_assign_multi: vocabulary %d has K=%d or no centres", v, K[v]);
+  const int64_t Ksum = assign_multi_ksum(V, K);
+  ANYLOC_REQUIRE(Ksum < (1ll << 31), "vlad_assign_multi: %lld centres in all", (long long)Ksum);
+  if (R == 0) return ANYLOC_OK;
+  AssignBufs ab;
+  if (!carve_assign_multi(ws, ws_bytes, R, D, Ksum, &ab)) {
+    set_error("vlad_assign_multi: workspace too small (%zu given, %zu needed)", ws_bytes,
+              anyloc_vlad_assign_multi_workspace_bytes(R, D, V, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  // Each vocabulary takes the route anyloc_vlad_assign takes for it alone: its buffers there are 256-byte aligned like
+  // these, so the GEMM shape check with N = K_v gives the same answer.  The FFMA and rescoring kernels may break
+  // near-ties differently, so a vocabulary that would take the FFMA kernel alone takes it here too.
+  std::vector<int> koff(V), fast(V);
+  bool any_fast = false;
+  for (int v = 0, off = 0; v < V; off += K[v], ++v) {
+    koff[v] = off;
+    vlad_centre_prep_kernel<<<K[v], 256, 0, st>>>(centers[v], K[v], D, dist_mode, ab.chat + (size_t)off * D,
+                                                  ab.cbias + off, ab.chat_tf32 + (size_t)off * D, ab.cnorm + off,
+                                                  nullptr, 0);
+    ANYLOC_CHECK_LAUNCH();
+    const EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, K[v]};
+    fast[v] = ab.coarse != nullptr && D <= 2048 && R >= 256 &&
+              gemm_tc_supported(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K[v], D, ep, ANYLOC_PAIR_TF32);
+    any_fast = any_fast || fast[v];
+    if (!fast[v]) {
+      const int sms = device_sm_count();
+      const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(((R + 1) / 2 + 7) / 8, (int64_t)sms * 8));
+      vlad_assign_kernel<2><<<blocks, 256, 0, st>>>(feats, nullptr, (int)R, R, D, K[v], ab.chat + (size_t)off * D,
+                                                    ab.cbias + off, labels + (size_t)v * R, nullptr);
+      ANYLOC_CHECK_LAUNCH();
+    }
+  }
+  if (!any_fast) return ANYLOC_OK;
+  // one tf32 GEMM over all sum K prepared centres per slice of rows, then the segmented rescoring, 32 vocabularies at
+  // a time
+  const int64_t S = assign_multi_slice(R, Ksum);
+  const EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, (int)Ksum};
+  for (int64_t r0 = 0; r0 < R; r0 += S) {
+    const int m = (int)std::min<int64_t>(S, R - r0);
+    const float* xs = feats + r0 * D;
+    int rc = gemm_tc_launch(xs, nullptr, D, ab.chat_tf32, nullptr, D, m, (int)Ksum, D, ep, ANYLOC_PAIR_TF32, st);
+    if (rc) return rc;
+    RescoreSegs segs;
+    segs.n = 0;
+    for (int v = 0; v < V; ++v) {
+      if (fast[v]) {
+        segs.koff[segs.n] = koff[v];
+        segs.k[segs.n] = K[v];
+        segs.labels[segs.n] = labels + (size_t)v * R + r0;
+        ++segs.n;
+      }
+      if (segs.n == ASSIGN_MULTI_SEGS || (v == V - 1 && segs.n > 0)) {
+        const int blocks = (m + 7) / 8;
+        if (D <= 512)
+          vlad_rescore_multi_kernel<4><<<blocks, 256, 0, st>>>(xs, m, D, (int)Ksum, ab.chat, ab.cbias, ab.cnorm,
+                                                               ab.coarse, segs);
+        else if (D <= 1024)
+          vlad_rescore_multi_kernel<8><<<blocks, 256, 0, st>>>(xs, m, D, (int)Ksum, ab.chat, ab.cbias, ab.cnorm,
+                                                               ab.coarse, segs);
+        else
+          vlad_rescore_multi_kernel<16><<<blocks, 256, 0, st>>>(xs, m, D, (int)Ksum, ab.chat, ab.cbias, ab.cnorm,
+                                                                ab.coarse, segs);
+        ANYLOC_CHECK_LAUNCH();
+        segs.n = 0;
+      }
+    }
+  }
+  return ANYLOC_OK;
 }
 
 // Prepared vocabulary blob (anyloc_vlad_prepare): c^ [K,D] | tf32(c^) [K,D] | bias [K] | |c^| [K].  Everything the
@@ -2064,6 +2320,56 @@ extern "C" int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels,
   if (!rc) rc = anyloc_kmeans_accumulate_round_tiled(x, labels, R, R, rows_per, D, K, k_tile, 0, ws, ws_bytes, stream);
   if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
   return rc;
+}
+
+extern "C" int anyloc_kmeans_accumulate_round_multi(const float* x, int V, const int32_t* const* labels, const int* K,
+                                                    int64_t R, int64_t round_rows, int64_t piece_rows, int D,
+                                                    int resume, void* const* ws, const size_t* ws_bytes,
+                                                    void* stream) {
+  ANYLOC_REQUIRE(x && labels && K && ws && ws_bytes, "kmeans_accumulate_round_multi: null pointer");
+  ANYLOC_REQUIRE(V > 0 && R >= 0 && D > 0 && piece_rows >= 0 && round_rows >= 0,
+                 "kmeans_accumulate_round_multi: bad dims V=%d R=%lld D=%d", V, (long long)R, D);
+  std::vector<KmeansBufs> b(V);
+  for (int v = 0; v < V; ++v) {
+    ANYLOC_REQUIRE(labels[v] && K[v] > 0, "kmeans_accumulate_round_multi: vocabulary %d has K=%d or no labels", v, K[v]);
+    ANYLOC_REQUIRE(((size_t)K[v] * ACC_COLS + K[v]) * 4 <= 220 * 1024,
+                   "kmeans_accumulate_round_multi: vocabulary %d has K=%d, beyond the untiled update's shared memory",
+                   v, K[v]);
+    if (!take_kmeans_bufs(ws[v], ws_bytes[v], R, D, K[v], &b[v])) {
+      set_error("kmeans_accumulate_round_multi: vocabulary %d's workspace is too small (%zu given, %zu needed)", v,
+                ws_bytes[v], anyloc_kmeans_round_workspace_bytes(R, D, K[v]));
+      return ANYLOC_ERR_WORKSPACE;
+    }
+  }
+  ANYLOC_REQUIRE(round_rows <= (int64_t)b[0].chunks * piece_rows,
+                 "kmeans_accumulate_round_multi: %lld rows do not fit %d pieces of %lld", (long long)round_rows,
+                 b[0].chunks, (long long)piece_rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(kmeans_accumulate_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         220 * 1024));
+  // consecutive vocabularies share a launch while their sums and counts fit the 220 KB
+  AccumSet set;
+  set.n = 0;
+  int used = 0;
+  for (int v = 0; v <= V; ++v) {
+    const int need = v < V ? (K[v] * ACC_COLS + K[v]) : 0;
+    if (set.n > 0 && (v == V || set.n == KMEANS_MULTI_SET || (size_t)(used + need) * 4 > 220 * 1024)) {
+      kmeans_accumulate_multi_kernel<<<dim3(cdiv(D, ACC_COLS), b[0].chunks), ACC_COLS, (size_t)used * 4, st>>>(
+          x, round_rows, piece_rows, D, resume, set);
+      ANYLOC_CHECK_LAUNCH();
+      set.n = 0;
+      used = 0;
+    }
+    if (v == V) break;
+    set.k[set.n] = K[v];
+    set.off[set.n] = used;
+    set.labels[set.n] = labels[v];
+    set.psums[set.n] = b[v].psums;
+    set.pcounts[set.n] = b[v].pcounts;
+    ++set.n;
+    used += need;
+  }
+  return ANYLOC_OK;
 }
 
 // ====================================================================================================================

@@ -1189,16 +1189,33 @@ def _pca_boxes(n, d, plan):
 
 def _host_fit_plan(X, dev, K, copies):
     """_kmeans_plan for host rows X on `dev`; None (the in-memory fit) for device rows."""
+    return _host_plan(X, dev, [K], copies, lambda lib, n, D: lib.anyloc_vlad_workspace_bytes(1, n, D, K))
+
+
+def _host_fit_plan_multi(X, dev, Ks, copies):
+    """_host_fit_plan for vocabularies of Ks[v] clusters fitted together (fit_vocabularies): the shared assignment's
+    workspace, every member's round workspace and one row of labels per member."""
+    arr = (C.c_int * len(Ks))(*Ks)
+    return _host_plan(X, dev, Ks, copies,
+                      lambda lib, n, D: lib.anyloc_vlad_assign_multi_workspace_bytes(n, D, len(Ks), arr))
+
+
+def _fit_ws_bytes(assign_bytes, upd_bytes, V):
+    """ws_bytes(n) of _kmeans_plan for V vocabularies fitted together: the assignment workspace of an n-row pass, the
+    members' round workspaces (upd_bytes in all; chunks * K * D partial sums each, whatever the round) and V rows of
+    n labels"""
+    return lambda n: assign_bytes(n) + upd_bytes + 4 * V * n
+
+
+def _host_plan(X, dev, Ks, copies, assign_bytes):
     if dev.type != "cuda" or X.is_cuda:
         return None
     lib = _lib.load()
     R, D = X.shape
     with torch.cuda.device(dev):
         chunks, rows_per = _kmeans_partition(R, D)
-        upd = lib.anyloc_kmeans_round_workspace_bytes(R, D, K)     # chunks * K * D partial sums, whatever the round
-
-        def ws_bytes(n):
-            return lib.anyloc_vlad_workspace_bytes(1, n, D, K) + upd + 4 * n
+        upd = sum(lib.anyloc_kmeans_round_workspace_bytes(R, D, K) for K in Ks)
+        ws_bytes = _fit_ws_bytes(lambda n: assign_bytes(lib, n, D), upd, len(Ks))
         budget = _device_budget(dev)
         return _kmeans_fit_plan(R, D, chunks, rows_per, budget, torch.cuda.mem_get_info(dev)[0], copies, ws_bytes,
                                 _STAGE_BYTES)
@@ -1315,98 +1332,253 @@ class _KMeans:
     def _fit_streamed(self, X, centroids, normalize, plan, dev):
         """fit_predict on host rows X [R,D] (any float dtype and strides) too large for the device, rows L2-normalised
         first when `normalize` (VLAD.fit).  Each Lloyd pass feeds the rows in rounds of P rows per chunk of the
-        in-memory update (_stream_rounds), so centres and labels are bit-identical to the in-memory fit's.  The first
-        `resident` rounds are copied and normalised once, in iteration 0; the others cross the host link every
-        iteration through two pinned staging buffers, the copy of one round overlapping the device work on the one
-        before.  The shift is read after every iteration: a speculative extra pass would cost a full transfer."""
-        lib = _lib.load()
-        P, resident = plan
+        in-memory update (_RoundFeed), so centres and labels are bit-identical to the in-memory fit's.  The shift is
+        read after every iteration: a speculative extra pass would cost a full transfer."""
         X = X.detach()
         R, D = X.shape
         K = self.n_clusters
-        tiled = _kmeans_tiled(K)
         with torch.cuda.device(dev):
-            chunks, rows_per = _kmeans_partition(R, D)
-            rounds = _stream_rounds(R, chunks, rows_per, P)
-            piece = [pcs[0][1] for pcs in rounds]                      # every chunk's piece but the last one's
-            sizes = [(chunks - 1) * pcs[0][1] + pcs[-1][1] for pcs in rounds]
-            offs = np.concatenate([[0], np.cumsum(sizes)]).tolist()
             if centroids is None:
-                init = np.random.choice(R, size=[K], replace=False)      # the in-memory fit's draw
-                c = _as_device_f32(X[torch.from_numpy(init)], dev)
-                if normalize:
-                    c = _normalize_rows_dev(c)
+                c = _streamed_init(X, K, normalize, dev)
             else:
                 c = _as_device_f32(centroids, dev)
-            kept = torch.empty(offs[resident], D, device=dev)
-            raw = [torch.empty(sizes[0], D, device=dev) for _ in range(2)]
-            host = [torch.empty(sizes[0], D, pin_memory=True) for _ in range(2)]
-            ws = _lib.workspaces.get(dev, lib.anyloc_kmeans_round_workspace_bytes(R, D, K), "kmeans_upd")
-            cs, xs = torch.cuda.current_stream(), torch.cuda.Stream()
-            copied, freed = [None, None], [None, None]
-            transfers = ((it, j) for it in range(self.max_iter) for j in range(0 if it == 0 else resident, len(rounds)))
-            staged = []
-
-            def stage():
-                """gather the next transferred round into a staging buffer and queue its copy to the device"""
-                t = next(transfers, None)
-                if t is None:
-                    return
-                j, s = t[1], len(staged) & 1
-                if copied[s] is not None:
-                    copied[s].synchronize()                            # the staging buffer's previous copy is done
-                for ci, (lo, m) in enumerate(rounds[j]):
-                    host[s][ci * piece[j]:ci * piece[j] + m].copy_(X[lo:lo + m])
-                with torch.cuda.stream(xs):
-                    if freed[s] is not None:
-                        xs.wait_event(freed[s])
-                    raw[s][:sizes[j]].copy_(host[s][:sizes[j]], non_blocking=True)
-                    copied[s] = torch.cuda.Event()
-                    copied[s].record(xs)
-                staged.append((t, s, copied[s]))
-
-            stage()
-            taken = 0
+            feed = _RoundFeed(X, normalize, plan, dev, self.max_iter)
+            ws = _lib.workspaces.get(dev, _lib.load().anyloc_kmeans_round_workspace_bytes(R, D, K), "kmeans_upd")
             for it in range(self.max_iter):
                 labels_r = []
-                for j in range(len(rounds)):
-                    x = kept[offs[j]:offs[j + 1]]
-                    if it == 0 or j >= resident:
-                        t, s, ev = staged[taken]
-                        taken += 1
-                        cs.wait_event(ev)
-                        x = raw[s][:sizes[j]]
-                        if normalize:
-                            x = _normalize_rows_dev(x)
-                        if j < resident:
-                            kept[offs[j]:offs[j + 1]].copy_(x)
+                for j, x in feed.iteration(it):
                     labels_r.append(self._assign(x, c))
-                    if tiled:
-                        _lib.check(lib.anyloc_kmeans_accumulate_round_tiled(
-                            _lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j], piece[j], D, K, 0, int(j > 0),
-                            _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_kmeans_accumulate_round_tiled")
-                    else:
-                        _lib.check(lib.anyloc_kmeans_accumulate_round(_lib.ptr(x), _lib.ptr(labels_r[-1]), R, sizes[j],
-                                                                      piece[j], D, K, int(j > 0), _lib.ptr(ws),
-                                                                      ws.numel(), _lib.stream_ptr()),
-                                   "anyloc_kmeans_accumulate_round")
-                    if it == 0 or j >= resident:
-                        freed[s] = torch.cuda.Event()
-                        freed[s].record(cs)
-                        stage()
+                    _accumulate_round(x, labels_r[-1], R, feed.sizes[j], feed.piece[j], K, int(j > 0), ws)
                 c_next, err = torch.empty_like(c), torch.zeros(1, device=dev)
-                _lib.check(lib.anyloc_kmeans_finalize(_lib.ptr(c), R, D, K, _lib.ptr(c_next), _lib.ptr(err),
-                                                      _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
-                           "anyloc_kmeans_finalize")
+                _finalize(c, R, c_next, err, ws)
                 labels, c = labels_r, c_next
                 if float(err) <= self.tol:
                     break
-            xs.synchronize()                                           # a round staged for an iteration not run
-            order = torch.from_numpy(np.concatenate([np.arange(lo, lo + m) for pcs in rounds for lo, m in pcs]))
+            feed.close()
             out = torch.empty(R, dtype=torch.int64)
-            out[order] = torch.cat(labels).to(torch.int64).cpu()
+            out[feed.order()] = torch.cat(labels).to(torch.int64).cpu()
         self.centroids = c.cpu()
         return out
+
+
+def _streamed_init(X, K, normalize, dev):
+    """the in-memory fit's random-choice init (numpy RNG), gathered from host rows X and normalised like the rows"""
+    init = np.random.choice(X.shape[0], size=[K], replace=False)
+    c = _as_device_f32(X[torch.from_numpy(init)], dev)
+    return _normalize_rows_dev(c) if normalize else c
+
+
+def _accumulate_round(x, labels, R, round_rows, piece, K, resume, ws):
+    """one round of a K-cluster k-means sum (anyloc_kmeans_accumulate_round, or its tiled form for K >= 437)"""
+    lib = _lib.load()
+    D = x.shape[1]
+    if _kmeans_tiled(K):
+        _lib.check(lib.anyloc_kmeans_accumulate_round_tiled(_lib.ptr(x), _lib.ptr(labels), R, round_rows, piece, D, K,
+                                                            0, resume, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                   "anyloc_kmeans_accumulate_round_tiled")
+    else:
+        _lib.check(lib.anyloc_kmeans_accumulate_round(_lib.ptr(x), _lib.ptr(labels), R, round_rows, piece, D, K,
+                                                      resume, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                   "anyloc_kmeans_accumulate_round")
+
+
+def _finalize(c, R, c_next, err, ws):
+    """anyloc_kmeans_finalize: the centres c_next and the shift err [1] from the sums in ws"""
+    K, D = c.shape
+    _lib.check(_lib.load().anyloc_kmeans_finalize(_lib.ptr(c), R, D, K, _lib.ptr(c_next), _lib.ptr(err), _lib.ptr(ws),
+                                                  ws.numel(), _lib.stream_ptr()), "anyloc_kmeans_finalize")
+
+
+class _RoundFeed:
+    """The rounds of a streamed k-means pass over host rows X [R,D] (any float dtype and strides), on the device, for
+    plan (P, resident) of _kmeans_plan: round j holds P rows of every chunk of the in-memory update (_stream_rounds),
+    chunk after chunk, so a pass that sums the rounds in order sums each chunk in row order.  Rows are L2-normalised
+    on the device when `normalize`.  The first `resident` rounds are copied and normalised once, in iteration 0; the
+    others cross the host link every iteration through two pinned staging buffers, the gather and copy of one round
+    overlapping the device work on the one before.  A round crosses the link once per iteration however much work is
+    enqueued on it.  Built and iterated under torch.cuda.device(dev)."""
+
+    def __init__(self, X, normalize, plan, dev, max_iter):
+        P, self.resident = plan
+        self.X, self.normalize = X, normalize
+        R, D = X.shape
+        chunks, rows_per = _kmeans_partition(R, D)
+        self.rounds = _stream_rounds(R, chunks, rows_per, P)
+        self.piece = [pcs[0][1] for pcs in self.rounds]                # every chunk's piece but the last one's
+        self.sizes = [(chunks - 1) * pcs[0][1] + pcs[-1][1] for pcs in self.rounds]
+        self.offs = np.concatenate([[0], np.cumsum(self.sizes)]).tolist()
+        self.kept = torch.empty(self.offs[self.resident], D, device=dev)
+        self.raw = [torch.empty(self.sizes[0], D, device=dev) for _ in range(2)]
+        self.host = [torch.empty(self.sizes[0], D, pin_memory=True) for _ in range(2)]
+        self.cs, self.xs = torch.cuda.current_stream(), torch.cuda.Stream()
+        self.copied, self.freed = [None, None], [None, None]
+        self.transfers = ((it, j) for it in range(max_iter)
+                          for j in range(0 if it == 0 else self.resident, len(self.rounds)))
+        self.staged, self.taken = [], 0
+        self._stage()
+
+    def _stage(self):
+        """gather the next transferred round into a staging buffer and queue its copy to the device"""
+        t = next(self.transfers, None)
+        if t is None:
+            return
+        j, s = t[1], len(self.staged) & 1
+        if self.copied[s] is not None:
+            self.copied[s].synchronize()                               # the staging buffer's previous copy is done
+        piece, host = self.piece[j], self.host[s]
+        for ci, (lo, m) in enumerate(self.rounds[j]):
+            host[ci * piece:ci * piece + m].copy_(self.X[lo:lo + m])
+        with torch.cuda.stream(self.xs):
+            if self.freed[s] is not None:
+                self.xs.wait_event(self.freed[s])
+            self.raw[s][:self.sizes[j]].copy_(host[:self.sizes[j]], non_blocking=True)
+            self.copied[s] = torch.cuda.Event()
+            self.copied[s].record(self.xs)
+        self.staged.append((t, s, self.copied[s]))
+
+    def iteration(self, it):
+        """yields (j, x) for every round j of Lloyd iteration `it`, x [sizes[j], D] the round's rows on the device; the
+        caller enqueues its work on x on the current stream before it asks for the next round"""
+        for j in range(len(self.rounds)):
+            x = self.kept[self.offs[j]:self.offs[j + 1]]
+            moved = it == 0 or j >= self.resident
+            if moved:
+                t, s, ev = self.staged[self.taken]
+                self.taken += 1
+                self.cs.wait_event(ev)
+                x = self.raw[s][:self.sizes[j]]
+                if self.normalize:
+                    x = _normalize_rows_dev(x)
+                if j < self.resident:
+                    self.kept[self.offs[j]:self.offs[j + 1]].copy_(x)
+            yield j, x
+            if moved:
+                self.freed[s] = torch.cuda.Event()
+                self.freed[s].record(self.cs)
+                self._stage()
+
+    def close(self):
+        self.xs.synchronize()                                          # a round staged for an iteration not run
+
+    def order(self):
+        """the host row of every row of the rounds, in round order"""
+        return torch.from_numpy(np.concatenate([np.arange(lo, lo + m) for pcs in self.rounds for lo, m in pcs]))
+
+
+def _assign_multi(x, centres, mode):
+    """labels [V, R] int32 of the rows x [R, D] against each of V centre sets (anyloc_vlad_assign_multi): row v is
+    _KMeans._assign(x, centres[v]) bit for bit"""
+    lib = _lib.load()
+    R, D = x.shape
+    V = len(centres)
+    Ks = (C.c_int * V)(*[c.shape[0] for c in centres])
+    ptrs = (C.c_void_p * V)(*[c.data_ptr() for c in centres])
+    labels = torch.empty(V, R, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        ws = _lib.workspaces.get(x.device, lib.anyloc_vlad_assign_multi_workspace_bytes(R, D, V, Ks), "kmeans")
+        _lib.check(lib.anyloc_vlad_assign_multi(_lib.ptr(x), R, D, V, ptrs, Ks, _lib.DIST[mode], _lib.ptr(labels),
+                                                _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_vlad_assign_multi")
+    return labels
+
+
+def _accumulate_round_multi(x, labels, Ks, ws, R, round_rows, piece, resume):
+    """one round of the k-means sums of V vocabularies of Ks[v] clusters on the same rows x: the members below K = 437
+    in one fused accumulate (anyloc_kmeans_accumulate_round_multi), the others in their own tiled round"""
+    lib = _lib.load()
+    D = x.shape[1]
+    fused = [v for v, K in enumerate(Ks) if not _kmeans_tiled(K)]
+    for v in range(len(Ks)):
+        if v not in fused:
+            _accumulate_round(x, labels[v], R, round_rows, piece, Ks[v], resume, ws[v])
+    if fused:
+        n = len(fused)
+        _lib.check(lib.anyloc_kmeans_accumulate_round_multi(
+            _lib.ptr(x), n, (C.c_void_p * n)(*[labels[v].data_ptr() for v in fused]),
+            (C.c_int * n)(*[Ks[v] for v in fused]), R, round_rows, piece, D, resume,
+            (C.c_void_p * n)(*[ws[v].data_ptr() for v in fused]), (C.c_size_t * n)(*[ws[v].numel() for v in fused]),
+            _lib.stream_ptr()), "anyloc_kmeans_accumulate_round_multi")
+
+
+def _finalize_multi(c, R, ws):
+    """anyloc_kmeans_finalize of every member -> (new centres, shifts [V] on the device)"""
+    nxt = [torch.empty_like(ci) for ci in c]
+    err = torch.zeros(len(c), device=c[0].device)
+    for v in range(len(c)):
+        _finalize(c[v], R, nxt[v], err[v:v + 1], ws[v])
+    return nxt, err
+
+
+def _lloyd_in_memory(kms, x, inits):
+    """the Lloyd loops of several k-means (kms, one _KMeans each, inits their random-choice draws) on the same device
+    rows x, each centre set bit for bit what kms[v].fit(x) gives.  Each iteration assigns the rows to every active
+    vocabulary at once and sums them in one fused pass.  As in fit_predict, iteration i + 1 is enqueued before the
+    shifts of iteration i are read; a member whose shift was within its tol keeps the centres of iteration i and takes
+    no part in later passes."""
+    R, D = x.shape
+    dev = x.device
+    n = len(kms)
+    with torch.cuda.device(dev):
+        c = [x[torch.from_numpy(i).to(dev)].contiguous() for i in inits]
+        ws = [torch.empty(_lib.load().anyloc_kmeans_round_workspace_bytes(R, D, km.n_clusters), dtype=torch.uint8,
+                          device=dev) for km in kms]
+        _, rows_per = _kmeans_partition(R, D)
+        final = [None] * n
+        hosts = [torch.empty(n, dtype=torch.float32).pin_memory() for _ in range(2)]
+        pending = None                              # (members, their next centres, host shifts, event) of iteration i
+        for it in range(max(km.max_iter for km in kms)):
+            act = [m for m in range(n) if final[m] is None and it < kms[m].max_iter]
+            if not act:
+                break
+            labels = _assign_multi(x, [c[m] for m in act], kms[0].mode)
+            _accumulate_round_multi(x, labels, [kms[m].n_clusters for m in act], [ws[m] for m in act], R, R,
+                                    rows_per, 0)
+            nxt, err = _finalize_multi([c[m] for m in act], R, [ws[m] for m in act])
+            host = hosts[it & 1]
+            host[:len(act)].copy_(err, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record()
+            if pending is not None:
+                pending[3].synchronize()
+                for i, m in enumerate(pending[0]):
+                    if final[m] is None and float(pending[2][i]) <= kms[m].tol:     # converged in the previous one
+                        final[m] = pending[1][i]
+            pending = (act, nxt, host, ev)
+            for i, m in enumerate(act):
+                c[m] = nxt[i]
+        if pending is not None:
+            pending[3].synchronize()
+        return [c[m] if final[m] is None else final[m] for m in range(n)]
+
+
+def _lloyd_streamed(kms, X, normalize, plan, dev):
+    """_lloyd_in_memory on host rows X too large for the device (plan of _host_fit_plan_multi), rows normalised on
+    the device when `normalize`: every round of _RoundFeed crosses the link once per iteration and is assigned and
+    summed for all active members before the next.  The shifts are read after every iteration, as in _fit_streamed.
+    The members' random-choice draws are taken here, in member order."""
+    R, D = X.shape
+    n = len(kms)
+    with torch.cuda.device(dev):
+        c = [_streamed_init(X, km.n_clusters, normalize, dev) for km in kms]
+        feed = _RoundFeed(X, normalize, plan, dev, max(km.max_iter for km in kms))
+        ws = [torch.empty(_lib.load().anyloc_kmeans_round_workspace_bytes(R, D, km.n_clusters), dtype=torch.uint8,
+                          device=dev) for km in kms]
+        final = [None] * n
+        for it in range(max(km.max_iter for km in kms)):
+            act = [m for m in range(n) if final[m] is None and it < kms[m].max_iter]
+            if not act:
+                break
+            for j, x in feed.iteration(it):
+                labels = _assign_multi(x, [c[m] for m in act], kms[0].mode)
+                _accumulate_round_multi(x, labels, [kms[m].n_clusters for m in act], [ws[m] for m in act], R,
+                                        feed.sizes[j], feed.piece[j], int(j > 0))
+            nxt, err = _finalize_multi([c[m] for m in act], R, [ws[m] for m in act])
+            err = err.cpu()
+            for i, m in enumerate(act):
+                c[m] = nxt[i]
+                if float(err[i]) <= kms[m].tol:
+                    final[m] = c[m]
+        feed.close()
+        return c
 
 
 VLAD_KERNEL_DESCRIPTION = ("VLAD: gemm_tc3_kernel<false, 0> (wgmma tf32 coarse scores straight from the fp32 features) -> "
@@ -1476,16 +1648,7 @@ class VLAD:
 
     # -- vocabulary (utilities.py:749-791)
     def fit(self, train_descs: Union[np.ndarray, torch.Tensor, None]):
-        self.kmeans = _KMeans(self.num_clusters, mode=self.mode)
-        self._centers_dev = {}
-        self._prepared_dev = None
-        if self.can_use_cache_vlad():
-            print("Using cached cluster centers")
-            self.c_centers = torch.load(f"{self.cache_dir}/c_centers.pt")
-            self.kmeans.centroids = self.c_centers
-            if self.desc_dim is None:
-                self.desc_dim = self.c_centers.shape[1]
-                print(f"Desc dim set to {self.desc_dim}")
+        if self._fit_from_cache():
             return
         if train_descs is None:
             raise ValueError("No training descriptors given")
@@ -1503,7 +1666,26 @@ class VLAD:
             if self.norm_descs:
                 x = _normalize_rows_dev(x)
             self.kmeans.fit(x)
-        self.c_centers = self.kmeans.centroids.cpu() if was_cpu else self.kmeans.centroids
+        self._set_vocabulary(self.kmeans.centroids.cpu() if was_cpu else self.kmeans.centroids)
+
+    def _fit_from_cache(self):
+        """the start of fit: a fresh k-means, and the cached vocabulary when there is one -> whether it was loaded"""
+        self.kmeans = _KMeans(self.num_clusters, mode=self.mode)
+        self._centers_dev = {}
+        self._prepared_dev = None
+        if not self.can_use_cache_vlad():
+            return False
+        print("Using cached cluster centers")
+        self.c_centers = torch.load(f"{self.cache_dir}/c_centers.pt")
+        self.kmeans.centroids = self.c_centers
+        if self.desc_dim is None:
+            self.desc_dim = self.c_centers.shape[1]
+            print(f"Desc dim set to {self.desc_dim}")
+        return True
+
+    def _set_vocabulary(self, c):
+        """the end of fit: the fitted centres c, written to the cache directory when there is one"""
+        self.c_centers = c
         self.kmeans.centroids = self.c_centers
         if self.cache_dir is not None:
             print("Caching cluster centers")
@@ -1763,6 +1945,70 @@ class VLAD:
 
 
 # ------------------------------------------------------------------ sibling aggregators (extension)
+def fit_vocabularies(vlads: List[VLAD], train_descs: Union[np.ndarray, torch.Tensor]) -> None:
+    """Fit every VLAD in `vlads` from one pass over `train_descs` per Lloyd iteration (extension: a sweep over the
+    vocabulary size, such as the reference's ablations over num_clusters, otherwise reads the rows once per K).
+
+    `train_descs` is what VLAD.fit takes: numpy, CPU or CUDA tensor, any float dtype or strides, host rows larger than
+    the device.  Afterwards every member is in exactly the state `for v in vlads: v.fit(train_descs)` leaves it in,
+    from the same numpy RNG state: c_centers (on the input's device), kmeans.centroids, desc_dim, the c_centers.pt of
+    a member with a cache_dir, and the numpy RNG state itself (the random-choice inits are drawn in member order).  A
+    member with cached centres loads them, draws nothing and takes no part in the pass; so does a member whose
+    cache_dir an earlier member writes, once that member's centres are saved.  Each member keeps its own
+    iteration count and convergence test and drops out of the passes once converged.
+
+    The members must agree in norm_descs and dist_mode (they share the normalised rows and the score GEMM); vlad_mode
+    and soft_temp do not enter the fit.  ValueError for an empty list, a VLAD listed twice or members that differ."""
+    vlads = list(vlads)
+    if not vlads:
+        raise ValueError("fit_vocabularies: no VLAD given")
+    first, twice = {}, []
+    for i, v in enumerate(vlads):
+        if id(v) in first:
+            twice.append(f"{first[id(v)]} and {i}")
+        first.setdefault(id(v), i)
+    if twice:
+        raise ValueError(f"fit_vocabularies: the same VLAD is listed more than once (members {', '.join(twice)})")
+    key = (bool(vlads[0].norm_descs), vlads[0].mode)
+    odd = [i for i, v in enumerate(vlads) if (bool(v.norm_descs), v.mode) != key]
+    if odd:
+        raise ValueError(f"fit_vocabularies: members {odd} differ from member 0 (norm_descs={key[0]}, "
+                         f"dist_mode={key[1]!r}) in norm_descs or dist_mode; the members share the rows and the scores")
+    todo, later, written = [], [], set()
+    for v in vlads:
+        if v.cache_dir is not None and v.cache_dir in written:
+            later.append(v)         # its own fit would load the centres an earlier member writes there
+        elif not v._fit_from_cache():
+            todo.append(v)
+            if v.cache_dir is not None:
+                written.add(v.cache_dir)
+    if not todo:
+        return
+    if train_descs is None:
+        raise ValueError("No training descriptors given")
+    if type(train_descs) == np.ndarray:
+        train_descs = torch.from_numpy(train_descs).to(torch.float32)
+    for v in todo:
+        if v.desc_dim is None:
+            v.desc_dim = train_descs.shape[1]
+    dev = _lib.require_cuda(train_descs.device if train_descs.is_cuda else None)
+    was_cpu = not train_descs.is_cuda
+    kms, norm = [v.kmeans for v in todo], bool(todo[0].norm_descs)
+    plan = _host_fit_plan_multi(train_descs, dev, [km.n_clusters for km in kms], copies=1 + norm)
+    if plan is not None:        # too large for the device: streamed, each round shared by all members
+        centres = _lloyd_streamed(kms, train_descs.detach(), norm, plan, dev)
+    else:
+        x = _as_device_f32(train_descs, dev)
+        if norm:
+            x = _normalize_rows_dev(x)
+        inits = [np.random.choice(x.shape[0], size=[km.n_clusters], replace=False) for km in kms]
+        centres = _lloyd_in_memory(kms, x, inits)
+    for v, c in zip(todo, centres):
+        v._set_vocabulary(c.cpu() if was_cpu else c)
+    for v in later:
+        v._fit_from_cache()
+
+
 _POOL = {"average": 0, "avg": 0, "mean": 0, "max": 1, "gem": 2}
 
 

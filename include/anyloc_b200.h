@@ -229,6 +229,23 @@ int anyloc_kmeans_accumulate_round_tiled(const float* x, const int32_t* labels, 
 int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels, const float* old_centers, int64_t R, int D,
                                int K, int k_tile, float* new_centers, float* err_out, void* ws, size_t ws_bytes,
                                void* stream);
+/* Several vocabularies fitted on the same rows (fit_vocabularies): V vocabularies of K[v] centres each.
+ * anyloc_vlad_assign_multi writes labels [V, R]; labels[v] equals anyloc_vlad_assign on vocabulary v alone, bit for
+ * bit.  Each row is read once by one tf32 coarse GEMM over all sum K centres (rows in slices of at most 2^26 / sum K,
+ * and at least 256) and once by the segmented rescoring.  A vocabulary for which anyloc_vlad_assign would take its
+ * FFMA kernel (R < 256, D > 2048, a shape the GEMM refuses) takes it here too.  Workspace:
+ * anyloc_vlad_assign_multi_workspace_bytes(R, D, V, K).
+ * anyloc_kmeans_accumulate_round_multi is anyloc_kmeans_accumulate_round for each vocabulary v, with its labels[v],
+ * K[v] and its own workspace ws[v] of anyloc_kmeans_round_workspace_bytes(R, D, K[v]) bytes: the partial sums are
+ * bitwise the same, and anyloc_kmeans_finalize finishes each one.  It reads each row once per launch; consecutive
+ * vocabularies share a launch while their sums and counts fit 220 KB of shared memory.  It refuses a K[v] that the
+ * untiled round refuses (K >= 437). */
+size_t anyloc_vlad_assign_multi_workspace_bytes(int64_t R, int D, int V, const int* K);
+int anyloc_vlad_assign_multi(const float* feats, int64_t R, int D, int V, const float* const* centers, const int* K,
+                             int dist_mode, int32_t* labels, void* ws, size_t ws_bytes, void* stream);
+int anyloc_kmeans_accumulate_round_multi(const float* x, int V, const int32_t* const* labels, const int* K, int64_t R,
+                                         int64_t round_rows, int64_t piece_rows, int D, int resume, void* const* ws,
+                                         const size_t* ws_bytes, void* stream);
 
 /* ------------------------------------------------------------- retrieval
  * Replaces the faiss part of get_top_k_recall (utilities.py:435-450): optional row
