@@ -376,6 +376,10 @@ extern "C" size_t anyloc_pca_colsum_workspace_bytes(int64_t rows, int cols) {
 extern "C" int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int cols, double* sum, void* ws,
                                  size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(x && sum && ws, "pca_colsum: null pointer");
+  // the PCA kernels read and write one element at a time: natural alignment is the whole contract, for any ld
+  ANYLOC_REQUIRE_ALIGNED(x, 4, "pca_colsum", "x", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(sum, 8, "pca_colsum", "sum", "fp64 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 8, "pca_colsum", "ws", "fp64 access");
   ANYLOC_REQUIRE(rows >= 0 && cols >= 0 && ld >= cols, "pca_colsum: rows=%lld cols=%d ld=%lld (rows >= 0, cols >= 0, "
                  "ld >= cols)", (long long)rows, cols, (long long)ld);
   if (ws_bytes < pca_colsum_workspace_bytes(rows, cols)) {
@@ -392,6 +396,10 @@ extern "C" int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64
                  mode == ANYLOC_PCA_SKETCH, "pca_accumulate: unknown mode %d", mode);
   const bool uses_u = mode == ANYLOC_PCA_VT || mode == ANYLOC_PCA_SKETCH;
   ANYLOC_REQUIRE(x && mu && out && (!uses_u || u || k == 0), "pca_accumulate: null pointer");
+  ANYLOC_REQUIRE_ALIGNED(x, 4, "pca_accumulate", "x", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(mu, 8, "pca_accumulate", "mu", "fp64 access");
+  ANYLOC_REQUIRE_ALIGNED(u, 8, "pca_accumulate", "u", "fp64 access");
+  ANYLOC_REQUIRE_ALIGNED(out, 8, "pca_accumulate", "out", "fp64 access");
   ANYLOC_REQUIRE(rows >= 0 && cols >= 0 && ld >= cols, "pca_accumulate: rows=%lld cols=%d ld=%lld (rows >= 0, "
                  "cols >= 0, ld >= cols)", (long long)rows, cols, (long long)ld);
   // out [M, N] += sum over K of A(kk, i) B(kk, j)
@@ -417,6 +425,7 @@ extern "C" int anyloc_pca_accumulate(int mode, const float* x, int64_t ld, int64
 extern "C" int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream) {
   ANYLOC_REQUIRE(a && m >= 0 && m <= 65535 * 32 && ld >= m, "pca_mirror: a=%p m=%d ld=%lld (0 <= m <= 65535*32, "
                  "ld >= m)", (void*)a, m, (long long)ld);
+  ANYLOC_REQUIRE_ALIGNED(a, 8, "pca_mirror", "a", "fp64 access");
   return pca_mirror_launch(a, m, ld, (cudaStream_t)stream);
 }
 

@@ -36,6 +36,12 @@ void set_error(const char* fmt, ...);
     }                                                                                  \
   } while (0)
 
+// Refuses a pointer that is not a multiple of `bytes` (a power of two): "<who>: <name> must be <bytes>-byte aligned
+// (<why>)".  A null pointer passes; the entries' null checks are their own.
+#define ANYLOC_REQUIRE_ALIGNED(p, bytes, who, name, why)                               \
+  ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(p) & ((uintptr_t)(bytes) - 1)) == 0,     \
+                 "%s: %s must be %d-byte aligned (%s)", who, name, (int)(bytes), why)
+
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 

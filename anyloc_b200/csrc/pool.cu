@@ -104,8 +104,9 @@ extern "C" int anyloc_pool(const float* feats, const int32_t* n_valid, int B, in
   ANYLOC_REQUIRE(B <= 65535, "pool: B=%d exceeds the grid limit", B);
   ANYLOC_REQUIRE(mode >= POOL_AVG && mode <= POOL_GEM, "pool: unknown mode %d", mode);
   ANYLOC_REQUIRE(mode != POOL_GEM || gem_p != 0.f, "pool: gem_p must be non-zero");
-  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(feats) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
-                 "pool: feats and out must be 16-byte aligned (float4 access)");
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, "pool", "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(out, 16, "pool", "out", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, "pool", "n_valid", "int32 access");
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   dim3 grid(cdiv(D, 128), B);

@@ -520,6 +520,17 @@ static bool carve_index(void* blob, size_t bytes, int64_t capacity, int Dv, int 
   return v->hi && (split || v->lo) && v->sq && v->dn && v->hdr;
 }
 
+// An index blob (resident or split, and a split index's host lo array) is written as float4 / uint2 rows, read by the
+// score GEMM's TMA (gemm_tc_supported's 16-byte test) and as uint4 by the rescoring and the split gather: every entry
+// that takes one requires 16 bytes, so a blob one of them would refuse is refused by all.
+#define ANYLOC_REQUIRE_BLOB(p, who, name) ANYLOC_REQUIRE_ALIGNED(p, 16, who, name, "float4, uint4 and TMA access")
+// a search's outputs: fp32 distances and int64 indices, one element at a time
+static int search_out_alignment(const char* who, const float* dist, const int64_t* idx) {
+  ANYLOC_REQUIRE_ALIGNED(dist, 4, who, "dist", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(idx, 8, who, "idx", "int64 access");
+  return ANYLOC_OK;
+}
+
 extern "C" size_t anyloc_index_bytes(int64_t capacity, int Dv, int normalize) {
   const size_t esz = index_uses_f16(Dv, normalize) ? 2 : 4;
   return 2 * align_up((size_t)capacity * Dv * esz, 256) + 2 * align_up((size_t)capacity * 4, 256) + 256 + 256;
@@ -528,6 +539,7 @@ extern "C" size_t anyloc_index_bytes(int64_t capacity, int Dv, int normalize) {
 // A fresh blob must be initialised once (clears the header) before the first anyloc_index_add.
 extern "C" int anyloc_index_init(void* index, size_t index_bytes, int64_t capacity, int Dv, int normalize, void* stream) {
   ANYLOC_REQUIRE(index, "index_init: null pointer");
+  ANYLOC_REQUIRE_BLOB(index, "index_init", "index");
   IndexView v;
   if (!carve_index(index, index_bytes, capacity, Dv, normalize, &v)) { set_error("index_init: blob too small"); return ANYLOC_ERR_WORKSPACE; }
   ANYLOC_CHECK_CUDA(cudaMemsetAsync(v.hdr, 0, 256, (cudaStream_t)stream));
@@ -540,6 +552,8 @@ extern "C" int anyloc_index_add(void* index, size_t index_bytes, int64_t capacit
   ANYLOC_REQUIRE(n_rows >= 0 && Dv > 0 && Dv % 4 == 0 && row_offset >= 0 && row_offset + n_rows <= capacity,
                  "index_add: bad dims n_rows=%d Dv=%d offset=%lld capacity=%lld", n_rows, Dv, (long long)row_offset,
                  (long long)capacity);
+  ANYLOC_REQUIRE_BLOB(index, "index_add", "index");
+  ANYLOC_REQUIRE_ALIGNED(rows, 16, "index_add", "rows", "float4 access");
   IndexView v;
   if (!carve_index(index, index_bytes, capacity, Dv, normalize, &v)) {
     set_error("index_add: blob too small (%zu given, %zu needed)", index_bytes, anyloc_index_bytes(capacity, Dv, normalize));
@@ -563,6 +577,8 @@ extern "C" int anyloc_index_add(void* index, size_t index_bytes, int64_t capacit
 extern "C" int anyloc_index_copy(void* dst, size_t dst_bytes, int64_t dst_capacity, const void* src, size_t src_bytes,
                                  int64_t src_capacity, int64_t n_rows, int Dv, int normalize, void* stream) {
   ANYLOC_REQUIRE(dst && src && n_rows >= 0 && n_rows <= src_capacity && n_rows <= dst_capacity, "index_copy: bad arguments");
+  ANYLOC_REQUIRE_BLOB(dst, "index_copy", "dst");
+  ANYLOC_REQUIRE_BLOB(src, "index_copy", "src");
   IndexView d, s;
   if (!carve_index(dst, dst_bytes, dst_capacity, Dv, normalize, &d) ||
       !carve_index(const_cast<void*>(src), src_bytes, src_capacity, Dv, normalize, &s)) {
@@ -679,6 +695,11 @@ extern "C" int anyloc_index_search(const void* index, size_t index_bytes, int64_
                  "index_search: bad dims n_db=%lld n_q=%d Dv=%d k=%d", (long long)n_db, n_q, Dv, k);
   ANYLOC_REQUIRE(Dv % 4 == 0, "index_search: Dv=%d must be a multiple of 4", Dv);
   ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "index_search: unknown metric %d", metric);
+  ANYLOC_REQUIRE_BLOB(index, "index_search", "index");
+  ANYLOC_REQUIRE_ALIGNED(qu, 16, "index_search", "qu", "float4 access");
+  ANYLOC_REQUIRE_BLOB(ws, "index_search", "ws");
+  const int rc = search_out_alignment("index_search", dist, idx);
+  if (rc) return rc;
   if (n_q == 0) return ANYLOC_OK;
   IndexView v;
   if (!carve_index(const_cast<void*>(index), index_bytes, capacity, Dv, normalize, &v)) {
@@ -704,6 +725,11 @@ extern "C" int anyloc_index_search_continue(const void* index, size_t index_byte
   ANYLOC_REQUIRE(Dv % 4 == 0, "index_search_continue: Dv=%d must be a multiple of 4", Dv);
   ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "index_search_continue: unknown metric %d",
                  metric);
+  ANYLOC_REQUIRE_BLOB(index, "index_search_continue", "index");
+  ANYLOC_REQUIRE_ALIGNED(qu, 16, "index_search_continue", "qu", "float4 access");
+  ANYLOC_REQUIRE_BLOB(ws, "index_search_continue", "ws");
+  const int rc = search_out_alignment("index_search_continue", dist, idx);
+  if (rc) return rc;
   if (n_q == 0) return ANYLOC_OK;
   IndexView v;
   if (!carve_index(const_cast<void*>(index), index_bytes, capacity, Dv, normalize, &v)) {
@@ -740,6 +766,7 @@ extern "C" int anyloc_index_split_init(void* index, size_t index_bytes, int64_t 
   ANYLOC_REQUIRE(index && capacity >= 0 && Dv > 0 && Dv % 8 == 0,
                  "index_split_init: bad arguments (capacity=%lld, Dv=%d must be a positive multiple of 8)",
                  (long long)capacity, Dv);
+  ANYLOC_REQUIRE_BLOB(index, "index_split_init", "index");
   IndexView v;
   if (!split_carve(index, index_bytes, capacity, Dv, &v)) { set_error("index_split_init: blob too small"); return ANYLOC_ERR_WORKSPACE; }
   ANYLOC_CHECK_CUDA(cudaMemsetAsync(v.hdr, 0, 256, (cudaStream_t)stream));
@@ -750,6 +777,8 @@ extern "C" int anyloc_index_split_copy(void* dst, size_t dst_bytes, int64_t dst_
                                        size_t src_bytes, int64_t src_capacity, int64_t n_rows, int Dv, void* stream) {
   ANYLOC_REQUIRE(dst && src && n_rows >= 0 && n_rows <= src_capacity && n_rows <= dst_capacity && Dv > 0 && Dv % 8 == 0,
                  "index_split_copy: bad arguments");
+  ANYLOC_REQUIRE_BLOB(dst, "index_split_copy", "dst");
+  ANYLOC_REQUIRE_BLOB(src, "index_split_copy", "src");
   IndexView d, s;
   if (!split_carve(dst, dst_bytes, dst_capacity, Dv, &d) || !split_carve(src, src_bytes, src_capacity, Dv, &s)) {
     set_error("index_split_copy: blob too small");
@@ -769,6 +798,9 @@ extern "C" int anyloc_index_split_add(void* index, size_t index_bytes, int64_t c
   ANYLOC_REQUIRE(n_rows >= 0 && Dv > 0 && Dv % 8 == 0 && row_offset >= 0 && row_offset + n_rows <= capacity,
                  "index_split_add: bad dims n_rows=%d Dv=%d (a multiple of 8) offset=%lld capacity=%lld", n_rows, Dv,
                  (long long)row_offset, (long long)capacity);
+  ANYLOC_REQUIRE_BLOB(index, "index_split_add", "index");
+  ANYLOC_REQUIRE_BLOB(lo, "index_split_add", "lo");
+  ANYLOC_REQUIRE_ALIGNED(rows, 16, "index_split_add", "rows", "float4 access");
   IndexView v;
   if (!split_carve(index, index_bytes, capacity, Dv, &v)) {
     set_error("index_split_add: blob too small (%zu given, %zu needed)", index_bytes, anyloc_index_split_bytes(capacity, Dv));
@@ -793,6 +825,9 @@ extern "C" int anyloc_index_split_piece(void* dst, size_t dst_bytes, int64_t dst
                  Dv > 0 && Dv % 8 == 0, "index_split_piece: bad arguments first=%lld n_rows=%lld capacity=%lld "
                  "dst_capacity=%lld Dv=%d", (long long)first, (long long)n_rows, (long long)capacity,
                  (long long)dst_capacity, Dv);
+  ANYLOC_REQUIRE_BLOB(dst, "index_split_piece", "dst");
+  ANYLOC_REQUIRE_BLOB(index, "index_split_piece", "index");
+  ANYLOC_REQUIRE_BLOB(lo, "index_split_piece", "lo");
   IndexView d, s;
   if (!carve_index(dst, dst_bytes, dst_capacity, Dv, 1, &d) || !split_carve(index, index_bytes, capacity, Dv, &s)) {
     set_error("index_split_piece: blob too small");
@@ -913,6 +948,10 @@ extern "C" int anyloc_index_split_search(const void* index, size_t index_bytes, 
                                          const float* qu, int n_q, int Dv, int k, void* ws, size_t ws_bytes,
                                          int64_t* counts, void* stream) {
   ANYLOC_REQUIRE(index && qu && ws && counts, "index_split_search: null pointer");
+  ANYLOC_REQUIRE_BLOB(index, "index_split_search", "index");
+  ANYLOC_REQUIRE_ALIGNED(qu, 16, "index_split_search", "qu", "float4 access");
+  ANYLOC_REQUIRE_BLOB(ws, "index_split_search", "ws");
+  ANYLOC_REQUIRE_ALIGNED(counts, 8, "index_split_search", "counts", "int64 host array");
   counts[0] = -1; counts[1] = 0;
   ANYLOC_REQUIRE(n_db > 0 && n_db <= capacity && n_db < (1ll << 31) && n_q >= 0 && Dv > 0 && Dv % 8 == 0 && k > 0,
                  "index_split_search: bad dims n_db=%lld n_q=%d Dv=%d (a multiple of 8) k=%d", (long long)n_db, n_q,
@@ -967,6 +1006,12 @@ extern "C" int anyloc_index_split_rescore(const void* index, size_t index_bytes,
                  k <= COARSE_K_MAX && n_unique >= 0 && n_unique <= std::min<int64_t>(n_db, (int64_t)n_q * CAND_MAX),
                  "index_split_rescore: bad dims n_db=%lld n_q=%d Dv=%d k=%d n_unique=%lld", (long long)n_db, n_q, Dv,
                  k, (long long)n_unique);
+  ANYLOC_REQUIRE_BLOB(index, "index_split_rescore", "index");
+  ANYLOC_REQUIRE_BLOB(lo, "index_split_rescore", "lo");
+  ANYLOC_REQUIRE_BLOB(ws, "index_split_rescore", "ws");
+  ANYLOC_REQUIRE_BLOB(stage, "index_split_rescore", "stage");
+  const int rc = search_out_alignment("index_split_rescore", dist, idx);
+  if (rc) return rc;
   IndexView v;
   SplitWs w;
   if (!split_carve(index, index_bytes, capacity, Dv, &v) || !carve_split_search(ws, ws_bytes, n_db, n_q, Dv, &w)) {
@@ -1021,6 +1066,11 @@ extern "C" int anyloc_topk(const float* db, const float* qu, int n_db, int n_q, 
   ANYLOC_REQUIRE(n_db > 0 && n_q >= 0 && Dv > 0 && k > 0, "topk: bad dims n_db=%d n_q=%d Dv=%d k=%d", n_db, n_q, Dv, k);
   ANYLOC_REQUIRE(Dv % 4 == 0, "topk: Dv=%d must be a multiple of 4", Dv);
   ANYLOC_REQUIRE(metric == ANYLOC_METRIC_IP || metric == ANYLOC_METRIC_L2, "topk: unknown metric %d", metric);
+  ANYLOC_REQUIRE_ALIGNED(db, 16, "topk", "db", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(qu, 16, "topk", "qu", "float4 access");
+  ANYLOC_REQUIRE_BLOB(ws, "topk", "ws");
+  int rc = search_out_alignment("topk", dist, idx);
+  if (rc) return rc;
   if (n_q == 0) return ANYLOC_OK;
   const size_t ib = anyloc_index_bytes(n_db, Dv, normalize);
   // the documented size, whichever pair format this call picks (it covers the carve below in every case)
@@ -1029,7 +1079,7 @@ extern "C" int anyloc_topk(const float* db, const float* qu, int n_db, int n_q, 
     set_error("topk: workspace too small (%zu given, %zu needed)", ws_bytes, need);
     return ANYLOC_ERR_WORKSPACE;
   }
-  int rc = anyloc_index_init(ws, ib, n_db, Dv, normalize, stream);
+  rc = anyloc_index_init(ws, ib, n_db, Dv, normalize, stream);
   if (rc) return rc;
   if ((rc = anyloc_index_add(ws, ib, n_db, 0, db, n_db, Dv, normalize, stream))) return rc;
   char* rest = (char*)ws + align_up(ib, 256);

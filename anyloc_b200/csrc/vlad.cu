@@ -1594,6 +1594,30 @@ int launch_normalize(float* vlad, const float* partial, int B, int D, int K, int
   ANYLOC_CHECK_LAUNCH();
   return ANYLOC_OK;
 }
+
+// The pointers every hard assignment hands its kernels.  feats and the workspace (c^, its tf32 copy, the bias and the
+// coarse scores) must pass gemm_tc_supported's 16-byte test, so that the route -- and with it the labels at near-ties --
+// never depends on where an accepted buffer sits; the FFMA and rescoring kernels read feats and c^ as float4 too.
+static int assign_alignment(const char* who, const float* feats, const int32_t* labels, const void* ws) {
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, who, "feats", "float4 and TMA access");
+  ANYLOC_REQUIRE_ALIGNED(labels, 4, who, "labels", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, who, "ws", "float4 and TMA access");
+  return ANYLOC_OK;
+}
+
+// The hard generates add the accumulations' float4 reads of the centres and float4 stores of the descriptors; a
+// prepared blob stands in for the workspace's c^ and tf32 copy, so it needs what the workspace needs.
+static int generate_alignment(const char* who, const float* feats, const int32_t* n_valid, const float* centers,
+                              const void* prepared, const float* vlad, const int32_t* labels_out, const void* ws) {
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, who, "feats", "float4 and TMA access");
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, who, "n_valid", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(centers, 16, who, "centers", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(prepared, 16, who, "prepared", "float4 and TMA access");
+  ANYLOC_REQUIRE_ALIGNED(vlad, 16, who, "vlad", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(labels_out, 4, who, "labels", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, who, "ws", "float4 and TMA access");
+  return ANYLOC_OK;
+}
 }  // namespace
 
 extern "C" size_t anyloc_vlad_workspace_bytes(int B, int N, int D, int K) {
@@ -1606,6 +1630,9 @@ extern "C" int anyloc_vlad_assign(const float* feats, const float* centers, int 
                                   void* stream) {
   ANYLOC_REQUIRE(feats && centers && labels && ws, "vlad_assign: null pointer");
   ANYLOC_REQUIRE(R >= 0 && D > 0 && K > 0 && D % 4 == 0, "vlad_assign: bad dims R=%d D=%d K=%d", R, D, K);
+  int rc = assign_alignment("vlad_assign", feats, labels, ws);
+  if (rc) return rc;
+  ANYLOC_REQUIRE_ALIGNED(centers, 4, "vlad_assign", "centers", "fp32 access");
   if (R == 0) return ANYLOC_OK;
   Workspace w(ws, ws_bytes);
   AssignBufs ab;
@@ -1653,8 +1680,13 @@ extern "C" int anyloc_vlad_assign_multi(const float* feats, int64_t R, int D, in
                  "vlad_assign_multi: bad dims R=%lld D=%d V=%d", (long long)R, D, V);
   ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
                  "vlad_assign_multi: unknown dist_mode %d", dist_mode);
-  for (int v = 0; v < V; ++v)
+  for (int v = 0; v < V; ++v) {
     ANYLOC_REQUIRE(K[v] > 0 && centers[v], "vlad_assign_multi: vocabulary %d has K=%d or no centres", v, K[v]);
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(centers[v]) & 3) == 0,
+                   "vlad_assign_multi: centers[%d] must be 4-byte aligned (fp32 access)", v);
+  }
+  const int rc0 = assign_alignment("vlad_assign_multi", feats, labels, ws);
+  if (rc0) return rc0;
   const int64_t Ksum = assign_multi_ksum(V, K);
   ANYLOC_REQUIRE(Ksum < (1ll << 31), "vlad_assign_multi: %lld centres in all", (long long)Ksum);
   if (R == 0) return ANYLOC_OK;
@@ -1750,6 +1782,9 @@ extern "C" int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_
   ANYLOC_REQUIRE(D > 0 && K > 0 && D % 4 == 0, "vlad_prepare: bad dims D=%d K=%d", D, K);
   ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
                  "vlad_prepare: unknown dist_mode %d", dist_mode);
+  // the blob's readers (the generates' assignment) need 16 bytes, so a blob they would refuse is refused here
+  ANYLOC_REQUIRE_ALIGNED(centers, 4, "vlad_prepare", "centers", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(prepared, 16, "vlad_prepare", "prepared", "float4 and TMA access");
   PreparedView pv;
   if (!carve_prepared(prepared, prepared_bytes, D, K, &pv)) { set_error("vlad_prepare: blob too small"); return ANYLOC_ERR_WORKSPACE; }
   vlad_centre_prep_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(centers, K, D, dist_mode, pv.chat, pv.cbias, pv.chat_tf32,
@@ -1780,6 +1815,9 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   ANYLOC_REQUIRE(D % 4 == 0, "vlad_generate: D=%d must be a multiple of 4", D);
   ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
                  "vlad_generate: unknown dist_mode %d", dist_mode);
+  int rc = generate_alignment(prepared ? "vlad_generate_prepared" : "vlad_generate", feats, n_valid, centers, prepared,
+                              vlad, labels_out, ws);
+  if (rc) return rc;
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
@@ -1803,8 +1841,7 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   const bool use_prep = prepared && carve_prepared(prepared, prepared_bytes, D, K, &pv);
   if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
-  int rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st,
-                         use_prep);
+  rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
   if (rc) return rc;
   if (acc3) {
     static unsigned long long attr_seen = 0;
@@ -1893,6 +1930,8 @@ extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_
                  "vlad_generate_sorted: unknown dist_mode %d", dist_mode);
   const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
   ANYLOC_REQUIRE(B <= 65535 && ztasks <= 65535, "vlad_generate_sorted: B=%d N=%d K=%d exceed the launch grid", B, N, K);
+  int rc = generate_alignment("vlad_generate_sorted", feats, n_valid, centers, prepared, vlad, labels_out, ws);
+  if (rc) return rc;
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
@@ -1910,8 +1949,7 @@ extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_
   const size_t R = (size_t)B * N;
   const int nslices = cdiv(D, ACC_COLS);
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
-  int rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st,
-                         use_prep);
+  rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
   if (rc) return rc;
   vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, N, D, K, norm_descs, tb);
   ANYLOC_CHECK_LAUNCH();
@@ -1957,6 +1995,14 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   ANYLOC_REQUIRE(B >= 0 && N >= 0 && D > 0 && K > 0, "vlad_generate_soft: bad dims");
   ANYLOC_REQUIRE(D % 4 == 0, "vlad_generate_soft: D=%d must be a multiple of 4", D);
   ANYLOC_REQUIRE(K <= 2048, "vlad_generate_soft: K=%d > 2048", K);
+  // the soft assignment reads feats and c^ (workspace) as float4; the accumulation reads the centres and writes the
+  // descriptors one fp32 at a time
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, "vlad_generate_soft", "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, "vlad_generate_soft", "n_valid", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(centers, 4, "vlad_generate_soft", "centers", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(vlad, 4, "vlad_generate_soft", "vlad", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(assign_out, 4, "vlad_generate_soft", "assign", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, "vlad_generate_soft", "ws", "float4 access");
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
@@ -2018,9 +2064,10 @@ int varlen_args(const char* who, const float* feats, int64_t R, const int64_t* r
                  "%s: bad dims B=%d R=%lld D=%d K=%d (B <= 65535, R < 2^31, D a multiple of 4)", who, B, (long long)R,
                  D, K);
   ANYLOC_REQUIRE(feats && row0 && len && vlad, "%s: null pointer", who);
-  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(feats) | reinterpret_cast<uintptr_t>(vlad)) & 15) == 0 &&
-                     (reinterpret_cast<uintptr_t>(row0) & 7) == 0 && (reinterpret_cast<uintptr_t>(len) & 3) == 0,
-                 "%s: feats and vlad must be 16-byte aligned (float4 access), row0 8-byte and len 4-byte", who);
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, who, "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(row0, 8, who, "row0", "int64 access");
+  ANYLOC_REQUIRE_ALIGNED(len, 4, who, "len", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(vlad, 16, who, "vlad", "float4 access");
   return ANYLOC_OK;
 }
 
@@ -2052,6 +2099,8 @@ extern "C" int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const 
   ANYLOC_REQUIRE(centers && ws, "vlad_generate_varlen: null pointer");
   ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN,
                  "vlad_generate_varlen: unknown dist_mode %d", dist_mode);
+  rc = generate_alignment("vlad_generate_varlen", feats, nullptr, centers, prepared, vlad, labels_out, ws);
+  if (rc) return rc;
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   int N = 0;                                        // the padded batch's row count: the longest image
@@ -2147,6 +2196,9 @@ extern "C" int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, c
   if (rc) return rc;
   ANYLOC_REQUIRE(centers && ws, "vlad_generate_soft_varlen: null pointer");
   ANYLOC_REQUIRE(K <= 2048, "vlad_generate_soft_varlen: K=%d > 2048", K);
+  ANYLOC_REQUIRE_ALIGNED(centers, 4, "vlad_generate_soft_varlen", "centers", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(assign_out, 4, "vlad_generate_soft_varlen", "assign", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, "vlad_generate_soft_varlen", "ws", "float4 access");
   if (B == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   int N = 0;
@@ -2192,6 +2244,19 @@ static int kmeans_chunks(int64_t R, int D) {
 constexpr int KMEANS_FIN_BLOCKS = 64;
 
 namespace {
+// Every k-means kernel reads and writes one fp32 or int32 at a time, the workspace's sums and counts included, so 4
+// bytes is the whole contract.  Null pointers are the ones the entry does not take.
+int kmeans_alignment(const char* who, const float* x, const int32_t* labels, const float* old_centers,
+                     const float* new_centers, const float* err_out, const void* ws) {
+  ANYLOC_REQUIRE_ALIGNED(x, 4, who, "x", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(labels, 4, who, "labels", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(old_centers, 4, who, "old_centers", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(new_centers, 4, who, "new_centers", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(err_out, 4, who, "err_out", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 4, who, "ws", "fp32 access");
+  return ANYLOC_OK;
+}
+
 struct KmeansBufs { float *psums, *pcounts, *perr; int chunks; };
 bool take_kmeans_bufs(void* ws, size_t ws_bytes, int64_t R, int D, int K, KmeansBufs* b) {
   b->chunks = kmeans_chunks(R, D);
@@ -2224,6 +2289,8 @@ extern "C" int anyloc_kmeans_accumulate_round(const float* x, const int32_t* lab
                                               int64_t piece_rows, int D, int K, int resume, void* ws, size_t ws_bytes,
                                               void* stream) {
   ANYLOC_REQUIRE(x && labels && ws, "kmeans_accumulate_round: null pointer");
+  int rc = kmeans_alignment("kmeans_accumulate_round", x, labels, nullptr, nullptr, nullptr, ws);
+  if (rc) return rc;
   ANYLOC_REQUIRE(R >= 0 && D > 0 && K > 0 && piece_rows >= 0 && round_rows >= 0,
                  "kmeans_accumulate_round: bad dims R=%lld D=%d K=%d", (long long)R, D, K);
   KmeansBufs b;
@@ -2250,6 +2317,8 @@ extern "C" int anyloc_kmeans_accumulate_round(const float* x, const int32_t* lab
 extern "C" int anyloc_kmeans_finalize(const float* old_centers, int64_t R, int D, int K, float* new_centers,
                                       float* err_out, void* ws, size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(old_centers && new_centers && err_out && ws, "kmeans_finalize: null pointer");
+  int rc = kmeans_alignment("kmeans_finalize", nullptr, nullptr, old_centers, new_centers, err_out, ws);
+  if (rc) return rc;
   KmeansBufs b;
   if (!take_kmeans_bufs(ws, ws_bytes, R, D, K, &b)) {
     set_error("kmeans_finalize: workspace too small (%zu given, %zu needed)", ws_bytes,
@@ -2269,9 +2338,11 @@ extern "C" int anyloc_kmeans_update(const float* x, const int32_t* labels, const
                                     int R, int D, int K, float* new_centers, float* err_out, void* ws,
                                     size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(x && labels && old_centers && new_centers && err_out && ws, "kmeans_update: null pointer");
+  int rc = kmeans_alignment("kmeans_update", x, labels, old_centers, new_centers, err_out, ws);
+  if (rc) return rc;
   int chunks;
   int64_t rows_per;
-  int rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
+  rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
   if (!rc) rc = anyloc_kmeans_accumulate_round(x, labels, R, R, rows_per, D, K, 0, ws, ws_bytes, stream);
   if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
   return rc;
@@ -2284,6 +2355,8 @@ extern "C" int anyloc_kmeans_accumulate_round_tiled(const float* x, const int32_
                                                     int64_t piece_rows, int D, int K, int k_tile, int resume, void* ws,
                                                     size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(x && labels && ws, "kmeans_accumulate_round_tiled: null pointer");
+  int rc = kmeans_alignment("kmeans_accumulate_round_tiled", x, labels, nullptr, nullptr, nullptr, ws);
+  if (rc) return rc;
   ANYLOC_REQUIRE(R >= 0 && D > 0 && K > 0 && piece_rows >= 0 && round_rows >= 0,
                  "kmeans_accumulate_round_tiled: bad dims R=%lld D=%d K=%d", (long long)R, D, K);
   ANYLOC_REQUIRE(k_tile >= 0 && k_tile <= KMEANS_MAX_TILE, "kmeans_accumulate_round_tiled: k_tile=%d not in [0, %d]",
@@ -2314,9 +2387,11 @@ extern "C" int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels,
                                           int D, int K, int k_tile, float* new_centers, float* err_out, void* ws,
                                           size_t ws_bytes, void* stream) {
   ANYLOC_REQUIRE(x && labels && old_centers && new_centers && err_out && ws, "kmeans_update_tiled: null pointer");
+  int rc = kmeans_alignment("kmeans_update_tiled", x, labels, old_centers, new_centers, err_out, ws);
+  if (rc) return rc;
   int chunks;
   int64_t rows_per;
-  int rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
+  rc = anyloc_kmeans_partition(R, D, &chunks, &rows_per);
   if (!rc) rc = anyloc_kmeans_accumulate_round_tiled(x, labels, R, R, rows_per, D, K, k_tile, 0, ws, ws_bytes, stream);
   if (!rc) rc = anyloc_kmeans_finalize(old_centers, R, D, K, new_centers, err_out, ws, ws_bytes, stream);
   return rc;
@@ -2327,8 +2402,15 @@ extern "C" int anyloc_kmeans_accumulate_round_multi(const float* x, int V, const
                                                     int resume, void* const* ws, const size_t* ws_bytes,
                                                     void* stream) {
   ANYLOC_REQUIRE(x && labels && K && ws && ws_bytes, "kmeans_accumulate_round_multi: null pointer");
+  ANYLOC_REQUIRE_ALIGNED(x, 4, "kmeans_accumulate_round_multi", "x", "fp32 access");
   ANYLOC_REQUIRE(V > 0 && R >= 0 && D > 0 && piece_rows >= 0 && round_rows >= 0,
                  "kmeans_accumulate_round_multi: bad dims V=%d R=%lld D=%d", V, (long long)R, D);
+  for (int v = 0; v < V; ++v) {
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(labels[v]) & 3) == 0,
+                   "kmeans_accumulate_round_multi: labels[%d] must be 4-byte aligned (int32 access)", v);
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(ws[v]) & 3) == 0,
+                   "kmeans_accumulate_round_multi: ws[%d] must be 4-byte aligned (fp32 access)", v);
+  }
   std::vector<KmeansBufs> b(V);
   for (int v = 0; v < V; ++v) {
     ANYLOC_REQUIRE(labels[v] && K[v] > 0, "kmeans_accumulate_round_multi: vocabulary %d has K=%d or no labels", v, K[v]);
@@ -2474,6 +2556,9 @@ extern "C" int anyloc_vlad_residuals(const float* feats, const float* centers, i
                                      float* out, void* stream) {
   ANYLOC_REQUIRE(feats && centers && out, "vlad_residuals: null pointer");
   ANYLOC_REQUIRE(N >= 0 && D > 0 && K > 0 && D % 4 == 0, "vlad_residuals: bad dims N=%d D=%d K=%d", N, D, K);
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, "vlad_residuals", "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(centers, 16, "vlad_residuals", "centers", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(out, 16, "vlad_residuals", "out", "float4 access");
   if (N == 0) return ANYLOC_OK;
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)N * D + (double)K * D + (double)N * K * D));
@@ -2491,6 +2576,12 @@ extern "C" int anyloc_vlad_from_residuals(const float* resid, const int32_t* lab
   ANYLOC_REQUIRE(resid && vlad && ws, "vlad_from_residuals: null pointer");
   ANYLOC_REQUIRE((labels != nullptr) != (assign != nullptr), "vlad_from_residuals: pass labels (hard) OR assign (soft)");
   ANYLOC_REQUIRE(N >= 0 && D > 0 && K > 0, "vlad_from_residuals: bad dims N=%d D=%d K=%d", N, D, K);
+  // scalar kernels throughout (the normalisation included)
+  ANYLOC_REQUIRE_ALIGNED(resid, 4, "vlad_from_residuals", "resid", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(labels, 4, "vlad_from_residuals", "labels", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(assign, 4, "vlad_from_residuals", "assign", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(vlad, 4, "vlad_from_residuals", "vlad", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 4, "vlad_from_residuals", "ws", "fp32 access");
   cudaStream_t st = (cudaStream_t)stream;
   const int nslices = cdiv(D, ACC_COLS);
   Workspace w(ws, ws_bytes);

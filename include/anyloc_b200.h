@@ -114,6 +114,10 @@ int anyloc_profile_read(double* ms, long long* groups, double* work);
  * feats [B,N,D] fp32 row-major, n_valid [B] (nullable; rows >= n_valid[b] ignored, ragged lists),
  * centers [K,D], vlad [B,K*D], labels [B,N] int32 (nullable; -1 for ignored rows).
  */
+/* Alignment (each entry below refuses a pointer short of it with ANYLOC_ERR_ARG, before anything runs, even with
+ * nothing to do): feats, centers, vlad, ws and a prepared blob 16-byte (float4 rows; feats and the workspace's centre
+ * copies also feed the tensor-core assignment, whose TMA needs 16 bytes, so an accepted buffer never changes the
+ * route); n_valid and labels 4-byte. */
 size_t anyloc_vlad_workspace_bytes(int B, int N, int D, int K);
 int anyloc_vlad_generate(const float* feats, const int32_t* n_valid, const float* centers,
                          int B, int N, int D, int K, int dist_mode, int norm_descs, int intra_norm,
@@ -125,6 +129,8 @@ int anyloc_vlad_generate(const float* feats, const int32_t* n_valid, const float
  * is anyloc_vlad_generate minus the per-call centre-prep launch, on every route.  It only reads the blob, so concurrent
  * calls may share one once anyloc_vlad_prepare has completed; the blob must be re-prepared whenever the centres (or dist_mode) change.  Results are
  * bitwise identical to anyloc_vlad_generate. */
+/* Alignment: anyloc_vlad_prepare centers 4-byte, prepared 16-byte (what its readers need); _prepared as
+ * anyloc_vlad_generate, prepared 16-byte. */
 size_t anyloc_vlad_prepared_bytes(int D, int K);
 int anyloc_vlad_prepare(const float* centers, int D, int K, int dist_mode, void* prepared, size_t prepared_bytes,
                         void* stream);
@@ -140,6 +146,7 @@ int anyloc_vlad_generate_prepared(const float* feats, const int32_t* n_valid, co
  * partial sums live in the workspace (anyloc_vlad_sorted_workspace_bytes), and every sum is taken in the order of
  * ACC3, so where ACC3 runs both give bitwise equal descriptors and labels.  Each image's descriptor is independent of
  * the other images of the batch.  No floating-point atomics. */
+/* Alignment of anyloc_vlad_generate_sorted: as anyloc_vlad_generate_prepared. */
 #define ANYLOC_VLAD_ROUTE_ACC3 0
 #define ANYLOC_VLAD_ROUTE_ACC2 1
 #define ANYLOC_VLAD_ROUTE_SORTED 2
@@ -153,6 +160,8 @@ int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_valid, cons
  *   V_k    = sum_q a[q,k] * sum_c (x^_q - c_c)          (the reference weights the residuals to ALL centres by
  *                                                        cluster k's probability, :881-884)
  *   then intra / global normalisation as above.  assign [B,N,K] (nullable) receives a; padded rows get 0. */
+/* Alignment: feats and ws 16-byte (float4 rows of x and of the normalised centres); n_valid, centers, vlad and
+ * assign 4-byte (the accumulation reads and writes one fp32 at a time). */
 int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_valid, const float* centers,
                               int B, int N, int D, int K, float soft_temp, int norm_descs, int intra_norm,
                               float* vlad, float* assign, void* ws, size_t ws_bytes, void* stream);
@@ -169,6 +178,8 @@ int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_valid, const 
  * labels [R] int32 (nullable): the padded call's label of each image row, -1 for rows of no image.  The soft form's
  * assign [R,K] (nullable) likewise: each image row's probabilities, 0 for rows of no image.  Workspaces:
  * anyloc_vlad_varlen_workspace_bytes(R, B, max len, D, K) and anyloc_vlad_soft_varlen_workspace_bytes(R, B, D, K). */
+/* Alignment: the padded entries' (anyloc_vlad_generate_prepared / anyloc_vlad_generate_soft) plus row0 8-byte, len
+ * 4-byte; the soft form's vlad stays 16-byte. */
 size_t anyloc_vlad_varlen_workspace_bytes(int64_t R, int B, int max_len, int D, int K);
 int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B,
                                 const float* centers, void* prepared, size_t prepared_bytes, int D, int K, int dist_mode,
@@ -182,20 +193,25 @@ int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, const int64_
 /* Residual tensor of VLAD.generate_res_vec (utilities.py:928-972): out[q,k,:] = x^_q - c_k for ALL (patch, centre)
  * pairs, [N,K,D] fp32 (x^ = F.normalize(x) when norm_descs).  The reference builds every descriptor from this tensor
  * and caches it per image (`<cache_id>_r.pt`); here it is only materialised when a caller asks for it. */
+/* Alignment: feats, centers and out 16-byte (float4). */
 int anyloc_vlad_residuals(const float* feats, const float* centers, int N, int D, int K, int norm_descs,
                           float* out, void* stream);
 /* Descriptor of ONE image from a residual tensor [N,K,D] plus either the hard labels [N] int32 (utilities.py:853-861)
  * or the soft assignment [N,K] (:879-887) -- the reference's cache path (`_r.pt` + `_l.pt` / `_s.pt`, :843-852,
  * :864-878), which needs no features.  Pass exactly one of labels / assign.  vlad [K*D]. */
+/* Alignment: every pointer 4-byte (scalar kernels). */
 size_t anyloc_vlad_from_residuals_workspace_bytes(int D, int K);
 int anyloc_vlad_from_residuals(const float* resid, const int32_t* labels, const float* assign, int N, int D, int K,
                                int intra_norm, float* vlad, void* ws, size_t ws_bytes, void* stream);
 /* labels only (fpk.KMeans.predict, utilities.py:849; also one Lloyd assignment step of VLAD.fit :786) */
+/* Alignment: feats and ws 16-byte (as anyloc_vlad_generate), centers and labels 4-byte (the centre prep reads fp32). */
 int anyloc_vlad_assign(const float* feats, const float* centers, int R, int D, int K, int dist_mode,
                        int32_t* labels, void* ws, size_t ws_bytes, void* stream);
 /* one Lloyd centroid update of fpk.KMeans.fit (utilities.py:786): new_c[k] = mean of members
  * (0 for empty clusters); err_out[0] = sum((new_c - old_c)^2).  Deterministic (per-chunk partial sums added in a
  * fixed order, no floating-point atomics).  Workspace: anyloc_kmeans_workspace_bytes(R, D, K). */
+/* Alignment of every k-means entry (update, _tiled, the rounds, _multi's labels[v] and ws[v], finalize): every pointer
+ * 4-byte; the kernels read and write one fp32 / int32 at a time. */
 size_t anyloc_kmeans_workspace_bytes(int R, int D, int K);
 int anyloc_kmeans_update(const float* x, const int32_t* labels, const float* old_centers, int R, int D,
                          int K, float* new_centers, float* err_out, void* ws, size_t ws_bytes,
@@ -240,6 +256,8 @@ int anyloc_kmeans_update_tiled(const float* x, const int32_t* labels, const floa
  * bitwise the same, and anyloc_kmeans_finalize finishes each one.  It reads each row once per launch; consecutive
  * vocabularies share a launch while their sums and counts fit 220 KB of shared memory.  It refuses a K[v] that the
  * untiled round refuses (K >= 437). */
+/* Alignment of anyloc_vlad_assign_multi: anyloc_vlad_assign's, each centers[v] 4-byte.  K, centers, labels (of
+ * _multi) and ws_bytes are host arrays of pointers / sizes, read on the CPU. */
 size_t anyloc_vlad_assign_multi_workspace_bytes(int64_t R, int D, int V, const int* K);
 int anyloc_vlad_assign_multi(const float* feats, int64_t R, int D, int V, const float* const* centers, const int* K,
                              int dist_mode, int32_t* labels, void* ws, size_t ws_bytes, void* stream);
@@ -253,6 +271,9 @@ int anyloc_kmeans_accumulate_round_multi(const float* x, int V, const int32_t* c
  * sorted best-first, lowest database index first among equal scores.
  * db [n_db,Dv], qu [n_q,Dv] fp32; dist [n_q,k] fp32; idx [n_q,k] int64.
  */
+/* Alignment of every retrieval entry (topk, index_*, index_split_*): db, qu, rows, ws, every index blob (index, dst,
+ * src), a split index's host lo array and the stage 16-byte (float4 / uint4 rows and the score GEMM's TMA); dist
+ * 4-byte; idx and the host counts 8-byte.  A blob or lo array is 16-byte in every entry that takes it. */
 size_t anyloc_topk_workspace_bytes(int n_db, int n_q, int Dv, int k);
 int anyloc_topk(const float* db, const float* qu, int n_db, int n_q, int Dv, int k, int metric,
                 int normalize, float* dist, int64_t* idx, void* ws, size_t ws_bytes, void* stream);
@@ -566,6 +587,7 @@ int anyloc_l2_normalize_rows(const float* x, int64_t rows, int D, int64_t ld_in,
  *
  * anyloc_pca_colsum (utilities.py:522-586, the mean pass): sum[c] += sum_r x[r, c], in fp64.  Workspace
  * anyloc_pca_colsum_workspace_bytes(rows, cols); a short one returns ANYLOC_ERR_WORKSPACE. */
+/* Alignment of the PCA entries: natural, for any ld -- x 4-byte; sum, ws, mu, u, out and a 8-byte. */
 size_t anyloc_pca_colsum_workspace_bytes(int64_t rows, int cols);
 int anyloc_pca_colsum(const float* x, int64_t ld, int64_t rows, int cols, double* sum, void* ws, size_t ws_bytes,
                       void* stream);
@@ -604,6 +626,7 @@ int anyloc_pca_mirror(double* a, int m, int64_t ld, void* stream);
 #define ANYLOC_POOL_AVG 0
 #define ANYLOC_POOL_MAX 1
 #define ANYLOC_POOL_GEM 2
+/* Alignment: feats and out 16-byte (float4), n_valid 4-byte. */
 int anyloc_pool(const float* feats, const int32_t* n_valid, int B, int N, int D, int mode, float gem_p,
                 int gem_use_abs, float* out, void* stream);
 /* The same pooling of a packed list: feats [R,D], image b = rows [row0[b], row0[b] + len[b]) (row0 [B] int64, len [B]
