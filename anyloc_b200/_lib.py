@@ -120,6 +120,22 @@ _SIGS = {
     "anyloc_kmeans_accumulate_round_multi": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int),
                                                        C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                                        C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_void_p]),
+    "anyloc_vlad_label_multi_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "anyloc_vlad_label_multi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_int64), C.c_int,
+                                          C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                          C.POINTER(C.c_size_t), C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_vlad_soft_assign_multi_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "anyloc_vlad_soft_assign_multi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int,
+                                                C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_float),
+                                                C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_void_p]),
+    "anyloc_vlad_accumulate_workspace_bytes": (C.c_size_t, [C.c_int] * 5),
+    "anyloc_vlad_accumulate": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 6 +
+                               [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "anyloc_vlad_accumulate_varlen": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int] +
+                                      [C.c_void_p] * 4 + [C.c_int] * 4 +
+                                      [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "anyloc_topk_workspace_bytes":(C.c_size_t, [C.c_int] * 4),
     "anyloc_topk": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 6 +
                     [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

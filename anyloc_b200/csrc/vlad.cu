@@ -1843,6 +1843,7 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
   rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
   if (rc) return rc;
+  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
   if (acc3) {
     static unsigned long long attr_seen = 0;
     if (first_use_on_this_device(&attr_seen)) {
@@ -1951,6 +1952,7 @@ extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
   rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
   if (rc) return rc;
+  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
   vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, N, D, K, norm_descs, tb);
   ANYLOC_CHECK_LAUNCH();
   vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, tb,
@@ -2028,6 +2030,7 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, n_valid, N, (int64_t)R, D, K, chat,
                                                                        soft_temp, assign, inv_norm);
   ANYLOC_CHECK_LAUNCH();
+  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
   vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N, D,
                                                                     K, norm_descs, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
@@ -2133,6 +2136,7 @@ extern "C" int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const 
   rc = launch_assign(feats, nullptr, 0, R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep,
                      (int64_t)B * N);
   if (rc) return rc;
+  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
   if (route == ANYLOC_VLAD_ROUTE_ACC3) {
     const size_t smem3 = acc3_smem_bytes(N, K);
     static unsigned long long attr_seen = 0;
@@ -2226,6 +2230,7 @@ extern "C" int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, c
   vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, nullptr, 0, R, D, K, chat, soft_temp,
                                                                        assign, inv_norm);
   ANYLOC_CHECK_LAUNCH();
+  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
   vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm, centers,
                                                                            D, K, norm_descs, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
@@ -2592,4 +2597,549 @@ extern "C" int anyloc_vlad_from_residuals(const float* resid, const int32_t* lab
   else vlad_from_residuals_soft_kernel<<<nslices, ACC_COLS, 0, st>>>(resid, assign, N, D, K, vlad, partial);
   ANYLOC_CHECK_LAUNCH();
   return launch_normalize(vlad, partial, 1, D, K, intra_norm, st);
+}
+
+// ====================================================================================================================
+// Several vocabularies' descriptors from one read of the features (generate_vocabularies).  The per-row passes are
+// shared: anyloc_vlad_label_multi labels each row against every hard vocabulary and writes its 1/|x| once, and
+// anyloc_vlad_soft_assign_multi writes every soft vocabulary's assignment from one read of each row.  Each member's
+// accumulation then runs alone from those per-row results (anyloc_vlad_accumulate / _varlen) with the kernels, route
+// and normalisation its own generate call takes, so every descriptor is bitwise that call's.  The kernels below are
+// new; the existing ones are launched unchanged, by launch_accumulate, whose launch sequences restate the host code of
+// vlad_generate_impl, anyloc_vlad_generate_sorted, anyloc_vlad_generate_varlen and the two soft entries (each of those
+// points back here): a change to one must be made to the other.
+// ====================================================================================================================
+namespace anyloc {
+
+// vlad_rescore_multi_kernel plus what the assignment of a generate call also writes: label -1 for the rows n_valid
+// leaves out of their image (row g of the call is row g % N_per_img of image g / N_per_img) and 1/max(|x|,1e-12).  x,
+// the labels of each segment and inv_norm point at row r0 of the call; R rows from there.
+template <int MAXV>
+__global__ void __launch_bounds__(256)
+vlad_rescore_multi_norm_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid, int N_per_img,
+                               int64_t r0, int64_t R, int D, int ldc, const float* __restrict__ chat,
+                               const float* __restrict__ cbias, const float* __restrict__ cnorm,
+                               const float* __restrict__ coarse /*[R,ldc]*/, const RescoreSegs segs,
+                               float* __restrict__ inv_norm) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (row >= R) return;
+  bool valid = true;
+  if (n_valid) {
+    const int64_t g = r0 + row;
+    valid = (int)(g % N_per_img) < n_valid[(int)(g / N_per_img)];
+  }
+  float4 v[MAXV];
+  const float xn = load_row<MAXV>(x, row, D, lane, v);
+  for (int s = 0; s < segs.n; ++s) {
+    const int k0 = segs.koff[s];
+    const int bestk = rescore_row<MAXV>(v, xn, lane, D, segs.k[s], coarse + row * ldc + k0, chat + (size_t)k0 * D,
+                                        cbias + k0, cnorm + k0);
+    if (lane == 0) segs.labels[s][row] = valid ? bestk : -1;
+  }
+  if (lane == 0 && inv_norm) inv_norm[row] = 1.0f / fmaxf(xn, 1e-12f);
+}
+
+// Soft assignment of several vocabularies whose normalised centres c / max(|c|, 1e-8) sit side by side in chat
+// [sum K, D]: segment s is columns [koff[s], koff[s] + k[s]) with temperature temp[s], written to assign[s] [R, k[s]].
+// It restates vlad_soft_assign_kernel operation for operation: the dot products x.c^ are taken once for all segments
+// (the same FMAs and warp_sum), each segment's temp / max(|x|, 1e-8) multiplies them afterwards, and the max, the
+// exp-sum and the scaling run lane-strided over the segment exactly as over a single vocabulary, so each segment's
+// probabilities are that kernel's bits.  Rows n_valid leaves out get exactly 0 (and inv_norm 0).
+constexpr int SOFT_MULTI_SEGS = 32;
+constexpr int SOFT_MULTI_ROWS = 2;
+constexpr int SOFT_MULTI_SMEM = 232448;                  // H100's opt-in shared memory per block
+struct SoftSegs {
+  int n;
+  int koff[SOFT_MULTI_SEGS], k[SOFT_MULTI_SEGS];
+  float temp[SOFT_MULTI_SEGS];
+  float* assign[SOFT_MULTI_SEGS];
+};
+
+template <int ROWS>
+__global__ void __launch_bounds__(256)
+vlad_soft_assign_multi_kernel(const float* __restrict__ x, const int32_t* __restrict__ n_valid, int N_per_img,
+                              int64_t R, int D, int ksum, const float* __restrict__ chat, const SoftSegs segs,
+                              float* __restrict__ inv_norm) {
+  extern __shared__ float scm_smem[];                  // [warps][ROWS][ksum] raw dot products, then probabilities
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  float* sc = scm_smem + (size_t)wib * ROWS * ksum;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int D4 = D >> 2;
+  for (int64_t r0 = warp * ROWS; r0 < R; r0 += nwarps * ROWS) {
+    const float4* xr[ROWS];
+    bool valid[ROWS];
+#pragma unroll
+    for (int i = 0; i < ROWS; ++i) {
+      int64_t r = r0 + i;
+      valid[i] = r < R;
+      if (valid[i] && n_valid) valid[i] = (int)(r % N_per_img) < n_valid[(int)(r / N_per_img)];
+      xr[i] = reinterpret_cast<const float4*>(x + (r < R ? r : r0) * (int64_t)D);
+    }
+    float ss[ROWS];
+#pragma unroll
+    for (int i = 0; i < ROWS; ++i) ss[i] = 0.f;
+    for (int d = lane; d < D4; d += 32) {
+#pragma unroll
+      for (int i = 0; i < ROWS; ++i) {
+        float4 v = __ldg(xr[i] + d);
+        ss[i] += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < ROWS; ++i) ss[i] = sqrtf(warp_sum(ss[i]));
+    for (int k = 0; k < ksum; ++k) {
+      const float4* cr = reinterpret_cast<const float4*>(chat + (size_t)k * D);
+      float acc[ROWS];
+#pragma unroll
+      for (int i = 0; i < ROWS; ++i) acc[i] = 0.f;
+      for (int d = lane; d < D4; d += 32) {
+        float4 c = __ldg(cr + d);
+#pragma unroll
+        for (int i = 0; i < ROWS; ++i) {
+          float4 v = __ldg(xr[i] + d);
+          acc[i] = fmaf(v.x, c.x, acc[i]); acc[i] = fmaf(v.y, c.y, acc[i]);
+          acc[i] = fmaf(v.z, c.z, acc[i]); acc[i] = fmaf(v.w, c.w, acc[i]);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < ROWS; ++i) {
+        const float s = warp_sum(acc[i]);
+        if (lane == 0) sc[i * ksum + k] = s;
+      }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < ROWS; ++i) {
+      int64_t r = r0 + i;
+      if (r >= R) continue;
+      if (!valid[i]) {        // padded row of a ragged batch: exactly 0, whatever it holds (its scores may be NaN)
+        for (int s = 0; s < segs.n; ++s)
+          for (int k = lane; k < segs.k[s]; k += 32) segs.assign[s][r * segs.k[s] + k] = 0.f;
+        if (lane == 0 && inv_norm) inv_norm[r] = 0.f;
+        continue;
+      }
+      for (int s = 0; s < segs.n; ++s) {
+        const int K = segs.k[s];
+        float* row = sc + i * ksum + segs.koff[s];
+        const float rx = segs.temp[s] / fmaxf(ss[i], 1e-8f);
+        float m = -INFINITY;
+        for (int k = lane; k < K; k += 32) { const float v = row[k] * rx; row[k] = v; m = fmaxf(m, v); }
+        m = warp_max(m);
+        float z = 0.f;
+        for (int k = lane; k < K; k += 32) { float e = expf(row[k] - m); row[k] = e; z += e; }
+        z = warp_sum(z);
+        const float iz = 1.0f / z;
+        float* a = segs.assign[s] + r * K;
+        for (int k = lane; k < K; k += 32) a[k] = row[k] * iz;
+      }
+      if (lane == 0 && inv_norm) inv_norm[r] = 1.0f / fmaxf(ss[i], 1e-12f);
+    }
+    __syncwarp();
+  }
+}
+
+}  // namespace anyloc
+
+namespace {
+// anyloc_vlad_label_multi's workspace: the prepared centres of all vocabularies side by side ([sum K, D] c^, its tf32
+// copy, bias, norms) and, for D <= 2048, one slice of coarse scores.  Unlike anyloc_vlad_assign_multi's, the slice is
+// there for R < 256 too: a member's route rows, not R, decide whether it takes the tensor-core route.  ws == nullptr:
+// dry run.
+size_t carve_label_multi(void* ws, size_t ws_bytes, int64_t R, int D, int64_t Ksum, AssignBufs* ab) {
+  Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  ab->chat = w.take<float>((size_t)Ksum * D);
+  ab->chat_tf32 = w.take<float>((size_t)Ksum * D);
+  ab->cbias = w.take<float>(Ksum);
+  ab->cnorm = w.take<float>(Ksum);
+  const bool coarse = D <= 2048 && R > 0;
+  ab->coarse = coarse ? w.take<float>((size_t)assign_multi_slice(R, Ksum) * Ksum) : nullptr;
+  const bool ok = ab->chat && ab->chat_tf32 && ab->cbias && ab->cnorm && (ab->coarse || !coarse);
+  return ok ? w.off : 0;
+}
+
+// anyloc_vlad_accumulate(_varlen)'s workspace for B images of up to N rows: the per-slice sums of squares, the
+// accumulate3 tickets on that route and the sorted route's per-image tables on that one (route < 0: soft, the sums
+// alone).  ws == nullptr: dry run.
+size_t carve_accumulate(void* ws, size_t ws_bytes, int B, int N, int D, int K, int route, float** partial,
+                        int32_t** done, SortedTables* tb) {
+  Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
+  *partial = w.take<float>((size_t)B * K * cdiv(D, ACC_COLS));
+  *done = route == ANYLOC_VLAD_ROUTE_ACC3 ? w.take<int32_t>((size_t)B) : nullptr;
+  bool ok = *partial && (route != ANYLOC_VLAD_ROUTE_ACC3 || *done);
+  if (route == ANYLOC_VLAD_ROUTE_SORTED) {
+    const size_t R = (size_t)B * N, K1 = (size_t)B * (K + 1);
+    tb->ooff = w.take<int64_t>(R);
+    tb->inv_s = w.take<float>(R);
+    tb->cntw = w.take<int>((size_t)B * ACC3_WARPS * K);
+    tb->start = w.take<int>(K1);
+    tb->tstart = w.take<int>(K1);
+    tb->sbase = w.take<int>(K1);
+    tb->task_k = w.take<int>((size_t)B * acc3_max_tasks(N, K));
+    tb->slots = w.take<float>((size_t)B * sorted_max_slots(N) * D);
+    ok = ok && tb->ooff && tb->inv_s && tb->cntw && tb->start && tb->tstart && tb->sbase && tb->task_k && tb->slots;
+  }
+  return ok ? w.off : 0;
+}
+
+// The pointers of both accumulate entries: the hard routes read feats and the centres and write the descriptors as
+// float4 (the sorted route's tables hold int64 and float4 slots); labels, soft weights, n_valid and 1/|x| are read one
+// 32-bit word at a time.
+int accumulate_alignment(const char* who, const float* feats, const int32_t* labels, const float* assign,
+                         const float* inv_norm, const float* centers, const float* vlad, const void* ws) {
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, who, "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(labels, 4, who, "labels", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(assign, 4, who, "assign", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(inv_norm, 4, who, "inv_norm", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(centers, 16, who, "centers", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(vlad, 16, who, "vlad", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, who, "ws", "float4 access");
+  return ANYLOC_OK;
+}
+
+// The accumulation and normalisation of B images from given labels (or soft weights) and 1/|x|: the kernels, launch
+// shapes and route of vlad_generate_impl / anyloc_vlad_generate_sorted / anyloc_vlad_generate_soft (padded,
+// rows.first(b) = b * N) or of anyloc_vlad_generate_varlen / _soft_varlen (packed), with N the longest image.  Those
+// entries keep their own copies of these launch sequences (attributes, occupancy and wait_all, grids, normalise); the
+// generate_vocabularies GPU tests hold each route of this function to them bit for bit, ACC3, ACC2, sorted and soft.
+template <bool PACKED>
+int launch_accumulate(const float* feats, const int32_t* n_valid, const int64_t* row0, const int32_t* len,
+                      const int32_t* labels, const float* assign, const float* inv_norm, const float* centers, int B,
+                      int N, int D, int K, int norm_descs, int intra_norm, float* vlad, void* ws, size_t ws_bytes,
+                      const char* who, cudaStream_t st) {
+  const int nslices = cdiv(D, ACC_COLS);
+  const int route = assign ? -1 : vlad_route(N, D, K);
+  const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
+  ANYLOC_REQUIRE(route != ANYLOC_VLAD_ROUTE_SORTED || ztasks <= 65535, "%s: N=%d K=%d exceed the launch grid", who, N,
+                 K);
+  float* partial;
+  int32_t* done;
+  SortedTables tb;
+  if (!carve_accumulate(ws, ws_bytes, B, N, D, K, route, &partial, &done, &tb)) {
+    size_t need = carve_accumulate(nullptr, 0, B, N, D, K, route, &partial, &done, &tb);
+    set_error("%s: workspace too small (%zu bytes given, %zu needed)", who, ws_bytes, need);
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  if (N == 0) {                                     // every image empty: zero descriptors, like the generate calls
+    ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st));
+    return ANYLOC_OK;
+  }
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D));
+  if (assign) {
+    if (PACKED)
+      vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm,
+                                                                               centers, D, K, norm_descs, vlad, partial);
+    else
+      vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N,
+                                                                        D, K, norm_descs, vlad, partial);
+    ANYLOC_CHECK_LAUNCH();
+    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  }
+  if (route == ANYLOC_VLAD_ROUTE_ACC3) {
+    const size_t smem3 = acc3_smem_bytes(N, K);
+    static unsigned long long attr_seen = 0;         // one flag word per instantiation, so per kernel
+    if (first_use_on_this_device(&attr_seen)) {
+      if (PACKED)
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_varlen_kernel,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+      else
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               100 * 1024));
+    }
+    ANYLOC_CHECK_CUDA(cudaMemsetAsync(done, 0, (size_t)B * sizeof(int32_t), st));
+    int occ = 0;
+    if (PACKED)
+      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_varlen_kernel,
+                                                                      ACC3_WARPS * 32, smem3));
+    else
+      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_kernel, ACC3_WARPS * 32,
+                                                                      smem3));
+    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
+    if (PACKED)
+      vlad_accumulate3_varlen_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
+          feats, labels, inv_norm, centers, row0, len, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
+    else
+      vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
+          feats, labels, inv_norm, centers, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
+    ANYLOC_CHECK_LAUNCH();
+    return ANYLOC_OK;
+  }
+  if (route == ANYLOC_VLAD_ROUTE_ACC2) {
+    const int warps = acc2_warps(K);
+    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
+    if (PACKED) {
+      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_varlen_kernel,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      vlad_accumulate2_varlen_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, row0, len,
+                                                                          D, K, norm_descs, warps, vlad, partial);
+    } else {
+      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)smem));
+      vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, N, D, K,
+                                                                   norm_descs, warps, vlad, partial);
+    }
+    ANYLOC_CHECK_LAUNCH();
+    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  }
+  if (PACKED) {
+    vlad_sort_varlen_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, row0, len, N, D, K, norm_descs, tb);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_accumulate_varlen_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(
+        feats, centers, row0, len, N, D, K, tb, vlad, partial);
+  } else {
+    vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, N, D, K, norm_descs, tb);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, tb,
+                                                                                        vlad, partial);
+  }
+  ANYLOC_CHECK_LAUNCH();
+  vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, partial);
+  ANYLOC_CHECK_LAUNCH();
+  return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+}
+}  // namespace
+
+extern "C" size_t anyloc_vlad_label_multi_workspace_bytes(int64_t R, int D, int V, const int* K) {
+  if (!K || V <= 0 || D <= 0 || R < 0) return 0;
+  for (int v = 0; v < V; ++v)
+    if (K[v] <= 0) return 0;
+  AssignBufs ab;
+  return carve_label_multi(nullptr, 0, R, D, assign_multi_ksum(V, K), &ab);
+}
+
+extern "C" int anyloc_vlad_label_multi(const float* feats, const int32_t* n_valid, int N, int64_t R,
+                                       const int64_t* route_rows, int D, int V, const float* const* centers,
+                                       void* const* prepared, const size_t* prepared_bytes, const int* K,
+                                       int dist_mode, int32_t* labels, float* inv_norm, void* ws, size_t ws_bytes,
+                                       void* stream) {
+  const char* who = "vlad_label_multi";
+  ANYLOC_REQUIRE(feats && centers && K && labels && inv_norm && ws, "%s: null pointer", who);
+  ANYLOC_REQUIRE(R >= 0 && R < (1ll << 31) && D > 0 && D % 4 == 0 && V > 0 && (!n_valid || (N > 0 && R % N == 0)),
+                 "%s: bad dims R=%lld N=%d D=%d V=%d (R < 2^31, D a multiple of 4, R a multiple of N with n_valid)",
+                 who, (long long)R, N, D, V);
+  ANYLOC_REQUIRE(dist_mode == ANYLOC_DIST_COSINE || dist_mode == ANYLOC_DIST_EUCLIDEAN, "%s: unknown dist_mode %d",
+                 who, dist_mode);
+  ANYLOC_REQUIRE(!prepared || prepared_bytes, "%s: prepared blobs without their sizes", who);
+  for (int v = 0; v < V; ++v) {
+    ANYLOC_REQUIRE(K[v] > 0 && centers[v], "%s: vocabulary %d has K=%d or no centres", who, v, K[v]);
+    ANYLOC_REQUIRE(!route_rows || route_rows[v] >= 0, "%s: route_rows[%d] = %lld", who, v,
+                   (long long)route_rows[v]);
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(centers[v]) & 3) == 0,
+                   "%s: centers[%d] must be 4-byte aligned (fp32 access)", who, v);
+    ANYLOC_REQUIRE(!prepared || (reinterpret_cast<uintptr_t>(prepared[v]) & 15) == 0,
+                   "%s: prepared[%d] must be 16-byte aligned (float4 and TMA access)", who, v);
+  }
+  int rc = assign_alignment(who, feats, labels, ws);
+  if (rc) return rc;
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, who, "n_valid", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(inv_norm, 4, who, "inv_norm", "fp32 access");
+  const int64_t Ksum = assign_multi_ksum(V, K);
+  ANYLOC_REQUIRE(Ksum < (1ll << 31), "%s: %lld centres in all", who, (long long)Ksum);
+  if (R == 0) return ANYLOC_OK;
+  AssignBufs ab;
+  if (!carve_label_multi(ws, ws_bytes, R, D, Ksum, &ab)) {
+    set_error("%s: workspace too small (%zu given, %zu needed)", who, ws_bytes,
+              anyloc_vlad_label_multi_workspace_bytes(R, D, V, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)Ksum * D));
+  // each vocabulary's centres from its prepared blob where one is given (what its own generate call reads), else
+  // prepared here by the same kernel
+  std::vector<int> koff(V), fast(V);
+  bool any_fast = false;
+  for (int v = 0, off = 0; v < V; off += K[v], ++v) {
+    koff[v] = off;
+    PreparedView pv;
+    if (prepared && prepared[v] && carve_prepared(prepared[v], prepared_bytes[v], D, K[v], &pv)) {
+      const size_t kd = (size_t)K[v] * D * 4, k4 = (size_t)K[v] * 4;
+      ANYLOC_CHECK_CUDA(cudaMemcpyAsync(ab.chat + (size_t)off * D, pv.chat, kd, cudaMemcpyDeviceToDevice, st));
+      ANYLOC_CHECK_CUDA(cudaMemcpyAsync(ab.chat_tf32 + (size_t)off * D, pv.chat_tf32, kd, cudaMemcpyDeviceToDevice, st));
+      ANYLOC_CHECK_CUDA(cudaMemcpyAsync(ab.cbias + off, pv.cbias, k4, cudaMemcpyDeviceToDevice, st));
+      ANYLOC_CHECK_CUDA(cudaMemcpyAsync(ab.cnorm + off, pv.cnorm, k4, cudaMemcpyDeviceToDevice, st));
+    } else {
+      vlad_centre_prep_kernel<<<K[v], 256, 0, st>>>(centers[v], K[v], D, dist_mode, ab.chat + (size_t)off * D,
+                                                    ab.cbias + off, ab.chat_tf32 + (size_t)off * D, ab.cnorm + off,
+                                                    nullptr, 0);
+      ANYLOC_CHECK_LAUNCH();
+    }
+    // launch_assign's test, with the rows of the member's own call (route_rows[v]) where it takes the route from
+    const EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, K[v]};
+    const int64_t rr = route_rows ? route_rows[v] : R;
+    fast[v] = ab.coarse != nullptr && D <= 2048 && rr >= 256 &&
+              gemm_tc_supported(feats, nullptr, D, ab.chat_tf32, nullptr, D, (int)R, K[v], D, ep, ANYLOC_PAIR_TF32);
+    any_fast = any_fast || fast[v];
+  }
+  // the FFMA members; the first writes 1/|x| when no member rescores (the rescoring writes it otherwise)
+  float* inv_ffma = any_fast ? nullptr : inv_norm;
+  for (int v = 0; v < V; ++v) {
+    if (fast[v]) continue;
+    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(((R + 1) / 2 + 7) / 8, (int64_t)device_sm_count() * 8));
+    vlad_assign_kernel<2><<<blocks, 256, 0, st>>>(feats, n_valid, n_valid ? N : (int)R, R, D, K[v],
+                                                  ab.chat + (size_t)koff[v] * D, ab.cbias + koff[v],
+                                                  labels + (size_t)v * R, inv_ffma);
+    ANYLOC_CHECK_LAUNCH();
+    inv_ffma = nullptr;
+  }
+  if (!any_fast) return ANYLOC_OK;
+  const int64_t S = assign_multi_slice(R, Ksum);
+  const EpiParams ep{ANYLOC_EPI_BIAS, ab.cbias, nullptr, nullptr, ab.coarse, nullptr, (int)Ksum};
+  for (int64_t r0 = 0; r0 < R; r0 += S) {
+    const int m = (int)std::min<int64_t>(S, R - r0);
+    const float* xs = feats + r0 * D;
+    rc = gemm_tc_launch(xs, nullptr, D, ab.chat_tf32, nullptr, D, m, (int)Ksum, D, ep, ANYLOC_PAIR_TF32, st);
+    if (rc) return rc;
+    RescoreSegs segs;
+    segs.n = 0;
+    float* inv = inv_norm + r0;                      // written by the slice's first rescoring launch
+    for (int v = 0; v < V; ++v) {
+      if (fast[v]) {
+        segs.koff[segs.n] = koff[v];
+        segs.k[segs.n] = K[v];
+        segs.labels[segs.n] = labels + (size_t)v * R + r0;
+        ++segs.n;
+      }
+      if (segs.n == ASSIGN_MULTI_SEGS || (v == V - 1 && segs.n > 0)) {
+        const int blocks = (m + 7) / 8;
+        const int Nn = n_valid ? N : 1;
+        if (D <= 512)
+          vlad_rescore_multi_norm_kernel<4><<<blocks, 256, 0, st>>>(xs, n_valid, Nn, r0, m, D, (int)Ksum, ab.chat,
+                                                                    ab.cbias, ab.cnorm, ab.coarse, segs, inv);
+        else if (D <= 1024)
+          vlad_rescore_multi_norm_kernel<8><<<blocks, 256, 0, st>>>(xs, n_valid, Nn, r0, m, D, (int)Ksum, ab.chat,
+                                                                    ab.cbias, ab.cnorm, ab.coarse, segs, inv);
+        else
+          vlad_rescore_multi_norm_kernel<16><<<blocks, 256, 0, st>>>(xs, n_valid, Nn, r0, m, D, (int)Ksum, ab.chat,
+                                                                     ab.cbias, ab.cnorm, ab.coarse, segs, inv);
+        ANYLOC_CHECK_LAUNCH();
+        segs.n = 0;
+        inv = nullptr;
+      }
+    }
+  }
+  return ANYLOC_OK;
+}
+
+extern "C" size_t anyloc_vlad_soft_assign_multi_workspace_bytes(int D, int V, const int* K) {
+  if (!K || V <= 0 || D <= 0) return 0;
+  for (int v = 0; v < V; ++v)
+    if (K[v] <= 0) return 0;
+  return align_up((size_t)assign_multi_ksum(V, K) * D * 4, 256);
+}
+
+extern "C" int anyloc_vlad_soft_assign_multi(const float* feats, const int32_t* n_valid, int N, int64_t R, int D, int V,
+                                             const float* const* centers, const int* K, const float* soft_temp,
+                                             float* const* assign, float* inv_norm, void* ws, size_t ws_bytes,
+                                             void* stream) {
+  const char* who = "vlad_soft_assign_multi";
+  ANYLOC_REQUIRE(feats && centers && K && soft_temp && assign && inv_norm && ws, "%s: null pointer", who);
+  ANYLOC_REQUIRE(R >= 0 && R < (1ll << 31) && D > 0 && D % 4 == 0 && V > 0 && (!n_valid || (N > 0 && R % N == 0)),
+                 "%s: bad dims R=%lld N=%d D=%d V=%d (R < 2^31, D a multiple of 4, R a multiple of N with n_valid)",
+                 who, (long long)R, N, D, V);
+  for (int v = 0; v < V; ++v) {
+    ANYLOC_REQUIRE(K[v] > 0 && K[v] <= 2048 && centers[v] && assign[v],
+                   "%s: vocabulary %d has K=%d (1..2048), no centres or no assignment", who, v, K[v]);
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(centers[v]) & 3) == 0,
+                   "%s: centers[%d] must be 4-byte aligned (fp32 access)", who, v);
+    ANYLOC_REQUIRE((reinterpret_cast<uintptr_t>(assign[v]) & 3) == 0,
+                   "%s: assign[%d] must be 4-byte aligned (fp32 access)", who, v);
+  }
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, who, "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, who, "n_valid", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(inv_norm, 4, who, "inv_norm", "fp32 access");
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, who, "ws", "float4 access");
+  if (R == 0) return ANYLOC_OK;
+  Workspace w(ws, ws_bytes);
+  const int64_t Ksum = assign_multi_ksum(V, K);
+  float* chat = w.take<float>((size_t)Ksum * D);
+  if (!chat) {
+    set_error("%s: workspace too small (%zu given, %zu needed)", who, ws_bytes,
+              anyloc_vlad_soft_assign_multi_workspace_bytes(D, V, K));
+    return ANYLOC_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)Ksum * D));
+  for (int v = 0, off = 0; v < V; off += K[v], ++v) {
+    vlad_soft_centre_prep_kernel<<<K[v], 256, 0, st>>>(centers[v], K[v], D, chat + (size_t)off * D);
+    ANYLOC_CHECK_LAUNCH();
+  }
+  // consecutive members share a launch while their scores fit a warp's share of shared memory (and at most
+  // SOFT_MULTI_SEGS of them); a launch of wider scores runs fewer warps per block
+  constexpr int ROWS = SOFT_MULTI_ROWS;
+  float* inv = inv_norm;                             // written by the first launch
+  for (int v0 = 0, off0 = 0; v0 < V;) {
+    SoftSegs segs;
+    segs.n = 0;
+    int ksum = 0;
+    while (v0 + segs.n < V && segs.n < SOFT_MULTI_SEGS &&
+           (size_t)(ksum + K[v0 + segs.n]) * ROWS * 4 <= (size_t)SOFT_MULTI_SMEM) {
+      const int v = v0 + segs.n;
+      segs.koff[segs.n] = ksum;
+      segs.k[segs.n] = K[v];
+      segs.temp[segs.n] = soft_temp[v];
+      segs.assign[segs.n] = assign[v];
+      ksum += K[v];
+      ++segs.n;
+    }
+    const int warps = (int)std::min<size_t>(8, (size_t)SOFT_MULTI_SMEM / ((size_t)ROWS * ksum * 4));
+    const size_t smem = (size_t)warps * ROWS * ksum * 4;
+    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_soft_assign_multi_kernel<ROWS>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int64_t blocks = std::min<int64_t>(((R + ROWS - 1) / ROWS + warps - 1) / warps,
+                                             (int64_t)device_sm_count() * 64 / warps);
+    vlad_soft_assign_multi_kernel<ROWS><<<(int)std::max<int64_t>(blocks, 1), warps * 32, smem, st>>>(
+        feats, n_valid, n_valid ? N : 1, R, D, ksum, chat + (size_t)off0 * D, segs, inv);
+    ANYLOC_CHECK_LAUNCH();
+    inv = nullptr;
+    v0 += segs.n;
+    off0 += ksum;
+  }
+  return ANYLOC_OK;
+}
+
+extern "C" size_t anyloc_vlad_accumulate_workspace_bytes(int B, int N, int D, int K, int soft) {
+  if (B < 0 || N < 0 || D <= 0 || K <= 0) return 0;
+  float* partial;
+  int32_t* done;
+  SortedTables tb;
+  return carve_accumulate(nullptr, 0, B, N, D, K, soft ? -1 : vlad_route(N, D, K), &partial, &done, &tb);
+}
+
+extern "C" int anyloc_vlad_accumulate(const float* feats, const int32_t* n_valid, const int32_t* labels,
+                                      const float* assign, const float* inv_norm, const float* centers, int B, int N,
+                                      int D, int K, int norm_descs, int intra_norm, float* vlad, void* ws,
+                                      size_t ws_bytes, void* stream) {
+  const char* who = "vlad_accumulate";
+  ANYLOC_REQUIRE(feats && inv_norm && centers && vlad && ws, "%s: null pointer", who);
+  ANYLOC_REQUIRE((labels != nullptr) != (assign != nullptr), "%s: pass labels (hard) OR assign (soft)", who);
+  ANYLOC_REQUIRE(B >= 0 && B <= 65535 && N >= 0 && D > 0 && K > 0 && D % 4 == 0 && (int64_t)B * N < (1ll << 31),
+                 "%s: bad dims B=%d N=%d D=%d K=%d (B <= 65535, B * N < 2^31, D a multiple of 4)", who, B, N, D, K);
+  int rc = accumulate_alignment(who, feats, labels, assign, inv_norm, centers, vlad, ws);
+  if (rc) return rc;
+  ANYLOC_REQUIRE_ALIGNED(n_valid, 4, who, "n_valid", "int32 access");
+  if (B == 0) return ANYLOC_OK;
+  return launch_accumulate<false>(feats, assign ? n_valid : nullptr, nullptr, nullptr, labels, assign, inv_norm,
+                                  centers, B, N, D, K, norm_descs, intra_norm, vlad, ws, ws_bytes, who,
+                                  (cudaStream_t)stream);
+}
+
+extern "C" int anyloc_vlad_accumulate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len,
+                                             int B, const int32_t* labels, const float* assign, const float* inv_norm,
+                                             const float* centers, int D, int K, int norm_descs, int intra_norm,
+                                             float* vlad, void* ws, size_t ws_bytes, void* stream) {
+  const char* who = "vlad_accumulate_varlen";
+  int rc = varlen_args(who, feats, R, row0, len, B, D, K, vlad);
+  if (rc) return rc;
+  ANYLOC_REQUIRE(inv_norm && centers && ws, "%s: null pointer", who);
+  ANYLOC_REQUIRE((labels != nullptr) != (assign != nullptr), "%s: pass labels (hard) OR assign (soft)", who);
+  rc = accumulate_alignment(who, feats, labels, assign, inv_norm, centers, vlad, ws);
+  if (rc) return rc;
+  if (B == 0) return ANYLOC_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int N = 0;                                        // the padded batch's row count: the longest image
+  rc = varlen_rows_check(row0, len, B, R, st, who, &N);
+  if (rc) return rc;
+  return launch_accumulate<true>(feats, nullptr, row0, len, labels, assign, inv_norm, centers, B, N, D, K, norm_descs,
+                                 intra_norm, vlad, ws, ws_bytes, who, st);
 }

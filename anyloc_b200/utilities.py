@@ -1389,6 +1389,43 @@ def _finalize(c, R, c_next, err, ws):
                                                   ws.numel(), _lib.stream_ptr()), "anyloc_kmeans_finalize")
 
 
+class _StagePair:
+    """The double buffering of a streamed pass (_RoundFeed, _ImageFeed): per slot a pinned host buffer and a device
+    buffer of `shape` fp32, and one copy stream.  fill(s, n, gather) waits until slot s's previous copy is done, lets
+    gather(host) write the first n rows of its host buffer and queues their copy to the device behind the slot's last
+    release; take(s, n) makes the current stream wait for that copy and returns the n device rows; release(s) records
+    the work queued so far on the current stream as the rows' last use.  So the gather and copy of one slot overlap
+    the device work on the other.  Built and used under torch.cuda.device(dev)."""
+
+    def __init__(self, shape, dev, slots=2):
+        self.host = [torch.empty(shape, pin_memory=True) for _ in range(slots)]
+        self.raw = [torch.empty(shape, device=dev) for _ in range(slots)]
+        self.cs, self.xs = torch.cuda.current_stream(), torch.cuda.Stream()
+        self.copied, self.freed = [None] * slots, [None] * slots
+
+    def fill(self, s, n, gather):
+        if self.copied[s] is not None:
+            self.copied[s].synchronize()                               # the staging buffer's previous copy is done
+        gather(self.host[s])
+        with torch.cuda.stream(self.xs):
+            if self.freed[s] is not None:
+                self.xs.wait_event(self.freed[s])
+            self.raw[s][:n].copy_(self.host[s][:n], non_blocking=True)
+            self.copied[s] = torch.cuda.Event()
+            self.copied[s].record(self.xs)
+
+    def take(self, s, n):
+        self.cs.wait_event(self.copied[s])
+        return self.raw[s][:n]
+
+    def release(self, s):
+        self.freed[s] = torch.cuda.Event()
+        self.freed[s].record(self.cs)
+
+    def close(self):
+        self.xs.synchronize()
+
+
 class _RoundFeed:
     """The rounds of a streamed k-means pass over host rows X [R,D] (any float dtype and strides), on the device, for
     plan (P, resident) of _kmeans_plan: round j holds P rows of every chunk of the in-memory update (_stream_rounds),
@@ -1408,10 +1445,7 @@ class _RoundFeed:
         self.sizes = [(chunks - 1) * pcs[0][1] + pcs[-1][1] for pcs in self.rounds]
         self.offs = np.concatenate([[0], np.cumsum(self.sizes)]).tolist()
         self.kept = torch.empty(self.offs[self.resident], D, device=dev)
-        self.raw = [torch.empty(self.sizes[0], D, device=dev) for _ in range(2)]
-        self.host = [torch.empty(self.sizes[0], D, pin_memory=True) for _ in range(2)]
-        self.cs, self.xs = torch.cuda.current_stream(), torch.cuda.Stream()
-        self.copied, self.freed = [None, None], [None, None]
+        self.pair = _StagePair((self.sizes[0], D), dev)
         self.transfers = ((it, j) for it in range(max_iter)
                           for j in range(0 if it == 0 else self.resident, len(self.rounds)))
         self.staged, self.taken = [], 0
@@ -1423,18 +1457,13 @@ class _RoundFeed:
         if t is None:
             return
         j, s = t[1], len(self.staged) & 1
-        if self.copied[s] is not None:
-            self.copied[s].synchronize()                               # the staging buffer's previous copy is done
-        piece, host = self.piece[j], self.host[s]
-        for ci, (lo, m) in enumerate(self.rounds[j]):
-            host[ci * piece:ci * piece + m].copy_(self.X[lo:lo + m])
-        with torch.cuda.stream(self.xs):
-            if self.freed[s] is not None:
-                self.xs.wait_event(self.freed[s])
-            self.raw[s][:self.sizes[j]].copy_(host[:self.sizes[j]], non_blocking=True)
-            self.copied[s] = torch.cuda.Event()
-            self.copied[s].record(self.xs)
-        self.staged.append((t, s, self.copied[s]))
+        piece = self.piece[j]
+
+        def gather(host):
+            for ci, (lo, m) in enumerate(self.rounds[j]):
+                host[ci * piece:ci * piece + m].copy_(self.X[lo:lo + m])
+        self.pair.fill(s, self.sizes[j], gather)
+        self.staged.append((t, s))
 
     def iteration(self, it):
         """yields (j, x) for every round j of Lloyd iteration `it`, x [sizes[j], D] the round's rows on the device; the
@@ -1443,22 +1472,20 @@ class _RoundFeed:
             x = self.kept[self.offs[j]:self.offs[j + 1]]
             moved = it == 0 or j >= self.resident
             if moved:
-                t, s, ev = self.staged[self.taken]
+                t, s = self.staged[self.taken]
                 self.taken += 1
-                self.cs.wait_event(ev)
-                x = self.raw[s][:self.sizes[j]]
+                x = self.pair.take(s, self.sizes[j])
                 if self.normalize:
                     x = _normalize_rows_dev(x)
                 if j < self.resident:
                     self.kept[self.offs[j]:self.offs[j + 1]].copy_(x)
             yield j, x
             if moved:
-                self.freed[s] = torch.cuda.Event()
-                self.freed[s].record(self.cs)
+                self.pair.release(s)
                 self._stage()
 
     def close(self):
-        self.xs.synchronize()                                          # a round staged for an iteration not run
+        self.pair.close()                                              # a round staged for an iteration not run
 
     def order(self):
         """the host row of every row of the rounds, in round order"""
@@ -1959,21 +1986,7 @@ def fit_vocabularies(vlads: List[VLAD], train_descs: Union[np.ndarray, torch.Ten
 
     The members must agree in norm_descs and dist_mode (they share the normalised rows and the score GEMM); vlad_mode
     and soft_temp do not enter the fit.  ValueError for an empty list, a VLAD listed twice or members that differ."""
-    vlads = list(vlads)
-    if not vlads:
-        raise ValueError("fit_vocabularies: no VLAD given")
-    first, twice = {}, []
-    for i, v in enumerate(vlads):
-        if id(v) in first:
-            twice.append(f"{first[id(v)]} and {i}")
-        first.setdefault(id(v), i)
-    if twice:
-        raise ValueError(f"fit_vocabularies: the same VLAD is listed more than once (members {', '.join(twice)})")
-    key = (bool(vlads[0].norm_descs), vlads[0].mode)
-    odd = [i for i, v in enumerate(vlads) if (bool(v.norm_descs), v.mode) != key]
-    if odd:
-        raise ValueError(f"fit_vocabularies: members {odd} differ from member 0 (norm_descs={key[0]}, "
-                         f"dist_mode={key[1]!r}) in norm_descs or dist_mode; the members share the rows and the scores")
+    vlads = _check_members(vlads, "fit_vocabularies", "the rows and the scores")
     todo, later, written = [], [], set()
     for v in vlads:
         if v.cache_dir is not None and v.cache_dir in written:
@@ -2007,6 +2020,257 @@ def fit_vocabularies(vlads: List[VLAD], train_descs: Union[np.ndarray, torch.Ten
         v._set_vocabulary(c.cpu() if was_cpu else c)
     for v in later:
         v._fit_from_cache()
+
+
+def _check_members(vlads, who, what):
+    """the rules fit_vocabularies and generate_vocabularies share: a non-empty list of distinct VLADs that agree in
+    norm_descs and dist_mode -> the list"""
+    vlads = list(vlads)
+    if not vlads:
+        raise ValueError(f"{who}: no VLAD given")
+    first, twice = {}, []
+    for i, v in enumerate(vlads):
+        if id(v) in first:
+            twice.append(f"{first[id(v)]} and {i}")
+        first.setdefault(id(v), i)
+    if twice:
+        raise ValueError(f"{who}: the same VLAD is listed more than once (members {', '.join(twice)})")
+    key = (bool(vlads[0].norm_descs), vlads[0].mode)
+    odd = [i for i, v in enumerate(vlads) if (bool(v.norm_descs), v.mode) != key]
+    if odd:
+        raise ValueError(f"{who}: members {odd} differ from member 0 (norm_descs={key[0]}, dist_mode={key[1]!r}) in "
+                         f"norm_descs or dist_mode; the members share {what}")
+    return vlads
+
+
+def _generate_call_images(v, X, host_tensor):
+    """the images per call that v.generate_multi(X) makes on a [n, N, D] input: a host tensor larger than
+    v._host_chunk_bytes in chunks of that size, anything else in one call"""
+    n, N, D = X.shape
+    if host_tensor and n * N * D * 4 > v._host_chunk_bytes:
+        return max(1, v._host_chunk_bytes // (N * D * 4))
+    return max(1, n)
+
+
+def _generate_pieces(i0, i1, steps, N):
+    """images [i0, i1) cut wherever one of member v's generate_multi calls ends (steps[v] = (images per call, n)) ->
+    [(p0, p1, route_rows)], route_rows[v] = the rows of member v's call that holds images p0 .. p1: their count picks
+    the member's assignment route"""
+    cuts = sorted({i0, i1} | {c for s, _ in steps for c in range((i0 // s + 1) * s, i1, s)})
+    return [(p0, p1, [N * (min(n, (p0 // s + 1) * s) - p0 // s * s) for s, n in steps])
+            for p0, p1 in zip(cuts[:-1], cuts[1:])]
+
+
+def _generate_chunk_bytes(b, N, D, hard_Ks, soft_Ks, staged):
+    """device bytes of a chunk of b images [b, N, D] in generate_vocabularies: its features (two staging copies when
+    they come from the host), every member's descriptors, the hard members' labels, 1/|x| and shared assignment
+    workspace, the soft members' assignments, 1/|x| and centres, and the largest accumulation workspace"""
+    lib = _lib.load()
+    R = b * N
+    need = 4 * b * D * (sum(hard_Ks) + sum(soft_Ks)) + (2 * 4 * R * D if staged else 0)
+    if hard_Ks:
+        need += (lib.anyloc_vlad_label_multi_workspace_bytes(R, D, len(hard_Ks), (C.c_int * len(hard_Ks))(*hard_Ks))
+                 + 4 * R * (len(hard_Ks) + 1))
+    if soft_Ks:
+        need += (lib.anyloc_vlad_soft_assign_multi_workspace_bytes(D, len(soft_Ks), (C.c_int * len(soft_Ks))(*soft_Ks))
+                 + 4 * R * (sum(soft_Ks) + 1))
+    return need + max([lib.anyloc_vlad_accumulate_workspace_bytes(b, N, D, K, 0) for K in hard_Ks] +
+                      [lib.anyloc_vlad_accumulate_workspace_bytes(b, N, D, K, 1) for K in soft_Ks])
+
+
+def _generate_plan(n, N, D, hard_Ks, soft_Ks, staged, budget, cap):
+    """images per chunk of generate_vocabularies on [n, N, D] features: the most, up to `cap`, whose
+    _generate_chunk_bytes fit `budget`.  MemoryError naming the bytes when not even one image fits."""
+    need1 = _generate_chunk_bytes(1, N, D, hard_Ks, soft_Ks, staged)
+    if need1 > budget:
+        raise MemoryError(f"generate_vocabularies: one image of {N} x {D} features needs {need1} bytes of device "
+                          f"memory (its features, every member's descriptor and the workspaces), {budget} are free")
+    lo, hi = 1, max(1, min(n, cap))
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if _generate_chunk_bytes(mid, N, D, hard_Ks, soft_Ks, staged) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
+def _generate_shared(vlads, x, outs, dev, route_rows=None, table=None):
+    """every member's descriptors of the device features x into outs[v] [B, K_v * D]: padded x [B, N, D] with
+    route_rows[v] (the rows of member v's own call), or packed x [R, D] with table = (row0, lens).  The hard members'
+    labels and 1/|x| come from one anyloc_vlad_label_multi, the soft members' assignments from one
+    anyloc_vlad_soft_assign_multi, then each member accumulates alone."""
+    lib = _lib.load()
+    D = x.shape[-1]
+    if table is None:
+        B, N = x.shape[0], x.shape[1]
+        R = B * N
+    else:
+        row0, lens = table
+        B, N, R = len(lens), max(lens), x.shape[0]
+        route_rows = [B * N] * len(vlads)
+        r0, ln = _table_dev(row0, lens, dev)
+    centres = [v._centers_on(dev) for v in vlads]
+    nd = int(bool(vlads[0].norm_descs))
+
+    def accumulate(i, labels, assign, inv):
+        v = vlads[i]
+        K = v.num_clusters
+        ws = _lib.workspaces.get(dev, lib.anyloc_vlad_accumulate_workspace_bytes(B, N, D, K, int(assign is not None)),
+                                 "vlad")
+        if table is None:
+            _lib.check(lib.anyloc_vlad_accumulate(
+                _lib.ptr(x), None, _lib.ptr(labels), _lib.ptr(assign), _lib.ptr(inv), _lib.ptr(centres[i]), B, N, D,
+                K, nd, int(bool(v.intra_norm)), _lib.ptr(outs[i]), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
+                "anyloc_vlad_accumulate")
+        else:
+            _lib.check(lib.anyloc_vlad_accumulate_varlen(
+                _lib.ptr(x), R, _lib.ptr(r0), _lib.ptr(ln), B, _lib.ptr(labels), _lib.ptr(assign), _lib.ptr(inv),
+                _lib.ptr(centres[i]), D, K, nd, int(bool(v.intra_norm)), _lib.ptr(outs[i]), _lib.ptr(ws), ws.numel(),
+                _lib.stream_ptr()), "anyloc_vlad_accumulate_varlen")
+
+    hard = [i for i, v in enumerate(vlads) if v.vlad_mode != "soft"]
+    soft = [i for i, v in enumerate(vlads) if v.vlad_mode == "soft"]
+    with torch.cuda.device(dev):
+        if hard:
+            V = len(hard)
+            Ks = (C.c_int * V)(*[vlads[i].num_clusters for i in hard])
+            preps = [vlads[i]._prepared_on(dev, centres[i]) for i in hard]
+            labels = torch.empty(V, R, dtype=torch.int32, device=dev)
+            inv = torch.empty(R, dtype=torch.float32, device=dev)
+            ws = _lib.workspaces.get(dev, lib.anyloc_vlad_label_multi_workspace_bytes(R, D, V, Ks), "vlad_multi")
+            _lib.check(lib.anyloc_vlad_label_multi(
+                _lib.ptr(x), None, 1, R, (C.c_int64 * V)(*[route_rows[i] for i in hard]), D, V,
+                (C.c_void_p * V)(*[centres[i].data_ptr() for i in hard]), (C.c_void_p * V)(*[p.data_ptr() for p in preps]),
+                (C.c_size_t * V)(*[p.numel() for p in preps]), Ks, _lib.DIST[vlads[0].mode], _lib.ptr(labels),
+                _lib.ptr(inv), _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "anyloc_vlad_label_multi")
+            for j, i in enumerate(hard):
+                accumulate(i, labels[j], None, inv)
+        if soft:
+            V = len(soft)
+            Ks = (C.c_int * V)(*[vlads[i].num_clusters for i in soft])
+            assign = [torch.empty(R, vlads[i].num_clusters, dtype=torch.float32, device=dev) for i in soft]
+            inv = torch.empty(R, dtype=torch.float32, device=dev)
+            ws = _lib.workspaces.get(dev, lib.anyloc_vlad_soft_assign_multi_workspace_bytes(D, V, Ks), "vlad_soft_multi")
+            _lib.check(lib.anyloc_vlad_soft_assign_multi(
+                _lib.ptr(x), None, 1, R, D, V, (C.c_void_p * V)(*[centres[i].data_ptr() for i in soft]), Ks,
+                (C.c_float * V)(*[float(vlads[i].soft_temp) for i in soft]),
+                (C.c_void_p * V)(*[a.data_ptr() for a in assign]), _lib.ptr(inv), _lib.ptr(ws), ws.numel(),
+                _lib.stream_ptr()), "anyloc_vlad_soft_assign_multi")
+            for j, i in enumerate(soft):
+                accumulate(i, None, assign[j], inv)
+
+
+class _ImageFeed:
+    """Chunks of images [i0, i1) of host features X [n, N, D] (torch CPU tensor of any float dtype and strides) on
+    the device as fp32, chunk c in slot c % 2 of a _StagePair: the gather and copy of one chunk overlap the device work
+    on the one before.  Built and used under torch.cuda.device(dev)."""
+
+    def __init__(self, X, step, dev):
+        n, N, D = X.shape
+        self.X = X
+        self.spans = [(i, min(n, i + step)) for i in range(0, n, step)]
+        self.pair = _StagePair((step, N, D), dev, slots=min(2, len(self.spans)))
+        self.stage(0)
+
+    def stage(self, c):
+        """gather chunk c into its staging buffer and queue its copy to the device"""
+        if c < len(self.spans):
+            i0, i1 = self.spans[c]
+            self.pair.fill(c & 1, i1 - i0, lambda host: host[:i1 - i0].copy_(self.X[i0:i1]))
+
+    def take(self, c):
+        """chunk c's features [i1 - i0, N, D] on the device, once the current stream has waited for their copy"""
+        i0, i1 = self.spans[c]
+        return self.pair.take(c & 1, i1 - i0)
+
+    def release(self, c):
+        """the work on chunk c is queued: its buffer may be refilled after it"""
+        self.pair.release(c & 1)
+
+    def close(self):
+        self.pair.close()
+
+
+def generate_vocabularies(vlads: List[VLAD], multi_query: Union[np.ndarray, torch.Tensor, list]) -> List[torch.Tensor]:
+    """Every VLAD's descriptors of `multi_query` from one read of the features (extension: a sweep over the
+    vocabulary size, such as the reference's ablations over num_clusters, otherwise reads the features, and for host
+    features moves them over the host link, once per vocabulary).
+
+    `multi_query` is what VLAD.generate_multi takes without cache_ids: a numpy array or a CPU or CUDA tensor
+    [n, N, D], or a list of [N_i, D] items (consecutive views of one CUDA buffer, as ext(list) returns, are read in
+    place).  Element i of the result is bit for bit vlads[i].generate_multi(multi_query), on the same device.  Members
+    may differ in num_clusters, vlad_mode, soft_temp and intra_norm; they must agree in norm_descs and dist_mode, as in
+    fit_vocabularies.  ValueError for an empty list, a VLAD listed twice, members that differ, or centres that do not
+    match D.  The per-image caches are not read or written.
+
+    The hard members' labels come from one shared assignment pass, the soft members' probabilities from one shared
+    pass, and each member then accumulates its descriptors alone.  Host [n, N, D] features are staged to the device in
+    chunks of images, once for all members, the copy of the next chunk overlapping the work on this one; a chunk is as
+    large as its features, every member's descriptors and the workspaces allow, and MemoryError names the bytes when
+    one image does not fit.  Device features are aggregated in chunks of the same size, lists in one pass."""
+    vlads = _check_members(vlads, "generate_vocabularies", "the features' norms and the assignment scores")
+    is_list = isinstance(multi_query, (list, tuple))
+    if is_list and len(multi_query) == 0:
+        return torch.stack([])      # generate_multi's failure on an empty list
+    for v in vlads:
+        assert v.kmeans is not None
+        assert v.c_centers is not None
+    D = int(multi_query[0].shape[-1]) if is_list else int(multi_query.shape[-1])
+    for v in vlads:
+        if tuple(v.c_centers.shape) != (v.num_clusters, D):
+            raise ValueError(f"cluster centres {tuple(v.c_centers.shape)} do not match K={v.num_clusters}, D={D}")
+    if is_list:
+        on_dev = all(isinstance(q, torch.Tensor) and q.is_cuda for q in multi_query)
+        dev = _lib.require_cuda(multi_query[0].device if on_dev else None)
+        feats, row0, lens = _pack_list(multi_query, dev)
+        outs = [torch.empty(len(lens), v.num_clusters * D, device=dev) for v in vlads]
+        _generate_shared(vlads, feats, outs, dev, table=(row0, lens))
+        return outs if on_dev else [o.cpu() for o in outs]
+    was_np = type(multi_query) == np.ndarray
+    on_dev = isinstance(multi_query, torch.Tensor) and multi_query.is_cuda
+    dev = _lib.require_cuda(multi_query.device if on_dev else None)
+    X = torch.from_numpy(multi_query) if was_np else multi_query.detach()
+    n, N, _ = X.shape
+    steps = [(_generate_call_images(v, X, not on_dev and not was_np), n) for v in vlads]
+    hard_Ks = [v.num_clusters for v in vlads if v.vlad_mode != "soft"]
+    soft_Ks = [v.num_clusters for v in vlads if v.vlad_mode == "soft"]
+    with torch.cuda.device(dev):
+        if on_dev:
+            x = _as_device_f32(X, dev)
+            res = [torch.empty(n, v.num_clusters * D, device=dev) for v in vlads]
+        else:
+            res = [torch.empty(n, v.num_clusters * D) for v in vlads]
+        if n == 0 or N == 0:                                           # zero descriptors, as the generate calls give
+            for o in res:
+                o.zero_()
+            return res
+        cap = 65535 if on_dev else max(1, min(65535, _STAGE_BYTES // (N * D * 4)))
+        # torch's cache is only released (a device synchronisation) when the free bytes alone would cut the batch
+        step = _generate_plan(n, N, D, hard_Ks, soft_Ks, not on_dev, _device_budget(dev, release_cache=False), cap)
+        if step < min(n, cap):
+            step = _generate_plan(n, N, D, hard_Ks, soft_Ks, not on_dev, _device_budget(dev), cap)
+        if on_dev:
+            for i0 in range(0, n, step):
+                i1 = min(n, i0 + step)
+                for p0, p1, rr in _generate_pieces(i0, i1, steps, N):
+                    _generate_shared(vlads, x[p0:p1], [o[p0:p1] for o in res], dev, route_rows=rr)
+            return res
+        feed = _ImageFeed(X, step, dev)
+        outs = [torch.empty(step, v.num_clusters * D, device=dev) for v in vlads]
+        try:
+            for c, (i0, i1) in enumerate(feed.spans):
+                xc = feed.take(c)
+                for p0, p1, rr in _generate_pieces(i0, i1, steps, N):
+                    _generate_shared(vlads, xc[p0 - i0:p1 - i0], [o[p0 - i0:p1 - i0] for o in outs], dev,
+                                     route_rows=rr)
+                feed.release(c)
+                feed.stage(c + 1)                                      # while the device works on chunk c
+                for r, o in zip(res, outs):
+                    r[i0:i1].copy_(o[:i1 - i0])
+        finally:
+            feed.close()
+        return res
 
 
 _POOL = {"average": 0, "avg": 0, "mean": 0, "max": 1, "gem": 2}

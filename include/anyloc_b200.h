@@ -264,6 +264,50 @@ int anyloc_vlad_assign_multi(const float* feats, int64_t R, int D, int V, const 
 int anyloc_kmeans_accumulate_round_multi(const float* x, int V, const int32_t* const* labels, const int* K, int64_t R,
                                          int64_t round_rows, int64_t piece_rows, int D, int resume, void* const* ws,
                                          const size_t* ws_bytes, void* stream);
+/* Several vocabularies' descriptors over the same features (generate_vocabularies): the per-row passes are shared,
+ * each member's accumulation runs alone.
+ * anyloc_vlad_label_multi writes labels [V, R] and inv_norm [R] = 1/max(|x|,1e-12) for R rows (a padded batch
+ * [R/N, N, D] with n_valid, nullable, as in anyloc_vlad_generate; or packed rows).  labels[v] and inv_norm are
+ * bitwise the labels and 1/|x| that vocabulary v's own generate call (anyloc_vlad_generate_prepared / _sorted /
+ * _varlen) computes, labels -1 for rows n_valid leaves out.  inv_norm is unspecified on those rows (when the members
+ * take different routes it may come from either; the accumulations never read it for a row labelled -1).  That call takes the tensor-core coarse pass plus exact rescoring
+ * or the FFMA kernel by its own row count, which may break near-ties differently: route_rows[v] (host array, nullable
+ * = R) is that count -- B * N of a padded call, B * max len of a packed one, whose R may be smaller.  Members on the
+ * coarse route share one tf32 GEMM over all their centres per slice of rows and one rescoring read of each row.
+ * prepared[v] (host array of anyloc_vlad_prepare blobs of prepared_bytes[v] bytes, nullable, entries nullable) stands
+ * in for the centre prep as in the generate calls.  Workspace: anyloc_vlad_label_multi_workspace_bytes(R, D, V, K).
+ * anyloc_vlad_soft_assign_multi writes each soft vocabulary's assignment assign[v] [R, K[v]] (K[v] <= 2048) at
+ * temperature soft_temp[v] and inv_norm [R], bitwise anyloc_vlad_generate_soft(_varlen)'s assign and 1/|x|: one read of
+ * each row and one dot product per (row, centre) for all members; rows n_valid leaves out get 0.  Workspace:
+ * anyloc_vlad_soft_assign_multi_workspace_bytes(D, V, K).
+ * anyloc_vlad_accumulate (padded [B,N,D]) and anyloc_vlad_accumulate_varlen (packed, table as above) run the
+ * accumulation and normalisation of the generate calls from given per-row results: pass labels [rows] (hard; the
+ * accumulation anyloc_vlad_generate_route(B, N, D, K) names, N the longest image for _varlen) OR assign [rows, K]
+ * (soft; n_valid as in anyloc_vlad_generate_soft, ignored by the hard routes, which skip label -1), with inv_norm
+ * [rows].  With the labels / assignment and inv_norm above the descriptors are bitwise the generate calls'.
+ * Workspace of both: anyloc_vlad_accumulate_workspace_bytes(B, N, D, K, soft) (N = the longest len for _varlen; soft
+ * != 0 sizes the soft accumulation, which needs only the sums of squares). */
+/* Alignment: label_multi as anyloc_vlad_assign_multi plus n_valid and inv_norm 4-byte and each prepared[v] 16-byte;
+ * soft_assign_multi feats and ws 16-byte, n_valid, inv_norm, each centers[v] and assign[v] 4-byte; the accumulates
+ * feats, centers, vlad and ws 16-byte, n_valid, labels, assign, inv_norm and len 4-byte, row0 8-byte.  K, centers,
+ * prepared, prepared_bytes, route_rows, soft_temp and the assign array are host arrays, read on the CPU. */
+size_t anyloc_vlad_label_multi_workspace_bytes(int64_t R, int D, int V, const int* K);
+int anyloc_vlad_label_multi(const float* feats, const int32_t* n_valid, int N, int64_t R, const int64_t* route_rows,
+                            int D, int V, const float* const* centers, void* const* prepared,
+                            const size_t* prepared_bytes, const int* K, int dist_mode, int32_t* labels, float* inv_norm,
+                            void* ws, size_t ws_bytes, void* stream);
+size_t anyloc_vlad_soft_assign_multi_workspace_bytes(int D, int V, const int* K);
+int anyloc_vlad_soft_assign_multi(const float* feats, const int32_t* n_valid, int N, int64_t R, int D, int V,
+                                  const float* const* centers, const int* K, const float* soft_temp,
+                                  float* const* assign, float* inv_norm, void* ws, size_t ws_bytes, void* stream);
+size_t anyloc_vlad_accumulate_workspace_bytes(int B, int N, int D, int K, int soft);
+int anyloc_vlad_accumulate(const float* feats, const int32_t* n_valid, const int32_t* labels, const float* assign,
+                           const float* inv_norm, const float* centers, int B, int N, int D, int K, int norm_descs,
+                           int intra_norm, float* vlad, void* ws, size_t ws_bytes, void* stream);
+int anyloc_vlad_accumulate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B,
+                                  const int32_t* labels, const float* assign, const float* inv_norm,
+                                  const float* centers, int D, int K, int norm_descs, int intra_norm, float* vlad,
+                                  void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------- retrieval
  * Replaces the faiss part of get_top_k_recall (utilities.py:435-450): optional row
