@@ -288,6 +288,7 @@ extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B,
     ANYLOC_REQUIRE(qkv_hi && o_hi, "attention: null pointer");
     ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", f.name);
     ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
+    ANYLOC_REQUIRE_ALIGNED(o_hi, 8, "attention", "o_hi", "64-bit stores of the tensor-core epilogue");
     if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0) {
       set_error("attention: the %s format runs on the tensor-core engine only, with a 16-byte aligned qkv", f.name);
       return ANYLOC_ERR_UNSUPPORTED;
@@ -298,6 +299,8 @@ extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B,
   }
   ANYLOC_REQUIRE(qkv_hi && o_hi && o_lo, "attention: null pointer");
   ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
+  ANYLOC_REQUIRE_ALIGNED(o_hi, 8, "attention", "o_hi", "64-bit stores of the tensor-core epilogue");
+  ANYLOC_REQUIRE_ALIGNED(o_lo, 8, "attention", "o_lo", "64-bit stores of the tensor-core epilogue");
   if (B == 0 || T == 0) return ANYLOC_OK;
   return attention_dispatch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, out_dtype == ANYLOC_PAIR_F16, engine,
                             (cudaStream_t)stream);
@@ -345,6 +348,8 @@ extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, i
   for (int k = 1; k < n; ++k)
     ANYLOC_REQUIRE(row0[by_row[k - 1]] + len[by_row[k - 1]] <= row0[by_row[k]],
                    "attention_varlen: images %d and %d overlap", by_row[k - 1], by_row[k]);
+  ANYLOC_REQUIRE_ALIGNED(o_hi, 8, "attention_varlen", "o_hi", "64-bit stores of the tensor-core epilogue");
+  ANYLOC_REQUIRE_ALIGNED(o_lo, 8, "attention_varlen", "o_lo", "64-bit stores of the tensor-core epilogue");
   if ((reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0 || (reinterpret_cast<uintptr_t>(qkv_lo) & 15) != 0) {
     set_error("attention_varlen: qkv_hi and qkv_lo must be 16-byte aligned (TMA and cp.async)");
     return ANYLOC_ERR_UNSUPPORTED;
@@ -527,6 +532,50 @@ int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights
   }
   return ANYLOC_OK;
 }
+// The alignment of every device pointer a forward reads or writes: ANYLOC_OK, or ANYLOC_ERR_ARG naming the pointer.
+// Whatever reaches the GEMM (weights, biases, LayerScale gammas) needs gemm_tc_supported's 16 bytes, so that an
+// accepted pointer never moves a GEMM off the tensor cores; the LayerNorm gains and biases are float4 loads, the outputs
+// float4 stores; ws needs what its strictest carved buffer needs (TMA), since Workspace::take aligns offsets, not
+// addresses.  The images, positional tables, cls and register tokens are read one fp32 at a time.  n_img images img[i]
+// and tables pos[i] (named img / pos_embed unless `list`), n_taps outputs taps[i].out (named out unless `taps_named`).
+int vit_alignment(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int n_img,
+                  const float* const* img, const float* const* pos, bool list, const AnylocVitTap* taps, int n_taps,
+                  bool taps_named, const void* ws) {
+  char name[64];
+  const char* gemm = "tensor-core GEMM operand";
+  ANYLOC_REQUIRE_ALIGNED(ws, 16, fn, "ws", "TMA and float4 access of the buffers carved from it");
+  ANYLOC_REQUIRE_ALIGNED(w->patch_w_hi, 16, fn, "w.patch_w_hi", gemm);
+  ANYLOC_REQUIRE_ALIGNED(w->patch_w_lo, 16, fn, "w.patch_w_lo", gemm);
+  ANYLOC_REQUIRE_ALIGNED(w->patch_b, 16, fn, "w.patch_b", gemm);
+  ANYLOC_REQUIRE_ALIGNED(w->cls_token, 4, fn, "w.cls_token", "fp32 access");
+  if (cfg->num_registers > 0) ANYLOC_REQUIRE_ALIGNED(w->register_tokens, 4, fn, "w.register_tokens", "fp32 access");
+  for (int l = 0; l < cfg->depth && w->blocks; ++l) {
+    const AnylocVitBlock& b = w->blocks[l];
+    const struct { const void* p; const char* field; int bytes; const char* why; } ptrs[] = {
+        {b.ln1_w, "ln1_w", 16, "float4 access"}, {b.ln1_b, "ln1_b", 16, "float4 access"},
+        {b.qkv_w_hi, "qkv_w_hi", 16, gemm}, {b.qkv_w_lo, "qkv_w_lo", 16, gemm}, {b.qkv_b, "qkv_b", 16, gemm},
+        {b.proj_w_hi, "proj_w_hi", 16, gemm}, {b.proj_w_lo, "proj_w_lo", 16, gemm}, {b.proj_b, "proj_b", 16, gemm},
+        {b.ls1, "ls1", 16, gemm}, {b.ln2_w, "ln2_w", 16, "float4 access"}, {b.ln2_b, "ln2_b", 16, "float4 access"},
+        {b.in_w_hi, "in_w_hi", 16, gemm}, {b.in_w_lo, "in_w_lo", 16, gemm}, {b.in_b, "in_b", 16, gemm},
+        {b.out_w_hi, "out_w_hi", 16, gemm}, {b.out_w_lo, "out_w_lo", 16, gemm}, {b.out_b, "out_b", 16, gemm},
+        {b.ls2, "ls2", 16, gemm}};
+    for (const auto& q : ptrs) {
+      snprintf(name, sizeof(name), "blocks[%d].%s", l, q.field);
+      ANYLOC_REQUIRE_ALIGNED(q.p, q.bytes, fn, name, q.why);
+    }
+  }
+  for (int i = 0; i < n_img; ++i) {
+    snprintf(name, sizeof(name), list ? "img[%d]" : "img", i);
+    ANYLOC_REQUIRE_ALIGNED(img[i], 4, fn, name, "fp32 access");
+    snprintf(name, sizeof(name), list ? "pos_embed[%d]" : "pos_embed", i);
+    ANYLOC_REQUIRE_ALIGNED(pos[i], 4, fn, name, "fp32 access");
+  }
+  for (int i = 0; i < n_taps; ++i) {
+    snprintf(name, sizeof(name), taps_named ? "taps[%d].out" : "out", i);
+    ANYLOC_REQUIRE_ALIGNED(taps[i].out, 16, fn, name, "float4 stores");
+  }
+  return ANYLOC_OK;
+}
 // Returns false (with the error text set) on an empty list, a bad layer or facet, a repeated tap or (need_out) a null
 // output.
 bool tap_plan(const char* fn, const AnylocVitCfg* cfg, const AnylocVitTap* taps, int n_taps, bool need_out,
@@ -703,7 +752,8 @@ static int vit_trunk(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const V
 
 static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B,
                             int H, int W, const float* pos_embed, const AnylocVitTap* taps, int n_taps, int use_cls,
-                            int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, cudaStream_t st) {
+                            int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, cudaStream_t st,
+                            bool taps_named) {
   ANYLOC_REQUIRE(cfg && w && img && pos_embed && ws, "%s: null pointer", fn);
   ANYLOC_REQUIRE(cfg->patch > 0 && H % cfg->patch == 0 && W % cfg->patch == 0 && H > 0 && W > 0,
                  "%s: H=%d W=%d must be positive multiples of the patch size %d", fn, H, W, cfg->patch);
@@ -715,6 +765,7 @@ static int vit_extract_taps(const char* fn, const AnylocVitCfg* cfg, const Anylo
   if (!registers_ok(fn, cfg, w)) return ANYLOC_ERR_ARG;
   int rc;
   if ((rc = format_check(fn, cfg, w, gemm_engine))) return rc;
+  if ((rc = vit_alignment(fn, cfg, w, 1, &img, &pos_embed, false, taps, n_taps, taps_named, ws))) return rc;
   const int R = cfg->num_registers;
   const int P = cfg->patch, N = (H / P) * (W / P), T = N + 1 + R, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P);
   const int M = B * T;
@@ -742,7 +793,7 @@ extern "C" int anyloc_vit_extract(const AnylocVitCfg* cfg, const AnylocVitWeight
   ANYLOC_REQUIRE(cfg && out, "vit_extract: null pointer");
   const AnylocVitTap tap{layer, facet, out};
   return vit_extract_taps("vit_extract", cfg, w, img, B, H, W, pos_embed, &tap, 1, use_cls, norm_descs, ws, ws_bytes,
-                          gemm_engine, (cudaStream_t)stream);
+                          gemm_engine, (cudaStream_t)stream, false);
 }
 
 extern "C" int anyloc_vit_extract_taps(const AnylocVitCfg* cfg, const AnylocVitWeights* w, const float* img, int B, int H,
@@ -750,7 +801,7 @@ extern "C" int anyloc_vit_extract_taps(const AnylocVitCfg* cfg, const AnylocVitW
                                        int norm_descs, void* ws, size_t ws_bytes, int gemm_engine, void* stream) {
   ANYLOC_REQUIRE(cfg, "vit_extract_taps: null pointer");
   return vit_extract_taps("vit_extract_taps", cfg, w, img, B, H, W, pos_embed, taps, n_taps, use_cls, norm_descs, ws,
-                          ws_bytes, gemm_engine, (cudaStream_t)stream);
+                          ws_bytes, gemm_engine, (cudaStream_t)stream, true);
 }
 
 namespace {
@@ -818,7 +869,7 @@ extern "C" size_t anyloc_vit_taps_varlen_workspace_bytes(const AnylocVitCfg* cfg
 static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
                                    const float* const* img, const int32_t* hw, const float* const* pos_embed,
                                    const AnylocVitTap* taps, int n_taps, int use_cls, int norm_descs, void* ws,
-                                   size_t ws_bytes, int gemm_engine, cudaStream_t st) {
+                                   size_t ws_bytes, int gemm_engine, cudaStream_t st, bool taps_named) {
   ANYLOC_REQUIRE(cfg && w && img && pos_embed && ws, "%s: null pointer", fn);
   TapPlan tp;
   if (!tap_plan(fn, cfg, taps, n_taps, true, &tp)) return ANYLOC_ERR_ARG;
@@ -837,6 +888,7 @@ static int vit_extract_taps_varlen(const char* fn, const AnylocVitCfg* cfg, cons
   if (!varlen_plan(cfg, B, hw, &p)) return ANYLOC_ERR_ARG;
   for (int i = 0; i < B; ++i)
     ANYLOC_REQUIRE(img[i] && pos_embed[i], "%s: null image or positional table %d", fn, i);
+  if ((rc = vit_alignment(fn, cfg, w, B, img, pos_embed, true, taps, n_taps, taps_named, ws))) return rc;
   const int P = cfg->patch, D = cfg->embed_dim, Kp = anyloc_vit_patch_k(P), M = p.n_tok;
   VitBuffers bf;
   if (!vit_carve(cfg, (size_t)p.n_patch, (size_t)M, tp.qkv32, ws, ws_bytes, &bf)) {
@@ -864,7 +916,7 @@ extern "C" int anyloc_vit_extract_varlen(const AnylocVitCfg* cfg, const AnylocVi
   ANYLOC_REQUIRE(cfg && out, "vit_extract_varlen: null pointer");
   const AnylocVitTap tap{layer, facet, out};
   return vit_extract_taps_varlen("vit_extract_varlen", cfg, w, B, img, hw, pos_embed, &tap, 1, use_cls, norm_descs, ws,
-                                 ws_bytes, gemm_engine, (cudaStream_t)stream);
+                                 ws_bytes, gemm_engine, (cudaStream_t)stream, false);
 }
 
 extern "C" int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeights* w, int B,
@@ -874,5 +926,5 @@ extern "C" int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const Any
                                               void* stream) {
   ANYLOC_REQUIRE(cfg, "vit_extract_taps_varlen: null pointer");
   return vit_extract_taps_varlen("vit_extract_taps_varlen", cfg, w, B, img, hw, pos_embed, taps, n_taps, use_cls,
-                                 norm_descs, ws, ws_bytes, gemm_engine, (cudaStream_t)stream);
+                                 norm_descs, ws, ws_bytes, gemm_engine, (cudaStream_t)stream, true);
 }

@@ -150,11 +150,12 @@ extern "C" int anyloc_pool_varlen(const float* feats, int64_t R, const int64_t* 
                  "pool_varlen: bad dims B=%d R=%lld D=%d (B <= 65535, D multiple of 4)", B, (long long)R, D);
   ANYLOC_REQUIRE(mode >= POOL_AVG && mode <= POOL_GEM, "pool_varlen: unknown mode %d", mode);
   ANYLOC_REQUIRE(mode != POOL_GEM || gem_p != 0.f, "pool_varlen: gem_p must be non-zero");
+  ANYLOC_REQUIRE_ALIGNED(feats, 16, "pool_varlen", "feats", "float4 access");
+  ANYLOC_REQUIRE_ALIGNED(row0, 8, "pool_varlen", "row0", "int64 access");
+  ANYLOC_REQUIRE_ALIGNED(len, 4, "pool_varlen", "len", "int32 access");
+  ANYLOC_REQUIRE_ALIGNED(out, 16, "pool_varlen", "out", "float4 access");
   if (B == 0) return ANYLOC_OK;
   ANYLOC_REQUIRE(feats && row0 && len && out, "pool_varlen: null pointer");
-  ANYLOC_REQUIRE(((reinterpret_cast<uintptr_t>(feats) | reinterpret_cast<uintptr_t>(out)) & 15) == 0 &&
-                     (reinterpret_cast<uintptr_t>(row0) & 7) == 0 && (reinterpret_cast<uintptr_t>(len) & 3) == 0,
-                 "pool_varlen: feats and out must be 16-byte aligned (float4 access), row0 8-byte and len 4-byte");
   cudaStream_t st = (cudaStream_t)stream;
   int max_len = 0;
   const int rc = varlen_rows_check(row0, len, B, R, st, "pool_varlen", &max_len);

@@ -140,7 +140,10 @@ class VitWeights:
         dev = self.device
 
         def f32(t):
-            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+            # the C side reads every weight pointer with float4 loads or TMA (16-byte aligned), and a contiguous view at
+            # an odd storage offset of a caller's buffer passes .contiguous() unchanged: such a view is copied
+            t = t.detach().to(device=dev, dtype=torch.float32).contiguous()
+            return t if t.data_ptr() % 16 == 0 else t.clone()
 
         def split(t, patch=False):
             """-> (hi, lo, alpha): the kernel-ready pair of a weight matrix and the accumulator scale

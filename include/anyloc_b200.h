@@ -420,7 +420,10 @@ typedef struct {
 
 /* Per-block device pointers.  Matrices are [out,in] row-major like nn.Linear.weight, supplied as
  * tf32 (hi,lo) pairs with hi+lo == fp32 weight (anyloc_split_tf32).  For SwiGLU, w_in rows are
- * interleaved (row 2j = w12[j], row 2j+1 = w12[hidden+j]) and b_in likewise. */
+ * interleaved (row 2j = w12[j], row 2j+1 = w12[hidden+j]) and b_in likewise.
+ * Alignment: every pointer of AnylocVitBlock 16-byte (the matrices, biases and LayerScale gammas are tensor-core GEMM
+ * operands, the LayerNorm gains and biases float4 loads); in AnylocVitWeights patch_w_hi, patch_w_lo and patch_b
+ * 16-byte, cls_token and register_tokens 4-byte; every AnylocVitTap out 16-byte. */
 typedef struct {
   const float *ln1_w, *ln1_b;
   const void *qkv_w_hi, *qkv_w_lo; const float *qkv_b;     /* [3D,D], [3D] */
@@ -482,6 +485,10 @@ typedef struct {
  * Workspace: single bf16's formula (2-byte GEMM inputs, no lo buffers), with A(x), n_p, M and H as above:
  *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(2 M D) + A(6 M D) + A(2 M H) [+ A(12 M D) for the fp32 qkv rows of the
  *   tap calls] + 4096 bytes. */
+/* Alignment of every anyloc_vit_extract* call: ws and out (each taps_host[i].out) 16-byte (TMA and float4 access;
+ * every buffer carved from ws inherits its alignment), img and pos_embed (each img[i] and pos_embed[i]) 4-byte, and the
+ * weights as stated with AnylocVitBlock above, for every block 0..depth-1.  Anything else returns ANYLOC_ERR_ARG naming
+ * the pointer, after the null, shape and tap checks and before the workspace size is checked or anything is launched. */
 /* padded patch-embed reduction length (3*14*14=588 -> multiple of 32) */
 int anyloc_vit_patch_k(int patch);
 size_t anyloc_vit_workspace_bytes(const AnylocVitCfg* cfg, int B, int H, int W);
@@ -600,7 +607,10 @@ int anyloc_quantize_fp8_tensor(const float* x, void* q, size_t n, float* scale_h
  * o_hi single bf16 [B,T,D], qkv_lo and o_lo NULL (else ANYLOC_ERR_ARG); one bf16 MMA per product, P rounded once to
  * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED).
  * out_dtype = ANYLOC_PAIR_F16X1: the same with single fp16 qkv_hi of 8 x and o_hi of 8 o (the hi arrays of the fp16
- * pairs); 1/64 folded into the logit scale and P = 1024 p, as for the fp16 pairs, P rounded once. */
+ * pairs); 1/64 folded into the logit scale and P = 1024 p, as for the fp16 pairs, P rounded once.
+ * Alignment: o_hi and o_lo 8-byte (64-bit stores of the tensor-core epilogue), else ANYLOC_ERR_ARG before anything is
+ * launched; a qkv that is not 16-byte aligned runs the SIMT kernel under ANYLOC_GEMM_AUTO (the single formats and
+ * ANYLOC_GEMM_TC3: ANYLOC_ERR_UNSUPPORTED). */
 int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                      void* o_hi, void* o_lo, int out_dtype, int engine, void* stream);
 /* The packed attention of the _varlen ViT calls, on n images of different lengths in one [rows, 3D] qkv buffer:
@@ -612,8 +622,8 @@ int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int
  * table (longest first) and launcher as the ViT; an image's rows are bit-identical to anyloc_attention on that image
  * alone (fp16 pairs: fed the tf32 pair of x) whatever the other images and the rows around it hold.
  * ANYLOC_ERR_ARG for a null pointer, n outside [1, ANYLOC_VIT_VARLEN_MAX_B], len[i] < 1, row0[i] < 0, overlapping
- * images, D != 64 heads, lo arrays with bf16 or without a pair format, or a bad fmt; ANYLOC_ERR_UNSUPPORTED for a qkv
- * that is not 16-byte aligned.  Both return before anything is launched. */
+ * images, D != 64 heads, lo arrays with bf16 or without a pair format, a bad fmt, or o_hi / o_lo not 8-byte aligned;
+ * ANYLOC_ERR_UNSUPPORTED for a qkv that is not 16-byte aligned.  Both return before anything is launched. */
 int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, int n, const int32_t* row0, const int32_t* len,
                             int D, int heads, void* o_hi, void* o_lo, int fmt, void* stream);
 /* y[r, :] = x[r, 0:D] / max(|x[r, 0:D]|, 1e-12) (F.normalize), x rows ld_in elements apart, y [rows, D] packed.
@@ -676,7 +686,8 @@ int anyloc_pool(const float* feats, const int32_t* n_valid, int B, int N, int D,
 /* The same pooling of a packed list: feats [R,D], image b = rows [row0[b], row0[b] + len[b]) (row0 [B] int64, len [B]
  * int32, device arrays; the table rules and refusals of anyloc_vlad_generate_varlen, out 16-byte aligned in vlad's
  * place).  Each image's rows are read in pool's order, so out[b] is bitwise anyloc_pool's for the padded batch with
- * n_valid = len; len = 0 gives NaN.  No workspace. */
+ * n_valid = len; len = 0 gives NaN.  No workspace.  Alignment: feats and out 16-byte, row0 8-byte, len 4-byte, checked
+ * before B = 0 returns. */
 int anyloc_pool_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len, int B, int D, int mode,
                        float gem_p, int gem_use_abs, float* out, void* stream);
 

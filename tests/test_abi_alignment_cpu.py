@@ -1,9 +1,11 @@
-"""Alignment checks of the pooling and pre-processing entry points, without a GPU.  anyloc_pool reads the features and
-writes the output with float4 accesses, anyloc_preprocess_u8 stores pairs of columns as float2 when Wc is even, and
-every pre-processing kernel stores fp32 elements, so a pointer those accesses would fault on is refused before any
-CUDA call: the placeholder device pointers here are never touched.  Calls with nothing to do (B = 0, n = 0) and
-aligned pointers still return OK without launching."""
+"""Alignment checks of the C entry points, without a GPU.  anyloc_pool reads the features and writes the output with
+float4 accesses, anyloc_preprocess_u8 stores pairs of columns as float2 when Wc is even, and every pre-processing kernel
+stores fp32 elements, so a pointer those accesses would fault on is refused before any CUDA call: the placeholder device
+pointers here are never touched.  Calls with nothing to do (B = 0, n = 0) and aligned pointers still return OK without
+launching.  The table ALIGN below does the same for every other entry that takes device pointers, and the header's
+prototypes and ViT structs are checked against it."""
 import ctypes as C
+import re
 
 import pytest
 
@@ -87,12 +89,30 @@ def test_preprocess_resize_and_list_alignment(lib):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# The alignment each VLAD, k-means, retrieval and PCA entry requires of each pointer it takes: the widest access any of
-# its routes makes through that pointer (float4 / uint4 / TMA: 16, int64 / fp64: 8, fp32 / int32: 4).  A workspace or
-# blob inherits the base's alignment in every buffer carved from it, so it needs what its strictest buffer needs.  Where
-# the pointer reaches the tensor-core GEMM it is 16 even when the fallback kernel would accept less, so that an accepted
-# buffer never changes the route.  test_abi_offsets_gpu.py hands every entry real buffers at the offsets this table
-# accepts.  DESIGN.md section 2 lists the kernels' 64- and 128-bit accesses that each entry traces back to.
+# The alignment each entry requires of each pointer it takes: the widest access any of its routes makes through that
+# pointer (float4 / uint4 / TMA: 16, int64 / fp64 / a 64-bit store: 8, fp32 / int32: 4).  A workspace or blob inherits
+# the base's alignment in every buffer carved from it, so it needs what its strictest buffer needs.  Where the pointer
+# reaches the tensor-core GEMM, TMA or the wgmma attention it is 16 even when the fallback kernel would accept less, so
+# that an accepted buffer never changes the route.  Host arrays of device pointers are named by element (centers[1]),
+# the fields of the ViT's structs as w.patch_b, blocks[1].ln2_w and taps[1].out.  test_abi_offsets_gpu.py and
+# test_abi_vit_offsets_gpu.py hand every entry real buffers at the offsets this table accepts.  DESIGN.md section 2
+# lists the kernels' 64- and 128-bit accesses that each entry traces back to.
+VIT_BLOCK_FIELDS = ("ln1_w", "ln1_b", "qkv_w_hi", "qkv_w_lo", "qkv_b", "proj_w_hi", "proj_w_lo", "proj_b", "ls1",
+                    "ln2_w", "ln2_b", "in_w_hi", "in_w_lo", "in_b", "out_w_hi", "out_w_lo", "out_b", "ls2")
+VIT_DEPTH = 2                   # two blocks and two taps / images, so that a check of element 0 alone is caught
+
+
+def _vit_row(images, outs):
+    """a ViT entry's row: the workspace, the weights of blocks 0..VIT_DEPTH-1, the images and positional tables (named
+    `images`), the outputs (named `outs`)"""
+    row = {"ws": 16, "w.patch_w_hi": 16, "w.patch_w_lo": 16, "w.patch_b": 16, "w.cls_token": 4,
+           "w.register_tokens": 4}
+    row.update({f"blocks[{l}].{f}": 16 for l in range(VIT_DEPTH) for f in VIT_BLOCK_FIELDS})
+    row.update({n: 4 for n in images})
+    row.update({n: 16 for n in outs})
+    return row
+
+
 ALIGN = {
     "anyloc_vlad_assign": {"feats": 16, "centers": 4, "labels": 4, "ws": 16},
     "anyloc_vlad_assign_multi": {"feats": 16, "centers[0]": 4, "centers[1]": 4, "labels": 4, "ws": 16},
@@ -131,10 +151,56 @@ ALIGN = {
     "anyloc_pca_accumulate": {"x": 4, "mu": 8, "u": 8, "out": 8},
     "anyloc_pca_mirror": {"a": 8},
     "anyloc_pool": {"feats": 16, "n_valid": 4, "out": 16},
+    "anyloc_pool_varlen": {"feats": 16, "row0": 8, "len": 4, "out": 16},
+    "anyloc_vlad_label_multi": {"feats": 16, "n_valid": 4, "centers[0]": 4, "centers[1]": 4, "prepared[0]": 16,
+                                "prepared[1]": 16, "labels": 4, "inv_norm": 4, "ws": 16},
+    "anyloc_vlad_soft_assign_multi": {"feats": 16, "n_valid": 4, "centers[0]": 4, "centers[1]": 4, "assign[0]": 4,
+                                      "assign[1]": 4, "inv_norm": 4, "ws": 16},
+    "anyloc_vlad_accumulate": {"feats": 16, "n_valid": 4, "labels": 4, "assign": 4, "inv_norm": 4, "centers": 16,
+                               "vlad": 16, "ws": 16},
+    "anyloc_vlad_accumulate_varlen": {"feats": 16, "row0": 8, "len": 4, "labels": 4, "assign": 4, "inv_norm": 4,
+                                      "centers": 16, "vlad": 16, "ws": 16},
+    # o: the 64-bit stores of attention_tc_kernel's epilogue (the SIMT and wgmma kernels store 32 bits)
+    "anyloc_attention": {"qkv_hi": 16, "qkv_lo": 16, "o_hi": 8, "o_lo": 8},
+    "anyloc_attention_varlen": {"qkv_hi": 16, "qkv_lo": 16, "o_hi": 8, "o_lo": 8},
+    "anyloc_vit_extract": _vit_row(("img", "pos_embed"), ("out",)),
+    "anyloc_vit_extract_taps": _vit_row(("img", "pos_embed"), ("taps[0].out", "taps[1].out")),
+    "anyloc_vit_extract_varlen": _vit_row(("img[0]", "img[1]", "pos_embed[0]", "pos_embed[1]"), ("out",)),
+    "anyloc_vit_extract_taps_varlen": _vit_row(("img[0]", "img[1]", "pos_embed[0]", "pos_embed[1]"),
+                                               ("taps[0].out", "taps[1].out")),
 }
 
-OK, WS = 0, _lib.ERR["workspace"]
+# Pointers whose alignment chooses a route instead of being refused, as documented: below 16 bytes a qkv runs
+# anyloc_attention's SIMT kernel under ANYLOC_GEMM_AUTO (B = 0 here: OK, nothing to run), and anyloc_attention_varlen
+# returns ANYLOC_ERR_UNSUPPORTED.  (entry, pointer) -> the code expected below the alignment.
+BELOW = {("anyloc_attention", "qkv_hi"): 0, ("anyloc_attention", "qkv_lo"): 0,
+         ("anyloc_attention_varlen", "qkv_hi"): _lib.ERR["unsupported"],
+         ("anyloc_attention_varlen", "qkv_lo"): _lib.ERR["unsupported"]}
+
+# The entries with device pointers that the table leaves out: why, and the tests that cover their alignment.
+EXEMPT = {
+    "anyloc_gemm_nt": ("alignment chooses the tensor-core or SIMT route under AUTO", "test_gemm_engine_gpu.py"),
+    "anyloc_layernorm_split": ("y_hi / y_lo need 4 elements of the output format", "test_vit_rows_cpu.py"),
+    "anyloc_preprocess_u8": ("out needs 8 bytes when Wc is even, 4 when odd", "test_abi_alignment_cpu.py"),
+    "anyloc_preprocess_resize_u8": ("fp32 stores only, refused above", "test_abi_alignment_cpu.py"),
+    "anyloc_preprocess_u8_varlen": ("fp32 stores only, refused above", "test_abi_alignment_cpu.py"),
+    "anyloc_l2_normalize_rows": ("one message names x and y together", "test_vit_rows_cpu.py"),
+    "anyloc_quantize_fp8_rows": ("one message names x, q and scales together", "test_fp8_edges_gpu.py"),
+    "anyloc_quantize_fp8_tensor": ("element-wise kernels, natural alignment", "test_fp8_kernels_gpu.py"),
+    "anyloc_split_tf32": ("element-wise kernel, natural alignment", "test_ops_gpu.py"),
+    "anyloc_split_f16": ("element-wise kernel, natural alignment", "test_f16x1_kernels_gpu.py"),
+    "anyloc_split_bf16": ("element-wise kernel, natural alignment", "test_bf16_kernels_gpu.py"),
+    "anyloc_allgather_desc": ("NCCL's all-gather reads and writes the buffers", "test_dist_gpu.py"),
+    "anyloc_device_info": ("host pointers only", "test_abi_cpu.py"),
+    "anyloc_profile_read": ("host pointers only", "test_retrieval_engine_gpu.py"),
+    "anyloc_kmeans_partition": ("host pointers only", "test_kmeans_stream_cpu.py"),
+}
+
+OK, WS, UNS = 0, _lib.ERR["workspace"], _lib.ERR["unsupported"]
 D_, K_ = 8, 4                   # every call below: 8 columns, 4 clusters
+VIT_CFG = _lib.VitCfg(384, VIT_DEPTH, 6, 0, 1536, 14, 0, 4)   # ViT-S/14, tf32 pairs, 4 register tokens
+VIT_TAPS = ((0, 0), (1, 3))     # block 0's query, block 1's token output
+VIT_HW = (C.c_int32 * 4)(28, 42, 42, 42)
 
 
 def _vp(*xs):
@@ -143,6 +209,32 @@ def _vp(*xs):
 
 def _counts(addr):
     return C.cast(C.c_void_p(addr), C.POINTER(C.c_int64))
+
+
+def _vit_weights(p):
+    """the AnylocVitWeights of the addresses p["w.*"] and p["blocks[l].*"]"""
+    blocks = (_lib.VitBlock * VIT_DEPTH)()
+    for l in range(VIT_DEPTH):
+        for f in VIT_BLOCK_FIELDS:
+            setattr(blocks[l], f, p[f"blocks[{l}].{f}"])
+    return _lib.VitWeightsStruct(p["w.patch_w_hi"], p["w.patch_w_lo"], p["w.patch_b"], p["w.cls_token"], blocks, 1.0,
+                                 p["w.register_tokens"])     # the struct keeps `blocks` alive
+
+
+def _vit_taps(p):
+    return (_lib.VitTap * 2)(*[_lib.VitTap(l, f, p[f"taps[{i}].out"]) for i, (l, f) in enumerate(VIT_TAPS)])
+
+
+def _attention_varlen(lib, p):
+    # no shape of this entry runs nothing, so the other qkv pointer is kept below 16 bytes: each call stops at the
+    # qkv check (ANYLOC_ERR_UNSUPPORTED), which follows the argument checks
+    hi, lo = p["qkv_hi"], p["qkv_lo"]
+    if lo != P:
+        hi = P + 8
+    else:
+        lo = P + 8
+    return lib.anyloc_attention_varlen(hi, lo, 2, (C.c_int32 * 2)(0, 70), (C.c_int32 * 2)(70, 50), 384, 6,
+                                       p["o_hi"], p["o_lo"], 0, None)
 
 
 # Each entry's call at a shape that does no device work even without the alignment checks: nothing to do (B, R, N,
@@ -223,6 +315,40 @@ def _calls(lib):
         "anyloc_pca_mirror": (OK, lambda p: lib.anyloc_pca_mirror(p["a"], 0, 3, None)),
         "anyloc_pool": (OK, lambda p: lib.anyloc_pool(p["feats"], p["n_valid"], 0, 9, 36, AVG, C.c_float(3.0), 0,
                                                       p["out"], None)),
+        "anyloc_pool_varlen": (OK, lambda p: lib.anyloc_pool_varlen(
+            p["feats"], 9, p["row0"], p["len"], 0, 36, AVG, C.c_float(3.0), 0, p["out"], None)),
+        "anyloc_vlad_label_multi": (OK, lambda p: lib.anyloc_vlad_label_multi(
+            p["feats"], p["n_valid"], 9, 0, None, D_, 2, _vp(p["centers[0]"], p["centers[1]"]),
+            _vp(p["prepared[0]"], p["prepared[1]"]), (C.c_size_t * 2)(1 << 20, 1 << 20), (C.c_int * 2)(K_, 3), 0,
+            p["labels"], p["inv_norm"], p["ws"], 1 << 20, None)),
+        "anyloc_vlad_soft_assign_multi": (OK, lambda p: lib.anyloc_vlad_soft_assign_multi(
+            p["feats"], p["n_valid"], 9, 0, D_, 2, _vp(p["centers[0]"], p["centers[1]"]), (C.c_int * 2)(K_, 3),
+            (C.c_float * 2)(0.1, 0.2), _vp(p["assign[0]"], p["assign[1]"]), p["inv_norm"], p["ws"], 1 << 20, None)),
+        # hard (labels) unless the case is the soft weights' pointer
+        "anyloc_vlad_accumulate": (OK, lambda p: lib.anyloc_vlad_accumulate(
+            p["feats"], p["n_valid"], None if p["assign"] != P else p["labels"],
+            p["assign"] if p["assign"] != P else None, p["inv_norm"], p["centers"], 0, 9, D_, K_, 1, 1, p["vlad"],
+            p["ws"], 1 << 20, None)),
+        "anyloc_vlad_accumulate_varlen": (OK, lambda p: lib.anyloc_vlad_accumulate_varlen(
+            p["feats"], 9, p["row0"], p["len"], 0, None if p["assign"] != P else p["labels"],
+            p["assign"] if p["assign"] != P else None, p["inv_norm"], p["centers"], D_, K_, 1, 1, p["vlad"], p["ws"],
+            1 << 20, None)),
+        "anyloc_attention": (OK, lambda p: lib.anyloc_attention(
+            p["qkv_hi"], p["qkv_lo"], 0, 64, 384, 6, p["o_hi"], p["o_lo"], 0, 0, None)),
+        "anyloc_attention_varlen": (UNS, lambda p: _attention_varlen(lib, p)),
+        # the ViT entries: a 0-byte workspace, refused after the pointers (the forward itself always launches)
+        "anyloc_vit_extract": (WS, lambda p: lib.anyloc_vit_extract(
+            C.byref(VIT_CFG), C.byref(_vit_weights(p)), p["img"], 1, 28, 42, p["pos_embed"], 1, 2, 0, 1, p["out"],
+            p["ws"], 0, 0, None)),
+        "anyloc_vit_extract_taps": (WS, lambda p: lib.anyloc_vit_extract_taps(
+            C.byref(VIT_CFG), C.byref(_vit_weights(p)), p["img"], 1, 28, 42, p["pos_embed"], _vit_taps(p), 2, 0, 1,
+            p["ws"], 0, 0, None)),
+        "anyloc_vit_extract_varlen": (WS, lambda p: lib.anyloc_vit_extract_varlen(
+            C.byref(VIT_CFG), C.byref(_vit_weights(p)), 2, _vp(p["img[0]"], p["img[1]"]), VIT_HW,
+            _vp(p["pos_embed[0]"], p["pos_embed[1]"]), 1, 2, 0, 1, p["out"], p["ws"], 0, 0, None)),
+        "anyloc_vit_extract_taps_varlen": (WS, lambda p: lib.anyloc_vit_extract_taps_varlen(
+            C.byref(VIT_CFG), C.byref(_vit_weights(p)), 2, _vp(p["img[0]"], p["img[1]"]), VIT_HW,
+            _vp(p["pos_embed[0]"], p["pos_embed[1]"]), _vit_taps(p), 2, 0, 1, p["ws"], 0, 0, None)),
     }
 
 
@@ -244,27 +370,70 @@ def test_entry_refuses_pointer_below_its_alignment(lib, entry, name):
     a = ALIGN[entry][name]
     for off in below(a):
         rc = call(dict(ptrs, **{name: base + off}))
+        if (entry, name) in BELOW:
+            assert rc == BELOW[entry, name], (entry, name, off, rc, _lib.last_error())
+            continue
         assert rc == ARG, (entry, name, off, rc, _lib.last_error())
         assert f"{name} must be {a}-byte aligned" in _lib.last_error(), (entry, name, off, _lib.last_error())
     for off in (a, 2 * a, 3 * a):
         assert call(dict(ptrs, **{name: base + off})) == expect, (entry, name, off, _lib.last_error())
 
 
-def test_table_covers_every_pointer_argument_of_the_entries(lib):
-    # the header's prototype of each entry names every pointer argument; each must be in the table (or be a host array
-    # the library reads on the CPU, or the stream)
+def _header():
     import os
-    import re
-    host_only = {"K", "ws_bytes", "stream"}
-    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include",
-                            "anyloc_b200.h")).read()
-    for entry, ptrs in ALIGN.items():
-        m = re.search(r"^int " + entry + r"\(([^)]*)\)", src, re.M)
-        assert m, entry
-        names = set()
-        for arg in m.group(1).split(","):
-            arg = arg.strip()
-            if "*" in arg:
-                names.add(re.sub(r"\W", "", arg.split("*")[-1]))
-        covered = {re.sub(r"\[\d+\]", "", n) for n in ptrs}
-        assert names - host_only == covered, (entry, names - host_only, covered)
+    return open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include",
+                             "anyloc_b200.h")).read()
+
+
+# arguments the library reads on the CPU (host arrays, sizes, the stream), of every entry and of one entry
+HOST_ARGS = {"K", "ws_bytes", "stream", "cfg", "hw", "route_rows", "prepared_bytes", "soft_temp"}
+HOST_ARGS_OF = {"anyloc_attention_varlen": {"row0", "len"}}
+
+
+def _argument_of(name):
+    """the prototype argument a table name goes through: centers[1] -> centers, w.patch_b / blocks[1].ln2_w -> w_host,
+    taps[1].out -> taps_host"""
+    if name.startswith(("w.", "blocks[")):
+        return "w_host"
+    if name.startswith("taps["):
+        return "taps_host"
+    return re.sub(r"\[\d+\]", "", name)
+
+
+def test_table_covers_every_pointer_argument_of_the_entries(lib):
+    # every `int anyloc_*(` prototype of the header that takes a pointer is in the table, with each of its device
+    # pointers, or exempt with a reason; a new entry with neither fails here
+    protos = {m.group(1): m.group(2) for m in re.finditer(r"^int (anyloc_\w+)\(([^)]*)\)", _header(), re.M)}
+    assert set(ALIGN) <= set(protos) and set(EXEMPT) <= set(protos), (set(ALIGN) | set(EXEMPT)) - set(protos)
+    assert not set(ALIGN) & set(EXEMPT)
+    for entry, args in protos.items():
+        names = {re.sub(r"\W", "", a.split("*")[-1]) for a in args.split(",") if "*" in a}
+        if not names:
+            continue
+        assert entry in ALIGN or entry in EXEMPT, f"{entry} takes pointers {sorted(names)} but has no row in ALIGN"
+        if entry in ALIGN:
+            covered = {_argument_of(n) for n in ALIGN[entry]}
+            assert names - HOST_ARGS - HOST_ARGS_OF.get(entry, set()) == covered, (entry, names, covered)
+    for entry, (reason, test) in EXEMPT.items():
+        assert reason and test.startswith("test_"), entry
+
+
+def _struct_pointers(src, struct):
+    body = re.search(r"typedef struct \{([^}]*)\} " + struct + ";", src).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    return {n for decl in body.split(";") for n in re.findall(r"\*\s*(\w+)", decl)}
+
+
+def test_vit_rows_cover_every_pointer_field_of_the_vit_structs():
+    # a pointer field added to AnylocVitBlock, AnylocVitWeights or AnylocVitTap needs its rows in every ViT entry, for
+    # every block and tap
+    src = _header()
+    block, weights, tap = (_struct_pointers(src, s) for s in ("AnylocVitBlock", "AnylocVitWeights", "AnylocVitTap"))
+    assert set(VIT_BLOCK_FIELDS) == block, block ^ set(VIT_BLOCK_FIELDS)
+    assert "blocks" in weights and tap == {"out"}
+    for entry in (e for e in ALIGN if e.startswith("anyloc_vit_extract")):
+        row = ALIGN[entry]
+        assert {f"w.{f}" for f in weights - {"blocks"}} <= set(row), entry
+        assert {f"blocks[{l}].{f}" for l in range(VIT_DEPTH) for f in block} <= set(row), entry
+        outs = {n for n in row if n.endswith("out")}
+        assert outs == ({f"taps[{i}].{f}" for i in range(2) for f in tap} if "taps" in entry else {"out"}), entry

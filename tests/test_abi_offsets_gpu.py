@@ -1,12 +1,13 @@
-"""Every VLAD, k-means, retrieval, PCA and pooling entry point at the pointer offsets its alignment table accepts
-(tests/test_abi_alignment_cpu.py ALIGN) but that torch allocations never produce: +16 and +48 bytes where 16 is
+"""Every VLAD, k-means, retrieval, PCA, pooling and attention entry point at the pointer offsets its alignment table
+accepts (tests/test_abi_alignment_cpu.py ALIGN) but that torch allocations never produce: +16 and +48 bytes where 16 is
 required, +8 where 8 is, +4 and +12 where 4 is (PCA's x also with an odd leading dimension).  Each buffer sits inside a
 NaN frame.  Each call must give, bit for bit, what the same call on 256-byte aligned buffers gives, with the same
 number of launches (the same route: tensor-core or FFMA assignment, accumulate3 / accumulate2 / sorted, the tiled
-k-means, the coarse or exact retrieval), and leave every frame intact.  No pointer below its alignment is ever passed
-here; the refusals are test_abi_alignment_cpu.py's.  One shape of the VLAD and of the retrieval family is also held to
-the fp64 bounds of test_vlad_engine_gpu.py / test_retrieval_engine_gpu.py at an offset.  The split index (host lo
-array) is left to test_retrieval_split_gpu.py's aligned buffers."""
+k-means, the coarse or exact retrieval, the attention kernel), and leave every frame intact.  No pointer below its
+alignment is ever passed here; the refusals are test_abi_alignment_cpu.py's.  One shape of the VLAD and of the
+retrieval family is also held to the fp64 bounds of test_vlad_engine_gpu.py / test_retrieval_engine_gpu.py at an
+offset.  The split index (host lo array) is left to test_retrieval_split_gpu.py's aligned buffers, the ViT entries to
+test_abi_vit_offsets_gpu.py."""
 import ctypes as C
 
 import pytest
@@ -270,6 +271,93 @@ def spec(L, entry, shape):
         bufs = dict(feats=rnd(B, N, D), n_valid=i32([N - 3 * b for b in range(B)]), out=B * D * 4)
         return bufs, ["out"], lambda p, n: lib.anyloc_pool(p["feats"], p["n_valid"], B, N, D, 2, C.c_float(3.0), 0,
                                                            p["out"], st)
+    if entry == "anyloc_pool_varlen":
+        D, lens = shape
+        row0, r = [], 3
+        for ln in lens:
+            row0.append(r)
+            r += ln
+        R, B = r + 2, len(lens)
+        bufs = dict(feats=rnd(R, D), row0=i64(row0), len=i32(lens), out=B * D * 4)
+        return bufs, ["out"], lambda p, n: lib.anyloc_pool_varlen(p["feats"], R, p["row0"], p["len"], B, D, 2,
+                                                                  C.c_float(3.0), 0, p["out"], st)
+    if entry in ("anyloc_vlad_label_multi", "anyloc_vlad_soft_assign_multi"):
+        R, N, D = shape
+        Ks = (C.c_int * 2)(16, 8)
+        x, c0 = vlad_inputs(R, D, 16)
+        c1 = vlad_inputs(8, D, 8, seed=5)[1]
+        bufs = {"feats": x, "n_valid": i32([N - 5 * b for b in range(R // N)]), "centers[0]": c0, "centers[1]": c1,
+                "inv_norm": R * 4}
+
+        def vp(p, *names):
+            return (C.c_void_p * len(names))(*[p[k].value for k in names])
+        if entry == "anyloc_vlad_label_multi":
+            bufs.update({"prepared[0]": prepared(L, c0, D, 16), "prepared[1]": prepared(L, c1, D, 8),
+                         "labels": 2 * R * 4, "ws": nb(lib, "anyloc_vlad_label_multi_workspace_bytes", R, D, 2, Ks)})
+            return bufs, ["labels", "inv_norm"], lambda p, n: lib.anyloc_vlad_label_multi(
+                p["feats"], p["n_valid"], N, R, None, D, 2, vp(p, "centers[0]", "centers[1]"),
+                vp(p, "prepared[0]", "prepared[1]"), (C.c_size_t * 2)(n["prepared[0]"], n["prepared[1]"]), Ks, 0,
+                p["labels"], p["inv_norm"], p["ws"], n["ws"], st)
+        bufs.update({"assign[0]": R * 16 * 4, "assign[1]": R * 8 * 4,
+                     "ws": nb(lib, "anyloc_vlad_soft_assign_multi_workspace_bytes", D, 2, Ks)})
+        return bufs, ["assign[0]", "assign[1]", "inv_norm"], lambda p, n: lib.anyloc_vlad_soft_assign_multi(
+            p["feats"], p["n_valid"], N, R, D, 2, vp(p, "centers[0]", "centers[1]"), Ks, (C.c_float * 2)(30.0, 10.0),
+            vp(p, "assign[0]", "assign[1]"), p["inv_norm"], p["ws"], n["ws"], st)
+    if entry in ("anyloc_vlad_accumulate", "anyloc_vlad_accumulate_varlen"):
+        # given per-row labels (some -1) or soft weights and 1/|x|: every accumulation route of the generate calls
+        if entry == "anyloc_vlad_accumulate":
+            B, N, D, K, soft = shape
+            R = B * N
+        else:
+            D, K, lens, soft = shape
+            B, R, N = len(lens), sum(lens) + 20, max(lens)
+        x, c = vlad_inputs(R, D, K)
+        lab = torch.randint(0, K, (R,), device="cuda", generator=g(9)).int()
+        lab[::7] = -1
+        bufs = dict(feats=x, labels=None if soft else lab, assign=torch.softmax(rnd(R, K, seed=3), 1) if soft else None,
+                    inv_norm=1.0 / x.norm(dim=1), centers=c, vlad=B * K * D * 4,
+                    ws=nb(lib, "anyloc_vlad_accumulate_workspace_bytes", B, N, D, K, int(soft)))
+        if entry == "anyloc_vlad_accumulate":
+            bufs["n_valid"] = i32([N - 7 * b for b in range(B)])
+            return bufs, ["vlad"], lambda p, n: lib.anyloc_vlad_accumulate(
+                p["feats"], p["n_valid"], p["labels"], p["assign"], p["inv_norm"], p["centers"], B, N, D, K, 1, 1,
+                p["vlad"], p["ws"], n["ws"], st)
+        row0, r = [], 10
+        for ln in lens:
+            row0.append(r)
+            r += ln
+        bufs.update(row0=i64(row0), len=i32(lens))
+        return bufs, ["vlad"], lambda p, n: lib.anyloc_vlad_accumulate_varlen(
+            p["feats"], R, p["row0"], p["len"], B, p["labels"], p["assign"], p["inv_norm"], p["centers"], D, K, 1, 1,
+            p["vlad"], p["ws"], n["ws"], st)
+    if entry in ("anyloc_attention", "anyloc_attention_varlen"):
+        # fmt: ANYLOC_PAIR_TF32 (fp32 pairs), _F16 (anyloc_attention: tf32 pairs in, fp16 pairs out; _varlen: fp16
+        # pairs of 8 x both ways), _BF16 / _F16X1 (one 2-byte array each way)
+        D, heads = 384, 6
+        if entry == "anyloc_attention":
+            B, T, fmt, engine = shape
+            rows = B * T
+        else:
+            (fmt,) = shape
+            row0, lens = (C.c_int32 * 2)(90, 0), (C.c_int32 * 2)(50, 70)     # out of order, rows 70..89 unused
+            rows = 150
+        x = 0.5 * rnd(rows, 3 * D, seed=6)
+        if fmt in (2, 4):
+            qkv = dict(qkv_hi=(x if fmt == 2 else 8 * x).to(torch.bfloat16 if fmt == 2 else torch.float16),
+                       qkv_lo=None)
+        elif fmt == 1 and entry == "anyloc_attention_varlen":
+            hi = (8 * x).half()
+            qkv = dict(qkv_hi=hi, qkv_lo=(8 * x - hi.float()).half())
+        else:
+            qkv = dict(qkv_hi=x, qkv_lo=1e-4 * rnd(rows, 3 * D, seed=7))
+        osz = rows * D * (4 if fmt == 0 else 2)
+        bufs = dict(qkv, o_hi=osz, o_lo=osz if fmt in (0, 1) else None)
+        outs = [o for o in ("o_hi", "o_lo") if bufs[o] is not None]
+        if entry == "anyloc_attention":
+            return bufs, outs, lambda p, n: lib.anyloc_attention(p["qkv_hi"], p["qkv_lo"], B, T, D, heads, p["o_hi"],
+                                                                 p["o_lo"], fmt, engine, st)
+        return bufs, outs, lambda p, n: lib.anyloc_attention_varlen(p["qkv_hi"], p["qkv_lo"], 2, row0, lens, D, heads,
+                                                                    p["o_hi"], p["o_lo"], fmt, st)
     raise KeyError(entry)
 
 
@@ -307,6 +395,18 @@ SHAPES = {
     "anyloc_pca_accumulate": [(300, 70, 73)],
     "anyloc_pca_mirror": [(0, 70, 73)],
     "anyloc_pool": [(2, 9, 36)],
+    "anyloc_pool_varlen": [(36, (9, 0, 5))],
+    # the coarse (R >= 256) and FFMA assignments
+    "anyloc_vlad_label_multi": [(255, 85, 128), (256, 128, 128)],
+    "anyloc_vlad_soft_assign_multi": [(200, 100, 128)],
+    # accumulate3, accumulate2, sorted and soft
+    "anyloc_vlad_accumulate": [(2, 300, 256, 16, False), (1, 5000, 128, 64, False), (1, 300, 64, 500, False),
+                               (2, 100, 128, 16, True)],
+    "anyloc_vlad_accumulate_varlen": [(256, 16, (150, 0, 120), False), (64, 500, (200, 90), False),
+                                      (128, 16, (60, 40), True)],
+    # the tensor-core, SIMT, fp16-pair, bf16 and fp16 kernels (ANYLOC_GEMM_AUTO = 0, _SIMT = 1)
+    "anyloc_attention": [(2, 70, 0, 0), (2, 70, 0, 1), (2, 70, 1, 0), (2, 70, 2, 0), (2, 70, 4, 0)],
+    "anyloc_attention_varlen": [(0,), (1,), (2,), (4,)],
 }
 CASES = [(e, i) for e in SHAPES for i in range(len(SHAPES[e]))]
 
