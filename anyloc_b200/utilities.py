@@ -189,18 +189,17 @@ class _PcaDev:
         if not 0 <= k <= min(n, d):
             raise ValueError(f"n_components={k} must be between 0 and min(n_samples, n_features)={min(n, d)} with "
                              "svd_solver='full'")
-        self.mean_ = x.mean(dim=0)
-        xd = (x - self.mean_).double()
-        if n <= d:
-            ev, u = torch.linalg.eigh(xd @ xd.T)
-            ev, u = ev.flip(0).clamp_min(0), u.flip(1)
-            s = ev.sqrt()
-            vt = (u[:, :k].T @ xd) / s[:k, None].clamp_min(1e-300)
+        return self.fit_shared(_pca_decompose(x))
+
+    def fit_shared(self, eig):
+        """fit() from _pca_decompose of the rows, the part of the fit that does not depend on k"""
+        mean, xd, s, vec, n = eig
+        k = self.n_components
+        self.mean_ = mean
+        if xd is not None:
+            vt = (vec[:, :k].T @ xd) / s[:k, None].clamp_min(1e-300)
         else:
-            ev, v = torch.linalg.eigh(xd.T @ xd)
-            ev, v = ev.flip(0).clamp_min(0), v.flip(1)
-            s = ev.sqrt()
-            vt = v[:, :k].T.contiguous()
+            vt = vec[:, :k].T.contiguous()
         return self._set_components(vt, s, n)
 
     def _set_components(self, vt, s, n):
@@ -223,38 +222,7 @@ class _PcaDev:
         if not 0 <= k <= min(n, d):
             raise ValueError(f"n_components={k} must be between 0 and min(n_samples, n_features)={min(n, d)} with "
                              "svd_solver='full'")
-        m = min(n, d)
-        boxes = _pca_boxes(n, d, plan)
-        with torch.cuda.device(dev):
-            mu = torch.zeros(d, dtype=torch.float64, device=dev)
-            a = torch.zeros(m, m, dtype=torch.float64, device=dev)
-            if n > d:
-                for x in _pca_staged(rows, boxes, dev):
-                    _pca_colsum(x, mu)
-                mu /= n
-                for x in _pca_staged(rows, boxes, dev):
-                    _pca_accumulate("cov", x, mu, a)
-            else:
-                for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
-                    _pca_colsum(x, mu[c0:c1])
-                    mu[c0:c1] /= n
-                    _pca_accumulate("gram", x, mu[c0:c1], a)
-            _lib.check(_lib.load().anyloc_pca_mirror(_lib.ptr(a), m, m, _lib.stream_ptr()), "anyloc_pca_mirror")
-            ev, vec = torch.linalg.eigh(a)
-            del a
-            ev, vec = ev.flip(0).clamp_min(0), vec.flip(1)
-            s = ev.sqrt()
-            if n <= d:
-                u = vec[:, :k].contiguous()
-                del vec
-                vt = torch.zeros(k, d, dtype=torch.float64, device=dev)
-                for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
-                    _pca_accumulate("vt", x, mu[c0:c1], vt[:, c0:c1], u)
-                vt /= s[:k, None].clamp_min(1e-300)
-            else:
-                vt = vec[:, :k].T.contiguous()
-            self.mean_ = mu.float()
-            return self._set_components(vt, s, n)
+        return _pca_fit_streamed_dims(rows, plan, [self], dev)[0]
 
     def fit_randomized(self, rows, w, P, dev):
         """`sklearn.decomposition.PCA(k, svd_solver="randomized")`'s fit with its default parameters (_randomized_svd:
@@ -269,43 +237,7 @@ class _PcaDev:
         if not 1 <= k <= min(n, d):
             raise ValueError(f"n_components={k} must be between 1 and min(n_samples, n_features)={min(n, d)} with "
                              "svd_solver='randomized'")
-        _, n_iter, transpose = _pca_randomized_params(n, d, k)
-        boxes = _pca_boxes(n, d, ("cov", P))
-        with torch.cuda.device(dev):
-            mu = torch.zeros(d, dtype=torch.float64, device=dev)
-            for x in _pca_staged(rows, boxes, dev):
-                _pca_colsum(x, mu)
-            mu /= n
-
-            def xw(q):                                  # Xc q: [n, width]
-                q, out = q.contiguous(), torch.zeros(n, q.shape[1], dtype=torch.float64, device=dev)
-                for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
-                    _pca_accumulate("sketch", x, mu, out[r0:r1], q)
-                return out
-
-            def xtw(q):                                 # Xc^T q: [d, width], summed over the row pieces
-                q, out = q.contiguous(), torch.zeros(q.shape[1], d, dtype=torch.float64, device=dev)
-                for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
-                    _pca_accumulate("vt", x, mu, out, q[r0:r1])
-                return out.T
-            a, at = (xtw, xw) if transpose else (xw, xtw)
-            q = torch.from_numpy(w).to(device=dev, dtype=torch.float64)
-            for _ in range(n_iter):
-                q = _lu_pl(a(q))
-                q = _lu_pl(at(q))
-            q = torch.linalg.qr(a(q)).Q
-            # the SVD of B = Q^T A [l, min(n, d)] through the QR of B^T = Q2 R: B = R^T Q2^T, R^T = U^ S W^T
-            q2, r = torch.linalg.qr(at(q))
-            uh, s, wt = torch.linalg.svd(r.T)
-            vt = wt @ q2.T
-            uq = q @ uh
-            del q, q2
-            u_rows, vt = (vt[:k].T, uq[:, :k].T) if transpose else (uq[:, :k], vt[:k])
-            sign = _flip_signs(vt)
-            scale = math.sqrt(n - 1) if self.whiten else s[:k]
-            self.fit_rows_ = (u_rows * (sign.T * scale)).float()
-            self.mean_ = mu.float()
-            return self._set_components(vt.contiguous(), s, n)
+        return _pca_randomized_group(rows, [self], [w], P, dev)[0]
 
     def transform(self, x):
         y = _gemm_nt_dev(x - self.mean_, self.components_)
@@ -314,6 +246,129 @@ class _PcaDev:
             scale[scale < torch.finfo(scale.dtype).eps] = torch.finfo(scale.dtype).eps
             y = y / scale
         return y
+
+
+def _pca_decompose(x):
+    """The part of _PcaDev.fit on device fp32 rows x [n, d] that does not depend on k: the mean, and the eigenvectors and
+    singular values (largest first) of the fp64 Gram (n <= d) or covariance matrix of the centred rows -> (mean, xd,
+    s, vec, n).  xd, the centred fp64 rows, is kept for the Gram route's vt only, else None."""
+    n, d = x.shape
+    mean = x.mean(dim=0)
+    xd = (x - mean).double()
+    ev, vec = torch.linalg.eigh(xd @ xd.T if n <= d else xd.T @ xd)
+    ev, vec = ev.flip(0).clamp_min(0), vec.flip(1)
+    return mean, (xd if n <= d else None), ev.sqrt(), vec, n
+
+
+def _pca_fit_streamed_dims(rows, plan, pcas, dev):
+    """_PcaDev.fit_streamed of every _PcaDev in `pcas` on the same rows (a _PcaRows): one mean pass, one accumulation
+    of the m x m matrix, one mirror and one eigh for all of them.  On the Gram route the vt pass stages each column slab
+    once and accumulates every member's u[:, :k]^T Xc on it, each at its own k -> pcas"""
+    n, d = rows.shape
+    m = min(n, d)
+    boxes = _pca_boxes(n, d, plan)
+    with torch.cuda.device(dev):
+        mu = torch.zeros(d, dtype=torch.float64, device=dev)
+        a = torch.zeros(m, m, dtype=torch.float64, device=dev)
+        if n > d:
+            for x in _pca_staged(rows, boxes, dev):
+                _pca_colsum(x, mu)
+            mu /= n
+            for x in _pca_staged(rows, boxes, dev):
+                _pca_accumulate("cov", x, mu, a)
+        else:
+            for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                _pca_colsum(x, mu[c0:c1])
+                mu[c0:c1] /= n
+                _pca_accumulate("gram", x, mu[c0:c1], a)
+        _lib.check(_lib.load().anyloc_pca_mirror(_lib.ptr(a), m, m, _lib.stream_ptr()), "anyloc_pca_mirror")
+        ev, vec = torch.linalg.eigh(a)
+        del a
+        ev, vec = ev.flip(0).clamp_min(0), vec.flip(1)
+        s = ev.sqrt()
+        if n <= d:
+            us = [vec[:, :p.n_components].contiguous() for p in pcas]
+            del vec
+            vts = [torch.zeros(u.shape[1], d, dtype=torch.float64, device=dev) for u in us]
+            for (_, _, c0, c1), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                for u, vt in zip(us, vts):
+                    _pca_accumulate("vt", x, mu[c0:c1], vt[:, c0:c1], u)
+            for vt in vts:
+                vt /= s[:vt.shape[0], None].clamp_min(1e-300)
+        else:
+            vts = [vec[:, :p.n_components].T.contiguous() for p in pcas]
+        for p, vt in zip(pcas, vts):
+            p.mean_ = mu.float()
+            p._set_components(vt, s, n)
+    return pcas
+
+
+def _pca_randomized_schedule(n, d, ks):
+    """The row passes of randomized fits of n x d rows at every k of ks run together (_pca_randomized_group), in order:
+    [(forward, [(member, then)])].  forward: the pass multiplies by A (Xc, or Xc^T when n < d), else by A^T; the
+    transpose depends on n < d only, so a pass has one direction for every member.  then: what the member does with
+    its product -- "lu" (a power iteration's normaliser), "qr" (the range's basis Q) or "svd" (B = Q^T A and its
+    decomposition, the member's last pass).  Members with n_iter = 4 leave after pass 9, those with 7 after pass 15."""
+    steps = [2 * _pca_randomized_params(n, d, k)[1] + 2 for k in ks]
+    return [(p % 2 == 0, [(i, "lu" if p < s - 2 else "qr" if p == s - 2 else "svd")
+                          for i, s in enumerate(steps) if p < s]) for p in range(max(steps))]
+
+
+def _pca_randomized_group(rows, pcas, ws, P, dev):
+    """_PcaDev.fit_randomized of every _PcaDev in `pcas` (test matrix ws[i]) on the same rows (a _PcaRows) read in row
+    pieces of P: one mean pass, then the passes of _pca_randomized_schedule.  Each pass stages every row piece once and
+    runs the sketch or vt accumulate of every member still running on it -> pcas"""
+    n, d = rows.shape
+    transpose = n < d
+    boxes = _pca_boxes(n, d, ("cov", P))
+    with torch.cuda.device(dev):
+        mu = torch.zeros(d, dtype=torch.float64, device=dev)
+        for x in _pca_staged(rows, boxes, dev):
+            _pca_colsum(x, mu)
+        mu /= n
+
+        def one_pass(forward, qs):
+            """Xc q ([n, width], "sketch") or Xc^T q ([d, width], summed over the row pieces) of every q"""
+            sketch = forward != transpose
+            qs = [q.contiguous() for q in qs]
+            outs = [torch.zeros(*((n, q.shape[1]) if sketch else (q.shape[1], d)), dtype=torch.float64, device=dev)
+                    for q in qs]
+            for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
+                for q, out in zip(qs, outs):
+                    if sketch:
+                        _pca_accumulate("sketch", x, mu, out[r0:r1], q)
+                    else:
+                        _pca_accumulate("vt", x, mu, out, q[r0:r1])
+            return outs if sketch else [out.T for out in outs]
+
+        qs = [torch.from_numpy(w).to(device=dev, dtype=torch.float64) for w in ws]
+        for forward, live in _pca_randomized_schedule(n, d, [p.n_components for p in pcas]):
+            for (i, then), y in zip(live, one_pass(forward, [qs[i] for i, _ in live])):
+                if then == "lu":
+                    qs[i] = _lu_pl(y)
+                elif then == "qr":
+                    qs[i] = torch.linalg.qr(y).Q
+                else:
+                    _pca_randomized_finish(pcas[i], qs[i], y, mu, n, transpose)
+                    qs[i] = None
+    return pcas
+
+
+def _pca_randomized_finish(pca, q, y, mu, n, transpose):
+    """The end of a randomized fit from Q and y = A^T Q: the SVD of B = Q^T A [l, min(n, d)] through the QR of
+    B^T = Q2 R: B = R^T Q2^T, R^T = U^ S W^T"""
+    k = pca.n_components
+    q2, r = torch.linalg.qr(y)
+    uh, s, wt = torch.linalg.svd(r.T)
+    vt = wt @ q2.T
+    uq = q @ uh
+    del q, q2
+    u_rows, vt = (vt[:k].T, uq[:, :k].T) if transpose else (uq[:, :k], vt[:k])
+    sign = _flip_signs(vt)
+    scale = math.sqrt(n - 1) if pca.whiten else s[:k]
+    pca.fit_rows_ = (u_rows * (sign.T * scale)).float()
+    pca.mean_ = mu.float()
+    pca._set_components(vt.contiguous(), s, n)
 
 
 def reduce_pca(train_descs: np.ndarray, test_descs: np.ndarray, lower_dim: int, low_factor: float = 0.0,
@@ -418,6 +473,9 @@ def _pca_staged(rows, boxes, dev):
     host = [torch.empty(cap, pin_memory=True) for _ in range(min(2, len(boxes)))]
     raw = [torch.empty(cap, device=dev) for _ in host]
     cs, xs = torch.cuda.current_stream(), torch.cuda.Stream()
+    # the stages come from torch's allocator on cs and may reuse memory that work already queued on cs still reads
+    # (the previous pass's last pieces): the side stream's copies into them start after that work
+    xs.wait_stream(cs)
     copied, freed = [None, None], [None, None]
 
     def stage(j):
@@ -466,13 +524,20 @@ def _pca_accumulate(mode, x, mu, out, u=None):
 def _pca_project_streamed(rows, project, k, dev):
     """project(x) (device rows -> [rows, k] fp32) of every row of `rows`, fed in row pieces of at most one staging
     buffer -> host fp32 [n, k]"""
+    return _pca_project_dims(rows, [project], [k], dev)[0]
+
+
+def _pca_project_dims(rows, projects, ks, dev):
+    """_pca_project_streamed of several projections (projects[i] -> [rows, ks[i]]): each row piece is staged once and
+    every projection runs on it -> [host fp32 [n, ks[i]]]"""
     n, d = rows.shape
-    out = torch.empty(n, k)
+    outs = [torch.empty(n, k) for k in ks]
     boxes = _pca_boxes(n, d, ("cov", max(1, min(n, _STAGE_BYTES // (4 * d)))))
     with torch.cuda.device(dev):
         for (r0, r1, _, _), x in zip(boxes, _pca_staged(rows, boxes, dev)):
-            out[r0:r1].copy_(project(x))
-    return out
+            for out, project in zip(outs, projects):
+                out[r0:r1].copy_(project(x))
+    return outs
 
 
 def _pca_fit_any(rows, k, dev):
@@ -546,22 +611,34 @@ def _pca_fit_randomized(rows, k, dev, whiten=False):
         raise ValueError(f"n_components={k} must be between 1 and min(n_samples, n_features)={min(n, d)} with "
                          "svd_solver='randomized'")
     f32 = all(q.dtype == torch.float32 for q in rows.parts)
-    p = rows.parts[0]
     P = min(n, _PCA_PIECE_MAX_ROWS)
-    if not (len(rows.parts) == 1 and p.device == dev and p.dtype == torch.float32 and p.stride(1) == 1 and
-            p.stride(0) >= d):
+    if not _pca_in_place(rows, dev):
         plan = _pca_randomized_plan(n, d, _pca_randomized_params(n, d, k)[0], _device_budget(dev), _STAGE_BYTES)
         if plan is None:
-            x = torch.empty(n, d, device=dev)
-            boxes = _pca_boxes(n, d, ("cov", max(1, min(n, _STAGE_BYTES // (4 * d)))))
-            with torch.cuda.device(dev):
-                for (r0, r1, _, _), piece in zip(boxes, _pca_staged(rows, boxes, dev)):
-                    x[r0:r1].copy_(piece)
-            rows = _PcaRows([x])
+            rows = _pca_upload(rows, dev)
         else:
             P = plan
     w = _pca_test_matrix(n, d, k, f32)
     return _PcaDev(k, whiten=whiten).fit_randomized(rows, w, P, dev)
+
+
+def _pca_in_place(rows, dev):
+    """whether a randomized fit reads `rows` (a _PcaRows) in place: one device fp32 matrix with unit column stride"""
+    p = rows.parts[0]
+    d = rows.shape[1]
+    return (len(rows.parts) == 1 and p.device == dev and p.dtype == torch.float32 and p.stride(1) == 1 and
+            p.stride(0) >= d)
+
+
+def _pca_upload(rows, dev):
+    """`rows` (a _PcaRows) uploaded once as one device fp32 matrix, through the pinned stages -> _PcaRows"""
+    n, d = rows.shape
+    x = torch.empty(n, d, device=dev)
+    boxes = _pca_boxes(n, d, ("cov", max(1, min(n, _STAGE_BYTES // (4 * d)))))
+    with torch.cuda.device(dev):
+        for (r0, r1, _, _), piece in zip(boxes, _pca_staged(rows, boxes, dev)):
+            x[r0:r1].copy_(piece)
+    return _PcaRows([x])
 
 
 def _reduce_pca_randomized(train_descs, test_descs, lower_dim, low_factor, fallback, whitening, dev):
@@ -586,6 +663,259 @@ def _reduce_pca_randomized(train_descs, test_descs, lower_dim, low_factor, fallb
     basis = torch.cat((pca.components_[:n_top], pca.components_[-n_low:])).contiguous()
     with torch.cuda.device(dev):
         return _gemm_nt_dev(tr - pca.mean_, basis).cpu(), _gemm_nt_dev(te - pca.mean_, basis).cpu()
+
+
+# ------------------------------------------------------------------ several PCA dimensions from one fit (extension)
+def reduce_pca_dims(train_descs: Union[np.ndarray, torch.Tensor], test_descs: Union[np.ndarray, torch.Tensor],
+                    lower_dims: List[int], low_factor: float = 0.0, fallback: int = 256, svd_solver: str = "full",
+                    whitening: bool = False) -> List[Tuple[np.ndarray, np.ndarray]]:
+    """reduce_pca at every dimension of `lower_dims`, sharing the work that does not depend on the dimension -> a list
+    of (train_i, test_i).  Element i equals, bit for bit and in type and dtype, reduce_pca(train_descs, test_descs,
+    lower_dims[i], low_factor, fallback, svd_solver, whitening) run in list order from the same numpy global generator
+    state, and numpy's generator ends where those calls leave it.  Dimensions may repeat and come in any order.
+
+    Shared: the exact fit's mean, Gram / covariance matrix and eigh (each member then takes its own vt at its own k);
+    the low_factor branch's exact `fallback` pre-reduction and full-basis fit; the randomized fits' mean pass and every
+    row pass of their power iterations (_pca_randomized_group).  Streamed passes stage each row piece once for all
+    members.  The randomized members draw their test matrices in list order, each its own draw.
+
+    Unlike the sequential calls, which stop at the first bad member, every refusal comes before any work and leaves
+    the generator untouched: ValueError for an empty list, a dimension out of range for the solver, or an exact fit
+    whose m = min(n_samples, n_features) is beyond what the eigensolver takes (_PCA_EIGH_MAX_M).  MemoryError only where
+    a member's own call would raise it; members that do not fit on the device together run in consecutive groups."""
+    assert 0 <= low_factor <= 1
+    dims = [int(k) for k in lower_dims]
+    as_np = type(train_descs) == np.ndarray
+    (n, d), n_te = train_descs.shape, test_descs.shape[0]
+    _pca_dims_check(n, d, n_te, dims, low_factor, fallback, svd_solver)
+    dev = _lib.require_cuda(None)
+    draws = [_pca_member_draws(n, d, n_te, k, low_factor, fallback, svd_solver) for k in dims]
+    if svd_solver == "randomized" and (low_factor == 0.0 or n < d):
+        outs = _reduce_pca_dims_randomized(train_descs, test_descs, dims, low_factor, fallback, whitening, draws, dev)
+    else:
+        outs = _reduce_pca_dims_exact(train_descs, test_descs, dims, low_factor, fallback, whitening, dev)
+        _pca_draw(sum(draws, []), False)        # randomized with low_factor, n >= d: the skips of the exact fits
+    return [(a.numpy(), b.numpy()) if as_np else (a, b) for a, b in outs]
+
+
+def _pca_dims_check(n, d, n_te, dims, low_factor, fallback, svd_solver):
+    """reduce_pca_dims' refusals, before any work: the messages of _PcaDev.fit and _pca_fit_randomized for the fits each
+    member's call would make, and the exact fits' m beyond _PCA_EIGH_MAX_M"""
+    if not dims:
+        raise ValueError("reduce_pca_dims: lower_dims is empty")
+
+    def full(k, rows, cols):
+        if not 0 <= k <= min(rows, cols):
+            raise ValueError(f"n_components={k} must be between 0 and min(n_samples, n_features)={min(rows, cols)} "
+                             "with svd_solver='full'")
+        if min(rows, cols) > _PCA_EIGH_MAX_M:
+            raise ValueError(f"reduce_pca_dims: m = min(n_samples, n_features) = {min(rows, cols)} is beyond the "
+                             f"{_PCA_EIGH_MAX_M} x {_PCA_EIGH_MAX_M} fp64 matrices the eigensolver (torch.linalg.eigh, "
+                             "cuSOLVER syevd) takes; svd_solver='randomized' has no such limit")
+
+    def randomized(k, rows, cols):
+        if not 1 <= k <= min(rows, cols):
+            raise ValueError(f"n_components={k} must be between 1 and min(n_samples, n_features)={min(rows, cols)} "
+                             "with svd_solver='randomized'")
+    if svd_solver == "randomized" and low_factor == 0.0:
+        for k in dims:
+            randomized(k, n, d)
+    elif low_factor == 0.0:
+        for k in dims:
+            full(k, n, d)
+    elif n < d:                     # the fallback pre-reduction, then the full basis of the [n, fallback] rows
+        (randomized if svd_solver == "randomized" else full)(fallback, n + n_te, d)
+        full(fallback, n, fallback)
+    else:                           # the full basis of the rows
+        full(d, n, d)
+
+
+def _pca_member_draws(n, d, n_te, k, low_factor, fallback, svd_solver):
+    """What reduce_pca(n x d training rows, n_te test rows, k, ...) takes from numpy's global generator, in order:
+    [(n', d', k', draw)], draw=True for _pca_test_matrix(n', d', k'), False for _pca_skip_test_matrix(n', d', k')"""
+    if svd_solver != "randomized":
+        return []
+    if low_factor == 0.0:
+        return [(n, d, k, True)]
+    if n < d:                       # the randomized fallback pre-reduction, then the exact full-basis fit's skip
+        return [(n + n_te, d, fallback, True), (n, fallback, fallback, False)]
+    return [(n, d, d, False)]
+
+
+def _pca_draw(draws, f32):
+    """Take `draws` (_pca_member_draws) from numpy's global generator in order -> the test matrices drawn"""
+    ws = []
+    for a, b, k, draw in draws:
+        if draw:
+            ws.append(_pca_test_matrix(a, b, k, f32))
+        else:
+            _pca_skip_test_matrix(a, b, k)
+    return ws
+
+
+def _pca_member_bytes(m, d, k):
+    """Device bytes one member of an exact sweep adds to the shared fit: its fp64 u [m, k] and vt [k, d], and its fp32
+    components [k, d]"""
+    return 8 * k * (m + d) + 4 * k * d
+
+
+def _pca_exact_groups(m, d, ks, fixed, budget):
+    """Consecutive groups of an exact sweep's members (dimensions ks) that share one fit: members join the group
+    before while its _pca_member_bytes, summed, fit the `budget` beside the `fixed` bytes of the fit itself
+    (_pca_in_memory_bytes in memory, the m x m matrix and its eigh streamed).  A member that does not fit with the
+    group starts the next -> [[member index]]"""
+    groups, used = [], 0
+    for i, k in enumerate(ks):
+        b = _pca_member_bytes(m, d, k)
+        if groups and fixed + used + b <= budget:
+            groups[-1].append(i)
+            used += b
+        else:
+            groups.append([i])
+            used = b
+    return groups
+
+
+def _pca_randomized_groups(n, d, ls, plans, in_place, budget, stage_bytes):
+    """Consecutive groups of a randomized sweep's members (ls[i] = k + 10 test vectors, plans[i] its own call's
+    _pca_randomized_plan, None for rows read in place) that run their fits together -> [(members, P, upload)].  The
+    mean pass's fp64 column sums depend on the row pieces, so a group's members are those whose own calls read the rows
+    in the same pieces: in place or uploaded in pieces of min(n, 2^20) rows, or streamed in pieces of plans[i] rows.
+    Members join the group before while the fits' matrices (_pca_randomized_bytes, summed) fit the `budget` beside the
+    rows: nothing for rows read in place, the uploaded rows (4 n d) beside the larger of the matrices and the upload's
+    two staging copies, or two device copies of a streamed piece.  A member that does not fit with the group starts
+    the next; alone, it runs as its own call does."""
+    piece = 4 * d * max(1, min(n, stage_bytes // (4 * d)))
+
+    def fits(mats, plan):
+        if in_place:
+            return mats <= budget
+        if plan is None:
+            return 4 * n * d + max(mats, 2 * piece) <= budget
+        return mats + 8 * d * plan <= budget
+    groups, mats = [], 0
+    for i, (l, plan) in enumerate(zip(ls, plans)):
+        b = _pca_randomized_bytes(n, d, l)
+        if groups and plans[groups[-1][0][-1]] == plan and fits(mats + b, plan):
+            groups[-1][0].append(i)
+            mats += b
+        else:
+            groups.append(([i], min(n, _PCA_PIECE_MAX_ROWS) if plan is None else plan, not in_place and plan is None))
+            mats = b
+    return groups
+
+
+def _pca_randomized_dims(rows, ks, whiten, draws, dev):
+    """_pca_fit_randomized(rows, ks[i], dev, whiten) for every i, group by group (_pca_randomized_groups): a group
+    takes its members' draws (_pca_member_draws) in list order, uploads the rows once if its members' own calls would,
+    and runs its fits together (_pca_randomized_group).  Yields (members, fitted _PcaDevs) per group."""
+    n, d = rows.shape
+    f32 = all(q.dtype == torch.float32 for q in rows.parts)
+    in_place = _pca_in_place(rows, dev)
+    ls = [_pca_randomized_params(n, d, k)[0] for k in ks]
+    budget = _device_budget(dev)
+    plans = [None if in_place else _pca_randomized_plan(n, d, l, budget, _STAGE_BYTES) for l in ls]
+    for group, P, upload in _pca_randomized_groups(n, d, ls, plans, in_place, budget, _STAGE_BYTES):
+        ws = _pca_draw(sum((draws[i] for i in group), []), f32)
+        pcas = [_PcaDev(ks[i], whiten=whiten) for i in group]
+        yield group, _pca_randomized_group(_pca_upload(rows, dev) if upload else rows, pcas, ws, P, dev)
+
+
+def _reduce_pca_dims_randomized(train_descs, test_descs, dims, low_factor, fallback, whitening, draws, dev):
+    """reduce_pca_dims for the routes of _reduce_pca_randomized -> [(tr, te) host tensors]"""
+    tr, te = _PcaRows([train_descs]), _PcaRows([test_descs])
+    outs = []
+    if low_factor == 0.0:
+        for group, pcas in _pca_randomized_dims(tr, dims, whitening, draws, dev):
+            tes = _pca_project_dims(te, [p.transform for p in pcas], [dims[i] for i in group], dev)
+            outs += [(p.fit_rows_.cpu(), t) for p, t in zip(pcas, tes)]
+        return outs
+    n = tr.shape[0]
+    # every member's own call draws its own fallback test matrix, so the pre-reductions are a randomized sweep too
+    for group, pcas in _pca_randomized_dims(_PcaRows(tr.parts + te.parts), [fallback] * len(dims), False, draws, dev):
+        for i, j in enumerate(group):
+            both, pcas[i] = pcas[i].fit_rows_, None
+            low_tr, low_te = both[:n].contiguous(), both[n:].contiguous()
+            print(f"Too few samples, fallback to {fallback}d first")
+            basis, mean = _pca_low_factor_basis(_pca_fit_any(_PcaRows([low_tr]), fallback, dev), dims[j], low_factor)
+            with torch.cuda.device(dev):
+                outs.append((_gemm_nt_dev(low_tr - mean, basis).cpu(), _gemm_nt_dev(low_te - mean, basis).cpu()))
+    return outs
+
+
+def _pca_low_factor_basis(pca, lower_dim, low_factor):
+    """reduce_pca's low_factor basis: the top n_top and bottom n_low components of a full-basis fit, printing the split
+    as reduce_pca does -> (basis, mean)"""
+    n_low = int(low_factor * lower_dim)
+    n_top = lower_dim - n_low
+    print(f"Up: {n_top}, Down: {n_low}")
+    return torch.cat((pca.components_[:n_top], pca.components_[-n_low:])).contiguous(), pca.mean_
+
+
+def _reduce_pca_dims_exact(train_descs, test_descs, dims, low_factor, fallback, whitening, dev):
+    """reduce_pca_dims for the exact routes of reduce_pca and _reduce_pca_streamed; the route is the one every member's
+    own call takes, as it does not depend on the dimension -> [(tr, te) host tensors]"""
+    (n, d), n_te = train_descs.shape, test_descs.shape[0]
+    n_fit, n_held = (n + n_te, n + n_te) if low_factor != 0.0 and n < d else (n, n_te)
+    budget = _device_budget(dev)
+    plan = _pca_plan(n_fit, d, n_held, budget, _STAGE_BYTES)
+    if low_factor != 0.0:
+        return _reduce_pca_dims_low_factor(train_descs, test_descs, dims, low_factor, fallback, plan, dev)
+    m, outs = min(n, d), []
+    if plan is None:
+        tr, te = _as_device_f32(train_descs, dev), _as_device_f32(test_descs, dev)
+        for group in _pca_exact_groups(m, d, dims, _pca_in_memory_bytes(n, d, n_te), budget):
+            eig = _pca_decompose(tr)
+            pcas = [_PcaDev(dims[i], whiten=whitening).fit_shared(eig) for i in group]
+            del eig
+            outs += [(p.transform(tr).cpu(), p.transform(te).cpu()) for p in pcas]
+        return outs
+    tr, te = _PcaRows([train_descs]), _PcaRows([test_descs])
+    for group in _pca_exact_groups(m, d, dims, 8 * _PCA_EIGH_MATRICES * m * m, budget):
+        pcas = _pca_fit_streamed_dims(tr, plan, [_PcaDev(dims[i], whiten=whitening) for i in group], dev)
+        projects, ks = [p.transform for p in pcas], [dims[i] for i in group]
+        outs += zip(_pca_project_dims(tr, projects, ks, dev), _pca_project_dims(te, projects, ks, dev))
+    return outs
+
+
+def _reduce_pca_dims_low_factor(train_descs, test_descs, dims, low_factor, fallback, plan, dev):
+    """reduce_pca_dims' exact low_factor branch: the fallback pre-reduction and the full-basis fit, which do not depend
+    on the dimension, once; then each member's own top / bottom basis.  In memory (plan None) as reduce_pca, else
+    streamed as _reduce_pca_streamed, whose final projections stage each row piece once for all members."""
+    n_samples, n_components = train_descs.shape
+    few = n_samples < n_components
+    if plan is None:
+        tr, te = _as_device_f32(train_descs, dev), _as_device_f32(test_descs, dev)
+        if few:
+            both = torch.cat((tr, te))
+            both = _PcaDev(fallback).fit(both).transform(both)
+            tr, te = both[:n_samples].contiguous(), both[n_samples:].contiguous()
+        pca = _PcaDev(tr.shape[1]).fit(tr)
+        outs = []
+        for k in dims:
+            if few:
+                print(f"Too few samples, fallback to {fallback}d first")
+            basis, mean = _pca_low_factor_basis(pca, k, low_factor)
+            outs.append((_gemm_nt_dev(tr - mean, basis).cpu(), _gemm_nt_dev(te - mean, basis).cpu()))
+        return outs
+    tr, te = _PcaRows([train_descs]), _PcaRows([test_descs])
+    if few:
+        pre = _PcaDev(fallback).fit_streamed(_PcaRows(tr.parts + te.parts), plan, dev)
+        tr = _PcaRows([_pca_project_streamed(tr, pre.transform, fallback, dev)])
+        te = _PcaRows([_pca_project_streamed(te, pre.transform, fallback, dev)])
+        pca = _pca_fit_any(tr, tr.shape[1], dev)
+    else:
+        pca = _PcaDev(n_components).fit_streamed(tr, plan, dev)
+    bases = []
+    for k in dims:
+        if few:
+            print(f"Too few samples, fallback to {fallback}d first")
+        bases.append(_pca_low_factor_basis(pca, k, low_factor))
+
+    def project(basis, mean):
+        return lambda x: _gemm_nt_dev(x - mean, basis)
+    projects, ks = [project(*b) for b in bases], [b[0].shape[0] for b in bases]
+    return list(zip(_pca_project_dims(tr, projects, ks, dev), _pca_project_dims(te, projects, ks, dev)))
 
 
 # ------------------------------------------------------------------ image pre-processing (extension)
