@@ -17,8 +17,8 @@ FACET = {"query": 0, "key": 1, "value": 2, "token": 3}
 FFN = {"mlp": 0, "swiglufused": 1}
 EPI = {"bias": 0, "bias_split": 1, "gelu_split": 2, "swiglu_split": 3, "ls_resid": 4}
 ENGINE = {"auto": 0, "simt": 1, "tc3": 2}
-# bf16 / fp8 / f16x1: single bf16 / e4m3 / fp16 (ANYLOC_PAIR_BF16 / _FP8 / _F16X1)
-PAIR = {"tf32": 0, "f16": 1, "bf16": 2, "fp8": 3, "f16x1": 4}
+# bf16 / fp8 / f16x1: single bf16 / e4m3 / fp16 (ANYLOC_PAIR_BF16 / _FP8 / _F16X1); bf16pair: bf16 pairs (_BF16X3)
+PAIR = {"tf32": 0, "f16": 1, "bf16": 2, "fp8": 3, "f16x1": 4, "bf16pair": 5}
 ACT_SCALE = 8.0     # kActScale in csrc/common.cuh
 VIT_VARLEN_MAX_B = 128      # ANYLOC_VIT_VARLEN_MAX_B: images per anyloc_vit_extract_varlen call
 PREPROCESS_VARLEN_BATCH = 64    # ANYLOC_PREPROCESS_VARLEN_BATCH: images per launch of anyloc_preprocess_u8_varlen

@@ -86,26 +86,29 @@ int pca_atb_launch(int, const float*, int64_t, const double*, const double*, int
                    int64_t, cudaStream_t);
 int pca_mirror_launch(double*, int, int64_t, cudaStream_t);
 
-// fmt: ANYLOC_PAIR_* of the operands.  The single formats run on the tensor cores only: they run the wgmma kernel at
-// every M (no SIMT route, so a row's result never depends on how many rows share the call) and refuse the SIMT
-// engine.  Single e4m3's a_lo holds A's fp32 row scales.
+// fmt: ANYLOC_PAIR_* of the operands.  The single formats and the bf16 pairs run on the tensor cores only: they run
+// the wgmma kernel at every M (no SIMT route, so a row's result never depends on how many rows share the call) and
+// refuse the SIMT engine.  Single e4m3's a_lo holds A's fp32 row scales; the bf16 pairs need both lo operands.
 static int gemm_dispatch(const void* a_hi, const void* a_lo, int lda, const void* b_hi, const void* b_lo,
                          int ldb, int M, int N, int K, const EpiParams& ep, int engine, int fmt, cudaStream_t st) {
   if (M == 0 || N == 0) return ANYLOC_OK;
   const FormatInfo& f = format_info(fmt);
   const double flops = 2.0 * M * N * K;
   if (f.tc_only) {
-    const bool a_lo_ok = f.row_scales ? a_lo && (reinterpret_cast<uintptr_t>(a_lo) & 3) == 0 : !a_lo;
-    if (engine == ANYLOC_GEMM_SIMT || !a_lo_ok || b_lo ||
-        !gemm_tc_supported(a_hi, nullptr, lda, b_hi, nullptr, ldb, M, N, K, ep, fmt)) {
+    const bool a_lo_ok = f.row_scales ? a_lo && (reinterpret_cast<uintptr_t>(a_lo) & 3) == 0 : f.lo ? a_lo != nullptr
+                                                                                                 : !a_lo;
+    const bool b_lo_ok = f.lo ? b_lo != nullptr : !b_lo;
+    if (engine == ANYLOC_GEMM_SIMT || !a_lo_ok || !b_lo_ok ||
+        !gemm_tc_supported(a_hi, f.lo ? a_lo : nullptr, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt)) {
       set_error("gemm: the %s format runs on the tensor-core engine only, with 16-byte aligned operands, K, lda and "
                 "ldb multiples of %d%s (M=%d N=%d K=%d lda=%d ldb=%d engine=%d)", f.name, 16 / f.esz,
-                f.row_scales ? ", A's row scales and no B lo operand" : " and no lo operands", M, N, K, lda, ldb,
+                f.row_scales ? ", A's row scales and no B lo operand" : f.lo ? " and both lo operands"
+                                                                          : " and no lo operands", M, N, K, lda, ldb,
                 engine);
       return ANYLOC_ERR_UNSUPPORTED;
     }
     ProfScope ps(PC_GEMM_TC, st, flops);
-    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, nullptr, ldb, M, N, K, ep, fmt, st);
+    return gemm_tc_launch(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt, st);
   }
   bool tc_ok = gemm_tc_supported(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep, fmt);
   if (engine == ANYLOC_GEMM_TC3 && !tc_ok) {
@@ -163,14 +166,17 @@ extern "C" int anyloc_gemm_nt(const void* a_hi, const void* a_lo, int lda, const
                               int ldo, int out_dtype, int engine, void* stream) {
   ANYLOC_REQUIRE(a_hi && b_hi && out, "gemm_nt: null pointer");
   ANYLOC_REQUIRE(M >= 0 && N >= 0 && K > 0, "gemm_nt: bad dims");
-  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_F16X1, "gemm_nt: bad in_dtype %d", in_dtype);
-  ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_F16X1 && out_dtype != ANYLOC_PAIR_FP8,
+  ANYLOC_REQUIRE(in_dtype >= ANYLOC_PAIR_TF32 && in_dtype <= ANYLOC_PAIR_BF16X3, "gemm_nt: bad in_dtype %d", in_dtype);
+  ANYLOC_REQUIRE(out_dtype >= ANYLOC_PAIR_TF32 && out_dtype <= ANYLOC_PAIR_BF16X3 && out_dtype != ANYLOC_PAIR_FP8,
                  "gemm_nt: bad out_dtype %d", out_dtype);
   ANYLOC_REQUIRE(epilogue >= ANYLOC_EPI_BIAS && epilogue <= ANYLOC_EPI_LS_RESID, "gemm_nt: bad epilogue %d", epilogue);
   const FormatInfo& f = format_info(in_dtype);
-  ANYLOC_REQUIRE(f.lo ? format_info(out_dtype).lo : out_dtype == f.out, "gemm_nt: %s inputs write %s outputs "
-                 "(in_dtype=%d out_dtype=%d)", f.name, f.lo ? "tf32-pair or fp16-pair" : format_info(f.out).name,
-                 in_dtype, out_dtype);
+  const bool either_pair = f.lo && !f.tc_only;     // tf32 or fp16 pair inputs write either of those pairs
+  ANYLOC_REQUIRE(either_pair ? out_dtype == ANYLOC_PAIR_TF32 || out_dtype == ANYLOC_PAIR_F16 : out_dtype == f.out,
+                 "gemm_nt: %s inputs write %s outputs (in_dtype=%d out_dtype=%d)", f.name,
+                 either_pair ? "tf32-pair or fp16-pair" : format_info(f.out).name, in_dtype, out_dtype);
+  if (f.lo && f.tc_only)
+    ANYLOC_REQUIRE(a_lo && b_lo, "gemm_nt: the %s format needs both lo operands (a_lo and b_lo)", f.name);
   if (f.row_scales)
     ANYLOC_REQUIRE(a_lo && !b_lo && !out_lo, "gemm_nt: %s inputs take A's row scales in a_lo, no b_lo and no out_lo",
                    f.name);
@@ -284,18 +290,23 @@ static int attention_dispatch(const float* qkv_hi, const float* qkv_lo, int B, i
 extern "C" int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int D, int heads,
                                 void* o_hi, void* o_lo, int out_dtype, int engine, void* stream) {
   const FormatInfo& f = format_info(out_dtype);
-  if (!f.lo && f.out == out_dtype) {     // single in and out: a format the qkv epilogue writes
+  if (f.tc_only && f.out == out_dtype) {     // a tensor-core-only format in and out: one the qkv epilogue writes
     ANYLOC_REQUIRE(qkv_hi && o_hi, "attention: null pointer");
-    ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", f.name);
+    if (f.lo)
+      ANYLOC_REQUIRE(qkv_lo && o_lo, "attention: the %s format needs qkv_lo and o_lo", f.name);
+    else
+      ANYLOC_REQUIRE(!qkv_lo && !o_lo, "attention: the %s format has no lo arrays (qkv_lo, o_lo must be NULL)", f.name);
     ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
     ANYLOC_REQUIRE_ALIGNED(o_hi, 8, "attention", "o_hi", "64-bit stores of the tensor-core epilogue");
-    if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0) {
+    ANYLOC_REQUIRE_ALIGNED(o_lo, 8, "attention", "o_lo", "64-bit stores of the tensor-core epilogue");
+    if (engine == ANYLOC_GEMM_SIMT || (reinterpret_cast<uintptr_t>(qkv_hi) & 15) != 0 ||
+        (reinterpret_cast<uintptr_t>(qkv_lo) & 15) != 0) {
       set_error("attention: the %s format runs on the tensor-core engine only, with a 16-byte aligned qkv", f.name);
       return ANYLOC_ERR_UNSUPPORTED;
     }
     if (B == 0 || T == 0) return ANYLOC_OK;
     ProfScope ps(PC_ATTENTION, (cudaStream_t)stream, 4.0 * B * (double)T * T * D);
-    return attention_tc_launch(qkv_hi, nullptr, B, T, D, heads, o_hi, nullptr, out_dtype, (cudaStream_t)stream);
+    return attention_tc_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, out_dtype, (cudaStream_t)stream);
   }
   ANYLOC_REQUIRE(qkv_hi && o_hi && o_lo, "attention: null pointer");
   ANYLOC_REQUIRE(D == heads * 64, "attention: head_dim must be 64 (D=%d heads=%d)", D, heads);
@@ -327,7 +338,7 @@ extern "C" int anyloc_attention_varlen(const void* qkv_hi, const void* qkv_lo, i
                                        const int32_t* len, int D, int heads, void* o_hi, void* o_lo, int fmt,
                                        void* stream) {
   ANYLOC_REQUIRE(fmt == ANYLOC_PAIR_TF32 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_BF16 ||
-                 fmt == ANYLOC_PAIR_F16X1, "attention_varlen: bad fmt %d", fmt);
+                 fmt == ANYLOC_PAIR_F16X1 || fmt == ANYLOC_PAIR_BF16X3, "attention_varlen: bad fmt %d", fmt);
   const FormatInfo& f = format_info(fmt);
   ANYLOC_REQUIRE(qkv_hi && o_hi && row0 && len, "attention_varlen: null pointer");
   if (!f.lo)
@@ -447,8 +458,9 @@ struct VitBuffers {
 // n_patch patch rows and M token rows in all; the fp32 qkv rows only when `qkv32`.  Each buffer is sized by the format
 // that fills it (format_info): the patch rows pa [n_patch, Kp] in the patch embedding's format, the LayerNorm rows y
 // [M, D] in pair_dtype, q, k, v [M, 3D] (which also hold the fp32 [M, D] output of a lone q/k/v tap) and the hidden
-// layer h [M, H] in the SPLIT output format; lo arrays where the format has them.  The pair formats' buffers hold fp32
-// words, so that either pair format fits (the SIMT attention of the fp16-pair precision takes tf32 pairs).  Single
+// layer h [M, H] in the SPLIT output format; lo arrays where the format has them.  The tf32 and fp16 pairs' buffers
+// hold fp32 words, so that either pair format fits (the SIMT attention of the fp16-pair precision takes tf32 pairs); the
+// bf16 pairs' hold bf16.  Single
 // e4m3 adds the LayerNorm rows' scales [M] in y_lo and the e4m3 hidden layer h8 [M, H] with its row scales [M], and its
 // attention writes its bf16 output [M, D] into h.
 size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, void* ws, size_t ws_bytes,
@@ -459,7 +471,7 @@ size_t vit_carve(const AnylocVitCfg* c, size_t n_patch, size_t M, bool qkv32, vo
   Workspace w(ws ? ws : (void*)256, ws ? ws_bytes : (size_t)-1 / 2);
   // n elements of fi's arrays: hi, and lo (or null)
   auto take = [&](const FormatInfo& fi, size_t n, float** hi, float** lo) {
-    const size_t esz = fi.lo ? sizeof(float) : fi.esz;
+    const size_t esz = fi.lo && !fi.tc_only ? sizeof(float) : fi.esz;     // tf32 / fp16 pairs: fp32 words
     *hi = (float*)w.take<uint8_t>(n * esz);
     *lo = fi.lo ? (float*)w.take<uint8_t>(n * esz) : nullptr;
   };
@@ -512,16 +524,21 @@ bool registers_ok(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeight
   return true;
 }
 // The operand format of the weights: ANYLOC_OK, or (error text set) ANYLOC_ERR_ARG for a single format's weights with
-// a non-null lo matrix, ANYLOC_ERR_UNSUPPORTED for a single format on the SIMT engine
+// a non-null lo matrix or bf16-pair weights with a null one, ANYLOC_ERR_UNSUPPORTED for either on the SIMT engine
 int format_check(const char* fn, const AnylocVitCfg* cfg, const AnylocVitWeights* w, int engine) {
   const FormatInfo& f = format_info(cfg->pair_dtype);
   if (!f.tc_only) return ANYLOC_OK;
-  bool lo = w->patch_w_lo != nullptr;
+  bool lo = w->patch_w_lo != nullptr, no_lo = w->patch_w_lo == nullptr;
   for (int l = 0; l < cfg->depth && w->blocks; ++l) {
     const AnylocVitBlock& b = w->blocks[l];
     lo = lo || b.qkv_w_lo || b.proj_w_lo || b.in_w_lo || b.out_w_lo;
+    no_lo = no_lo || !b.qkv_w_lo || !b.proj_w_lo || !b.in_w_lo || !b.out_w_lo;
   }
-  if (lo) {
+  if (f.lo && no_lo) {
+    set_error("%s: pair_dtype %s takes %s weights; every *_w_lo must be non-NULL", fn, f.id, f.name);
+    return ANYLOC_ERR_ARG;
+  }
+  if (!f.lo && lo) {
     set_error("%s: pair_dtype %s takes %s block weights and %s patch weights; every *_w_lo must be NULL", fn, f.id,
               f.name, format_info(f.patch).name);
     return ANYLOC_ERR_ARG;
@@ -680,7 +697,7 @@ static int vit_block(const AnylocVitCfg* c, const AnylocVitBlock& wb, const VitB
       return rc;
   } else if (f.tc_only) {
     ProfScope ps(PC_ATTENTION, st, 4.0 * sq.B * (double)sq.T * sq.T * D);
-    if ((rc = attention_tc_launch(bf.qkv, nullptr, sq.B, sq.T, D, c->num_heads, o_hi, nullptr, attn_fmt, st))) return rc;
+    if ((rc = attention_tc_launch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, o_hi, o_lo, attn_fmt, st))) return rc;
   } else if ((rc = attention_dispatch(bf.qkv, bf.qkv_lo, sq.B, sq.T, D, c->num_heads, bf.y_hi, bf.y_lo,
                                       fmt == ANYLOC_PAIR_F16, engine, st, attn_fmt == ANYLOC_PAIR_F16))) {
     return rc;

@@ -253,14 +253,15 @@ int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, in
 int attention_wg_varlen_launch(const void* qkv_hi, const void* qkv_lo, const VarlenAttnTable& tab, int D, int heads,
                                void* o_hi, void* o_lo, int fmt, cudaStream_t st);
 
-// qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, or single bf16 or single fp16
-// with qkv_lo unused); o_{hi,lo}: [B*T, D] of the same kind (single formats: o_hi only).  The 2-byte formats run attention_wg.cu's kernel.
+// qkv_{hi,lo}: [B*T, 3D] in the format fmt (ANYLOC_PAIR_*: tf32 pairs, fp16 pairs of 8*x, bf16 pairs, or single bf16 or
+// single fp16 with qkv_lo unused); o_{hi,lo}: [B*T, D] of the same kind (single formats: o_hi only).  The 2-byte formats
+// run attention_wg.cu's kernel; the mma.sync kernel here takes the tf32 pairs only.
 int attention_tc_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
                         int fmt, cudaStream_t st) {
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(B <= 65535 && heads <= 65535, "attention_tc: grid too large (B=%d heads=%d)", B, heads);
-  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1)
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1 || fmt == ANYLOC_PAIR_BF16X3)
     return attention_wg_launch(qkv_hi, qkv_lo, B, T, D, heads, o_hi, o_lo, fmt, st);
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen))
@@ -279,7 +280,7 @@ int attention_tc_varlen_launch(const void* qkv_hi, const void* qkv_lo, const Var
   using namespace atc;
   ANYLOC_REQUIRE(D == heads * HD, "attention_tc: head_dim must be 64 (D=%d heads=%d)", D, heads);
   ANYLOC_REQUIRE(heads <= 65535, "attention_tc: grid too large (heads=%d)", heads);
-  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1)
+  if (fmt == ANYLOC_PAIR_BF16 || fmt == ANYLOC_PAIR_F16 || fmt == ANYLOC_PAIR_F16X1 || fmt == ANYLOC_PAIR_BF16X3)
     return attention_wg_varlen_launch(qkv_hi, qkv_lo, tab, D, heads, o_hi, o_lo, fmt, st);
   static unsigned long long attr_seen = 0;
   if (first_use_on_this_device(&attr_seen))

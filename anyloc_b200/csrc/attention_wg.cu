@@ -7,6 +7,8 @@
 //   ANYLOC_PAIR_F16X1: q, k, v are one fp16 array, the hi half of the fp16 pairs of 8*x; one term per product, the
 //                      pairs' scales (1/64 in the logit scale, P = 1024 p rounded once to its hi half); output the hi of
 //                      8*o.
+//   ANYLOC_PAIR_BF16X3: q, k, v are bf16 pairs (hi, lo) of x, no scale; both products 3-term as for the fp16 pairs, P
+//                      (unscaled) split into bf16 pairs; output bf16 pairs of o.
 // The arithmetic is that of the mma.sync kernel it replaced (attention_tc.cu keeps it for tf32 pairs): P = 1024 p split
 // into fp16 pairs, 1/kActScale^2 and log2(e) folded into the logit scale, ex2.approx, and each 64-key block's P.V
 // accumulated from zero by the tensor core and then added to the running output with round-to-nearest fp32 adds.
@@ -331,8 +333,9 @@ static int launch(const void* qkv_hi, const void* qkv_lo, int imgs, int rows, in
 
 }  // namespace awg
 
-// qkv_{hi,lo}: [B*T, 3D] in the format fmt: fp16 pairs of 8*x (ANYLOC_PAIR_F16), or one array (qkv_lo and o_lo
-// unused) of bf16 (_BF16) or of the hi halves of those fp16 pairs (_F16X1); o_{hi,lo}: [B*T, D] of the same kind.
+// qkv_{hi,lo}: [B*T, 3D] in the format fmt: fp16 pairs of 8*x (ANYLOC_PAIR_F16), bf16 pairs of x (_BF16X3), or one
+// array (qkv_lo and o_lo unused) of bf16 (_BF16) or of the hi halves of those fp16 pairs (_F16X1); o_{hi,lo}: [B*T, D]
+// of the same kind.
 // 16-byte aligned (the caller checks).
 int attention_wg_launch(const void* qkv_hi, const void* qkv_lo, int B, int T, int D, int heads, void* o_hi, void* o_lo,
                         int fmt, cudaStream_t st) {

@@ -119,6 +119,12 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
   return r;
 }
+// bf16 pair format (ANYLOC_PAIR_BF16X3): hi = bf16_rn(x), lo = bf16_rn(x - hi); x - hi is exact in fp32 (hi keeps x's
+// leading 8 bits, so the difference fits in 24).  Two values -> packed (hi, lo) words; `a` in the low 16 bits.
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
+  hi2 = pack_bf16x2(a, b);
+  lo2 = pack_bf16x2(a - __uint_as_float(hi2 << 16), b - __uint_as_float(hi2 & 0xffff0000u));
+}
 
 // Single e4m3 format (ANYLOC_PAIR_FP8): a row (activations) or a matrix (weights) is one e4m3 array q = e4m3_rn(x / s)
 // with one power-of-two scale s, x ~ q s.  s = 2^k with k the smallest integer that puts max|x| / s <= 448 (e4m3's

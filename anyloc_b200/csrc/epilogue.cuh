@@ -13,8 +13,8 @@ struct EpiParams {
   float* out_lo;        // [M,ldo] (SPLIT modes)
   int ldo;
   float alpha = 1.0f;   // accumulator scale (1/(s_A*s_B) for fp16-pair inputs, else 1)
-  int out_fmt = ANYLOC_PAIR_TF32;   // SPLIT output format (ANYLOC_PAIR_*): the pair GEMMs write tf32 or fp16 pairs by it
-                                    // at run time; the single formats write Fmt<FMT>::OUT
+  int out_fmt = ANYLOC_PAIR_TF32;   // SPLIT output format (ANYLOC_PAIR_*): the tf32 and fp16 pair GEMMs write tf32 or
+                                    // fp16 pairs by it at run time; the other formats write Fmt<FMT>::OUT
   const int* gate = nullptr;   // device flag (nullable): tensor-core GEMM kernels return immediately when *gate == 0 (conditional fallbacks without a host sync)
   const float* row_scale = nullptr;   // [M] e4m3 A operand's row scales (single e4m3 GEMM only): acc of row m times row_scale[m]
 };
@@ -25,11 +25,11 @@ __device__ __forceinline__ void split_put1(const EpiParams& p, size_t o, float v
   typedef typename Fmt<OUT>::T T;
   put1<OUT>(reinterpret_cast<T*>(p.out), reinterpret_cast<T*>(p.out_lo), o, v);
 }
-// SPLIT output of a GEMM on FMT inputs (the SIMT engine's pair GEMMs take the default): Fmt<FMT>::OUT, or for the pair
-// inputs the pair format ep.out_fmt names, chosen at run time
+// SPLIT output of a GEMM on FMT inputs (the SIMT engine's pair GEMMs take the default): Fmt<FMT>::OUT, or for the tf32
+// and fp16 pair inputs the pair format ep.out_fmt names, chosen at run time (fixed_out)
 template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void epi_store_split(const EpiParams& p, size_t o, float v) {
-  if constexpr (!Fmt<FMT>::LO) split_put1<Fmt<FMT>::OUT>(p, o, v);
+  if constexpr (fixed_out<FMT>()) split_put1<Fmt<FMT>::OUT>(p, o, v);
   else if (p.out_fmt != ANYLOC_PAIR_TF32) split_put1<ANYLOC_PAIR_F16>(p, o, v);
   else split_put1<ANYLOC_PAIR_TF32>(p, o, v);
 }

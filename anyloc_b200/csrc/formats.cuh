@@ -81,6 +81,25 @@ template <> struct Fmt<ANYLOC_PAIR_F16X1> {   // single fp16: the hi of Fmt<ANYL
   }
 };
 
+template <> struct Fmt<ANYLOC_PAIR_BF16X3> {  // bf16 pairs: hi = bf16_rn(x), lo = bf16_rn(x - hi), no scale
+  typedef __nv_bfloat16 T;
+  static constexpr bool LO = true, SCALED = false;
+  typedef uint32_t W2;
+  static constexpr int OUT = ANYLOC_PAIR_BF16X3;
+  static __device__ __forceinline__ void split1(float x, T& h, T& l) {
+    h = __float2bfloat16_rn(x);
+    l = __float2bfloat16_rn(x - __bfloat162float(h));
+  }
+  static __device__ __forceinline__ void split2(float a, float b, W2& h, W2& l) { split_bf16x2(a, b, h, l); }
+  static __device__ __forceinline__ void pack2(float a, float b, uint32_t& h, uint32_t& l) { split_bf16x2(a, b, h, l); }
+  static __device__ __forceinline__ void put4(T* hi, T* lo, size_t i, float a, float b, float c, float d) {
+    uint2 h, l;
+    split_bf16x2(a, b, h.x, l.x);
+    split_bf16x2(c, d, h.y, l.y);
+    reinterpret_cast<uint2*>(hi)[i] = h; reinterpret_cast<uint2*>(lo)[i] = l;
+  }
+};
+
 // single e4m3: sizes only.  Its writers (LayerNorm's row scale, the quantisers) scale by a power of two per row or
 // tensor, a different kind of store; the A operand's lo slot holds those fp32 row scales.
 template <> struct Fmt<ANYLOC_PAIR_FP8> {
@@ -116,9 +135,14 @@ inline auto fmt_switch(int fmt, F&& f) {
     case ANYLOC_PAIR_BF16: return f(std::integral_constant<int, ANYLOC_PAIR_BF16>());
     case ANYLOC_PAIR_FP8: return f(std::integral_constant<int, ANYLOC_PAIR_FP8>());
     case ANYLOC_PAIR_F16X1: return f(std::integral_constant<int, ANYLOC_PAIR_F16X1>());
+    case ANYLOC_PAIR_BF16X3: return f(std::integral_constant<int, ANYLOC_PAIR_BF16X3>());
     default: return f(std::integral_constant<int, ANYLOC_PAIR_TF32>());
   }
 }
+
+// The SPLIT output format of a GEMM on FMT inputs is Fmt<FMT>::OUT, fixed at compile time -- except for the tf32 and
+// fp16 pairs, whose GEMMs write either of those two pair formats as EpiParams::out_fmt says at run time
+template <int FMT> __host__ __device__ constexpr bool fixed_out() { return !Fmt<FMT>::LO || FMT == ANYLOC_PAIR_BF16X3; }
 
 // Host-side facts of a format
 struct FormatInfo {
@@ -138,8 +162,9 @@ inline const FormatInfo& format_info(int fmt) {
       {"single-bf16", "ANYLOC_PAIR_BF16", 2, false, false, true, ANYLOC_PAIR_BF16, ANYLOC_PAIR_BF16},
       {"single-e4m3", "ANYLOC_PAIR_FP8", 1, false, true, true, ANYLOC_PAIR_BF16, ANYLOC_PAIR_BF16},
       {"single-fp16", "ANYLOC_PAIR_F16X1", 2, false, false, true, ANYLOC_PAIR_F16X1, ANYLOC_PAIR_F16X1},
+      {"bf16-pair", "ANYLOC_PAIR_BF16X3", 2, true, false, true, ANYLOC_PAIR_BF16X3, ANYLOC_PAIR_BF16X3},
   };
-  return table[fmt >= ANYLOC_PAIR_TF32 && fmt <= ANYLOC_PAIR_F16X1 ? fmt : ANYLOC_PAIR_TF32];
+  return table[fmt >= ANYLOC_PAIR_TF32 && fmt <= ANYLOC_PAIR_BF16X3 ? fmt : ANYLOC_PAIR_TF32];
 }
 
 }  // namespace anyloc

@@ -1,8 +1,9 @@
 // wgmma GEMM engine:  C[M,N] = (A_hi+A_lo)[M,K] . (B_hi+B_lo)[N,K]^T  + fused epilogue,
 // fp32-equivalent accuracy through the 3-term split
 //      A.B ~= A_hi.B_hi + A_lo.B_hi + A_hi.B_lo
-// where (hi, lo) are tf32 pairs (two fp32 words, consumed as tf32) or fp16 pairs of s*x, materialised by the producer
-// kernels (LayerNorm / previous epilogue / weight prep).
+// where (hi, lo) are tf32 pairs (two fp32 words, consumed as tf32), fp16 pairs of s*x or bf16 pairs of x (not
+// fp32-equivalent: about 16 significant bits), materialised by the producer kernels (LayerNorm / previous epilogue /
+// weight prep).
 //
 // Structure (one persistent CTA per SM, 3 warpgroups = 384 threads, CTA tile 128 x 128):
 //   warpgroup 0 : TMA producer -- one thread streams cp.async.bulk.tensor 2D, 128B-swizzled K-major boxes of 128 bytes
@@ -62,7 +63,8 @@ constexpr int CHUNK_KB_F16 = 8;            // (24 / 96 wgmma k-steps per chunk)
 // The single-bf16 pass keeps the round-to-nearest chunks of the fp16 pairs (CHUNK_KB_F16: 32 wgmmas per chunk).  Its
 // second 64-register accumulator fits without spills (ptxas -v), the chunk add is 64 FADDs per thread per 32 wgmmas,
 // and it keeps the accumulation term of the error (c u sqrt(K) |A||B|, u = 2^-24) that of the f16x3 GEMMs, so the
-// operands' own bf16 rounding (2^-8 relative) is the only new error term.
+// operands' own bf16 rounding (2^-8 relative) is the only new error term.  The bf16 pairs (ANYLOC_PAIR_BF16X3) take the
+// same chunks with the fp16 pairs' 96 wgmmas each, so their error over the fp16 pairs' is that of the operands' split.
 constexpr int CHUNK_KB_COARSE = 32;        // hi-only fp16 coarse pass (retrieval): <= 128 k-steps per chunk, the bound
                                            // topk.cu re-scores against
 // The e4m3 pass promotes the tensor core's partial sums into the round-to-nearest fp32 accumulator every k-block (128
@@ -85,7 +87,7 @@ __device__ __forceinline__ void split_put2(const EpiParams& ep, size_t o, float 
 }
 template <int FMT = ANYLOC_PAIR_TF32>
 __device__ __forceinline__ void store_split2(const EpiParams& ep, size_t o, float a, float b) {
-  if constexpr (!Fmt<FMT>::LO) split_put2<Fmt<FMT>::OUT>(ep, o, a, b);
+  if constexpr (fixed_out<FMT>()) split_put2<Fmt<FMT>::OUT>(ep, o, a, b);
   else if (ep.out_fmt != ANYLOC_PAIR_TF32) split_put2<ANYLOC_PAIR_F16>(ep, o, a, b);
   else split_put2<ANYLOC_PAIR_TF32>(ep, o, a, b);
 }
@@ -463,7 +465,7 @@ gemm_tc3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                                          n0, N, sum)
     if (mode == ANYLOC_EPI_BIAS) ANYLOC_EPI_STAGED(OUT_F32, false, false);
     else if (mode == ANYLOC_EPI_LS_RESID) ANYLOC_EPI_STAGED(OUT_F32, false, true);
-    else if constexpr (!Fmt<FMT>::LO) {      // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> the single output format
+    else if constexpr (fixed_out<FMT>()) {   // BIAS_SPLIT / GELU_SPLIT / SWIGLU_SPLIT -> the format's own output
       if (mode == ANYLOC_EPI_SWIGLU_SPLIT) ANYLOC_EPI_STAGED(Fmt<FMT>::OUT, true, false);
       else ANYLOC_EPI_STAGED(Fmt<FMT>::OUT, false, false);
     } else if (mode == ANYLOC_EPI_SWIGLU_SPLIT) {    // -> tf32 or fp16 pairs, as ep.out_fmt says
@@ -500,7 +502,7 @@ static EncodeTiledFn get_encode() {
 static CUtensorMapDataType map_dtype(int fmt) {
   switch (fmt) {
     case ANYLOC_PAIR_FP8: return CU_TENSOR_MAP_DATA_TYPE_UINT8;
-    case ANYLOC_PAIR_BF16: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    case ANYLOC_PAIR_BF16: case ANYLOC_PAIR_BF16X3: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     case ANYLOC_PAIR_F16: case ANYLOC_PAIR_F16X1: return CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     default: return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   }
@@ -615,7 +617,7 @@ static int launch_impl(const void* a_hi, const void* a_lo, int lda, const void* 
   // A gated launch is a conditional fallback that usually returns at once: it keeps the register epilogue, so it
   // encodes no output maps and asks for the same shared memory as the coarse pass it follows (a launch that asked
   // for more would make the SM switch its shared-memory configuration back and forth).
-  const int out = Fmt<FMT>::LO ? (ep.out_fmt != ANYLOC_PAIR_TF32 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32) : Fmt<FMT>::OUT;
+  const int out = fixed_out<FMT>() ? Fmt<FMT>::OUT : (ep.out_fmt != ANYLOC_PAIR_TF32 ? ANYLOC_PAIR_F16 : ANYLOC_PAIR_TF32);
   if (CF::STAGED && ep.gate == nullptr && (rc = make_epi_maps(ep, out, M, N, &mo, &mo_lo, &mr, &staged))) return rc;
   const int smem = staged ? CF::SMEM_BYTES_STAGED : CF::SMEM_BYTES;
   g_last_staged = staged ? 1 : 0;
@@ -639,8 +641,9 @@ static int gemm_chunk_env() {
   return chunk_env;
 }
 
-// C = A . B^T + epilogue of fmt operands.  The pair formats take lo operands (a_lo, b_lo nullable); the single formats
-// take none, except single e4m3, whose a_lo holds A's fp32 row scales [M].  The single bf16 and fp16 GEMMs accumulate
+// C = A . B^T + epilogue of fmt operands.  The tf32 and fp16 pairs take lo operands (a_lo, b_lo nullable), the bf16
+// pairs both of them (the caller checks); the single formats take none, except single e4m3, whose a_lo holds A's fp32
+// row scales [M].  The bf16 pairs run the fp16 pairs' 3-term pipeline with the bf16 wgmma and their chunks.  The single bf16 and fp16 GEMMs accumulate
 // in the fp16 pairs' round-to-nearest chunks (CHUNK_KB_F16), single e4m3 promotes every CHUNK_KB_FP8 k-blocks.  The
 // single formats have their own instantiations, so the hi-only coarse passes (<F16 | TF32, 0>) keep their register
 // epilogue and shared memory.
@@ -665,6 +668,9 @@ int gemm_tc_launch(const void* a_hi, const void* a_lo, int lda, const void* b_hi
   static int skip_epi = -1;
   if (skip_epi < 0) { const char* e = getenv("ANYLOC_GEMM_DEBUG_SKIP_EPI"); skip_epi = e ? atoi(e) : 0; }
   if (skip_epi && ((skip_epi >> ep_in.mode) & 1)) ep.mode = -1;
+  if (fmt == ANYLOC_PAIR_BF16X3)
+    return launch_impl<ANYLOC_PAIR_BF16X3, 3>(a_hi, a_lo, lda, b_hi, b_lo, ldb, M, N, K, ep,
+                                              chunk_env > 0 ? chunk_env : tc::CHUNK_KB_F16, st);
   const bool f16 = fmt == ANYLOC_PAIR_F16;
   const int lom = (a_lo ? 1 : 0) | (b_lo ? 2 : 0);
   // hi-only fp16 pass = the retrieval's coarse scores, whose error bound allows long chunks

@@ -101,14 +101,14 @@ __device__ __forceinline__ void fence_regs(float* d) {
                : ANYLOC_WG_D64 : "l"(adesc), "l"(bdesc), "r"(scale_d))
 
 // D[64 x 128] (+)= A[64 x K] . B[128 x K]^T of FMT operands, both K-major in shared memory; 32 bytes of K per
-// instruction: K = 8 (tf32), 16 (fp16, bf16) or 32 (e4m3).
+// instruction: K = 8 (tf32), 16 (fp16, bf16, either pairs' halves) or 32 (e4m3).
 // Accumulator layout (per warpgroup thread t, warp w = t / 32, lane l): d[4j + {0,1}] = row 16w + l/4, columns
 // 8j + 2(l%4) + {0,1}; d[4j + {2,3}] = row 16w + l/4 + 8, same columns.
 template <int FMT>
 __device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
   if constexpr (FMT == ANYLOC_PAIR_TF32) ANYLOC_WG_M64N128("k8.f32.tf32.tf32", "");
   else if constexpr (FMT == ANYLOC_PAIR_FP8) ANYLOC_WG_M64N128("k32.f32.e4m3.e4m3", "");
-  else if constexpr (FMT == ANYLOC_PAIR_BF16) ANYLOC_WG_M64N128("k16.f32.bf16.bf16", ", 0, 0");
+  else if constexpr (FMT == ANYLOC_PAIR_BF16 || FMT == ANYLOC_PAIR_BF16X3) ANYLOC_WG_M64N128("k16.f32.bf16.bf16", ", 0, 0");
   else ANYLOC_WG_M64N128("k16.f32.f16.f16", ", 0, 0");     // fp16 pairs, single fp16
 }
 #undef ANYLOC_WG_M64N128
@@ -152,7 +152,7 @@ __device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
 // row 16w + l/4 + 8.
 template <int FMT>
 __device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (FMT == ANYLOC_PAIR_BF16)
+  if constexpr (FMT == ANYLOC_PAIR_BF16 || FMT == ANYLOC_PAIR_BF16X3)
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR ", %32, %33, p, 1, 1, 0, 0;\n\t}"
                  : ANYLOC_WG_D32 : "l"(adesc), "l"(bdesc), "r"(scale_d));
@@ -168,7 +168,7 @@ __device__ __forceinline__ void wgmma_m64n64_ss(float* d, uint64_t adesc, uint64
 // wgmma, two n8 column groups per k16 step.
 template <int FMT>
 __device__ __forceinline__ void wgmma_m64n64_rs_tb(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
-  if constexpr (FMT == ANYLOC_PAIR_BF16)
+  if constexpr (FMT == ANYLOC_PAIR_BF16 || FMT == ANYLOC_PAIR_BF16X3)
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " ANYLOC_WG_D32_STR
                  ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"

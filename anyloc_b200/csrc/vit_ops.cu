@@ -279,7 +279,8 @@ __device__ __forceinline__ void qkv_tap_put(int lane, int D4, const float4 (&v)[
 // One fp32 row [q | k | v] of a tapped layer's qkv GEMM (3D columns, one warp, each element read once) -> the
 // attention's operands of the row in the format fmt (ANYLOC_PAIR_* but e4m3, or FMT_NONE for none), as the qkv GEMM's
 // split epilogue writes them, and the rows of the requested facets (out[f] != null), through facet_row's arithmetic.
-template <int MAXV>     // float4 per lane and third: D <= 128 * MAXV
+// FIXED != FMT_NONE: the format is FIXED (or FMT_NONE) and is not looked up among the others.
+template <int MAXV, int FIXED = FMT_NONE>     // float4 per lane and third: D <= 128 * MAXV
 __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ src, int D, int fmt, void* hi,
                                             void* lo, const QkvTapOuts& o, int64_t orow, int do_norm) {
   const int D4 = D >> 2;
@@ -290,7 +291,9 @@ __device__ __forceinline__ void qkv_tap_row(int lane, const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < MAXV; ++i)
       if (lane + i * 32 < D4) v[i] = xr[lane + i * 32];
-    if (fmt == ANYLOC_PAIR_BF16) qkv_tap_put<ANYLOC_PAIR_BF16, MAXV>(lane, D4, v, hi, lo, f, D);
+    if constexpr (FIXED != FMT_NONE) {
+      if (fmt == FIXED) qkv_tap_put<FIXED, MAXV>(lane, D4, v, hi, lo, f, D);
+    } else if (fmt == ANYLOC_PAIR_BF16) qkv_tap_put<ANYLOC_PAIR_BF16, MAXV>(lane, D4, v, hi, lo, f, D);
     else if (fmt == ANYLOC_PAIR_F16X1) qkv_tap_put<ANYLOC_PAIR_F16X1, MAXV>(lane, D4, v, hi, lo, f, D);
     else if (fmt == ANYLOC_PAIR_F16) qkv_tap_put<ANYLOC_PAIR_F16, MAXV>(lane, D4, v, hi, lo, f, D);
     else if (fmt == ANYLOC_PAIR_TF32) qkv_tap_put<ANYLOC_PAIR_TF32, MAXV>(lane, D4, v, hi, lo, f, D);
@@ -336,6 +339,33 @@ qkv_tap_varlen_kernel(const float* __restrict__ src, const __grid_constant__ Var
   const size_t e = (size_t)row * 3 * D * (fmt == ANYLOC_PAIR_TF32 ? 4 : 2);
   qkv_tap_row<MAXV>(lane, src + (size_t)row * 3 * D, D, fmt, fmt != FMT_NONE ? (char*)hi + e : nullptr,
                     lo ? (char*)lo + e : nullptr, o, orow, do_norm);
+}
+
+// The two kernels above with the operand format FMT fixed at compile time (the bf16 pairs), separate so that those
+// kernels keep the code they have
+template <int MAXV, int FMT>
+__global__ void __launch_bounds__(256)
+qkv_tap_fmt_kernel(const float* __restrict__ src, int M, int T, int D, void* hi, void* lo, const QkvTapOuts o,
+                   int use_cls, int do_norm) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= M) return;
+  const int b = row / T, t = row - b * T;
+  const int64_t orow = use_cls ? row : (t == 0 ? -1 : row - b - 1);
+  const size_t e = (size_t)row * 3 * D * sizeof(typename Fmt<FMT>::T);
+  qkv_tap_row<MAXV, FMT>(lane, src + (size_t)row * 3 * D, D, FMT, (char*)hi + e, (char*)lo + e, o, orow, do_norm);
+}
+template <int MAXV, int FMT>
+__global__ void __launch_bounds__(256)
+qkv_tap_fmt_varlen_kernel(const float* __restrict__ src, const __grid_constant__ VarlenImgTable tab, int M, int D,
+                          void* hi, void* lo, const QkvTapOuts o, int use_cls, int do_norm) {
+  const int lane = threadIdx.x & 31;
+  const int row = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (row >= M) return;
+  const int i = varlen_image_of(tab, row, 0);
+  const int64_t orow = use_cls ? row : (row == tab.tok0[i] ? -1 : row - i - 1);
+  const size_t e = (size_t)row * 3 * D * sizeof(typename Fmt<FMT>::T);
+  qkv_tap_row<MAXV, FMT>(lane, src + (size_t)row * 3 * D, D, FMT, (char*)hi + e, (char*)lo + e, o, orow, do_norm);
 }
 
 // gather token rows [B, T, ld] (skipping cls unless use_cls, column offset col0) -> [B, T', D] then normalise
@@ -492,7 +522,12 @@ int launch_facet_out_varlen(const float* src, const VarlenImgTable& tab, int row
 template <int MAXV>
 static void qkv_tap_launch(const float* src, int M, int T, const VarlenImgTable* tab, int D, int fmt, void* hi,
                            void* lo, const QkvTapOuts& o, int use_cls, int do_norm, cudaStream_t st) {
-  if (tab) qkv_tap_varlen_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, fmt, hi, lo, o, use_cls, do_norm);
+  constexpr int X3 = ANYLOC_PAIR_BF16X3;
+  if (fmt == X3 && tab)
+    qkv_tap_fmt_varlen_kernel<MAXV, X3><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, hi, lo, o, use_cls, do_norm);
+  else if (fmt == X3)
+    qkv_tap_fmt_kernel<MAXV, X3><<<cdiv(M, 8), 256, 0, st>>>(src, M, T, D, hi, lo, o, use_cls, do_norm);
+  else if (tab) qkv_tap_varlen_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, *tab, M, D, fmt, hi, lo, o, use_cls, do_norm);
   else qkv_tap_kernel<MAXV><<<cdiv(M, 8), 256, 0, st>>>(src, M, T, D, fmt, hi, lo, o, use_cls, do_norm);
 }
 int launch_qkv_tap(const float* src, int M, int T, const VarlenImgTable* tab, int D, int fmt, void* hi, void* lo,

@@ -1101,19 +1101,20 @@ class _HookHandle:
         pass
 
 
-PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16", "fp8", "f16x1")
+PRECISIONS = ("auto", "tf32x3", "f16x3", "bf16", "fp8", "f16x1", "bf16pair")
 # precisions whose GEMM operands are fp16 (scaled by 8): an operand beyond fp16's range overflows, which the guard catches
 _FP16_RANGE = ("f16x3", "f16x1")
 
 
 def resolve_precision(precision, gemm_engine="auto"):
     """The extractor's precision: the argument, else $ANYLOC_B200_PRECISION, else "auto".  ValueError on an unknown
-    name, and on "bf16", "fp8" or "f16x1" with gemm_engine="simt" (single bf16, e4m3 and fp16 run on the tensor cores
-    only)."""
+    name, and on "bf16", "fp8", "f16x1" or "bf16pair" with gemm_engine="simt" (single bf16, e4m3 and fp16 and the bf16
+    pairs run on the tensor cores only)."""
     precision = precision or os.environ.get("ANYLOC_B200_PRECISION", "auto")
     if precision not in PRECISIONS:
-        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3', 'bf16', 'fp8' or 'f16x1', got {precision!r}")
-    if precision in ("bf16", "fp8", "f16x1") and gemm_engine == "simt":
+        raise ValueError(f"precision must be 'auto', 'tf32x3', 'f16x3', 'bf16', 'fp8', 'f16x1' or 'bf16pair', got "
+                         f"{precision!r}")
+    if precision in ("bf16", "fp8", "f16x1", "bf16pair") and gemm_engine == "simt":
         raise ValueError(f"precision={precision!r} runs on the tensor cores only; use gemm_engine='auto' or 'tc3'")
     return precision
 
@@ -1132,7 +1133,7 @@ class _GuardedExtractor:
         self.precision = "f16x3" if self._auto else precision
         self.dino_model = _vit.VitWeights(dino_model, sd, dev, depth=self._depth(),
                                           pair={"f16x3": "f16", "tf32x3": "tf32", "bf16": "bf16",
-                                                "fp8": "fp8", "f16x1": "f16x1"}[self.precision])
+                                                "fp8": "fp8", "f16x1": "f16x1", "bf16pair": "bf16pair"}[self.precision])
         self.gemm_engine = gemm_engine
         self.fh_handle = _HookHandle()
         self._hook_out = None
@@ -1218,6 +1219,14 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
     fp32 in "bf16" stays fp32.  It keeps fp16's range, so the f16x3 overflow guard applies, and an
     overflow raises naming "bf16" (same speed, fp32's exponent range) as the way out.  Not a
     parity mode; it needs gemm_engine "auto" or "tc3".
+    "bf16pair" sits between the parity formats and the single-MMA ones, and is also never chosen by
+    "auto": every GEMM and attention operand is a bf16 pair, hi = bf16_rn(x), lo = bf16_rn(x - hi)
+    (about 16 significant bits), with three bf16 MMAs per product like f16x3, the same operand
+    bytes and fp32's exponent range -- no scale and no overflow guard, so activations that overflow
+    f16x3 stay finite.  What stays fp32 in "bf16" stays fp32.  Its error is that of products
+    rounded to about 16 significant bits (2^-16 relative, where f16x3 and tf32x3 keep about 22),
+    so it is not a parity mode, and its effect on recall with trained checkpoints has not been
+    measured.  It needs gemm_engine "auto" or "tc3".
 
     `dino_model` may also name a backbone with register tokens, `dinov2_vit{s,b,l,g}14_reg`.  As
     in the reference, only row 0 (cls) is dropped, so its 4 register rows come first: an output
@@ -1254,8 +1263,8 @@ class DinoV2ExtractFeatures(_GuardedExtractor):
         """img [B,3,H,W] -> [B, (1 +) R + N, D] (R = 4 register rows for the *_reg models, else 0); or a list/tuple of
         differently sized images [3,H_i,W_i] / [1,3,H_i,W_i], all on the extractor's device -> a list of [n_i, D] (views of one packed output), computed in one forward
         pass; item i is bit-identical to self(img[i][None])[0] when both run the tensor-core GEMMs (under "auto" a lone
-        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16", "fp8" or "f16x1", which always
-        run them)."""
+        image of fewer than 32 tokens takes the SIMT GEMMs, except with precision "bf16", "fp8", "f16x1" or "bf16pair",
+        which always run them)."""
         return self._guarded(img)
 
     def __del__(self):

@@ -112,7 +112,9 @@ class VitWeights:
     round-to-nearest bf16 copy of each weight matrix, half the bytes of the pairs; a fast mode, not a parity mode) or
     "fp8" (one e4m3 copy of each block weight matrix with a power-of-two scale, a quarter of the pairs' bytes, and a bf16
     patch embedding; a faster mode, not a parity mode) or "f16x1" (the hi array of the "f16" pair of each weight matrix
-    alone, bit for bit, half the bytes of the pairs; bf16's speed with 3 more significant bits, not a parity mode)."""
+    alone, bit for bit, half the bytes of the pairs; bf16's speed with 3 more significant bits, not a parity mode) or
+    "bf16pair" (bf16 pairs hi = bf16_rn(w), lo = bf16_rn(w - hi), the bytes of the "f16" pairs with fp32's exponent range
+    and no scale; three MMAs per product like the pairs, about 16 significant bits, not a parity mode)."""
 
     def __init__(self, name, state_dict, device, depth=None, pair="tf32"):
         if name not in ARCHS:
@@ -149,9 +151,20 @@ class VitWeights:
             """-> (hi, lo, alpha): the kernel-ready pair of a weight matrix and the accumulator scale
             1/(s_act*s_w) its GEMM epilogue applies (1.0 for tf32 pairs; bf16: (bf16_rn(w), None, 1.0); fp8 block
             matrices: (e4m3_rn(w / s_w), None, s_w), the patch embedding as bf16; f16x1: the f16 pair's (hi, None,
-            alpha))."""
+            alpha); bf16pair: (bf16_rn(w), bf16_rn(w - hi), 1.0), anyloc_split_bf16 of w and of the exact fp32
+            remainder)."""
             t = f32(t)
             with torch.cuda.device(dev):
+                if pair == "bf16pair":
+                    hi = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
+                    lo = torch.empty(t.shape, dtype=torch.bfloat16, device=dev)
+                    _lib.check(lib.anyloc_split_bf16(_lib.ptr(t), _lib.ptr(hi), t.numel(), _lib.stream_ptr()),
+                               "split_bf16")
+                    rem = t - hi.float()           # exact: hi holds w's leading 8 bits
+                    _lib.check(lib.anyloc_split_bf16(_lib.ptr(rem), _lib.ptr(lo), t.numel(), _lib.stream_ptr()),
+                               "split_bf16")
+                    self._keep += [hi, lo]
+                    return hi, lo, 1.0
                 if pair == "fp8" and not patch:
                     q = torch.empty(t.shape, dtype=torch.float8_e4m3fn, device=dev)
                     s_w = C.c_float()

@@ -82,6 +82,17 @@ extern "C" {
                                       |s x| > 65504 overflows to Inf.  Tensor-core engine only (wgmma GEMM at every
                                       M, wgmma attention).  Accumulators, LayerNorm statistics, softmax, the residual
                                       stream and every feature output stay fp32. */
+#define ANYLOC_PAIR_BF16X3 5       /* bf16 pairs, NOT fp32-equivalent: two bf16 arrays, hi = bf16_rn(x) and
+                                      lo = bf16_rn(x - hi) (x - hi is exact in fp32), about 16 significant bits with
+                                      fp32's exponent range; no scale (alpha 1 for activations and weights alike).  Both
+                                      lo arrays are mandatory: a NULL a_lo, b_lo, out_lo (SPLIT epilogues) or y_lo returns
+                                      ANYLOC_ERR_ARG (without its lo an operand is ANYLOC_PAIR_BF16).  Three bf16 MMAs
+                                      per product, hi.hi + lo.hi + hi.lo, accumulated in fp32 with the fp16 pairs'
+                                      round-to-nearest chunks.  The SPLIT epilogues, LayerNorm, im2col, the qkv tap and
+                                      the attention write bf16 pairs.  Tensor-core engine only (wgmma GEMM at every M,
+                                      wgmma attention): ANYLOC_GEMM_SIMT returns ANYLOC_ERR_UNSUPPORTED.  Accumulators,
+                                      LayerNorm statistics, softmax, the residual stream and every feature output stay
+                                      fp32.  Values beyond bf16's largest finite value (~3.39e38) round to Inf. */
 /* GEMM engines */
 #define ANYLOC_GEMM_AUTO 0
 #define ANYLOC_GEMM_SIMT 1         /* fp32 FFMA (validation / odd shapes)               */
@@ -485,6 +496,17 @@ typedef struct {
  * Workspace: single bf16's formula (2-byte GEMM inputs, no lo buffers), with A(x), n_p, M and H as above:
  *   A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + A(2 M D) + A(6 M D) + A(2 M H) [+ A(12 M D) for the fp32 qkv rows of the
  *   tap calls] + 4096 bytes. */
+/* bf16 pairs (pair_dtype = ANYLOC_PAIR_BF16X3), fp32's exponent range at the fp16 pairs' speed: the weight matrices are
+ * bf16 pairs (hi = anyloc_split_bf16 of w, lo = anyloc_split_bf16 of the fp32 remainder w - hi) with every *_w_lo
+ * non-NULL and every *_alpha 1; LayerNorm, im2col, the qkv epilogue / tap and the attention write bf16 pairs; the GEMMs
+ * and the attention run three bf16 MMAs per product.  What stays fp32 under single bf16 stays fp32.  Not a parity
+ * mode: products keep about 16 significant bits, where the tf32 and fp16 pairs keep about 22; no scale, so nothing
+ * overflows short of bf16's largest finite value.  A NULL *_w_lo returns ANYLOC_ERR_ARG and gemm_engine =
+ * ANYLOC_GEMM_SIMT ANYLOC_ERR_UNSUPPORTED, before anything is launched.  Every GEMM runs on the tensor cores whatever
+ * M, so single, list (_varlen) and tap calls are bit-identical.
+ * Workspace: the 2-byte buffers of single bf16, each with its lo buffer, with A(x), n_p, M and H as above:
+ *   2 A(2 n_p Kp) + A(4 n_p D) + A(4 M D) + 2 A(2 M D) + 2 A(6 M D) + 2 A(2 M H) [+ A(12 M D) for the fp32 qkv rows of
+ *   the tap calls] + 4096 bytes. */
 /* Alignment of every anyloc_vit_extract* call: ws and out (each taps_host[i].out) 16-byte (TMA and float4 access;
  * every buffer carved from ws inherits its alignment), img and pos_embed (each img[i] and pos_embed[i]) 4-byte, and the
  * weights as stated with AnylocVitBlock above, for every block 0..depth-1.  Anything else returns ANYLOC_ERR_ARG naming
@@ -565,6 +587,9 @@ int anyloc_vit_extract_taps_varlen(const AnylocVitCfg* cfg, const AnylocVitWeigh
 /* in_dtype = out_dtype = ANYLOC_PAIR_F16X1: C = alpha A . B^T of single fp16 operands (a_lo, b_lo, out_lo NULL, else
  * ANYLOC_ERR_ARG; single fp16 in with another out_dtype, or the reverse, ANYLOC_ERR_ARG); the SPLIT epilogues write
  * one fp16 array, the hi of the fp16 pair of 8 v, BIAS / LS_RESID fp32.  Tensor-core engine only, at every M. */
+/* in_dtype = out_dtype = ANYLOC_PAIR_BF16X3: C = alpha (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo) of bf16-pair operands, a_lo
+ * and b_lo mandatory (NULL: ANYLOC_ERR_ARG), out_lo mandatory for the SPLIT epilogues, which write the bf16 pair of v;
+ * bf16 pairs in with another out_dtype, or the reverse, ANYLOC_ERR_ARG.  Tensor-core engine only, at every M. */
 /* in_dtype = ANYLOC_PAIR_FP8, out_dtype = ANYLOC_PAIR_BF16: C = (s_r[m] alpha) (A . B^T) with A e4m3 [M, K] and its
  * fp32 row scales s_r in a_lo, B e4m3 (b_lo NULL) and alpha = s_w; out_lo NULL; the SPLIT epilogues write one bf16
  * array, BIAS / LS_RESID fp32.  K, lda and ldb multiples of 16.  Tensor-core engine only, at every M. */
@@ -583,6 +608,7 @@ int anyloc_split_bf16(const float* x, void* y, size_t n, void* stream);
  * out_dtype = ANYLOC_PAIR_TF32 / _F16: y_hi, y_lo [M, D] the pair of y (fp16 pairs: of 8 y);
  * out_dtype = ANYLOC_PAIR_BF16: y_hi = bf16_rn(LayerNorm(x)), y_lo NULL (else ANYLOC_ERR_ARG);
  * out_dtype = ANYLOC_PAIR_F16X1: y_hi = the hi array of the fp16 pair of 8 y, y_lo NULL (else ANYLOC_ERR_ARG);
+ * out_dtype = ANYLOC_PAIR_BF16X3: y_hi, y_lo [M, D] the bf16 pair of y (y_lo NULL: ANYLOC_ERR_ARG);
  * out_dtype = ANYLOC_PAIR_FP8: y_hi = e4m3 rows of LayerNorm(x) [M, D], y_lo = their fp32 scales [M].
  * D a multiple of 4 in [4, 2048].  ANYLOC_ERR_ARG before anything is launched for a null pointer, M < 0, D outside that
  * range, x, w or b not 16-byte aligned, or y_hi / y_lo not aligned to 4 of their elements (fp8: y_hi and the scales
@@ -608,6 +634,8 @@ int anyloc_quantize_fp8_tensor(const float* x, void* q, size_t n, float* scale_h
  * bf16, softmax in fp32; tensor cores only (ANYLOC_GEMM_SIMT: ANYLOC_ERR_UNSUPPORTED).
  * out_dtype = ANYLOC_PAIR_F16X1: the same with single fp16 qkv_hi of 8 x and o_hi of 8 o (the hi arrays of the fp16
  * pairs); 1/64 folded into the logit scale and P = 1024 p, as for the fp16 pairs, P rounded once.
+ * out_dtype = ANYLOC_PAIR_BF16X3: qkv and o are bf16 pairs [B,T,3D] / [B,T,D], qkv_lo and o_lo mandatory (NULL:
+ * ANYLOC_ERR_ARG); three bf16 MMAs per product, P split into a bf16 pair; tensor cores only, as for single bf16.
  * Alignment: o_hi and o_lo 8-byte (64-bit stores of the tensor-core epilogue), else ANYLOC_ERR_ARG before anything is
  * launched; a qkv that is not 16-byte aligned runs the SIMT kernel under ANYLOC_GEMM_AUTO (the single formats and
  * ANYLOC_GEMM_TC3: ANYLOC_ERR_UNSUPPORTED). */
@@ -617,8 +645,8 @@ int anyloc_attention(const float* qkv_hi, const float* qkv_lo, int B, int T, int
  * row0, len HOST int32 [n]; image i's q|k|v rows are [row0[i], row0[i] + len[i]) and its output rows the same rows of
  * o [rows, D].  Images may lie in any order with gaps between them; rows outside every image are neither used nor
  * written.  The operands are in the format fmt of the ViT's qkv epilogue, not converted: ANYLOC_PAIR_TF32 (tf32
- * pairs), ANYLOC_PAIR_F16 (fp16 pairs of 8*x, output pairs of 8*o), ANYLOC_PAIR_BF16 or ANYLOC_PAIR_F16X1 (qkv_lo, o_lo
- * NULL).  The same
+ * pairs), ANYLOC_PAIR_F16 (fp16 pairs of 8*x, output pairs of 8*o), ANYLOC_PAIR_BF16X3 (bf16 pairs), ANYLOC_PAIR_BF16 or
+ * ANYLOC_PAIR_F16X1 (qkv_lo, o_lo NULL).  The same
  * table (longest first) and launcher as the ViT; an image's rows are bit-identical to anyloc_attention on that image
  * alone (fp16 pairs: fed the tf32 pair of x) whatever the other images and the rows around it hold.
  * ANYLOC_ERR_ARG for a null pointer, n outside [1, ANYLOC_VIT_VARLEN_MAX_B], len[i] < 1, row0[i] < 0, overlapping
