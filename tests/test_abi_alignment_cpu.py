@@ -170,12 +170,21 @@ ALIGN = {
                                                ("taps[0].out", "taps[1].out")),
 }
 
-# Pointers whose alignment chooses a route instead of being refused, as documented: below 16 bytes a qkv runs
-# anyloc_attention's SIMT kernel under ANYLOC_GEMM_AUTO (B = 0 here: OK, nothing to run), and anyloc_attention_varlen
-# returns ANYLOC_ERR_UNSUPPORTED.  (entry, pointer) -> the code expected below the alignment.
-BELOW = {("anyloc_attention", "qkv_hi"): 0, ("anyloc_attention", "qkv_lo"): 0,
-         ("anyloc_attention_varlen", "qkv_hi"): _lib.ERR["unsupported"],
-         ("anyloc_attention_varlen", "qkv_lo"): _lib.ERR["unsupported"]}
+# The attention entries' rows hold for every format they take; their refusals run in the tf32 pairs (format 0) and
+# again in the bf16 pairs.
+X3 = _lib.PAIR["bf16pair"]
+ATTENTION_FMTS = (0, X3)
+
+# Pointers whose alignment chooses a route instead of being refused, as documented: below 16 bytes a tf32-pair qkv runs
+# anyloc_attention's SIMT kernel under ANYLOC_GEMM_AUTO (B = 0 here: OK, nothing to run); a bf16-pair qkv has no SIMT
+# kernel, and anyloc_attention returns ANYLOC_ERR_UNSUPPORTED even at B = 0 (it checks the qkv before the empty batch);
+# anyloc_attention_varlen returns ANYLOC_ERR_UNSUPPORTED in both formats.  (entry, pointer, format) -> the code
+# expected below the alignment.
+BELOW = {("anyloc_attention", "qkv_hi", 0): 0, ("anyloc_attention", "qkv_lo", 0): 0,
+         ("anyloc_attention", "qkv_hi", X3): _lib.ERR["unsupported"],
+         ("anyloc_attention", "qkv_lo", X3): _lib.ERR["unsupported"]}
+BELOW.update({("anyloc_attention_varlen", n, f): _lib.ERR["unsupported"] for n in ("qkv_hi", "qkv_lo")
+              for f in ATTENTION_FMTS})
 
 # The entries with device pointers that the table leaves out: why, and the tests that cover their alignment.
 EXEMPT = {
@@ -225,7 +234,7 @@ def _vit_taps(p):
     return (_lib.VitTap * 2)(*[_lib.VitTap(l, f, p[f"taps[{i}].out"]) for i, (l, f) in enumerate(VIT_TAPS)])
 
 
-def _attention_varlen(lib, p):
+def _attention_varlen(lib, p, fmt):
     # no shape of this entry runs nothing, so the other qkv pointer is kept below 16 bytes: each call stops at the
     # qkv check (ANYLOC_ERR_UNSUPPORTED), which follows the argument checks
     hi, lo = p["qkv_hi"], p["qkv_lo"]
@@ -234,14 +243,15 @@ def _attention_varlen(lib, p):
     else:
         lo = P + 8
     return lib.anyloc_attention_varlen(hi, lo, 2, (C.c_int32 * 2)(0, 70), (C.c_int32 * 2)(70, 50), 384, 6,
-                                       p["o_hi"], p["o_lo"], 0, None)
+                                       p["o_hi"], p["o_lo"], fmt, None)
 
 
 # Each entry's call at a shape that does no device work even without the alignment checks: nothing to do (B, R, N,
 # n_q, n_rows, rows = 0: -> OK), or, where even an empty call would launch or copy something (the k-means, the index
 # headers, the prepared blob, the residual descriptors), a workspace or blob of 0 bytes (-> ANYLOC_ERR_WORKSPACE, the
-# refusal that follows the pointer checks).  p[name] is the address handed for that pointer.
-def _calls(lib):
+# refusal that follows the pointer checks).  p[name] is the address handed for that pointer; fmt the attention
+# entries' format.
+def _calls(lib, fmt=0):
     ib = lib.anyloc_index_bytes(4, D_, 1)
     sb = lib.anyloc_index_split_bytes(4, D_)
     return {
@@ -334,8 +344,8 @@ def _calls(lib):
             p["assign"] if p["assign"] != P else None, p["inv_norm"], p["centers"], D_, K_, 1, 1, p["vlad"], p["ws"],
             1 << 20, None)),
         "anyloc_attention": (OK, lambda p: lib.anyloc_attention(
-            p["qkv_hi"], p["qkv_lo"], 0, 64, 384, 6, p["o_hi"], p["o_lo"], 0, 0, None)),
-        "anyloc_attention_varlen": (UNS, lambda p: _attention_varlen(lib, p)),
+            p["qkv_hi"], p["qkv_lo"], 0, 64, 384, 6, p["o_hi"], p["o_lo"], fmt, 0, None)),
+        "anyloc_attention_varlen": (UNS, lambda p: _attention_varlen(lib, p, fmt)),
         # the ViT entries: a 0-byte workspace, refused after the pointers (the forward itself always launches)
         "anyloc_vit_extract": (WS, lambda p: lib.anyloc_vit_extract(
             C.byref(VIT_CFG), C.byref(_vit_weights(p)), p["img"], 1, 28, 42, p["pos_embed"], 1, 2, 0, 1, p["out"],
@@ -361,22 +371,34 @@ CASES = [(e, n) for e, ptrs in ALIGN.items() for n in ptrs]
 _HOST = C.c_int64 * 8                           # split_search writes counts[0..1] on the host: a real array
 
 
-@pytest.mark.parametrize("entry,name", CASES, ids=[f"{e[7:]}-{n}" for e, n in CASES])
-def test_entry_refuses_pointer_below_its_alignment(lib, entry, name):
-    expect, call = _calls(lib)[entry]
+def refuses_below_alignment(lib, entry, name, fmt=0):
+    expect, call = _calls(lib, fmt)[entry]
     host = _HOST()
     base = C.addressof(host) if name == "counts" else P
     ptrs = {n: (C.addressof(host) if n == "counts" else P) for n in ALIGN[entry]}
     a = ALIGN[entry][name]
     for off in below(a):
         rc = call(dict(ptrs, **{name: base + off}))
-        if (entry, name) in BELOW:
-            assert rc == BELOW[entry, name], (entry, name, off, rc, _lib.last_error())
+        if (entry, name, fmt) in BELOW:
+            assert rc == BELOW[entry, name, fmt], (entry, name, fmt, off, rc, _lib.last_error())
             continue
         assert rc == ARG, (entry, name, off, rc, _lib.last_error())
         assert f"{name} must be {a}-byte aligned" in _lib.last_error(), (entry, name, off, _lib.last_error())
     for off in (a, 2 * a, 3 * a):
         assert call(dict(ptrs, **{name: base + off})) == expect, (entry, name, off, _lib.last_error())
+
+
+@pytest.mark.parametrize("entry,name", CASES, ids=[f"{e[7:]}-{n}" for e, n in CASES])
+def test_entry_refuses_pointer_below_its_alignment(lib, entry, name):
+    refuses_below_alignment(lib, entry, name)
+
+
+ATTENTION_CASES = [(e, n) for e in ("anyloc_attention", "anyloc_attention_varlen") for n in ALIGN[e]]
+
+
+@pytest.mark.parametrize("entry,name", ATTENTION_CASES, ids=[f"{e[7:]}-{n}" for e, n in ATTENTION_CASES])
+def test_bf16pair_attention_refuses_pointer_below_its_alignment(lib, entry, name):
+    refuses_below_alignment(lib, entry, name, X3)
 
 
 def _header():

@@ -332,7 +332,7 @@ def spec(L, entry, shape):
             p["vlad"], p["ws"], n["ws"], st)
     if entry in ("anyloc_attention", "anyloc_attention_varlen"):
         # fmt: ANYLOC_PAIR_TF32 (fp32 pairs), _F16 (anyloc_attention: tf32 pairs in, fp16 pairs out; _varlen: fp16
-        # pairs of 8 x both ways), _BF16 / _F16X1 (one 2-byte array each way)
+        # pairs of 8 x both ways), _BF16 / _F16X1 (one 2-byte array each way), _BF16X3 (bf16 pairs both ways)
         D, heads = 384, 6
         if entry == "anyloc_attention":
             B, T, fmt, engine = shape
@@ -348,10 +348,13 @@ def spec(L, entry, shape):
         elif fmt == 1 and entry == "anyloc_attention_varlen":
             hi = (8 * x).half()
             qkv = dict(qkv_hi=hi, qkv_lo=(8 * x - hi.float()).half())
+        elif fmt == 5:
+            hi = x.bfloat16()
+            qkv = dict(qkv_hi=hi, qkv_lo=(x - hi.float()).bfloat16())
         else:
             qkv = dict(qkv_hi=x, qkv_lo=1e-4 * rnd(rows, 3 * D, seed=7))
         osz = rows * D * (4 if fmt == 0 else 2)
-        bufs = dict(qkv, o_hi=osz, o_lo=osz if fmt in (0, 1) else None)
+        bufs = dict(qkv, o_hi=osz, o_lo=osz if fmt in (0, 1, 5) else None)
         outs = [o for o in ("o_hi", "o_lo") if bufs[o] is not None]
         if entry == "anyloc_attention":
             return bufs, outs, lambda p, n: lib.anyloc_attention(p["qkv_hi"], p["qkv_lo"], B, T, D, heads, p["o_hi"],
@@ -404,9 +407,9 @@ SHAPES = {
                                (2, 100, 128, 16, True)],
     "anyloc_vlad_accumulate_varlen": [(256, 16, (150, 0, 120), False), (64, 500, (200, 90), False),
                                       (128, 16, (60, 40), True)],
-    # the tensor-core, SIMT, fp16-pair, bf16 and fp16 kernels (ANYLOC_GEMM_AUTO = 0, _SIMT = 1)
-    "anyloc_attention": [(2, 70, 0, 0), (2, 70, 0, 1), (2, 70, 1, 0), (2, 70, 2, 0), (2, 70, 4, 0)],
-    "anyloc_attention_varlen": [(0,), (1,), (2,), (4,)],
+    # the tensor-core, SIMT, fp16-pair, bf16, fp16 and bf16-pair kernels (ANYLOC_GEMM_AUTO = 0, _SIMT = 1)
+    "anyloc_attention": [(2, 70, 0, 0), (2, 70, 0, 1), (2, 70, 1, 0), (2, 70, 2, 0), (2, 70, 4, 0), (2, 70, 5, 0)],
+    "anyloc_attention_varlen": [(0,), (1,), (2,), (4,), (5,)],
 }
 CASES = [(e, i) for e in SHAPES for i in range(len(SHAPES[e]))]
 

@@ -1,12 +1,13 @@
 """The four anyloc_vit_extract* entries at the pointer offsets their rows of the alignment table accept
 (tests/test_abi_alignment_cpu.py ALIGN): every weight, image, positional table, output and the workspace at +16 / +48
-bytes (16 required) or +4 / +12 (4 required) past a 256-byte boundary, inside NaN frames, in the five weight formats,
+bytes (16 required) or +4 / +12 (4 required) past a 256-byte boundary, inside NaN frames, in the six weight formats,
 on a 2-block ViT-S/14 without and with 4 register tokens.  Each call must give, bit for bit, what the same call on
 256-byte aligned buffers gives, with the same number of launches, the same number of tensor-core and SIMT GEMM groups
 (the profiler's gemm_tc / gemm_simt counts: an accepted buffer never moves a GEMM off its route) and intact frames.
 The single and tap calls run two 56x56 images (32 patch rows and 34 / 42 token rows: the tensor-core GEMMs under
-ANYLOC_GEMM_AUTO); the list calls run a 28x42 and a 42x42 image (15 patch rows: the pair formats' patch GEMM takes the
-SIMT kernel there, so both GEMM engines read offset weights).  The single calls return block 1's value facet, the tap
+ANYLOC_GEMM_AUTO); the list calls run a 28x42 and a 42x42 image (15 patch rows: the tf32 and fp16 pairs' patch GEMM takes
+the SIMT kernel there, so both GEMM engines read offset weights; the single formats and the bf16 pairs have no SIMT
+kernel).  The single calls return block 1's value facet, the tap
 calls block 0's query (below the deepest layer: qkv_tap_kernel writes it) and block 1's token output
 (facet_out_kernel).  One ViT-S forward at full depth is also held to
 test_vit_accuracy_gpu.py's fp64 bounds at offsets, and VitWeights is shown to copy a state dict of misaligned views
@@ -22,7 +23,7 @@ from tests.test_abi_offsets_gpu import L, accepted, run  # noqa: F401  (L: the l
 
 pytestmark = pytest.mark.gpu
 
-PAIRS = ("tf32", "f16", "bf16", "fp8", "f16x1")
+PAIRS = ("tf32", "f16", "bf16", "fp8", "f16x1", "bf16pair")
 KINDS = {"single": "anyloc_vit_extract", "taps": "anyloc_vit_extract_taps", "varlen": "anyloc_vit_extract_varlen",
          "taps_varlen": "anyloc_vit_extract_taps_varlen"}
 TAPS = ((0, "query"), (1, "token"))
@@ -155,7 +156,7 @@ def test_vit_offsets_match_aligned_call(L, pair, regs, kind):
     ref_groups = groups[0]
     assert rc == 0 and intact, (rc, L.last_error())
     assert all(torch.isfinite(ref[o].view(torch.float32)).all() for o in outs)
-    if kind in ("single", "taps") or pair in ("bf16", "fp8", "f16x1"):
+    if kind in ("single", "taps") or pair in ("bf16", "fp8", "f16x1", "bf16pair"):
         assert ref_groups[1] == 0, ref_groups          # M >= 32 or a single format: tensor cores only
     else:
         assert ref_groups[1] > 0, ref_groups           # the 15-row patch GEMM: SIMT

@@ -1,7 +1,8 @@
 """The 2-byte attention kernel works on 128-query tiles of two 64-row halves, one per consumer warpgroup; a half whose
 rows all lie at or beyond T does no work.  Sequence lengths around those edges (one half active or both, the second
 half with one row, several key blocks behind a partial tile, the c2 and c1 lengths), fp16 pairs against fp64 under
-the bound of test_attention_edges_gpu, and bf16 against fp64 under the bound of test_bf16_kernels_gpu.  The fp16-pair
+the bound of test_attention_edges_gpu, bf16 and single fp16 against fp64 under the bounds of test_bf16_kernels_gpu
+and test_f16x1_kernels_gpu (the bf16 pairs' tile edges are test_bf16x3_edges_gpu's).  The fp16-pair
 and tf32 outputs, hi and lo, are written inside NaN canaries that must stay intact."""
 import pytest
 import torch
@@ -31,6 +32,12 @@ def test_f16_pairs_at_tile_edges(L, T, kind):
 @pytest.mark.parametrize("T", TS)
 def test_bf16_at_tile_edges(L, T):
     from tests.test_bf16_kernels_gpu import test_attention_against_fp64
+    test_attention_against_fp64(L, T)
+
+
+@pytest.mark.parametrize("T", TS)
+def test_f16x1_at_tile_edges(L, T):
+    from tests.test_f16x1_kernels_gpu import test_attention_against_fp64
     test_attention_against_fp64(L, T)
 
 

@@ -1,7 +1,9 @@
-"""The packed attention of the list calls (anyloc_attention_varlen: attention_wg_varlen_kernel for fp16 pairs and single
-bf16, attention_tc_varlen_kernel for tf32 pairs), image by image against fp64 softmax(q k^T / 8) v of that image
-alone, under the bounds of the padded kernels: test_attention_edges_gpu's (c = 32, u = 2^-24) for the pair formats on
-the fp32 inputs, test_bf16_kernels_gpu.attn_bound for bf16 on the bf16-rounded operands.  For fp16 pairs the bound
+"""The packed attention of the list calls (anyloc_attention_varlen: attention_wg_varlen_kernel for fp16 and bf16 pairs,
+single bf16 and single fp16, attention_tc_varlen_kernel for tf32 pairs), image by image against fp64
+softmax(q k^T / 8) v of that image alone, under the bounds of the padded kernels: test_attention_edges_gpu's (c = 32,
+u = 2^-24) for the tf32 and fp16 pairs on the fp32 inputs, the attn_bound of test_bf16_kernels_gpu,
+test_bf16x3_kernels_gpu and test_f16x1_kernels_gpu for bf16, bf16 pairs and single fp16 on the values of the operands
+the kernel reads (the bf16 rounding, the bf16 pair, the fp16 rounding of 8 x over 8).  For fp16 pairs the bound
 adds the format's absolute floor (f16_floor): a one-key image with a value of about 1e-5 is off by some 500 times
 the relative bound alone, in the packed and the padded kernel alike, because the lo half of its fp16 pair underflows.
 
@@ -19,12 +21,16 @@ import torch
 
 from tests.test_attention_edges_gpu import C_ATT, U, reference, structured, to_qkv
 from tests.test_bf16_kernels_gpu import attn_bound, to_bf16
+from tests.test_bf16x3_kernels_gpu import attn_bound as pair_attn_bound, pair_of
+from tests.test_f16x1_kernels_gpu import attn_bound as f16x1_attn_bound
 from tests.util import dptr, split_f16, split_tf32
 
 pytestmark = pytest.mark.gpu
 
-FMTS = ["tf32", "f16", "bf16"]
-DTYPE = {"tf32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16}
+FMTS = ["tf32", "f16", "bf16", "bf16pair", "f16x1"]
+SINGLE = ("bf16", "f16x1")      # one array each way, no lo
+DTYPE = {"tf32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16, "bf16pair": torch.bfloat16,
+         "f16x1": torch.float16}
 BITS = {torch.float32: torch.int32, torch.float16: torch.int16, torch.bfloat16: torch.int16}
 CANARY = {torch.float32: 0x7FC0DEAD, torch.float16: 0x7EAD, torch.bfloat16: 0x7FDA}   # quiet NaNs no kernel writes
 LEAD = 16
@@ -58,11 +64,15 @@ def layout(lens, gap=0):
 
 
 def operands(L, x, fmt):
-    """the fp32 rows x [rows, 3D] in the format the qkv epilogue writes: (hi, lo) or (bf16, None)"""
+    """the fp32 rows x [rows, 3D] in the format the qkv epilogue writes: (hi, lo), (bf16, None) or (fp16 of 8 x, None)"""
     if fmt == "tf32":
         return split_tf32(L, x)
     if fmt == "f16":
         return split_f16(L, x, L.ACT_SCALE)
+    if fmt == "bf16pair":
+        return pair_of(x)
+    if fmt == "f16x1":
+        return split_f16(L, x, L.ACT_SCALE)[0], None
     return to_bf16(L, x), None
 
 
@@ -108,16 +118,17 @@ def packed(L, ops, row0, lens, heads, fmt, rows):
 
 
 def padded(L, x, ops, r, T, heads, fmt):
-    """anyloc_attention on image (rows [r, r + T)) alone: the tf32 pair of its fp32 rows for the pair formats (fp16
-    pairs: converted inside, hi + lo = x), its bf16 rows for bf16 -> (o_hi, o_lo) [T, D]"""
+    """anyloc_attention on image (rows [r, r + T)) alone: the tf32 pair of its fp32 rows for the tf32 and fp16 pairs
+    (fp16 pairs: converted inside, hi + lo = x), its rows of the packed operands for the formats the qkv epilogue
+    writes as such (bf16, bf16 pairs, single fp16) -> (o_hi, o_lo) [T, D]"""
     D = 64 * heads
     dt = DTYPE[fmt]
-    if fmt == "bf16":
-        q_hi, q_lo = ops[0][r:r + T].contiguous(), None
-    else:
+    if fmt in ("tf32", "f16"):
         q_hi, q_lo = split_tf32(L, x[r:r + T].contiguous())
+    else:
+        q_hi, q_lo = (None if a is None else a[r:r + T].contiguous() for a in ops)
     o_hi = canary_buf(T, D, dt)
-    o_lo = canary_buf(T, D, dt) if fmt != "bf16" else None
+    o_lo = canary_buf(T, D, dt) if fmt not in SINGLE else None
     L.check(L.load().anyloc_attention(dptr(q_hi), dptr(q_lo), 1, T, D, heads, dptr(o_hi, LEAD), dptr(o_lo, LEAD),
                                       L.PAIR[fmt], L.ENGINE["tc3"], L.stream_ptr()), "attention")
     torch.cuda.synchronize()
@@ -145,6 +156,8 @@ def value(L, out, fmt):
     hi, lo = out
     if fmt == "bf16":
         return hi.double()
+    if fmt == "f16x1":
+        return hi.double() / L.ACT_SCALE
     o = hi.double() + lo.double()
     return o / L.ACT_SCALE if fmt == "f16" else o
 
@@ -174,8 +187,14 @@ def worst_share(L, x, ops, out, row0, lens, heads, fmt, logit_term=True):
     for r, T in zip(row0, lens):
         got = got_all[r:r + T]
         assert bool(torch.isfinite(got).all()), (fmt, r, T)
-        if fmt == "bf16":
-            ref, bound = attn_bound(ops[0][r:r + T].double().reshape(1, T, 3, heads, 64))
+        if fmt in ("bf16", "bf16pair", "f16x1"):
+            if fmt == "bf16":
+                X, bound_of = ops[0][r:r + T].double(), attn_bound
+            elif fmt == "bf16pair":
+                X, bound_of = ops[0][r:r + T].double() + ops[1][r:r + T].double(), pair_attn_bound
+            else:
+                X, bound_of = ops[0][r:r + T].double() / L.ACT_SCALE, f16x1_attn_bound
+            ref, bound = bound_of(X.reshape(1, T, 3, heads, 64))
             ref, bound = (t[0].transpose(0, 1).reshape(T, D) for t in (ref, bound))
         else:
             ref, scale = reference(x[None, r:r + T], heads, logit_term)
@@ -331,9 +350,9 @@ def test_refusals_write_nothing(L, fmt):
     lens = [65, 130]
     x, row0, rows = images("flat", lens, heads, seed=0)
     hi, lo = operands(L, x, fmt)
-    other = "tf32" if fmt == "bf16" else "bf16"
+    other = "tf32" if fmt in SINGLE else "bf16"
     a, b = dptr(hi), dptr(lo)
-    b_bad = dptr(hi) if fmt == "bf16" else dptr(None)         # a lo array for bf16, none for a pair format
+    b_bad = dptr(hi) if fmt in SINGLE else dptr(None)         # a lo array for a single format, none for a pair
     cases = [(a, b, [0, 64], lens, heads, fmt, ARG),             # overlapping images
              (a, b, [-1, 65], lens, heads, fmt, ARG),
              (a, b, row0, [0, 130], heads, fmt, ARG),
@@ -346,7 +365,7 @@ def test_refusals_write_nothing(L, fmt):
         dt = DTYPE[fmt]
         o_hi, o_lo = canary_buf(rows, D, dt), canary_buf(rows, D, dt)
         rc = lib.anyloc_attention_varlen(qh, ql, 2, (C.c_int32 * 2)(*r0), (C.c_int32 * 2)(*ln), D, h,
-                                         dptr(o_hi, LEAD), dptr(o_lo if f != "bf16" else None, LEAD), L.PAIR[f],
+                                         dptr(o_hi, LEAD), dptr(o_lo if f not in SINGLE else None, LEAD), L.PAIR[f],
                                          L.stream_ptr())
         torch.cuda.synchronize()
         assert rc == want, (fmt, r0, ln, h, f, rc, L.last_error())

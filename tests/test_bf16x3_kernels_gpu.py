@@ -109,8 +109,10 @@ def operands(L, M, N, K, seed, lda=None, ldb=None):
 
 
 # ---------------------------------------------------------------------------------------------------------- GEMM
-def run_gemm(L, epi, M, N, K, *, ldo=None, use_bias=True, seed=0, lda=None, ldb=None, engine="auto"):
-    """one bf16pair GEMM with canaries -> (got, fp64 reference, bound, staged)"""
+def run_gemm(L, epi, M, N, K, *, ldo=None, alpha=1.0, use_bias=True, seed=0, lda=None, ldb=None, engine="auto",
+             resid="plain"):
+    """one bf16pair GEMM with canaries -> (got, fp64 reference, bound, staged).  The LS_RESID residual is a plain
+    buffer of its own ("plain"), one inside canaries ("separate") or the output itself ("in_place", as in the ViT)"""
     (a_hi, a_lo), (b_hi, b_lo) = operands(L, M, N, K, seed, lda, ldb)
     A, B = a_hi[:, :K].double() + a_lo[:, :K].double(), b_hi[:, :K].double() + b_lo[:, :K].double()
     n_out = N // 2 if epi == "swiglu_split" else N
@@ -119,22 +121,30 @@ def run_gemm(L, epi, M, N, K, *, ldo=None, use_bias=True, seed=0, lda=None, ldb=
     g = torch.Generator(device="cuda").manual_seed(seed + 1)
     bias = torch.randn(N, device="cuda", generator=g) * 0.1 if use_bias else None
     gamma = torch.randn(N, device="cuda", generator=g) if epi == "ls_resid" else None
-    resid = torch.randn(LEAD + M * ldo, device="cuda", generator=g) if epi == "ls_resid" else None
     out = canaries(M, ldo, split)
     out_lo = canaries(M, ldo, True) if split else None
-    rc = gemm_nt(L, a_hi, a_lo, b_hi, b_lo, M, N, K, pair="bf16pair", epi=epi, bias=bias, gamma=gamma, resid=resid,
-                 out=out, out_lo=out_lo, ldo=ldo, lda=lda, ldb=ldb, out_off=LEAD, engine=engine)
+    resid_buf, resid_t = None, None
+    if epi == "ls_resid":
+        if resid == "plain":
+            resid_buf = torch.randn(LEAD + M * ldo, device="cuda", generator=g)
+        else:
+            resid_buf = out if resid == "in_place" else canaries(M, ldo, False)
+            window(resid_buf, M, ldo, N).copy_(torch.randn(M, N, device="cuda", generator=g))
+        resid_t = window(resid_buf, M, ldo, N).clone()
+    rc = gemm_nt(L, a_hi, a_lo, b_hi, b_lo, M, N, K, pair="bf16pair", alpha=alpha, epi=epi, bias=bias, gamma=gamma,
+                 resid=resid_buf, out=out, out_lo=out_lo, ldo=ldo, lda=lda, ldb=ldb, out_off=LEAD, engine=engine)
     torch.cuda.synchronize()
     assert rc == 0, L.last_error()
     staged = L.load().anyloc_gemm_tc_last_staged()
     esz = 2 if split else 4
     assert staged == int((ldo * esz) % 16 == 0 and (n_out * esz) % 16 == 0), (epi, M, N, K, ldo, staged)
     assert untouched_outside(out, M, ldo, n_out) == 0, (epi, M, N, K, ldo)
-    ref, err = reference(dict(A=A, B=B), K, epi, 1.0, bias, gamma,
-                         window(resid, M, ldo, N) if resid is not None else None)
-    dropped = a_lo[:, :K].double().abs() @ b_lo[:, :K].double().abs().T
+    if resid == "separate" and resid_buf is not None:
+        assert untouched_outside(resid_buf, M, ldo, N) == 0, (epi, M, N, K, ldo)
+    ref, err = reference(dict(A=A, B=B), K, epi, alpha, bias, gamma, resid_t)
+    dropped = abs(alpha) * (a_lo[:, :K].double().abs() @ b_lo[:, :K].double().abs().T)
     if epi == "swiglu_split":       # the dropped term enters through x1 (|silu'| <= 1.1) and x2
-        x = A @ B.T + (bias.double() if bias is not None else 0)
+        x = A @ B.T * alpha + (bias.double() if bias is not None else 0)
         s1 = torch.nn.functional.silu(x[:, 0::2])
         err = err + 1.1 * dropped[:, 0::2] * x[:, 1::2].abs() + s1.abs() * dropped[:, 1::2] + \
             1.1 * dropped[:, 0::2] * dropped[:, 1::2]
