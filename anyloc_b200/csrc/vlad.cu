@@ -435,242 +435,60 @@ static inline size_t acc3_smem_bytes(int N, int K) {
   return ((size_t)4 * N + 3 * (size_t)(K + 1) + (size_t)ACC3_WARPS * K + 2 * (size_t)K + acc3_max_tasks(N, K) + 4) * 4 +
          (size_t)acc3_max_slots(N) * 512;
 }
-__global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
-vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
-                        const float* __restrict__ inv_norm, const float* __restrict__ centers, int N, int D, int K,
-                        int norm_descs, int intra_norm, float* vlad, float* partial_ss /* [B,K,nslices] */,
-                        int32_t* done /* [B], zero on entry */, int wait_all) {
-  extern __shared__ __align__(16) int sm3[];
-  int* ooff = sm3;                                          // [N] n * D of the rows, sorted by label (stable)
-  int* lab = ooff + N;                                      // [N]
-  float* inv_s = reinterpret_cast<float*>(lab + N);         // [N] 1/|x| in the same sorted order
-  int* start = reinterpret_cast<int*>(inv_s + N);           // [K+1] first sorted position of cluster k
-  int* tstart = start + K + 1;                              // [K+1] first task of cluster k
-  int* sbase = tstart + K + 1;                              // [K+1] first partial-sum slot of a multi-task cluster
-  int* cntw = sbase + K + 1;                                // [ACC3_WARPS][K]
-  float* kss = reinterpret_cast<float*>(cntw + ACC3_WARPS * K);   // [K]
-  float* ksq = kss + K;                                     // [K]
-  int* task_k = reinterpret_cast<int*>(ksq + K);            // [max_tasks]
-  float* inv = reinterpret_cast<float*>(task_k + acc3_max_tasks_dev(N, K));   // [N] 1/|x| in row order (prologue only)
-  float* slots = reinterpret_cast<float*>(sm3) +
-                 (((size_t)4 * N + 3 * (size_t)(K + 1) + (size_t)ACC3_WARPS * K + 2 * (size_t)K + acc3_max_tasks_dev(N, K) + 3) & ~(size_t)3);
-  __shared__ int next_task, s_last;
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  // images in reverse order: the assignment pass streamed them in ascending order, so the last ones are the most
-  // likely to still sit in L2 when this kernel starts
-  const int b = (int)gridDim.y - 1 - (int)blockIdx.y, slice = blockIdx.x, nslices = gridDim.x;
-  const int col = slice * 128 + lane * 4;
-  const bool colok = col < D;                               // D % 4 == 0
-  for (int n = t; n < N; n += blockDim.x) {
-    lab[n] = labels[(size_t)b * N + n];
-    inv[n] = norm_descs ? inv_norm[(size_t)b * N + n] : 1.0f;
-  }
-  for (int i = t; i < ACC3_WARPS * K; i += blockDim.x) cntw[i] = 0;
-  if (t == 0) next_task = 0;
-  __syncthreads();
-  // per-warp histograms over contiguous row chunks
-  const int chunk = (((N + ACC3_WARPS - 1) / ACC3_WARPS) + 31) & ~31;
-  const int r0 = min(N, w * chunk), r1 = min(N, r0 + chunk);
-  for (int n = r0 + lane; n < r1; n += 32) { const int l = lab[n]; if (l >= 0) atomicAdd(&cntw[w * K + l], 1); }
-  __syncthreads();
-  for (int k = t; k < K; k += blockDim.x) {                 // exclusive prefix over the warps, cluster totals
-    int tot = 0;
-    for (int ww = 0; ww < ACC3_WARPS; ++ww) { const int c = cntw[ww * K + k]; cntw[ww * K + k] = tot; tot += c; }
-    start[k] = tot;
-  }
-  __syncthreads();
-  if (w == 0) {                                             // exclusive scans: rows, tasks, partial-sum slots
-    int run_r = 0, run_t = 0, run_s = 0;
-    for (int k0 = 0; k0 < K; k0 += 32) {
-      const int k = k0 + lane;
-      const int c = k < K ? start[k] : 0;
-      const int nt = k < K ? max(1, (c + ACC3_SEG - 1) / ACC3_SEG) : 0;
-      const int ns = nt > 1 ? nt : 0;
-      int ir = c, it = nt, is = ns;
+
+// One task's sum in this lane's 4 columns: sum over the sorted positions [s, e) of one cluster of x * (1/|x|) - c.
+// xb points at the columns in the image's first row, ck at the cluster's centre; ooff / inv_s hold each row's offset
+// n * D and 1/|x| in sorted order (int in accumulate3's shared memory, int64_t in the sorted route's workspace).  Zero
+// for columns past D (colok false).  accumulate3 and the sorted route both sum their tasks here, so their descriptors
+// are bitwise equal.  The in-flight bytes live in registers (8 x 16 B per lane = 4 KB per warp; 4 CTAs x 8 warps ->
+// 128 KB per SM), so the loop is kept lean: row offsets and 1/|x| were laid out in sorted order by the placement pass.
+template <class Off>
+__device__ __forceinline__ float4 task_sum(bool colok, const float* ck, const float* xb, const Off* ooff,
+                                           const float* inv_s, int s, int e) {
+  const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(ck)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (colok) {
+    constexpr int U = 8;
+    int i = s;
+    for (; i + U <= e; i += U) {
+      float4 v[U];
 #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int yr = __shfl_up_sync(0xffffffffu, ir, o), yt = __shfl_up_sync(0xffffffffu, it, o),
-                  ys = __shfl_up_sync(0xffffffffu, is, o);
-        if (lane >= o) { ir += yr; it += yt; is += ys; }
+      for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const float sc = inv_s[i + u];
+        a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
       }
-      if (k < K) { start[k] = run_r + ir - c; tstart[k] = run_t + it - nt; sbase[k] = run_s + is - ns; }
-      run_r += __shfl_sync(0xffffffffu, ir, 31);
-      run_t += __shfl_sync(0xffffffffu, it, 31);
-      run_s += __shfl_sync(0xffffffffu, is, 31);
     }
-    if (lane == 0) { start[K] = run_r; tstart[K] = run_t; sbase[K] = run_s; }
-  }
-  __syncthreads();
-  for (int k = t; k < K; k += blockDim.x)                   // task table
-    for (int q = tstart[k]; q < tstart[k + 1]; ++q) task_k[q] = k;
-  for (int n0 = r0; n0 < r1; n0 += 32) {                    // stable placement
-    const int n = n0 + lane;
-    const int l = n < r1 ? lab[n] : -1;
-    const bool active = l >= 0;
-    const float iv = active ? inv[n] : 1.0f;
-    const unsigned am = __ballot_sync(0xffffffffu, active);
-    unsigned peers = 0; int rank = 0;
-    if (active) {
-      peers = __match_any_sync(am, l);
-      rank = __popc(peers & ((1u << lane) - 1u));
-      const int pos = start[l] + cntw[w * K + l] + rank;
-      ooff[pos] = n * D;
-      inv_s[pos] = iv;
-    }
-    __syncwarp();
-    if (active && rank == 0) cntw[w * K + l] += __popc(peers);
-    __syncwarp();
-  }
-  __syncthreads();
-  // tasks -> registers.  Every warp grabs its NEXT task one task early.
-  const float* xb = x + (size_t)b * N * D + col;
-  const int ntasks = tstart[K];
-  auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
-  int q = grab();
-  while (q < ntasks) {
-    const int qn = grab();
-    const int k = task_k[q];
-    const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
-    const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
-    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (colok) {
-      // The in-flight bytes live in registers (8 x 16 B per lane = 4 KB per warp; 4 CTAs x 8 warps -> 128 KB per SM),
-      // so the loop is kept lean: row offsets and 1/|x| were laid out in sorted order by the placement pass.
-      constexpr int U = 8;
-      int i = s;
-      for (; i + U <= e; i += U) {
-        float4 v[U];
+    if (i < e) {                                             // tail: < U rows, same order
+      float4 v[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
+      for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
+      for (int u = 0; u < U; ++u) {
+        if (i + u < e) {
           const float sc = inv_s[i + u];
           a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
         }
       }
-      if (i < e) {                                           // tail: < U rows, same order
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (i + u < e) {
-            const float sc = inv_s[i + u];
-            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-          }
-        }
-      }
-    }
-    if (nt == 1) {
-      if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
-      if (lane == 0) kss[k] = ss;
-    } else {
-      *reinterpret_cast<float4*>(slots + (size_t)(sbase[k] + seg) * 128 + lane * 4) = a;
-    }
-    q = qn;
-  }
-  __syncthreads();
-  for (int k = w; k < K; k += ACC3_WARPS) {                 // clusters of several tasks: combine in task order
-    const int nt = tstart[k + 1] - tstart[k];
-    if (nt <= 1) continue;
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int q = 0; q < nt; ++q) {
-      const float4 p = *reinterpret_cast<const float4*>(slots + (size_t)(sbase[k] + q) * 128 + lane * 4);
-      a.x += p.x; a.y += p.y; a.z += p.z; a.w += p.w;
-    }
-    if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-    const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
-    if (lane == 0) kss[k] = ss;
-  }
-  __syncthreads();
-  for (int k = t; k < K; k += blockDim.x) partial_ss[((size_t)b * K + k) * nslices + slice] = kss[k];
-  __syncthreads();
-  if (t == 0) {
-    __threadfence();      // cumulative: orders every write the barrier above made visible to this thread (the pattern of
-                          // cooperative-groups grid sync), instead of 256 per-thread fences
-    s_last = (atomicAdd(&done[b], 1) == nslices - 1);
-  }
-  __syncthreads();
-  if (wait_all) {
-    // Whole grid co-resident (checked on the host): every slice-CTA waits until all slices of its image have published
-    // their sums of squares, derives the SAME scales in the same order, and normalises ITS OWN 128-column slice -- the
-    // normalisation is spread over all CTAs of the image instead of serialising K*D elements behind the last one
-    // (measured tail of the last-CTA variant: 10 us of 41 at c2, 30-40 us of 130 at c5).
-    if (t == 0) {
-      const long long t0 = clock64();
-      for (;;) {
-        int v;
-        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(done + b) : "memory");
-        if (v >= nslices) break;
-        __nanosleep(64);
-        if (clock64() - t0 > 8000000000LL) __trap();      // never hang the GPU
-      }
-    }
-    __syncthreads();
-    const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
-    const int nq = K * 32;                                  // float4 elements of this slice
-    constexpr int UW = 8;
-    for (int i0 = t; i0 < nq; i0 += blockDim.x * UW) {
-      float4 v[UW];
-#pragma unroll
-      for (int u = 0; u < UW; ++u) {
-        const int i = i0 + u * blockDim.x, c4 = slice * 128 + (i & 31) * 4;
-        if (i < nq && c4 < D) v[u] = __ldcg(reinterpret_cast<const float4*>(vlad + ((size_t)b * K + (i >> 5)) * D + c4));
-      }
-#pragma unroll
-      for (int u = 0; u < UW; ++u) {
-        const int i = i0 + u * blockDim.x, c4 = slice * 128 + (i & 31) * 4;
-        if (i < nq && c4 < D) {
-          const float sc = kss[i >> 5];
-          v[u].x = (v[u].x * sc) * g; v[u].y = (v[u].y * sc) * g; v[u].z = (v[u].z * sc) * g; v[u].w = (v[u].w * sc) * g;
-          *reinterpret_cast<float4*>(vlad + ((size_t)b * K + (i >> 5)) * D + c4) = v[u];
-        }
-      }
-    }
-    return;
-  }
-  if (!s_last) return;
-  // ---- last CTA of this image: intra- and global normalisation (same factors as vlad_normalize_kernel)
-  __threadfence();
-  if (t == 0) done[b] = 0;
-  const float g = vlad_norm_factors(partial_ss, b, K, nslices, intra_norm, kss, ksq);
-  float4* vb = reinterpret_cast<float4*>(vlad + (size_t)b * K * D);
-  const int D4 = D >> 2, total4 = K * D4;
-  constexpr int UN = 8;                                     // loads batched ahead of the stores (L2 latency chain)
-  for (int i0 = t; i0 < total4; i0 += blockDim.x * UN) {
-    float4 v[UN];
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      const int i = i0 + u * blockDim.x;
-      if (i < total4) v[u] = __ldcg(vb + i);
-    }
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      const int i = i0 + u * blockDim.x;
-      if (i < total4) {
-        const float sc = kss[i / D4];
-        // two separate multiplications like F.normalize(intra) then F.normalize(global)
-        v[u].x = (v[u].x * sc) * g; v[u].y = (v[u].y * sc) * g; v[u].z = (v[u].z * sc) * g; v[u].w = (v[u].w * sc) * g;
-        vb[i] = v[u];
-      }
     }
   }
+  return a;
 }
 
-// accumulate3 on packed images: image b is rows [row0[b], row0[b] + len[b]) of x, labels and inv_norm, and N >= every
-// len[b] sizes the shared-memory layout.  A copy of accumulate3 that differs only in where it finds an image's rows
-// (rows.first / rows.count), so the padded kernel keeps its code.  The stable label order, the tasks and their sums
-// depend on the image's rows alone, not on N or on the row chunks of the histogram pass: an image's descriptor is
-// bitwise accumulate3's for the same rows.
-__global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
-vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
-                               const float* __restrict__ inv_norm, const float* __restrict__ centers,
-                               const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D, int K,
-                               int norm_descs, int intra_norm, float* vlad, float* partial_ss, int32_t* done,
-                               int wait_all) {
-  const PackedRows rows{row0, len};
+// A lane's share of a cluster's sum of squares: x*x, then y, z and w by fma.  accumulate3 and the sorted accumulate
+// spell it out because a sum of products leaves the fused pair to the compiler, which picks it per kernel, and their
+// descriptors must agree bit for bit.  vlad_sorted_combine_kernel still writes the sum of products (sum_sq there costs
+// it a register); it compiles to this order today, and test_vlad_large_k_gpu's multi-task layouts hold it there.
+__device__ __forceinline__ float sum_sq(float4 a) { return fmaf(a.w, a.w, fmaf(a.z, a.z, fmaf(a.y, a.y, a.x * a.x))); }
+
+// Image b is rows.count(b) <= N rows from rows.first(b) of x, labels and inv_norm (PaddedRows / PackedRows,
+// common.cuh); N sizes the shared-memory layout.
+template <class Rows>
+__device__ __forceinline__ void accumulate3_image(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                                                  const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                                                  Rows rows, int N, int D, int K, int norm_descs, int intra_norm,
+                                                  float* vlad, float* partial_ss, int32_t* done, int wait_all) {
   extern __shared__ __align__(16) int sm3[];
   int* ooff = sm3;                                          // [N] n * D of the rows, sorted by label (stable)
   int* lab = ooff + N;                                      // [N]
@@ -764,39 +582,10 @@ vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __res
     const int k = task_k[q];
     const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
     const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
-    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (colok) {
-      // The in-flight bytes live in registers (8 x 16 B per lane = 4 KB per warp; 4 CTAs x 8 warps -> 128 KB per SM),
-      // so the loop is kept lean: row offsets and 1/|x| were laid out in sorted order by the placement pass.
-      constexpr int U = 8;
-      int i = s;
-      for (; i + U <= e; i += U) {
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const float sc = inv_s[i + u];
-          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-        }
-      }
-      if (i < e) {                                           // tail: < U rows, same order
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (i + u < e) {
-            const float sc = inv_s[i + u];
-            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-          }
-        }
-      }
-    }
+    const float4 a = task_sum(colok, centers + (size_t)k * D + col, xb, ooff, inv_s, s, e);
     if (nt == 1) {
       if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+      const float ss = warp_sum(sum_sq(a));
       if (lane == 0) kss[k] = ss;
     } else {
       *reinterpret_cast<float4*>(slots + (size_t)(sbase[k] + seg) * 128 + lane * 4) = a;
@@ -813,7 +602,7 @@ vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __res
       a.x += p.x; a.y += p.y; a.z += p.z; a.w += p.w;
     }
     if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-    const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+    const float ss = warp_sum(sum_sq(a));
     if (lane == 0) kss[k] = ss;
   }
   __syncthreads();
@@ -889,6 +678,28 @@ vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __res
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
+vlad_accumulate3_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                        const float* __restrict__ inv_norm, const float* __restrict__ centers, int N, int D, int K,
+                        int norm_descs, int intra_norm, float* vlad, float* partial_ss /* [B,K,nslices] */,
+                        int32_t* done /* [B], zero on entry */, int wait_all) {
+  accumulate3_image(x, labels, inv_norm, centers, PaddedRows{nullptr, N}, N, D, K, norm_descs, intra_norm, vlad,
+                    partial_ss, done, wait_all);
+}
+
+// packed images: image b is rows [row0[b], row0[b] + len[b]) of x, labels and inv_norm, and N >= every len[b] sizes
+// the shared-memory layout.  The stable label order, the tasks and their sums depend on the image's rows alone, not on
+// N or on the row chunks of the histogram pass: an image's descriptor is bitwise accumulate3's for the same rows.
+__global__ void __launch_bounds__(ACC3_WARPS * 32, 4)
+vlad_accumulate3_varlen_kernel(const float* __restrict__ x, const int32_t* __restrict__ labels,
+                               const float* __restrict__ inv_norm, const float* __restrict__ centers,
+                               const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D, int K,
+                               int norm_descs, int intra_norm, float* vlad, float* partial_ss, int32_t* done,
+                               int wait_all) {
+  accumulate3_image(x, labels, inv_norm, centers, PackedRows{row0, len}, N, D, K, norm_descs, intra_norm, vlad,
+                    partial_ss, done, wait_all);
 }
 
 // columns per slice: every VLAD path cuts D into 128-column slices (one thread per column in the kernels below)
@@ -1096,7 +907,7 @@ vlad_normalize_kernel(float* __restrict__ vlad, const float* __restrict__ partia
 // accumulate3's summation order with its per-image tables in the workspace instead of shared memory, so no (N, K) is
 // out of reach.  vlad_sort_kernel (CTA per image) builds the stable label order of the rows, the tasks of <= 64 rows
 // of one cluster and the slot bases of multi-task clusters exactly as accumulate3's prologue does;
-// vlad_sorted_accumulate_kernel sums each task in registers with accumulate3's loop; vlad_sorted_combine_kernel adds
+// vlad_sorted_accumulate_kernel sums each task in registers with accumulate3's task_sum; vlad_sorted_combine_kernel adds
 // the slots of multi-task clusters in task order; vlad_normalize_kernel then applies the factors of vlad_norm_factors.
 // Every sum has accumulate3's order, so the descriptors are bitwise those of accumulate3 wherever it runs.
 constexpr int SORTED_TASKS_PER_CTA = 64;
@@ -1197,79 +1008,11 @@ vlad_sort_varlen_kernel(const int32_t* __restrict__ labels, const float* __restr
 
 // CTA = (128-column slice, image, range of SORTED_TASKS_PER_CTA tasks); warps grab the range's tasks dynamically.  A
 // single-task cluster's sum goes straight to the descriptor with its sum of squares; a multi-task cluster's to its
-// slot.  The loop body is accumulate3's, term for term.
-__global__ void __launch_bounds__(ACC3_WARPS * 32)
-vlad_sorted_accumulate_kernel(const float* __restrict__ x, const float* __restrict__ centers, int N, int D, int K,
-                              SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
-  __shared__ int next_task;
-  const int b = blockIdx.y, slice = blockIdx.x, nslices = gridDim.x, lane = threadIdx.x & 31;
-  const int maxT = acc3_max_tasks_dev(N, K), maxS = 2 * (N / ACC3_SEG) + 2;
-  const int* start = tb.start + (size_t)b * (K + 1);
-  const int* tstart = tb.tstart + (size_t)b * (K + 1);
-  const int* sbase = tb.sbase + (size_t)b * (K + 1);
-  const int* task_k = tb.task_k + (size_t)b * maxT;
-  const int64_t* ooff = tb.ooff + (size_t)b * N;
-  const float* inv_s = tb.inv_s + (size_t)b * N;
-  const int q0 = blockIdx.z * SORTED_TASKS_PER_CTA, q1 = min(tstart[K], q0 + SORTED_TASKS_PER_CTA);
-  if (q0 >= q1) return;
-  if (threadIdx.x == 0) next_task = q0;
-  __syncthreads();
-  const int col = slice * 128 + lane * 4;
-  const bool colok = col < D;
-  const float* xb = x + (size_t)b * N * D + col;
-  auto grab = [&]() { int q = 0; if (lane == 0) q = atomicAdd(&next_task, 1); return __shfl_sync(0xffffffffu, q, 0); };
-  int q = grab();
-  while (q < q1) {
-    const int qn = grab();
-    const int k = task_k[q];
-    const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
-    const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
-    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (colok) {
-      constexpr int U = 8;
-      int i = s;
-      for (; i + U <= e; i += U) {
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const float sc = inv_s[i + u];
-          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-        }
-      }
-      if (i < e) {
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (i + u < e) {
-            const float sc = inv_s[i + u];
-            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-          }
-        }
-      }
-    }
-    if (nt == 1) {
-      if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
-      if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
-    } else if (colok) {
-      *reinterpret_cast<float4*>(tb.slots + ((size_t)b * maxS + sbase[k] + seg) * D + col) = a;
-    }
-    q = qn;
-  }
-}
-
-// The same on packed images (image b's rows start at row0[b] of x; N sizes the tables): a copy that differs only in
-// the image's first row, so the padded kernel keeps its code.
-__global__ void __launch_bounds__(ACC3_WARPS * 32)
-vlad_sorted_accumulate_varlen_kernel(const float* __restrict__ x, const float* __restrict__ centers,
-                                     const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D,
-                                     int K, SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
-  const PackedRows rows{row0, len};
+// slot.  Image b's rows start at rows.first(b) of x; N sizes the tables.
+template <class Rows>
+__device__ __forceinline__ void sorted_accumulate_image(const float* __restrict__ x, const float* __restrict__ centers,
+                                                        Rows rows, int N, int D, int K, SortedTables tb,
+                                                        float* __restrict__ vlad, float* __restrict__ partial_ss) {
   __shared__ int next_task;
   const int b = blockIdx.y, slice = blockIdx.x, nslices = gridDim.x, lane = threadIdx.x & 31;
   const int maxT = acc3_max_tasks_dev(N, K), maxS = 2 * (N / ACC3_SEG) + 2;
@@ -1293,43 +1036,29 @@ vlad_sorted_accumulate_varlen_kernel(const float* __restrict__ x, const float* _
     const int k = task_k[q];
     const int seg = q - tstart[k], nt = tstart[k + 1] - tstart[k];
     const int s = start[k] + seg * ACC3_SEG, e = min(start[k + 1], s + ACC3_SEG);
-    const float4 c = colok ? __ldg(reinterpret_cast<const float4*>(centers + (size_t)k * D + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (colok) {
-      constexpr int U = 8;
-      int i = s;
-      for (; i + U <= e; i += U) {
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const float sc = inv_s[i + u];
-          a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-        }
-      }
-      if (i < e) {
-        float4 v[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) if (i + u < e) v[u] = __ldg(reinterpret_cast<const float4*>(xb + ooff[i + u]));
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (i + u < e) {
-            const float sc = inv_s[i + u];
-            a.x += v[u].x * sc - c.x; a.y += v[u].y * sc - c.y; a.z += v[u].z * sc - c.z; a.w += v[u].w * sc - c.w;
-          }
-        }
-      }
-    }
+    const float4 a = task_sum(colok, centers + (size_t)k * D + col, xb, ooff, inv_s, s, e);
     if (nt == 1) {
       if (colok) *reinterpret_cast<float4*>(vlad + ((size_t)b * K + k) * D + col) = a;
-      const float ss = warp_sum(a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w);
+      const float ss = warp_sum(sum_sq(a));
       if (lane == 0) partial_ss[((size_t)b * K + k) * nslices + slice] = ss;
     } else if (colok) {
       *reinterpret_cast<float4*>(tb.slots + ((size_t)b * maxS + sbase[k] + seg) * D + col) = a;
     }
     q = qn;
   }
+}
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sorted_accumulate_kernel(const float* __restrict__ x, const float* __restrict__ centers, int N, int D, int K,
+                              SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  sorted_accumulate_image(x, centers, PaddedRows{nullptr, N}, N, D, K, tb, vlad, partial_ss);
+}
+
+__global__ void __launch_bounds__(ACC3_WARPS * 32)
+vlad_sorted_accumulate_varlen_kernel(const float* __restrict__ x, const float* __restrict__ centers,
+                                     const int64_t* __restrict__ row0, const int32_t* __restrict__ len, int N, int D,
+                                     int K, SortedTables tb, float* __restrict__ vlad, float* __restrict__ partial_ss) {
+  sorted_accumulate_image(x, centers, PackedRows{row0, len}, N, D, K, tb, vlad, partial_ss);
 }
 
 // CTA = (128-column slice, image): clusters of several tasks, their slots added in task order (accumulate3's combine)
@@ -1771,6 +1500,15 @@ static size_t carve_prepared(void* blob, size_t bytes, int D, int K, PreparedVie
   return pv->chat && pv->chat_tf32 && pv->cbias && pv->cnorm ? w.off : 0;
 }
 
+// A prepared vocabulary stands in for the per-call centre prep: its c^, tf32 copy, bias and norms replace the
+// workspace's in ab.  -> false (ab untouched) without a blob or when the blob is too small for (D, K).
+static bool use_prepared(void* prepared, size_t prepared_bytes, int D, int K, AssignBufs* ab) {
+  PreparedView pv;
+  if (!prepared || !carve_prepared(prepared, prepared_bytes, D, K, &pv)) return false;
+  ab->chat = pv.chat; ab->chat_tf32 = pv.chat_tf32; ab->cbias = pv.cbias; ab->cnorm = pv.cnorm;
+  return true;
+}
+
 extern "C" size_t anyloc_vlad_prepared_bytes(int D, int K) {
   PreparedView pv;
   return carve_prepared(nullptr, 0, D, K, &pv);
@@ -1807,6 +1545,91 @@ static int vlad_route(int N, int D, int K) {
   return acc2_warps(K) >= 1 ? ANYLOC_VLAD_ROUTE_ACC2 : ANYLOC_VLAD_ROUTE_SORTED;
 }
 
+// The accumulation and normalisation of B images of up to N rows (N > 0) from their labels (or soft weights) and 1/|x|,
+// padded (image b at rows b * N; n_valid for the soft accumulate) or packed (row0 / len).  route is the hard
+// accumulation's (ANYLOC_VLAD_ROUTE_*; -1 with soft weights) and partial, done (ACC3: the tickets, zero on entry) and
+// tb (sorted: the tables) the workspace it needs.  Every generate and accumulate entry launches its accumulation here.
+template <bool PACKED>
+static int launch_accumulate(const float* feats, const int32_t* n_valid, const int64_t* row0, const int32_t* len,
+                             const int32_t* labels, const float* assign, const float* inv_norm, const float* centers,
+                             int B, int N, int D, int K, int norm_descs, int intra_norm, float* vlad, int route,
+                             float* partial, int32_t* done, const SortedTables* tb, cudaStream_t st) {
+  const int nslices = cdiv(D, ACC_COLS);
+  if (assign) {
+    if (PACKED)
+      vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm,
+                                                                               centers, D, K, norm_descs, vlad, partial);
+    else
+      vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N,
+                                                                        D, K, norm_descs, vlad, partial);
+    ANYLOC_CHECK_LAUNCH();
+    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  }
+  if (route == ANYLOC_VLAD_ROUTE_ACC3) {
+    const size_t smem3 = acc3_smem_bytes(N, K);
+    static unsigned long long attr_seen = 0;         // one flag word per instantiation, so per kernel
+    if (first_use_on_this_device(&attr_seen)) {
+      if (PACKED)
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_varlen_kernel,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+      else
+        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               100 * 1024));
+    }
+    // all CTAs co-resident -> the slice-CTAs of an image may wait for each other (distributed normalisation);
+    // otherwise the image's last CTA normalises alone
+    int occ = 0;
+    if (PACKED)
+      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_varlen_kernel,
+                                                                      ACC3_WARPS * 32, smem3));
+    else
+      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_kernel, ACC3_WARPS * 32,
+                                                                      smem3));
+    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
+    if (PACKED)
+      vlad_accumulate3_varlen_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
+          feats, labels, inv_norm, centers, row0, len, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
+    else
+      vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
+          feats, labels, inv_norm, centers, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
+    ANYLOC_CHECK_LAUNCH();
+    return ANYLOC_OK;
+  }
+  if (route == ANYLOC_VLAD_ROUTE_ACC2) {
+    const int warps = acc2_warps(K);
+    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
+    if (PACKED) {
+      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_varlen_kernel,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      vlad_accumulate2_varlen_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, row0, len,
+                                                                          D, K, norm_descs, warps, vlad, partial);
+    } else {
+      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)smem));
+      vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, N, D, K,
+                                                                   norm_descs, warps, vlad, partial);
+    }
+    ANYLOC_CHECK_LAUNCH();
+    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  }
+  const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
+  if (PACKED) {
+    vlad_sort_varlen_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, row0, len, N, D, K, norm_descs, *tb);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_accumulate_varlen_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(
+        feats, centers, row0, len, N, D, K, *tb, vlad, partial);
+  } else {
+    vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, N, D, K, norm_descs, *tb);
+    ANYLOC_CHECK_LAUNCH();
+    vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, *tb,
+                                                                                        vlad, partial);
+  }
+  ANYLOC_CHECK_LAUNCH();
+  vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, *tb, vlad, partial);
+  ANYLOC_CHECK_LAUNCH();
+  return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+}
+
 static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const float* centers, void* prepared,
                               size_t prepared_bytes, int B, int N, int D, int K, int dist_mode, int norm_descs,
                               int intra_norm, float* vlad, int32_t* labels_out, void* ws, size_t ws_bytes, void* stream) {
@@ -1822,7 +1645,6 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) { ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st)); return ANYLOC_OK; }
   const size_t R = (size_t)B * N;
-  const int nslices = cdiv(D, ACC_COLS);
   const size_t smem3 = acc3_smem_bytes(N, K);
   const bool fits3 = vlad_route(N, D, K) == ANYLOC_VLAD_ROUTE_ACC3;
   HardBufs hb;
@@ -1837,36 +1659,15 @@ static int vlad_generate_impl(const float* feats, const int32_t* n_valid, const 
   ANYLOC_REQUIRE(acc3 || warps >= 1, "vlad_generate: K=%d N=%d needs %zu B shared memory (accumulate3 has 100 KB)", K,
                  N, smem3);
   // a prepared vocabulary replaces the per-call centre prep on every route
-  PreparedView pv;
-  const bool use_prep = prepared && carve_prepared(prepared, prepared_bytes, D, K, &pv);
-  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
+  const bool use_prep = use_prepared(prepared, prepared_bytes, D, K, &ab);
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
   rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
   if (rc) return rc;
-  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
-  if (acc3) {
-    static unsigned long long attr_seen = 0;
-    if (first_use_on_this_device(&attr_seen)) {
-      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    }
-    // all CTAs co-resident -> the slice-CTAs of an image may wait for each other (distributed normalisation);
-    // otherwise the image's last CTA normalises alone
-    int occ = 0;
-    ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_kernel, ACC3_WARPS * 32, smem3));
-    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
-    vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(feats, hb.labels, hb.inv_norm, centers, N,
-                                                                             D, K, norm_descs, intra_norm, vlad,
-                                                                             hb.partial, ab.done, wait_all);
-    ANYLOC_CHECK_LAUNCH();
-  } else {
-    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, hb.labels, hb.inv_norm, centers, N, D, K,
-                                                                 norm_descs, warps, vlad, hb.partial);
-    ANYLOC_CHECK_LAUNCH();
-    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
-    if (rc) return rc;
-  }
+  // the assignment cleared the tickets
+  rc = launch_accumulate<false>(feats, nullptr, nullptr, nullptr, hb.labels, nullptr, hb.inv_norm, centers, B, N, D, K,
+                                norm_descs, intra_norm, vlad, acc3 ? ANYLOC_VLAD_ROUTE_ACC3 : ANYLOC_VLAD_ROUTE_ACC2,
+                                hb.partial, ab.done, nullptr, st);
+  if (rc) return rc;
   if (labels_out)
     ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, hb.labels, R * 4, cudaMemcpyDeviceToDevice, st));
   return ANYLOC_OK;
@@ -1894,13 +1695,8 @@ extern "C" int anyloc_vlad_generate_route(int B, int N, int D, int K) {
   return vlad_route(N, D, K);
 }
 
-// The sorted route's workspace: carve_hard's buffers for R feature rows without the tickets, then the per-image tables
-// of B images of up to N rows.  With ws == nullptr a dry run; returns the bytes taken, 0 when the workspace is too small.
-static size_t carve_sorted(void* ws, size_t ws_bytes, size_t R_feats, int B, int N, int D, int K, HardBufs* hb,
-                           SortedTables* tb) {
-  const size_t off = carve_hard(ws, ws_bytes, R_feats, B, D, K, false, hb);
-  if (!off) return 0;
-  Workspace w(ws ? (void*)((char*)ws + off) : (void*)256, ws ? ws_bytes - off : (size_t)-1 / 2);
+// The sorted route's per-image tables of B images of up to N rows, taken from w; false when w is too small.
+static bool take_sorted_tables(Workspace& w, int B, int N, int D, int K, SortedTables* tb) {
   const size_t R = (size_t)B * N, K1 = (size_t)B * (K + 1);
   tb->ooff = w.take<int64_t>(R);
   tb->inv_s = w.take<float>(R);
@@ -1910,8 +1706,17 @@ static size_t carve_sorted(void* ws, size_t ws_bytes, size_t R_feats, int B, int
   tb->sbase = w.take<int>(K1);
   tb->task_k = w.take<int>((size_t)B * acc3_max_tasks(N, K));
   tb->slots = w.take<float>((size_t)B * sorted_max_slots(N) * D);
-  const bool ok = tb->ooff && tb->inv_s && tb->cntw && tb->start && tb->tstart && tb->sbase && tb->task_k && tb->slots;
-  return ok ? off + w.off : 0;
+  return tb->ooff && tb->inv_s && tb->cntw && tb->start && tb->tstart && tb->sbase && tb->task_k && tb->slots;
+}
+
+// The sorted route's workspace: carve_hard's buffers for R feature rows without the tickets, then the per-image tables
+// of B images of up to N rows.  With ws == nullptr a dry run; returns the bytes taken, 0 when the workspace is too small.
+static size_t carve_sorted(void* ws, size_t ws_bytes, size_t R_feats, int B, int N, int D, int K, HardBufs* hb,
+                           SortedTables* tb) {
+  const size_t off = carve_hard(ws, ws_bytes, R_feats, B, D, K, false, hb);
+  if (!off) return 0;
+  Workspace w(ws ? (void*)((char*)ws + off) : (void*)256, ws ? ws_bytes - off : (size_t)-1 / 2);
+  return take_sorted_tables(w, B, N, D, K, tb) ? off + w.off : 0;
 }
 
 extern "C" size_t anyloc_vlad_sorted_workspace_bytes(int B, int N, int D, int K) {
@@ -1943,24 +1748,14 @@ extern "C" int anyloc_vlad_generate_sorted(const float* feats, const int32_t* n_
               anyloc_vlad_sorted_workspace_bytes(B, N, D, K));
     return ANYLOC_ERR_WORKSPACE;
   }
-  AssignBufs& ab = hb.ab;
-  PreparedView pv;
-  const bool use_prep = carve_prepared(prepared, prepared_bytes, D, K, &pv);
-  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
+  const bool use_prep = use_prepared(prepared, prepared_bytes, D, K, &hb.ab);
   const size_t R = (size_t)B * N;
-  const int nslices = cdiv(D, ACC_COLS);
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D + (double)K * D));
-  rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep);
+  rc = launch_assign(feats, n_valid, N, (int64_t)R, D, K, centers, dist_mode, hb.ab, hb.labels, hb.inv_norm, st,
+                     use_prep);
   if (rc) return rc;
-  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
-  vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, N, D, K, norm_descs, tb);
-  ANYLOC_CHECK_LAUNCH();
-  vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, tb,
-                                                                                      vlad, hb.partial);
-  ANYLOC_CHECK_LAUNCH();
-  vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, hb.partial);
-  ANYLOC_CHECK_LAUNCH();
-  rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
+  rc = launch_accumulate<false>(feats, nullptr, nullptr, nullptr, hb.labels, nullptr, hb.inv_norm, centers, B, N, D, K,
+                                norm_descs, intra_norm, vlad, ANYLOC_VLAD_ROUTE_SORTED, hb.partial, nullptr, &tb, st);
   if (rc) return rc;
   if (labels_out)
     ANYLOC_CHECK_CUDA(cudaMemcpyAsync(labels_out, hb.labels, R * 4, cudaMemcpyDeviceToDevice, st));
@@ -2030,11 +1825,8 @@ extern "C" int anyloc_vlad_generate_soft(const float* feats, const int32_t* n_va
   vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, n_valid, N, (int64_t)R, D, K, chat,
                                                                        soft_temp, assign, inv_norm);
   ANYLOC_CHECK_LAUNCH();
-  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
-  vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N, D,
-                                                                    K, norm_descs, vlad, partial);
-  ANYLOC_CHECK_LAUNCH();
-  int rc = launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  int rc = launch_accumulate<false>(feats, n_valid, nullptr, nullptr, nullptr, assign, inv_norm, centers, B, N, D, K,
+                                   norm_descs, intra_norm, vlad, -1, partial, nullptr, nullptr, st);
   if (rc) return rc;
   if (assign_out)
     ANYLOC_CHECK_CUDA(cudaMemcpyAsync(assign_out, assign, R * K * 4, cudaMemcpyDeviceToDevice, st));
@@ -2110,7 +1902,6 @@ extern "C" int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const 
   rc = varlen_rows_check(row0, len, B, R, st, "vlad_generate_varlen", &N);
   if (rc) return rc;
   const int route = vlad_route(N, D, K);
-  const int nslices = cdiv(D, ACC_COLS);
   const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
   ANYLOC_REQUIRE(route != ANYLOC_VLAD_ROUTE_SORTED || ztasks <= 65535,
                  "vlad_generate_varlen: N=%d K=%d exceed the launch grid", N, K);
@@ -2128,51 +1919,15 @@ extern "C" int anyloc_vlad_generate_varlen(const float* feats, int64_t R, const 
     ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st));
     return labels_out ? varlen_rows_out(nullptr, row0, len, B, R, 1, 0xff, labels_out, st) : ANYLOC_OK;
   }
-  AssignBufs& ab = hb.ab;
-  PreparedView pv;
-  const bool use_prep = prepared && carve_prepared(prepared, prepared_bytes, D, K, &pv);
-  if (use_prep) { ab.chat = pv.chat; ab.chat_tf32 = pv.chat_tf32; ab.cbias = pv.cbias; ab.cnorm = pv.cnorm; }
+  const bool use_prep = use_prepared(prepared, prepared_bytes, D, K, &hb.ab);
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)B * K * D + (double)K * D));
-  rc = launch_assign(feats, nullptr, 0, R, D, K, centers, dist_mode, ab, hb.labels, hb.inv_norm, st, use_prep,
+  rc = launch_assign(feats, nullptr, 0, R, D, K, centers, dist_mode, hb.ab, hb.labels, hb.inv_norm, st, use_prep,
                      (int64_t)B * N);
   if (rc) return rc;
-  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
-  if (route == ANYLOC_VLAD_ROUTE_ACC3) {
-    const size_t smem3 = acc3_smem_bytes(N, K);
-    static unsigned long long attr_seen = 0;
-    if (first_use_on_this_device(&attr_seen)) {
-      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             100 * 1024));
-    }
-    int occ = 0;
-    ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_varlen_kernel,
-                                                                    ACC3_WARPS * 32, smem3));
-    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
-    vlad_accumulate3_varlen_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
-        feats, hb.labels, hb.inv_norm, centers, row0, len, N, D, K, norm_descs, intra_norm, vlad, hb.partial, ab.done,
-        wait_all);
-    ANYLOC_CHECK_LAUNCH();
-  } else if (route == ANYLOC_VLAD_ROUTE_ACC2) {
-    const int warps = acc2_warps(K);
-    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
-    ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_varlen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem));
-    vlad_accumulate2_varlen_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, hb.labels, hb.inv_norm, centers, row0,
-                                                                        len, D, K, norm_descs, warps, vlad, hb.partial);
-    ANYLOC_CHECK_LAUNCH();
-    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
-    if (rc) return rc;
-  } else {
-    vlad_sort_varlen_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(hb.labels, hb.inv_norm, row0, len, N, D, K, norm_descs, tb);
-    ANYLOC_CHECK_LAUNCH();
-    vlad_sorted_accumulate_varlen_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(
-        feats, centers, row0, len, N, D, K, tb, vlad, hb.partial);
-    ANYLOC_CHECK_LAUNCH();
-    vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, hb.partial);
-    ANYLOC_CHECK_LAUNCH();
-    rc = launch_normalize(vlad, hb.partial, B, D, K, intra_norm, st);
-    if (rc) return rc;
-  }
+  // the assignment cleared the tickets of the ACC3 route
+  rc = launch_accumulate<true>(feats, nullptr, row0, len, hb.labels, nullptr, hb.inv_norm, centers, B, N, D, K,
+                               norm_descs, intra_norm, vlad, route, hb.partial, hb.ab.done, &tb, st);
+  if (rc) return rc;
   return labels_out ? varlen_rows_out(hb.labels, row0, len, B, R, 1, 0xff, labels_out, st) : ANYLOC_OK;
 }
 
@@ -2218,7 +1973,6 @@ extern "C" int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, c
     ANYLOC_CHECK_CUDA(cudaMemsetAsync(vlad, 0, (size_t)B * K * D * 4, st));
     return assign_out ? varlen_rows_out(nullptr, row0, len, B, R, K, 0, assign_out, st) : ANYLOC_OK;
   }
-  const int nslices = cdiv(D, ACC_COLS);
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)R * D + (double)B * K * D + (double)K * D));
   vlad_soft_centre_prep_kernel<<<K, 256, 0, st>>>(centers, K, D, chat);
   ANYLOC_CHECK_LAUNCH();
@@ -2230,11 +1984,8 @@ extern "C" int anyloc_vlad_generate_soft_varlen(const float* feats, int64_t R, c
   vlad_soft_assign_kernel<ROWS><<<std::max(blocks, 1), 256, smem, st>>>(feats, nullptr, 0, R, D, K, chat, soft_temp,
                                                                        assign, inv_norm);
   ANYLOC_CHECK_LAUNCH();
-  // launch_accumulate (below) restates this accumulation for given labels / weights: keep the two in step
-  vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm, centers,
-                                                                           D, K, norm_descs, vlad, partial);
-  ANYLOC_CHECK_LAUNCH();
-  rc = launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  rc = launch_accumulate<true>(feats, nullptr, row0, len, nullptr, assign, inv_norm, centers, B, N, D, K, norm_descs,
+                               intra_norm, vlad, -1, partial, nullptr, nullptr, st);
   if (rc) return rc;
   return assign_out ? varlen_rows_out(assign, row0, len, B, R, K, 0, assign_out, st) : ANYLOC_OK;
 }
@@ -2604,10 +2355,8 @@ extern "C" int anyloc_vlad_from_residuals(const float* resid, const int32_t* lab
 // shared: anyloc_vlad_label_multi labels each row against every hard vocabulary and writes its 1/|x| once, and
 // anyloc_vlad_soft_assign_multi writes every soft vocabulary's assignment from one read of each row.  Each member's
 // accumulation then runs alone from those per-row results (anyloc_vlad_accumulate / _varlen) with the kernels, route
-// and normalisation its own generate call takes, so every descriptor is bitwise that call's.  The kernels below are
-// new; the existing ones are launched unchanged, by launch_accumulate, whose launch sequences restate the host code of
-// vlad_generate_impl, anyloc_vlad_generate_sorted, anyloc_vlad_generate_varlen and the two soft entries (each of those
-// points back here): a change to one must be made to the other.
+// and normalisation its own generate call takes (launch_accumulate, which launches every generate call's
+// accumulation), so every descriptor is bitwise that call's.
 // ====================================================================================================================
 namespace anyloc {
 
@@ -2768,18 +2517,7 @@ size_t carve_accumulate(void* ws, size_t ws_bytes, int B, int N, int D, int K, i
   *partial = w.take<float>((size_t)B * K * cdiv(D, ACC_COLS));
   *done = route == ANYLOC_VLAD_ROUTE_ACC3 ? w.take<int32_t>((size_t)B) : nullptr;
   bool ok = *partial && (route != ANYLOC_VLAD_ROUTE_ACC3 || *done);
-  if (route == ANYLOC_VLAD_ROUTE_SORTED) {
-    const size_t R = (size_t)B * N, K1 = (size_t)B * (K + 1);
-    tb->ooff = w.take<int64_t>(R);
-    tb->inv_s = w.take<float>(R);
-    tb->cntw = w.take<int>((size_t)B * ACC3_WARPS * K);
-    tb->start = w.take<int>(K1);
-    tb->tstart = w.take<int>(K1);
-    tb->sbase = w.take<int>(K1);
-    tb->task_k = w.take<int>((size_t)B * acc3_max_tasks(N, K));
-    tb->slots = w.take<float>((size_t)B * sorted_max_slots(N) * D);
-    ok = ok && tb->ooff && tb->inv_s && tb->cntw && tb->start && tb->tstart && tb->sbase && tb->task_k && tb->slots;
-  }
+  if (route == ANYLOC_VLAD_ROUTE_SORTED) ok = take_sorted_tables(w, B, N, D, K, tb) && ok;
   return ok ? w.off : 0;
 }
 
@@ -2798,17 +2536,12 @@ int accumulate_alignment(const char* who, const float* feats, const int32_t* lab
   return ANYLOC_OK;
 }
 
-// The accumulation and normalisation of B images from given labels (or soft weights) and 1/|x|: the kernels, launch
-// shapes and route of vlad_generate_impl / anyloc_vlad_generate_sorted / anyloc_vlad_generate_soft (padded,
-// rows.first(b) = b * N) or of anyloc_vlad_generate_varlen / _soft_varlen (packed), with N the longest image.  Those
-// entries keep their own copies of these launch sequences (attributes, occupancy and wait_all, grids, normalise); the
-// generate_vocabularies GPU tests hold each route of this function to them bit for bit, ACC3, ACC2, sorted and soft.
+// anyloc_vlad_accumulate(_varlen) after their refusals: the route, the workspace and the tickets, then the launches
 template <bool PACKED>
-int launch_accumulate(const float* feats, const int32_t* n_valid, const int64_t* row0, const int32_t* len,
-                      const int32_t* labels, const float* assign, const float* inv_norm, const float* centers, int B,
-                      int N, int D, int K, int norm_descs, int intra_norm, float* vlad, void* ws, size_t ws_bytes,
-                      const char* who, cudaStream_t st) {
-  const int nslices = cdiv(D, ACC_COLS);
+int accumulate_call(const float* feats, const int32_t* n_valid, const int64_t* row0, const int32_t* len,
+                    const int32_t* labels, const float* assign, const float* inv_norm, const float* centers, int B,
+                    int N, int D, int K, int norm_descs, int intra_norm, float* vlad, void* ws, size_t ws_bytes,
+                    const char* who, cudaStream_t st) {
   const int route = assign ? -1 : vlad_route(N, D, K);
   const int ztasks = cdiv(acc3_max_tasks(N, K), SORTED_TASKS_PER_CTA);
   ANYLOC_REQUIRE(route != ANYLOC_VLAD_ROUTE_SORTED || ztasks <= 65535, "%s: N=%d K=%d exceed the launch grid", who, N,
@@ -2826,77 +2559,9 @@ int launch_accumulate(const float* feats, const int32_t* n_valid, const int64_t*
     return ANYLOC_OK;
   }
   ProfScope ps(PC_VLAD, st, 4.0 * ((double)B * N * D + (double)B * K * D));
-  if (assign) {
-    if (PACKED)
-      vlad_soft_accumulate_varlen_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, row0, len, assign, inv_norm,
-                                                                               centers, D, K, norm_descs, vlad, partial);
-    else
-      vlad_soft_accumulate_kernel<<<dim3(nslices, B), ACC_COLS, 0, st>>>(feats, n_valid, assign, inv_norm, centers, N,
-                                                                        D, K, norm_descs, vlad, partial);
-    ANYLOC_CHECK_LAUNCH();
-    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
-  }
-  if (route == ANYLOC_VLAD_ROUTE_ACC3) {
-    const size_t smem3 = acc3_smem_bytes(N, K);
-    static unsigned long long attr_seen = 0;         // one flag word per instantiation, so per kernel
-    if (first_use_on_this_device(&attr_seen)) {
-      if (PACKED)
-        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_varlen_kernel,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-      else
-        ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               100 * 1024));
-    }
-    ANYLOC_CHECK_CUDA(cudaMemsetAsync(done, 0, (size_t)B * sizeof(int32_t), st));
-    int occ = 0;
-    if (PACKED)
-      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_varlen_kernel,
-                                                                      ACC3_WARPS * 32, smem3));
-    else
-      ANYLOC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vlad_accumulate3_kernel, ACC3_WARPS * 32,
-                                                                      smem3));
-    const int wait_all = (long long)nslices * B <= (long long)occ * device_sm_count() ? 1 : 0;
-    if (PACKED)
-      vlad_accumulate3_varlen_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
-          feats, labels, inv_norm, centers, row0, len, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
-    else
-      vlad_accumulate3_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, smem3, st>>>(
-          feats, labels, inv_norm, centers, N, D, K, norm_descs, intra_norm, vlad, partial, done, wait_all);
-    ANYLOC_CHECK_LAUNCH();
-    return ANYLOC_OK;
-  }
-  if (route == ANYLOC_VLAD_ROUTE_ACC2) {
-    const int warps = acc2_warps(K);
-    const size_t smem = (size_t)(1 + warps) * K * 128 * 4;
-    if (PACKED) {
-      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_varlen_kernel,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      vlad_accumulate2_varlen_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, row0, len,
-                                                                          D, K, norm_descs, warps, vlad, partial);
-    } else {
-      ANYLOC_CHECK_CUDA(cudaFuncSetAttribute(vlad_accumulate2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem));
-      vlad_accumulate2_kernel<<<dim3(nslices, B), 128, smem, st>>>(feats, labels, inv_norm, centers, N, D, K,
-                                                                   norm_descs, warps, vlad, partial);
-    }
-    ANYLOC_CHECK_LAUNCH();
-    return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
-  }
-  if (PACKED) {
-    vlad_sort_varlen_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, row0, len, N, D, K, norm_descs, tb);
-    ANYLOC_CHECK_LAUNCH();
-    vlad_sorted_accumulate_varlen_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(
-        feats, centers, row0, len, N, D, K, tb, vlad, partial);
-  } else {
-    vlad_sort_kernel<<<B, ACC3_WARPS * 32, 0, st>>>(labels, inv_norm, N, D, K, norm_descs, tb);
-    ANYLOC_CHECK_LAUNCH();
-    vlad_sorted_accumulate_kernel<<<dim3(nslices, B, ztasks), ACC3_WARPS * 32, 0, st>>>(feats, centers, N, D, K, tb,
-                                                                                        vlad, partial);
-  }
-  ANYLOC_CHECK_LAUNCH();
-  vlad_sorted_combine_kernel<<<dim3(nslices, B), ACC3_WARPS * 32, 0, st>>>(N, D, K, tb, vlad, partial);
-  ANYLOC_CHECK_LAUNCH();
-  return launch_normalize(vlad, partial, B, D, K, intra_norm, st);
+  if (done) ANYLOC_CHECK_CUDA(cudaMemsetAsync(done, 0, (size_t)B * sizeof(int32_t), st));
+  return launch_accumulate<PACKED>(feats, n_valid, row0, len, labels, assign, inv_norm, centers, B, N, D, K, norm_descs,
+                                   intra_norm, vlad, route, partial, done, &tb, st);
 }
 }  // namespace
 
@@ -3119,9 +2784,8 @@ extern "C" int anyloc_vlad_accumulate(const float* feats, const int32_t* n_valid
   if (rc) return rc;
   ANYLOC_REQUIRE_ALIGNED(n_valid, 4, who, "n_valid", "int32 access");
   if (B == 0) return ANYLOC_OK;
-  return launch_accumulate<false>(feats, assign ? n_valid : nullptr, nullptr, nullptr, labels, assign, inv_norm,
-                                  centers, B, N, D, K, norm_descs, intra_norm, vlad, ws, ws_bytes, who,
-                                  (cudaStream_t)stream);
+  return accumulate_call<false>(feats, assign ? n_valid : nullptr, nullptr, nullptr, labels, assign, inv_norm, centers,
+                                B, N, D, K, norm_descs, intra_norm, vlad, ws, ws_bytes, who, (cudaStream_t)stream);
 }
 
 extern "C" int anyloc_vlad_accumulate_varlen(const float* feats, int64_t R, const int64_t* row0, const int32_t* len,
@@ -3140,6 +2804,6 @@ extern "C" int anyloc_vlad_accumulate_varlen(const float* feats, int64_t R, cons
   int N = 0;                                        // the padded batch's row count: the longest image
   rc = varlen_rows_check(row0, len, B, R, st, who, &N);
   if (rc) return rc;
-  return launch_accumulate<true>(feats, nullptr, row0, len, labels, assign, inv_norm, centers, B, N, D, K, norm_descs,
-                                 intra_norm, vlad, ws, ws_bytes, who, st);
+  return accumulate_call<true>(feats, nullptr, row0, len, labels, assign, inv_norm, centers, B, N, D, K, norm_descs,
+                               intra_norm, vlad, ws, ws_bytes, who, st);
 }
